@@ -1,17 +1,21 @@
 #!/usr/bin/env python
-"""bench.py — tokens/sec of the Llama-2-7B fine-tune step (BASELINE.json metric) on N B200s.
+"""bench.py — tokens/sec of a Llama-architecture fine-tune step (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR   # + what the last timed step computed
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...     # the HF/PyTorch CPU path of the reference's image
 
 A "step" is one optimiser step of the fine-tune hot path: forward, loss, backward, (gradient
 all-reduce), global-norm clip, AdamW over `per_device_batch` packed 4096-token sequences per
-GPU (HF TrainingArguments default per_device_train_batch_size = 8, run as 8 accumulation
-micro-steps of one sequence), synthetic token ids, random-init weights of the named arch.
+GPU (HF TrainingArguments default per_device_train_batch_size = 8, run as accumulation
+micro-steps of `micro_batch` sequences), synthetic token ids, random-init weights of the named arch.
+The model is Sheared-LLaMA-2.7B (princeton-nlp, the Llama-2 architecture at d 2560, ffn 6912, 32 layers,
+20 heads of 128): a Llama-2-7B fine-tune needs ~121 GB for its weights, fp32 master copy, gradient and
+Adam moments alone, which one 80 GB H100 does not hold.
 
-Printed line (rank 0): the contract keys + `roofline` (tcgen05 GEMM kernel, CUDA-event timed
+Printed line (rank 0): the contract keys + `roofline` (wgmma GEMM kernel, CUDA-event timed
 live inside the timed region) + `cpu_baseline` (the oracle port timed on host cores, N=1 only)
 + `e2e` (same metric through the public host-buffer API) + `clocks`.
 """
@@ -29,8 +33,20 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "tokens/sec Llama-2-7B fine-tune at 1/2/4/8 B200; % tensor-core roofline"
-FLOPS_PER_TOKEN = 42.864e9  # SURVEY.md §8d: 6*N_mm + 6*L*S*d at S=4096, no recompute credit
+METRIC = "tokens/sec Sheared-LLaMA-2.7B fine-tune at 1/2/4/8 H100; % tensor-core roofline"
+# vocab, hidden, ffn, layers, heads, kv heads, head_dim, seq, rms eps, rope theta (Sheared-LLaMA-2.7B config.json)
+WORKLOAD_ARCH = (32000, 2560, 6912, 32, 20, 20, 128, 4096, 1e-5, 10000.0)
+WORKLOAD_NAME = "Sheared-LLaMA-2.7B"
+
+
+def flops_per_token():
+    """SURVEY.md §8d: 6*N_mm + 6*L*S*d at S=4096, no recompute credit (N_mm: the matmul weights incl. lm_head)."""
+    V, d, f, L, H, Hkv, dh, S = WORKLOAD_ARCH[:8]
+    n_mm = L * (d * H * dh + 2 * d * Hkv * dh + H * dh * d + 3 * d * f) + V * d
+    return 6.0 * n_mm + 6.0 * L * S * d
+
+
+FLOPS_PER_TOKEN = flops_per_token()   # 17.73e9
 
 
 def peaks():
@@ -39,11 +55,12 @@ def peaks():
         d = json.load(open(p))
         return dict(burst=d["bf16_tflops"], sustained=d["bf16_tflops_sustained"], hbm=d["hbm_gbs"],
                     source="measured")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (dense bf16, HBM3), for a card allowed 700 W: not reached, a scale only
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -67,6 +84,8 @@ class ClockSampler:
     def stop(self):
         if self.proc:
             self.proc.terminate()
+            self.proc.wait()
+            self.proc = None
         sm, mx, reasons = [], 0.0, set()
         for r in self.rows:
             try:
@@ -133,7 +152,7 @@ class CpuSample:
         import torch
         from oracle import llama_oracle as O
         self.torch, self.O = torch, O
-        a = O.LLAMA2_7B
+        a = O.Arch(*WORKLOAD_ARCH)
         self.a = a
         g = torch.Generator().manual_seed(0)
         one = O.Arch(a.vocab_size, a.hidden_size, a.intermediate_size, 1, a.num_heads, a.num_kv_heads,
@@ -189,9 +208,9 @@ class CpuSample:
         return t_layer, t_head
 
 
-def cpu_measure(repeats: int, budget_s: float):
-    """Median over `repeats` samples (at least 3; fewer only if one sample alone exceeds the budget).
-    Returns (tokens/s of the full 32-layer step, description dict)."""
+def cpu_measure(repeats: int, budget_s: float, exact: bool = False):
+    """Median over `repeats` samples (at least 3; fewer only if one sample alone exceeds the budget), or over exactly
+    `repeats` samples when `exact`. Returns (tokens/s of the full 32-layer step, description dict)."""
     threads, sweep, avail = cpu_pick_threads()
     smp = CpuSample()
     t0 = time.perf_counter()
@@ -200,6 +219,8 @@ def cpu_measure(repeats: int, budget_s: float):
     n = max(3, min(repeats, int(budget_s / max(t_one, 1e-3))))
     if t_one > budget_s:
         n = 1
+    if exact:
+        n = max(1, repeats)
     t_runs = time.perf_counter()
     runs = [smp.run() for _ in range(n)]
     timed_wall = time.perf_counter() - t_runs
@@ -208,7 +229,7 @@ def cpu_measure(repeats: int, budget_s: float):
     med = per_seq[len(per_seq) // 2]
     value = CpuSample.TOKENS / med
     desc = dict(value=round(value, 3), unit="tokens/s", cores=threads, kind="port",
-                sample=(f"oracle port (fp32 torch, HF semantics): 1 of 32 true-width Llama-2-7B decoder layers "
+                sample=(f"oracle port (fp32 torch, HF semantics): 1 of 32 true-width {WORKLOAD_NAME} decoder layers "
                         f"fwd + bwd + AdamW on a full {CpuSample.TOKENS}-token sequence, plus final norm + lm_head + CE fwd/bwd "
                         f"(the real loss); step = 32 x layer + head per sequence, no extrapolation in tokens; "
                         f"median of {n} repeats after 1 warm-up"),
@@ -225,14 +246,15 @@ def cpu_baseline(budget_s: float = 40.0):
 
 def run_reference(args):
     """--impl reference: the reference's own path for this metric is the HF/PyTorch trainer
-    image (un-vendored, examples/llama2-7b/finetuned-model.yaml:6); transformers.Trainer cannot
+    image (un-vendored, examples/llama2-7b/finetuned-model.yaml:6), run here at the workload's size;
+    transformers.Trainer cannot
     be imported here (no `accelerate`), so its CPU path is the oracle port: same torch ops, host
     cores. Each step is the bounded sample of cpu_measure (one layer + head at full sequence
-    length); at most ~4 minutes of samples are timed whatever --steps says, never fewer than 3."""
+    length); exactly --steps samples are timed, their median reported."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    value, secs_per_seq, desc = cpu_measure(args.steps, 220.0)
+    value, secs_per_seq, desc = cpu_measure(args.steps, 220.0, exact=True)
     line = dict(impl="reference", metric=METRIC, value=round(value, 3), unit="tokens/s", n_gpus=args.gpus,
                 steps=args.steps, warmup=args.warmup, ms_per_step=round(secs_per_seq * 1e3 * PER_DEVICE_BATCH, 1),
                 higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32", data="synthetic",
@@ -253,34 +275,14 @@ PER_DEVICE_BATCH = 8
 RECOMPUTE = False
 MICRO_BATCH = 2   # sequences per accumulation micro-step: T = 8192 rows per GEMM (see workload_config)
 SHARD_STATE = False
-def gemm_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture of THIS kernel
-    family at THIS micro-batch's shape (profiles/r02_ncu_gemm_mb2_banded.json for M = 8192 tokens, r02_ncu_gemm.json
-    for M = 4096; written from the .ncu-rep by tools/ncu_gemm_json.py): the forward gate|up GEMM, with the dgrad and
-    accumulating-wgrad captures beside it."""
-    name = "r02_ncu_gemm_mb2_banded.json" if MICRO_BATCH == 2 else "r02_ncu_gemm.json"
-    path = os.path.join(ROOT, "profiles", name)
-    try:
-        j = json.load(open(path))
-        d = j["kernels"]
-        f = d["fwd_gateup"]
-        return dict(bytes=f["dram_read_bytes"] + f["dram_write_bytes"],
-                    note=(f"dram__bytes_read+write of one forward gate|up GEMM launch (M{j.get('tokens', 4096)} N22016 K4096) = "
-                          f"{f['traffic_over_algorithmic']}x its {f['algorithmic_bytes'] / 1e6:.0f} MB algorithmic; dgrad "
-                          f"{d['dgrad_gateup']['traffic_over_algorithmic']}x, accumulating wgrad "
-                          f"{d['wgrad_gateup_acc']['traffic_over_algorithmic']}x (profiles/{name}, ncu --set full)"))
-    except Exception:  # noqa: BLE001
-        return dict(bytes=None, note=f"profiles/{name} missing")
-
-
 def workload_config(n_gpus: int):
-    return dict(workload="Llama-2-7B bf16 causal-LM fine-tune, seq 4096 (BASELINE.json configs[1])",
+    return dict(workload=f"{WORKLOAD_NAME} bf16 causal-LM fine-tune, seq 4096 (BASELINE.json configs[1])",
                 global_batch=PER_DEVICE_BATCH * n_gpus, seq_len=4096, per_device_batch=PER_DEVICE_BATCH,
                 micro_batch=MICRO_BATCH, parallelism=f"dp{n_gpus}" + ("-sharded-state" if SHARD_STATE and n_gpus > 1 else ""),
                 optimizer="AdamW fp32 master, clip 1.0" + (", activation recomputation" if RECOMPUTE else ""),
-                l2="working set (13.5 GB bf16 weights + activations per micro-step) >> 126 MB L2; no flush needed",
-                micro_batch_note=("the per-device batch of 8 sequences runs as 4 accumulation micro-steps of 2: the N = 4096 "
-                                  "GEMMs then have 512 instead of 256 output tiles for 74 CTA pairs (98.8 % instead of 86.5 % wave "
+                l2="working set (5.4 GB bf16 weights + activations per micro-step) >> 50 MB L2; no flush needed",
+                micro_batch_note=("the per-device batch of 8 sequences runs as 4 accumulation micro-steps of 2: the N = 2560 "
+                                  "GEMMs then have 640 instead of 320 128x256 output tiles for 132 SMs (97 % instead of 81 % wave "
                                   "efficiency); same arithmetic as 8 x 1 (tests/test_engine.py 'accumulate' vs 'full')"))
 
 
@@ -307,16 +309,15 @@ def run_ours(args):
         dist.init_process_group("gloo", rank=rank, world_size=world)  # control plane only
     torch.cuda.set_device(local)
     # The decode metric runs FIRST (its engine is destroyed before the fine-tune model is built): each leg is an
-    # independent measurement, and after ~40 s of fine-tune steps at the 1 kW power cap the decode leg read 1.7 %
-    # lower than alone (profiles/r02_decode_v4_tiled.json vs the embedded object of r02_bench_n1_v14.json).
+    # independent measurement, and a power-capped card runs the decode leg slower after a long fine-tune region.
     decode_obj = None
     if world == 1 and not args.no_decode:
         try:
-            decode_obj = decode_leg(local)
+            decode_obj = decode_leg(local, dump_dir=args.dump_outputs)
         except Exception as ex:  # noqa: BLE001 -- the fine-tune line must not be lost to the second metric
             decode_obj = dict(error=f"{type(ex).__name__}: {ex}")
         torch.cuda.empty_cache()
-    arch = LlamaArch.llama2_7b(4096)
+    arch = LlamaArch(*WORKLOAD_ARCH)
     if args.layers:  # development knob; a reduced model is NOT the benchmark and is labelled so
         arch.num_layers = args.layers
     S, nseq = arch.max_seq_len, args.per_device_batch
@@ -339,8 +340,7 @@ def run_ours(args):
     g = torch.Generator().manual_seed(1234 + rank)
     n_prof = min(args.steps, 3)               # GEMM-bracketed steps for the roofline leg, outside both timed regions
     # every step of every region sees a FRESH batch: a 7B model memorises a 32k-token batch of random ids
-    # after one exposure (round 1's e2e region re-used the resident region's batches and printed loss 2.7
-    # where fresh uniform tokens cannot go below ln 32000 = 10.4)
+    # after one exposure (fresh uniform tokens cannot go below ln 32000 = 10.4)
     n_batches = args.warmup + 2 * args.steps + n_prof
     host_ids = torch.randint(0, arch.vocab_size, (n_batches, nseq, S), generator=g, dtype=torch.int32).pin_memory()
     dev_ids = host_ids[: args.warmup + args.steps].cuda()
@@ -372,17 +372,21 @@ def run_ours(args):
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    barrier()
-    e.timer_start()
-    for i in range(args.steps):
-        p = dev_ids[args.warmup + i].data_ptr()
-        e.train_step_resident(p, p, nseq, n_valid, lr=5e-5)
-    ms = e.timer_stop()
-    barrier()
-    clocks = sampler.stop() if rank == 0 else None
+    try:
+        barrier()
+        e.timer_start()
+        for i in range(args.steps):
+            p = dev_ids[args.warmup + i].data_ptr()
+            e.train_step_resident(p, p, nseq, n_valid, lr=5e-5)
+        ms = e.timer_stop()
+        barrier()
+    finally:
+        clocks = sampler.stop() if rank == 0 else None
     launches = e.launch_count() - launches0
     loss_res, gn_res = e.read_scalars()
     require_finite("resident timed region", loss_res, gn_res)
+    if args.dump_outputs and rank == 0:
+        dump_train_outputs(args.dump_outputs, e, loss_res, gn_res)
 
     # ---- timed region 2: end to end through the host-buffer API ----
     barrier()
@@ -441,17 +445,15 @@ def run_ours(args):
         roofline=dict(bound="tensor", achieved=round(achieved, 1) if achieved else None,
                       peak=pk["sustained"], unit="TFLOP/s",
                       frac=round(achieved / pk["sustained"], 4) if achieved else None,
-                      # DRAM bytes of ONE launch (gate|up forward, M4096 N22016 K4096) read from the committed
-                      # `ncu --set full` capture; its algorithmic bytes are 394 MB (A 33.5 + B 180.4 + D 180.4)
-                      traffic=gemm_traffic()["bytes"], traffic_note=gemm_traffic()["note"],
-                      kernel="gemm_bf16_kernel (tcgen05)", launches=int(gemm_launches),
+                      traffic=None, traffic_note="not measured",
+                      kernel="gemm_bf16_kernel (wgmma)", launches=int(gemm_launches),
                       share_of_step=round(gemm_ms / ms_prof, 4), profiled_steps=n_prof,
-                      peak_source=f"{pk['source']} sustained cuBLAS bf16 (kernel timed inside a long step)"),
+                      peak_source=pk["source"]),
         model_flops=dict(per_token=FLOPS_PER_TOKEN,
                          achieved_tflops_per_gpu=round(value / world * FLOPS_PER_TOKEN / 1e12, 1),
                          frac_of_sustained_peak=round(value / world * FLOPS_PER_TOKEN / 1e12 / pk["sustained"], 4),
                          frac_of_burst_peak=round(value / world * FLOPS_PER_TOKEN / 1e12 / pk["burst"], 4)),
-        clocks=clocks, loss=round(float(loss), 4), grad_norm=round(float(gn), 4),
+        clocks=clocks, gpu=gpu_name(local), loss=round(float(loss), 4), grad_norm=round(float(gn), 4),
         device_gb=round(e.device_bytes() / 1e9, 1),
     )
     if per_rank:
@@ -468,7 +470,7 @@ def run_ours(args):
 # decode leg (BASELINE.json configs[3], SURVEY.md 8d second metric): Falcon-7B-Instruct layout,
 # random-init bf16 weights, batch 32, context 1024, greedy, through b200w_infer_step with HOST buffers
 # --------------------------------------------------------------------------------------------
-def decode_leg(device: int = 0, batch: int = 32, ctx: int = 1024, steps: int = 64, warm: int = 4):
+def decode_leg(device: int = 0, batch: int = 32, ctx: int = 1024, steps: int = 64, warm: int = 4, dump_dir=None):
     import numpy as np
 
     from runbooks_b200.infer import InferEngine, ServeArch
@@ -509,6 +511,9 @@ def decode_leg(device: int = 0, batch: int = 32, ctx: int = 1024, steps: int = 6
     ms = e.timer_stop()
     wall = (time.perf_counter() - t0) * 1e3
     launches = e.launch_count() - launches0
+    if dump_dir:   # the greedy tokens of the last timed decode step
+        os.makedirs(dump_dir, exist_ok=True)
+        np.save(os.path.join(dump_dir, "decode_tokens.npy"), np.asarray(tok, dtype=np.float64))
     n_params = sum(int(np.prod(s)) for _, s in e.infer_params())
     kv_bytes = batch * (ctx + warm + steps // 2) * arch.num_layers * 2 * arch.num_kv_heads * arch.head_dim * 2
     bytes_step = 2 * n_params + kv_bytes
@@ -516,7 +521,7 @@ def decode_leg(device: int = 0, batch: int = 32, ctx: int = 1024, steps: int = 6
     per = max(ms, wall) / steps
     e.close()
     return dict(
-        metric="Falcon-7B greedy decode tokens/s, batch 32, context 1024, 1xB200 (BASELINE.json configs[3])",
+        metric="Falcon-7B greedy decode tokens/s, batch 32, context 1024, 1xH100 (BASELINE.json configs[3])",
         value=round(batch / (per / 1e3), 1), unit="tokens/s", ms_per_step=round(per, 3),
         device_ms_per_step=round(ms / steps, 3), steps=steps, dtype="bf16", data="synthetic (random-init weights, random prompts)",
         e2e=dict(value=round(batch / (wall / steps / 1e3), 1), unit="tokens/s", h2d_bytes_per_step=3 * batch * 4,
@@ -526,9 +531,45 @@ def decode_leg(device: int = 0, batch: int = 32, ctx: int = 1024, steps: int = 6
                       frac=round(bytes_step / (per / 1e3) / 1e9 / pk["hbm"], 4), traffic=None,
                       algorithmic_bytes_per_step=int(bytes_step), params=n_params,
                       note="bytes = 2 x parameters (every weight read once per step, the tied embedding as lm_head) "
-                           "+ K/V of batch x context; peak = measured copy bandwidth (MEASURED_PEAKS.json)"),
+                           f"+ K/V of batch x context; peak: {pk['source']}"),
         prefill=dict(tokens=batch * ctx, seconds=round(prefill_s, 3), tokens_per_s=round(batch * ctx / prefill_s, 1),
                      note="one-pass prompt ingestion (b200w_infer_prefill), 4 calls of 8 x 1024 tokens"))
+
+
+DUMP_SAMPLE = 1 << 20   # updated-weight elements sampled per dumped tensor (4 MB of fp32 each)
+
+
+def dump_train_outputs(d: str, e, loss: float, gnorm: float):
+    """What the last timed step computed, as a caller of the step sees it: the loss and global gradient norm
+    it returned, and the weights it left (fp32 master and the bf16 copy the next forward reads) for one tensor
+    of each kind, sampled at fixed seeded positions. Same arguments -> same inputs -> comparable files."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "loss.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(d, "grad_norm.npy"), np.array([gnorm], dtype=np.float64))
+    shapes = dict(e.params())
+    rng = np.random.default_rng(0)
+    last = max(int(k.split(".")[2]) for k in shapes if k.startswith("model.layers."))
+    for name in ("model.embed_tokens.weight", "model.layers.0.self_attn.q_proj.weight",
+                 f"model.layers.{last}.mlp.down_proj.weight", "model.norm.weight", "lm_head.weight"):
+        shape = shapes[name]
+        n = int(np.prod(shape))
+        idx = np.sort(rng.choice(n, size=min(n, DUMP_SAMPLE), replace=False))
+        key = name.replace("model.", "").replace(".weight", "").replace(f"layers.{last}.", "layers.last.").replace(".", "_")
+        np.save(os.path.join(d, f"master_{key}.npy"), e.read_state(name, shape, "master").reshape(-1)[idx].astype(np.float32))
+        bits = e.read_tensor(name, shape, bf16_bits=True).reshape(-1)[idx].astype(np.uint32) << 16   # bf16 -> fp32, exact
+        np.save(os.path.join(d, f"weight_{key}.npy"), bits.view(np.float32))
+
+
+def gpu_name(device: int) -> dict:
+    """The card a number was measured on: its name and power limit (read-only nvidia-smi query)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
+                              "-i", str(device)], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clk = (c.strip() for c in out.split(","))
+        return dict(name=name, power_limit=power, sm_max_clock=clk)
+    except Exception:  # noqa: BLE001
+        return dict(name=None, power_limit=None, sm_max_clock=None)
 
 
 _REAL_STDOUT = None
@@ -571,6 +612,9 @@ def main():
     ap.add_argument("--shard-state", action="store_true", default=bool(os.environ.get("B200W_SHARD_STATE")),
                     help="N>1: fp32 master / Adam moments sharded over the ranks (reduce-scatter + all-gather)")
     ap.add_argument("--decode-only", action="store_true", help="run only the decode leg and print its object")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy: loss, grad norm "
+                         "and a fixed seeded sample of the updated weights (and the decode leg's last tokens)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     MICRO_BATCH = args.micro_batch
@@ -579,11 +623,10 @@ def main():
     # A rank that fails must EXIT, at once: its peers are inside a collective that can no longer
     # complete, and the launcher only tears the job down when a worker process ends. Interpreter
     # teardown (destructors -> NCCL / CUDA shutdown on a dead context) can block, so skip it.
-    # (profiles/r01_n8_failure.txt: one rank raised, did not exit, and 7 GPUs spun for 10 minutes.)
     code = 0
     try:
         if args.decode_only:
-            emit(decode_leg(int(os.environ.get("LOCAL_RANK", "0"))))
+            emit(decode_leg(int(os.environ.get("LOCAL_RANK", "0")), dump_dir=args.dump_outputs))
         elif args.impl == "reference":
             run_reference(args)
         else:

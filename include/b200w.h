@@ -1,4 +1,4 @@
-/* b200w — C ABI of the B200-native fine-tune / serve worker.
+/* b200w — C ABI of the Hopper-native (H100, sm_90a) fine-tune / serve worker.
  *
  * The reference (substratusai/runbooks) is a Go operator with no FFI of its own: its boundary to
  * the hot path is the container contract (docs/container-contract.md) and the Pod spec built by
@@ -6,7 +6,7 @@
  * internal/controller/server_controller.go:114-205 (server Deployment). The arithmetic lives in
  * the un-vendored trainer image (examples/llama2-7b/finetuned-model.yaml:6). This header is the
  * C boundary a Go host (cgo), the Python host in runbooks_b200/ (ctypes) or a C++ host binds to
- * in order to run that arithmetic on a B200; INTEGRATION.md shows each binding.
+ * in order to run that arithmetic on an H100; INTEGRATION.md shows each binding.
  *
  * Conventions (SURVEY.md §8b): extern "C"; opaque context; every function returns 0 on success
  * and a negative b200w_status on failure, with b200w_last_error() giving the message; no C++
@@ -212,7 +212,7 @@ B200W_API int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int3
  * as padding after them), lengths[n_seqs] in 1..min(padded_len, max_ctx), padded_len a multiple of 128.
  * K/V of the real positions land in cache slots[b] at positions [0, lengths[b]); next_tokens (HOST,
  * n_seqs) = greedy token after each prompt; logits_out HOST float [n_seqs, vocab] or NULL. Runs the
- * big-M tcgen05 GEMMs and the flash-attention forward of the fine-tune path instead of `length`
+ * big-M wgmma GEMMs and the flash-attention forward of the fine-tune path instead of `length`
  * sweeps over the weights. Decode continues with b200w_infer_step at position lengths[b]. */
 B200W_API int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* lengths,
                         const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
@@ -279,7 +279,7 @@ B200W_API int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, 
                    int step, float gscale);
 /* returns sqrt(sum g^2) in *norm_out (HOST) */
 B200W_API int b200w_op_grad_norm(b200w_ctx* ctx, const void* g, int g_bf16, int64_t n, float* norm_out);
-/* Robustness hook: overwrites ALL shared memory (227 KB) and all 512 TMEM columns of every SM with
+/* Robustness hook: overwrites ALL shared memory a block may use (227 KB) on every SM with
  * `pattern` (e.g. 0x7FC07FC0: NaN as bf16 pairs and as fp32). A kernel may never depend on on-chip
  * state left by whatever ran before it (another library's kernel, e.g. NCCL's, leaves arbitrary
  * bits there): tests poison, run an op, and require results bit-identical to the clean run. */

@@ -1,4 +1,4 @@
-"""runbooks_b200 — B200-native (sm_100a) fine-tune worker behind the substratus container contract.
+"""runbooks_b200 — Hopper-native (H100, sm_90a) fine-tune worker behind the substratus container contract.
 
 Only what the hot path needs lives here: csrc/ (CUDA kernels + the C ABI of include/b200w.h),
 _lib.py (ctypes binding), engine.py (host wrapper), worker.py (container-contract entry point).

@@ -1,28 +1,22 @@
-// Causal flash attention forward / backward on tcgen05 (sm_100a), head_dim = 128.
+// Causal flash attention forward / backward on Hopper tensor cores (sm_90a wgmma), head_dim = 128.
 // Oracle: F.scaled_dot_product_attention(q, k, v, is_causal=True) as called by HF
 // LlamaAttention with _attn_implementation == "sdpa" (SURVEY.md §8 a7).
 //
-// Common structure of the three kernels (CTA = 10 warps):
-//   warp 9        TMA producer (lane 0): every load, gated by per-buffer "free" mbarriers;
-//   warp 8        MMA issuer (lane 0): a lean in-order stream of tcgen05.mma with precomputed
-//                 descriptor words (profiles/r01_ncu_attention_v3.txt: a single control thread doing
-//                 both jobs executed ~380 SASS instructions per block and WAS the bottleneck);
-//   warps 0..7    compute: a TMEM lane is a matrix row; warp w touches lane quarter (w & 3) and
-//                 column half (w >> 2) of each 64-column score block, i.e. TWO threads per row, so
-//                 every SM sub-partition has >= 2 warps of MUFU/FMA work to overlap;
-//   handoffs      mbarriers only (tcgen05.commit -> compute, 256-thread arrive -> control).
-// The score MMAs of block i+1 are issued before the compute warps start block i (double-buffered
-// TMEM), so the tensor pipe runs under the softmax instead of after it.
+// Common structure of the three kernels (CTA = 9 warps):
+//   warp 8        TMA producer (lane 0): every load, gated by per-buffer "free" mbarriers;
+//   warps 0..7    two consumer warpgroups; warpgroup wg owns 64 rows of the CTA's 128-row tile and keeps
+//                 its scores and accumulators in registers. A row's scores live in the 4 threads of a
+//                 lane quad (wgmma accumulator layout, ptx.cuh), so row reductions are two shuffles, and
+//                 the bf16 probabilities feed the second product as the register A operand -- P and dS
+//                 never go through shared memory.
+//   handoffs      full barriers (TMA bytes) and free barriers (one arrival per consumer warp).
 //
-// forward       CTA = (128-query tile, head, sequence), 64-key blocks, 2 CTAs / SM:
-//                 S = Q K^T -> TMEM;  P = 2^(S - m) -> smem bf16 (SW128 K-major)
-//                 O += P V accumulated IN TMEM; rescaled (tcgen05.ld/st) only when the running max
-//                 grows by more than 2^8 ("lazy rescale"); the final O / l is exact either way.
-// backward dKdV CTA = (128-key block, kv head, sequence), 64-query blocks, transposed form:
-//                 S^T = K Q^T, dP^T = V dO^T -> TMEM;  P^T, dS^T -> smem;
-//                 dV += P^T dO,  dK += dS^T Q   (TMEM accumulators across the whole loop)
+// forward       CTA = (128-query tile, head, sequence), 64-key blocks:
+//                 S = Q K^T;  P = 2^(S - m) (online softmax);  O = O * alpha + P V
+// backward dKdV CTA = (128-key block, kv head, sequence), 64-query blocks in four 16-query slices,
+//                 transposed form: S^T = K Q^T, dP^T = V dO^T;  dV += P^T dO,  dK += dS^T Q
 // backward dQ   CTA = (128-query tile, head, sequence), 64-key blocks: S, dP recomputed,
-//                 dQ += dS K accumulated in TMEM — no global atomics, no fp32 staging buffer.
+//                 dQ += dS K -- no global atomics, no fp32 staging buffer.
 #include "host_common.h"
 #include "ops.h"
 #include "ptx.cuh"
@@ -35,9 +29,9 @@ using bf16 = __nv_bfloat16;
 constexpr int DH = 128;
 constexpr int ATOM64 = 64 * 128;    // bytes of a [64 rows x 128 B] swizzle-atom column
 constexpr int ATOM128 = 128 * 128;  // bytes of a [128 rows x 128 B] one
-constexpr int NCOMPUTE = 256;
-constexpr int NTHREADS = 320;  // 8 compute warps + MMA warp (8) + TMA warp (9)
-constexpr float LAZY_RESCALE_LOG2 = 8.f;
+constexpr int NTHREADS = 288;       // 2 consumer warpgroups + TMA warp (8)
+constexpr int TMA_WARP = 8;
+constexpr int NCONSUMER_WARPS = 8;
 
 __device__ __forceinline__ void require_1024_aligned(const void* p) {
   if (smem_u32(p) & 1023u) {
@@ -45,176 +39,56 @@ __device__ __forceinline__ void require_1024_aligned(const void* p) {
     __trap();
   }
 }
-// B200W_WHATIF_* macros build TIMING-ONLY variants (wrong numerics) for same-box what-if experiments
-// (tools/build_variant.sh, tools/ab_variants.sh); none is defined in the product build.
 __device__ __forceinline__ float ex2(float x) {  // one MUFU.EX2
-#ifdef B200W_WHATIF_NOEXP
-  return fmaf(x, 1e-3f, 1.f);   // what if the exponentials were free
-#else
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-#endif
 }
-__device__ __forceinline__ void compute_bar_sync() {  // the 256 compute threads only (forward)
-  asm volatile("bar.sync 1, 256;" ::: "memory");
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-// The backward kernels use 16 compute warps (4 threads per row, 16 score columns each): with 2
-// warps per SM sub-partition their ~370-instruction block body ran at 6 cycles per instruction
-// (profiles/r01_ncu_attention_v6.txt) and set the pace instead of the tensor pipe.
-constexpr int BWD_NCOMPUTE = 512;
-constexpr int BWD_NTHREADS = 576;  // + MMA warp (16) + TMA warp (17)
-__device__ __forceinline__ void bwd_compute_bar_sync() {
-  asm volatile("bar.sync 1, 512;" ::: "memory");
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// 32 fp32 TMEM columns of this thread's lane -> bf16 in global memory
-__device__ __forceinline__ void tmem_row32_to_global(uint32_t taddr, __nv_bfloat16* dst) {
-  uint32_t r[32];
-  tmem_ld32(taddr, r);
-  tmem_ld_wait();
+// fp32 accumulator columns [16 kk, 16 kk + 16) -> the bf16 A fragment of the kk-th K = 16 slice
+template <int R>
+__device__ __forceinline__ void to_afrag(const float (&s)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+  a[1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+  a[2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+  a[3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+}
+// one free-barrier arrival per consumer warp, after its warpgroup's MMAs that read the buffer retired
+__device__ __forceinline__ void warp_release(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+// D[64 x N] = A[64 x dh] B[N x dh]^T, both K-major with the two dh halves `a_atom` / `b_atom` bytes apart
+template <int N, int R>
+__device__ __forceinline__ void mma_over_dh(float (&d)[R], uint32_t a_addr, uint32_t a_atom, uint32_t b_addr,
+                                            uint32_t b_atom) {
+  const uint64_t da = wg_desc(a_addr, 16), db = wg_desc(b_addr, 16);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    uint4 u;
-    u.x = pack_bf16x2(__uint_as_float(r[i * 8 + 0]), __uint_as_float(r[i * 8 + 1]));
-    u.y = pack_bf16x2(__uint_as_float(r[i * 8 + 2]), __uint_as_float(r[i * 8 + 3]));
-    u.z = pack_bf16x2(__uint_as_float(r[i * 8 + 4]), __uint_as_float(r[i * 8 + 5]));
-    u.w = pack_bf16x2(__uint_as_float(r[i * 8 + 6]), __uint_as_float(r[i * 8 + 7]));
-    reinterpret_cast<uint4*>(dst)[i] = u;
-  }
+  for (int kk = 0; kk < DH / 16; ++kk)
+    Wgmma<N>::template ss<0, 0>(d, desc_add(da, (kk / 4) * a_atom + (kk % 4) * 32),
+                                desc_add(db, (kk / 4) * b_atom + (kk % 4) * 32), kk != 0);
 }
-
-// The MMA-issuing thread is a single in-order instruction stream: everything it executes per
-// MMA delays the tensor pipe. Descriptors are therefore kept as precomputed 32-bit halves — the
-// high word is a constant per layout, the low word is (smem address >> 4) | LBO field, and
-// stepping along K is one integer add.
-constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO 1024, version 1, SW128
-__device__ __forceinline__ uint32_t desc_lo_k(uint32_t smem_addr) {   // K-major (LBO unused = 16)
-  return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-__device__ __forceinline__ uint32_t desc_lo_mn(uint32_t smem_addr) {  // MN-major, atoms ATOM64 apart
-  return ((smem_addr & 0x3FFFFu) >> 4) | ((ATOM64 >> 4) << 16);
-}
-// The MMA warp runs its loop CONVERGENTLY (all 32 lanes: loop control, barrier waits, descriptor
-// arithmetic — ptxas keeps all of it in uniform registers) and each tcgen05 instruction is
-// guarded by an `elect.sync` predicate inside the same asm block, so exactly one lane issues.
-// With the issue code inside an `if (lane == 0)` region ptxas instead wrapped every UTCHMMA in an
-// ELECT / BRA.U.ANY loop with R2UR moves (~12 instructions per MMA) and the issuing thread, not
-// the tensor pipe, paced the kernels (profiles/r01_ncu_attention_v7.txt).
-template <bool ACC>
-__device__ __forceinline__ void mma_raw(bool, uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(DESC_HI), "r"(idesc), "r"(ACC ? 1u : 0u)
-      : "memory");
-}
-__device__ __forceinline__ void mma_raw_dyn(bool, uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo,
-                                            uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(DESC_HI), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// A operand from TMEM (bf16 pairs, 8 columns per K = 16 step; lane = row), B from smem.
-// Used by the dQ kernel for Q, dO (constant per CTA) and dS (written by the compute warps with
-// tcgen05.st over the dP columns they just consumed). Measured effect (same-box ncu A/B,
-// profiles/r01_attn_ab_v9.txt): kernel 234 -> 212 us with the tensor-core smem pipe at 25 % busy,
-// i.e. smem bandwidth was NOT the binding limit; the per-block softmax/dS phase of the compute
-// warps is (DESIGN.md 3.2).
-template <bool ACC>
-__device__ __forceinline__ void mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(b_lo), "r"(DESC_HI), "r"(idesc), "r"(ACC ? 1u : 0u)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ts_dyn(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t idesc,
-                                           uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(b_lo), "r"(DESC_HI), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// D = A[128 x dh, TMEM] * B[K-major, 2 atoms `b_atom16` apart]^T : 8 MMAs, the first overwrites
-__device__ __forceinline__ void mma_ts_kmajor_dh(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo,
-                                                 uint32_t b_atom16, uint32_t idesc) {
-  mma_ts<false>(tmem_d, tmem_a, b_lo, idesc);
+// D[64 x dh] += A (registers, KS slices of K = 16) * B[K rows x dh], B MN-major with the two dh atoms ATOM64 apart
+template <int KS>
+__device__ __forceinline__ void mma_pv(float (&d)[64], const uint32_t (&a)[KS][4], uint32_t b_addr) {
+  const uint64_t db = wg_desc(b_addr, ATOM64);
 #pragma unroll
-  for (int k = 1; k < DH / 16; ++k)
-    mma_ts<true>(tmem_d, tmem_a + k * 8, b_lo + (k / 4) * b_atom16 + (k % 4) * 2, idesc);
+  for (int kk = 0; kk < KS; ++kk) Wgmma<DH>::template rs<1>(d, a[kk], desc_add(db, kk * 2048), 1u);
 }
-// D (+)= A[128 x 64, TMEM] * B[MN-major: N = dh (2 atoms, ATOM64 apart), K = 64 rows] : 4 MMAs
-__device__ __forceinline__ void mma_ts_a64_bmn(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t idesc,
-                                               uint32_t accumulate_first) {
-  mma_ts_dyn(tmem_d, tmem_a, b_lo, idesc, accumulate_first);
+// 64 fp32 accumulator registers (a 64 x 128 tile of the warpgroup) * mul -> bf16 rows r and r + 8 of `base`
+__device__ __forceinline__ void store_rows_bf16(const float (&o)[64], bf16* row0, bf16* row1, float mul0, float mul1) {
+  const int c = 2 * (threadIdx.x & 3);
 #pragma unroll
-  for (int k = 1; k < 4; ++k) mma_ts<true>(tmem_d, tmem_a + k * 8, b_lo + k * (2048 >> 4), idesc);
-}
-
-// K-major x K-major over dh = 128: operands are 2 atoms along the contraction, `*_atom16` apart
-// (in 16-byte units). a_lo / b_lo: desc_lo_k() of the first atom. 8 MMAs, the first overwrites.
-__device__ __forceinline__ void mma_kmajor_dh(bool leader, uint32_t tmem_d, uint32_t a_lo,
-                                              uint32_t a_atom16, uint32_t b_lo, uint32_t b_atom16,
-                                              uint32_t idesc) {
-  mma_raw<false>(leader, tmem_d, a_lo, b_lo, idesc);
-#pragma unroll
-  for (int k = 1; k < DH / 16; ++k)
-    mma_raw<true>(leader, tmem_d, a_lo + (k / 4) * a_atom16 + (k % 4) * 2,
-                  b_lo + (k / 4) * b_atom16 + (k % 4) * 2, idesc);
-}
-// D (+)= A[128 x 64, K-major, one atom] * B[MN-major: N = dh (2 atoms, ATOM64 apart), K = 64 rows]
-// a_lo: desc_lo_k(A), b_lo: desc_lo_mn(B). 4 MMAs.
-__device__ __forceinline__ void mma_a64_bmn(bool leader, uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo,
-                                            uint32_t idesc, uint32_t accumulate_first) {
-  mma_raw_dyn(leader, tmem_d, a_lo, b_lo, idesc, accumulate_first);
-#pragma unroll
-  for (int k = 1; k < 4; ++k) mma_raw<true>(leader, tmem_d, a_lo + k * 2, b_lo + k * (2048 >> 4), idesc);
-}
-// convergent: one elected lane commits
-__device__ __forceinline__ void commit_if(bool, uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-__device__ __forceinline__ uint4 pack8(const float (&p)[8]) {
-  uint4 u;
-  u.x = pack_bf16x2(p[0], p[1]); u.y = pack_bf16x2(p[2], p[3]);
-  u.z = pack_bf16x2(p[4], p[5]); u.w = pack_bf16x2(p[6], p[7]);
-  return u;
-}
-// 64 fp32 TMEM columns [col0, col0+64) of this thread's lane -> bf16 row in global memory
-__device__ __forceinline__ void tmem_row64_to_global(uint32_t taddr, bf16* dst, float mul) {
-#pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    uint32_t r[32];
-    tmem_ld32(taddr + c * 32, r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float o8[8] = {__uint_as_float(r[i * 8 + 0]) * mul, __uint_as_float(r[i * 8 + 1]) * mul,
-                           __uint_as_float(r[i * 8 + 2]) * mul, __uint_as_float(r[i * 8 + 3]) * mul,
-                           __uint_as_float(r[i * 8 + 4]) * mul, __uint_as_float(r[i * 8 + 5]) * mul,
-                           __uint_as_float(r[i * 8 + 6]) * mul, __uint_as_float(r[i * 8 + 7]) * mul};
-      reinterpret_cast<uint4*>(dst + c * 32)[i] = pack8(o8);
-    }
+  for (int j = 0; j < 16; ++j) {
+    *reinterpret_cast<uint32_t*>(row0 + 8 * j + c) = pack_bf16x2(o[4 * j] * mul0, o[4 * j + 1] * mul0);
+    *reinterpret_cast<uint32_t*>(row1 + 8 * j + c) = pack_bf16x2(o[4 * j + 2] * mul1, o[4 * j + 3] * mul1);
   }
 }
 
@@ -222,16 +96,9 @@ __device__ __forceinline__ void tmem_row64_to_global(uint32_t taddr, bf16* dst, 
 // forward
 // ==========================================================================================
 constexpr int FWD_BQ = 128, FWD_BKV = 64;
-#ifdef B200W_WHATIF_1CTA
-constexpr int FWD_WHATIF_PAD = 100 * 1024;   // what if only one forward CTA were resident per SM
-#else
-constexpr int FWD_WHATIF_PAD = 0;
-#endif
-constexpr int FWD_SMEM = FWD_WHATIF_PAD + 2 * ATOM128 /*Q*/ + 2 * 2 * ATOM64 /*K x2*/ + 2 * 2 * ATOM64 /*V x2*/ +
-                         ATOM128 /*P*/ + 256 /*barriers*/;
-constexpr int FWD_TMEM_COLS = 256;  // S[2]: [0,64) [64,128)   O: [128,256)
+constexpr int FWD_SMEM = 2 * ATOM128 /*Q*/ + 2 * 2 * ATOM64 /*K x2*/ + 2 * 2 * ATOM64 /*V x2*/ + 256 /*barriers*/;
 
-__global__ void __launch_bounds__(NTHREADS, 2)
+__global__ void __launch_bounds__(NTHREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, int ld_out,
                 float* __restrict__ lse2, int k_off, int v_off, int B, int S, int H, int Hkv,
                 float scale_log2) {
@@ -240,15 +107,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   uint8_t* sQ = smem;                      // 2 atoms (dh halves) x [128 x 128 B]
   uint8_t* sK = sQ + 2 * ATOM128;          // 2 bufs x 2 atoms x [64 x 128 B]
   uint8_t* sV = sK + 2 * 2 * ATOM64;       // 2 bufs x 2 atoms x [64 kv rows x 128 B]
-  uint8_t* sP = sV + 2 * 2 * ATOM64;       // [128 x 128 B]
-  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sP + ATOM128);
-  uint64_t* bar_k = bar_q + 1;  // [2]
-  uint64_t* bar_v = bar_k + 2;  // [2]
-  uint64_t* bar_s = bar_v + 2;  // [2] S(j) in TMEM
-  uint64_t* bar_o = bar_s + 2;  //     PV(j) retired
-  uint64_t* bar_p = bar_o + 1;  //     P(j) in smem (256 arrivals)
-  uint64_t* bar_vfree = bar_p + 1;  // [2] PV that read V buffer b retired (for the TMA warp)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_vfree + 2);
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + 2 * 2 * ATOM64);
+  uint64_t* bar_k = bar_q + 1;      // [2]
+  uint64_t* bar_v = bar_k + 2;      // [2]
+  uint64_t* bar_kfree = bar_v + 2;  // [2] the S MMAs that read K buffer b retired
+  uint64_t* bar_vfree = bar_kfree + 2;  // [2] the PV MMAs that read V buffer b retired
 
   const int nq = S / FWD_BQ;
   const int bh = blockIdx.x % (B * H);
@@ -266,225 +129,146 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
     for (int i = 0; i < 2; ++i) {
       mbar_init(&bar_k[i], 1);
       mbar_init(&bar_v[i], 1);
-      mbar_init(&bar_s[i], 1);
-      mbar_init(&bar_vfree[i], 1);
+      mbar_init(&bar_kfree[i], NCONSUMER_WARPS);
+      mbar_init(&bar_vfree[i], NCONSUMER_WARPS);
     }
-    mbar_init(bar_o, 1);
-    mbar_init(bar_p, NCOMPUTE / 32);
     fence_barrier_init();
   }
-  if (warp == 8) tmem_alloc(tmem_slot, FWD_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_O = tmem_base + 128;
 
-  if (warp == 9) {
-    // =============================== TMA producer ===============================
+  if (warp == TMA_WARP) {
     if (lane == 0) {
-      auto load_k = [&](int j) {
-        const int buf = j & 1;
-        mbar_arrive_expect_tx(&bar_k[buf], 2 * ATOM64);
-#pragma unroll
-        for (int a = 0; a < 2; ++a)
-          tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_k[buf], k_off + hk * DH + a * 64,
-                      tok0 + j * FWD_BKV);
-      };
-      auto load_v = [&](int j) {
-        const int buf = j & 1;
-        mbar_arrive_expect_tx(&bar_v[buf], 2 * ATOM64);
-#pragma unroll
-        for (int a = 0; a < 2; ++a)
-          tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_v[buf], v_off + hk * DH + a * 64,
-                      tok0 + j * FWD_BKV);
-      };
       mbar_arrive_expect_tx(bar_q, 2 * ATOM128);
 #pragma unroll
       for (int a = 0; a < 2; ++a)
 #pragma unroll
         for (int r = 0; r < 2; ++r)
-          tma_load_2d(sQ + a * ATOM128 + r * ATOM64, &tm_qkv, bar_q, h * DH + a * 64,
-                      tok0 + q0 + r * 64);
-      load_k(0);
-      load_v(0);
-      load_k(1);  // njb >= 2 always
-      load_v(1);
-      for (int j = 0; j + 2 < njb; ++j) {
-        const int buf = j & 1;
-        mbar_wait(&bar_s[buf], (j >> 1) & 1);      // S(j) retired: its K buffer is free
-        load_k(j + 2);
-        mbar_wait(&bar_vfree[buf], (j >> 1) & 1);  // PV(j) retired: its V buffer is free
-        load_v(j + 2);
-      }
-    }
-  } else if (warp == 8) {
-    // =============================== MMA issuer ===============================
-    {  // the whole warp runs this loop; only `leader` issues
-      const bool leader = lane == 0;
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, FWD_BKV, false, false);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, DH, false, true);
-      constexpr uint32_t BUF16 = (2 * ATOM64) >> 4, A128 = ATOM128 >> 4, A64 = ATOM64 >> 4;
-      const uint32_t q_lo = desc_lo_k(smem_u32(sQ)), k_lo = desc_lo_k(smem_u32(sK));
-      const uint32_t p_lo = desc_lo_k(smem_u32(sP)), v_lo = desc_lo_mn(smem_u32(sV));
-      mbar_wait(bar_q, 0);
-      mbar_wait(&bar_k[0], 0);
-      tc_fence_after();
-      mma_kmajor_dh(leader, tmem_base, q_lo, A128, k_lo, A64, idesc_s);  // S(0)
-      commit_if(leader, &bar_s[0]);
+          tma_load_2d(sQ + a * ATOM128 + r * ATOM64, &tm_qkv, bar_q, h * DH + a * 64, tok0 + q0 + r * 64);
       for (int j = 0; j < njb; ++j) {
-        const uint32_t buf = j & 1;
-        if (j + 1 < njb) {  // S buffer buf^1 was drained by the compute warps before bar_p(j-1)
-          mbar_wait(&bar_k[buf ^ 1], ((j + 1) >> 1) & 1);
-          tc_fence_after();
-          mma_kmajor_dh(leader, tmem_base + (buf ^ 1) * 64, q_lo, A128, k_lo + (buf ^ 1) * BUF16, A64, idesc_s);
-          commit_if(leader, &bar_s[buf ^ 1]);
-        }
-        mbar_wait(bar_p, j & 1);  // P(j) written (and S(j) drained)
-        mbar_wait(&bar_v[buf], (j >> 1) & 1);
-        tc_fence_after();
-        mma_a64_bmn(leader, tmem_O, p_lo, v_lo + buf * BUF16, idesc_o, j != 0);
-        commit_if(leader, bar_o);
-        commit_if(leader, &bar_vfree[buf]);
+        const int buf = j & 1;
+        if (j >= 2) mbar_wait(&bar_kfree[buf], ((j >> 1) - 1) & 1);
+        mbar_arrive_expect_tx(&bar_k[buf], 2 * ATOM64);
+#pragma unroll
+        for (int a = 0; a < 2; ++a)
+          tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_k[buf], k_off + hk * DH + a * 64, tok0 + j * FWD_BKV);
+        if (j >= 2) mbar_wait(&bar_vfree[buf], ((j >> 1) - 1) & 1);
+        mbar_arrive_expect_tx(&bar_v[buf], 2 * ATOM64);
+#pragma unroll
+        for (int a = 0; a < 2; ++a)
+          tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_v[buf], v_off + hk * DH + a * 64, tok0 + j * FWD_BKV);
       }
     }
-  } else {
-    // =============================== compute ===============================
-    const int q = warp & 3, hc = warp >> 2;
-    const int row_local = q * 32 + lane;   // TMEM lane == query row inside the tile
-    const int row_seq = q0 + row_local;    // query position inside the sequence
-    const uint32_t lane_base = (q * 32u) << 16;
-    float m_used = -INFINITY, l_part = 0.f;  // l_part: this thread's half of the row sum
-
-    for (int j = 0; j < njb; ++j) {
-      const int buf = j & 1;
-      mbar_wait(&bar_s[buf], (j >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      // the whole 64-column row is needed for the row max (both half-row threads derive the same one), but
-      // only `mine` is exponentiated: two separately named arrays, selected by ADDRESS (hc), keep everything
-      // in registers (round 1 indexed sr[hc] dynamically, which ptxas put in local memory: 44 B of spills)
-      uint32_t mine[32], other[32];
-      tmem_ld32(tmem_base + buf * 64 + lane_base + hc * 32, mine);
-#ifdef B200W_WHATIF_NOOTHER
-#pragma unroll
-      for (int c = 0; c < 32; ++c) other[c] = 0u;   // what if the row maximum needed only this thread's half
-#else
-      tmem_ld32(tmem_base + buf * 64 + lane_base + (hc ^ 1) * 32, other);
-#endif
-      tmem_ld_wait();
-
-      const int col0 = j * FWD_BKV;
-      const bool diag = (col0 + FWD_BKV - 1) > q0;  // block reaches past the first row's diagonal
-      float mx = -INFINITY;
-      if (diag) {
-        const int cm = col0 + hc * 32, co = col0 + (hc ^ 1) * 32;
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          float sm_ = __uint_as_float(mine[c]);
-          if (cm + c > row_seq) sm_ = -INFINITY;
-          mine[c] = __float_as_uint(sm_);
-          float so_ = __uint_as_float(other[c]);
-          if (co + c > row_seq) so_ = -INFINITY;
-          mx = fmaxf(mx, fmaxf(sm_, so_));
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mx = fmaxf(mx, fmaxf(__uint_as_float(mine[c]), __uint_as_float(other[c])));
-      }
-      mx *= scale_log2;  // scale > 0, so max commutes with it
-      // lazy rescale: keep the old reference max unless the new one is > 2^8 above it. Block 0 always
-      // sets it (column 0 is visible to every row), so m_used is finite from then on.
-      const bool grow = mx > m_used + LAZY_RESCALE_LOG2;
-      const float m_new = grow ? mx : m_used;
-      const float alpha = grow ? ex2(m_used - m_new) : 1.f;
-      uint4 pk[4];
-      float psum = 0.f;
-#pragma unroll
-      for (int c8 = 0; c8 < 4; ++c8) {
-        float p8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          p8[e] = ex2(fmaf(__uint_as_float(mine[c8 * 8 + e]), scale_log2, -m_new));
-          psum += p8[e];
-        }
-        pk[c8] = pack8(p8);
-      }
-      l_part = l_part * alpha + psum;
-      m_used = m_new;
-
-      if (j > 0) {
-        mbar_wait(bar_o, (j - 1) & 1);  // PV(j-1) retired: P smem and O are free
-        __syncwarp();
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, grow)) {  // rare after the first blocks; my 64 of O's columns
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {  // 16 columns at a time: pk[] is live across this, registers are tight
-            uint32_t r[16];
-            tmem_ld16(tmem_O + lane_base + hc * 64 + c * 16, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-            tmem_st16(tmem_O + lane_base + hc * 64 + c * 16, r);
-          }
-          tmem_st_wait();
-        }
-      }
-#pragma unroll
-      for (int c8 = 0; c8 < 4; ++c8)
-        *reinterpret_cast<uint4*>(sP + sw128_offset(row_local, hc * 4 + c8)) = pk[c8];
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();                      // orders the other 31 lanes' writes before lane 0's arrive
-      if (lane == 0) mbar_arrive(bar_p);  // one arrival per compute warp (round 1: one per thread)
-    }
-
-    mbar_wait(bar_o, (njb - 1) & 1);
-    __syncwarp();
-    tc_fence_after();
-    // combine the two half-row sums through smem (P is dead now)
-    float* sL = reinterpret_cast<float*>(sP);
-    sL[hc * 128 + row_local] = l_part;
-    compute_bar_sync();
-    const float l_row = l_part + sL[(hc ^ 1) * 128 + row_local];
-    bf16* orow = out + static_cast<size_t>(tok0 + row_seq) * ld_out + h * DH + hc * 64;
-    tmem_row64_to_global(tmem_O + lane_base + hc * 64, orow, 1.f / l_row);
-    if (hc == 0)
-      lse2[static_cast<size_t>(h) * (static_cast<size_t>(B) * S) + tok0 + row_seq] =
-          m_used + log2f(l_row);
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, FWD_TMEM_COLS);
+  // =============================== consumers ===============================
+  const int wg = warp >> 2, wi = warp & 3;
+  const int row0 = q0 + wg * 64 + wi * 16 + (lane >> 2);  // query positions of this thread's two rows
+  const int row1 = row0 + 8;
+  const int last_j = 2 * qi + wg;  // the last key block that holds a key <= this warpgroup's last row
+  const uint32_t q_addr = smem_u32(sQ) + wg * ATOM64;
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  mbar_wait(bar_q, 0);
+
+  for (int j = 0; j < njb; ++j) {
+    const int buf = j & 1;
+    if (j > last_j) {  // fully masked for every row of this warpgroup: nothing to compute, but the release waits
+      // for the block's loads, so that each warp's arrival counts toward this block's phase and never toward the
+      // phase of the block before it in the same buffer (a warp running ahead would otherwise free that buffer
+      // while another warp of the warpgroup still reads it)
+      mbar_wait(&bar_k[buf], (j >> 1) & 1);
+      warp_release(&bar_kfree[buf]);
+      mbar_wait(&bar_v[buf], (j >> 1) & 1);
+      warp_release(&bar_vfree[buf]);
+      continue;
+    }
+    float s[32];
+    mbar_wait(&bar_k[buf], (j >> 1) & 1);
+    wg_fence();
+    mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(s);
+    warp_release(&bar_kfree[buf]);
+
+    const int col0 = j * FWD_BKV + 2 * (lane & 3);
+    if (j * FWD_BKV + FWD_BKV - 1 > q0 + wg * 64) {  // the block reaches past the first row's diagonal
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * jj + e;
+          if (col > row0) s[4 * jj + e] = -INFINITY;
+          if (col > row1) s[4 * jj + 2 + e] = -INFINITY;
+        }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+      mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
+    }
+    // scale > 0, so max commutes with it; block 0 holds key 0, visible to every row, so m is finite from then on
+    const float mn0 = fmaxf(m0, quad_max(mx0) * scale_log2), mn1 = fmaxf(m1, quad_max(mx1) * scale_log2);
+    const float alpha0 = ex2(m0 - mn0), alpha1 = ex2(m1 - mn1);
+    m0 = mn0;
+    m1 = mn1;
+    float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      s[4 * jj] = ex2(fmaf(s[4 * jj], scale_log2, -mn0));
+      s[4 * jj + 1] = ex2(fmaf(s[4 * jj + 1], scale_log2, -mn0));
+      s[4 * jj + 2] = ex2(fmaf(s[4 * jj + 2], scale_log2, -mn1));
+      s[4 * jj + 3] = ex2(fmaf(s[4 * jj + 3], scale_log2, -mn1));
+      ps0 += s[4 * jj] + s[4 * jj + 1];
+      ps1 += s[4 * jj + 2] + s[4 * jj + 3];
+    }
+    l0 = l0 * alpha0 + ps0;  // this thread's part of the row sums (the quad's alphas are equal)
+    l1 = l1 * alpha1 + ps1;
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, pa[kk]);
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      o[4 * jj] *= alpha0;
+      o[4 * jj + 1] *= alpha0;
+      o[4 * jj + 2] *= alpha1;
+      o[4 * jj + 3] *= alpha1;
+    }
+    mbar_wait(&bar_v[buf], (j >> 1) & 1);
+    wg_fence();
+    mma_pv<4>(o, pa, smem_u32(sV + buf * 2 * ATOM64));
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(o);
+    warp_release(&bar_vfree[buf]);
+  }
+
+  l0 = quad_sum(l0);
+  l1 = quad_sum(l1);
+  bf16* orow0 = out + static_cast<size_t>(tok0 + row0) * ld_out + h * DH;
+  bf16* orow1 = out + static_cast<size_t>(tok0 + row1) * ld_out + h * DH;
+  store_rows_bf16(o, orow0, orow1, 1.f / l0, 1.f / l1);
+  if ((lane & 3) == 0) {
+    float* lrow = lse2 + static_cast<size_t>(h) * (static_cast<size_t>(B) * S) + tok0;
+    lrow[row0] = m0 + log2f(l0);
+    lrow[row1] = m1 + log2f(l1);
   }
 }
 
 // ==========================================================================================
 // backward, part 1: dK, dV
 // ==========================================================================================
-constexpr int BWD_BKV = 128, BWD_BQ = 64;
-constexpr int KV_SMEM = 2 * ATOM128 /*K*/ + 2 * ATOM128 /*V*/ + 3 * 2 * ATOM64 /*Q x3*/ +
-                        3 * 2 * ATOM64 /*dO x3*/ + 2 * ATOM128 /*P^T x2*/ + 2 * ATOM128 /*dS^T x2*/ +
-                        2 * 2 * 64 * 4 /*lse, delta x2*/ + 256;
-// S^T[2]: [0,64) [64,128)   dP^T[2]: [128,192) [192,256)   dV: [256,384)   dK: [384,512)
-constexpr int KV_TMEM_COLS = 512;
+constexpr int BWD_BKV = 128, BWD_BQ = 64, BWD_QH = 16;
+constexpr int KV_SMEM = 2 * ATOM128 /*K*/ + 2 * ATOM128 /*V*/ + 3 * 2 * ATOM64 /*Q x3*/ + 3 * 2 * ATOM64 /*dO x3*/ + 256;
 
-// bar_p ("P^T, dS^T of block `it` are in the staging tile") exists once per staging buffer. With a
-// single barrier the kernel was free of stale reads (the block-wide barrier at the end of every
-// iteration keeps the compute warps together) but not of an ABA hazard: the compute warps need
-// nothing from the MMA warp to run block it+1 once its score MMAs are issued, so an MMA warp held up
-// for a whole compute iteration right after issuing them saw bar_p complete twice and waited for a
-// parity that had flipped back -- a permanent hang (tools/protocol_model.py: ~0.3 % of adversarial
-// schedules; the end state, TMA warp parked on bar_qfree[0] parity 0, is what the 8-GPU run of
-// profiles/r01_n8_failure.txt trapped on). One barrier per stage is the change that fixed the dQ
-// kernel's race; a thread reaches the same stage again only after bar_s(it+2), which the MMA warp
-// commits after it has passed this barrier for `it`.
-constexpr int KV_NBARP = 2;
-
-__global__ void __launch_bounds__(BWD_NTHREADS, 1)
+// dV and dK stay in registers for the whole loop (128 per thread). A 9-warp block puts 3 warps on one of the SM's
+// four 16 K-register sub-partitions, so a thread may hold 168 registers: the query block is taken 16 queries at a
+// time (m64n16 score tiles) to keep the scores, their bf16 fragments and both accumulators inside that.
+__global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta,
                      bf16* __restrict__ dqkv, int ld_qkv, int k_off, int v_off, int B, int S, int H,
@@ -495,16 +279,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   uint8_t* sV = sK + 2 * ATOM128;
   uint8_t* sQ = sV + 2 * ATOM128;           // 3 bufs x 2 atoms x [64 q x 128 B]
   uint8_t* sdO = sQ + 3 * 2 * ATOM64;
-  uint8_t* sP = sdO + 3 * 2 * ATOM64;       // 2 bufs x P^T  [128 kv x 64 q]
-  uint8_t* sdS = sP + 2 * ATOM128;          // 2 bufs x dS^T [128 kv x 64 q]
-  float* sStat = reinterpret_cast<float*>(sdS + 2 * ATOM128);  // [2 bufs][lse 64 | delta*scale 64]
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sStat + 2 * 128);
-  uint64_t* bar_q = bar_kv + 1;  // [3]
-  uint64_t* bar_s = bar_q + 3;   // [2] S^T, dP^T (it) in TMEM
-  uint64_t* bar_d = bar_s + 2;   // [2] dV/dK MMAs that read P/dS buffer b retired
-  uint64_t* bar_p = bar_d + 2;   // [KV_NBARP] P^T, dS^T (it) in smem (BWD_NCOMPUTE arrivals)
-  uint64_t* bar_qfree = bar_p + KV_NBARP;  // [3] MMAs that read Q/dO buffer b retired (for the TMA warp)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_qfree + 3);
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sdO + 3 * 2 * ATOM64);
+  uint64_t* bar_q = bar_kv + 1;      // [3] Q, dO block in smem
+  uint64_t* bar_qfree = bar_q + 3;   // [3] MMAs that read Q/dO buffer b retired
 
   const int G = H / Hkv;
   const int jb = blockIdx.x / (B * Hkv);  // earliest key blocks (longest query loops) first
@@ -523,236 +300,143 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     mbar_init(bar_kv, 1);
     for (int i = 0; i < 3; ++i) {
       mbar_init(&bar_q[i], 1);
-      mbar_init(&bar_qfree[i], 1);
+      mbar_init(&bar_qfree[i], NCONSUMER_WARPS);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_s[i], 1);
-      mbar_init(&bar_d[i], 1);
-    }
-    for (int i = 0; i < KV_NBARP; ++i) mbar_init(&bar_p[i], BWD_NCOMPUTE / 32);
     fence_barrier_init();
   }
-  if (warp == 16) tmem_alloc(tmem_slot, KV_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_dV = tmem_base + 256, tmem_dK = tmem_base + 384;
 
-  // iteration `it` = (query head hk*G + it / nqb, query block 2 jb + it % nqb): walked with running
-  // counters (a division and a modulo per thread and iteration showed up in the instruction census)
+  // iteration `it` = (query head hk*G + it / nqb, query block 2 jb + it % nqb), walked with running counters
   struct IterPos {
     int h, qb;
     __device__ __forceinline__ void next(int nqb_) { if (++qb == nqb_) { qb = 0; ++h; } }
   };
   const int qb_base = 2 * jb;
 
-  if (warp == 17) {
-    // =============================== TMA producer ===============================
+  if (warp == TMA_WARP) {
     if (lane == 0) {
-      IterPos ip{hk * G, 0};
-      auto load_q = [&](int buf) {  // loads the block at `ip`, then advances it
-        mbar_arrive_expect_tx(&bar_q[buf], 4 * ATOM64);
-        const int h = ip.h, row = tok0 + (qb_base + ip.qb) * BWD_BQ;
-        ip.next(nqb);
-#pragma unroll
-        for (int a = 0; a < 2; ++a) {
-          tma_load_2d(sQ + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_q[buf], h * DH + a * 64, row);
-          tma_load_2d(sdO + (buf * 2 + a) * ATOM64, &tm_do, &bar_q[buf], h * DH + a * 64, row);
-        }
-      };
       mbar_arrive_expect_tx(bar_kv, 4 * ATOM128);
 #pragma unroll
       for (int a = 0; a < 2; ++a)
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-          tma_load_2d(sK + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, k_off + hk * DH + a * 64,
-                      tok0 + kv0 + r * 64);
-          tma_load_2d(sV + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, v_off + hk * DH + a * 64,
-                      tok0 + kv0 + r * 64);
+          tma_load_2d(sK + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, k_off + hk * DH + a * 64, tok0 + kv0 + r * 64);
+          tma_load_2d(sV + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, v_off + hk * DH + a * 64, tok0 + kv0 + r * 64);
         }
-      load_q(0);
-      if (n_iter > 1) load_q(1);
-      if (n_iter > 2) load_q(2);
+      IterPos ip{hk * G, 0};
       int buf = 0;
       uint32_t par = 0;
-      for (int it = 0; it + 3 < n_iter; ++it) {  // block it+3 reuses block it's buffer
-        mbar_wait(&bar_qfree[buf], par);
-        load_q(buf);
+      for (int it = 0; it < n_iter; ++it) {  // block it reuses block it-3's buffer
+        if (it >= 3) mbar_wait(&bar_qfree[buf], par ^ 1);
+        mbar_arrive_expect_tx(&bar_q[buf], 4 * ATOM64);
+        const int row = tok0 + (qb_base + ip.qb) * BWD_BQ;
+#pragma unroll
+        for (int a = 0; a < 2; ++a) {
+          tma_load_2d(sQ + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_q[buf], ip.h * DH + a * 64, row);
+          tma_load_2d(sdO + (buf * 2 + a) * ATOM64, &tm_do, &bar_q[buf], ip.h * DH + a * 64, row);
+        }
+        ip.next(nqb);
         if (++buf == 3) { buf = 0; par ^= 1; }
       }
     }
-  } else if (warp == 16) {
-    // =============================== MMA issuer ===============================
-    {  // the whole warp runs this loop; only `leader` issues
-      const bool leader = lane == 0;
-      constexpr uint32_t idesc_st = make_idesc_bf16(128, BWD_BQ, false, false);  // S^T, dP^T
-      constexpr uint32_t idesc_dv = make_idesc_bf16(128, DH, false, true);       // dV, dK
-      constexpr uint32_t BUF16 = (2 * ATOM64) >> 4, A128 = ATOM128 >> 4, A64 = ATOM64 >> 4;
-      const uint32_t k_lo = desc_lo_k(smem_u32(sK)), v_lo = desc_lo_k(smem_u32(sV));
-      const uint32_t q_lo = desc_lo_k(smem_u32(sQ)), do_lo = desc_lo_k(smem_u32(sdO));
-      const uint32_t q_mn = desc_lo_mn(smem_u32(sQ)), do_mn = desc_lo_mn(smem_u32(sdO));
-      const uint32_t p_lo = desc_lo_k(smem_u32(sP)), ds_lo = desc_lo_k(smem_u32(sdS));
-      auto issue_scores = [&](uint32_t tb, uint32_t qb) {  // S^T = K Q^T, dP^T = V dO^T -> TMEM bufs tb
-        mma_kmajor_dh(leader, tmem_base + tb * 64, k_lo, A128, q_lo + qb * BUF16, A64, idesc_st);
-        mma_kmajor_dh(leader, tmem_base + 128 + tb * 64, v_lo, A128, do_lo + qb * BUF16, A64, idesc_st);
-        commit_if(leader, &bar_s[tb]);
-      };
-      mbar_wait(bar_kv, 0);
-      mbar_wait(&bar_q[0], 0);
-      tc_fence_after();
-      issue_scores(0, 0);
-      uint32_t qb = 0, qpar = 0;  // buffer / parity of block `it`
-      for (int it = 0; it < n_iter; ++it) {
-        uint32_t nqb_ = qb + 1, npar = qpar;
-        if (nqb_ == 3) { nqb_ = 0; npar ^= 1; }
-        if (it + 1 < n_iter) {  // TMEM score buffers (it+1)&1 were drained before bar_p(it-1)
-          mbar_wait(&bar_q[nqb_], npar);
-          tc_fence_after();
-          issue_scores((it + 1) & 1, nqb_);
-        }
-        mbar_wait(&bar_p[it & 1], (it >> 1) & 1);
-        tc_fence_after();
-        // dV += P^T dO, dK += dS^T Q : A K-major [128 kv x 64 q], B MN-major (N = dh, K = q rows)
-        const uint32_t pb = (it & 1) * A128;  // P/dS staging buffer of this block
-        mma_a64_bmn(leader, tmem_dV, p_lo + pb, do_mn + qb * BUF16, idesc_dv, it != 0);
-        mma_a64_bmn(leader, tmem_dK, ds_lo + pb, q_mn + qb * BUF16, idesc_dv, it != 0);
-        commit_if(leader, &bar_d[it & 1]);
-        commit_if(leader, &bar_qfree[qb]);
-        qb = nqb_;
-        qpar = npar;
-      }
-    }
-  } else {
-    // =============================== compute ===============================
-    const int q = warp & 3, hc = warp >> 2;    // hc: which 16 of the block's 64 query columns
-    const int row_local = q * 32 + lane;       // TMEM lane == key row inside the block
-    const int kv_seq = kv0 + row_local;        // key position inside the sequence
-    const uint32_t lane_base = (q * 32u) << 16;
-    // lse / delta*scale of the 64 query rows of a block: fetched into a register one iteration
-    // ahead by 128 of the compute threads, parked in smem just before the per-iteration bar.sync
-    auto fetch_stat = [&](const IterPos& p) -> float {
-      const size_t base = static_cast<size_t>(p.h) * Ttot + tok0 + (qb_base + p.qb) * BWD_BQ;
-      return (tid < 64) ? lse2[base + tid] : delta[base + tid - 64];
-    };
-    // (delta arrives pre-multiplied by the scale: attn_bwd_delta)
-    IterPos cur{hk * G, 0};
-    if (tid < 128) sStat[tid] = fetch_stat(cur);
-    bwd_compute_bar_sync();
-
-    for (int it = 0; it < n_iter; ++it) {
-      const int tb = it & 1;
-      const int q_seq0 = (qb_base + cur.qb) * BWD_BQ;
-      cur.next(nqb);  // now the position of block it + 1
-      float stat_next = 0.f;
-      const bool have_next = (it + 1 < n_iter) && tid < 128;
-      if (have_next) stat_next = fetch_stat(cur);  // latency hidden behind this block's math
-      mbar_wait(&bar_s[tb], (it >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      uint32_t s_r[16], dp_r[16];
-      tmem_ld16(tmem_base + tb * 64 + lane_base + hc * 16, s_r);
-#ifdef B200W_WHATIF_NODP
-      tmem_ld_wait();   // what if dP^T did not have to be read from TMEM
-#pragma unroll
-      for (int c = 0; c < 16; ++c) dp_r[c] = s_r[c];
-#else
-      tmem_ld16(tmem_base + 128 + tb * 64 + lane_base + hc * 16, dp_r);
-      tmem_ld_wait();
-#endif
-      // staging buffer tb was last read by the dV/dK MMAs of block it-2
-      if (it >= 2) mbar_wait(&bar_d[tb], ((it >> 1) - 1) & 1);
-      const float4* st_lse = reinterpret_cast<const float4*>(sStat + tb * 128 + hc * 16);
-      const float4* st_dl = reinterpret_cast<const float4*>(sStat + tb * 128 + 64 + hc * 16);
-      const bool diag = (q_seq0 < kv0 + BWD_BKV);  // some (q, kv) pairs of this block are masked
-#pragma unroll
-      for (int c8 = 0; c8 < 2; ++c8) {
-        const float4 l0 = st_lse[c8 * 2], l1 = st_lse[c8 * 2 + 1];
-        const float4 d0 = st_dl[c8 * 2], d1 = st_dl[c8 * 2 + 1];
-        const float lse8[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-        const float dl8[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-        float p[8], ds[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e)
-          p[e] = ex2(fmaf(__uint_as_float(s_r[c8 * 8 + e]), scale_log2, -lse8[e]));
-        if (diag) {  // only the 2 blocks that straddle the diagonal pay for the mask
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (q_seq0 + hc * 16 + c8 * 8 + e < kv_seq) p[e] = 0.f;
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e)  // dS = P (dP - delta) * scale, with delta*scale precomputed
-          ds[e] = p[e] * fmaf(__uint_as_float(dp_r[c8 * 8 + e]), scale, -dl8[e]);
-        const uint32_t off = tb * ATOM128 + sw128_offset(row_local, hc * 2 + c8);
-        *reinterpret_cast<uint4*>(sP + off) = pack8(p);
-        *reinterpret_cast<uint4*>(sdS + off) = pack8(ds);
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_p[tb]);  // one arrival per compute warp
-      if (have_next) sStat[(tb ^ 1) * 128 + tid] = stat_next;
-      // stats(it+1) visible; stats(it) no longer read. With one bar_p per stage the protocol no longer NEEDS
-      // this block-wide barrier, and a variant with warp-private statistics rows and no barrier was built
-      // and measured in round 2: 4 % SLOWER (303.9 vs 292.6 us, same-box ncu A/B,
-      // profiles/r02_attn_ab_dkdv_barrier.txt) -- the barrier keeps the 16 warps in phase, which is what the
-      // shared TMEM / staging double-buffering wants. Kept.
-      bwd_compute_bar_sync();
-    }
-
-    mbar_wait(&bar_d[(n_iter - 1) & 1], ((n_iter - 1) >> 1) & 1);  // commits are cumulative
-    __syncwarp();
-    tc_fence_after();
-    // dV, dK: lane = key row; this thread stores 32 of the 128 dh columns of each
-    bf16* dvrow = dqkv + static_cast<size_t>(tok0 + kv_seq) * ld_qkv + v_off + hk * DH + hc * 32;
-    bf16* dkrow = dqkv + static_cast<size_t>(tok0 + kv_seq) * ld_qkv + k_off + hk * DH + hc * 32;
-    tmem_row32_to_global(tmem_dV + lane_base + hc * 32, dvrow);
-    tmem_row32_to_global(tmem_dK + lane_base + hc * 32, dkrow);
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 16) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, KV_TMEM_COLS);
+  // =============================== consumers: warpgroup wg owns keys [kv0 + 64 wg, kv0 + 64 wg + 64) =========
+  const int wg = warp >> 2, wi = warp & 3;
+  const int kv_a = kv0 + wg * 64 + wi * 16 + (lane >> 2);  // key positions of this thread's two rows
+  const int kv_b = kv_a + 8;
+  const uint32_t k_addr = smem_u32(sK) + wg * ATOM64, v_addr = smem_u32(sV) + wg * ATOM64;
+  float dv[64], dk[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  mbar_wait(bar_kv, 0);
+
+  IterPos cur{hk * G, 0};
+  int buf = 0;
+  uint32_t par = 0;
+  for (int it = 0; it < n_iter; ++it) {
+    const int q_seq0 = (qb_base + cur.qb) * BWD_BQ;
+    const float* lse_h = lse2 + static_cast<size_t>(cur.h) * Ttot + tok0;
+    const float* dl_h = delta + static_cast<size_t>(cur.h) * Ttot + tok0;   // pre-multiplied by the scale
+    mbar_wait(&bar_q[buf], par);
+#pragma unroll 1
+    for (int hq = 0; hq < BWD_BQ / BWD_QH; ++hq) {
+      const int qh0 = q_seq0 + hq * BWD_QH;
+      if (qh0 + BWD_QH - 1 < kv0 + wg * 64) continue;  // every query of the slice precedes every key: P = 0
+      const uint32_t qrow = smem_u32(sQ + buf * 2 * ATOM64) + hq * BWD_QH * 128;
+      const uint32_t dorow = smem_u32(sdO + buf * 2 * ATOM64) + hq * BWD_QH * 128;
+      float st[BWD_QH / 2], dpt[BWD_QH / 2];
+      wg_fence();
+      mma_over_dh<BWD_QH>(st, k_addr, ATOM128, qrow, ATOM64);
+      mma_over_dh<BWD_QH>(dpt, v_addr, ATOM128, dorow, ATOM64);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(st);
+      wg_fence_regs(dpt);
+      const bool diag = qh0 < kv0 + wg * 64 + 64;  // some (q, kv) pairs of this slice are masked
+#pragma unroll
+      for (int jj = 0; jj < BWD_QH / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int q = qh0 + 8 * jj + 2 * (lane & 3) + e;
+          const float lse = lse_h[q], dl = dl_h[q];
+          float pa_ = ex2(fmaf(st[4 * jj + e], scale_log2, -lse));
+          float pb_ = ex2(fmaf(st[4 * jj + 2 + e], scale_log2, -lse));
+          if (diag) {
+            if (q < kv_a) pa_ = 0.f;
+            if (q < kv_b) pb_ = 0.f;
+          }
+          st[4 * jj + e] = pa_;
+          st[4 * jj + 2 + e] = pb_;
+          // dS = P (dP - delta) * scale, with delta*scale precomputed
+          dpt[4 * jj + e] = pa_ * fmaf(dpt[4 * jj + e], scale, -dl);
+          dpt[4 * jj + 2 + e] = pb_ * fmaf(dpt[4 * jj + 2 + e], scale, -dl);
+        }
+      uint32_t pa[BWD_QH / 16][4], dsa[BWD_QH / 16][4];
+#pragma unroll
+      for (int kk = 0; kk < BWD_QH / 16; ++kk) {
+        to_afrag(st, kk, pa[kk]);
+        to_afrag(dpt, kk, dsa[kk]);
+      }
+      wg_fence();
+      mma_pv<BWD_QH / 16>(dv, pa, dorow);
+      mma_pv<BWD_QH / 16>(dk, dsa, qrow);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(dv);
+      wg_fence_regs(dk);
+    }
+    warp_release(&bar_qfree[buf]);
+    cur.next(nqb);
+    if (++buf == 3) { buf = 0; par ^= 1; }
   }
+
+  bf16* base_a = dqkv + static_cast<size_t>(tok0 + kv_a) * ld_qkv + hk * DH;
+  bf16* base_b = dqkv + static_cast<size_t>(tok0 + kv_b) * ld_qkv + hk * DH;
+  store_rows_bf16(dv, base_a + v_off, base_b + v_off, 1.f, 1.f);
+  store_rows_bf16(dk, base_a + k_off, base_b + k_off, 1.f, 1.f);
 }
 
 // ==========================================================================================
 // backward, part 2: dQ
 // ==========================================================================================
 constexpr int DQ_BQ = 128, DQ_BKV = 64;
-// operands need 96 KB; asking for > half of the SM's shared memory keeps one CTA per SM, which the
-// 512-column TMEM allocation assumes (a second resident CTA would only spin in tcgen05.alloc)
-constexpr int DQ_SMEM = 120 * 1024;
-static_assert(3 * 2 * ATOM64 + 3 * 2 * ATOM64 + 256 <= DQ_SMEM, "dQ kernel shared memory");
-// S[2]: [0,64) [64,128)   dP[2]: [128,192) [192,256) (dS bf16 re-uses the first 32 columns of the
-// dP buffer it was computed from)   dQ: [256,384)   Q bf16: [384,448)   dO bf16: [448,512)
-constexpr int DQ_TMEM_COLS = 512;
+constexpr int DQ_SMEM = 2 * ATOM128 /*Q*/ + 2 * ATOM128 /*dO*/ + 3 * 2 * ATOM64 /*K x3*/ + 3 * 2 * ATOM64 /*V x3*/ + 256;
 
-__global__ void __launch_bounds__(BWD_NTHREADS, 1)
-attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const bf16* __restrict__ qkv,
-                   const bf16* __restrict__ dout, int ld_out, const float* __restrict__ lse2,
-                   const float* __restrict__ delta, bf16* __restrict__ dqkv, int ld_qkv, int k_off,
-                   int v_off, int B, int S, int H, int Hkv, float scale, float scale_log2) {
+__global__ void __launch_bounds__(NTHREADS, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
+                   const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
+                   int ld_qkv, int k_off, int v_off, int B, int S, int H, int Hkv, float scale, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   require_1024_aligned(smem);
-  uint8_t* sK = smem;                      // 3 bufs x 2 atoms x [64 kv x 128 B]
+  uint8_t* sQ = smem;                      // 2 atoms (dh halves) x [128 q x 128 B]
+  uint8_t* sdO = sQ + 2 * ATOM128;
+  uint8_t* sK = sdO + 2 * ATOM128;         // 3 bufs x 2 atoms x [64 kv x 128 B]
   uint8_t* sV = sK + 3 * 2 * ATOM64;
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sV + 3 * 2 * ATOM64);  // [3]
-  uint64_t* bar_s = bar_kv + 3;       // [2] S, dP (j) in TMEM
-  uint64_t* bar_dq = bar_s + 2;       //     dQ MMAs of the last block retired
-  // [2], one per TMEM stage: dS (j) in TMEM and S/dP (j) drained (512 arrivals). It MUST be per
-  // stage: the lane quarters are coupled only through this barrier, a quarter may run one block
-  // ahead (S/dP (j+1) are issued early), and with a single barrier its arrival for j+1 would
-  // complete phase j before a slower quarter has written dS (j) -- the dQ MMA then reads that
-  // quarter's stale dP bits (found by tools/stress_attn.py: 1.2 % of launches, one quarter of one
-  // CTA wrong, NaN or not). With a barrier per stage a thread reaches the same stage again only
-  // after bar_s (j+2), which the MMA warp commits after it has passed this barrier for j.
-  uint64_t* bar_p = bar_dq + 1;
-  uint64_t* bar_kvfree = bar_p + 2;   // [3] MMAs that read K/V buffer b retired (for the TMA warp)
-  uint64_t* bar_qready = bar_kvfree + 3;  // Q, dO rows are in TMEM (512 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_qready + 1);
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + 3 * 2 * ATOM64);  // Q, dO tile in smem
+  uint64_t* bar_kv = bar_q + 1;        // [3]
+  uint64_t* bar_kvfree = bar_kv + 3;   // [3] MMAs that read K/V buffer b retired
 
   const int nq = S / DQ_BQ;
   const int bh = blockIdx.x % (B * H);
@@ -766,161 +450,102 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const bf16* __res
 
   if (tid == 0) {
     tma_prefetch_desc(&tm_qkv);
+    tma_prefetch_desc(&tm_do);
+    mbar_init(bar_q, 1);
     for (int i = 0; i < 3; ++i) {
       mbar_init(&bar_kv[i], 1);
-      mbar_init(&bar_kvfree[i], 1);
+      mbar_init(&bar_kvfree[i], NCONSUMER_WARPS);
     }
-    for (int i = 0; i < 2; ++i) mbar_init(&bar_s[i], 1);
-    mbar_init(bar_dq, 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&bar_p[i], BWD_NCOMPUTE / 32);
-    mbar_init(bar_qready, BWD_NCOMPUTE / 32);
     fence_barrier_init();
   }
-  if (warp == 16) tmem_alloc(tmem_slot, DQ_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_dQ = tmem_base + 256, tmem_Q = tmem_base + 384, tmem_dO = tmem_base + 448;
 
-  if (warp == 17) {
-    // =============================== TMA producer ===============================
+  if (warp == TMA_WARP) {
     if (lane == 0) {
-      auto load_kv = [&](int j, int buf) {
+      mbar_arrive_expect_tx(bar_q, 4 * ATOM128);
+#pragma unroll
+      for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          tma_load_2d(sQ + a * ATOM128 + r * ATOM64, &tm_qkv, bar_q, h * DH + a * 64, tok0 + q0 + r * 64);
+          tma_load_2d(sdO + a * ATOM128 + r * ATOM64, &tm_do, bar_q, h * DH + a * 64, tok0 + q0 + r * 64);
+        }
+      int buf = 0;
+      uint32_t par = 0;
+      for (int j = 0; j < njb; ++j) {  // block j reuses block j-3's buffer
+        if (j >= 3) mbar_wait(&bar_kvfree[buf], par ^ 1);
         mbar_arrive_expect_tx(&bar_kv[buf], 4 * ATOM64);
 #pragma unroll
         for (int a = 0; a < 2; ++a) {
-          tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], k_off + hk * DH + a * 64,
-                      tok0 + j * DQ_BKV);
-          tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], v_off + hk * DH + a * 64,
-                      tok0 + j * DQ_BKV);
+          tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], k_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
+          tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], v_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
         }
-      };
-      load_kv(0, 0);
-      load_kv(1, 1);  // njb >= 2 always
-      if (njb > 2) load_kv(2, 2);
-      int buf = 0;
-      uint32_t par = 0;
-      for (int j = 0; j + 3 < njb; ++j) {  // block j+3 reuses block j's buffer
-        mbar_wait(&bar_kvfree[buf], par);
-        load_kv(j + 3, buf);
         if (++buf == 3) { buf = 0; par ^= 1; }
       }
     }
-  } else if (warp == 16) {
-    // =============================== MMA issuer (convergent warp) ===============================
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, DQ_BKV, false, false);  // S, dP
-      constexpr uint32_t idesc_dq = make_idesc_bf16(128, DH, false, true);      // dQ
-      constexpr uint32_t BUF16 = (2 * ATOM64) >> 4, A64 = ATOM64 >> 4;
-      const uint32_t k_lo = desc_lo_k(smem_u32(sK)), v_lo = desc_lo_k(smem_u32(sV));
-      const uint32_t k_mn = desc_lo_mn(smem_u32(sK));
-      auto issue_scores = [&](uint32_t tb, uint32_t kb) {  // S = Q K^T, dP = dO V^T -> TMEM bufs tb
-        mma_ts_kmajor_dh(tmem_base + tb * 64, tmem_Q, k_lo + kb * BUF16, A64, idesc_s);
-        mma_ts_kmajor_dh(tmem_base + 128 + tb * 64, tmem_dO, v_lo + kb * BUF16, A64, idesc_s);
-        commit_if(true, &bar_s[tb]);
-      };
-      mbar_wait(bar_qready, 0);
-      mbar_wait(&bar_kv[0], 0);
-      tc_fence_after();
-      issue_scores(0, 0);
-      uint32_t kb = 0, kpar = 0;  // buffer / parity of block j
-      for (int j = 0; j < njb; ++j) {
-        uint32_t nkb = kb + 1, npar = kpar;
-        if (nkb == 3) { nkb = 0; npar ^= 1; }
-        if (j + 1 < njb) {  // TMEM buffers (j+1)&1 hold dS(j-1): its dQ MMA was issued last iteration
-          mbar_wait(&bar_kv[nkb], npar);
-          tc_fence_after();
-          issue_scores((j + 1) & 1, nkb);
-        }
-        mbar_wait(&bar_p[j & 1], (j >> 1) & 1);
-        tc_fence_after();
-        // dQ += dS K : A = dS (bf16 in TMEM, over dP buffer j&1), B = K as MN-major (N = dh, K = kv rows)
-        mma_ts_a64_bmn(tmem_dQ, tmem_base + 128 + (j & 1) * 64, k_mn + kb * BUF16, idesc_dq, j != 0);
-        if (j + 1 == njb) commit_if(true, bar_dq);
-        commit_if(true, &bar_kvfree[kb]);
-        kb = nkb;
-        kpar = npar;
-      }
-    }
-  } else {
-    // =============================== compute (16 warps: 4 threads per query row) =================
-    const int q = warp & 3, hc = warp >> 2;
-    const int row_local = q * 32 + lane;
-    const int row_seq = q0 + row_local;
-    const uint32_t lane_base = (q * 32u) << 16;
-    // this thread's 32 of the 128 dh elements of its Q and dO rows -> TMEM (16 packed columns each)
-    {
-      const uint4* qsrc = reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(tok0 + row_seq) * ld_qkv + h * DH + hc * 32);
-      const uint4* dsrc = reinterpret_cast<const uint4*>(dout + static_cast<size_t>(tok0 + row_seq) * ld_out + h * DH + hc * 32);
-      uint32_t rq[16], rd[16];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint4 a = qsrc[i], d4 = dsrc[i];
-        rq[i * 4 + 0] = a.x; rq[i * 4 + 1] = a.y; rq[i * 4 + 2] = a.z; rq[i * 4 + 3] = a.w;
-        rd[i * 4 + 0] = d4.x; rd[i * 4 + 1] = d4.y; rd[i * 4 + 2] = d4.z; rd[i * 4 + 3] = d4.w;
-      }
-      tmem_st16(tmem_Q + lane_base + hc * 16, rq);
-      tmem_st16(tmem_dO + lane_base + hc * 16, rd);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_qready);
-    }
-    const size_t stat_idx = static_cast<size_t>(h) * (static_cast<size_t>(B) * S) + tok0 + row_seq;
-    const float my_lse = lse2[stat_idx];
-    const float my_dl = delta[stat_idx];   // pre-multiplied by the scale (attn_bwd_delta)
-
-    for (int j = 0; j < njb; ++j) {
-      const int tb = j & 1;
-      mbar_wait(&bar_s[tb], (j >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      uint32_t s_r[16], dp_r[16];
-      tmem_ld16(tmem_base + tb * 64 + lane_base + hc * 16, s_r);
-      tmem_ld16(tmem_base + 128 + tb * 64 + lane_base + hc * 16, dp_r);
-      tmem_ld_wait();
-      const int col0 = j * DQ_BKV + hc * 16;
-      const bool diag = (j * DQ_BKV + DQ_BKV - 1) > q0;
-      uint32_t dsp[8];
-#pragma unroll
-      for (int c8 = 0; c8 < 2; ++c8) {
-        float p[8], ds[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) p[e] = ex2(fmaf(__uint_as_float(s_r[c8 * 8 + e]), scale_log2, -my_lse));
-        if (diag) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (col0 + c8 * 8 + e > row_seq) p[e] = 0.f;
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) ds[e] = p[e] * fmaf(__uint_as_float(dp_r[c8 * 8 + e]), scale, -my_dl);
-        const uint4 u = pack8(ds);
-        dsp[c8 * 4 + 0] = u.x; dsp[c8 * 4 + 1] = u.y; dsp[c8 * 4 + 2] = u.z; dsp[c8 * 4 + 3] = u.w;
-      }
-      // dS overwrites columns of the dP buffer that the other three threads of this row read:
-      // wait until the whole lane quarter has its dP values in registers
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + q) : "memory");
-      tmem_st8(tmem_base + 128 + tb * 64 + lane_base + hc * 8, dsp);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_p[tb]);  // one arrival per compute warp
-    }
-
-    mbar_wait(bar_dq, 0);
-    __syncwarp();
-    tc_fence_after();
-    bf16* dqrow = dqkv + static_cast<size_t>(tok0 + row_seq) * ld_qkv + h * DH + hc * 32;
-    tmem_row32_to_global(tmem_dQ + lane_base + hc * 32, dqrow);
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 16) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, DQ_TMEM_COLS);
+  // =============================== consumers: warpgroup wg owns query rows [q0 + 64 wg, q0 + 64 wg + 64) =======
+  const int wg = warp >> 2, wi = warp & 3;
+  const int row0 = q0 + wg * 64 + wi * 16 + (lane >> 2);
+  const int row1 = row0 + 8;
+  const int last_j = 2 * qi + wg;
+  const size_t stat = static_cast<size_t>(h) * (static_cast<size_t>(B) * S) + tok0;
+  const float lse0 = lse2[stat + row0], lse1 = lse2[stat + row1];
+  const float dl0 = delta[stat + row0], dl1 = delta[stat + row1];   // pre-multiplied by the scale
+  const uint32_t q_addr = smem_u32(sQ) + wg * ATOM64, do_addr = smem_u32(sdO) + wg * ATOM64;
+  float dq[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+  mbar_wait(bar_q, 0);
+
+  int buf = 0;
+  uint32_t par = 0;
+  for (int j = 0; j < njb; ++j) {
+    if (j <= last_j) {
+      float s[32], dp[32];
+      mbar_wait(&bar_kv[buf], par);
+      wg_fence();
+      mma_over_dh<DQ_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
+      mma_over_dh<DQ_BKV>(dp, do_addr, ATOM128, smem_u32(sV + buf * 2 * ATOM64), ATOM64);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(s);
+      wg_fence_regs(dp);
+      const bool diag = j * DQ_BKV + DQ_BKV - 1 > q0 + wg * 64;
+      const int col0 = j * DQ_BKV + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * jj + e;
+          float p0 = ex2(fmaf(s[4 * jj + e], scale_log2, -lse0));
+          float p1 = ex2(fmaf(s[4 * jj + 2 + e], scale_log2, -lse1));
+          if (diag) {
+            if (col > row0) p0 = 0.f;
+            if (col > row1) p1 = 0.f;
+          }
+          s[4 * jj + e] = p0 * fmaf(dp[4 * jj + e], scale, -dl0);     // dS
+          s[4 * jj + 2 + e] = p1 * fmaf(dp[4 * jj + 2 + e], scale, -dl1);
+        }
+      uint32_t dsa[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, dsa[kk]);
+      wg_fence();
+      mma_pv<4>(dq, dsa, smem_u32(sK + buf * 2 * ATOM64));  // dQ += dS K, K read MN-major (N = dh)
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(dq);
+    } else {
+      mbar_wait(&bar_kv[buf], par);  // a skipped block is released after its loads landed (see the forward)
+    }
+    warp_release(&bar_kvfree[buf]);
+    if (++buf == 3) { buf = 0; par ^= 1; }
   }
+
+  store_rows_bf16(dq, dqkv + static_cast<size_t>(tok0 + row0) * ld_qkv + h * DH,
+                  dqkv + static_cast<size_t>(tok0 + row1) * ld_qkv + h * DH, 1.f, 1.f);
 }
 
 template <typename K>
@@ -961,13 +586,13 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
     set_smem(attn_bwd_dq_kernel, DQ_SMEM);
   });
   const float scale_log2 = scale * 1.4426950408889634f;
-  attn_bwd_dkdv_kernel<<<(S / BWD_BKV) * B * Hkv, BWD_NTHREADS, KV_SMEM, s>>>(
+  attn_bwd_dkdv_kernel<<<(S / BWD_BKV) * B * Hkv, NTHREADS, KV_SMEM, s>>>(
       tm_qkv, tm_do, lse2, delta, static_cast<bf16*>(dqkv), ld_qkv, k_off, v_off, B, S, H, Hkv, scale,
       scale_log2);
   B200W_CUDA(cudaGetLastError());
-  attn_bwd_dq_kernel<<<(S / DQ_BQ) * B * H, BWD_NTHREADS, DQ_SMEM, s>>>(
-      tm_qkv, static_cast<const bf16*>(qkv), static_cast<const bf16*>(dout), ld_out, lse2, delta,
-      static_cast<bf16*>(dqkv), ld_qkv, k_off, v_off, B, S, H, Hkv, scale, scale_log2);
+  attn_bwd_dq_kernel<<<(S / DQ_BQ) * B * H, NTHREADS, DQ_SMEM, s>>>(
+      tm_qkv, tm_do, lse2, delta, static_cast<bf16*>(dqkv), ld_qkv, k_off, v_off, B, S, H, Hkv, scale,
+      scale_log2);
   B200W_CUDA(cudaGetLastError());
 }
 

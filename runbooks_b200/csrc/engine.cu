@@ -155,29 +155,12 @@ __global__ void init_normal_kernel(float* master, bf16* w, size_t n, uint64_t se
     if (w) w[j] = __float2bfloat16_rn(r);
   }
 }
-// Fills this SM's shared memory and all 512 TMEM columns with `pattern` (b200w_op_poison_onchip).
-constexpr int POISON_SMEM = 227 * 1024 - 64;
+// Fills this SM's shared memory (all 227 KB a block may use) with `pattern` (b200w_op_poison_onchip).
+constexpr int POISON_SMEM = 227 * 1024;
 __global__ void __launch_bounds__(128, 1) poison_onchip_kernel(uint32_t pattern) {
   extern __shared__ __align__(16) uint32_t poison_sm[];
-  __shared__ uint32_t slot;
   for (int i = threadIdx.x; i < POISON_SMEM / 4; i += blockDim.x) poison_sm[i] = pattern;
-  const int warp = threadIdx.x >> 5;
-  if (warp == 0) tmem_alloc(&slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t base = slot + ((warp * 32u) << 16);
-  uint32_t r[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) r[i] = pattern;
-  for (int col = 0; col < 512; col += 32) tmem_st32(base + col, r);
-  tmem_st_wait();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(slot, 512);
-  }
   // keep the smem stores alive
   if (poison_sm[(threadIdx.x * 977) % (POISON_SMEM / 4)] != pattern) __trap();
 }
@@ -718,9 +701,7 @@ void loss_micro(b200w_ctx* c, const int32_t* labels, int nseq) {
 //   sync               as overlap, but the host drains c->stream before enqueuing each all-reduce
 //   serial             per-matrix, but c->stream waits for each all-reduce: never concurrent with compute
 //   end                one all-reduce of the whole gradient after the backward
-// Round 1 fell back to `end` for more than 2 ranks after an 8-rank run stalled in the dK/dV kernel
-// (profiles/r01_n8_failure.txt); that kernel's barrier protocol is fixed (attention.cu, one bar_p per
-// stage) and overlap is the default for every rank count.
+// Overlap is the default for every rank count.
 enum class ArMode { Overlap, Sync, Serial, End };
 ArMode ar_mode() {
   const char* m = getenv("B200W_AR_MODE");
@@ -1219,8 +1200,8 @@ int b200w_create(int device, b200w_ctx** out) {
     B200W_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     B200W_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-      g_create_error = std::string("b200w is built for sm_100a only; device is ") + prop.name;
+    if (prop.major != 9 || prop.minor != 0) {
+      g_create_error = std::string("b200w is built for sm_90a only; device is ") + prop.name;
       return B200W_ERR_CUDA;
     }
     auto c = std::make_unique<b200w_ctx>();
@@ -1244,8 +1225,8 @@ void b200w_destroy(b200w_ctx* ctx) {
   // After a device fault (e.g. the bounded mbarrier wait trapped) or an NCCL error, waiting for the
   // device or for a clean communicator shutdown can block for ever: peers are still inside a
   // collective that will never complete. Abort instead, so that this process can exit and the
-  // launcher can tear the job down (profiles/r01_n8_failure.txt: a rank that failed but did not
-  // exit kept 7 GPUs spinning for 10 minutes).
+  // launcher can tear the job down (a rank that fails but does not exit keeps its peers spinning
+  // inside the collective).
   const bool dead = ctx->poisoned || cudaDeviceSynchronize() != cudaSuccess;
   if (ctx->comm) {
     if (!dead) nccl().CommDestroy(ctx->comm);
@@ -1598,9 +1579,8 @@ int b200w_comm_init(b200w_ctx* ctx, int rank, int nranks, const void* id128) {
     // (one per SM, ~200 KB of shared memory each) cannot share an SM, so the two are given disjoint
     // SM budgets: NCCL is capped at R CTAs (NCCL_MAX_CTAS, unless the user set it) and the GEMMs of
     // that backward launch on SMs - R. B200W_AR_SM_RESERVE overrides R (0: no partition).
-    // R = 8: the whole 13.5 GB exchange has the last micro-step's backward (~200 ms) to hide in, so even 8 CTAs
-    // are an order of magnitude more bandwidth than it needs; every reserved SM costs the GEMMs of that
-    // backward 1/148 (profiles/r02_bench_n8*.json: R = 16 vs no partition vs R = 8).
+    // R = 8: the whole 13.5 GB exchange has the last micro-step's backward to hide in, so even 8 CTAs are far
+    // more bandwidth than it needs; every reserved SM costs the GEMMs of that backward 1/132 of an H100.
     int reserve = 8;
     if (const char* e = getenv("B200W_AR_SM_RESERVE")) reserve = atoi(e);
     if (reserve < 0 || reserve > 64) reserve = 8;

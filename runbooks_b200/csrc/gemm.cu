@@ -1,4 +1,4 @@
-// bf16 x bf16 -> fp32-accumulate GEMM on tcgen05 tensor cores (sm_100a), TMA-fed.
+// bf16 x bf16 -> fp32-accumulate GEMM on Hopper tensor cores (sm_90a wgmma), TMA-fed.
 //
 //   D[M,N] = op(A)[M,K] * op(B)[N,K]^T  (+ C[M,N])
 //
@@ -7,12 +7,13 @@
 //   forward   Y  = X  W^T   : A = X  [T,in]  K-major,  B = W  [out,in] K-major
 //   dgrad     dX = dY W     : A = dY [T,out] K-major,  B = W  [out,in] read MN-major (K = out)
 //   wgrad     dW = dY^T X   : A = dY [T,out] read MN-major, B = X [T,in] read MN-major (K = T)
-// so no operand is ever transposed through HBM.
+// so no operand is ever transposed through HBM (wgmma reads 16-bit operands in either major order).
 //
 // Structure: persistent CTAs (one per SM), 128 x BLOCK_N output tiles, K in 64-element
-// (= one 128-byte swizzle atom) blocks; warp 0 = TMA producer, warp 1 = tcgen05.mma issuer
-// (single elected thread), warp 2 = TMEM allocator, warps 4..7 = epilogue. Two TMEM accumulator
-// stages so the epilogue of tile i overlaps the MMAs of tile i+1.
+// (= one 128-byte swizzle atom) blocks; warp 8 = TMA producer, warps 0..7 = two consumer
+// warpgroups that each own 64 rows of the tile and accumulate them in registers with wgmma.
+// The producer runs ahead across tile boundaries, so the next tile's operands stream in while the
+// consumers write the previous tile out.
 #include <mutex>
 
 #include "host_common.h"
@@ -26,9 +27,9 @@ static int pick_raster(int M, int N, int K, int tile_m, int tile_n);
 
 // Tile raster: `raster` = n_fast | (group << 1). Tiles run along the fast dimension (N when n_fast, else M), but
 // only `group` tiles wide; a band of `group` fast-dimension tiles is swept across the whole slow dimension
-// before the next band starts (group 0 = the whole extent). The band's operand panels (group x 256 x K x 2 bytes,
-// chosen <= 34 MB by pick_raster) are what every wave of tiles re-reads, and they stay in L2; the other operand
-// is streamed once per band.
+// before the next band starts (group 0 = the whole extent). The band's operand panels (chosen by pick_raster to
+// fit the L2 budget) are what every wave of tiles re-reads, and they stay in L2; the other operand is streamed
+// once per band.
 __host__ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int raster, int& mi, int& ni) {
   const int n_fast = raster & 1, group = raster >> 1;
   const int fast_total = n_fast ? num_n : num_m, slow_total = n_fast ? num_m : num_n;
@@ -52,226 +53,134 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one SWIZZLE_128B atom row
-constexpr int UMMA_K = 16;
-constexpr int GEMM_THREADS = 256;
+constexpr int WG_K = 16;     // K of one wgmma
+constexpr int GEMM_THREADS = 288;  // two consumer warpgroups + one producer warp
+constexpr int PRODUCER_WARP = 8;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
+// a consumer warpgroup's 64 rows of the A stage: 64 rows x 128 B (K-major) or the second 64-element MN atom
+// column (MN-major, the producer loads the atom columns 64 K rows x 128 B = 8 KB apart) -- 8 KB either way
+constexpr int A_HALF_BYTES = 64 * 128;
+constexpr int PAIR_N = 256;    // tile width of the 2-CTA cluster kernel (block_n = 512)
 
 template <int BLOCK_N>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // 4 x 48 KB, 6 x 32 KB, 8 x 24 KB, 9 x 20 KB: the narrow tiles exist for decode (M <= 128), where
-  // the job is to keep every SM streaming weights, not to feed the tensor pipe
+  // 4 x 48 KB, 6 x 32 KB, 8 x 24 KB, 9 x 20 KB of the 227 KB a block may use: the narrow tiles exist for
+  // small M, where the job is to keep every SM streaming weights, not to feed the tensor pipe
   static constexpr int STAGES = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128) ? 6 : (BLOCK_N == 64) ? 8 : 9;
-  static constexpr int TMEM_COLS = (2 * BLOCK_N < 32) ? 32 : 2 * BLOCK_N;  // two accumulator stages
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// ---- epilogue helpers ------------------------------------------------------------------------
-// One thread owns one output row; a "chunk" is 32 consecutive columns of it. The optional addend C
-// (residual stream / running gradient) is fetched into registers one chunk AHEAD of its use, so
-// its global-memory latency sits under the previous chunk's tcgen05.ld + stores instead of in
-// front of them (profiles/r01_ncu_gemm_pair.txt: the synchronous version lost 20 points of
-// tensor-pipe activity on accumulating wgrads).
-template <typename OutT> struct CChunk;
-template <> struct CChunk<__nv_bfloat16> { using vec = uint4; uint4 v[4]; };   // 32 bf16
-template <> struct CChunk<float> { using vec = float4; float4 v[8]; };          // 32 fp32
-
-template <typename OutT>
-__device__ __forceinline__ void load_c_chunk(CChunk<OutT>& c, const OutT* crow, int ncols_valid) {
-  if (ncols_valid >= 32) {
-    using vec = typename CChunk<OutT>::vec;
-    const vec* p = reinterpret_cast<const vec*>(crow);
-#pragma unroll
-    for (int i = 0; i < static_cast<int>(sizeof(c.v) / sizeof(c.v[0])); ++i) c.v[i] = p[i];
-  }
-}
-
 // Epilogue extras of the bf16-output GEMM (nn.Linear(bias=True) + activation of the OPT family): v + bias[col]
-// (+ C) -> act. bias points at this chunk's 32 columns (16-byte aligned); act: 0 none, 1 ReLU.
+// (+ C) -> act. bias: [N] bf16; act: 0 none, 1 ReLU.
 // d2 (fp32-output GEMMs only): a second, bf16-rounded copy of the output with the same row stride -- the
 // last accumulation micro-step's wgrad writes the gradient's NCCL wire copy from the registers that hold the
-// fp32 sum, instead of a separate cast pass re-reading 27 GB (engine.cu exchange_one).
+// fp32 sum, instead of a separate cast pass re-reading the fp32 gradient (engine.cu exchange_one).
 struct EpiExtra {
   const __nv_bfloat16* bias;
   int act;
   __nv_bfloat16* d2;
 };
-__device__ __forceinline__ void apply_bias(float (&v)[32], const __nv_bfloat16* bias, int ncols_valid) {
-  if (ncols_valid >= 32) {
-    const uint4* bp = reinterpret_cast<const uint4*>(bias);   // same address in every thread: one broadcast load each
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint4 u = bp[i];
-      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = unpack_bf16x2(w[j]);
-        v[i * 8 + j * 2] += f.x;
-        v[i * 8 + j * 2 + 1] += f.y;
-      }
+
+// one output row's columns (col, col + 1); `two`: col + 1 < N. col is even and rows are 16-byte aligned, so
+// the pair is one 4-byte (bf16) or 8-byte (fp32) access.
+__device__ __forceinline__ void store_pair(__nv_bfloat16* d, const __nv_bfloat16* c, float v0, float v1, bool two,
+                                           const __nv_bfloat16* bias, int act, __nv_bfloat16* /*d2: fp32 only*/) {
+  if (two) {
+    if (bias) {
+      const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(bias));
+      v0 += b.x;
+      v1 += b.y;
     }
+    if (c) {
+      const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(c));
+      v0 += f.x;
+      v1 += f.y;
+    }
+    if (act == 1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+    *reinterpret_cast<uint32_t*>(d) = pack_bf16x2(v0, v1);
   } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (i < ncols_valid) v[i] += __bfloat162float(bias[i]);
+    if (bias) v0 += __bfloat162float(bias[0]);
+    if (c) v0 += __bfloat162float(c[0]);
+    if (act == 1) v0 = fmaxf(v0, 0.f);
+    d[0] = __float2bfloat16_rn(v0);
   }
 }
-
-__device__ __forceinline__ void store_chunk32(__nv_bfloat16* drow, const __nv_bfloat16* crow,
-                                              const CChunk<__nv_bfloat16>& cc, const float (&v)[32],
-                                              int ncols_valid, bool has_c, int act = 0,
-                                              __nv_bfloat16* /*d2row: fp32 outputs only*/ = nullptr) {
-  if (ncols_valid >= 32) {
-    uint4 out[4];
-    uint32_t* o = reinterpret_cast<uint32_t*>(out);
-    if (has_c) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t cw[4] = {cc.v[i].x, cc.v[i].y, cc.v[i].z, cc.v[i].w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 f = unpack_bf16x2(cw[j]);
-          float a0 = v[i * 8 + j * 2] + f.x, a1 = v[i * 8 + j * 2 + 1] + f.y;
-          if (act == 1) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-          o[i * 4 + j] = pack_bf16x2(a0, a1);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        float a0 = v[2 * i], a1 = v[2 * i + 1];
-        if (act == 1) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-        o[i] = pack_bf16x2(a0, a1);
-      }
+__device__ __forceinline__ void store_pair(float* d, const float* c, float v0, float v1, bool two,
+                                           const __nv_bfloat16* /*bias*/, int /*act*/, __nv_bfloat16* d2) {
+  if (two) {
+    if (c) {
+      const float2 f = *reinterpret_cast<const float2*>(c);
+      v0 += f.x;
+      v1 += f.y;
     }
-    uint4* d4 = reinterpret_cast<uint4*>(drow);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) d4[i] = out[i];
+    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
+    if (d2) *reinterpret_cast<uint32_t*>(d2) = pack_bf16x2(v0, v1);
   } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      if (i < ncols_valid) {
-        float x = v[i];
-        if (has_c) x += __bfloat162float(crow[i]);
-        if (act == 1) x = fmaxf(x, 0.f);
-        drow[i] = __float2bfloat16_rn(x);
-      }
-    }
+    if (c) v0 += c[0];
+    d[0] = v0;
+    if (d2) d2[0] = __float2bfloat16_rn(v0);
   }
 }
 
-__device__ __forceinline__ void store_chunk32(float* drow, const float* crow, const CChunk<float>& cc,
-                                              const float (&v)[32], int ncols_valid, bool has_c, int /*act*/ = 0,
-                                              __nv_bfloat16* d2row = nullptr) {
-  if (ncols_valid >= 32) {
-    float4* d4 = reinterpret_cast<float4*>(drow);
-    uint4* w4 = reinterpret_cast<uint4*>(d2row);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float4 o0 = make_float4(v[8 * i], v[8 * i + 1], v[8 * i + 2], v[8 * i + 3]);
-      float4 o1 = make_float4(v[8 * i + 4], v[8 * i + 5], v[8 * i + 6], v[8 * i + 7]);
-      if (has_c) {
-        const float4 c0 = cc.v[2 * i], c1 = cc.v[2 * i + 1];
-        o0.x += c0.x; o0.y += c0.y; o0.z += c0.z; o0.w += c0.w;
-        o1.x += c1.x; o1.y += c1.y; o1.z += c1.z; o1.w += c1.w;
-      }
-      d4[2 * i] = o0;
-      d4[2 * i + 1] = o1;
-      if (d2row)
-        w4[i] = make_uint4(pack_bf16x2(o0.x, o0.y), pack_bf16x2(o0.z, o0.w), pack_bf16x2(o1.x, o1.y),
-                           pack_bf16x2(o1.z, o1.w));
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (i < ncols_valid) {
-        const float o = v[i] + (has_c ? crow[i] : 0.f);
-        drow[i] = o;
-        if (d2row) d2row[i] = __float2bfloat16_rn(o);
-      }
-  }
+// PAIR: the CTA is one of a 2-CTA cluster that computes a 256 x 256 tile (the CTA of cluster rank r owns rows
+// [128 r, 128 r + 128)). The two CTAs need the same 256 x 64 B block per K step: each loads one half of it and
+// multicasts that half into both CTAs' stage, so B is read from L2 once per cluster instead of once per CTA. A stage
+// may be refilled only when BOTH CTAs' consumers are done with it, so every consumer warp releases it in both CTAs
+// (the free barriers count 16 arrivals), and the CTAs meet at a cluster barrier before the first remote operation
+// and before they exit.
+// a consumer warp is done with a stage: one arrival on its free barrier (in both CTAs of a pair)
+template <bool PAIR>
+__device__ __forceinline__ void release_stage(uint64_t* bar, uint32_t rank) {
+  mbar_arrive(bar);
+  if constexpr (PAIR) mbar_arrive_cluster(bar, rank ^ 1);
 }
 
-// TMEM accumulator rows -> global for one 128 x NCOLS tile half owned by this warp's lane quarter.
-template <int NCOLS, typename OutT>
-__device__ __forceinline__ void epilogue_tile(uint32_t tmem_row_addr, OutT* drow, const OutT* crow,
-                                              bool row_ok, int ncols_total,
-                                              EpiExtra ex = EpiExtra{nullptr, 0, nullptr}) {
-  const bool has_c = crow != nullptr;
-  CChunk<OutT> cc_next;
-  if (has_c && row_ok) load_c_chunk<OutT>(cc_next, crow, ncols_total);
-#pragma unroll 1
-  for (int c = 0; c < NCOLS / 32; ++c) {
-    const CChunk<OutT> cc = cc_next;
-    const int ncols = ncols_total - c * 32;
-    if (has_c && row_ok && c + 1 < NCOLS / 32) load_c_chunk<OutT>(cc_next, crow + (c + 1) * 32, ncols - 32);
-    uint32_t r[32];
-    tmem_ld32(tmem_row_addr + c * 32, r);
-    tmem_ld_wait();
-    if (row_ok && ncols > 0) {
-      float v[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-      if (ex.bias) apply_bias(v, ex.bias + c * 32, ncols);
-      store_chunk32(drow + c * 32, has_c ? crow + c * 32 : nullptr, cc, v, ncols, has_c, ex.act,
-                    ex.d2 ? ex.d2 + c * 32 : nullptr);
-    }
-  }
-}
-
-template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 OutT* D, const OutT* C, int M, int N, int K, int ldd, int n_fast, EpiExtra ex) {
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB, OutT* D, const OutT* C, int M,
+                                          int N, int K, int ldd, int n_fast, const EpiExtra& ex) {
   using cfg = Cfg<BLOCK_N>;
   constexpr int STAGES = cfg::STAGES;
+  constexpr int TILE_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;  // [2] accumulator ready for the epilogue
-  uint64_t* tempty_bar = tfull_bar + 2;      // [2] accumulator drained by the epilogue
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(tmA);
+    tma_prefetch_desc(tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 128);
+      mbar_init(&empty_bar[s], PAIR ? 16 : 8);  // one arrival per consumer warp (of both CTAs)
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, cfg::TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if constexpr (PAIR) cluster_sync_all();
+  else __syncthreads();
 
-  const int num_m = (M + BLOCK_M - 1) / BLOCK_M;
+  const int num_m = (M + TILE_M - 1) / TILE_M;
   const int num_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  const int first = PAIR ? (blockIdx.x >> 1) : blockIdx.x;
+  const int stride = PAIR ? (gridDim.x >> 1) : gridDim.x;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        // raster order: the operand that does NOT fit in L2 is made the slow index (launch())
+      for (int tile = first; tile < num_tiles; tile += stride) {
         int mi, ni;
         tile_coords(tile, num_m, num_n, n_fast, mi, ni);
-        const int m0 = mi * BLOCK_M, n0 = ni * BLOCK_N;
+        const int m0 = mi * TILE_M + rank * BLOCK_M, n0 = ni * BLOCK_N;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * cfg::STAGE_BYTES;
@@ -279,326 +188,172 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           mbar_arrive_expect_tx(&full_bar[stage], cfg::STAGE_BYTES);
           const int k0 = kb * BLOCK_K;
           if constexpr (!A_MN) {
-            tma_load_2d(sa, &tmA, &full_bar[stage], k0, m0);  // box [128 rows(m), 64 k]
+            tma_load_2d(sa, tmA, &full_bar[stage], k0, m0);  // box [128 rows(m), 64 k]
           } else {
             // global is [K rows, M cols]; one box = [64 k-rows, 64 m] = one MN atom column
 #pragma unroll
             for (int a = 0; a < BLOCK_M / 64; ++a)
-              tma_load_2d(sa + a * (BLOCK_K * 128), &tmA, &full_bar[stage], m0 + a * 64, k0);
+              tma_load_2d(sa + a * (BLOCK_K * 128), tmA, &full_bar[stage], m0 + a * 64, k0);
           }
-          if constexpr (!B_MN) {
-            tma_load_2d(sb, &tmB, &full_bar[stage], k0, n0);  // box [BLOCK_N rows(n), 64 k]
+          if constexpr (PAIR) {  // this CTA's half of B, into both CTAs
+            if constexpr (!B_MN) {
+              tma_load_2d_multicast(sb + rank * (BLOCK_N / 2) * 128, tmB, &full_bar[stage], k0,
+                                    n0 + rank * (BLOCK_N / 2), 0x3);  // box [128 rows(n), 64 k]
+            } else {
+#pragma unroll
+              for (int a = 0; a < BLOCK_N / 128; ++a) {
+                const int atom = rank * (BLOCK_N / 128) + a;
+                tma_load_2d_multicast(sb + atom * (BLOCK_K * 128), tmB, &full_bar[stage], n0 + atom * 64, k0, 0x3);
+              }
+            }
+          } else if constexpr (!B_MN) {
+            tma_load_2d(sb, tmB, &full_bar[stage], k0, n0);  // box [BLOCK_N rows(n), 64 k]
           } else {
 #pragma unroll
             for (int a = 0; a < BLOCK_N / 64; ++a)
-              tma_load_2d(sb + a * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + a * 64, k0);
+              tma_load_2d(sb + a * (BLOCK_K * 128), tmB, &full_bar[stage], n0 + a * 64, k0);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: convergent warp, elect.sync-predicated issue ==========
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BLOCK_N, A_MN, B_MN);
-      // K-major: next UMMA_K = +32 B inside the atom row. MN-major: next 16 K-rows = +2048 B.
-      constexpr uint32_t a_kstep = (A_MN ? (UMMA_K * 128) : (UMMA_K * 2)) >> 4;
-      constexpr uint32_t b_kstep = (B_MN ? (UMMA_K * 128) : (UMMA_K * 2)) >> 4;
-      constexpr uint32_t a_lbo = A_MN ? (BLOCK_K * 128) : 16;
-      constexpr uint32_t b_lbo = B_MN ? (BLOCK_K * 128) : 16;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * cfg::STAGE_BYTES);
-          const uint32_t a_lo = make_desc_lo(sa, a_lbo), b_lo = make_desc_lo(sa + A_STAGE_BYTES, b_lbo);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            tc_mma_bf16_elect(tmem_d, a_lo + k * a_kstep, b_lo + k * b_kstep, idesc, (kb | k) != 0);
-          tc_commit_elect(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_elect(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: TMEM -> registers -> global =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may touch
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  } else {
+    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the CTA's 128 ==========
+    const int wg = warp >> 2, wi = warp & 3;
+    constexpr uint32_t a_kstep = A_MN ? (WG_K * 128) : (WG_K * 2);
+    constexpr uint32_t b_kstep = B_MN ? (WG_K * 128) : (WG_K * 2);
+    constexpr uint32_t a_lbo = A_MN ? (BLOCK_K * 128) : 16;
+    constexpr uint32_t b_lbo = B_MN ? (BLOCK_K * 128) : 16;
+    float acc[BLOCK_N / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = first; tile < num_tiles; tile += stride) {
       int mi, ni;
       tile_coords(tile, num_m, num_n, n_fast, mi, ni);
-      const int m0 = mi * BLOCK_M, n0 = ni * BLOCK_N;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      __syncwarp();
-      tc_fence_after();
-      const int row = m0 + q * 32 + lane;
-      const bool row_ok = row < M;
-      OutT* drow = D + static_cast<size_t>(row) * ldd + n0;
-      const OutT* crow = C ? C + static_cast<size_t>(row) * ldd + n0 : nullptr;
-      epilogue_tile<BLOCK_N, OutT>(tmem_addr(tmem_base, q * 32, acc * BLOCK_N), drow, crow, row_ok, N - n0,
-                                   EpiExtra{ex.bias ? ex.bias + n0 : nullptr, ex.act,
-                                            ex.d2 ? ex.d2 + static_cast<size_t>(row) * ldd + n0 : nullptr});
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      const int m0 = mi * TILE_M + rank * BLOCK_M, n0 = ni * BLOCK_N;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * cfg::STAGE_BYTES);
+        const uint64_t da = wg_desc(sa + wg * A_HALF_BYTES, a_lbo), db = wg_desc(sa + A_STAGE_BYTES, b_lbo);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WG_K; ++k)
+          Wgmma<BLOCK_N>::template ss<A_MN, B_MN>(acc, desc_add(da, k * a_kstep), desc_add(db, k * b_kstep),
+                                                  (kb | k) != 0);
+        wg_commit();
+        // the previous k-block's MMAs have retired once at most this one is in flight: free its stage
+        wg_wait<1>();
+        if (prev >= 0 && lane == 0) release_stage<PAIR>(&empty_bar[prev], rank);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg_wait<0>();
+      wg_fence_regs(acc);
+      if (lane == 0) release_stage<PAIR>(&empty_bar[prev], rank);
+
+      // epilogue: registers -> global (the producer is already loading the next tile)
+      const int r0 = m0 + wg * 64 + wi * 16 + (lane >> 2);
+      const int c0 = n0 + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int col = c0 + 8 * j;
+        if (col >= N) continue;
+        const bool two = col + 1 < N;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= M) continue;
+          const size_t off = static_cast<size_t>(row) * ldd + col;
+          store_pair(D + off, C ? C + off : nullptr, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], two,
+                     ex.bias ? ex.bias + col : nullptr, ex.act, ex.d2 ? ex.d2 + off : nullptr);
+        }
+      }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, cfg::TMEM_COLS);
+  if constexpr (PAIR) {
+    __syncwarp();
+    cluster_sync_all();  // nobody leaves while the peer may still multicast into its smem or arrive on its barriers
   }
 }
 
-// ==========================================================================================
-// CTA-pair variant: cluster of 2 CTAs computes a 256 x 256 tile with tcgen05.mma.cta_group::2.
-// Each CTA stages its own 128 rows of A and HALF of B (128 of the 256 N columns), so per-SM
-// shared-memory traffic per MMA drops by a third and 6 pipeline stages fit instead of 4.
-// Barriers: full[] live in the leader (rank 0) and collect both CTAs' TMA bytes; empty[] and
-// tfull[] exist in both CTAs and are signalled by the leader's multicast tcgen05.commit;
-// tempty[] live in the leader and collect one arrival per epilogue warp of both CTAs.
-// ==========================================================================================
-constexpr int PAIR_N = 256;
-constexpr int PAIR_STAGE_BYTES = A_STAGE_BYTES + (PAIR_N / 2) * BLOCK_K * 2;  // 32 KB
-constexpr int PAIR_STAGES = 6;
-constexpr int PAIR_SMEM_BYTES = PAIR_STAGES * PAIR_STAGE_BYTES + 1024 + 256;
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 OutT* D, const OutT* C, int M, int N, int K, int ldd, int n_fast, EpiExtra ex) {
+  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(&tmA, &tmB, D, C, M, N, K, ldd, n_fast, ex);
+}
 
+// 256 x 256 tiles on a 2-CTA cluster with the B operand multicast (block_n = 512)
 template <bool A_MN, bool B_MN, typename OutT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       OutT* D, const OutT* C, int M, int N, int K, int ldd, int n_fast, EpiExtra ex) {
-  constexpr int STAGES = PAIR_STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * PAIR_STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;  // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;      // [2] (used in the leader only)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 8);  // 4 epilogue warps x 2 CTAs
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_pair(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();     // CTA-scope ordering of the tmem_slot write that racecheck can see (the cluster
-                       // barrier below already orders it; compute-sanitizer does not model that one)
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_m = (M + 255) / 256;
-  const int num_n = (N + PAIR_N - 1) / PAIR_N;
-  const int num_tiles = num_m * num_n;
-  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        int mi, ni;
-        tile_coords(tile, num_m, num_n, n_fast, mi, ni);
-        const int m0 = mi * 256 + rank * 128;                 // my 128 rows of A
-        const int n0 = ni * PAIR_N + rank * (PAIR_N / 2);     // my B half
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * PAIR_STAGE_BYTES;
-          uint8_t* sb = sa + A_STAGE_BYTES;
-          // only the leader's barrier counts bytes: both CTAs' TMA traffic lands on it
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * PAIR_STAGE_BYTES);
-          const int k0 = kb * BLOCK_K;
-          if constexpr (!A_MN) {
-            tma_load_2d_pair(sa, &tmA, &full_bar[stage], k0, m0);
-          } else {
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-              tma_load_2d_pair(sa + a * (BLOCK_K * 128), &tmA, &full_bar[stage], m0 + a * 64, k0);
-          }
-          if constexpr (!B_MN) {
-            tma_load_2d_pair(sb, &tmB, &full_bar[stage], k0, n0);  // box [128 rows(n), 64 k]
-          } else {
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-              tma_load_2d_pair(sb + a * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + a * 64, k0);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {  // CTA-uniform: the whole warp of the leader CTA runs the loop, one lane issues
-      constexpr uint32_t idesc = make_idesc_bf16(256, PAIR_N, A_MN, B_MN);
-      constexpr uint32_t a_kstep = (A_MN ? (UMMA_K * 128) : (UMMA_K * 2)) >> 4;
-      constexpr uint32_t b_kstep = (B_MN ? (UMMA_K * 128) : (UMMA_K * 2)) >> 4;
-      constexpr uint32_t a_lbo = A_MN ? (BLOCK_K * 128) : 16;
-      constexpr uint32_t b_lbo = B_MN ? (BLOCK_K * 128) : 16;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * PAIR_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * PAIR_STAGE_BYTES);
-          const uint32_t a_lo = make_desc_lo(sa, a_lbo), b_lo = make_desc_lo(sa + A_STAGE_BYTES, b_lbo);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            tc_mma_bf16_pair_elect(tmem_d, a_lo + k * a_kstep, b_lo + k * b_kstep, idesc, (kb | k) != 0);
-          tc_commit_pair_elect(&empty_bar[stage]);  // frees the slot in both CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_pair_elect(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-      int mi, ni;
-      tile_coords(tile, num_m, num_n, n_fast, mi, ni);
-      const int m0 = mi * 256 + rank * 128, n0 = ni * PAIR_N;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      __syncwarp();
-      tc_fence_after();
-      const int row = m0 + q * 32 + lane;
-      const bool row_ok = row < M;
-      OutT* drow = D + static_cast<size_t>(row) * ldd + n0;
-      const OutT* crow = C ? C + static_cast<size_t>(row) * ldd + n0 : nullptr;
-      epilogue_tile<PAIR_N, OutT>(tmem_addr(tmem_base, q * 32, acc * PAIR_N), drow, crow, row_ok, N - n0,
-                                  EpiExtra{ex.bias ? ex.bias + n0 : nullptr, ex.act,
-                                           ex.d2 ? ex.d2 + static_cast<size_t>(row) * ldd + n0 : nullptr});
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], 0);  // the leader's MMA thread waits on it
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncwarp();        // the .aligned cluster barrier wants whole warps
-  cluster_sync_all();  // nobody leaves while the peer may still touch its smem / barriers / TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
+  gemm_body<PAIR_N, A_MN, B_MN, OutT, true>(&tmA, &tmB, D, C, M, N, K, ldd, n_fast, ex);
 }
 
-template <bool A_MN, bool B_MN, typename OutT>
-void launch_pair(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, int K, int lda,
-                 int ldb, int ldd, EpiExtra ex, cudaStream_t stream) {
-  CUtensorMap tmA = A_MN ? make_tmap_bf16_2d(A, K, M, lda, BLOCK_K, 64)
-                         : make_tmap_bf16_2d(A, M, K, lda, BLOCK_M, BLOCK_K);
-  CUtensorMap tmB = B_MN ? make_tmap_bf16_2d(B, K, N, ldb, BLOCK_K, 64)
-                         : make_tmap_bf16_2d(B, N, K, ldb, PAIR_N / 2, BLOCK_K);
-  auto kern = gemm_bf16_pair_kernel<A_MN, B_MN, OutT>;
-  static PerDeviceOnce once;
-  once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR_SMEM_BYTES));
-  });
-  const int num_tiles = ((M + 255) / 256) * ((N + PAIR_N - 1) / PAIR_N);
-  const int max_clusters = (sm_count() - gemm_sm_reserve()) / 2;
-  const int clusters = num_tiles < max_clusters ? num_tiles : max_clusters;
-  kern<<<clusters * 2, GEMM_THREADS, PAIR_SMEM_BYTES, stream>>>(tmA, tmB, D, C, M, N, K, ldd,
-                                                                pick_raster(M, N, K, 256, PAIR_N), ex);
-  B200W_CUDA(cudaGetLastError());
-}
-
-template <typename OutT>
-void dispatch_pair(bool a_mn, bool b_mn, const void* A, const void* B, OutT* D, const OutT* C, int M,
-                   int N, int K, int lda, int ldb, int ldd, EpiExtra ex, cudaStream_t s) {
-  if (!a_mn && !b_mn) launch_pair<false, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else if (!a_mn && b_mn) launch_pair<false, true, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else if (a_mn && b_mn) launch_pair<true, true, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else launch_pair<true, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-}
-
-template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR = false>
 void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, int K, int lda,
             int ldb, int ldd, EpiExtra ex, cudaStream_t stream) {
   using cfg = Cfg<BLOCK_N>;
+  constexpr int TILE_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
   // A: K-major => global [M rows, K cols]; MN-major => global [K rows, M cols]
   CUtensorMap tmA = A_MN ? make_tmap_bf16_2d(A, K, M, lda, BLOCK_K, 64)
                          : make_tmap_bf16_2d(A, M, K, lda, BLOCK_M, BLOCK_K);
   CUtensorMap tmB = B_MN ? make_tmap_bf16_2d(B, K, N, ldb, BLOCK_K, 64)
-                         : make_tmap_bf16_2d(B, N, K, ldb, BLOCK_N, BLOCK_K);
-  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, OutT>;
+                         : make_tmap_bf16_2d(B, N, K, ldb, PAIR ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
+  void (*kern)(CUtensorMap, CUtensorMap, OutT*, const OutT*, int, int, int, int, int, EpiExtra);
+  if constexpr (PAIR) kern = gemm_bf16_pair_kernel<A_MN, B_MN, OutT>;
+  else kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, OutT>;
   static PerDeviceOnce once;  // per template instantiation
   once.run([&] {
     B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     cfg::SMEM_BYTES));
   });
-  const int num_tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BLOCK_N - 1) / BLOCK_N);
-  const int sms = sm_count() - gemm_sm_reserve();
-  const int grid = num_tiles < sms ? num_tiles : sms;
+  const int num_tiles = ((M + TILE_M - 1) / TILE_M) * ((N + BLOCK_N - 1) / BLOCK_N);
+  const int slots = (sm_count() - gemm_sm_reserve()) / (PAIR ? 2 : 1);
+  const int grid = (num_tiles < slots ? num_tiles : slots) * (PAIR ? 2 : 1);
   kern<<<grid, GEMM_THREADS, cfg::SMEM_BYTES, stream>>>(tmA, tmB, D, C, M, N, K, ldd,
-                                                        pick_raster(M, N, K, BLOCK_M, BLOCK_N), ex);
+                                                        pick_raster(M, N, K, TILE_M, BLOCK_N), ex);
   B200W_CUDA(cudaGetLastError());
 }
 
+// BLOCK_N = 512 selects the 2-CTA cluster kernel (256 x 256 tiles). Narrow tiles take any operand order: a B operand
+// read MN-major is loaded in 64-column swizzle atoms, so a 32-wide request with an MN-major B runs 64 wide.
 template <int BLOCK_N, typename OutT>
 void dispatch_major(bool a_mn, bool b_mn, const void* A, const void* B, OutT* D, const OutT* C,
                     int M, int N, int K, int lda, int ldb, int ldd, EpiExtra ex, cudaStream_t s) {
-  if constexpr (BLOCK_N < 128) {  // decode tiles: weights are always K-major there
-    B200W_CHECK(!a_mn && !b_mn, "narrow tiles support K-major operands only");
-    launch<BLOCK_N, false, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+  constexpr bool PAIR = BLOCK_N == 512;
+  constexpr int BN = PAIR ? PAIR_N : BLOCK_N;
+  if constexpr (BLOCK_N == 32) {
+    if (b_mn) {
+      dispatch_major<64, OutT>(a_mn, b_mn, A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    } else if (a_mn) {
+      launch<32, true, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    } else {
+      launch<32, false, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    }
     return;
+  } else {
+    if (!a_mn && !b_mn) launch<BN, false, false, OutT, PAIR>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    else if (!a_mn && b_mn) launch<BN, false, true, OutT, PAIR>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    else if (a_mn && b_mn) launch<BN, true, true, OutT, PAIR>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
+    else launch<BN, true, false, OutT, PAIR>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
   }
-  if (!a_mn && !b_mn) launch<BLOCK_N, false, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else if (!a_mn && b_mn) launch<BLOCK_N, false, true, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else if (a_mn && b_mn) launch<BLOCK_N, true, true, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
-  else launch<BLOCK_N, true, false, OutT>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, s);
 }
 
 }  // namespace
 
 // ==========================================================================================
 // Decode GEMM ("swap-AB"): out[M, N] = X[M, K] W[N, K]^T (+ C) for M <= 128 rows (a decode batch).
-// The weights are the 128-row A operand and the batch is a narrow B operand (UMMA N = MPAD), so
+// The weights are the 128-row A operand and the batch is a narrow B operand (wgmma N = MPAD), so
 // every byte a pipeline stage holds is a weight byte streamed from HBM — the job here is HBM
 // bandwidth, not tensor throughput. Grid = (N tiles, K splits): the 36-tile projections of a
 // 7B model are split along K so that all SMs stream. The K-splits of one output tile form a
 // THREAD-BLOCK CLUSTER: each CTA parks its fp32 partial tile in its own shared memory and, after a
 // cluster barrier, reduces 1/splits of the tile by reading the peers' copies over distributed shared
-// memory -- no global workspace, no atomics, no fences. (Round 2's first version met in global memory
-// through red.global.add: with 8 splits the 1.2 M same-address atomics of the K = 22720 GEMM cost
-// ~11 us of a 57 us launch, profiles/r02_ncu_decode.txt.)
+// memory -- no global workspace, no atomics, no fences (meeting in global memory through red.global.add
+// would put ~1.2 M same-address atomics into the K = 22720 GEMM of Falcon-7B at 8 splits).
 // ==========================================================================================
 // epilogue activation of the decode GEMM: 0 = none, 1 = exact (erf) GeLU -- transformers
 // get_activation("gelu"), what FalconMLP applies between its two projections -- 2 = ReLU (OPT)
@@ -647,11 +402,12 @@ struct DecodeCfg {
 
 // Programmatic dependent launch: every decode-step kernel is launched with the
 // programmatic-stream-serialization attribute. This kernel's CTAs become resident while the previous
-// kernel is still running, set up barriers / TMEM and -- the point -- fill their whole TMA pipeline with
+// kernel is still running, set up their barriers and -- the point -- fill their whole TMA pipeline with
 // WEIGHT tiles, which no kernel of the step writes; only then pdl_wait() (predecessor complete and
-// visible), and the activation tiles X follow. The ~5-8 us of launch latency + pipeline fill that each of
-// the ~130 GEMMs of a decode step used to expose (profiles/r02_decode_launches.txt: 33 us per launch for
-// a 6-25 us HBM floor) are spent under the predecessor instead.
+// visible), and the activation tiles X follow. The launch latency + pipeline fill that each of the
+// GEMMs of a decode step would otherwise expose is spent under the predecessor instead.
+// Warpgroup wg accumulates output features [64 wg, 64 wg + 64) of the 128-feature tile (the weights are
+// the wgmma A operand, the batch rows its N dimension) in registers.
 template <int MPAD>
 __global__ void __launch_bounds__(GEMM_THREADS, 2)
 gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
@@ -664,8 +420,6 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* done_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
   static_assert(MPAD * BLOCK_M * 4 <= STAGES * cfg::STAGE_BYTES, "the partial tile must fit in the pipeline stages");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -682,18 +436,13 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
-    mbar_init(done_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, MPAD < 32 ? 32 : MPAD);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // pipeline fill with weight tiles only (independent of the predecessor) ...
       const int pre = nkb < STAGES ? nkb : STAGES;
@@ -721,55 +470,57 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, MPAD, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * cfg::STAGE_BYTES);
-        const uint32_t a_lo = make_desc_lo(sa, 16), b_lo = make_desc_lo(sa + A_STAGE_BYTES, 16);
+  } else {
+    const int wg = warp >> 2, wi = warp & 3;
+    float acc[MPAD / 2];
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int i = 0; i < nkb; ++i) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * cfg::STAGE_BYTES);
+      const uint64_t da = wg_desc(sa + wg * A_HALF_BYTES, 16), db = wg_desc(sa + A_STAGE_BYTES, 16);
+      wg_fence();
 #pragma unroll
-        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-          tc_mma_bf16_elect(tmem_base, a_lo + k * 2, b_lo + k * 2, idesc, (i | k) != 0);
-        tc_commit_elect(&empty_bar[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      tc_commit_elect(done_bar);
+      for (int k = 0; k < BLOCK_K / WG_K; ++k)
+        Wgmma<MPAD>::template ss<0, 0>(acc, desc_add(da, k * WG_K * 2), desc_add(db, k * WG_K * 2), (i | k) != 0);
+      wg_commit();
+      wg_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    // lane of TMEM = output feature n; column = batch row b
-    const int q = warp & 3;
-    const int n = n0 + q * 32 + lane;
-    const bool n_ok = n < N;
-    pdl_wait();  // this warp reads C / writes out: both shared with the predecessor
-    mbar_wait(done_bar, 0);
-    __syncwarp();
-    tc_fence_after();
-    // every MMA has retired, so every pipeline stage has been consumed: the stage memory is free and holds
-    // this CTA's partial tile part[b][n_local] (fp32, MPAD x 128) for the cluster reduction
-    float* part = reinterpret_cast<float*>(smem);
-    uint32_t r[32];
-#pragma unroll 1
-    for (int c = 0; c < MPAD / 32; ++c) {
-      tmem_ld32(tmem_addr(tmem_base, q * 32, c * 32), r);
-      tmem_ld_wait();
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    pdl_wait();  // C is read / out written below: both shared with the predecessor
+    // acc[4 j + 2 h + e]: output feature nl = 64 wg + 16 wi + lane / 4 + 8 h of the tile, batch row b = 8 j + 2 (lane % 4) + e
+    const int nl0 = wg * 64 + wi * 16 + (lane >> 2);
+    if (split) {
+      // every MMA of BOTH warpgroups must have read its stages before the stage memory holds this CTA's
+      // partial tile part[b][n_local] (fp32, MPAD x 128) for the cluster reduction
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      float* part = reinterpret_cast<float*>(smem);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int b = c * 32 + j;
-        const float v = __uint_as_float(r[j]);
-        if (split) part[b * BLOCK_M + q * 32 + lane] = v;   // 32 lanes -> 128 contiguous bytes: conflict-free
-        else if (n_ok && b < M) decode_store(epi, b, n, v);
-      }
+      for (int j = 0; j < MPAD / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) part[(8 * j + 2 * (lane & 3) + e) * BLOCK_M + nl0 + 8 * h] = acc[4 * j + 2 * h + e];
+    } else {
+#pragma unroll
+      for (int j = 0; j < MPAD / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = n0 + nl0 + 8 * h, b = 8 * j + 2 * (lane & 3) + e;
+            if (n < N && b < M) decode_store(epi, b, n, acc[4 * j + 2 * h + e]);
+          }
     }
   }
   if (split) {
     // cluster = the K-splits of this N tile. After the barrier CTA `rank` owns output features
     // [rank * 128 / splits, (rank + 1) * 128 / splits) of the tile and sums them over all the peers' partials.
     const uint32_t nsplit = gridDim.y, rank = cluster_ctarank();
-    tc_fence_before();
     __syncwarp();
     cluster_sync_all();
     const float* part = reinterpret_cast<const float*>(smem);
@@ -785,12 +536,6 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     }
     __syncwarp();
     cluster_sync_all();  // nobody leaves while a peer may still read its partial tile
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, MPAD < 32 ? 32 : MPAD);
   }
 }
 
@@ -818,12 +563,8 @@ int max_active_decode_clusters(int splits) {
     lc.numAttrs = 1;
     int n = 0;
     B200W_CUDA(cudaOccupancyMaxActiveClusters(&n, gemm_decode_kernel<MPAD>, &lc));
-    // The occupancy queries answer for ONE CTA of this kernel per SM (measured on B200: 74 / 45 / 33 / 26 / 22 /
-    // 15 / 15 clusters of 2..8 CTAs, i.e. 148 CTAs at size 2; cudaOccupancyMaxActiveBlocksPerMultiprocessor = 1),
-    // although two 101 KB CTAs fit the 228 KB of an SM and ncu reports two resident
-    // (launch__occupancy_limit_shared_mem = 2, profiles/r02_ncu_decode.txt). Same-box sweeps agree with TWICE the
-    // figure: 36 clusters of 4, 5 or 6 CTAs run as one wave (3.21-3.50 ms per decode step on two boxes), 36
-    // clusters of 7 or 8 do not (3.55-3.78 ms) -- profiles/r02_decode_split_sweep.txt.
+    // Two ~101 KB CTAs fit the 228 KB of an SM. When the cluster query answers for only one CTA per SM (no more
+    // CTAs in its clusters than the device has SMs), the second resident CTA is counted here.
     int smem_sm = 0, dev2 = 0;
     B200W_CUDA(cudaGetDevice(&dev2));
     B200W_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev2));
@@ -851,11 +592,9 @@ void launch_decode(const void* X, int ldx, const void* W, int ldw, const void* w
   const int n_tiles = (N + BLOCK_M - 1) / BLOCK_M;
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
   // split K until two CTAs per SM are in flight, keeping at least 8 K-blocks per split; the splits of a tile
-  // are one cluster (portable size limit 8). A cluster lives inside one GPC (16-20 SMs): 8-CTA clusters at 2
-  // CTAs per SM do not tile every GPC, and when the clusters of a launch exceed what the chip holds at once the
-  // stragglers run as a second wave on a nearly idle machine (ncu, profiles/r02_ncu_decode_tiled.txt: the
-  // 36 x 8 launch of Falcon's [dense | 4h_to_h] took 55.5 us against 43 us for the same bytes unsplit). So
-  // the split is the LARGEST one whose clusters are all co-resident (cudaOccupancyMaxActiveClusters).
+  // are one cluster (portable size limit 8). A cluster lives inside one GPC: when the clusters of a launch exceed
+  // what the chip holds at once, the stragglers run as a second wave on a nearly idle machine. So the split is
+  // the LARGEST one whose clusters are all co-resident (cudaOccupancyMaxActiveClusters).
   int splits = 1;
   if (allow_split) {
     int want = 2 * sm_count() / n_tiles;
@@ -926,24 +665,23 @@ void retile_weights(const void* W, int ldw, void* out, int N, int K, cudaStream_
 
 // Tile raster order. M-fastest re-reads A once per wave of N-tiles unless A stays in L2; N-fastest
 // does the same to B. Keep the order whose re-streamed operand fits in L2, else re-stream the
-// smaller one. (profiles/r01_ncu_gemm_pair.txt: wgrad of gate|up read 2.9 GB for 214 MB of
-// operands with the wrong order.)
+// smaller one. (With the wrong order the wgrad of Llama-2-7B's gate|up re-streams its 180 MB
+// operand once per wave.)
 static int pick_n_fast(int M, int N, int K) {
-  const double a_bytes = 2.0 * M * K, b_bytes = 2.0 * N * K, l2_budget = 64e6;
+  const double a_bytes = 2.0 * M * K, b_bytes = 2.0 * N * K, l2_budget = 25e6;   // half of H100's 50 MB L2
   if (a_bytes <= l2_budget) return 0;
   if (b_bytes <= l2_budget) return 1;
   return b_bytes < a_bytes ? 1 : 0;
 }
 
-// Raster for tile_coords. An operand that every wave of tiles re-reads stays in L2 only up to ~34 MB: B200's 126 MB
-// L2 is two partitions, and at micro-batch 2 the 67 MB operands of the Llama-2-7B GEMMs (M = 8192 x K = 4096 bf16)
-// were re-fetched wave after wave -- ncu --set full at M = 8192 before this: 2.76x / 2.06x the algorithmic DRAM bytes
-// for the gate|up forward / accumulating wgrad against 1.04x / 1.07x at M = 4096 (profiles/r02_ncu_gemm_mb2.json,
-// r02_ncu_gemm.json). Cost model: the fast-dimension operand is read once, the other once per band.
+// Raster for tile_coords. An operand that every wave of tiles re-reads stays in L2 only while it is well inside
+// one of H100's two 25 MB L2 partitions: at micro-batch 2 the 67 MB operands of the Llama-2-7B GEMMs (M = 8192 x
+// K = 4096 bf16) would be re-fetched wave after wave. Bands of panels of ~13.5 MB in total are swept instead.
+// Cost model: the fast-dimension operand is read once, the other once per band.
 static int pick_raster(int M, int N, int K, int tile_m, int tile_n) {
   static const bool grouped = [] { const char* v = getenv("B200W_GEMM_RASTER_BANDS"); return !(v && v[0] == '0'); }();
-  static const double budget = [] { const char* v = getenv("B200W_GEMM_BAND_MB"); return (v ? atof(v) : 34.0) * 1e6; }();
-  const double a = 2.0 * M * K, b = 2.0 * N * K, resident = 40e6, max_panel = 8.5e6;
+  static const double budget = [] { const char* v = getenv("B200W_GEMM_BAND_MB"); return (v ? atof(v) : 13.5) * 1e6; }();
+  const double a = 2.0 * M * K, b = 2.0 * N * K, resident = 16e6, max_panel = 3.4e6;
   const double pa = 2.0 * tile_m * K, pb = 2.0 * tile_n * K;
   auto bands = [&](double fast, double panel) -> double {
     if (fast <= resident) return 1.0;
@@ -954,9 +692,9 @@ static int pick_raster(int M, int N, int K, int tile_m, int tile_n) {
   const double ga = bands(a, pa), gb = bands(b, pb);
   static const bool square = [] { const char* v = getenv("B200W_GEMM_LONGK_SQUARE"); return !(v && v[0] == '0'); }();
   if (grouped && square && ga < 0 && gb < 0) {
-    // long K: no band of panels can stay resident, but the ~74 tiles in flight march through K together and share
+    // long K: no band of panels can stay resident, but the tiles in flight march through K together and share
     // the k-slices they are on, so a wave costs (rows + columns of tiles it spans) panels: make the wave square
-    // (8 x ~9 tiles) instead of a 16 x 4.6 strip -- 17 panels per wave instead of 20.6
+    // (8 tiles wide) instead of a long strip
     const int n_fast = pick_n_fast(M, N, K);
     const int fast_tiles = n_fast ? (N + tile_n - 1) / tile_n : (M + tile_m - 1) / tile_m;
     return n_fast | ((fast_tiles >= 12 ? 8 : 0) << 1);
@@ -1003,7 +741,7 @@ void gemm_decode(const void* X, const void* W, void* out, const void* C, float* 
 }
 
 // Public launcher (C++). out_fp32: D/C are float, else bf16. C may alias D (accumulate in place).
-// block_n: 0 = auto, else 128 or 256.
+// block_n: 0 = auto, 32 / 64 / 128 / 256 = 128 x block_n tiles, 512 = 256 x 256 tiles on a 2-CTA cluster.
 void gemm_bf16(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
                const void* C, bool out_fp32, int ldd, int M, int N, int K, int block_n,
                cudaStream_t stream) {
@@ -1026,12 +764,6 @@ void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, i
                   (reinterpret_cast<uintptr_t>(D) & 15) == 0,
               "operands must be 16-byte aligned");
   if (block_n == 0) {
-    // Large problems: CTA pairs (256 x 256 tiles, cta_group::2) — measured 8-11 % faster than the
-    // single-CTA kernel at Llama-2-7B shapes (profiles/r01_perf_probe_pair.json).
-    const long tiles_pair = static_cast<long>((M + 255) / 256) * ((N + 255) / 256);
-    if (M >= 256 && N >= 256 && tiles_pair >= sm_count() / 2) block_n = 512;
-  }
-  if (block_n == 0) {
     // widest tile that still gives every SM a tile; K-major-only narrow tiles when M fits one tile
     const long m_tiles = (M + 127) / 128;
     const bool narrow_ok = !a_mn && !b_mn && !out_fp32;
@@ -1041,44 +773,23 @@ void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, i
       if (N >= bn && m_tiles * ((N + bn - 1) / bn) >= sm_count()) { block_n = bn; break; }
     }
   }
-  if (block_n == 512) {  // CTA-pair kernel: 256 x 256 tiles on tcgen05.mma.cta_group::2
-    if (out_fp32)
-      dispatch_pair<float>(a_mn, b_mn, A, B, static_cast<float*>(D), static_cast<const float*>(C), M, N,
-                           K, lda, ldb, ldd, ex, stream);
-    else
-      dispatch_pair<__nv_bfloat16>(a_mn, b_mn, A, B, static_cast<__nv_bfloat16*>(D),
-                                   static_cast<const __nv_bfloat16*>(C), M, N, K, lda, ldb, ldd, ex, stream);
-    return;
-  }
-  B200W_CHECK(block_n == 32 || block_n == 64 || block_n == 128 || block_n == 256,
-              "block_n must be 0, 32, 64, 128, 256 or 512 (CTA pair)");
-  if (block_n < 128) {
-    B200W_CHECK(!out_fp32, "narrow tiles write bf16");
-    if (block_n == 64)
-      dispatch_major<64, __nv_bfloat16>(a_mn, b_mn, A, B, static_cast<__nv_bfloat16*>(D),
-                                        static_cast<const __nv_bfloat16*>(C), M, N, K, lda, ldb, ldd, ex, stream);
-    else
-      dispatch_major<32, __nv_bfloat16>(a_mn, b_mn, A, B, static_cast<__nv_bfloat16*>(D),
-                                        static_cast<const __nv_bfloat16*>(C), M, N, K, lda, ldb, ldd, ex, stream);
-    return;
-  }
-  if (out_fp32) {
-    if (block_n == 256)
-      dispatch_major<256, float>(a_mn, b_mn, A, B, static_cast<float*>(D),
-                                 static_cast<const float*>(C), M, N, K, lda, ldb, ldd, ex, stream);
-    else
-      dispatch_major<128, float>(a_mn, b_mn, A, B, static_cast<float*>(D),
-                                 static_cast<const float*>(C), M, N, K, lda, ldb, ldd, ex, stream);
-  } else {
-    if (block_n == 256)
-      dispatch_major<256, __nv_bfloat16>(a_mn, b_mn, A, B, static_cast<__nv_bfloat16*>(D),
-                                         static_cast<const __nv_bfloat16*>(C), M, N, K, lda, ldb,
-                                         ldd, ex, stream);
-    else
-      dispatch_major<128, __nv_bfloat16>(a_mn, b_mn, A, B, static_cast<__nv_bfloat16*>(D),
-                                         static_cast<const __nv_bfloat16*>(C), M, N, K, lda, ldb,
-                                         ldd, ex, stream);
-  }
+  B200W_CHECK(block_n == 32 || block_n == 64 || block_n == 128 || block_n == 256 || block_n == 512,
+              "block_n must be 0, 32, 64, 128, 256 or 512 (2-CTA cluster)");
+  B200W_CHECK(block_n >= 128 || !out_fp32, "narrow tiles write bf16");
+  auto run = [&](auto out_tag) {
+    using T = decltype(out_tag);
+    T* d = static_cast<T*>(D);
+    const T* c = static_cast<const T*>(C);
+    switch (block_n) {
+      case 32: dispatch_major<32, T>(a_mn, b_mn, A, B, d, c, M, N, K, lda, ldb, ldd, ex, stream); break;
+      case 64: dispatch_major<64, T>(a_mn, b_mn, A, B, d, c, M, N, K, lda, ldb, ldd, ex, stream); break;
+      case 128: dispatch_major<128, T>(a_mn, b_mn, A, B, d, c, M, N, K, lda, ldb, ldd, ex, stream); break;
+      case 256: dispatch_major<256, T>(a_mn, b_mn, A, B, d, c, M, N, K, lda, ldb, ldd, ex, stream); break;
+      default: dispatch_major<512, T>(a_mn, b_mn, A, B, d, c, M, N, K, lda, ldb, ldd, ex, stream); break;
+    }
+  };
+  if (out_fp32) run(float{});
+  else run(__nv_bfloat16{});
 }
 
 // Host-side view of the tile raster for tests (no device needed): the raster word pick_raster chooses for a shape and,

@@ -1,5 +1,5 @@
 // Server engine (SURVEY.md 8 a14; started by server_controller.go:149-173): prompt PREFILL in one pass
-// (big-M tcgen05 GEMMs + the training flash-attention forward) and batched greedy DECODE, one new token
+// (big-M wgmma GEMMs + the training flash-attention forward) and batched greedy DECODE, one new token
 // per cache slot per step. Families:
 //   FALCON  (HF models/falcon/modeling_falcon.py, falcon-7b layout: multi_query, parallel_attn,
 //            one input_layernorm per layer, bias-free linears, LayerNorm with bias, exact GeLU,
@@ -10,14 +10,14 @@
 //            (test/system.sh:46-78, examples/facebook-opt-125m/base-server.yaml)
 // Decode at batch 32 is HBM-bound on the weights (SURVEY.md 8d: 13.84 GB per step for Falcon-7B).
 // What the step is built from:
-//   * swap-AB split-K tcgen05 GEMM (gemm.cu gemm_decode_kernel): every byte a pipeline stage holds is a
+//   * swap-AB split-K wgmma GEMM (gemm.cu gemm_decode_kernel): every byte a pipeline stage holds is a
 //     weight byte. Falcon's parallel block needs only TWO of them per layer: [q k v | dense_h_to_4h]
 //     share the LayerNorm output (one launch, N = 22848) and [dense | dense_4h_to_h] share the residual
 //     sum (one launch over the K-concatenated operand [attention out | gelu(h_to_4h)], K = 22720).
 //   * programmatic dependent launch through the whole step: each kernel's CTAs are resident and -- for
 //     the GEMMs -- already streaming weights while the predecessor finishes.
 //   * MQA/GQA decode attention ON THE TENSOR CORES (decode_attn_tc_kernel): the query heads that share a
-//     kv head are the M dimension of a tcgen05 MMA (Falcon-7B: 71 of 128 rows), S = Q K^T and O = P V
+//     kv head are the M dimension of a wgmma tile (Falcon-7B: 71 of 128 rows), S = Q K^T and O = P V
 //     per 128-key block, partial (max, sum, O) per block merged by a second kernel.
 #include <math.h>
 #include <math.h>
@@ -372,20 +372,21 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
-// Decode attention on tcgen05 for grouped / multi-query models. CTA = (128-key block, kv head, row).
-// The G = H / Hkv query heads of the group are rows of a 128-row MMA tile (zero rows above G):
-//   S[128, 128 keys] = Q K^T   (A = Q K-major from smem, B = K block K-major, TMA from the cache)
-//   P = 2^(S * scale_log2 - m) per head row (thread = TMEM lane), keys >= len masked to 0, bf16 -> smem
-//   O[128, DH] = P V           (A = P K-major, B = V block MN-major)
+// Decode attention on the tensor cores (wgmma) for grouped / multi-query models. CTA = (128-key block,
+// kv head, row). The G = H / Hkv query heads of the group are rows of a 128-row tile (zero rows above G),
+// warpgroup wg owning rows [64 wg, 64 wg + 64) (a warpgroup whose rows are all padding has nothing to do):
+//   S[64, 128 keys] = Q K^T   (A = Q K-major from smem, B = K block K-major, TMA from the cache)
+//   P = 2^(S * scale_log2 - m) per head row, keys >= len masked to 0, bf16 in registers
+//   O[64, DH] = P V           (A = P from registers, B = V block MN-major)
 // and the block's (m, l, O) go to a small fp32 workspace; decode_attn_merge_kernel combines the blocks
-// of a row. Every barrier is used exactly once (parity 0). The KV cache is zero-initialised, so rows of
-// the last block beyond `len` are finite (stale or zero) and their P is exactly 0.
+// of a row. The KV cache is zero-initialised, so rows of the last block beyond `len` are finite (stale or
+// zero) and their P is exactly 0.
 // ------------------------------------------------------------------------------------------------
 constexpr int TC_KB = 128;          // keys per CTA
-constexpr int TC_THREADS = 160;     // warps 0-3: one thread per head row; warp 4: TMA + MMA issue + TMEM
+constexpr int TC_THREADS = 256;     // two warpgroups; thread 0 also issues the TMA loads
 constexpr int TC_ATOM = 128 * 128;  // bytes of a [128 rows x 128 B] swizzle atom
 template <int DH>
-constexpr int tc_smem_bytes() { return (3 * (DH / 64) + 2) * TC_ATOM + 1024 + 64; }
+constexpr int tc_smem_bytes() { return 3 * (DH / 64) * TC_ATOM + 1024 + 64; }
 
 __device__ __forceinline__ float ex2f(float x) {
   float y;
@@ -394,14 +395,14 @@ __device__ __forceinline__ float ex2f(float x) {
 }
 
 template <int DH>
-__global__ void __launch_bounds__(TC_THREADS, DH == 64 ? 2 : 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                       const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
                       const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
                       int H, int Hkv, int max_ctx, int nsplit, float scale_log2) {
   constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
   const int split = blockIdx.x, hk = blockIdx.y, r = blockIdx.z;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
   if (tid == 0) pdl_trigger();
   pdl_wait();  // q / cache rows / pos come from the kernels before this one
   const int len = pos[r] + 1;
@@ -415,153 +416,108 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
   uint8_t* sQ = smem;                  // NA atoms [128 head rows x 128 B]
   uint8_t* sK = sQ + NA * TC_ATOM;     // NA atoms [128 keys x 128 B]
   uint8_t* sV = sK + NA * TC_ATOM;     // NA atoms [128 keys x 128 B] (MN-major B: N = dh)
-  uint8_t* sP = sV + NA * TC_ATOM;     // 2 atoms  [128 head rows x 64 keys]
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sP + 2 * TC_ATOM);
-  uint64_t* bar_q = bar_kv + 1;   // Q rows written (128 arrivals)
-  uint64_t* bar_s = bar_q + 1;    // S in TMEM
-  uint64_t* bar_p = bar_s + 1;    // P in smem (128 arrivals)
-  uint64_t* bar_o = bar_p + 1;    // O in TMEM
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_o + 1);
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sV + NA * TC_ATOM);
 
   if (tid == 0) {
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
     mbar_init(bar_kv, 1);
-    mbar_init(bar_q, 128);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, 128);
-    mbar_init(bar_o, 1);
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_O = tmem_base + 128;
-
-  if (warp == 4) {
-    // ---- control warp (convergent; one elected lane issues) ----
+  if (tid == 0) {
     const int row0 = slot[r] * max_ctx + k0;  // first cache row of this block
-    if ((tid & 31) == 0) {
-      mbar_arrive_expect_tx(bar_kv, 2 * NA * TC_ATOM);
+    mbar_arrive_expect_tx(bar_kv, 2 * NA * TC_ATOM);
 #pragma unroll
-      for (int a = 0; a < NA; ++a) {
-        tma_load_2d(sK + a * TC_ATOM, &tm_k, bar_kv, hk * DH + a * 64, row0);
-        tma_load_2d(sV + a * TC_ATOM, &tm_v, bar_kv, hk * DH + a * 64, row0);
-      }
-    }
-    __syncwarp();
-    constexpr uint32_t idesc_s = make_idesc_bf16(128, TC_KB, false, false);
-    constexpr uint32_t idesc_o = make_idesc_bf16(128, DH, false, true);
-    constexpr uint32_t A16 = TC_ATOM >> 4;
-    const uint32_t q_lo = make_desc_lo(smem_u32(sQ), 16), k_lo = make_desc_lo(smem_u32(sK), 16);
-    const uint32_t p_lo = make_desc_lo(smem_u32(sP), 16), v_lo = make_desc_lo(smem_u32(sV), TC_ATOM);
-    mbar_wait(bar_q, 0);
-    mbar_wait(bar_kv, 0);
-    tc_fence_after();
-#pragma unroll
-    for (int k = 0; k < DH / 16; ++k)  // S = Q K^T over dh: 32 B steps inside an atom row, then the next atom
-      tc_mma_bf16_elect(tmem_base, q_lo + (k / 4) * A16 + (k % 4) * 2, k_lo + (k / 4) * A16 + (k % 4) * 2, idesc_s,
-                        k != 0);
-    tc_commit_elect(bar_s);
-    mbar_wait(bar_p, 0);
-    tc_fence_after();
-#pragma unroll
-    for (int k = 0; k < TC_KB / 16; ++k)  // O = P V over the 128 keys: A steps as above, B 16 key rows = 2048 B
-      tc_mma_bf16_elect(tmem_O, p_lo + (k / 4) * A16 + (k % 4) * 2, v_lo + k * (2048 >> 4), idesc_o, k != 0);
-    tc_commit_elect(bar_o);
-  } else {
-    // ---- compute: thread = head row g of the group ----
-    const int g = tid;  // 0..127
-    {
-      const bool real = g < G;
-      const uint4* src = reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(r) * ld + (hk * G + (real ? g : 0)) * DH);
-#pragma unroll
-      for (int c = 0; c < DH / 8; ++c) {
-        const uint4 v = real ? src[c] : make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4*>(sQ + (c / 8) * TC_ATOM + sw128_offset(g, c % 8)) = v;
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(bar_q);
-    }
-    const uint32_t lane_base = ((warp * 32u) << 16);
-    mbar_wait(bar_s, 0);
-    __syncwarp();
-    tc_fence_after();
-    const int valid = min(TC_KB, len - k0);
-    // pass 1: row maximum (S is re-read from TMEM in pass 2: cheaper than 128 live registers)
-    float m = -INFINITY;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t sr[32];
-      tmem_ld32(tmem_base + lane_base + c * 32, sr);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (c * 32 + j < valid) m = fmaxf(m, __uint_as_float(sr[j]));
-    }
-    m *= scale_log2;  // scale > 0 commutes with max; key 0 of the block is always valid, so m is finite
-    // pass 2: P = 2^(S * scale_log2 - m), masked keys exactly 0, as bf16 into the K-major staging tile
-    float l = 0.f;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t sr[32];
-      tmem_ld32(tmem_base + lane_base + c * 32, sr);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j8 = 0; j8 < 4; ++j8) {
-        uint32_t w[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int j = j8 * 8 + 2 * e;
-          float p0 = ex2f(fmaf(__uint_as_float(sr[j]), scale_log2, -m));
-          float p1 = ex2f(fmaf(__uint_as_float(sr[j + 1]), scale_log2, -m));
-          if (c * 32 + j >= valid) p0 = 0.f;
-          if (c * 32 + j + 1 >= valid) p1 = 0.f;
-          // the row sum runs over the bf16-rounded values the PV product will see
-          const uint32_t pk = pack_bf16x2(p0, p1);
-          const float2 pr = unpack_bf16x2(pk);
-          l += pr.x + pr.y;
-          w[e] = pk;
-        }
-        const int key8 = c * 4 + j8;  // 16-byte chunk index along the 128 keys
-        *reinterpret_cast<uint4*>(sP + (key8 / 8) * TC_ATOM + sw128_offset(g, key8 % 8)) =
-            make_uint4(w[0], w[1], w[2], w[3]);
-      }
-    }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    mbar_arrive(bar_p);
-    mbar_wait(bar_o, 0);
-    __syncwarp();
-    tc_fence_after();
-    if (warp * 32 < G) {  // warp-uniform: the .sync.aligned TMEM loads need all 32 lanes; stores are per row
-      const bool real = g < G;
-      const int h = hk * G + (real ? g : 0);
-      const size_t pidx = (static_cast<size_t>(r) * H + h) * nsplit + split;
-      if (real) part_ml[pidx] = make_float2(m, l);
-      float* po = part_o + pidx * DH;
-#pragma unroll
-      for (int c = 0; c < DH / 32; ++c) {
-        uint32_t o[32];
-        tmem_ld32(tmem_O + lane_base + c * 32, o);
-        tmem_ld_wait();
-        if (real) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            reinterpret_cast<float4*>(po + c * 32)[i] =
-                make_float4(__uint_as_float(o[4 * i]), __uint_as_float(o[4 * i + 1]),
-                            __uint_as_float(o[4 * i + 2]), __uint_as_float(o[4 * i + 3]));
-        }
-      }
+    for (int a = 0; a < NA; ++a) {
+      tma_load_2d(sK + a * TC_ATOM, &tm_k, bar_kv, hk * DH + a * 64, row0);
+      tma_load_2d(sV + a * TC_ATOM, &tm_v, bar_kv, hk * DH + a * 64, row0);
     }
   }
-  tc_fence_before();
+  // the group's query rows (zero above G) -> the K-major A tile
+  for (int i = tid; i < 128 * (DH / 8); i += TC_THREADS) {
+    const int g = i / (DH / 8), c = i % (DH / 8);
+    const uint4 v = g < G ? reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(r) * ld + (hk * G + g) * DH)[c]
+                          : make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4*>(sQ + (c / 8) * TC_ATOM + sw128_offset(g, c % 8)) = v;
+  }
+  fence_proxy_async_smem();
   __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+  const int wg = tid >> 7, wi = (tid >> 5) & 3;
+  if (wg * 64 >= G) return;  // warpgroup-uniform: every row of this warpgroup is padding
+  mbar_wait(bar_kv, 0);
+
+  float s[TC_KB / 2];
+  {
+    const uint64_t da = wg_desc(smem_u32(sQ) + wg * 64 * 128, 16), db = wg_desc(smem_u32(sK), 16);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < DH / 16; ++kk)  // over dh: 32 B steps inside an atom row, then the next atom
+      Wgmma<TC_KB>::template ss<0, 0>(s, desc_add(da, (kk / 4) * TC_ATOM + (kk % 4) * 32),
+                                      desc_add(db, (kk / 4) * TC_ATOM + (kk % 4) * 32), kk != 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(s);
+  }
+  const int valid = min(TC_KB, len - k0);
+  const int c0 = 2 * (lane & 3);
+  float m[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int jj = 0; jj < TC_KB / 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      if (8 * jj + c0 + e < valid) {
+        m[0] = fmaxf(m[0], s[4 * jj + e]);
+        m[1] = fmaxf(m[1], s[4 * jj + 2 + e]);
+      }
+  float l[2] = {0.f, 0.f};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+    m[h] *= scale_log2;  // scale > 0 commutes with max; key 0 of the block is always valid, so m is finite
+  }
+  uint32_t pa[TC_KB / 16][4];
+#pragma unroll
+  for (int jj = 0; jj < TC_KB / 8; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float p0 = ex2f(fmaf(s[4 * jj + 2 * h], scale_log2, -m[h]));
+      float p1 = ex2f(fmaf(s[4 * jj + 2 * h + 1], scale_log2, -m[h]));
+      if (8 * jj + c0 >= valid) p0 = 0.f;
+      if (8 * jj + c0 + 1 >= valid) p1 = 0.f;
+      // the row sum runs over the bf16-rounded values the PV product will see
+      const uint32_t pk = pack_bf16x2(p0, p1);
+      const float2 pr = unpack_bf16x2(pk);
+      l[h] += pr.x + pr.y;
+      pa[jj / 2][(jj & 1) * 2 + h] = pk;  // A fragment of the K = 16 slice jj / 2 (to_afrag's layout)
+    }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+  }
+  float o[DH / 2];
+  {
+    const uint64_t dv = wg_desc(smem_u32(sV), TC_ATOM);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < TC_KB / 16; ++kk)  // over the 128 keys: 16 key rows = 2048 B
+      Wgmma<DH>::template rs<1>(o, pa[kk], desc_add(dv, kk * 2048), kk != 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(o);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int g = wg * 64 + wi * 16 + (lane >> 2) + 8 * h;
+    if (g >= G) continue;
+    const size_t pidx = (static_cast<size_t>(r) * H + hk * G + g) * nsplit + split;
+    if ((lane & 3) == 0) part_ml[pidx] = make_float2(m[h], l[h]);
+    float* po = part_o + pidx * DH + c0;
+#pragma unroll
+    for (int jj = 0; jj < DH / 8; ++jj)
+      *reinterpret_cast<float2*>(po + 8 * jj) = make_float2(o[4 * jj + 2 * h], o[4 * jj + 2 * h + 1]);
   }
 }
 
@@ -579,7 +535,7 @@ __global__ void decode_attn_merge_kernel(const float* __restrict__ part_o, const
   const int ns = (pos[r] + TC_KB) / TC_KB;  // ceil((pos + 1) / 128)
   const size_t base = (static_cast<size_t>(r) * H + h) * nsplit;
   // one pass, four blocks at a time with every load issued before the first use: the loop is a chain of
-  // L2 round trips otherwise (6.3 us per launch in profiles/r02_decode_launches_v1.txt for ~100 KB of data).
+  // L2 round trips otherwise.
   // Online form: the running maximum M rescales the sums accumulated so far.
   float M = -INFINITY, num = 0.f, den = 0.f;
   for (int s0 = 0; s0 < ns; s0 += 4) {
@@ -1262,7 +1218,7 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
 }
 
 // Prompt ingestion in ONE pass (round 1 fed prompts through b200w_infer_step one token per weight
-// sweep): big-M tcgen05 GEMMs over all n_seqs * padded_len tokens, the training flash-attention
+// sweep): big-M wgmma GEMMs over all n_seqs * padded_len tokens, the training flash-attention
 // forward (causal within each sequence), K/V of the real positions written to the cache slots, and the
 // greedy token after each prompt. Padding tokens sit AFTER the real ones, so causality keeps them
 // from influencing any real position.

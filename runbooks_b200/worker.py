@@ -1,4 +1,4 @@
-"""Container entry point of the B200 fine-tune worker — what the trainer Job's container "model"
+"""Container entry point of the H100 fine-tune worker — what the trainer Job's container "model"
 runs (internal/controller/model_controller.go:330-337: image + command from the Model spec).
 
     python -m runbooks_b200.worker train         # ENTRYPOINT of the trainer image

@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (forward + backward) vs the oracle's masked-softmax attention
+"""wgmma flash attention (forward + backward) vs the oracle's masked-softmax attention
 (== F.scaled_dot_product_attention(is_causal=True)) in fp32 on the same bf16-rounded q, k, v.
 
 Tolerance. P is rounded to bf16 before the PV / dV / dK / dQ contractions and the outputs are
@@ -107,8 +107,8 @@ def test_attention_long_sequence_properties(engine):
 @pytest.mark.parametrize("B,S,H,Hkv,iters", [(1, 4096, 32, 32, 500), (2, 2048, 8, 2, 300)])
 def test_attention_is_race_free(engine, B, S, H, Hkv, iters):
     """The kernels have no atomics, so repeated launches on fixed inputs must be BIT-identical.
-    Single-shot parity cannot see an intermittent race: a dQ build whose lane quarters were coupled
-    through one mbarrier shared by two TMEM stages passed every parity test and was wrong (one
+    Single-shot parity cannot see an intermittent race: an earlier dQ build whose warps were coupled
+    through one mbarrier shared by two accumulator stages passed every parity test and was wrong (one
     quarter of one CTA, sometimes NaN) in 1.2 % of launches at this size -- which surfaced only as
     NaN gradients in a 2-GPU run. 500 launches catch a 1 % race with probability 0.993."""
     dh = 128

@@ -210,7 +210,7 @@ def test_real_width_layer_at_full_sequence_length():
     """BASELINE's sizes: one decoder layer of true Llama-2-7B width (d 4096, ffn 11008, 32 heads) on
     a full 4096-token sequence, forward + backward through the engine vs the oracle evaluated in
     fp32 ON THE SAME GPU (the CPU oracle would need minutes). Small vocabulary keeps it light. This
-    exercises the CTA-pair GEMM, the real attention grid (1024 CTAs) and the S = 4096 RoPE table."""
+    exercises the widest-tile GEMM, the real attention grid (1024 CTAs) and the S = 4096 RoPE table."""
     oa = O.Arch(1024, 4096, 11008, 1, 32, 32, 128, 4096, 1e-5, 10000.0)
     params = O.seeded_params(oa, 31)
     rng = np.random.default_rng(5)

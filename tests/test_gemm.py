@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs an fp32 torch reference of the same op (bf16 inputs, fp32 accumulate).
+"""wgmma GEMM vs an fp32 torch reference of the same op (bf16 inputs, fp32 accumulate).
 Tolerances: fp32 output 2e-5 relative Frobenius (accumulation order only); bf16 output 3e-3
 (one round-to-nearest bf16 per element: rms 2^-9/sqrt(3) = 1.1e-3)."""
 import pytest
@@ -21,7 +21,7 @@ def _operands(M, N, K, a_mn, b_mn, seed=0):
     return Ad, Bd, ref
 
 
-@pytest.mark.parametrize("block_n", [128, 256, 512])  # 512 = CTA-pair kernel (cta_group::2)
+@pytest.mark.parametrize("block_n", [128, 256, 512])  # 512 = 256 x 256 tiles on a 2-CTA cluster
 @pytest.mark.parametrize("a_mn,b_mn", [(0, 0), (0, 1), (1, 1), (1, 0)])
 @pytest.mark.parametrize("M,N,K", SHAPES)
 def test_gemm_f32_out(engine, M, N, K, a_mn, b_mn, block_n):
@@ -98,6 +98,18 @@ def test_gemm_narrow_decode_tiles(engine, M, N, K, block_n):
     assert rel_err(D.float(), ref + res.float()) < 3e-3
 
 
+@pytest.mark.parametrize("block_n", [32, 64])
+@pytest.mark.parametrize("a_mn,b_mn", [(1, 0), (0, 1), (1, 1)])
+@pytest.mark.parametrize("M,N,K", [(32, 4544, 1024), (8, 328, 136), (200, 96, 72)])  # MN-major rows: 16-byte aligned
+def test_gemm_narrow_tiles_with_mn_major_operands(engine, M, N, K, a_mn, b_mn, block_n):
+    """Narrow tiles with operands read MN-major (an MN-major B runs 64 wide) against the fp32 reference."""
+    Ad, Bd, ref = _operands(M, N, K, a_mn, b_mn, seed=8)
+    res = torch.randn(M, N, generator=torch.Generator().manual_seed(9)).bfloat16()
+    D = torch.zeros(M, N, device="cuda", dtype=torch.bfloat16)
+    call(engine, "b200w_op_gemm", Ad, a_mn, Ad.shape[1], Bd, b_mn, Bd.shape[1], D, dev(res), 0, N, M, N, K, block_n)
+    assert rel_err(D.float(), ref + res.float()) < 3e-3
+
+
 @pytest.mark.parametrize("split_k", [0, 1])
 @pytest.mark.parametrize("M,N,K", [(32, 4544, 1024), (1, 4672, 4544), (7, 328, 136), (100, 520, 2048), (33, 4544, 18176)])
 def test_gemm_decode_swap_ab(engine, M, N, K, split_k):
@@ -168,8 +180,8 @@ def test_gemm_bias_relu_epilogue(engine, M, N, K, bn, act, resid):
 
 
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn,f32", [
-    (8192, 4352, 4096, 0, 0, 0),    # forward at micro-batch 2: A = 67 MB -> M-fastest in bands of 16 tiles (2 bands)
-    (5120, 4352, 8192, 1, 1, 1),    # accumulating wgrad: B = 71 MB -> N-fastest in bands of 8 + 8 + 1 tiles
+    (8192, 4352, 4096, 0, 0, 0),    # forward at micro-batch 2: A = 67 MB, B = 36 MB -> N-fastest in bands of 6 tiles
+    (5120, 4352, 8192, 1, 1, 1),    # accumulating wgrad: A = 84 MB, B = 71 MB -> M-fastest in bands of 6 tiles
 ])
 def test_gemm_banded_raster_at_shapes_that_exceed_l2(engine, M, N, K, a_mn, b_mn, f32):
     """Operands larger than what stays in L2 switch the tile raster to bands (gemm.cu pick_raster / tile_coords);

@@ -1,7 +1,7 @@
 """The GEMM's tile raster (gemm.cu pick_raster / tile_coords) checked on the host through the C ABI -- no GPU:
 every output tile is visited exactly once for any shape, the band structure is what DESIGN.md 3.1 says at the
-Llama-2-7B micro-batch-2 shapes, and the env switch turns it off. The DRAM-traffic effect is measured on the GPU
-(profiles/r02_gemm_raster_ab.txt); tests/test_gemm.py runs two banded shapes on the device."""
+Llama-2-7B micro-batch-2 shapes, and the env switch turns it off. tests/test_gemm.py runs two banded shapes on
+the device."""
 import ctypes as C
 import os
 import subprocess
@@ -38,22 +38,24 @@ def test_every_tile_is_visited_exactly_once(seed):
 
 
 def test_bands_at_the_llama2_7b_micro_batch_2_shapes():
+    """At the 128 x 256 tiles the step's GEMMs run."""
     T, d, f = 8192, 4096, 11008
-    # gate|up forward: A (67 MB) is swept in 2 bands of 16 row tiles (33.5 MB each); M is the fast dimension
-    n_fast, band, coords = raster(T, 2 * f, d)
-    assert (n_fast, band) == (0, 16)
-    first_band = coords[: 16 * 86]
-    assert first_band[:, 0].max() == 15 and set(first_band[:, 1]) == set(range(86))    # 16 rows x all 86 columns
-    assert (coords[:16, 0] == np.arange(16)).all() and (coords[:16, 1] == 0).all()     # fast dimension first
-    # accumulating wgrad of gate|up: B (67 MB) in 2 bands of 8 column tiles, N fast
-    n_fast, band, _ = raster(2 * f, d, T)
-    assert (n_fast, band) == (1, 8)
-    # micro-batch 1: the re-read operand (33.5 MB) stays in L2 as a whole, no bands (round 2's earlier behaviour)
-    assert raster(4096, 2 * f, d, want_coords=False)[:2] == (0, 0)
-    # long K (gate|up dgrad, K = 22016): one panel is 11 MB, no band can stay; square waves of 8 column tiles
-    assert raster(T, d, 2 * f, want_coords=False)[:2] == (1, 8)
+    # gate|up forward: A (67 MB) is swept in bands of 12 row tiles (12.6 MB each); M is the fast dimension
+    n_fast, band, coords = raster(T, 2 * f, d, tm=128)
+    assert (n_fast, band) == (0, 12)
+    first_band = coords[: 12 * 86]
+    assert first_band[:, 0].max() == 11 and set(first_band[:, 1]) == set(range(86))   # 12 rows x all 86 columns
+    assert (coords[:12, 0] == np.arange(12)).all() and (coords[:12, 1] == 0).all()    # fast dimension first
+    # accumulating wgrad of gate|up (K = 8192): a 256-column B panel (4.2 MB) is too large to band, the 128-row A
+    # panels (2.1 MB) are not -- A (360 MB) is swept in bands of 6 row tiles, M fast
+    n_fast, band, _ = raster(2 * f, d, T, tm=128)
+    assert (n_fast, band) == (0, 6)
+    # micro-batch 1: the re-read operand (33.5 MB) does not stay in a 50 MB L2 as a whole either: bands of 12 row tiles
+    assert raster(4096, 2 * f, d, tm=128, want_coords=False)[:2] == (0, 12)
+    # long K (gate|up dgrad, K = 22016): no panel fits a band; square waves of 8 column tiles
+    assert raster(T, d, 2 * f, tm=128, want_coords=False)[:2] == (1, 8)
     # small problems are untouched
-    assert raster(512, 512, 256, want_coords=False)[1] == 0
+    assert raster(512, 512, 256, tm=128, want_coords=False)[1] == 0
 
 
 def test_env_switch_restores_the_unbanded_raster():

@@ -2,7 +2,7 @@
 SURVEY.md 8 a15) through the CUDA fine-tune engine, against the golden captured from the real HF
 OPTForCausalLM + torch.optim.AdamW (tests/golden/opt_tiny.npz, oracle/make_golden.py run_opt) and the
 fp32 oracle restatement (oracle/opt_oracle.py). head_dim is 64: on the device every head is stored
-zero-padded to 128 so that the dh = 128 tcgen05 attention kernels serve it (DESIGN.md 3.6); load /
+zero-padded to 128 so that the dh = 128 wgmma attention kernels serve it (DESIGN.md 3.6); load /
 read_tensor see the dense HF shapes.
 
 Tolerances as in tests/test_engine.py: loss / grad-norm / updated weights 1e-3 (north_star), logits

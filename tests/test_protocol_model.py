@@ -1,8 +1,9 @@
-"""The warp / mbarrier protocols of the attention kernels under adversarial schedules (CPU model,
-tools/protocol_model.py). The model must FIND the bug round 1 shipped (dQ kernel, one "dS ready"
-barrier for two TMEM stages -- wrong in 1.2 % of launches on hardware while every parity test
-passed) and find nothing in the protocols attention.cu ships now. It is a model of the
-synchronisation structure, not of the CUDA code: change one, change the other.
+"""The warp / mbarrier protocols of the tensor-core kernels under adversarial schedules (CPU model,
+tools/protocol_model.py). The model must FIND the bugs of earlier protocols (the tcgen05 dQ kernel's one
+"dS ready" barrier for two TMEM stages -- wrong in 1.2 % of launches on hardware while every parity test
+passed -- and the sm_90a skip path that freed a slot without waiting for its loads) and find nothing in the
+protocols gemm.cu and attention.cu ship now (`wg_*`: a TMA producer, consumer warps, full / free barrier per
+slot). It is a model of the synchronisation structure, not of the CUDA code: change one, change the other.
 A clean result over random schedules is evidence, not proof."""
 import os
 import sys
@@ -35,9 +36,11 @@ def test_model_finds_the_same_hazard_in_the_v3_to_v8_dq_protocol():
 
 
 def test_shipped_dq_protocol_is_clean():
-    _clean(pm.dq_kernel, njb=8, per_stage_bar_p=True)
-    _clean(pm.dq_kernel, njb=2, per_stage_bar_p=True)      # the shortest loop a CTA can have
-    _clean(pm.dq_kernel, njb=3, per_stage_bar_p=True)
+    """attn_bwd_dq_kernel: 3-slot K/V ring; each warpgroup skips the key blocks past its last row but waits for
+    their loads before freeing them. Without that wait the model finds the slot overwritten or a phase left short."""
+    for njb in (2, 3, 4, 8):                                # the shortest loop a CTA can have, fewer / more than 3 slots
+        _clean(pm.wg_dq_kernel, njb=njb)
+    _broken(pm.wg_dq_kernel, "landed", njb=8, skip_waits_full=False)
 
 
 def test_round1_dkdv_protocol_had_no_stale_reads_but_an_aba_deadlock():
@@ -57,24 +60,29 @@ def test_round1_dkdv_protocol_had_no_stale_reads_but_an_aba_deadlock():
 
 
 def test_shipped_dkdv_protocol_is_clean():
-    """One bar_p per staging buffer: the only dK/dV protocol in attention.cu since round 2."""
-    for n_iter in (2, 3, 4, 9):                              # fewer / more blocks than Q/dO buffers
-        _clean(pm.dkdv_kernel, n_iter=n_iter, per_stage_bar_p=True)
-    ok, first, other = pm.explore(pm.dkdv_kernel, 2000, seed=3, n_iter=2, per_stage_bar_p=True)
+    """attn_bwd_dkdv_kernel: 3-slot Q/dO ring, every warp waits on every block."""
+    for n_iter in (2, 3, 4, 9):                              # fewer / more blocks than Q/dO slots
+        _clean(pm.wg_dkdv_kernel, n_iter=n_iter)
+    ok, first, other = pm.explore(pm.wg_dkdv_kernel, 2000, seed=3, n_iter=4)
     assert (ok, first, other) == (2000, None, {})
 
 
-def test_shipped_forward_protocol_is_clean_and_needs_its_bar_o_wait():
-    for njb in (1, 2, 8):
-        _clean(pm.fwd_kernel, njb=njb)
-    _broken(pm.fwd_kernel, "PV MMA", njb=8, wait_bar_o=False)
+def test_shipped_forward_protocol_is_clean_and_needs_its_free_waits():
+    """attn_fwd_kernel: 2-slot K and V rings; warpgroup 0 skips the last key block (waiting for its loads). The
+    producer's wait on the free barrier before refilling a slot is load-bearing."""
+    for njb in (2, 4, 8):
+        _clean(pm.wg_fwd_kernel, njb=njb)
+    _broken(pm.wg_fwd_kernel, "stale", njb=8, wait_free=False)
+    _broken(pm.wg_fwd_kernel, "landed", njb=8, skip_waits_full=False)
 
 
 def test_pair_gemm_ring_protocol_is_clean():
-    """gemm_bf16_pair_kernel: a full/empty pair per pipeline stage and a tfull/tempty pair per accumulator
-    stage -- per-stage barriers, so no ABA; checked anyway, including fewer k-blocks than stages, one
-    tile, and the 8-arrival accumulator release collected from both CTAs."""
-    for kw in (dict(num_tiles=5, num_kb=7), dict(num_tiles=1, num_kb=1), dict(num_tiles=3, num_kb=2, stages=6),
-               dict(num_tiles=4, num_kb=13, stages=6)):
-        ok, first, other = pm.explore(pm.gemm_pair_kernel, 300, seed=2, **kw)
+    """gemm_bf16_kernel and the 2-CTA cluster gemm_bf16_pair_kernel: the operand ring over every k-block of every
+    tile, each slot freed one k-block late; in the cluster each CTA multicasts its half of a slot into both CTAs and
+    every consumer warp frees the slot in both (16 arrivals). With local releases only, a CTA's producer overwrites
+    the peer's slot while it is being read -- the model must see that."""
+    for kw in (dict(num_items=13), dict(num_items=1), dict(num_items=13, ctas=2), dict(num_items=1, ctas=2),
+               dict(num_items=3, ctas=2, stages=6), dict(num_items=25, ctas=2, stages=4)):
+        ok, first, other = pm.explore(pm.wg_gemm_kernel, 300, seed=2, **kw)
         assert (ok, first, other) == (300, None, {}), (kw, first, other)
+    _broken(pm.wg_gemm_kernel, "landed", num_items=13, ctas=2, remote_release=False)

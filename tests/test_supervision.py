@@ -1,7 +1,7 @@
 """Failure protocol of the N-rank launchers (CPU, no GPU): one rank down must end the job in
 seconds with exit code 1 -- the reference's Job has backoffLimit 0 for GPU workloads
 (internal/controller/model_controller.go:294-303), so a hung trainer is a hung Model.
-Motivated by profiles/r01_n8_failure.txt: a rank that failed but did not exit kept seven GPUs
+Motivated by a multi-GPU run in which a rank that failed but did not exit kept seven GPUs
 spinning in a collective for ten minutes."""
 import multiprocessing as mp
 import os

@@ -13,8 +13,10 @@ that an extra agent retires one at a time, so `tcgen05.commit` arrives only afte
 before it has executed. Buffers carry tags ("what is in here"); every consumer asserts the tag it
 needs. A run ends in OK, a Violation (stale / overwritten data) or a deadlock.
 
-attention.cu's dQ kernel is modelled in its v9 (single bar_p) and v10 (bar_p per stage) forms, the
-dK/dV and forward kernels in their shipped forms plus variants. tests/test_protocol_model.py requires
+The first models below are the protocols of the earlier tcgen05 kernels (an MMA warp, tensor memory, staging
+tiles): the v9 / v10 dQ kernel, the dK/dV and forward kernels and the CTA-pair GEMM. They stay as the record of
+what the model found and as checks of its sensitivity. The sm_90a kernels that ship now (wgmma, a TMA
+producer and consumer warpgroups) share one operand-ring protocol, modelled by `wg_ring_kernel`. tests/test_protocol_model.py requires
 that the model FINDS the v9 bug. It also found something nobody had seen on hardware: the shipped
 dK/dV protocol (one bar_p) is free of stale reads but not of an ABA deadlock -- if the MMA warp is
 held up for a whole compute iteration right after issuing the next block's score MMAs, the compute
@@ -479,6 +481,133 @@ def gemm_pair_kernel(num_tiles, num_kb, rng, stages=3, epi_warps=4):
     return res
 
 
+# ---------------------------------------------------------------------------------------------
+# The sm_90a kernels (gemm.cu, attention.cu): every operand ring is the same protocol. A TMA producer
+# thread fills slot i % depth for item i once the slot's FREE barrier has completed the phase of item
+# i - depth; TMA copies land asynchronously and in any order, each completing its bytes on the slot's
+# FULL barrier; consumer warps wait on FULL, read the slot with wgmma and arrive on FREE once those
+# MMAs have retired. Modelled:
+#   * `lag` = 1: the GEMM consumers free slot i - 1 only after issuing item i (wgmma.wait_group 1);
+#   * `skip(g, i)`: warpgroup g does not read item i (the forward's key block above a warpgroup's diagonal, the dQ
+#     kernel's blocks past a warpgroup's last row) but still waits on its FULL barrier before releasing it. The
+#     model found why (`skip_waits_full=False`): the warps of a warpgroup are scheduled independently, and a warp
+#     that frees a skipped item at once can complete the FREE phase of the item before it in the same slot while
+#     another warp still reads that item -- the producer then overwrites it, or a phase is left short for ever;
+#   * `ctas` = 2: the cluster GEMM -- each CTA's producer multicasts its half of the slot into both
+#     CTAs, and (`remote_release`) every consumer warp arrives on FREE in both CTAs.
+# A copy landing in a slot that a consumer is still reading, or a consumer finding a half that does not
+# belong to its item, is a Violation.
+# ---------------------------------------------------------------------------------------------
+def wg_ring_kernel(n_items, depth, rng, ctas=1, warpgroups=2, warps=2, lag=0, skip=None, wait_free=True,
+                   remote_release=True, skip_waits_full=True):
+    skip = skip or (lambda g, i: False)
+    n_cons = warpgroups * warps
+    full = [[Mbar(ctas) for _ in range(depth)] for _ in range(ctas)]      # one completion per landed half
+    free = [[Mbar(n_cons * (ctas if remote_release else 1)) for _ in range(depth)] for _ in range(ctas)]
+    slot = [[[None] * ctas for _ in range(depth)] for _ in range(ctas)]   # [cta][slot][half] = item
+    reading = [[set() for _ in range(depth)] for _ in range(ctas)]
+    inflight = []                                                          # issued, not yet landed copies
+    state = dict(producers=ctas, read=[[[] for _ in range(n_cons)] for _ in range(ctas)])
+
+    def producer(r):
+        for i in range(n_items):
+            b = i % depth
+            if i >= depth and wait_free:
+                yield (lambda b=b, i=i: free[r][b].passed(((i // depth) - 1) & 1))
+            for dst in range(ctas):                                        # multicast: the same half into every CTA
+                inflight.append((dst, b, r, i))
+            yield None
+        state["producers"] -= 1
+
+    def dma():
+        while True:
+            if inflight:
+                dst, b, half, i = inflight.pop(rng.randrange(len(inflight)))
+                if reading[dst][b]:
+                    raise Violation(f"copy of item {i} landed in CTA {dst} slot {b} while {sorted(reading[dst][b])} read it")
+                slot[dst][b][half] = i
+                full[dst][b].arrive()
+                yield None
+            elif state["producers"] == 0:
+                return
+            else:
+                yield (lambda: bool(inflight) or state["producers"] == 0)
+
+    def release(c, b):
+        free[c][b].arrive()
+        if ctas == 2 and remote_release:
+            free[c ^ 1][b].arrive()
+
+    def consumer(c, g, w):
+        me = (c, g, w)
+        prev = None
+        for i in range(n_items):
+            b = i % depth
+            if skip(g, i):
+                if skip_waits_full:
+                    yield (lambda b=b, i=i: full[c][b].passed((i // depth) & 1))
+                release(c, b)
+                yield None
+                continue
+            yield (lambda b=b, i=i: full[c][b].passed((i // depth) & 1))
+            reading[c][b].add(me)
+            if slot[c][b] != [i] * ctas:
+                raise Violation(f"consumer {me} found {slot[c][b]} in slot {b} while on item {i} (stale)")
+            state["read"][c][g * warps + w].append(i)
+            yield None                                                     # the MMAs read the slot
+            if lag and prev is not None:
+                reading[c][prev].discard(me)
+                release(c, prev)
+            if lag:
+                prev = b
+            else:
+                reading[c][b].discard(me)
+                release(c, b)
+            yield None
+        if prev is not None:
+            reading[c][prev].discard(me)
+            release(c, prev)
+
+    agents = {"dma": dma()}
+    for r in range(ctas):
+        agents[f"tma{r}"] = producer(r)
+        for g in range(warpgroups):
+            for w in range(warps):
+                agents[f"c{r}{g}{w}"] = consumer(r, g, w)
+    res = run(agents, rng)
+    if res == "ok":
+        for c in range(ctas):
+            for g in range(warpgroups):
+                want = [i for i in range(n_items) if not skip(g, i)]
+                for w in range(warps):
+                    if state["read"][c][g * warps + w] != want:
+                        raise Violation(f"consumer {(c, g, w)} read items {state['read'][c][g * warps + w]}")
+    return res
+
+
+def wg_fwd_kernel(njb, rng, **kw):
+    """attn_fwd_kernel's K ring and V ring (2 slots each): warpgroup 0 skips the last key block, which lies above
+    its diagonal"""
+    return wg_ring_kernel(njb, 2, rng, skip=lambda g, j: g == 0 and j == njb - 1, **kw)
+
+
+def wg_dq_kernel(njb, rng, **kw):
+    """attn_bwd_dq_kernel's K/V ring (3 slots): warpgroup g skips the key blocks past njb - 2 + g"""
+    return wg_ring_kernel(njb, 3, rng, skip=lambda g, j: j > njb - 2 + g, **kw)
+
+
+def wg_dkdv_kernel(n_iter, rng, **kw):
+    """attn_bwd_dkdv_kernel's Q/dO ring (3 slots): every warpgroup waits on every block (its 16-query slices
+    before its keys are skipped after the wait)"""
+    return wg_ring_kernel(n_iter, 3, rng, **kw)
+
+
+def wg_gemm_kernel(num_items, rng, stages=4, ctas=1, **kw):
+    """gemm_bf16_kernel (ctas = 1) and gemm_bf16_pair_kernel (ctas = 2): the operand ring over all k-blocks of
+    all tiles of a CTA, each slot freed one k-block late"""
+    return wg_ring_kernel(num_items, stages, rng, ctas=ctas, lag=1, **kw)
+
+
 def explore(kernel, trials, seed=0, **kw):
     """-> (#ok, first violation or None, other outcomes)"""
     ok, first, other = 0, None, {}
@@ -507,6 +636,11 @@ if __name__ == "__main__":
                          ("dK/dV per stage, no block barrier", dkdv_kernel, dict(n_iter=9, per_stage_bar_p=True, block_barrier=False)),
                          ("dK/dV without the block barrier", dkdv_kernel, dict(n_iter=9, block_barrier=False)),
                          ("pair GEMM, 5 tiles x 7 k-blocks", gemm_pair_kernel, dict(num_tiles=5, num_kb=7)),
-                         ("pair GEMM, 1 tile x 1 k-block", gemm_pair_kernel, dict(num_tiles=1, num_kb=1))]:
+                         ("pair GEMM, 1 tile x 1 k-block", gemm_pair_kernel, dict(num_tiles=1, num_kb=1)),
+                         ("sm_90a forward", wg_fwd_kernel, dict(njb=8)),
+                         ("sm_90a dQ", wg_dq_kernel, dict(njb=8)),
+                         ("sm_90a dK/dV", wg_dkdv_kernel, dict(n_iter=9)),
+                         ("sm_90a cluster GEMM", wg_gemm_kernel, dict(num_items=13, ctas=2)),
+                         ("sm_90a cluster GEMM, local release", wg_gemm_kernel, dict(num_items=13, ctas=2, remote_release=False))]:
         ok, first, other = explore(fn, 2000, **kw)
         print(f"{name:36s} ok {ok:4d}/2000   first violation: {first}   other: {other}")
