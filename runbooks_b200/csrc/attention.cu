@@ -2,21 +2,28 @@
 // Oracle: F.scaled_dot_product_attention(q, k, v, is_causal=True) as called by HF
 // LlamaAttention with _attn_implementation == "sdpa" (SURVEY.md §8 a7).
 //
-// Common structure of the three kernels (CTA = 9 warps):
-//   warp 8        TMA producer (lane 0): every load, gated by per-buffer "free" mbarriers;
-//   warps 0..7    two consumer warpgroups; warpgroup wg owns 64 rows of the CTA's 128-row tile and keeps
-//                 its scores and accumulators in registers. A row's scores live in the 4 threads of a
+// Common structure of the three kernels (CTA = 3 warpgroups, 384 threads):
+//   warpgroup 2   TMA producer (one thread issues every load, gated by per-buffer "free" mbarriers). It gives
+//                 its registers back (setmaxnreg.dec to PRODUCER_REGS) so the consumers can hold CONSUMER_REGS.
+//   warpgroups    two consumers; warpgroup wg owns 64 rows of the CTA's 128-row tile and keeps
+//   0, 1          its scores and accumulators in registers. A row's scores live in the 4 threads of a
 //                 lane quad (wgmma accumulator layout, ptx.cuh), so row reductions are two shuffles, and
 //                 the bf16 probabilities feed the second product as the register A operand -- P and dS
 //                 never go through shared memory.
 //   handoffs      full barriers (TMA bytes) and free barriers (one arrival per consumer warp).
+//   pipelining    a warpgroup keeps a product in flight while it does its exp / mask work: block i's score
+//                 product is issued ahead of block i - 1's accumulating product (P V, dV / dK, dQ), and the
+//                 probabilities of block i are computed while that one still runs. The buffer the accumulating
+//                 product reads is therefore freed one block late ("lag 1").
 //
 // forward       CTA = (128-query tile, head, sequence), 64-key blocks:
 //                 S = Q K^T;  P = 2^(S - m) (online softmax);  O = O * alpha + P V
-// backward dKdV CTA = (128-key block, kv head, sequence), 64-query blocks in four 16-query slices,
-//                 transposed form: S^T = K Q^T, dP^T = V dO^T;  dV += P^T dO,  dK += dS^T Q
+// backward dKdV CTA = (128-key block, kv head, sequence), whole 64-query blocks, transposed form:
+//                 S^T = K Q^T, dP^T = V dO^T (m64n64);  dV += P^T dO,  dK += dS^T Q (m64n128, K = 64)
 // backward dQ   CTA = (128-query tile, head, sequence), 64-key blocks: S, dP recomputed,
 //                 dQ += dS K -- no global atomics, no fp32 staging buffer.
+// Every per-element operation and every accumulation order is the same as in a schedule that waits for each
+// product, so the pipelining does not change a bit of the results.
 #include "host_common.h"
 #include "ops.h"
 #include "ptx.cuh"
@@ -29,9 +36,11 @@ using bf16 = __nv_bfloat16;
 constexpr int DH = 128;
 constexpr int ATOM64 = 64 * 128;    // bytes of a [64 rows x 128 B] swizzle-atom column
 constexpr int ATOM128 = 128 * 128;  // bytes of a [128 rows x 128 B] one
-constexpr int NTHREADS = 288;       // 2 consumer warpgroups + TMA warp (8)
-constexpr int TMA_WARP = 8;
+constexpr int NTHREADS = 384;       // 2 consumer warpgroups + the producer warpgroup
+constexpr int PRODUCER_WG = 2;
 constexpr int NCONSUMER_WARPS = 8;
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 240;  // 128 x 24 + 256 x 240 <= 64 K registers
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 65536, "register budget of one CTA per SM");
 
 __device__ __forceinline__ void require_1024_aligned(const void* p) {
   if (smem_u32(p) & 1023u) {
@@ -136,8 +145,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   }
   __syncthreads();
 
-  if (warp == TMA_WARP) {
-    if (lane == 0) {
+  if (warp >> 2 == PRODUCER_WG) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (tid == PRODUCER_WG * 128) {
       mbar_arrive_expect_tx(bar_q, 2 * ATOM128);
 #pragma unroll
       for (int a = 0; a < 2; ++a)
@@ -162,6 +172,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   }
 
   // =============================== consumers ===============================
+  // Block j: S(j) is in flight on entry, issued before PV(j - 1). The softmax of block j runs while PV(j - 1)
+  // is still in flight; O is rescaled once PV(j - 1) retired, then S(j + 1) and PV(j) are issued.
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wi = warp & 3;
   const int row0 = q0 + wg * 64 + wi * 16 + (lane >> 2);  // query positions of this thread's two rows
   const int row1 = row0 + 8;
@@ -171,29 +184,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
 #pragma unroll
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  mbar_wait(bar_q, 0);
-
-  for (int j = 0; j < njb; ++j) {
-    const int buf = j & 1;
-    if (j > last_j) {  // fully masked for every row of this warpgroup: nothing to compute, but the release waits
-      // for the block's loads, so that each warp's arrival counts toward this block's phase and never toward the
-      // phase of the block before it in the same buffer (a warp running ahead would otherwise free that buffer
-      // while another warp of the warpgroup still reads it)
-      mbar_wait(&bar_k[buf], (j >> 1) & 1);
-      warp_release(&bar_kfree[buf]);
-      mbar_wait(&bar_v[buf], (j >> 1) & 1);
-      warp_release(&bar_vfree[buf]);
-      continue;
-    }
-    float s[32];
-    mbar_wait(&bar_k[buf], (j >> 1) & 1);
-    wg_fence();
-    mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
-    wg_commit();
-    wg_wait<0>();
-    wg_fence_regs(s);
-    warp_release(&bar_kfree[buf]);
-
+  float s[32];
+  uint32_t pa[4][4];
+  float alpha0, alpha1;
+  // online softmax of block j's scores in s: masks them, updates m and l, leaves P in s and O's rescale in alpha
+  auto softmax = [&](int j) {
     const int col0 = j * FWD_BKV + 2 * (lane & 3);
     if (j * FWD_BKV + FWD_BKV - 1 > q0 + wg * 64) {  // the block reaches past the first row's diagonal
 #pragma unroll
@@ -213,7 +208,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
     }
     // scale > 0, so max commutes with it; block 0 holds key 0, visible to every row, so m is finite from then on
     const float mn0 = fmaxf(m0, quad_max(mx0) * scale_log2), mn1 = fmaxf(m1, quad_max(mx1) * scale_log2);
-    const float alpha0 = ex2(m0 - mn0), alpha1 = ex2(m1 - mn1);
+    alpha0 = ex2(m0 - mn0);
+    alpha1 = ex2(m1 - mn1);
     m0 = mn0;
     m1 = mn1;
     float ps0 = 0.f, ps1 = 0.f;
@@ -228,7 +224,36 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
     }
     l0 = l0 * alpha0 + ps0;  // this thread's part of the row sums (the quad's alphas are equal)
     l1 = l1 * alpha1 + ps1;
-    uint32_t pa[4][4];
+  };
+
+  mbar_wait(bar_q, 0);
+  mbar_wait(&bar_k[0], 0);  // block 0 holds key 0, which every row sees: no warpgroup skips it
+  wg_fence();
+  mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK), ATOM64);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_regs(s);
+  warp_release(&bar_kfree[0]);
+  softmax(0);  // O is still 0: its rescale is a no-op
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, pa[kk]);
+
+  for (int j = 1; j <= last_j; ++j) {
+    const int buf = j & 1;
+    mbar_wait(&bar_k[buf], (j >> 1) & 1);
+    wg_fence();
+    mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
+    wg_commit();
+    mbar_wait(&bar_v[buf ^ 1], ((j - 1) >> 1) & 1);
+    mma_pv<4>(o, pa, smem_u32(sV + (buf ^ 1) * 2 * ATOM64));
+    wg_commit();
+    wg_wait<1>();  // S(j) retired; PV(j - 1) may still run
+    wg_fence_regs(s);
+    warp_release(&bar_kfree[buf]);
+    softmax(j);
+    wg_wait<0>();  // PV(j - 1) retired: O may be rescaled, pa rewritten and V(j - 1) freed
+    wg_fence_regs(o);
+    warp_release(&bar_vfree[buf ^ 1]);
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, pa[kk]);
 #pragma unroll
@@ -238,13 +263,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
       o[4 * jj + 2] *= alpha1;
       o[4 * jj + 3] *= alpha1;
     }
-    mbar_wait(&bar_v[buf], (j >> 1) & 1);
-    wg_fence();
-    mma_pv<4>(o, pa, smem_u32(sV + buf * 2 * ATOM64));
-    wg_commit();
-    wg_wait<0>();
-    wg_fence_regs(o);
-    warp_release(&bar_vfree[buf]);
+  }
+  mbar_wait(&bar_v[last_j & 1], (last_j >> 1) & 1);
+  wg_fence();
+  mma_pv<4>(o, pa, smem_u32(sV + (last_j & 1) * 2 * ATOM64));
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_regs(o);
+  warp_release(&bar_vfree[last_j & 1]);
+  // Blocks past last_j are fully masked for every row of this warpgroup: nothing to compute, but the release
+  // waits for the block's loads, so that each warp's arrival counts toward this block's phase and never toward
+  // the phase of the block before it in the same buffer (a warp running ahead would otherwise free that buffer
+  // while another warp of the warpgroup still reads it).
+  for (int j = last_j + 1; j < njb; ++j) {
+    mbar_wait(&bar_k[j & 1], (j >> 1) & 1);
+    warp_release(&bar_kfree[j & 1]);
+    mbar_wait(&bar_v[j & 1], (j >> 1) & 1);
+    warp_release(&bar_vfree[j & 1]);
   }
 
   l0 = quad_sum(l0);
@@ -262,12 +297,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
 // ==========================================================================================
 // backward, part 1: dK, dV
 // ==========================================================================================
-constexpr int BWD_BKV = 128, BWD_BQ = 64, BWD_QH = 16;
-constexpr int KV_SMEM = 2 * ATOM128 /*K*/ + 2 * ATOM128 /*V*/ + 3 * 2 * ATOM64 /*Q x3*/ + 3 * 2 * ATOM64 /*dO x3*/ + 256;
+constexpr int BWD_BKV = 128, BWD_BQ = 64, KV_STAGES = 4;
+constexpr int KV_STAT = 2 * BWD_BQ * 4;  // bytes of a block's lse and delta rows (fp32)
+constexpr int KV_SMEM = 2 * ATOM128 /*K*/ + 2 * ATOM128 /*V*/ + KV_STAGES * 2 * ATOM64 /*Q*/ +
+                        KV_STAGES * 2 * ATOM64 /*dO*/ + KV_STAGES * KV_STAT /*lse, delta*/ + 256;
 
-// dV and dK stay in registers for the whole loop (128 per thread). A 9-warp block puts 3 warps on one of the SM's
-// four 16 K-register sub-partitions, so a thread may hold 168 registers: the query block is taken 16 queries at a
-// time (m64n16 score tiles) to keep the scores, their bf16 fragments and both accumulators inside that.
+// dV and dK stay in registers for the whole loop (128 per thread). A 64-query block is taken whole: S^T and dP^T
+// (32 fp32 registers each) become P^T and dS^T as bf16 A fragments (16 each) before block i + 1's scores are issued
+// into the same registers, so the peak is dV + dK + one block's scores + one block's fragments.
+// Block i's dV / dK products stay in flight while block i + 1's scores run, so Q/dO buffer i is freed one block
+// late; the fourth buffer keeps two blocks of loads ahead of the products.
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta,
@@ -277,11 +316,12 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   require_1024_aligned(smem);
   uint8_t* sK = smem;                       // 2 atoms (dh halves) x [128 kv x 128 B]
   uint8_t* sV = sK + 2 * ATOM128;
-  uint8_t* sQ = sV + 2 * ATOM128;           // 3 bufs x 2 atoms x [64 q x 128 B]
-  uint8_t* sdO = sQ + 3 * 2 * ATOM64;
-  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sdO + 3 * 2 * ATOM64);
-  uint64_t* bar_q = bar_kv + 1;      // [3] Q, dO block in smem
-  uint64_t* bar_qfree = bar_q + 3;   // [3] MMAs that read Q/dO buffer b retired
+  uint8_t* sQ = sV + 2 * ATOM128;           // KV_STAGES bufs x 2 atoms x [64 q x 128 B]
+  uint8_t* sdO = sQ + KV_STAGES * 2 * ATOM64;
+  float* sStat = reinterpret_cast<float*>(sdO + KV_STAGES * 2 * ATOM64);  // KV_STAGES x {lse[64], delta[64]}
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sStat + KV_STAGES * 2 * BWD_BQ);
+  uint64_t* bar_q = bar_kv + 1;               // [KV_STAGES] Q, dO block and its lse, delta in smem
+  uint64_t* bar_qfree = bar_q + KV_STAGES;    // [KV_STAGES] MMAs that read Q/dO buffer b retired
 
   const int G = H / Hkv;
   const int jb = blockIdx.x / (B * Hkv);  // earliest key blocks (longest query loops) first
@@ -298,7 +338,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_do);
     mbar_init(bar_kv, 1);
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < KV_STAGES; ++i) {
       mbar_init(&bar_q[i], 1);
       mbar_init(&bar_qfree[i], NCONSUMER_WARPS);
     }
@@ -313,8 +353,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   };
   const int qb_base = 2 * jb;
 
-  if (warp == TMA_WARP) {
-    if (lane == 0) {
+  if (warp >> 2 == PRODUCER_WG) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (tid == PRODUCER_WG * 128) {
       mbar_arrive_expect_tx(bar_kv, 4 * ATOM128);
 #pragma unroll
       for (int a = 0; a < 2; ++a)
@@ -326,91 +367,128 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
       IterPos ip{hk * G, 0};
       int buf = 0;
       uint32_t par = 0;
-      for (int it = 0; it < n_iter; ++it) {  // block it reuses block it-3's buffer
-        if (it >= 3) mbar_wait(&bar_qfree[buf], par ^ 1);
-        mbar_arrive_expect_tx(&bar_q[buf], 4 * ATOM64);
-        const int row = tok0 + (qb_base + ip.qb) * BWD_BQ;
+      // block it reuses block it-KV_STAGES's buffer; the last KV_STAGES passes load nothing and only wait for the
+      // release of the last blocks (the consumers' waits are unbounded, this one is not)
+      for (int it = 0; it < n_iter + KV_STAGES; ++it) {
+        if (it >= KV_STAGES) mbar_wait(&bar_qfree[buf], par ^ 1);
+        if (it < n_iter) {
+          mbar_arrive_expect_tx(&bar_q[buf], 4 * ATOM64 + KV_STAT);
+          const int row = tok0 + (qb_base + ip.qb) * BWD_BQ;
 #pragma unroll
-        for (int a = 0; a < 2; ++a) {
-          tma_load_2d(sQ + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_q[buf], ip.h * DH + a * 64, row);
-          tma_load_2d(sdO + (buf * 2 + a) * ATOM64, &tm_do, &bar_q[buf], ip.h * DH + a * 64, row);
+          for (int a = 0; a < 2; ++a) {
+            tma_load_2d(sQ + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_q[buf], ip.h * DH + a * 64, row);
+            tma_load_2d(sdO + (buf * 2 + a) * ATOM64, &tm_do, &bar_q[buf], ip.h * DH + a * 64, row);
+          }
+          const size_t stat = static_cast<size_t>(ip.h) * Ttot + row;
+          bulk_load_1d(sStat + buf * 2 * BWD_BQ, lse2 + stat, BWD_BQ * 4, &bar_q[buf]);
+          bulk_load_1d(sStat + buf * 2 * BWD_BQ + BWD_BQ, delta + stat, BWD_BQ * 4, &bar_q[buf]);
+          ip.next(nqb);
         }
-        ip.next(nqb);
-        if (++buf == 3) { buf = 0; par ^= 1; }
+        if (++buf == KV_STAGES) { buf = 0; par ^= 1; }
       }
     }
     return;
   }
 
   // =============================== consumers: warpgroup wg owns keys [kv0 + 64 wg, kv0 + 64 wg + 64) =========
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wi = warp & 3;
-  const int kv_a = kv0 + wg * 64 + wi * 16 + (lane >> 2);  // key positions of this thread's two rows
+  const int kv_first = kv0 + wg * 64;
+  const int kv_a = kv_first + wi * 16 + (lane >> 2);  // key positions of this thread's two rows
   const int kv_b = kv_a + 8;
   const uint32_t k_addr = smem_u32(sK) + wg * ATOM64, v_addr = smem_u32(sV) + wg * ATOM64;
   float dv[64], dk[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
-  mbar_wait(bar_kv, 0);
+  float st[32], dpt[32];
+  uint32_t pa[4][4], dsa[4][4];
+  auto issue_st = [&](int bf) {
+    wg_fence();
+    mma_over_dh<BWD_BQ>(st, k_addr, ATOM128, smem_u32(sQ + bf * 2 * ATOM64), ATOM64);
+    wg_commit();
+  };
+  auto issue_dvdk = [&](int bf) {
+    wg_fence();
+    mma_pv<BWD_BQ / 16>(dv, pa, smem_u32(sdO + bf * 2 * ATOM64));
+    mma_pv<BWD_BQ / 16>(dk, dsa, smem_u32(sQ + bf * 2 * ATOM64));
+    wg_commit();
+  };
+  // P^T of the block in buffer bf, in place of S^T. A block whose queries all precede this warpgroup's keys comes
+  // out as P = 0 and adds exact zeros to dV and dK.
+  auto probs = [&](int bf, int q_seq0) {
+    const float* lse_s = sStat + bf * 2 * BWD_BQ;
+    const bool diag = q_seq0 < kv_first + 64;  // some (q, kv) pairs of this block are masked
+#pragma unroll
+    for (int jj = 0; jj < BWD_BQ / 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int q = 8 * jj + 2 * (lane & 3) + e;
+        const float lse = lse_s[q];
+        float pa_ = ex2(fmaf(st[4 * jj + e], scale_log2, -lse));
+        float pb_ = ex2(fmaf(st[4 * jj + 2 + e], scale_log2, -lse));
+        if (diag) {
+          if (q_seq0 + q < kv_a) pa_ = 0.f;
+          if (q_seq0 + q < kv_b) pb_ = 0.f;
+        }
+        st[4 * jj + e] = pa_;
+        st[4 * jj + 2 + e] = pb_;
+      }
+  };
+  // dP^T of the block in buffer bf, then dS^T and both bf16 A fragments
+  auto grads = [&](int bf) {
+    wg_fence();
+    mma_over_dh<BWD_BQ>(dpt, v_addr, ATOM128, smem_u32(sdO + bf * 2 * ATOM64), ATOM64);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(dpt);
+    const float* dl_s = sStat + bf * 2 * BWD_BQ + BWD_BQ;  // delta, pre-multiplied by the scale
+#pragma unroll
+    for (int jj = 0; jj < BWD_BQ / 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        // dS = P (dP - delta) * scale, with delta*scale precomputed
+        const float dl = dl_s[8 * jj + 2 * (lane & 3) + e];
+        dpt[4 * jj + e] = st[4 * jj + e] * fmaf(dpt[4 * jj + e], scale, -dl);
+        dpt[4 * jj + 2 + e] = st[4 * jj + 2 + e] * fmaf(dpt[4 * jj + 2 + e], scale, -dl);
+      }
+#pragma unroll
+    for (int kk = 0; kk < BWD_BQ / 16; ++kk) {
+      to_afrag(st, kk, pa[kk]);
+      to_afrag(dpt, kk, dsa[kk]);
+    }
+  };
 
+  // Block i (i > 0): S^T(i) is issued ahead of dV/dK(i - 1), P^T(i) computed while dV/dK(i - 1) runs; once that
+  // retired, block i - 1's buffer is freed and dP^T(i) issued.
   IterPos cur{hk * G, 0};
   int buf = 0;
   uint32_t par = 0;
-  for (int it = 0; it < n_iter; ++it) {
-    const int q_seq0 = (qb_base + cur.qb) * BWD_BQ;
-    const float* lse_h = lse2 + static_cast<size_t>(cur.h) * Ttot + tok0;
-    const float* dl_h = delta + static_cast<size_t>(cur.h) * Ttot + tok0;   // pre-multiplied by the scale
-    mbar_wait(&bar_q[buf], par);
-#pragma unroll 1
-    for (int hq = 0; hq < BWD_BQ / BWD_QH; ++hq) {
-      const int qh0 = q_seq0 + hq * BWD_QH;
-      if (qh0 + BWD_QH - 1 < kv0 + wg * 64) continue;  // every query of the slice precedes every key: P = 0
-      const uint32_t qrow = smem_u32(sQ + buf * 2 * ATOM64) + hq * BWD_QH * 128;
-      const uint32_t dorow = smem_u32(sdO + buf * 2 * ATOM64) + hq * BWD_QH * 128;
-      float st[BWD_QH / 2], dpt[BWD_QH / 2];
-      wg_fence();
-      mma_over_dh<BWD_QH>(st, k_addr, ATOM128, qrow, ATOM64);
-      mma_over_dh<BWD_QH>(dpt, v_addr, ATOM128, dorow, ATOM64);
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(st);
-      wg_fence_regs(dpt);
-      const bool diag = qh0 < kv0 + wg * 64 + 64;  // some (q, kv) pairs of this slice are masked
-#pragma unroll
-      for (int jj = 0; jj < BWD_QH / 8; ++jj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int q = qh0 + 8 * jj + 2 * (lane & 3) + e;
-          const float lse = lse_h[q], dl = dl_h[q];
-          float pa_ = ex2(fmaf(st[4 * jj + e], scale_log2, -lse));
-          float pb_ = ex2(fmaf(st[4 * jj + 2 + e], scale_log2, -lse));
-          if (diag) {
-            if (q < kv_a) pa_ = 0.f;
-            if (q < kv_b) pb_ = 0.f;
-          }
-          st[4 * jj + e] = pa_;
-          st[4 * jj + 2 + e] = pb_;
-          // dS = P (dP - delta) * scale, with delta*scale precomputed
-          dpt[4 * jj + e] = pa_ * fmaf(dpt[4 * jj + e], scale, -dl);
-          dpt[4 * jj + 2 + e] = pb_ * fmaf(dpt[4 * jj + 2 + e], scale, -dl);
-        }
-      uint32_t pa[BWD_QH / 16][4], dsa[BWD_QH / 16][4];
-#pragma unroll
-      for (int kk = 0; kk < BWD_QH / 16; ++kk) {
-        to_afrag(st, kk, pa[kk]);
-        to_afrag(dpt, kk, dsa[kk]);
-      }
-      wg_fence();
-      mma_pv<BWD_QH / 16>(dv, pa, dorow);
-      mma_pv<BWD_QH / 16>(dk, dsa, qrow);
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(dv);
-      wg_fence_regs(dk);
-    }
-    warp_release(&bar_qfree[buf]);
+  mbar_wait_unbounded(bar_kv, 0);
+  mbar_wait_unbounded(&bar_q[0], 0);
+  issue_st(0);
+  wg_wait<0>();
+  wg_fence_regs(st);
+  probs(0, qb_base * BWD_BQ);
+  grads(0);
+  for (int it = 1; it < n_iter; ++it) {
+    const int prev = buf;
     cur.next(nqb);
-    if (++buf == 3) { buf = 0; par ^= 1; }
+    if (++buf == KV_STAGES) { buf = 0; par ^= 1; }
+    mbar_wait_unbounded(&bar_q[buf], par);
+    issue_st(buf);
+    issue_dvdk(prev);
+    wg_wait<1>();  // S^T(i) retired; dV/dK(i - 1) may still run
+    wg_fence_regs(st);
+    probs(buf, (qb_base + cur.qb) * BWD_BQ);
+    wg_wait<0>();  // dV/dK(i - 1) retired: its Q/dO buffer is free and pa / dsa may be rewritten
+    warp_release(&bar_qfree[prev]);
+    grads(buf);
   }
+  issue_dvdk(buf);
+  wg_wait<0>();
+  wg_fence_regs(dv);
+  wg_fence_regs(dk);
+  warp_release(&bar_qfree[buf]);
 
   bf16* base_a = dqkv + static_cast<size_t>(tok0 + kv_a) * ld_qkv + hk * DH;
   bf16* base_b = dqkv + static_cast<size_t>(tok0 + kv_b) * ld_qkv + hk * DH;
@@ -421,9 +499,12 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
 // ==========================================================================================
 // backward, part 2: dQ
 // ==========================================================================================
-constexpr int DQ_BQ = 128, DQ_BKV = 64;
-constexpr int DQ_SMEM = 2 * ATOM128 /*Q*/ + 2 * ATOM128 /*dO*/ + 3 * 2 * ATOM64 /*K x3*/ + 3 * 2 * ATOM64 /*V x3*/ + 256;
+constexpr int DQ_BQ = 128, DQ_BKV = 64, DQ_STAGES = 4;
+constexpr int DQ_SMEM = 2 * ATOM128 /*Q*/ + 2 * ATOM128 /*dO*/ + DQ_STAGES * 2 * ATOM64 /*K*/ +
+                        DQ_STAGES * 2 * ATOM64 /*V*/ + 256;
 
+// Block j's dQ product stays in flight while block j + 1's S and dP run, so K/V buffer j is freed one block late;
+// the fourth buffer keeps two blocks of loads ahead of the products.
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                    const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
@@ -432,11 +513,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   require_1024_aligned(smem);
   uint8_t* sQ = smem;                      // 2 atoms (dh halves) x [128 q x 128 B]
   uint8_t* sdO = sQ + 2 * ATOM128;
-  uint8_t* sK = sdO + 2 * ATOM128;         // 3 bufs x 2 atoms x [64 kv x 128 B]
-  uint8_t* sV = sK + 3 * 2 * ATOM64;
-  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + 3 * 2 * ATOM64);  // Q, dO tile in smem
-  uint64_t* bar_kv = bar_q + 1;        // [3]
-  uint64_t* bar_kvfree = bar_kv + 3;   // [3] MMAs that read K/V buffer b retired
+  uint8_t* sK = sdO + 2 * ATOM128;         // DQ_STAGES bufs x 2 atoms x [64 kv x 128 B]
+  uint8_t* sV = sK + DQ_STAGES * 2 * ATOM64;
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + DQ_STAGES * 2 * ATOM64);  // Q, dO tile in smem
+  uint64_t* bar_kv = bar_q + 1;                // [DQ_STAGES]
+  uint64_t* bar_kvfree = bar_kv + DQ_STAGES;   // [DQ_STAGES] MMAs that read K/V buffer b retired
 
   const int nq = S / DQ_BQ;
   const int bh = blockIdx.x % (B * H);
@@ -452,7 +533,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_do);
     mbar_init(bar_q, 1);
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < DQ_STAGES; ++i) {
       mbar_init(&bar_kv[i], 1);
       mbar_init(&bar_kvfree[i], NCONSUMER_WARPS);
     }
@@ -460,8 +541,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   }
   __syncthreads();
 
-  if (warp == TMA_WARP) {
-    if (lane == 0) {
+  if (warp >> 2 == PRODUCER_WG) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (tid == PRODUCER_WG * 128) {
       mbar_arrive_expect_tx(bar_q, 4 * ATOM128);
 #pragma unroll
       for (int a = 0; a < 2; ++a)
@@ -472,21 +554,26 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
         }
       int buf = 0;
       uint32_t par = 0;
-      for (int j = 0; j < njb; ++j) {  // block j reuses block j-3's buffer
-        if (j >= 3) mbar_wait(&bar_kvfree[buf], par ^ 1);
-        mbar_arrive_expect_tx(&bar_kv[buf], 4 * ATOM64);
+      // block j reuses block j-DQ_STAGES's buffer; the last DQ_STAGES passes load nothing and only wait for the
+      // release of the last blocks (the consumers' waits are unbounded, this one is not)
+      for (int j = 0; j < njb + DQ_STAGES; ++j) {
+        if (j >= DQ_STAGES) mbar_wait(&bar_kvfree[buf], par ^ 1);
+        if (j < njb) {
+          mbar_arrive_expect_tx(&bar_kv[buf], 4 * ATOM64);
 #pragma unroll
-        for (int a = 0; a < 2; ++a) {
-          tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], k_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
-          tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], v_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
+          for (int a = 0; a < 2; ++a) {
+            tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], k_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
+            tma_load_2d(sV + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_kv[buf], v_off + hk * DH + a * 64, tok0 + j * DQ_BKV);
+          }
         }
-        if (++buf == 3) { buf = 0; par ^= 1; }
+        if (++buf == DQ_STAGES) { buf = 0; par ^= 1; }
       }
     }
     return;
   }
 
   // =============================== consumers: warpgroup wg owns query rows [q0 + 64 wg, q0 + 64 wg + 64) =======
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wi = warp & 3;
   const int row0 = q0 + wg * 64 + wi * 16 + (lane >> 2);
   const int row1 = row0 + 8;
@@ -498,50 +585,85 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   float dq[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) dq[i] = 0.f;
-  mbar_wait(bar_q, 0);
+  float s[32], dp[32];
+  uint32_t dsa[4][4];
+  auto issue_s = [&](int bf) {
+    wg_fence();
+    mma_over_dh<DQ_BKV>(s, q_addr, ATOM128, smem_u32(sK + bf * 2 * ATOM64), ATOM64);
+    wg_commit();
+  };
+  auto issue_dq = [&](int bf) {  // dQ += dS K, K read MN-major (N = dh)
+    wg_fence();
+    mma_pv<4>(dq, dsa, smem_u32(sK + bf * 2 * ATOM64));
+    wg_commit();
+  };
+  auto probs = [&](int j) {  // P of block j, in place of S
+    const bool diag = j * DQ_BKV + DQ_BKV - 1 > q0 + wg * 64;
+    const int col0 = j * DQ_BKV + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = col0 + 8 * jj + e;
+        float p0 = ex2(fmaf(s[4 * jj + e], scale_log2, -lse0));
+        float p1 = ex2(fmaf(s[4 * jj + 2 + e], scale_log2, -lse1));
+        if (diag) {
+          if (col > row0) p0 = 0.f;
+          if (col > row1) p1 = 0.f;
+        }
+        s[4 * jj + e] = p0;
+        s[4 * jj + 2 + e] = p1;
+      }
+  };
+  auto grads = [&](int bf) {  // dP of the block in buffer bf, then dS and its bf16 A fragments
+    wg_fence();
+    mma_over_dh<DQ_BKV>(dp, do_addr, ATOM128, smem_u32(sV + bf * 2 * ATOM64), ATOM64);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(dp);
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {  // dS
+      s[i] *= fmaf(dp[i], scale, -dl0);
+      s[i + 1] *= fmaf(dp[i + 1], scale, -dl0);
+      s[i + 2] *= fmaf(dp[i + 2], scale, -dl1);
+      s[i + 3] *= fmaf(dp[i + 3], scale, -dl1);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, dsa[kk]);
+  };
 
+  // Block j (j > 0): S(j) is issued ahead of dQ(j - 1), P(j) computed while dQ(j - 1) runs; once that retired,
+  // block j - 1's buffer is freed and dP(j) issued.
   int buf = 0;
   uint32_t par = 0;
-  for (int j = 0; j < njb; ++j) {
-    if (j <= last_j) {
-      float s[32], dp[32];
-      mbar_wait(&bar_kv[buf], par);
-      wg_fence();
-      mma_over_dh<DQ_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
-      mma_over_dh<DQ_BKV>(dp, do_addr, ATOM128, smem_u32(sV + buf * 2 * ATOM64), ATOM64);
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(s);
-      wg_fence_regs(dp);
-      const bool diag = j * DQ_BKV + DQ_BKV - 1 > q0 + wg * 64;
-      const int col0 = j * DQ_BKV + 2 * (lane & 3);
-#pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = col0 + 8 * jj + e;
-          float p0 = ex2(fmaf(s[4 * jj + e], scale_log2, -lse0));
-          float p1 = ex2(fmaf(s[4 * jj + 2 + e], scale_log2, -lse1));
-          if (diag) {
-            if (col > row0) p0 = 0.f;
-            if (col > row1) p1 = 0.f;
-          }
-          s[4 * jj + e] = p0 * fmaf(dp[4 * jj + e], scale, -dl0);     // dS
-          s[4 * jj + 2 + e] = p1 * fmaf(dp[4 * jj + 2 + e], scale, -dl1);
-        }
-      uint32_t dsa[4][4];
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, dsa[kk]);
-      wg_fence();
-      mma_pv<4>(dq, dsa, smem_u32(sK + buf * 2 * ATOM64));  // dQ += dS K, K read MN-major (N = dh)
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(dq);
-    } else {
-      mbar_wait(&bar_kv[buf], par);  // a skipped block is released after its loads landed (see the forward)
-    }
+  mbar_wait_unbounded(bar_q, 0);
+  mbar_wait_unbounded(&bar_kv[0], 0);  // block 0 holds key 0, which every row sees: no warpgroup skips it
+  issue_s(0);
+  wg_wait<0>();
+  wg_fence_regs(s);
+  probs(0);
+  grads(0);
+  for (int j = 1; j <= last_j; ++j) {
+    const int prev = buf;
+    if (++buf == DQ_STAGES) { buf = 0; par ^= 1; }
+    mbar_wait_unbounded(&bar_kv[buf], par);
+    issue_s(buf);
+    issue_dq(prev);
+    wg_wait<1>();  // S(j) retired; dQ(j - 1) may still run
+    wg_fence_regs(s);
+    probs(j);
+    wg_wait<0>();  // dQ(j - 1) retired: its K/V buffer is free and dsa may be rewritten
+    warp_release(&bar_kvfree[prev]);
+    grads(buf);
+  }
+  issue_dq(buf);
+  wg_wait<0>();
+  wg_fence_regs(dq);
+  warp_release(&bar_kvfree[buf]);
+  for (int j = last_j + 1; j < njb; ++j) {  // a skipped block is released after its loads landed (see the forward)
+    if (++buf == DQ_STAGES) { buf = 0; par ^= 1; }
+    mbar_wait_unbounded(&bar_kv[buf], par);
     warp_release(&bar_kvfree[buf]);
-    if (++buf == 3) { buf = 0; par ^= 1; }
   }
 
   store_rows_bf16(dq, dqkv + static_cast<size_t>(tok0 + row0) * ld_qkv + h * DH,

@@ -77,6 +77,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait_hint(bar, parity, 1000u))
     if (++polls > B200W_WAIT_LIMIT_POLLS) __trap();
 }
+// A wait without the bound, for consumer code that runs after setmaxnreg.inc: a trap reachable there makes ptxas
+// spill as if the thread held only the launch's register share. Only where a bounded wait covers the same failure:
+// the block's producer waits (bounded) for the release of every buffer, the last ones included, so a consumer stuck
+// here leaves the producer to trap.
+__device__ __forceinline__ void mbar_wait_unbounded(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait_hint(bar, parity, 1000u)) {
+  }
+}
 
 // generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
@@ -130,6 +138,20 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_sr
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(gmem_src)), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
+}
+
+// ------------------------------------------------------------------------------------------
+// register reallocation between warpgroups: every warp of a warpgroup executes the same one. A producer warpgroup
+// gives registers back (dec) so that the consumer warpgroups can take them (inc); the block's total must stay
+// within the 64 K registers of an SM, so a 384-thread block can run 1 x 24 + 2 x 240 per thread.
+// ------------------------------------------------------------------------------------------
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ------------------------------------------------------------------------------------------

@@ -499,7 +499,7 @@ def gemm_pair_kernel(num_tiles, num_kb, rng, stages=3, epi_warps=4):
 # belong to its item, is a Violation.
 # ---------------------------------------------------------------------------------------------
 def wg_ring_kernel(n_items, depth, rng, ctas=1, warpgroups=2, warps=2, lag=0, skip=None, wait_free=True,
-                   remote_release=True, skip_waits_full=True):
+                   remote_release=True, skip_waits_full=True, release_early=False):
     skip = skip or (lambda g, i: False)
     n_cons = warpgroups * warps
     full = [[Mbar(ctas) for _ in range(depth)] for _ in range(ctas)]      # one completion per landed half
@@ -555,9 +555,12 @@ def wg_ring_kernel(n_items, depth, rng, ctas=1, warpgroups=2, warps=2, lag=0, sk
                 raise Violation(f"consumer {me} found {slot[c][b]} in slot {b} while on item {i} (stale)")
             state["read"][c][g * warps + w].append(i)
             yield None                                                     # the MMAs read the slot
+            if release_early:                                              # freed at issue, not once they retired
+                release(c, b)
             if lag and prev is not None:
                 reading[c][prev].discard(me)
-                release(c, prev)
+                if not release_early:
+                    release(c, prev)
             if lag:
                 prev = b
             else:
@@ -566,7 +569,8 @@ def wg_ring_kernel(n_items, depth, rng, ctas=1, warpgroups=2, warps=2, lag=0, sk
             yield None
         if prev is not None:
             reading[c][prev].discard(me)
-            release(c, prev)
+            if not release_early:
+                release(c, prev)
 
     agents = {"dma": dma()}
     for r in range(ctas):
@@ -600,6 +604,25 @@ def wg_dkdv_kernel(n_iter, rng, **kw):
     """attn_bwd_dkdv_kernel's Q/dO ring (3 slots): every warpgroup waits on every block (its 16-query slices
     before its keys are skipped after the wait)"""
     return wg_ring_kernel(n_iter, 3, rng, **kw)
+
+
+# The pipelined attention rings: a warpgroup leaves block i's accumulating product (P V, dV / dK, dQ) in flight while
+# block i + 1's scores run, and frees the buffer that product reads one block late (lag 1). `release_early` frees it
+# at issue instead, the hazard the lag exists for.
+def wg_fwd_v_kernel(njb, rng, **kw):
+    """attn_fwd_kernel's V ring (2 slots, lag 1; its K ring is wg_fwd_kernel's): warpgroup 0 skips the last key
+    block after waiting for its loads"""
+    return wg_ring_kernel(njb, 2, rng, lag=1, skip=lambda g, j: g == 0 and j == njb - 1, **kw)
+
+
+def wg_dq_lag_kernel(njb, rng, **kw):
+    """attn_bwd_dq_kernel's K/V ring (4 slots, lag 1): warpgroup g skips the key blocks past njb - 2 + g"""
+    return wg_ring_kernel(njb, 4, rng, lag=1, skip=lambda g, j: j > njb - 2 + g, **kw)
+
+
+def wg_dkdv_lag_kernel(n_iter, rng, **kw):
+    """attn_bwd_dkdv_kernel's Q/dO ring (4 slots, lag 1): every warpgroup computes every block"""
+    return wg_ring_kernel(n_iter, 4, rng, lag=1, **kw)
 
 
 def wg_gemm_kernel(num_items, rng, stages=4, ctas=1, **kw):
