@@ -170,6 +170,18 @@ B200W_API int b200w_forward_backward(b200w_ctx* ctx, const int32_t* ids, const i
  * (HOST float [n_seqs * max_seq_len], 0 where ignored) or NULL. n_seqs <= micro_batch. */
 B200W_API int b200w_forward(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, int n_seqs,
                   float* logits_out, float* nll_out, float* loss_out);
+/* Padding-free packing (HF DataCollatorWithFlattening, TRL padding_free): the three calls above with
+ * positions, HOST int32 [n_seqs, max_seq_len] with HF position_ids semantics -- every row starts at 0, each
+ * later entry is 0 (a new document starts there) or the previous entry + 1. RoPE rotates each token by its
+ * position and attention stays inside each document (query q sees key k iff k <= q and no document starts in
+ * (k, q]). Labels are the caller's, as in HF (the collator sets -100 at each document start). Anything else in
+ * positions is B200W_ERR_INVALID. Llama family only: OPT and Falcon return B200W_ERR_INVALID. */
+B200W_API int b200w_train_step_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels,
+                          const int32_t* positions, int n_seqs, float lr, float* loss_out, float* gnorm_out);
+B200W_API int b200w_forward_backward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels,
+                                const int32_t* positions, int n_seqs, float* loss_out);
+B200W_API int b200w_forward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels,
+                       const int32_t* positions, int n_seqs, float* logits_out, float* nll_out, float* loss_out);
 /* Number of kernels the library launched since the context was created (bench.py's
  * gpu_launches) and device bytes currently allocated. */
 B200W_API int64_t b200w_launch_count(const b200w_ctx* ctx);
@@ -262,6 +274,9 @@ B200W_API int b200w_op_rmsnorm_bwd(b200w_ctx* ctx, const void* dy, const void* x
  * buf [T, ld]; position = t % S */
 B200W_API int b200w_op_rope(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
                   int inverse);
+/* the same rotation at position = positions[t] (DEVICE int32 [T], each < S) */
+B200W_API int b200w_op_rope_positions(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh,
+                            float theta, int inverse, const int32_t* positions);
 B200W_API int b200w_op_swiglu_fwd(b200w_ctx* ctx, const void* gu, void* h, int T, int f);
 B200W_API int b200w_op_swiglu_bwd(b200w_ctx* ctx, const void* dh, const void* gu, void* dgu, int T, int f);
 /* labels (unshifted, int32 [T]) -> nll fp32 [T]; logits overwritten by dlogits * inv_n */
@@ -273,6 +288,15 @@ B200W_API int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);
+/* Per-document attention: positions DEVICE int32 [B * S] with the position_ids semantics of
+ * b200w_train_step_docs (not validated here); the library derives the document bounds from them. */
+B200W_API int b200w_op_attention_fwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                                void* out, int ld_out, float* lse2, const int32_t* positions, int B, int S,
+                                int H, int Hkv, float scale);
+B200W_API int b200w_op_attention_bwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                                const void* out, const void* dout, int ld_out, const float* lse2,
+                                float* delta, void* dqkv, const int32_t* positions, int B, int S, int H,
+                                int Hkv, float scale);
 /* g: fp32, or bf16 when g_bf16 != 0 (the data-parallel wire copy) */
 B200W_API int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, const void* g, int g_bf16,
                    void* w_bf16, int64_t n, float lr, float beta1, float beta2, float eps, float wd,

@@ -74,6 +74,9 @@ PROTOTYPES = {
     "b200w_profile_read": (C.c_int, [c_ctx, C.POINTER(C.c_double), C.POINTER(C.c_double), i64p]),
     "b200w_forward_backward": (C.c_int, [c_ctx, vp, vp, C.c_int, f32p]),
     "b200w_forward": (C.c_int, [c_ctx, vp, vp, C.c_int, vp, vp, f32p]),
+    "b200w_train_step_docs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_float, f32p, f32p]),
+    "b200w_forward_backward_docs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, f32p]),
+    "b200w_forward_docs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp, f32p]),
     "b200w_launch_count": (C.c_int64, [c_ctx]),
     "b200w_device_bytes": (C.c_int64, [c_ctx]),
     "b200w_infer_init": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int]),
@@ -103,6 +106,8 @@ PROTOTYPES = {
     "b200w_op_rmsnorm_bwd": (C.c_int, [c_ctx, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int]),
     "b200w_op_rope": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                 C.c_int]),
+    "b200w_op_rope_positions": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                          C.c_int, vp]),
     "b200w_op_swiglu_fwd": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
     "b200w_op_swiglu_bwd": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int]),
     "b200w_op_ce": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float]),
@@ -110,6 +115,10 @@ PROTOTYPES = {
                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
+    "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,
+                                              C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
+    "b200w_op_attention_bwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
+                                              vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_adamw": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, vp, C.c_int64, C.c_float, C.c_float,
                                  C.c_float, C.c_float, C.c_float, C.c_int, C.c_float]),
     "b200w_op_grad_norm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int64, f32p]),

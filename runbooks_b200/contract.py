@@ -48,6 +48,7 @@ class TrainParams:
     label_smoothing_factor: float = 0.0
     average_tokens_across_devices: str = "true"
     gradient_checkpointing: str = "false"   # TrainingArguments.gradient_checkpointing: activation recomputation (same results)
+    padding_free: str = "false"       # TRL SFTConfig.padding_free: each packed record attends only to itself (pack_documents)
     save_steps: int = 500
     logging_steps: int = 1
     seed: int = 42
@@ -110,6 +111,8 @@ def load_params(path: Optional[str] = None, environ: Optional[Dict[str, str]] = 
                          "normalises by the global target count (the TrainingArguments default)")
     if str(p.gradient_checkpointing).strip().lower() not in ("true", "false", "1", "0"):
         raise ValueError(f"gradient_checkpointing={p.gradient_checkpointing!r}: expected true or false")
+    if str(p.padding_free).strip().lower() not in ("true", "false", "1", "0"):
+        raise ValueError(f"padding_free={p.padding_free!r}: expected true or false")
     if p.warmup_steps < 0:
         raise ValueError("warmup_steps must be >= 0")
     if p.gradient_accumulation_steps < 1 or p.per_device_train_batch_size < 1:
@@ -119,6 +122,10 @@ def load_params(path: Optional[str] = None, environ: Optional[Dict[str, str]] = 
 
 def wants_recompute(p: TrainParams) -> bool:
     return str(p.gradient_checkpointing).strip().lower() in ("true", "1")
+
+
+def wants_padding_free(p: TrainParams) -> bool:
+    return str(p.padding_free).strip().lower() in ("true", "1")
 
 
 def warmup_steps_for(total_steps: int, warmup_steps: float) -> int:
@@ -224,6 +231,40 @@ def pack_sequences(docs: Iterable[List[int]], seq_len: int, bos_id: Optional[int
     ids[: len(stream)] = stream
     labels[: len(stream)] = stream
     return ids.reshape(n, seq_len), labels.reshape(n, seq_len)
+
+
+def pack_documents(docs: Iterable[List[int]], seq_len: int, bos_id: Optional[int],
+                   eos_id: Optional[int]) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Padding-free packing (HF DataCollatorWithFlattening, TRL padding_free): the token stream and row cut of
+    pack_sequences, plus position_ids that restart at 0 at every document start, which makes each document attend
+    only to itself (b200w_train_step_docs). A document cut by a row end continues in the next row as a new
+    document, so every position is < seq_len. As the collator does, the label of every document start (row starts
+    included) is -100. The eos padding of the last row is one more document, with labels -100.
+    Returns (ids, labels, positions), each int32 [n, seq_len]."""
+    stream: List[int] = []
+    starts: List[int] = []
+    for d in docs:
+        piece = ([bos_id] if bos_id is not None else []) + list(d) + ([eos_id] if eos_id is not None else [])
+        if piece:
+            starts.append(len(stream))
+            stream.extend(piece)
+    if not stream:
+        raise ValueError("dataset is empty after tokenisation")
+    n = (len(stream) + seq_len - 1) // seq_len
+    total = n * seq_len
+    ids = np.full(total, eos_id if eos_id is not None else 0, dtype=np.int32)
+    ids[: len(stream)] = stream
+    is_start = np.zeros(total, dtype=bool)
+    is_start[starts] = True
+    is_start[::seq_len] = True
+    if len(stream) < total:
+        is_start[len(stream)] = True
+    labels = ids.copy()
+    labels[len(stream):] = -100
+    labels[is_start] = -100
+    idx = np.arange(total)
+    positions = (idx - np.maximum.accumulate(np.where(is_start, idx, 0))).astype(np.int32)
+    return ids.reshape(n, seq_len), labels.reshape(n, seq_len), positions.reshape(n, seq_len)
 
 
 # ------------------------------------------------------------------------------------------------

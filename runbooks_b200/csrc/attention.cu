@@ -24,6 +24,11 @@
 //                 dQ += dS K -- no global atomics, no fp32 staging buffer.
 // Every per-element operation and every accumulation order is the same as in a schedule that waits for each
 // product, so the pipelining does not change a bit of the results.
+//
+// Document mode (template flag DOCS, packed rows of several documents): query q sees key k iff
+// doc_start[q] <= k <= q. The tiles walk only the key / query blocks that the bounds of their first / last row
+// allow (both bounds are non-decreasing along a row); inside that range the per-element compare masks the rest,
+// and a block wholly masked for one warpgroup is computed anyway and adds exact zeros (no new ring protocol).
 #include "host_common.h"
 #include "ops.h"
 #include "ptx.cuh"
@@ -107,10 +112,11 @@ __device__ __forceinline__ void store_rows_bf16(const float (&o)[64], bf16* row0
 constexpr int FWD_BQ = 128, FWD_BKV = 64;
 constexpr int FWD_SMEM = 2 * ATOM128 /*Q*/ + 2 * 2 * ATOM64 /*K x2*/ + 2 * 2 * ATOM64 /*V x2*/ + 256 /*barriers*/;
 
+template <bool DOCS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, int ld_out,
-                float* __restrict__ lse2, int k_off, int v_off, int B, int S, int H, int Hkv,
-                float scale_log2) {
+                float* __restrict__ lse2, const int* __restrict__ doc_start, int k_off, int v_off, int B, int S,
+                int H, int Hkv, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   require_1024_aligned(smem);
   uint8_t* sQ = smem;                      // 2 atoms (dh halves) x [128 x 128 B]
@@ -130,6 +136,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   const int tok0 = b * S;                // first token of this sequence
   const int q0 = qi * FWD_BQ;            // first query row inside the sequence
   const int njb = 2 * qi + 2;            // causal: key blocks [0, njb)
+  // document mode: key blocks [j0, njb). doc_start is non-decreasing, so no row of the tile sees a key before the
+  // first row's document; j0 <= 2 qi, so a CTA walks at least two blocks, as without documents
+  const int j0 = DOCS ? doc_start[tok0 + q0] / FWD_BKV : 0;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
@@ -154,14 +163,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
 #pragma unroll
         for (int r = 0; r < 2; ++r)
           tma_load_2d(sQ + a * ATOM128 + r * ATOM64, &tm_qkv, bar_q, h * DH + a * 64, tok0 + q0 + r * 64);
-      for (int j = 0; j < njb; ++j) {
-        const int buf = j & 1;
-        if (j >= 2) mbar_wait(&bar_kfree[buf], ((j >> 1) - 1) & 1);
+      for (int j = j0; j < njb; ++j) {
+        const int i = j - j0;  // ring position
+        const int buf = i & 1;
+        if (i >= 2) mbar_wait(&bar_kfree[buf], ((i >> 1) - 1) & 1);
         mbar_arrive_expect_tx(&bar_k[buf], 2 * ATOM64);
 #pragma unroll
         for (int a = 0; a < 2; ++a)
           tma_load_2d(sK + (buf * 2 + a) * ATOM64, &tm_qkv, &bar_k[buf], k_off + hk * DH + a * 64, tok0 + j * FWD_BKV);
-        if (j >= 2) mbar_wait(&bar_vfree[buf], ((j >> 1) - 1) & 1);
+        if (i >= 2) mbar_wait(&bar_vfree[buf], ((i >> 1) - 1) & 1);
         mbar_arrive_expect_tx(&bar_v[buf], 2 * ATOM64);
 #pragma unroll
         for (int a = 0; a < 2; ++a)
@@ -179,6 +189,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   const int row0 = q0 + wg * 64 + wi * 16 + (lane >> 2);  // query positions of this thread's two rows
   const int row1 = row0 + 8;
   const int last_j = 2 * qi + wg;  // the last key block that holds a key <= this warpgroup's last row
+  // document mode: the first key each row sees (ds0 <= ds1)
+  const int ds0 = DOCS ? doc_start[tok0 + row0] : 0, ds1 = DOCS ? doc_start[tok0 + row1] : 0;
   const uint32_t q_addr = smem_u32(sQ) + wg * ATOM64;
   float o[64];
 #pragma unroll
@@ -200,25 +212,38 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
           if (col > row1) s[4 * jj + 2 + e] = -INFINITY;
         }
     }
+    if (DOCS) {  // unconditional: a branch on the rows' own bounds diverges, and ptxas then serializes the wgmmas
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * jj + e;
+          if (col < ds0) s[4 * jj + e] = -INFINITY;
+          if (col < ds1) s[4 * jj + 2 + e] = -INFINITY;
+        }
+    }
     float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
       mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
       mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
     }
-    // scale > 0, so max commutes with it; block 0 holds key 0, visible to every row, so m is finite from then on
+    // scale > 0, so max commutes with it. Without documents block 0 holds key 0, visible to every row, so m is
+    // finite from then on. In document mode a row's first blocks may be wholly masked and leave m = -inf: the
+    // exponentials then take 0 as their reference, so P and alpha come out 0 rather than NaN.
     const float mn0 = fmaxf(m0, quad_max(mx0) * scale_log2), mn1 = fmaxf(m1, quad_max(mx1) * scale_log2);
-    alpha0 = ex2(m0 - mn0);
-    alpha1 = ex2(m1 - mn1);
+    const float r0 = DOCS && mn0 == -INFINITY ? 0.f : mn0, r1 = DOCS && mn1 == -INFINITY ? 0.f : mn1;
+    alpha0 = ex2(m0 - r0);
+    alpha1 = ex2(m1 - r1);
     m0 = mn0;
     m1 = mn1;
     float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
-      s[4 * jj] = ex2(fmaf(s[4 * jj], scale_log2, -mn0));
-      s[4 * jj + 1] = ex2(fmaf(s[4 * jj + 1], scale_log2, -mn0));
-      s[4 * jj + 2] = ex2(fmaf(s[4 * jj + 2], scale_log2, -mn1));
-      s[4 * jj + 3] = ex2(fmaf(s[4 * jj + 3], scale_log2, -mn1));
+      s[4 * jj] = ex2(fmaf(s[4 * jj], scale_log2, -r0));
+      s[4 * jj + 1] = ex2(fmaf(s[4 * jj + 1], scale_log2, -r0));
+      s[4 * jj + 2] = ex2(fmaf(s[4 * jj + 2], scale_log2, -r1));
+      s[4 * jj + 3] = ex2(fmaf(s[4 * jj + 3], scale_log2, -r1));
       ps0 += s[4 * jj] + s[4 * jj + 1];
       ps1 += s[4 * jj + 2] + s[4 * jj + 3];
     }
@@ -227,24 +252,28 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
   };
 
   mbar_wait(bar_q, 0);
-  mbar_wait(&bar_k[0], 0);  // block 0 holds key 0, which every row sees: no warpgroup skips it
+  mbar_wait(&bar_k[0], 0);  // block j0 <= 2 qi is in both warpgroups' range: no warpgroup skips it
   wg_fence();
   mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK), ATOM64);
   wg_commit();
   wg_wait<0>();
   wg_fence_regs(s);
   warp_release(&bar_kfree[0]);
-  softmax(0);  // O is still 0: its rescale is a no-op
+  softmax(j0);  // O is still 0: its rescale is a no-op
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) to_afrag(s, kk, pa[kk]);
 
-  for (int j = 1; j <= last_j; ++j) {
-    const int buf = j & 1;
-    mbar_wait(&bar_k[buf], (j >> 1) & 1);
+  for (int j = j0 + 1; j <= last_j; ++j) {
+    const int i = j - j0;
+    const int buf = i & 1;
+    mbar_wait(&bar_k[buf], (i >> 1) & 1);
     wg_fence();
     mma_over_dh<FWD_BKV>(s, q_addr, ATOM128, smem_u32(sK + buf * 2 * ATOM64), ATOM64);
     wg_commit();
-    mbar_wait(&bar_v[buf ^ 1], ((j - 1) >> 1) & 1);
+    mbar_wait(&bar_v[buf ^ 1], ((i - 1) >> 1) & 1);
+    // ptxas puts a warpgroup.arrive here itself; behind the loaded loop bound of document mode it counts that one
+    // as divergent and serializes every wgmma, so document mode issues the fence explicitly
+    if (DOCS) wg_fence();
     mma_pv<4>(o, pa, smem_u32(sV + (buf ^ 1) * 2 * ATOM64));
     wg_commit();
     wg_wait<1>();  // S(j) retired; PV(j - 1) may still run
@@ -264,22 +293,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ o
       o[4 * jj + 3] *= alpha1;
     }
   }
-  mbar_wait(&bar_v[last_j & 1], (last_j >> 1) & 1);
+  const int il = last_j - j0;
+  mbar_wait(&bar_v[il & 1], (il >> 1) & 1);
   wg_fence();
-  mma_pv<4>(o, pa, smem_u32(sV + (last_j & 1) * 2 * ATOM64));
+  mma_pv<4>(o, pa, smem_u32(sV + (il & 1) * 2 * ATOM64));
   wg_commit();
   wg_wait<0>();
   wg_fence_regs(o);
-  warp_release(&bar_vfree[last_j & 1]);
+  warp_release(&bar_vfree[il & 1]);
   // Blocks past last_j are fully masked for every row of this warpgroup: nothing to compute, but the release
   // waits for the block's loads, so that each warp's arrival counts toward this block's phase and never toward
   // the phase of the block before it in the same buffer (a warp running ahead would otherwise free that buffer
   // while another warp of the warpgroup still reads it).
-  for (int j = last_j + 1; j < njb; ++j) {
-    mbar_wait(&bar_k[j & 1], (j >> 1) & 1);
-    warp_release(&bar_kfree[j & 1]);
-    mbar_wait(&bar_v[j & 1], (j >> 1) & 1);
-    warp_release(&bar_vfree[j & 1]);
+  for (int i = il + 1; i < njb - j0; ++i) {
+    mbar_wait(&bar_k[i & 1], (i >> 1) & 1);
+    warp_release(&bar_kfree[i & 1]);
+    mbar_wait(&bar_v[i & 1], (i >> 1) & 1);
+    warp_release(&bar_vfree[i & 1]);
   }
 
   l0 = quad_sum(l0);
@@ -301,17 +331,19 @@ constexpr int BWD_BKV = 128, BWD_BQ = 64, KV_STAGES = 4;
 constexpr int KV_STAT = 2 * BWD_BQ * 4;  // bytes of a block's lse and delta rows (fp32)
 constexpr int KV_SMEM = 2 * ATOM128 /*K*/ + 2 * ATOM128 /*V*/ + KV_STAGES * 2 * ATOM64 /*Q*/ +
                         KV_STAGES * 2 * ATOM64 /*dO*/ + KV_STAGES * KV_STAT /*lse, delta*/ + 256;
+constexpr int KV_DOC = BWD_BKV * 4;  // document mode: the CTA's keys' doc_end, after the barriers
 
 // dV and dK stay in registers for the whole loop (128 per thread). A 64-query block is taken whole: S^T and dP^T
 // (32 fp32 registers each) become P^T and dS^T as bf16 A fragments (16 each) before block i + 1's scores are issued
 // into the same registers, so the peak is dV + dK + one block's scores + one block's fragments.
 // Block i's dV / dK products stay in flight while block i + 1's scores run, so Q/dO buffer i is freed one block
 // late; the fourth buffer keeps two blocks of loads ahead of the products.
+template <bool DOCS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta,
-                     bf16* __restrict__ dqkv, int ld_qkv, int k_off, int v_off, int B, int S, int H,
-                     int Hkv, float scale, float scale_log2) {
+                     const int* __restrict__ doc_end, bf16* __restrict__ dqkv, int ld_qkv, int k_off, int v_off,
+                     int B, int S, int H, int Hkv, float scale, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   require_1024_aligned(smem);
   uint8_t* sK = smem;                       // 2 atoms (dh halves) x [128 kv x 128 B]
@@ -322,6 +354,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sStat + KV_STAGES * 2 * BWD_BQ);
   uint64_t* bar_q = bar_kv + 1;               // [KV_STAGES] Q, dO block and its lse, delta in smem
   uint64_t* bar_qfree = bar_q + KV_STAGES;    // [KV_STAGES] MMAs that read Q/dO buffer b retired
+  const int* sEnd = reinterpret_cast<const int*>(reinterpret_cast<uint8_t*>(bar_kv) + 256);  // DOCS: [128]
 
   const int G = H / Hkv;
   const int jb = blockIdx.x / (B * Hkv);  // earliest key blocks (longest query loops) first
@@ -329,7 +362,10 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   const int hk = bhk % Hkv, b = bhk / Hkv;
   const int tok0 = b * S;
   const int kv0 = jb * BWD_BKV;
-  const int nqb = S / BWD_BQ - 2 * jb;  // query blocks [2 jb, S/64) see this key block
+  // query blocks [2 jb, S/64) see this key block; in document mode only those before the end of the last key's
+  // document (doc_end is non-decreasing and > kv0 + 127, so at least two blocks, as without documents)
+  const int qb_end = DOCS ? (doc_end[tok0 + kv0 + BWD_BKV - 1] + BWD_BQ - 1) / BWD_BQ : S / BWD_BQ;
+  const int nqb = qb_end - 2 * jb;
   const int n_iter = G * nqb;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const size_t Ttot = static_cast<size_t>(B) * S;
@@ -356,7 +392,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
   if (warp >> 2 == PRODUCER_WG) {
     setmaxnreg_dec<PRODUCER_REGS>();
     if (tid == PRODUCER_WG * 128) {
-      mbar_arrive_expect_tx(bar_kv, 4 * ATOM128);
+      mbar_arrive_expect_tx(bar_kv, 4 * ATOM128 + (DOCS ? KV_DOC : 0));
 #pragma unroll
       for (int a = 0; a < 2; ++a)
 #pragma unroll
@@ -364,6 +400,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
           tma_load_2d(sK + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, k_off + hk * DH + a * 64, tok0 + kv0 + r * 64);
           tma_load_2d(sV + a * ATOM128 + r * ATOM64, &tm_qkv, bar_kv, v_off + hk * DH + a * 64, tok0 + kv0 + r * 64);
         }
+      if (DOCS) bulk_load_1d(const_cast<int*>(sEnd), doc_end + tok0 + kv0, KV_DOC, bar_kv);
       IterPos ip{hk * G, 0};
       int buf = 0;
       uint32_t par = 0;
@@ -413,11 +450,14 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     mma_pv<BWD_BQ / 16>(dk, dsa, smem_u32(sQ + bf * 2 * ATOM64));
     wg_commit();
   };
-  // P^T of the block in buffer bf, in place of S^T. A block whose queries all precede this warpgroup's keys comes
-  // out as P = 0 and adds exact zeros to dV and dK.
+  // P^T of the block in buffer bf, in place of S^T. A block whose queries all precede this warpgroup's keys (or,
+  // in document mode, all follow their documents) comes out as P = 0 and adds exact zeros to dV and dK.
   auto probs = [&](int bf, int q_seq0) {
     const float* lse_s = sStat + bf * 2 * BWD_BQ;
     const bool diag = q_seq0 < kv_first + 64;  // some (q, kv) pairs of this block are masked
+    // document mode: one past the last query that sees each row's key, read from shared memory per block (held
+    // in registers across the loop, the two bounds make ptxas spill)
+    const int de_a = DOCS ? sEnd[kv_a - kv0] : 0, de_b = DOCS ? sEnd[kv_b - kv0] : 0;
 #pragma unroll
     for (int jj = 0; jj < BWD_BQ / 8; ++jj)
 #pragma unroll
@@ -429,6 +469,10 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         if (diag) {
           if (q_seq0 + q < kv_a) pa_ = 0.f;
           if (q_seq0 + q < kv_b) pb_ = 0.f;
+        }
+        if (DOCS) {  // queries past a row's document
+          if (q_seq0 + q >= de_a) pa_ = 0.f;
+          if (q_seq0 + q >= de_b) pb_ = 0.f;
         }
         st[4 * jj + e] = pa_;
         st[4 * jj + 2 + e] = pb_;
@@ -505,10 +549,12 @@ constexpr int DQ_SMEM = 2 * ATOM128 /*Q*/ + 2 * ATOM128 /*dO*/ + DQ_STAGES * 2 *
 
 // Block j's dQ product stays in flight while block j + 1's S and dP run, so K/V buffer j is freed one block late;
 // the fourth buffer keeps two blocks of loads ahead of the products.
+template <bool DOCS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
-                   const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
-                   int ld_qkv, int k_off, int v_off, int B, int S, int H, int Hkv, float scale, float scale_log2) {
+                   const float* __restrict__ lse2, const float* __restrict__ delta,
+                   const int* __restrict__ doc_start, bf16* __restrict__ dqkv, int ld_qkv, int k_off, int v_off,
+                   int B, int S, int H, int Hkv, float scale, float scale_log2) {
   extern __shared__ __align__(1024) uint8_t smem[];
   require_1024_aligned(smem);
   uint8_t* sQ = smem;                      // 2 atoms (dh halves) x [128 q x 128 B]
@@ -527,6 +573,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   const int tok0 = b * S;
   const int q0 = qi * DQ_BQ;
   const int njb = 2 * qi + 2;
+  const int j0 = DOCS ? doc_start[tok0 + q0] / DQ_BKV : 0;  // key blocks [j0, njb), as in the forward
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
@@ -556,8 +603,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
       uint32_t par = 0;
       // block j reuses block j-DQ_STAGES's buffer; the last DQ_STAGES passes load nothing and only wait for the
       // release of the last blocks (the consumers' waits are unbounded, this one is not)
-      for (int j = 0; j < njb + DQ_STAGES; ++j) {
-        if (j >= DQ_STAGES) mbar_wait(&bar_kvfree[buf], par ^ 1);
+      for (int j = j0; j < njb + DQ_STAGES; ++j) {
+        if (j >= j0 + DQ_STAGES) mbar_wait(&bar_kvfree[buf], par ^ 1);
         if (j < njb) {
           mbar_arrive_expect_tx(&bar_kv[buf], 4 * ATOM64);
 #pragma unroll
@@ -581,6 +628,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   const size_t stat = static_cast<size_t>(h) * (static_cast<size_t>(B) * S) + tok0;
   const float lse0 = lse2[stat + row0], lse1 = lse2[stat + row1];
   const float dl0 = delta[stat + row0], dl1 = delta[stat + row1];   // pre-multiplied by the scale
+  const int ds0 = DOCS ? doc_start[tok0 + row0] : 0, ds1 = DOCS ? doc_start[tok0 + row1] : 0;
   const uint32_t q_addr = smem_u32(sQ) + wg * ATOM64, do_addr = smem_u32(sdO) + wg * ATOM64;
   float dq[64];
 #pragma unroll
@@ -599,6 +647,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   };
   auto probs = [&](int j) {  // P of block j, in place of S
     const bool diag = j * DQ_BKV + DQ_BKV - 1 > q0 + wg * 64;
+    const bool before = DOCS && j * DQ_BKV < ds1;  // the block starts before a row's document
     const int col0 = j * DQ_BKV + 2 * (lane & 3);
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj)
@@ -610,6 +659,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
         if (diag) {
           if (col > row0) p0 = 0.f;
           if (col > row1) p1 = 0.f;
+        }
+        if (before) {
+          if (col < ds0) p0 = 0.f;
+          if (col < ds1) p1 = 0.f;
         }
         s[4 * jj + e] = p0;
         s[4 * jj + 2 + e] = p1;
@@ -637,13 +690,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_cons
   int buf = 0;
   uint32_t par = 0;
   mbar_wait_unbounded(bar_q, 0);
-  mbar_wait_unbounded(&bar_kv[0], 0);  // block 0 holds key 0, which every row sees: no warpgroup skips it
+  mbar_wait_unbounded(&bar_kv[0], 0);  // block j0 <= 2 qi is in both warpgroups' range: no warpgroup skips it
   issue_s(0);
   wg_wait<0>();
   wg_fence_regs(s);
-  probs(0);
+  probs(j0);
   grads(0);
-  for (int j = 1; j <= last_j; ++j) {
+  for (int j = j0 + 1; j <= last_j; ++j) {
     const int prev = buf;
     if (++buf == DQ_STAGES) { buf = 0; par ^= 1; }
     mbar_wait_unbounded(&bar_kv[buf], par);
@@ -678,24 +731,31 @@ void set_smem(K kern, int bytes) {
 }  // namespace
 
 void attention_fwd(const void* qkv, int ld_qkv, int k_off, int v_off, void* out, int ld_out,
-                   float* lse2, int B, int S, int H, int Hkv, float scale, cudaStream_t s) {
+                   float* lse2, int B, int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs) {
   B200W_CHECK(S % 128 == 0, "sequence length must be a multiple of 128");
   B200W_CHECK(H % Hkv == 0 && ld_out % 8 == 0, "bad head configuration");
   const size_t T = static_cast<size_t>(B) * S;
   CUtensorMap tm = make_tmap_bf16_2d(qkv, T, ld_qkv, ld_qkv, 64, 64);
   static PerDeviceOnce once;
-  once.run([&] { set_smem(attn_fwd_kernel, FWD_SMEM); });
+  once.run([&] {
+    set_smem(attn_fwd_kernel<false>, FWD_SMEM);
+    set_smem(attn_fwd_kernel<true>, FWD_SMEM);
+  });
   const int grid = (S / FWD_BQ) * B * H;
   const float scale_log2 = scale * 1.4426950408889634f;
-  attn_fwd_kernel<<<grid, NTHREADS, FWD_SMEM, s>>>(tm, static_cast<bf16*>(out), ld_out, lse2, k_off,
-                                                   v_off, B, S, H, Hkv, scale_log2);
+  if (docs)
+    attn_fwd_kernel<true><<<grid, NTHREADS, FWD_SMEM, s>>>(tm, static_cast<bf16*>(out), ld_out, lse2, docs->start,
+                                                           k_off, v_off, B, S, H, Hkv, scale_log2);
+  else
+    attn_fwd_kernel<false><<<grid, NTHREADS, FWD_SMEM, s>>>(tm, static_cast<bf16*>(out), ld_out, lse2, nullptr,
+                                                            k_off, v_off, B, S, H, Hkv, scale_log2);
   B200W_CUDA(cudaGetLastError());
 }
 
 // dqkv receives dq (column 0), dk (k_off), dv (v_off), all bf16. delta: [H, T] fp32 scratch.
 void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void* out,
                    const void* dout, int ld_out, const float* lse2, float* delta, void* dqkv, int B,
-                   int S, int H, int Hkv, float scale, cudaStream_t s) {
+                   int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs) {
   B200W_CHECK(S % 128 == 0, "sequence length must be a multiple of 128");
   B200W_CHECK(H % Hkv == 0, "bad head configuration");
   const size_t T = static_cast<size_t>(B) * S;
@@ -704,17 +764,27 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
   CUtensorMap tm_do = make_tmap_bf16_2d(dout, T, ld_out, ld_out, 64, 64);
   static PerDeviceOnce once;
   once.run([&] {
-    set_smem(attn_bwd_dkdv_kernel, KV_SMEM);
-    set_smem(attn_bwd_dq_kernel, DQ_SMEM);
+    set_smem(attn_bwd_dkdv_kernel<false>, KV_SMEM);
+    set_smem(attn_bwd_dq_kernel<false>, DQ_SMEM);
+    set_smem(attn_bwd_dkdv_kernel<true>, KV_SMEM + KV_DOC);
+    set_smem(attn_bwd_dq_kernel<true>, DQ_SMEM);
   });
   const float scale_log2 = scale * 1.4426950408889634f;
-  attn_bwd_dkdv_kernel<<<(S / BWD_BKV) * B * Hkv, NTHREADS, KV_SMEM, s>>>(
-      tm_qkv, tm_do, lse2, delta, static_cast<bf16*>(dqkv), ld_qkv, k_off, v_off, B, S, H, Hkv, scale,
-      scale_log2);
-  B200W_CUDA(cudaGetLastError());
-  attn_bwd_dq_kernel<<<(S / DQ_BQ) * B * H, NTHREADS, DQ_SMEM, s>>>(
-      tm_qkv, tm_do, lse2, delta, static_cast<bf16*>(dqkv), ld_qkv, k_off, v_off, B, S, H, Hkv, scale,
-      scale_log2);
+  const dim3 g_kv((S / BWD_BKV) * B * Hkv), g_q((S / DQ_BQ) * B * H);
+  bf16* d = static_cast<bf16*>(dqkv);
+  if (docs) {
+    attn_bwd_dkdv_kernel<true><<<g_kv, NTHREADS, KV_SMEM + KV_DOC, s>>>(tm_qkv, tm_do, lse2, delta, docs->end, d, ld_qkv,
+                                                               k_off, v_off, B, S, H, Hkv, scale, scale_log2);
+    B200W_CUDA(cudaGetLastError());
+    attn_bwd_dq_kernel<true><<<g_q, NTHREADS, DQ_SMEM, s>>>(tm_qkv, tm_do, lse2, delta, docs->start, d, ld_qkv,
+                                                            k_off, v_off, B, S, H, Hkv, scale, scale_log2);
+  } else {
+    attn_bwd_dkdv_kernel<false><<<g_kv, NTHREADS, KV_SMEM, s>>>(tm_qkv, tm_do, lse2, delta, nullptr, d, ld_qkv,
+                                                                k_off, v_off, B, S, H, Hkv, scale, scale_log2);
+    B200W_CUDA(cudaGetLastError());
+    attn_bwd_dq_kernel<false><<<g_q, NTHREADS, DQ_SMEM, s>>>(tm_qkv, tm_do, lse2, delta, nullptr, d, ld_qkv,
+                                                             k_off, v_off, B, S, H, Hkv, scale, scale_log2);
+  }
   B200W_CUDA(cudaGetLastError());
 }
 

@@ -223,6 +223,9 @@ struct b200w_ctx {
   size_t ids_cap = 0;
   int32_t* pinned = nullptr;
   size_t pinned_cap = 0;
+  // per-document attention (the _docs calls): the batch's positions and the DocBounds derived from them
+  int32_t *pos_dev = nullptr, *doc_start = nullptr, *doc_end = nullptr;
+  size_t docs_cap = 0;
   bf16 *dh_a = nullptr, *dh_b = nullptr, *dn = nullptr, *dact = nullptr, *dgu = nullptr,
        *dattn = nullptr, *dqkv = nullptr;
   float *delta = nullptr, *dw_partial = nullptr;
@@ -558,7 +561,9 @@ void egemm(b200w_ctx* c, const void* A, bool a_mn, int lda, const void* B, bool 
 // ---- forward of one micro-batch (ids already on device): Llama family ------------------------
 // One Llama decoder layer: x's buffers receive the activations the backward needs, h_next the layer's output
 // (nullptr in the recompute pass of the backward, which stops before the down projection).
-void forward_layer_llama(b200w_ctx* c, int l, const bf16* h_in, bf16* h_next, b200w_ctx::LayerA& x, int nseq) {
+// docs (nullable): RoPE at the documents' positions and attention within each document.
+void forward_layer_llama(b200w_ctx* c, int l, const bf16* h_in, bf16* h_next, b200w_ctx::LayerA& x, int nseq,
+                         const DocBounds* docs) {
   const b200w_arch& a = c->arch;
   const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
   const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
@@ -569,8 +574,8 @@ void forward_layer_llama(b200w_ctx* c, int l, const bf16* h_in, bf16* h_next, b2
   const auto& p = c->lp[l];
   rmsnorm_fwd(h_in, c->w + p.ln1, x.n1, x.rstd1, T, d, a.rms_norm_eps, s); ++n;
   egemm(c, x.n1, false, d, c->w + p.wqkv, false, d, x.qkv, nullptr, false, qkvd, T, qkvd, d);
-  rope_apply(x.qkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, false, s); ++n;
-  attention_fwd(x.qkv, qkvd, qd, qd + kd, x.attn, qd, x.lse, nseq, S, H, Hkv, scale, s); ++n;
+  rope_apply(x.qkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, false, s, 0, docs ? docs->pos : nullptr); ++n;
+  attention_fwd(x.qkv, qkvd, qd, qd + kd, x.attn, qd, x.lse, nseq, S, H, Hkv, scale, s, docs); ++n;
   egemm(c, x.attn, false, qd, c->w + p.wo, false, qd, x.h_mid, h_in, false, d, T, d, qd);
   rmsnorm_fwd(x.h_mid, c->w + p.ln2, x.n2, x.rstd2, T, d, a.rms_norm_eps, s); ++n;
   egemm(c, x.n2, false, d, c->w + p.wgu, false, d, x.gu, nullptr, false, 2 * f, T, 2 * f, d);
@@ -578,7 +583,7 @@ void forward_layer_llama(b200w_ctx* c, int l, const bf16* h_in, bf16* h_next, b2
   if (h_next) egemm(c, x.act, false, f, c->w + p.wd, false, f, h_next, x.h_mid, false, d, T, d, f);
 }
 
-void forward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq) {
+void forward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, const DocBounds* docs) {
   const b200w_arch& a = c->arch;
   const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size;
   cudaStream_t s = c->stream;
@@ -592,7 +597,7 @@ void forward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq) {
     bf16* h_in = c->training ? x.h_in : h;
     bf16* h_next = c->training ? (l + 1 < L ? c->la[l + 1].h_in : c->h_final)
                                : (h == c->la[0].h_in ? c->h_final : c->la[0].h_in);
-    forward_layer_llama(c, l, h_in, h_next, x, nseq);
+    forward_layer_llama(c, l, h_in, h_next, x, nseq, docs);
     h = h_next;
   }
   // in training mode h == h_final; in forward-only mode h is whichever buffer came last
@@ -679,10 +684,11 @@ void forward_micro_falcon(b200w_ctx* c, const int32_t* ids, int nseq) {
   if (c->training && h != c->h_final) throw Error("internal: residual stream bookkeeping");
 }
 
-void forward_micro(b200w_ctx* c, const int32_t* ids, int nseq) {
+// docs: Llama family only (check_docs_family refuses the others before any GPU work)
+void forward_micro(b200w_ctx* c, const int32_t* ids, int nseq, const DocBounds* docs = nullptr) {
   if (is_opt(c->arch)) forward_micro_opt(c, ids, nseq);
   else if (is_falcon(c->arch)) forward_micro_falcon(c, ids, nseq);
-  else forward_micro_llama(c, ids, nseq);
+  else forward_micro_llama(c, ids, nseq, docs);
 }
 
 // loss + dlogits (in place); the normaliser 1 / num_items_in_batch is the device scalar c->inv_n
@@ -756,7 +762,8 @@ void allreduce_range(b200w_ctx* c, size_t off, size_t count, bool precast = fals
 
 // backward of one micro-batch. first: overwrite gradients instead of accumulating.
 // overlap_ar: launch the all-reduce of each matrix as soon as its gradient is final.
-void backward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar) {
+void backward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar,
+                          const DocBounds* docs) {
   const b200w_arch& a = c->arch;
   const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
   const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, V = a.vocab_size;
@@ -786,7 +793,7 @@ void backward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, bool first
     const size_t o_q = p.wqkv, o_o = p.wo, o_gu = p.wgu, o_d = p.wd;
     // activation recomputation: the layer's forward again, from its saved input into the shared buffers (the same
     // kernels on the same operands: bit-identical activations, hence bit-identical gradients)
-    if (c->recompute) forward_layer_llama(c, l, x.h_in, nullptr, x, nseq);
+    if (c->recompute) forward_layer_llama(c, l, x.h_in, nullptr, x, nseq, docs);
     // h_next = h_mid + act Wd^T
     egemm(c, dh_cur, false, d, c->w + o_d, true, f, c->dact, nullptr, false, f, T, f, d);
     egemm(c, dh_cur, true, d, x.act, true, f, g + o_d, acc(o_d), true, f, d, f, T, nullptr, 0, wire(o_d));
@@ -803,8 +810,8 @@ void backward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, bool first
     egemm(c, dh_cur, true, d, x.attn, true, qd, g + o_o, acc(o_o), true, qd, d, qd, T, nullptr, 0, wire(o_o));
     arw(o_o, static_cast<size_t>(d) * qd);
     attention_bwd(x.qkv, qkvd, qd, qd + kd, x.attn, c->dattn, qd, x.lse, c->delta, c->dqkv, nseq, S, H,
-                  Hkv, scale, s); n += 3;
-    rope_apply(c->dqkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, true, s); ++n;
+                  Hkv, scale, s, docs); n += 3;
+    rope_apply(c->dqkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, true, s, 0, docs ? docs->pos : nullptr); ++n;
     egemm(c, c->dqkv, false, qkvd, c->w + o_q, true, d, c->dn, nullptr, false, d, T, d, qkvd);
     egemm(c, c->dqkv, true, qkvd, x.n1, true, d, g + o_q, acc(o_q), true, d, qkvd, d, T, nullptr, 0, wire(o_q));
     arw(o_q, static_cast<size_t>(qkvd) * d);
@@ -931,13 +938,14 @@ void backward_micro_falcon(b200w_ctx* c, const int32_t* ids, int nseq, bool firs
   ar(0, c->n_zero_prefix);
 }
 
-void backward_micro(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar) {
+void backward_micro(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar,
+                    const DocBounds* docs) {
   // while the all-reduce runs under the backward, the persistent GEMMs leave NCCL its SMs
   if (overlap_ar) gemm_set_sm_reserve(c->ar_sm_reserve);
   try {
     if (is_opt(c->arch)) backward_micro_opt(c, ids, nseq, first, overlap_ar);
     else if (is_falcon(c->arch)) backward_micro_falcon(c, ids, nseq, first, overlap_ar);
-    else backward_micro_llama(c, ids, nseq, first, overlap_ar);
+    else backward_micro_llama(c, ids, nseq, first, overlap_ar, docs);
   } catch (...) {
     gemm_set_sm_reserve(0);
     throw;
@@ -996,6 +1004,50 @@ void upload_batch(b200w_ctx* c, const int32_t* ids, const int32_t* labels, size_
                              cudaMemcpyHostToDevice, c->stream));
 }
 
+// Per-document attention is built for the Llama family only: OPT's learned positions and Falcon's path take no
+// positions. Checked before any GPU work.
+void check_docs_family(const b200w_ctx* c) {
+  B200W_CHECK(!is_opt(c->arch) && !is_falcon(c->arch),
+              "per-document attention (positions) is built for the Llama family only");
+}
+
+// positions: HOST int32 [n_seqs, S] with HF position_ids semantics (DataCollatorWithFlattening): every row starts
+// at 0 and each later entry is 0 (a new document) or the previous entry + 1, hence < S. Uploaded, and the
+// DocBounds of the whole batch derived from them on the device.
+void upload_positions(b200w_ctx* c, const int32_t* positions, int n_seqs) {
+  const int S = c->arch.max_seq_len;
+  for (int r = 0; r < n_seqs; ++r) {
+    const int32_t* p = positions + static_cast<size_t>(r) * S;
+    if (p[0] != 0) throw Error("check failed: positions of row " + std::to_string(r) + " do not start at 0");
+    for (int i = 1; i < S; ++i)
+      if (p[i] != 0 && p[i] != p[i - 1] + 1)
+        throw Error("check failed: positions[" + std::to_string(r) + "][" + std::to_string(i) + "] = " +
+                    std::to_string(p[i]) + " is neither 0 (a new document) nor the previous position + 1");
+  }
+  const size_t n = static_cast<size_t>(n_seqs) * S;
+  if (c->docs_cap < n) {
+    if (c->pos_dev) {  // every kernel that read the old buffers was enqueued before this point
+      B200W_CUDA(cudaStreamSynchronize(c->stream));
+      c->release(c->pos_dev);
+      c->release(c->doc_start);
+      c->release(c->doc_end);
+    }
+    c->pos_dev = c->alloc<int32_t>(n);
+    c->doc_start = c->alloc<int32_t>(n);
+    c->doc_end = c->alloc<int32_t>(n);
+    c->docs_cap = n;
+  }
+  // pageable source: the call returns once the bytes are staged, so the caller's array may go
+  B200W_CUDA(cudaMemcpyAsync(c->pos_dev, positions, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  doc_bounds(c->pos_dev, c->doc_start, c->doc_end, static_cast<int>(n), S, c->stream); ++c->launches;
+}
+
+// the DocBounds of the rows [row0, ...) of the uploaded batch
+DocBounds docs_at(const b200w_ctx* c, size_t row0) {
+  const size_t off = row0 * c->arch.max_seq_len;
+  return DocBounds{c->pos_dev + off, c->doc_start + off, c->doc_end + off};
+}
+
 // HF Trainer under DDP (transformers 5.5 trainer.py:2140-2143, average_tokens_across_devices = True,
 // the TrainingArguments default): num_items_in_batch is gathered and SUMMED over the ranks, each
 // rank's loss is sum(nll_r) / n_global * world (trainer.py:2013-2018) and DDP's mean removes the
@@ -1030,9 +1082,9 @@ void set_global_count(b200w_ctx* c, long nvalid_local) {
 // forward + loss + backward over a batch that is already on the device. nvalid = this rank's count
 // of target tokens; with a communicator the gradients returned are those of the GLOBAL batch
 // (sum over ranks of sum(nll) / n_global), all-reduced into the bf16 wire copy c->gw, and scal[0] is
-// the global loss.
+// the global loss. docs: the batch's positions were uploaded (upload_positions): per-document attention.
 void fwd_bwd_device(b200w_ctx* c, const int32_t* ids_dev, const int32_t* labels_dev, int n_seqs,
-                    long nvalid, bool allow_overlap) {
+                    long nvalid, bool allow_overlap, bool docs = false) {
   const int S = c->arch.max_seq_len, mb = c->micro_batch;
   B200W_CHECK(c->has_model && c->training, "model not initialised for training");
   B200W_CHECK(n_seqs > 0 && n_seqs % mb == 0, "n_seqs must be a positive multiple of micro_batch");
@@ -1047,9 +1099,11 @@ void fwd_bwd_device(b200w_ctx* c, const int32_t* ids_dev, const int32_t* labels_
   for (int mi = 0; mi < n_micro; ++mi) {
     const int32_t* mids = ids_dev + static_cast<size_t>(mi) * mb * S;
     const int32_t* mlab = labels_dev + static_cast<size_t>(mi) * mb * S;
+    const DocBounds db = docs ? docs_at(c, static_cast<size_t>(mi) * mb) : DocBounds{};
+    const DocBounds* mdocs = docs ? &db : nullptr;
     {
       NvtxRange r("b200w forward");
-      forward_micro(c, mids, mb);
+      forward_micro(c, mids, mb, mdocs);
     }
     {
       NvtxRange r("b200w loss");
@@ -1057,7 +1111,7 @@ void fwd_bwd_device(b200w_ctx* c, const int32_t* ids_dev, const int32_t* labels_
     }
     const bool ar = allow_overlap && c->comm && mi == n_micro - 1;
     NvtxRange r(ar ? "b200w backward + gradient exchange" : "b200w backward");
-    backward_micro(c, mids, mb, mi == 0, ar);
+    backward_micro(c, mids, mb, mi == 0, ar, mdocs);
   }
   if (c->comm) {
     if (!allow_overlap) allreduce_range(c, 0, c->n_elems);
@@ -1070,14 +1124,17 @@ void fwd_bwd_device(b200w_ctx* c, const int32_t* ids_dev, const int32_t* labels_
   }
 }
 
+// positions (nullable): HOST [n_seqs, S], per-document attention (upload_positions)
 void fwd_bwd_all(b200w_ctx* c, const int32_t* ids, const int32_t* labels, int n_seqs,
-                 bool allow_overlap) {
+                 bool allow_overlap, const int32_t* positions = nullptr) {
   const int S = c->arch.max_seq_len;
   B200W_CHECK(c->has_model && c->training, "model not initialised for training");
   B200W_CHECK(n_seqs > 0, "empty batch");
+  if (positions) check_docs_family(c);
   const long nvalid = count_valid(labels, n_seqs, S);
   upload_batch(c, ids, labels, static_cast<size_t>(n_seqs) * S);
-  fwd_bwd_device(c, c->ids_dev, c->labels_dev, n_seqs, nvalid, allow_overlap);
+  if (positions) upload_positions(c, positions, n_seqs);
+  fwd_bwd_device(c, c->ids_dev, c->labels_dev, n_seqs, nvalid, allow_overlap, positions != nullptr);
 }
 
 // all-reduce is complete on c->stream; global-norm clip + AdamW over the flat parameter space.
@@ -1151,6 +1208,72 @@ bool owned_part(const b200w_ctx* c, const Param& p, OwnedPart* out) {
     return true;
   }
   return false;
+}
+
+// The bodies of b200w_forward_backward, b200w_train_step and b200w_forward. positions (nullable, HOST
+// [n_seqs, S]): per-document attention, the _docs forms.
+void forward_backward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
+                           int n_seqs, float* loss_out) {
+  B200W_CHECK(ids && labels, "NULL batch");
+  fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/false, positions);
+  // the reduced gradients live in the bf16 wire copy: widen them for b200w_read_state(kind = 1)
+  if (ctx->comm && !ctx->shard) { cast_bf16_to_f32(ctx->gw, ctx->g, ctx->n_elems, ctx->stream); ++ctx->launches; }
+  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost,
+                             ctx->stream));
+  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (loss_out) *loss_out = ctx->host_scal[0];
+}
+
+void train_step_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
+                     int n_seqs, float lr, float* loss_out, float* gnorm_out) {
+  B200W_CHECK(ids && labels, "NULL batch");
+  fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/true, positions);
+  optimizer_step(ctx, lr);
+  cudaStream_t s = ctx->stream;
+  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  B200W_CUDA(cudaStreamSynchronize(s));
+  if (loss_out) *loss_out = ctx->host_scal[0];
+  if (gnorm_out) *gnorm_out = ctx->host_scal[2];
+}
+
+void forward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions, int n_seqs,
+                  float* logits_out, float* nll_out, float* loss_out) {
+  B200W_CHECK(ctx->has_model && ids, "no model / NULL ids");
+  B200W_CHECK(n_seqs >= 1 && n_seqs <= ctx->micro_batch, "n_seqs must be <= micro_batch");
+  if (positions) check_docs_family(ctx);
+  const int S = ctx->arch.max_seq_len, V = ctx->arch.vocab_size;
+  const size_t T = static_cast<size_t>(n_seqs) * S;
+  std::vector<int32_t> dummy;
+  if (!labels) { dummy.assign(T, -100); }
+  upload_batch(ctx, ids, labels ? labels : dummy.data(), T);
+  DocBounds db{};
+  if (positions) {
+    upload_positions(ctx, positions, n_seqs);
+    db = docs_at(ctx, 0);
+  }
+  forward_micro(ctx, ctx->ids_dev, n_seqs, positions ? &db : nullptr);
+  if (logits_out) {
+    void* scratch = nullptr;
+    B200W_CUDA(cudaMalloc(&scratch, T * V * 4));
+    cast_bf16_to_f32(ctx->logits, static_cast<float*>(scratch), T * V, ctx->stream);
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    B200W_CUDA(cudaMemcpy(logits_out, scratch, T * V * 4, cudaMemcpyDeviceToHost));
+    cudaFree(scratch);
+  }
+  if (labels && (nll_out || loss_out)) {
+    const long nvalid = count_valid(labels, n_seqs, S);
+    set_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, nvalid);
+    inv_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, ctx->inv_n);
+    B200W_CUDA(cudaGetLastError());
+    B200W_CUDA(cudaMemsetAsync(ctx->scal, 0, 8 * sizeof(float), ctx->stream));
+    loss_micro(ctx, ctx->labels_dev, n_seqs);
+    B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float),
+                               cudaMemcpyDeviceToHost, ctx->stream));
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (nll_out) B200W_CUDA(cudaMemcpy(nll_out, ctx->nll, T * 4, cudaMemcpyDeviceToHost));
+    if (loss_out) *loss_out = ctx->host_scal[0];
+  }
+  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
 }
 
 }  // namespace
@@ -1621,29 +1744,25 @@ int b200w_comm_init(b200w_ctx* ctx, int rank, int nranks, const void* id128) {
 
 int b200w_forward_backward(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, int n_seqs,
                            float* loss_out) {
+  return guarded(ctx, [&] { forward_backward_call(ctx, ids, labels, nullptr, n_seqs, loss_out); });
+}
+int b200w_forward_backward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
+                                int n_seqs, float* loss_out) {
   return guarded(ctx, [&] {
-    B200W_CHECK(ids && labels, "NULL batch");
-    fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/false);
-    // the reduced gradients live in the bf16 wire copy: widen them for b200w_read_state(kind = 1)
-    if (ctx->comm && !ctx->shard) { cast_bf16_to_f32(ctx->gw, ctx->g, ctx->n_elems, ctx->stream); ++ctx->launches; }
-    B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost,
-                               ctx->stream));
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (loss_out) *loss_out = ctx->host_scal[0];
+    B200W_CHECK(positions, "NULL positions");
+    forward_backward_call(ctx, ids, labels, positions, n_seqs, loss_out);
   });
 }
 
 int b200w_train_step(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, int n_seqs, float lr,
                      float* loss_out, float* gnorm_out) {
+  return guarded(ctx, [&] { train_step_call(ctx, ids, labels, nullptr, n_seqs, lr, loss_out, gnorm_out); });
+}
+int b200w_train_step_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
+                          int n_seqs, float lr, float* loss_out, float* gnorm_out) {
   return guarded(ctx, [&] {
-    B200W_CHECK(ids && labels, "NULL batch");
-    fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/true);
-    optimizer_step(ctx, lr);
-    cudaStream_t s = ctx->stream;
-    B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, s));
-    B200W_CUDA(cudaStreamSynchronize(s));
-    if (loss_out) *loss_out = ctx->host_scal[0];
-    if (gnorm_out) *gnorm_out = ctx->host_scal[2];
+    B200W_CHECK(positions, "NULL positions");
+    train_step_call(ctx, ids, labels, positions, n_seqs, lr, loss_out, gnorm_out);
   });
 }
 
@@ -1711,37 +1830,13 @@ int b200w_profile_read(b200w_ctx* ctx, double* ms_out, double* flops_out, int64_
 
 int b200w_forward(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, int n_seqs,
                   float* logits_out, float* nll_out, float* loss_out) {
+  return guarded(ctx, [&] { forward_call(ctx, ids, labels, nullptr, n_seqs, logits_out, nll_out, loss_out); });
+}
+int b200w_forward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
+                       int n_seqs, float* logits_out, float* nll_out, float* loss_out) {
   return guarded(ctx, [&] {
-    B200W_CHECK(ctx->has_model && ids, "no model / NULL ids");
-    B200W_CHECK(n_seqs >= 1 && n_seqs <= ctx->micro_batch, "n_seqs must be <= micro_batch");
-    const int S = ctx->arch.max_seq_len, V = ctx->arch.vocab_size;
-    const size_t T = static_cast<size_t>(n_seqs) * S;
-    std::vector<int32_t> dummy;
-    if (!labels) { dummy.assign(T, -100); }
-    upload_batch(ctx, ids, labels ? labels : dummy.data(), T);
-    forward_micro(ctx, ctx->ids_dev, n_seqs);
-    if (logits_out) {
-      void* scratch = nullptr;
-      B200W_CUDA(cudaMalloc(&scratch, T * V * 4));
-      cast_bf16_to_f32(ctx->logits, static_cast<float*>(scratch), T * V, ctx->stream);
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-      B200W_CUDA(cudaMemcpy(logits_out, scratch, T * V * 4, cudaMemcpyDeviceToHost));
-      cudaFree(scratch);
-    }
-    if (labels && (nll_out || loss_out)) {
-      const long nvalid = count_valid(labels, n_seqs, S);
-      set_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, nvalid);
-      inv_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, ctx->inv_n);
-      B200W_CUDA(cudaGetLastError());
-      B200W_CUDA(cudaMemsetAsync(ctx->scal, 0, 8 * sizeof(float), ctx->stream));
-      loss_micro(ctx, ctx->labels_dev, n_seqs);
-      B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float),
-                                 cudaMemcpyDeviceToHost, ctx->stream));
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-      if (nll_out) B200W_CUDA(cudaMemcpy(nll_out, ctx->nll, T * 4, cudaMemcpyDeviceToHost));
-      if (loss_out) *loss_out = ctx->host_scal[0];
-    }
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    B200W_CHECK(positions, "NULL positions");
+    forward_call(ctx, ids, labels, positions, n_seqs, logits_out, nll_out, loss_out);
   });
 }
 
@@ -1900,6 +1995,65 @@ int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_of
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {
   HOOK(attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv,
                      scale, ctx->stream));
+}
+}  // extern "C"
+
+namespace {
+// runs f(DocBounds) with the bounds of device positions [B * S] derived into scratch (doc_bounds)
+template <typename F>
+void with_doc_bounds(b200w_ctx* ctx, const int32_t* positions, int B, int S, F&& f) {
+  B200W_CHECK(positions, "NULL positions");
+  const size_t T = static_cast<size_t>(B) * S;
+  int32_t* se = nullptr;
+  B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&se), 2 * T * sizeof(int32_t)));
+  try {
+    doc_bounds(positions, se, se + T, static_cast<int>(T), S, ctx->stream);
+    ++ctx->launches;
+    const DocBounds db{positions, se, se + T};
+    f(db);
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+  } catch (...) { cudaFree(se); throw; }
+  cudaFree(se);
+}
+}  // namespace
+
+extern "C" {
+
+int b200w_op_attention_fwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off, void* out,
+                                int ld_out, float* lse2, const int32_t* positions, int B, int S, int H, int Hkv,
+                                float scale) {
+  return guarded(ctx, [&] {
+    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
+      attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx->stream, &db);
+      ++ctx->launches;
+    });
+  });
+}
+int b200w_op_attention_bwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                                const void* out, const void* dout, int ld_out, const float* lse2, float* delta,
+                                void* dqkv, const int32_t* positions, int B, int S, int H, int Hkv, float scale) {
+  return guarded(ctx, [&] {
+    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
+      attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv, scale,
+                    ctx->stream, &db);
+      ctx->launches += 3;
+    });
+  });
+}
+int b200w_op_rope_positions(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
+                            int inverse, const int32_t* positions) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(positions, "NULL positions");
+    float2* tab = nullptr;
+    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&tab), static_cast<size_t>(S) * (dh / 2) * sizeof(float2)));
+    try {
+      rope_table(tab, S, dh, theta, ctx->stream);
+      rope_apply(buf, ld, tab, T, S, nheads, dh, inverse != 0, ctx->stream, 0, positions);
+      ++ctx->launches;
+      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    } catch (...) { cudaFree(tab); throw; }
+    cudaFree(tab);
+  });
 }
 int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, const void* g, int g_bf16,
                    void* w_bf16, int64_t n, float lr, float beta1, float beta2, float eps, float wd,

@@ -272,7 +272,8 @@ __global__ void rmsnorm_dw_reduce_kernel(const float* __restrict__ dw_partial, f
 // apply_rotary_pos_emb; inv_freq = theta^(-2i/dh))
 // ------------------------------------------------------------------------------------------
 __global__ void rope_apply_kernel(bf16* buf, int ld, const float2* __restrict__ tab, int T, int S,
-                                  int nheads, int dh, int head_stride, float sgn) {
+                                  int nheads, int dh, int head_stride, float sgn,
+                                  const int32_t* __restrict__ positions) {
   const int half = dh / 2;
   const int per_head = half / 8;  // threads per (token, head)
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -281,7 +282,7 @@ __global__ void rope_apply_kernel(bf16* buf, int ld, const float2* __restrict__ 
   const int i0 = static_cast<int>(idx % per_head) * 8;
   const int h = static_cast<int>((idx / per_head) % nheads);
   const int t = static_cast<int>(idx / (static_cast<long long>(per_head) * nheads));
-  const int pos = t % S;
+  const int pos = positions ? positions[t] : t % S;
   bf16* p = buf + static_cast<size_t>(t) * ld + h * head_stride + i0;
   float x1[8], x2[8], o1[8], o2[8];
   load8(p, x1);
@@ -295,6 +296,24 @@ __global__ void rope_apply_kernel(bf16* buf, int ld, const float2* __restrict__ 
   }
   store8(p, o1);
   store8(p + half, o2);
+}
+
+// Document bounds of token t = b * S + i: start = i - pos[t]; end = the first i' > i whose document starts after
+// i (start is non-decreasing along a row, so a binary search over the row), or S.
+__global__ void doc_bounds_kernel(const int32_t* __restrict__ pos, int32_t* __restrict__ start,
+                                  int32_t* __restrict__ end, int T, int S) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  const int i = t % S;
+  const int32_t* row = pos + (t - i);
+  int lo = i + 1, hi = S;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (mid - row[mid] > i) hi = mid;
+    else lo = mid + 1;
+  }
+  start[t] = min(max(i - row[i], 0), i);
+  end[t] = lo;  // in [i + 1, S]
 }
 
 // ------------------------------------------------------------------------------------------
@@ -872,13 +891,20 @@ void rope_table(float2* tab, int S, int dh, float theta, cudaStream_t s) {
   B200W_CUDA(cudaStreamSynchronize(s));  // h goes out of scope
 }
 void rope_apply(void* buf, int ld, const float2* tab, int T, int S, int nheads, int dh,
-                bool inverse, cudaStream_t s, int head_stride) {
+                bool inverse, cudaStream_t s, int head_stride, const int32_t* positions) {
   if (head_stride == 0) head_stride = dh;
   B200W_CHECK(dh % 16 == 0 && ld % 8 == 0 && head_stride % 8 == 0 && head_stride >= dh,
               "head_dim must be a multiple of 16");
   const long long total = static_cast<long long>(T) * nheads * (dh / 16);
   rope_apply_kernel<<<blocks_for(total, 256), 256, 0, s>>>(static_cast<bf16*>(buf), ld, tab, T, S,
-                                                           nheads, dh, head_stride, inverse ? -1.f : 1.f);
+                                                           nheads, dh, head_stride, inverse ? -1.f : 1.f,
+                                                           positions);
+  B200W_CUDA(cudaGetLastError());
+}
+
+void doc_bounds(const int32_t* pos, int32_t* start, int32_t* end, int T, int S, cudaStream_t s) {
+  B200W_CHECK(S > 0 && T % S == 0, "T must be a multiple of S");
+  doc_bounds_kernel<<<blocks_for(T, 256), 256, 0, s>>>(pos, start, end, T, S);
   B200W_CUDA(cudaGetLastError());
 }
 

@@ -55,16 +55,26 @@ void gemm_decode_ex(const void* X, int ldx, const void* W, int ldw, const GemmDe
                     unsigned* counters, int M, int N, int K, cudaStream_t s);
 
 // ---- attention.cu --------------------------------------------------------------------------
+// Per-document attention inside packed rows (HF position_ids that restart at 0 for each document):
+// pos [T] the positions, start [T] = the sequence-local index of the token's document's first token
+// (t % S - pos[t]), end [T] = one past its last one. Query q sees key k iff start[q] <= k <= q.
+struct DocBounds {
+  const int32_t* pos;
+  const int32_t* start;
+  const int32_t* end;
+};
 // Causal self-attention over packed sequences. qkv: [T, ld_qkv] with q at column 0, k at
 // column k_off, v at column v_off (head h at +h*128); T = B*S; head_dim fixed at 128.
 // out: [T, ld_out] (head h at column h*128); lse2: [H, T] fp32 (log2-domain logsumexp).
+// docs (nullable): attend within each document only (DocBounds).
 void attention_fwd(const void* qkv, int ld_qkv, int k_off, int v_off, void* out, int ld_out,
-                   float* lse2, int B, int S, int H, int Hkv, float scale, cudaStream_t s);
+                   float* lse2, int B, int S, int H, int Hkv, float scale, cudaStream_t s,
+                   const DocBounds* docs = nullptr);
 // dqkv [T, ld_qkv] receives dq (column 0), dk (k_off), dv (v_off) in bf16; three launches
 // (delta, dK/dV, dQ), no global atomics. delta: [H, T] fp32 scratch.
 void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void* out,
                    const void* dout, int ld_out, const float* lse2, float* delta, void* dqkv, int B,
-                   int S, int H, int Hkv, float scale, cudaStream_t s);
+                   int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs = nullptr);
 
 // ---- ops.cu --------------------------------------------------------------------------------
 // out[t] = table[ids[t]] (+ pos_table[t % S + pos_offset] when pos_table != nullptr: OPT's learned
@@ -87,10 +97,15 @@ void rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd
 // cos/sin table for rotate_half RoPE: tab[pos*(dh/2) + i] = {cos, sin}(pos * theta^(-2i/dh))
 void rope_table(float2* tab, int S, int dh, float theta, cudaStream_t s);
 // in-place rotation of `nheads` consecutive heads starting at column 0 of buf [T, ld];
-// position = t % S. inverse=true applies the transpose (backward pass).
+// position = positions[t] (int32 [T], each < S) or, when positions == nullptr, t % S. inverse=true applies the
+// transpose (backward pass).
 // head_stride: distance between heads in elements (0 = dh; > dh when 64-wide heads are stored padded).
 void rope_apply(void* buf, int ld, const float2* tab, int T, int S, int nheads, int dh,
-                bool inverse, cudaStream_t s, int head_stride = 0);
+                bool inverse, cudaStream_t s, int head_stride = 0, const int32_t* positions = nullptr);
+// start / end of DocBounds from positions [T] (rows of S). The one place the bounds are derived. Positions that
+// break the layout (a row starting at 0, each entry 0 or the previous + 1) are the caller's to reject; the
+// bounds are clamped so that the attention loops stay in range whatever they hold.
+void doc_bounds(const int32_t* pos, int32_t* start, int32_t* end, int T, int S, cudaStream_t s);
 
 // gu: [T, 2f] (gate | up); h: [T, f] = silu(gate) * up
 void swiglu_fwd(const void* gu, void* h, int T, int f, cudaStream_t s);

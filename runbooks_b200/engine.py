@@ -361,14 +361,23 @@ class Engine:
         self._check(self._lib.b200w_comm_init(self._h, rank, nranks, buf))
 
     # -- the hot path -------------------------------------------------------------------------
-    def train_step(self, ids, labels, lr: float = 5e-5) -> Tuple[float, float]:
+    def train_step(self, ids, labels, lr: float = 5e-5, positions=None) -> Tuple[float, float]:
         """ids/labels: [n_seqs, seq_len] host integer arrays (labels unshifted, -100 ignored).
+        positions (optional, same shape): HF position_ids of packed documents (contract.pack_documents); each
+        document then attends only to itself (b200w_train_step_docs).
         Runs fwd + loss + bwd + all-reduce + clip + AdamW; returns (loss, grad_norm)."""
         ids, labels = _as_i32(ids), _as_i32(labels)
         assert ids.shape == labels.shape and ids.shape[1] == self.arch.max_seq_len
         loss, gn = C.c_float(), C.c_float()
-        self._check(self._lib.b200w_train_step(self._h, ids.ctypes.data, labels.ctypes.data,
-                                               ids.shape[0], lr, C.byref(loss), C.byref(gn)))
+        if positions is None:
+            self._check(self._lib.b200w_train_step(self._h, ids.ctypes.data, labels.ctypes.data,
+                                                   ids.shape[0], lr, C.byref(loss), C.byref(gn)))
+        else:
+            pos = _as_i32(positions)
+            assert pos.shape == ids.shape
+            self._check(self._lib.b200w_train_step_docs(self._h, ids.ctypes.data, labels.ctypes.data,
+                                                        pos.ctypes.data, ids.shape[0], lr, C.byref(loss),
+                                                        C.byref(gn)))
         return loss.value, gn.value
 
     def train_step_resident(self, ids_dev_ptr: int, labels_dev_ptr: int, n_seqs: int, n_valid: int,
@@ -398,14 +407,20 @@ class Engine:
         self._check(self._lib.b200w_profile_read(self._h, C.byref(ms), C.byref(fl), C.byref(n)))
         return ms.value, fl.value, n.value
 
-    def forward_backward(self, ids, labels) -> float:
+    def forward_backward(self, ids, labels, positions=None) -> float:
         ids, labels = _as_i32(ids), _as_i32(labels)
         loss = C.c_float()
-        self._check(self._lib.b200w_forward_backward(self._h, ids.ctypes.data, labels.ctypes.data,
-                                                     ids.shape[0], C.byref(loss)))
+        if positions is None:
+            self._check(self._lib.b200w_forward_backward(self._h, ids.ctypes.data, labels.ctypes.data,
+                                                         ids.shape[0], C.byref(loss)))
+        else:
+            pos = _as_i32(positions)
+            assert pos.shape == ids.shape
+            self._check(self._lib.b200w_forward_backward_docs(self._h, ids.ctypes.data, labels.ctypes.data,
+                                                              pos.ctypes.data, ids.shape[0], C.byref(loss)))
         return loss.value
 
-    def forward(self, ids, labels=None, want_logits: bool = True):
+    def forward(self, ids, labels=None, want_logits: bool = True, positions=None):
         """Returns (logits [T,V] float32 or None, nll [T] or None, loss or None)."""
         ids = _as_i32(ids)
         T = ids.size
@@ -413,10 +428,17 @@ class Engine:
         lab = _as_i32(labels) if labels is not None else None
         nll = np.empty(T, dtype=np.float32) if lab is not None else None
         loss = C.c_float()
-        self._check(self._lib.b200w_forward(
-            self._h, ids.ctypes.data, lab.ctypes.data if lab is not None else None, ids.shape[0],
-            logits.ctypes.data if want_logits else None, nll.ctypes.data if nll is not None else None,
-            C.byref(loss)))
+        outs = (logits.ctypes.data if want_logits else None, nll.ctypes.data if nll is not None else None,
+                C.byref(loss))
+        if positions is None:
+            self._check(self._lib.b200w_forward(
+                self._h, ids.ctypes.data, lab.ctypes.data if lab is not None else None, ids.shape[0], *outs))
+        else:
+            pos = _as_i32(positions)
+            assert pos.shape == ids.shape
+            self._check(self._lib.b200w_forward_docs(
+                self._h, ids.ctypes.data, lab.ctypes.data if lab is not None else None, pos.ctypes.data,
+                ids.shape[0], *outs))
         return logits, nll, (loss.value if lab is not None else None)
 
     def launch_count(self) -> int:

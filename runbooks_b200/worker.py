@@ -46,10 +46,21 @@ def visible_gpus() -> int:
     return max(1, len(glob.glob("/dev/nvidia[0-9]*")))
 
 
-def build_dataset(params: TrainParams, model_dir: str, data_dir: str, seq_len: int):
+def _records(params: TrainParams, model_dir: str, data_dir: str):
     tok = contract.Tokenizer(model_dir)
     docs = (tok.encode(contract.render(r, params.prompt_template)) for r in contract.iter_records(data_dir))
+    return docs, tok
+
+
+def build_dataset(params: TrainParams, model_dir: str, data_dir: str, seq_len: int):
+    docs, tok = _records(params, model_dir, data_dir)
     return contract.pack_sequences(docs, seq_len, tok.bos_id, tok.eos_id)
+
+
+def build_documents(params: TrainParams, model_dir: str, data_dir: str, seq_len: int):
+    """padding_free: (ids, labels, positions) of contract.pack_documents."""
+    docs, tok = _records(params, model_dir, data_dir)
+    return contract.pack_documents(docs, seq_len, tok.bos_id, tok.eos_id)
 
 
 def plan_steps(n_seqs: int, params: TrainParams, world: int):
@@ -60,7 +71,7 @@ def plan_steps(n_seqs: int, params: TrainParams, world: int):
 
 
 def train_rank(rank: int, world: int, uid: bytes, content: str) -> None:
-    from .engine import Engine, arch_from_hf_config
+    from .engine import Engine, LlamaArch, arch_from_hf_config
 
     model_dir, data_dir = os.path.join(content, "model"), os.path.join(content, "data")
     out_dir = os.path.join(content, "artifacts")
@@ -71,6 +82,9 @@ def train_rank(rank: int, world: int, uid: bytes, content: str) -> None:
     if seq_len % 128:
         raise ValueError(f"max_seq_length {seq_len} must be a multiple of 128")
     arch = arch_from_hf_config(hf_cfg, seq_len)   # llama | opt; unimplemented variants raise
+    padding_free = contract.wants_padding_free(params)
+    if padding_free and not isinstance(arch, LlamaArch):
+        raise ValueError(f"padding_free is implemented for the Llama family only, not {hf_cfg.get('model_type')!r}")
 
     t0 = time.time()
     eng = Engine(rank)
@@ -99,11 +113,16 @@ def train_rank(rank: int, world: int, uid: bytes, content: str) -> None:
     if world > 1:
         eng.comm_init(rank, world, uid)
 
-    ids, labels = build_dataset(params, model_dir, data_dir, seq_len)
+    if padding_free:
+        ids, labels, positions = build_documents(params, model_dir, data_dir, seq_len)
+    else:
+        (ids, labels), positions = build_dataset(params, model_dir, data_dir, seq_len), None
     per_step, steps_per_epoch, total_steps = plan_steps(len(ids), params, world)
     if len(ids) < per_step:  # tiny datasets: repeat rows so that one full step exists
         reps = (per_step + len(ids) - 1) // len(ids)
         ids, labels = np.tile(ids, (reps, 1)), np.tile(labels, (reps, 1))
+        if positions is not None:
+            positions = np.tile(positions, (reps, 1))
     per_rank = per_step // world
     warmup = contract.warmup_steps_for(total_steps, params.warmup_steps)
     if rank == 0:
@@ -112,7 +131,8 @@ def train_rank(rank: int, world: int, uid: bytes, content: str) -> None:
             checkpoint_read_gb_per_s=round(load_bytes / 1e9 / max(load_seconds, 1e-9), 3),
             sequences=int(len(ids)), seq_len=seq_len, world_size=world, total_steps=total_steps,
             global_batch=per_step, load_seconds=round(time.time() - t0, 2), device_gb=round(eng.device_bytes() / 1e9, 2),
-            warmup_steps=warmup, ignored_params=sorted(params.extra))
+            warmup_steps=warmup, ignored_params=sorted(params.extra), padding_free=padding_free,
+            documents=int((positions == 0).sum()) if positions is not None else None)
 
     rng = np.random.default_rng(params.seed)
     order: List[int] = []
@@ -124,7 +144,10 @@ def train_rank(rank: int, world: int, uid: bytes, content: str) -> None:
         batch, order = order[:per_step], order[per_step:]
         mine = batch[rank::world]                           # SURVEY.md §8e: rank r takes sequences [r::N]
         lr = contract.linear_lr(step, total_steps, params.learning_rate, warmup)
-        loss, gnorm = eng.train_step(ids[mine], labels[mine], lr=lr)
+        if positions is None:
+            loss, gnorm = eng.train_step(ids[mine], labels[mine], lr=lr)
+        else:
+            loss, gnorm = eng.train_step(ids[mine], labels[mine], lr=lr, positions=positions[mine])
         step += 1
         if rank == 0 and step % max(1, params.logging_steps) == 0:
             now = time.time()
