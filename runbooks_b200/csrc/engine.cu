@@ -287,6 +287,10 @@ namespace {
 bool is_opt(const b200w_arch& a) { return a.family == B200W_FAMILY_OPT; }
 bool is_falcon(const b200w_arch& a) { return a.family == B200W_FAMILY_FALCON; }
 bool has_layernorm(const b200w_arch& a) { return is_opt(a) || is_falcon(a); }
+// Llama's gate and up projections form one [2 f, d] matrix; OPT's fc1 and Falcon's dense_h_to_4h are [f, d]
+bool gated_mlp(const b200w_arch& a) { return !is_opt(a) && !is_falcon(a); }
+// the lm_head is the embedding matrix (OPT, Falcon)
+bool tied_head(const b200w_ctx* c) { return c->p_lm == c->p_embed; }
 int qd_of(const b200w_ctx* c) { return c->arch.num_heads * c->dhp; }
 int kd_of(const b200w_ctx* c) { return c->arch.num_kv_heads * c->dhp; }
 int qkv_dim(const b200w_ctx* c) { return qd_of(c) + 2 * kd_of(c); }
@@ -558,147 +562,113 @@ void egemm(b200w_ctx* c, const void* A, bool a_mn, int lda, const void* B, bool 
   }
 }
 
-// ---- forward of one micro-batch (ids already on device): Llama family ------------------------
-// One Llama decoder layer: x's buffers receive the activations the backward needs, h_next the layer's output
+// ---- forward of one micro-batch (ids already on device) ------------------------------------------
+// The shapes of a micro-batch of nseq sequences. qd / kd / qkvd are over the device's head width dhp; dh is the
+// model's head_dim, which sets the attention scale and the RoPE width.
+struct Dims {
+  int nseq, S, T, d, f, H, Hkv, dh, qd, kd, qkvd, V;
+  float scale, eps;
+  Dims(const b200w_ctx* c, int n_seqs)
+      : nseq(n_seqs), S(c->arch.max_seq_len), T(nseq * S), d(c->arch.hidden_size), f(c->arch.intermediate_size),
+        H(c->arch.num_heads), Hkv(c->arch.num_kv_heads), dh(c->arch.head_dim), qd(qd_of(c)), kd(kd_of(c)),
+        qkvd(qkv_dim(c)), V(c->arch.vocab_size), scale(1.f / sqrtf(static_cast<float>(dh))),
+        eps(c->arch.rms_norm_eps) {}
+};
+
+// One Llama decoder layer: c->la[l] receives the activations the backward needs, h_next the layer's output
 // (nullptr in the recompute pass of the backward, which stops before the down projection).
 // docs (nullable): RoPE at the documents' positions and attention within each document.
-void forward_layer_llama(b200w_ctx* c, int l, const bf16* h_in, bf16* h_next, b200w_ctx::LayerA& x, int nseq,
-                         const DocBounds* docs) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
-  const int qd = H * dh, kd = Hkv * dh, qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(dh));
+void forward_layer_llama(b200w_ctx* c, const Dims& m, int l, const bf16* h_in, bf16* h_next, const DocBounds* docs) {
   cudaStream_t s = c->stream;
   int64_t& n = c->launches;
+  auto& x = c->la[l];
   const auto& p = c->lp[l];
-  rmsnorm_fwd(h_in, c->w + p.ln1, x.n1, x.rstd1, T, d, a.rms_norm_eps, s); ++n;
-  egemm(c, x.n1, false, d, c->w + p.wqkv, false, d, x.qkv, nullptr, false, qkvd, T, qkvd, d);
-  rope_apply(x.qkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, false, s, 0, docs ? docs->pos : nullptr); ++n;
-  attention_fwd(x.qkv, qkvd, qd, qd + kd, x.attn, qd, x.lse, nseq, S, H, Hkv, scale, s, docs); ++n;
-  egemm(c, x.attn, false, qd, c->w + p.wo, false, qd, x.h_mid, h_in, false, d, T, d, qd);
-  rmsnorm_fwd(x.h_mid, c->w + p.ln2, x.n2, x.rstd2, T, d, a.rms_norm_eps, s); ++n;
-  egemm(c, x.n2, false, d, c->w + p.wgu, false, d, x.gu, nullptr, false, 2 * f, T, 2 * f, d);
-  swiglu_fwd(x.gu, x.act, T, f, s); ++n;
-  if (h_next) egemm(c, x.act, false, f, c->w + p.wd, false, f, h_next, x.h_mid, false, d, T, d, f);
+  rmsnorm_fwd(h_in, c->w + p.ln1, x.n1, x.rstd1, m.T, m.d, m.eps, s); ++n;
+  egemm(c, x.n1, false, m.d, c->w + p.wqkv, false, m.d, x.qkv, nullptr, false, m.qkvd, m.T, m.qkvd, m.d);
+  rope_apply(x.qkv, m.qkvd, c->rope_tab, m.T, m.S, m.H + m.Hkv, m.dh, false, s, 0, docs ? docs->pos : nullptr); ++n;
+  attention_fwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, m.qd, x.lse, m.nseq, m.S, m.H, m.Hkv, m.scale, s, docs); ++n;
+  egemm(c, x.attn, false, m.qd, c->w + p.wo, false, m.qd, x.h_mid, h_in, false, m.d, m.T, m.d, m.qd);
+  rmsnorm_fwd(x.h_mid, c->w + p.ln2, x.n2, x.rstd2, m.T, m.d, m.eps, s); ++n;
+  egemm(c, x.n2, false, m.d, c->w + p.wgu, false, m.d, x.gu, nullptr, false, 2 * m.f, m.T, 2 * m.f, m.d);
+  swiglu_fwd(x.gu, x.act, m.T, m.f, s); ++n;
+  if (h_next) egemm(c, x.act, false, m.f, c->w + p.wd, false, m.f, h_next, x.h_mid, false, m.d, m.T, m.d, m.f);
 }
 
-void forward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, const DocBounds* docs) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size;
-  cudaStream_t s = c->stream;
-  int64_t& n = c->launches;
-  const int L = a.num_layers;
-
-  bf16* h = c->la[0].h_in;
-  embed_fwd(ids, c->w + c->p_embed, nullptr, h, T, d, a.vocab_size, S, 0, s); ++n;
-  for (int l = 0; l < L; ++l) {
-    auto& x = c->la[l];
-    bf16* h_in = c->training ? x.h_in : h;
-    bf16* h_next = c->training ? (l + 1 < L ? c->la[l + 1].h_in : c->h_final)
-                               : (h == c->la[0].h_in ? c->h_final : c->la[0].h_in);
-    forward_layer_llama(c, l, h_in, h_next, x, nseq, docs);
-    h = h_next;
-  }
-  // in training mode h == h_final; in forward-only mode h is whichever buffer came last
-  rmsnorm_fwd(h, c->w + c->p_norm, c->nf, c->rstdf, T, d, a.rms_norm_eps, s); ++n;
-  egemm(c, c->nf, false, d, c->w + c->p_lm, false, d, c->logits, nullptr, false, a.vocab_size, T,
-            a.vocab_size, d);
-  if (c->training && h != c->h_final) throw Error("internal: residual stream bookkeeping");
-}
-
-// ---- OPT family (HF models/opt/modeling_opt.py OPTDecoder / OPTDecoderLayer, pre-LN) -----------
+// OPT decoder layer (HF models/opt/modeling_opt.py OPTDecoderLayer, pre-LN).
 // q is scaled by head_dim^-0.5 inside the attention kernel (HF scales q after q_proj and calls the
 // attention with scaling 1.0: the same product, and the factor 1/8 is exact in bf16).
-void forward_micro_opt(b200w_ctx* c, const int32_t* ids, int nseq) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads;
-  const int qd = qd_of(c), kd = kd_of(c), qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(a.head_dim));
-  const float eps = a.rms_norm_eps;
+void forward_layer_opt(b200w_ctx* c, const Dims& m, int l, const bf16* h_in, bf16* h_next) {
   cudaStream_t s = c->stream;
   int64_t& n = c->launches;
-  const int L = a.num_layers;
-
-  bf16* h = c->la[0].h_in;
-  embed_fwd(ids, c->w + c->p_embed, c->w + c->p_pos, h, T, d, a.vocab_size, S, OPT_POS_OFFSET, s); ++n;
-  for (int l = 0; l < L; ++l) {
-    auto& x = c->la[l];
-    const auto& p = c->lp[l];
-    bf16* h_in = c->training ? x.h_in : h;
-    bf16* h_next = c->training ? (l + 1 < L ? c->la[l + 1].h_in : c->h_final)
-                               : (h == c->la[0].h_in ? c->h_final : c->la[0].h_in);
-    layernorm_fwd(h_in, c->w + p.ln1, c->w + p.ln1b, x.n1, x.mean1, x.rstd1, T, d, eps, s); ++n;
-    // nn.Linear(bias=True): the bias (and fc1's ReLU) ride in the GEMM epilogue, added in fp32 before the one
-    // rounding to bf16
-    egemm(c, x.n1, false, d, c->w + p.wqkv, false, d, x.qkv, nullptr, false, qkvd, T, qkvd, d, c->w + p.bqkv, 0);
-    attention_fwd(x.qkv, qkvd, qd, qd + kd, x.attn, qd, x.lse, nseq, S, H, Hkv, scale, s); ++n;
-    egemm(c, x.attn, false, qd, c->w + p.wo, false, qd, x.h_mid, h_in, false, d, T, d, qd, c->w + p.bo, 0);
-    layernorm_fwd(x.h_mid, c->w + p.ln2, c->w + p.ln2b, x.n2, x.mean2, x.rstd2, T, d, eps, s); ++n;
-    egemm(c, x.n2, false, d, c->w + p.wgu, false, d, x.act, nullptr, false, f, T, f, d, c->w + p.b1, 1);  // ReLU
-    egemm(c, x.act, false, f, c->w + p.wd, false, f, h_next, x.h_mid, false, d, T, d, f, c->w + p.b2, 0);
-    h = h_next;
-  }
-  layernorm_fwd(h, c->w + c->p_norm, c->w + c->p_normb, c->nf, c->meanf, c->rstdf, T, d, eps, s); ++n;
-  egemm(c, c->nf, false, d, c->w + c->p_lm, false, d, c->logits, nullptr, false, a.vocab_size, T,
-        a.vocab_size, d);
-  if (c->training && h != c->h_final) throw Error("internal: residual stream bookkeeping");
+  auto& x = c->la[l];
+  const auto& p = c->lp[l];
+  layernorm_fwd(h_in, c->w + p.ln1, c->w + p.ln1b, x.n1, x.mean1, x.rstd1, m.T, m.d, m.eps, s); ++n;
+  // nn.Linear(bias=True): the bias (and fc1's ReLU) ride in the GEMM epilogue, added in fp32 before the one
+  // rounding to bf16
+  egemm(c, x.n1, false, m.d, c->w + p.wqkv, false, m.d, x.qkv, nullptr, false, m.qkvd, m.T, m.qkvd, m.d,
+        c->w + p.bqkv, 0);
+  attention_fwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, m.qd, x.lse, m.nseq, m.S, m.H, m.Hkv, m.scale, s); ++n;
+  egemm(c, x.attn, false, m.qd, c->w + p.wo, false, m.qd, x.h_mid, h_in, false, m.d, m.T, m.d, m.qd, c->w + p.bo, 0);
+  layernorm_fwd(x.h_mid, c->w + p.ln2, c->w + p.ln2b, x.n2, x.mean2, x.rstd2, m.T, m.d, m.eps, s); ++n;
+  egemm(c, x.n2, false, m.d, c->w + p.wgu, false, m.d, x.act, nullptr, false, m.f, m.T, m.f, m.d, c->w + p.b1, 1);  // ReLU
+  egemm(c, x.act, false, m.f, c->w + p.wd, false, m.f, h_next, x.h_mid, false, m.d, m.T, m.d, m.f, c->w + p.b2, 0);
 }
 
-// ---- Falcon family (HF models/falcon/modeling_falcon.py FalconDecoderLayer.forward :580-650 with
+// Falcon decoder layer (HF models/falcon/modeling_falcon.py FalconDecoderLayer.forward :580-650 with
 // parallel_attn and one input_layernorm): ln = LN(h); h' = h + dense(attn(ln)) + 4h_to_h(gelu(h_to_4h(ln))).
 // Multi-query attention: H query heads share one key/value head (the GQA path with Hkv = 1).
-void forward_micro_falcon(b200w_ctx* c, const int32_t* ids, int nseq) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads;
-  const int qd = qd_of(c), kd = kd_of(c), qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(a.head_dim));
-  const float eps = a.rms_norm_eps;
+void forward_layer_falcon(b200w_ctx* c, const Dims& m, int l, const bf16* h_in, bf16* h_next) {
   cudaStream_t s = c->stream;
   int64_t& n = c->launches;
-  const int L = a.num_layers;
-
-  bf16* h = c->la[0].h_in;
-  embed_fwd(ids, c->w + c->p_embed, nullptr, h, T, d, a.vocab_size, S, 0, s); ++n;
-  for (int l = 0; l < L; ++l) {
-    auto& x = c->la[l];
-    const auto& p = c->lp[l];
-    bf16* h_in = c->training ? x.h_in : h;
-    bf16* h_next = c->training ? (l + 1 < L ? c->la[l + 1].h_in : c->h_final)
-                               : (h == c->la[0].h_in ? c->h_final : c->la[0].h_in);
-    layernorm_fwd(h_in, c->w + p.ln1, c->w + p.ln1b, x.n1, x.mean1, x.rstd1, T, d, eps, s); ++n;
-    egemm(c, x.n1, false, d, c->w + p.wqkv, false, d, x.qkv, nullptr, false, qkvd, T, qkvd, d);
-    rope_apply(x.qkv, qkvd, c->rope_tab, T, S, H + Hkv, a.head_dim, false, s, c->dhp); ++n;
-    attention_fwd(x.qkv, qkvd, qd, qd + kd, x.attn, qd, x.lse, nseq, S, H, Hkv, scale, s); ++n;
-    egemm(c, x.attn, false, qd, c->w + p.wo, false, qd, x.h_mid, h_in, false, d, T, d, qd);
-    egemm(c, x.n1, false, d, c->w + p.wgu, false, d, x.gu, nullptr, false, f, T, f, d);
-    gelu_fwd(x.gu, x.act, static_cast<size_t>(T) * f, s); ++n;
-    egemm(c, x.act, false, f, c->w + p.wd, false, f, h_next, x.h_mid, false, d, T, d, f);
-    h = h_next;
-  }
-  layernorm_fwd(h, c->w + c->p_norm, c->w + c->p_normb, c->nf, c->meanf, c->rstdf, T, d, eps, s); ++n;
-  egemm(c, c->nf, false, d, c->w + c->p_lm, false, d, c->logits, nullptr, false, a.vocab_size, T,
-        a.vocab_size, d);
-  if (c->training && h != c->h_final) throw Error("internal: residual stream bookkeeping");
+  auto& x = c->la[l];
+  const auto& p = c->lp[l];
+  layernorm_fwd(h_in, c->w + p.ln1, c->w + p.ln1b, x.n1, x.mean1, x.rstd1, m.T, m.d, m.eps, s); ++n;
+  egemm(c, x.n1, false, m.d, c->w + p.wqkv, false, m.d, x.qkv, nullptr, false, m.qkvd, m.T, m.qkvd, m.d);
+  rope_apply(x.qkv, m.qkvd, c->rope_tab, m.T, m.S, m.H + m.Hkv, m.dh, false, s, c->dhp); ++n;
+  attention_fwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, m.qd, x.lse, m.nseq, m.S, m.H, m.Hkv, m.scale, s); ++n;
+  egemm(c, x.attn, false, m.qd, c->w + p.wo, false, m.qd, x.h_mid, h_in, false, m.d, m.T, m.d, m.qd);
+  egemm(c, x.n1, false, m.d, c->w + p.wgu, false, m.d, x.gu, nullptr, false, m.f, m.T, m.f, m.d);
+  gelu_fwd(x.gu, x.act, static_cast<size_t>(m.T) * m.f, s); ++n;
+  egemm(c, x.act, false, m.f, c->w + p.wd, false, m.f, h_next, x.h_mid, false, m.d, m.T, m.d, m.f);
 }
 
 // docs: Llama family only (check_docs_family refuses the others before any GPU work)
 void forward_micro(b200w_ctx* c, const int32_t* ids, int nseq, const DocBounds* docs = nullptr) {
-  if (is_opt(c->arch)) forward_micro_opt(c, ids, nseq);
-  else if (is_falcon(c->arch)) forward_micro_falcon(c, ids, nseq);
-  else forward_micro_llama(c, ids, nseq, docs);
+  const Dims m(c, nseq);
+  const bool opt = is_opt(c->arch), falcon = is_falcon(c->arch);
+  cudaStream_t s = c->stream;
+  int64_t& n = c->launches;
+  const int L = c->arch.num_layers;
+
+  bf16* h = c->la[0].h_in;
+  embed_fwd(ids, c->w + c->p_embed, opt ? c->w + c->p_pos : nullptr, h, m.T, m.d, m.V, m.S,
+            opt ? OPT_POS_OFFSET : 0, s); ++n;
+  for (int l = 0; l < L; ++l) {
+    bf16* h_in = c->training ? c->la[l].h_in : h;
+    bf16* h_next = c->training ? (l + 1 < L ? c->la[l + 1].h_in : c->h_final)
+                               : (h == c->la[0].h_in ? c->h_final : c->la[0].h_in);
+    if (opt) forward_layer_opt(c, m, l, h_in, h_next);
+    else if (falcon) forward_layer_falcon(c, m, l, h_in, h_next);
+    else forward_layer_llama(c, m, l, h_in, h_next, docs);
+    h = h_next;
+  }
+  // in training mode h == h_final; in forward-only mode h is whichever buffer came last
+  if (has_layernorm(c->arch))
+    layernorm_fwd(h, c->w + c->p_norm, c->w + c->p_normb, c->nf, c->meanf, c->rstdf, m.T, m.d, m.eps, s);
+  else
+    rmsnorm_fwd(h, c->w + c->p_norm, c->nf, c->rstdf, m.T, m.d, m.eps, s);
+  ++n;
+  egemm(c, c->nf, false, m.d, c->w + c->p_lm, false, m.d, c->logits, nullptr, false, m.V, m.T, m.V, m.d);
+  if (c->training && h != c->h_final) throw Error("internal: residual stream bookkeeping");
 }
 
 // loss + dlogits (in place); the normaliser 1 / num_items_in_batch is the device scalar c->inv_n
 void loss_micro(b200w_ctx* c, const int32_t* labels, int nseq) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S;
+  const Dims m(c, nseq);
   cudaStream_t s = c->stream;
-  ce_shift_targets(labels, c->targets, T, S, s); ++c->launches;
-  ce_loss_fwd_bwd(c->logits, c->targets, c->nll, T, a.vocab_size, c->inv_n, s); ++c->launches;
-  reduce_sum_f32(c->nll, c->scal + 0, T, c->inv_n, s); ++c->launches;
+  ce_shift_targets(labels, c->targets, m.T, m.S, s); ++c->launches;
+  ce_loss_fwd_bwd(c->logits, c->targets, c->nll, m.T, m.V, c->inv_n, s); ++c->launches;
+  reduce_sum_f32(c->nll, c->scal + 0, m.T, c->inv_n, s); ++c->launches;
 }
 
 // B200W_AR_MODE (debugging aid, same arithmetic in every mode):
@@ -760,192 +730,157 @@ void allreduce_range(b200w_ctx* c, size_t off, size_t count, bool precast = fals
   if (!any) throw Error("internal: gradient exchange request does not match the exchange ranges");
 }
 
+// Where one micro-step's weight gradients go. first: the micro-step overwrites the gradients instead of
+// accumulating them. overlap_ar: each range's gradient exchange starts as soon as the range is final.
+struct GradOut {
+  b200w_ctx* c;
+  int T;
+  bool first, overlap_ar;
+  // dW [M, N] (+)= dy[T, M]^T x[T, N] into the gradient at off, then the exchange of that matrix; the GEMM epilogue
+  // writes its bf16 wire copy itself
+  void wgrad(size_t off, const void* dy, int M, const void* x, int N) const {
+    egemm(c, dy, true, M, x, true, N, c->g + off, first ? nullptr : c->g + off, true, N, M, N, T, nullptr, 0,
+          overlap_ar ? c->gw + off : nullptr);
+    if (overlap_ar) allreduce_range(c, off, static_cast<size_t>(M) * N, true);
+  }
+  void exchange(size_t off, size_t count) const {
+    if (overlap_ar) allreduce_range(c, off, count);
+  }
+};
+
+// The backward of one decoder layer takes the gradient of its output in dh_cur and leaves the gradient of its
+// input there; dh_alt is the other buffer of the pair.
+void backward_layer_llama(b200w_ctx* c, const Dims& m, const GradOut& go, int l, bf16*& dh_cur, bf16*& dh_alt,
+                          const DocBounds* docs) {
+  cudaStream_t s = c->stream;
+  int64_t& n = c->launches;
+  float* g = c->g;
+  auto& x = c->la[l];
+  const auto& p = c->lp[l];
+  // activation recomputation: the layer's forward again, from its saved input into the shared buffers (the same
+  // kernels on the same operands: bit-identical activations, hence bit-identical gradients)
+  if (c->recompute) forward_layer_llama(c, m, l, x.h_in, nullptr, docs);
+  // h_next = h_mid + act Wd^T
+  egemm(c, dh_cur, false, m.d, c->w + p.wd, true, m.f, c->dact, nullptr, false, m.f, m.T, m.f, m.d);
+  go.wgrad(p.wd, dh_cur, m.d, x.act, m.f);
+  swiglu_bwd(c->dact, x.gu, c->dgu, m.T, m.f, s); ++n;
+  egemm(c, c->dgu, false, 2 * m.f, c->w + p.wgu, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, 2 * m.f);
+  go.wgrad(p.wgu, c->dgu, 2 * m.f, x.n2, m.d);
+  // dh_mid = dh + rmsnorm_bwd(dn2)
+  rmsnorm_bwd(c->dn, x.h_mid, c->w + p.ln2, x.rstd2, dh_cur, dh_alt, g + p.ln2, c->dw_partial, m.T, m.d, s); n += 2;
+  std::swap(dh_cur, dh_alt);
+  // h_mid = h_in + attn Wo^T
+  egemm(c, dh_cur, false, m.d, c->w + p.wo, true, m.qd, c->dattn, nullptr, false, m.qd, m.T, m.qd, m.d);
+  go.wgrad(p.wo, dh_cur, m.d, x.attn, m.qd);
+  attention_bwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, c->dattn, m.qd, x.lse, c->delta, c->dqkv, m.nseq, m.S,
+                m.H, m.Hkv, m.scale, s, docs); n += 3;
+  rope_apply(c->dqkv, m.qkvd, c->rope_tab, m.T, m.S, m.H + m.Hkv, m.dh, true, s, 0, docs ? docs->pos : nullptr); ++n;
+  egemm(c, c->dqkv, false, m.qkvd, c->w + p.wqkv, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.qkvd);
+  go.wgrad(p.wqkv, c->dqkv, m.qkvd, x.n1, m.d);
+  rmsnorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.rstd1, dh_cur, dh_alt, g + p.ln1, c->dw_partial, m.T, m.d, s); n += 2;
+  std::swap(dh_cur, dh_alt);
+}
+
+// OPT: bias gradients are column sums of the projection's output gradient.
+void backward_layer_opt(b200w_ctx* c, const Dims& m, const GradOut& go, int l, bf16*& dh_cur, bf16*& dh_alt) {
+  cudaStream_t s = c->stream;
+  int64_t& n = c->launches;
+  float* g = c->g;
+  float* part = c->dw_partial;
+  auto& x = c->la[l];
+  const auto& p = c->lp[l];
+  // h_next = h_mid + act W2^T + b2
+  colsum_add(dh_cur, g + p.b2, part, m.T, m.d, m.d, s); n += 2;
+  egemm(c, dh_cur, false, m.d, c->w + p.wd, true, m.f, c->dact, nullptr, false, m.f, m.T, m.f, m.d);
+  go.wgrad(p.wd, dh_cur, m.d, x.act, m.f);
+  // act = relu(n2 W1^T + b1)
+  relu_bwd(c->dact, x.act, c->dact, static_cast<size_t>(m.T) * m.f, s); ++n;
+  colsum_add(c->dact, g + p.b1, part, m.T, m.f, m.f, s); n += 2;
+  egemm(c, c->dact, false, m.f, c->w + p.wgu, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.f);
+  go.wgrad(p.wgu, c->dact, m.f, x.n2, m.d);
+  layernorm_bwd(c->dn, x.h_mid, c->w + p.ln2, x.mean2, x.rstd2, dh_cur, dh_alt, g + p.ln2, g + p.ln2b, part,
+                m.T, m.d, s); n += 3;
+  std::swap(dh_cur, dh_alt);
+  // h_mid = h_in + attn Wo^T + bo
+  colsum_add(dh_cur, g + p.bo, part, m.T, m.d, m.d, s); n += 2;
+  egemm(c, dh_cur, false, m.d, c->w + p.wo, true, m.qd, c->dattn, nullptr, false, m.qd, m.T, m.qd, m.d);
+  go.wgrad(p.wo, dh_cur, m.d, x.attn, m.qd);
+  attention_bwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, c->dattn, m.qd, x.lse, c->delta, c->dqkv, m.nseq, m.S,
+                m.H, m.Hkv, m.scale, s); n += 3;
+  colsum_add(c->dqkv, g + p.bqkv, part, m.T, m.qkvd, m.qkvd, s); n += 2;
+  egemm(c, c->dqkv, false, m.qkvd, c->w + p.wqkv, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.qkvd);
+  go.wgrad(p.wqkv, c->dqkv, m.qkvd, x.n1, m.d);
+  layernorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.mean1, x.rstd1, dh_cur, dh_alt, g + p.ln1, g + p.ln1b, part,
+                m.T, m.d, s); n += 3;
+  std::swap(dh_cur, dh_alt);
+}
+
+// Falcon: both branches read the same LayerNorm output, so its gradient is the sum of the MLP branch's (written
+// first) and the attention branch's (accumulated by the qkv dgrad GEMM's C operand).
+void backward_layer_falcon(b200w_ctx* c, const Dims& m, const GradOut& go, int l, bf16*& dh_cur, bf16*& dh_alt) {
+  cudaStream_t s = c->stream;
+  int64_t& n = c->launches;
+  float* g = c->g;
+  auto& x = c->la[l];
+  const auto& p = c->lp[l];
+  // MLP branch: h' += gelu(ln W1^T) W2^T
+  egemm(c, dh_cur, false, m.d, c->w + p.wd, true, m.f, c->dact, nullptr, false, m.f, m.T, m.f, m.d);
+  go.wgrad(p.wd, dh_cur, m.d, x.act, m.f);
+  gelu_bwd(c->dact, x.gu, c->dact, static_cast<size_t>(m.T) * m.f, s); ++n;
+  egemm(c, c->dact, false, m.f, c->w + p.wgu, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.f);
+  go.wgrad(p.wgu, c->dact, m.f, x.n1, m.d);
+  // attention branch: h' += attn Wo^T
+  egemm(c, dh_cur, false, m.d, c->w + p.wo, true, m.qd, c->dattn, nullptr, false, m.qd, m.T, m.qd, m.d);
+  go.wgrad(p.wo, dh_cur, m.d, x.attn, m.qd);
+  attention_bwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, c->dattn, m.qd, x.lse, c->delta, c->dqkv, m.nseq, m.S,
+                m.H, m.Hkv, m.scale, s); n += 3;
+  rope_apply(c->dqkv, m.qkvd, c->rope_tab, m.T, m.S, m.H + m.Hkv, m.dh, true, s, c->dhp); ++n;
+  egemm(c, c->dqkv, false, m.qkvd, c->w + p.wqkv, true, m.d, c->dn, c->dn, false, m.d, m.T, m.d, m.qkvd);
+  go.wgrad(p.wqkv, c->dqkv, m.qkvd, x.n1, m.d);
+  layernorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.mean1, x.rstd1, dh_cur, dh_alt, g + p.ln1, g + p.ln1b,
+                c->dw_partial, m.T, m.d, s); n += 3;
+  std::swap(dh_cur, dh_alt);
+}
+
 // backward of one micro-batch. first: overwrite gradients instead of accumulating.
 // overlap_ar: launch the all-reduce of each matrix as soon as its gradient is final.
-void backward_micro_llama(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar,
-                          const DocBounds* docs) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, V = a.vocab_size;
-  const int qd = H * dh, kd = Hkv * dh, qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(dh));
-  cudaStream_t s = c->stream;
-  int64_t& n = c->launches;
-  const int L = a.num_layers;
-  float* g = c->g;
-  auto acc = [&](size_t off) -> const void* { return first ? nullptr : g + off; };
-  auto ar = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count); };
-  // matrices whose exchange follows their wgrad at once: the GEMM epilogue writes the bf16 wire copy itself
-  auto wire = [&](size_t off) -> void* { return overlap_ar ? c->gw + off : nullptr; };
-  auto arw = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count, true); };
-
-  // lm_head: dnf = dlogits W ; dW += dlogits^T nf
-  egemm(c, c->logits, false, V, c->w + c->p_lm, true, d, c->dn, nullptr, false, d, T, d, V);
-  egemm(c, c->logits, true, V, c->nf, true, d, g + c->p_lm, acc(c->p_lm), true, d, V, d, T, nullptr, 0, wire(c->p_lm));
-  arw(c->p_lm, static_cast<size_t>(V) * d);
-  bf16* dh_cur = c->dh_a;
-  bf16* dh_alt = c->dh_b;
-  rmsnorm_bwd(c->dn, c->h_final, c->w + c->p_norm, c->rstdf, nullptr, dh_cur, g + c->p_norm, c->dw_partial, T, d, s); n += 2;
-
-  for (int l = L - 1; l >= 0; --l) {
-    auto& x = c->la[l];
-    const auto& p = c->lp[l];
-    const size_t o_q = p.wqkv, o_o = p.wo, o_gu = p.wgu, o_d = p.wd;
-    // activation recomputation: the layer's forward again, from its saved input into the shared buffers (the same
-    // kernels on the same operands: bit-identical activations, hence bit-identical gradients)
-    if (c->recompute) forward_layer_llama(c, l, x.h_in, nullptr, x, nseq, docs);
-    // h_next = h_mid + act Wd^T
-    egemm(c, dh_cur, false, d, c->w + o_d, true, f, c->dact, nullptr, false, f, T, f, d);
-    egemm(c, dh_cur, true, d, x.act, true, f, g + o_d, acc(o_d), true, f, d, f, T, nullptr, 0, wire(o_d));
-    arw(o_d, static_cast<size_t>(d) * f);
-    swiglu_bwd(c->dact, x.gu, c->dgu, T, f, s); ++n;
-    egemm(c, c->dgu, false, 2 * f, c->w + o_gu, true, d, c->dn, nullptr, false, d, T, d, 2 * f);
-    egemm(c, c->dgu, true, 2 * f, x.n2, true, d, g + o_gu, acc(o_gu), true, d, 2 * f, d, T, nullptr, 0, wire(o_gu));
-    arw(o_gu, static_cast<size_t>(2) * f * d);
-    // dh_mid = dh + rmsnorm_bwd(dn2)
-    rmsnorm_bwd(c->dn, x.h_mid, c->w + p.ln2, x.rstd2, dh_cur, dh_alt, g + p.ln2, c->dw_partial, T, d, s); n += 2;
-    std::swap(dh_cur, dh_alt);
-    // h_mid = h_in + attn Wo^T
-    egemm(c, dh_cur, false, d, c->w + o_o, true, qd, c->dattn, nullptr, false, qd, T, qd, d);
-    egemm(c, dh_cur, true, d, x.attn, true, qd, g + o_o, acc(o_o), true, qd, d, qd, T, nullptr, 0, wire(o_o));
-    arw(o_o, static_cast<size_t>(d) * qd);
-    attention_bwd(x.qkv, qkvd, qd, qd + kd, x.attn, c->dattn, qd, x.lse, c->delta, c->dqkv, nseq, S, H,
-                  Hkv, scale, s, docs); n += 3;
-    rope_apply(c->dqkv, qkvd, c->rope_tab, T, S, H + Hkv, dh, true, s, 0, docs ? docs->pos : nullptr); ++n;
-    egemm(c, c->dqkv, false, qkvd, c->w + o_q, true, d, c->dn, nullptr, false, d, T, d, qkvd);
-    egemm(c, c->dqkv, true, qkvd, x.n1, true, d, g + o_q, acc(o_q), true, d, qkvd, d, T, nullptr, 0, wire(o_q));
-    arw(o_q, static_cast<size_t>(qkvd) * d);
-    rmsnorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.rstd1, dh_cur, dh_alt, g + p.ln1, c->dw_partial, T, d, s); n += 2;
-    std::swap(dh_cur, dh_alt);
-  }
-  embed_bwd(ids, dh_cur, g + c->p_embed, nullptr, T, d, V, a.pad_token_id, S, 0, s); ++n;
-  ar(0, c->n_zero_prefix);
-}
-
-// OPT backward. Bias gradients are column sums of the projection's output gradient; the tied
-// lm_head accumulates into the embedding gradient (zeroed with the prefix at the start of a step,
-// so that wgrad always accumulates) before embed_bwd adds the lookup rows.
-void backward_micro_opt(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, V = a.vocab_size;
-  const int qd = qd_of(c), kd = kd_of(c), qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(a.head_dim));
-  cudaStream_t s = c->stream;
-  int64_t& n = c->launches;
-  const int L = a.num_layers;
-  float* g = c->g;
-  float* part = c->dw_partial;
-  auto acc = [&](size_t off) -> const void* { return first ? nullptr : g + off; };
-  auto ar = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count); };
-  // matrices whose exchange follows their wgrad at once: the GEMM epilogue writes the bf16 wire copy itself
-  auto wire = [&](size_t off) -> void* { return overlap_ar ? c->gw + off : nullptr; };
-  auto arw = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count, true); };
-
-  egemm(c, c->logits, false, V, c->w + c->p_lm, true, d, c->dn, nullptr, false, d, T, d, V);
-  egemm(c, c->logits, true, V, c->nf, true, d, g + c->p_embed, g + c->p_embed, true, d, V, d, T);
-  bf16* dh_cur = c->dh_a;
-  bf16* dh_alt = c->dh_b;
-  layernorm_bwd(c->dn, c->h_final, c->w + c->p_norm, c->meanf, c->rstdf, nullptr, dh_cur, g + c->p_norm,
-                g + c->p_normb, part, T, d, s); n += 3;
-  for (int l = L - 1; l >= 0; --l) {
-    auto& x = c->la[l];
-    const auto& p = c->lp[l];
-    // h_next = h_mid + act W2^T + b2
-    colsum_add(dh_cur, g + p.b2, part, T, d, d, s); n += 2;
-    egemm(c, dh_cur, false, d, c->w + p.wd, true, f, c->dact, nullptr, false, f, T, f, d);
-    egemm(c, dh_cur, true, d, x.act, true, f, g + p.wd, acc(p.wd), true, f, d, f, T, nullptr, 0, wire(p.wd));
-    arw(p.wd, static_cast<size_t>(d) * f);
-    // act = relu(n2 W1^T + b1)
-    relu_bwd(c->dact, x.act, c->dact, static_cast<size_t>(T) * f, s); ++n;
-    colsum_add(c->dact, g + p.b1, part, T, f, f, s); n += 2;
-    egemm(c, c->dact, false, f, c->w + p.wgu, true, d, c->dn, nullptr, false, d, T, d, f);
-    egemm(c, c->dact, true, f, x.n2, true, d, g + p.wgu, acc(p.wgu), true, d, f, d, T, nullptr, 0, wire(p.wgu));
-    arw(p.wgu, static_cast<size_t>(f) * d);
-    layernorm_bwd(c->dn, x.h_mid, c->w + p.ln2, x.mean2, x.rstd2, dh_cur, dh_alt, g + p.ln2, g + p.ln2b, part,
-                  T, d, s); n += 3;
-    std::swap(dh_cur, dh_alt);
-    // h_mid = h_in + attn Wo^T + bo
-    colsum_add(dh_cur, g + p.bo, part, T, d, d, s); n += 2;
-    egemm(c, dh_cur, false, d, c->w + p.wo, true, qd, c->dattn, nullptr, false, qd, T, qd, d);
-    egemm(c, dh_cur, true, d, x.attn, true, qd, g + p.wo, acc(p.wo), true, qd, d, qd, T, nullptr, 0, wire(p.wo));
-    arw(p.wo, static_cast<size_t>(d) * qd);
-    attention_bwd(x.qkv, qkvd, qd, qd + kd, x.attn, c->dattn, qd, x.lse, c->delta, c->dqkv, nseq, S, H,
-                  Hkv, scale, s); n += 3;
-    colsum_add(c->dqkv, g + p.bqkv, part, T, qkvd, qkvd, s); n += 2;
-    egemm(c, c->dqkv, false, qkvd, c->w + p.wqkv, true, d, c->dn, nullptr, false, d, T, d, qkvd);
-    egemm(c, c->dqkv, true, qkvd, x.n1, true, d, g + p.wqkv, acc(p.wqkv), true, d, qkvd, d, T, nullptr, 0, wire(p.wqkv));
-    arw(p.wqkv, static_cast<size_t>(qkvd) * d);
-    layernorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.mean1, x.rstd1, dh_cur, dh_alt, g + p.ln1, g + p.ln1b, part,
-                  T, d, s); n += 3;
-    std::swap(dh_cur, dh_alt);
-  }
-  embed_bwd(ids, dh_cur, g + c->p_embed, g + c->p_pos, T, d, V, a.pad_token_id, S, OPT_POS_OFFSET, s); ++n;
-  ar(0, c->n_zero_prefix);
-}
-
-// Falcon backward. Both branches read the same LayerNorm output, so its gradient is the sum of the MLP
-// branch's (written first) and the attention branch's (accumulated by the qkv dgrad GEMM's C operand).
-void backward_micro_falcon(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar) {
-  const b200w_arch& a = c->arch;
-  const int S = a.max_seq_len, T = nseq * S, d = a.hidden_size, f = a.intermediate_size;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, V = a.vocab_size;
-  const int qd = qd_of(c), kd = kd_of(c), qkvd = qkv_dim(c);
-  const float scale = 1.f / sqrtf(static_cast<float>(a.head_dim));
-  cudaStream_t s = c->stream;
-  int64_t& n = c->launches;
-  const int L = a.num_layers;
-  float* g = c->g;
-  float* part = c->dw_partial;
-  auto acc = [&](size_t off) -> const void* { return first ? nullptr : g + off; };
-  auto ar = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count); };
-  // matrices whose exchange follows their wgrad at once: the GEMM epilogue writes the bf16 wire copy itself
-  auto wire = [&](size_t off) -> void* { return overlap_ar ? c->gw + off : nullptr; };
-  auto arw = [&](size_t off, size_t count) { if (overlap_ar) allreduce_range(c, off, count, true); };
-
-  egemm(c, c->logits, false, V, c->w + c->p_lm, true, d, c->dn, nullptr, false, d, T, d, V);
-  egemm(c, c->logits, true, V, c->nf, true, d, g + c->p_embed, g + c->p_embed, true, d, V, d, T);
-  bf16* dh_cur = c->dh_a;
-  bf16* dh_alt = c->dh_b;
-  layernorm_bwd(c->dn, c->h_final, c->w + c->p_norm, c->meanf, c->rstdf, nullptr, dh_cur, g + c->p_norm,
-                g + c->p_normb, part, T, d, s); n += 3;
-  for (int l = L - 1; l >= 0; --l) {
-    auto& x = c->la[l];
-    const auto& p = c->lp[l];
-    // MLP branch: h' += gelu(ln W1^T) W2^T
-    egemm(c, dh_cur, false, d, c->w + p.wd, true, f, c->dact, nullptr, false, f, T, f, d);
-    egemm(c, dh_cur, true, d, x.act, true, f, g + p.wd, acc(p.wd), true, f, d, f, T, nullptr, 0, wire(p.wd));
-    arw(p.wd, static_cast<size_t>(d) * f);
-    gelu_bwd(c->dact, x.gu, c->dact, static_cast<size_t>(T) * f, s); ++n;
-    egemm(c, c->dact, false, f, c->w + p.wgu, true, d, c->dn, nullptr, false, d, T, d, f);
-    egemm(c, c->dact, true, f, x.n1, true, d, g + p.wgu, acc(p.wgu), true, d, f, d, T, nullptr, 0, wire(p.wgu));
-    arw(p.wgu, static_cast<size_t>(f) * d);
-    // attention branch: h' += attn Wo^T
-    egemm(c, dh_cur, false, d, c->w + p.wo, true, qd, c->dattn, nullptr, false, qd, T, qd, d);
-    egemm(c, dh_cur, true, d, x.attn, true, qd, g + p.wo, acc(p.wo), true, qd, d, qd, T, nullptr, 0, wire(p.wo));
-    arw(p.wo, static_cast<size_t>(d) * qd);
-    attention_bwd(x.qkv, qkvd, qd, qd + kd, x.attn, c->dattn, qd, x.lse, c->delta, c->dqkv, nseq, S, H,
-                  Hkv, scale, s); n += 3;
-    rope_apply(c->dqkv, qkvd, c->rope_tab, T, S, H + Hkv, a.head_dim, true, s, c->dhp); ++n;
-    egemm(c, c->dqkv, false, qkvd, c->w + p.wqkv, true, d, c->dn, c->dn, false, d, T, d, qkvd);
-    egemm(c, c->dqkv, true, qkvd, x.n1, true, d, g + p.wqkv, acc(p.wqkv), true, d, qkvd, d, T, nullptr, 0, wire(p.wqkv));
-    arw(p.wqkv, static_cast<size_t>(qkvd) * d);
-    layernorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.mean1, x.rstd1, dh_cur, dh_alt, g + p.ln1, g + p.ln1b, part,
-                  T, d, s); n += 3;
-    std::swap(dh_cur, dh_alt);
-  }
-  embed_bwd(ids, dh_cur, g + c->p_embed, nullptr, T, d, V, a.pad_token_id, S, 0, s); ++n;
-  ar(0, c->n_zero_prefix);
-}
-
 void backward_micro(b200w_ctx* c, const int32_t* ids, int nseq, bool first, bool overlap_ar,
                     const DocBounds* docs) {
+  const Dims m(c, nseq);
+  const b200w_arch& a = c->arch;
+  const bool opt = is_opt(a), falcon = is_falcon(a);
+  cudaStream_t s = c->stream;
+  int64_t& n = c->launches;
+  float* g = c->g;
+  const GradOut go{c, m.T, first, overlap_ar};
   // while the all-reduce runs under the backward, the persistent GEMMs leave NCCL its SMs
   if (overlap_ar) gemm_set_sm_reserve(c->ar_sm_reserve);
   try {
-    if (is_opt(c->arch)) backward_micro_opt(c, ids, nseq, first, overlap_ar);
-    else if (is_falcon(c->arch)) backward_micro_falcon(c, ids, nseq, first, overlap_ar);
-    else backward_micro_llama(c, ids, nseq, first, overlap_ar, docs);
+    // lm_head: dnf = dlogits W ; dW += dlogits^T nf
+    egemm(c, c->logits, false, m.V, c->w + c->p_lm, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.V);
+    // A tied head's gradient is the embedding's, zeroed with the prefix at the start of the step: the wgrad always
+    // accumulates, embed_bwd adds the lookup rows to it, and it is exchanged with the prefix.
+    if (tied_head(c))
+      egemm(c, c->logits, true, m.V, c->nf, true, m.d, g + c->p_lm, g + c->p_lm, true, m.d, m.V, m.d, m.T);
+    else
+      go.wgrad(c->p_lm, c->logits, m.V, c->nf, m.d);
+    bf16* dh_cur = c->dh_a;
+    bf16* dh_alt = c->dh_b;
+    if (has_layernorm(a)) {
+      layernorm_bwd(c->dn, c->h_final, c->w + c->p_norm, c->meanf, c->rstdf, nullptr, dh_cur, g + c->p_norm,
+                    g + c->p_normb, c->dw_partial, m.T, m.d, s); n += 3;
+    } else {
+      rmsnorm_bwd(c->dn, c->h_final, c->w + c->p_norm, c->rstdf, nullptr, dh_cur, g + c->p_norm, c->dw_partial,
+                  m.T, m.d, s); n += 2;
+    }
+    for (int l = a.num_layers - 1; l >= 0; --l) {
+      if (opt) backward_layer_opt(c, m, go, l, dh_cur, dh_alt);
+      else if (falcon) backward_layer_falcon(c, m, go, l, dh_cur, dh_alt);
+      else backward_layer_llama(c, m, go, l, dh_cur, dh_alt, docs);
+    }
+    embed_bwd(ids, dh_cur, g + c->p_embed, opt ? g + c->p_pos : nullptr, m.T, m.d, m.V, a.pad_token_id, m.S,
+              opt ? OPT_POS_OFFSET : 0, s); ++n;
+    go.exchange(0, c->n_zero_prefix);
   } catch (...) {
     gemm_set_sm_reserve(0);
     throw;
@@ -1048,6 +983,13 @@ DocBounds docs_at(const b200w_ctx* c, size_t row0) {
   return DocBounds{c->pos_dev + off, c->doc_start + off, c->doc_end + off};
 }
 
+// the loss normaliser of a target count taken on this process alone: cnt_dev = nvalid, inv_n = 1 / nvalid
+void set_count(b200w_ctx* c, long nvalid) {
+  set_count_kernel<<<1, 1, 0, c->stream>>>(c->cnt_dev, nvalid);
+  inv_count_kernel<<<1, 1, 0, c->stream>>>(c->cnt_dev, c->inv_n);
+  B200W_CUDA(cudaGetLastError());
+}
+
 // HF Trainer under DDP (transformers 5.5 trainer.py:2140-2143, average_tokens_across_devices = True,
 // the TrainingArguments default): num_items_in_batch is gathered and SUMMED over the ranks, each
 // rank's loss is sum(nll_r) / n_global * world (trainer.py:2013-2018) and DDP's mean removes the
@@ -1059,9 +1001,7 @@ DocBounds docs_at(const b200w_ctx* c, size_t row0) {
 // 8-byte all-reduce every step).
 void set_global_count(b200w_ctx* c, long nvalid_local) {
   if (!c->comm) {
-    set_count_kernel<<<1, 1, 0, c->stream>>>(c->cnt_dev, nvalid_local);
-    inv_count_kernel<<<1, 1, 0, c->stream>>>(c->cnt_dev, c->inv_n);
-    B200W_CUDA(cudaGetLastError());
+    set_count(c, nvalid_local);
     c->launches += 2;
     return;
   }
@@ -1210,6 +1150,14 @@ bool owned_part(const b200w_ctx* c, const Param& p, OwnedPart* out) {
   return false;
 }
 
+// loss and grad-norm (each nullable) from the device scalars, once the main stream has drained
+void read_scalars(b200w_ctx* ctx, float* loss_out, float* gnorm_out) {
+  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (loss_out) *loss_out = ctx->host_scal[0];
+  if (gnorm_out) *gnorm_out = ctx->host_scal[2];
+}
+
 // The bodies of b200w_forward_backward, b200w_train_step and b200w_forward. positions (nullable, HOST
 // [n_seqs, S]): per-document attention, the _docs forms.
 void forward_backward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
@@ -1218,10 +1166,7 @@ void forward_backward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* la
   fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/false, positions);
   // the reduced gradients live in the bf16 wire copy: widen them for b200w_read_state(kind = 1)
   if (ctx->comm && !ctx->shard) { cast_bf16_to_f32(ctx->gw, ctx->g, ctx->n_elems, ctx->stream); ++ctx->launches; }
-  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost,
-                             ctx->stream));
-  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (loss_out) *loss_out = ctx->host_scal[0];
+  read_scalars(ctx, loss_out, nullptr);
 }
 
 void train_step_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions,
@@ -1229,11 +1174,7 @@ void train_step_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, 
   B200W_CHECK(ids && labels, "NULL batch");
   fwd_bwd_all(ctx, ids, labels, n_seqs, /*allow_overlap=*/true, positions);
   optimizer_step(ctx, lr);
-  cudaStream_t s = ctx->stream;
-  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  B200W_CUDA(cudaStreamSynchronize(s));
-  if (loss_out) *loss_out = ctx->host_scal[0];
-  if (gnorm_out) *gnorm_out = ctx->host_scal[2];
+  read_scalars(ctx, loss_out, gnorm_out);
 }
 
 void forward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, const int32_t* positions, int n_seqs,
@@ -1261,17 +1202,11 @@ void forward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, con
     cudaFree(scratch);
   }
   if (labels && (nll_out || loss_out)) {
-    const long nvalid = count_valid(labels, n_seqs, S);
-    set_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, nvalid);
-    inv_count_kernel<<<1, 1, 0, ctx->stream>>>(ctx->cnt_dev, ctx->inv_n);
-    B200W_CUDA(cudaGetLastError());
+    set_count(ctx, count_valid(labels, n_seqs, S));
     B200W_CUDA(cudaMemsetAsync(ctx->scal, 0, 8 * sizeof(float), ctx->stream));
     loss_micro(ctx, ctx->labels_dev, n_seqs);
-    B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float),
-                               cudaMemcpyDeviceToHost, ctx->stream));
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    read_scalars(ctx, loss_out, nullptr);
     if (nll_out) B200W_CUDA(cudaMemcpy(nll_out, ctx->nll, T * 4, cudaMemcpyDeviceToHost));
-    if (loss_out) *loss_out = ctx->host_scal[0];
   }
   B200W_CUDA(cudaStreamSynchronize(ctx->stream));
 }
@@ -1438,10 +1373,10 @@ int b200w_model_init(b200w_ctx* ctx, const b200w_arch* arch, const b200w_hparams
       for (const auto& lp : ctx->lp) {
         mats.push_back({lp.wqkv, qkvd * d});
         mats.push_back({lp.wo, d * qd});
-        mats.push_back({lp.wgu, (opt || falcon ? f : 2 * f) * d});
+        mats.push_back({lp.wgu, (gated_mlp(ctx->arch) ? 2 * f : f) * d});
         mats.push_back({lp.wd, d * f});
       }
-      if (!opt && !falcon) mats.push_back({ctx->p_lm, V * d});
+      if (!tied_head(ctx)) mats.push_back({ctx->p_lm, V * d});
       build_ranges(ctx, mats);
       size_t covered = 0;
       for (const auto& rg : ctx->ranges) {
@@ -1778,11 +1713,7 @@ int b200w_train_step_resident(b200w_ctx* ctx, const int32_t* ids_dev, const int3
 int b200w_read_scalars(b200w_ctx* ctx, float* loss_out, float* gnorm_out) {
   return guarded(ctx, [&] {
     B200W_CHECK(ctx->has_model, "no model");
-    B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost,
-                               ctx->stream));
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (loss_out) *loss_out = ctx->host_scal[0];
-    if (gnorm_out) *gnorm_out = ctx->host_scal[2];
+    read_scalars(ctx, loss_out, gnorm_out);
   });
 }
 
