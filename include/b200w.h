@@ -198,7 +198,7 @@ typedef struct {
   int32_t num_heads;
   int32_t num_kv_heads;      /* Falcon-7B multi_query: 1                                        */
   int32_t head_dim;          /* 64 or 128                                                       */
-  int32_t max_ctx;           /* KV-cache length per slot                                        */
+  int32_t max_ctx;           /* KV-cache length per slot (paged cache: longest single request)  */
   float norm_eps;
   float rope_theta;
   int32_t tie_embeddings;    /* lm_head shares the embedding matrix (Falcon, OPT)               */
@@ -230,6 +230,22 @@ B200W_API int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const i
                         const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
                         float* logits_out);
 B200W_API int64_t b200w_infer_device_bytes(b200w_ctx* ctx);
+/* Paged KV cache: instead of max_batch x max_ctx positions per layer, K and V are pools of n_pages pages of
+ * 128 positions each, shared by all slots; arch->max_ctx is the longest single request. A slot serves
+ * steps and prefills only at positions inside the pages it holds (B200W_ERR_INVALID otherwise).
+ * prefill_tokens: the prefill workspace, allocated here (>= max_ctx rounded up to 128); a prefill with
+ * n_seqs * padded_len > prefill_tokens is B200W_ERR_INVALID. */
+B200W_API int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
+                                     int64_t prefill_tokens);
+/* Releases what `slot` holds, then gives it ceil(n_tokens / 128) pages (n_tokens in 1..max_ctx) from a LIFO
+ * free list. B200W_ERR_OOM when too few pages are free; nothing changes then. The page table reaches the
+ * device before the next step or prefill. The four page calls return B200W_ERR_STATE on a contiguous cache. */
+B200W_API int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens);
+B200W_API int b200w_infer_release(b200w_ctx* ctx, int slot);
+B200W_API int b200w_infer_kv_pages(b200w_ctx* ctx, int64_t* total, int64_t* free_pages);
+/* Test aid: the pages `slot` holds, in position order, into out[0 .. cap). Returns their count (>= 0) or a
+ * negative B200W_ERR_*. */
+B200W_API int b200w_infer_slot_pages(b200w_ctx* ctx, int slot, int32_t* out, int cap);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.

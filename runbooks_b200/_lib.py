@@ -87,6 +87,11 @@ PROTOTYPES = {
     "b200w_infer_step": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp]),
     "b200w_infer_prefill": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "b200w_infer_device_bytes": (C.c_int64, [c_ctx]),
+    "b200w_infer_init_paged": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int, C.c_int, C.c_int64]),
+    "b200w_infer_reserve": (C.c_int, [c_ctx, C.c_int, C.c_int]),
+    "b200w_infer_release": (C.c_int, [c_ctx, C.c_int]),
+    "b200w_infer_kv_pages": (C.c_int, [c_ctx, i64p, i64p]),
+    "b200w_infer_slot_pages": (C.c_int, [c_ctx, C.c_int, vp, C.c_int]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,

@@ -25,6 +25,7 @@
 
 #include <algorithm>
 #include <memory>
+#include <stdexcept>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -152,12 +153,26 @@ __global__ void gelu_strided_kernel(bf16* x, int T, int N, int ld) {
   *reinterpret_cast<uint4*>(x + t * ld + c) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
+// KV-cache layouts. Contiguous: a layer's cache is [max_batch][max_ctx] rows of kd elements. Paged
+// (b200w_infer_init_paged): a layer's cache is a pool of pages of KV_PAGE rows, and position p of a slot
+// lives in row table[slot][p / KV_PAGE] * KV_PAGE + p % KV_PAGE. A page is one 128-key block of the
+// tensor-core decode attention, so a block is always one TMA box inside one page.
+constexpr int KV_PAGE = 128;
+template <bool PAGED>
+__device__ __forceinline__ size_t cache_row(int slot, int p, int max_ctx, const int32_t* __restrict__ table,
+                                            int tpages) {
+  if constexpr (PAGED) return static_cast<size_t>(table[slot * tpages + p / KV_PAGE]) * KV_PAGE + p % KV_PAGE;
+  else return static_cast<size_t>(slot) * max_ctx + p;
+}
+
 // Decode: rotate_half RoPE on the q heads (in place) and on k (rope != 0; OPT has none); k and v are
 // written into the cache at [slot][pos]. One thread per (row, head, pair index).
+template <bool PAGED>
 __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* __restrict__ inv_freq,
                                    const int32_t* __restrict__ pos, const int32_t* __restrict__ slot,
                                    bf16* __restrict__ kcache, bf16* __restrict__ vcache, int n, int H,
-                                   int Hkv, int dh, int max_ctx, int rope) {
+                                   int Hkv, int dh, int max_ctx, int rope, const int32_t* __restrict__ table,
+                                   int tpages) {
   pdl_trigger();
   pdl_wait();
   const int half = dh / 2;
@@ -181,7 +196,7 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* 
     }
   } else {
     const int hk = h - H;
-    const size_t off = ((static_cast<size_t>(slot[r]) * max_ctx + p) * Hkv + hk) * dh;
+    const size_t off = (cache_row<PAGED>(slot[r], p, max_ctx, table, tpages) * Hkv + hk) * dh;
     kcache[off + i] = o1;
     kcache[off + i + half] = o2;
     const bf16* vsrc = qkv + static_cast<size_t>(r) * ld + (H + Hkv + hk) * dh;
@@ -193,11 +208,13 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* 
 // Prefill: token t = b * S + p of sequence b. q / k (rotated when rope != 0) and v go to the attention
 // input `dst` [T, (H + 2 Hkv) * dhp] (heads at stride dhp >= dh; the padding columns are zero from
 // allocation and never written) and, for real positions p < len[b], k / v also into cache slot[b].
+template <bool PAGED>
 __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
                                             int ld_dst, const float* __restrict__ inv_freq,
                                             const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
                                             bf16* __restrict__ kcache, bf16* __restrict__ vcache, int T, int S,
-                                            int H, int Hkv, int dh, int dhp, int max_ctx, int rope) {
+                                            int H, int Hkv, int dh, int dhp, int max_ctx, int rope,
+                                            const int32_t* __restrict__ table, int tpages) {
   const int half = dh / 2, HT = H + 2 * Hkv;
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(T) * HT * half;
@@ -221,7 +238,7 @@ __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld
   if (h >= H && p < lens[b]) {
     const bool is_k = h < H + Hkv;
     const int hk = is_k ? h - H : h - H - Hkv;
-    const size_t off = ((static_cast<size_t>(slot[b]) * max_ctx + p) * Hkv + hk) * dh;
+    const size_t off = (cache_row<PAGED>(slot[b], p, max_ctx, table, tpages) * Hkv + hk) * dh;
     bf16* c = is_k ? kcache : vcache;
     c[off + i] = o1;
     c[off + i + half] = o2;
@@ -254,12 +271,12 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* 
 // group of GT query heads that share that kv head): every K/V row is read once per block.
 constexpr int ATT_GT = 8;
 constexpr int ATT_THREADS = 256;
-template <int DH>
+template <int DH, bool PAGED>
 __global__ void __launch_bounds__(ATT_THREADS)
 decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache,
                    const bf16* __restrict__ vcache, const int32_t* __restrict__ pos,
                    const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
-                   int max_ctx, int sc_stride, float scale) {
+                   int max_ctx, int sc_stride, float scale, const int32_t* __restrict__ table, int tpages) {
   extern __shared__ float sm[];
   pdl_trigger();
   pdl_wait();
@@ -276,10 +293,15 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
     sq[g * DH + c] = __bfloat162float(qkv[static_cast<size_t>(r) * ld + (hk * G + g0 + g) * DH + c]) * scale;
   }
   __syncthreads();
-  const size_t cbase = static_cast<size_t>(slot[r]) * max_ctx;
+  const size_t cbase = static_cast<size_t>(slot[r]) * max_ctx;   // contiguous
+  const int32_t* prow = table + slot[r] * tpages;                 // paged: the slot's page-table row
+  auto crow = [&](int t) -> size_t {                              // cache row of key position t
+    if constexpr (PAGED) return static_cast<size_t>(prow[t / KV_PAGE]) * KV_PAGE + t % KV_PAGE;
+    else return cbase + t;
+  };
   // scores: one key position per thread, the K row lives in registers for all ng heads
   for (int t = tid; t < len; t += ATT_THREADS) {
-    const uint4* krow = reinterpret_cast<const uint4*>(kcache + ((cbase + t) * Hkv + hk) * DH);
+    const uint4* krow = reinterpret_cast<const uint4*>(kcache + (crow(t) * Hkv + hk) * DH);
     float acc[ATT_GT];
 #pragma unroll
     for (int g = 0; g < ATT_GT; ++g) acc[g] = 0.f;
@@ -330,7 +352,7 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int t = t0 + u * SLICES;
-      vv[u] = t < len ? *reinterpret_cast<const uint4*>(vcache + ((cbase + t) * Hkv + hk) * DH + dg * 8)
+      vv[u] = t < len ? *reinterpret_cast<const uint4*>(vcache + (crow(t) * Hkv + hk) * DH + dg * 8)
                       : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
@@ -394,12 +416,14 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-template <int DH>
+static_assert(TC_KB == KV_PAGE, "a key block of the tensor-core decode attention is one cache page");
+template <int DH, bool PAGED>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                       const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
                       const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
-                      int H, int Hkv, int max_ctx, int nsplit, float scale_log2) {
+                      int H, int Hkv, int max_ctx, int nsplit, float scale_log2, const int32_t* __restrict__ table,
+                      int tpages) {
   constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
   const int split = blockIdx.x, hk = blockIdx.y, r = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31;
@@ -426,7 +450,8 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
   }
   __syncthreads();
   if (tid == 0) {
-    const int row0 = slot[r] * max_ctx + k0;  // first cache row of this block
+    // first cache row of this block (paged: the first row of page `split` of the slot)
+    const int row0 = PAGED ? table[slot[r] * tpages + split] * KV_PAGE : slot[r] * max_ctx + k0;
     mbar_arrive_expect_tx(bar_kv, 2 * NA * TC_ATOM);
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
@@ -636,7 +661,19 @@ struct Infer {
   // decode activations [max_batch, *]
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
-  bf16 *kc = nullptr, *vc = nullptr;  // [L][max_batch][max_ctx][Hkv*dh], zero-initialised
+  bf16 *kc = nullptr, *vc = nullptr;  // [L][layer_rows()][Hkv*dh], zero-initialised
+  // paged layout (n_pages > 0): page table [max_batch][tpages] on the device, written from pinned staging by
+  // b200w_infer_reserve; `held` is its host mirror (the pages a slot owns, in table order), `free_pages` a
+  // LIFO stack of the others
+  int n_pages = 0, tpages = 0;
+  int32_t* table = nullptr;
+  int32_t* table_pin = nullptr;
+  std::vector<int32_t> free_pages;
+  std::vector<std::vector<int32_t>> held;
+  size_t pf_limit = 0;  // paged: tokens of the preallocated prefill workspace, the most one prefill call takes
+  size_t layer_rows() const {
+    return n_pages ? static_cast<size_t>(n_pages) * KV_PAGE : static_cast<size_t>(max_batch) * a.max_ctx;
+  }
   float* inv_freq = nullptr;
   float* ws = nullptr;          // split-K workspace [max_batch, max N] (kept zeroed)
   unsigned* counters = nullptr;
@@ -681,6 +718,7 @@ struct Infer {
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
     if (pin) cudaFreeHost(pin);
     if (pf_pin) cudaFreeHost(pf_pin);
+    if (table_pin) cudaFreeHost(table_pin);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -772,6 +810,11 @@ void build(Infer* m) {
   else m->p_lm = add_dense(m, "lm_head.weight", a.vocab_size, d);
 }
 
+// a call that does not fit the context's configuration (B200W_ERR_STATE)
+struct StateError : std::runtime_error {
+  using std::runtime_error::runtime_error;
+};
+
 template <typename F>
 int iguard(b200w_ctx* ctx, F&& f) {
   if (!ctx) return B200W_ERR_INVALID;
@@ -785,6 +828,9 @@ int iguard(b200w_ctx* ctx, F&& f) {
   } catch (const Error& e) {
     ctx_set_error(ctx, e.what());
     return std::string(e.what()).rfind("check failed", 0) == 0 ? B200W_ERR_INVALID : B200W_ERR_CUDA;
+  } catch (const StateError& e) {
+    ctx_set_error(ctx, e.what());
+    return B200W_ERR_STATE;
   } catch (const std::exception& e) {
     ctx_set_error(ctx, e.what());
     return B200W_ERR_INVALID;
@@ -841,28 +887,36 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
   const auto& a = m->a;
   const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, G = H / Hkv;
   const float scale = 1.f / sqrtf(static_cast<float>(dh));
-  const size_t layer_cache = static_cast<size_t>(m->max_batch) * a.max_ctx * m->kd;
-  bf16* kc = m->kc + layer * layer_cache;
-  bf16* vc = m->vc + layer * layer_cache;
+  const uint64_t rows = m->layer_rows();
+  const bool paged = m->n_pages > 0;
+  bf16* kc = m->kc + layer * rows * m->kd;
+  bf16* vc = m->vc + layer * rows * m->kd;
   if (G >= 4) {
     // grouped / multi-query: the group is the M dimension of a tensor-core tile
-    const uint64_t rows = static_cast<uint64_t>(m->max_batch) * a.max_ctx;
     CUtensorMap tk = make_tmap_bf16_2d(kc, rows, m->kd, m->kd, TC_KB, 64);
     CUtensorMap tv = make_tmap_bf16_2d(vc, rows, m->kd, m->kd, TC_KB, 64);
     const float scale_log2 = scale * 1.4426950408889634f;
     const dim3 grid(m->nsplit, Hkv, n);
     if (dh == 64) {
       static PerDeviceOnce once;
-      once.run([&] { B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<64>())); });
-      launch_pdl(decode_attn_tc_kernel<64>, grid, dim3(TC_THREADS), tc_smem_bytes<64>(), s, tk, tv, m->qkv, m->qkvd,
-                 m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, a.max_ctx, m->nsplit, scale_log2);
+      once.run([&] {
+        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<64>()));
+        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<64>()));
+      });
+      launch_pdl(paged ? decode_attn_tc_kernel<64, true> : decode_attn_tc_kernel<64, false>, grid, dim3(TC_THREADS),
+                 tc_smem_bytes<64>(), s, tk, tv, m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv,
+                 a.max_ctx, m->nsplit, scale_log2, m->table, m->tpages);
       launch_pdl(decode_attn_merge_kernel<64>, dim3(cdiv(H, 4), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
                  out, ldo, H, m->nsplit);
     } else {
       static PerDeviceOnce once;
-      once.run([&] { B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<128>())); });
-      launch_pdl(decode_attn_tc_kernel<128>, grid, dim3(TC_THREADS), tc_smem_bytes<128>(), s, tk, tv, m->qkv, m->qkvd,
-                 m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, a.max_ctx, m->nsplit, scale_log2);
+      once.run([&] {
+        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<128>()));
+        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<128>()));
+      });
+      launch_pdl(paged ? decode_attn_tc_kernel<128, true> : decode_attn_tc_kernel<128, false>, grid, dim3(TC_THREADS),
+                 tc_smem_bytes<128>(), s, tk, tv, m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv,
+                 a.max_ctx, m->nsplit, scale_log2, m->table, m->tpages);
       launch_pdl(decode_attn_merge_kernel<128>, dim3(cdiv(H, 2), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
                  out, ldo, H, m->nsplit);
     }
@@ -876,15 +930,15 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
   B200W_CHECK(att_smem <= 200 * 1024, "max_ctx too large for the decode attention kernel");
   static PerDeviceOnce once;
   once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   });
-  if (dh == 64)
-    launch_pdl(decode_attn_kernel<64>, agrid, dim3(ATT_THREADS), att_smem, s, m->qkv, m->qkvd, kc, vc, m->pos, m->slot,
-               out, ldo, H, Hkv, a.max_ctx, sc_stride, scale);
-  else
-    launch_pdl(decode_attn_kernel<128>, agrid, dim3(ATT_THREADS), att_smem, s, m->qkv, m->qkvd, kc, vc, m->pos, m->slot,
-               out, ldo, H, Hkv, a.max_ctx, sc_stride, scale);
+  auto kern = dh == 64 ? (paged ? decode_attn_kernel<64, true> : decode_attn_kernel<64, false>)
+                       : (paged ? decode_attn_kernel<128, true> : decode_attn_kernel<128, false>);
+  launch_pdl(kern, agrid, dim3(ATT_THREADS), att_smem, s, m->qkv, m->qkvd, kc, vc, m->pos, m->slot, out, ldo, H, Hkv,
+             a.max_ctx, sc_stride, scale, m->table, m->tpages);
   ++nl;
 }
 
@@ -900,7 +954,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
             V = a.vocab_size;
   const int qd = m->qd, qkvd = m->qkvd;
   const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
-  const size_t layer_cache = static_cast<size_t>(B) * a.max_ctx * m->kd;
+  const size_t layer_cache = m->layer_rows() * m->kd;
+  auto rope_append = m->n_pages ? rope_append_kernel<true> : rope_append_kernel<false>;
   B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin + B, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin + 2 * B, n * 4, cudaMemcpyHostToDevice, s));
@@ -923,8 +978,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       o1.out2 = m->cat + qd; o1.ldo2 = m->ld_cat; o1.n_split = qkvd;
       o1.act = 1; o1.act_from = qkvd;   // exact GeLU on the MLP half only
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd + f, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1); ++nl;
+      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1, m->table, m->tpages); ++nl;
       decode_attention(m, s, n, l, m->cat, m->ld_cat, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -935,8 +990,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd; o1.bias = m->w + p.bqkv;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 0); ++nl;
+      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, a.max_ctx, 0, m->table, m->tpages); ++nl;
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d; o2.bias = m->w + p.bo;
@@ -953,8 +1008,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1); ++nl;
+      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1, m->table, m->tpages); ++nl;
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -1012,75 +1067,197 @@ void ensure_prefill(Infer* m, size_t T) {
   m->pf_cap = T;
 }
 
+// pinned staging of one prefill call: tokens [T] | lengths | slots | last rows [max_batch each]
+void ensure_prefill_pin(Infer* m, size_t T) {
+  const size_t need = T + 3 * static_cast<size_t>(m->max_batch);
+  if (m->pf_pin_cap >= need) return;
+  if (m->pf_pin) cudaFreeHost(m->pf_pin);
+  m->pf_pin = nullptr;
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pf_pin), need * sizeof(int32_t)));
+  m->pf_pin_cap = need;
+}
+
+Infer* paged_model(b200w_ctx* ctx) {
+  Infer* m = model(ctx);
+  if (m->n_pages == 0) throw StateError("the KV cache is not paged (b200w_infer_init_paged)");
+  return m;
+}
+
+// Paged mode: positions [0, n_tokens) of `slot` must lie in pages the slot holds (the host mirror of the table).
+void check_paged_slot(const Infer* m, int slot, long long n_tokens) {
+  if (m->n_pages == 0) return;
+  const size_t held = m->held[slot].size();
+  B200W_CHECK(held > 0, "cache slot holds no KV pages (b200w_infer_reserve)");
+  B200W_CHECK(n_tokens <= static_cast<long long>(held) * KV_PAGE, "position beyond the KV pages the slot holds");
+}
+
+void release_pages(Infer* m, int slot) {
+  auto& h = m->held[slot];
+  m->free_pages.insert(m->free_pages.end(), h.begin(), h.end());
+  h.clear();
+}
+
+// b200w_infer_init (n_pages == 0) and b200w_infer_init_paged
+void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages, int64_t prefill_tokens) {
+  B200W_CHECK(arch != nullptr && max_batch >= 1 && max_batch <= 128, "bad arch / max_batch (1..128)");
+  B200W_CHECK(ctx_infer_slot(ctx) == nullptr, "inference model already initialised");
+  B200W_CHECK(arch->family == B200W_FAMILY_LLAMA || arch->family == B200W_FAMILY_FALCON ||
+                  arch->family == B200W_FAMILY_OPT, "unknown family");
+  B200W_CHECK(arch->head_dim == 64 || arch->head_dim == 128, "head_dim must be 64 or 128");
+  B200W_CHECK(arch->num_heads % arch->num_kv_heads == 0, "heads must be a multiple of kv heads");
+  B200W_CHECK(arch->hidden_size % 8 == 0 && arch->intermediate_size % 8 == 0 && arch->vocab_size % 8 == 0,
+              "sizes must be multiples of 8");
+  B200W_CHECK(arch->hidden_size <= 256 * 8 * LN_MAXP, "hidden_size too large for the decode LayerNorm");
+  B200W_CHECK(arch->max_ctx >= 1 && arch->max_ctx <= 8192, "max_ctx must be in 1..8192");
+  if (arch->family == B200W_FAMILY_OPT)
+    B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
+  const int64_t ctx_rounded = cdiv(arch->max_ctx, KV_PAGE) * static_cast<int64_t>(KV_PAGE);
+  if (n_pages) {
+    // a page index times KV_PAGE is an int32 TMA row coordinate
+    B200W_CHECK(n_pages >= 1 && n_pages <= (1 << 24), "n_pages must be in 1..2^24");
+    B200W_CHECK(prefill_tokens >= ctx_rounded && prefill_tokens <= (1 << 20),
+                "prefill_tokens must be in [max_ctx rounded up to 128, 2^20]");
+  }
+  auto m = std::make_unique<Infer>();
+  m->a = *arch;
+  m->max_batch = max_batch;
+  m->n_pages = n_pages;
+  if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
+  m->lt.resize(arch->num_layers);   // all-null when the tiled copies are disabled
+  build(m.get());
+  const auto& a = m->a;
+  const size_t B = max_batch, d = a.hidden_size, f = a.intermediate_size;
+  const size_t qd = m->qd, kd = m->kd;
+  m->w = m->alloc<bf16>(m->n_elems);
+  m->h = m->alloc<bf16>(B * d);
+  m->h2 = m->alloc<bf16>(B * d);
+  m->nrm = m->alloc<bf16>(B * d);
+  m->qkv = m->alloc<bf16>(B * (qd + 2 * kd));
+  m->cat = m->alloc<bf16>(B * m->ld_cat);
+  const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
+  m->mid = m->alloc<bf16>(B * fmid);
+  m->act = m->alloc<bf16>(B * f);
+  m->logits = m->alloc<bf16>(B * a.vocab_size);
+  const size_t cache = static_cast<size_t>(a.num_layers) * m->layer_rows() * kd;
+  m->kc = m->alloc<bf16>(cache);
+  m->vc = m->alloc<bf16>(cache);
+  // zero: the tensor-core decode attention multiplies P = 0 by whatever the rows beyond a slot's length hold
+  // (a page handed out again holds zeros or K/V an earlier request wrote: finite either way)
+  B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
+  B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
+  m->nsplit = (a.max_ctx + TC_KB - 1) / TC_KB;
+  if (n_pages) {
+    m->tpages = m->nsplit;
+    const size_t tab = B * m->tpages;
+    m->table = m->alloc<int32_t>(tab);
+    B200W_CUDA(cudaMemset(m->table, 0, tab * sizeof(int32_t)));
+    B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->table_pin), tab * sizeof(int32_t)));
+    memset(m->table_pin, 0, tab * sizeof(int32_t));
+    for (int p = n_pages - 1; p >= 0; --p) m->free_pages.push_back(p);   // page 0 is handed out first
+    m->held.assign(B, {});
+    // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
+    m->pf_limit = static_cast<size_t>(prefill_tokens);
+    ensure_prefill(m.get(), m->pf_limit);
+    ensure_prefill_pin(m.get(), m->pf_limit);
+  }
+  if (a.num_heads / a.num_kv_heads >= 4) {
+    m->part_o = m->alloc<float>(B * a.num_heads * m->nsplit * a.head_dim);
+    m->part_ml = m->alloc<float2>(B * a.num_heads * m->nsplit);
+  }
+  m->tok = m->alloc<int32_t>(B);
+  m->pos = m->alloc<int32_t>(B);
+  m->slot = m->alloc<int32_t>(B);
+  m->next = m->alloc<int32_t>(B);
+  m->pf_len = m->alloc<int32_t>(B);
+  m->pf_slot = m->alloc<int32_t>(B);
+  m->pf_last = m->alloc<int32_t>(B);
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin), 4 * B * sizeof(int32_t)));
+  m->inv_freq = m->alloc<float>(a.head_dim / 2);
+  const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + qd + 2 * kd, d});
+  m->ws = m->alloc<float>(B * max_n);
+  m->counters = m->alloc<unsigned>((max_n + 127) / 128);
+  B200W_CUDA(cudaMemset(m->ws, 0, B * max_n * sizeof(float)));
+  B200W_CUDA(cudaMemset(m->counters, 0, ((max_n + 127) / 128) * sizeof(unsigned)));
+  std::vector<float> inv(a.head_dim / 2);
+  for (int i = 0; i < a.head_dim / 2; ++i)
+    inv[i] = static_cast<float>(1.0 / pow(static_cast<double>(a.rope_theta > 0 ? a.rope_theta : 10000.0),
+                                          2.0 * i / a.head_dim));
+  B200W_CUDA(cudaMemcpy(m->inv_freq, inv.data(), inv.size() * 4, cudaMemcpyHostToDevice));
+  ctx_set_infer(ctx, m.release(), infer_destroy);
+}
+
 }  // namespace
 
 extern "C" {
 
 int b200w_infer_init(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch) {
+  return iguard(ctx, [&] { init_infer(ctx, arch, max_batch, 0, 0); });
+}
+
+int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
+                           int64_t prefill_tokens) {
   return iguard(ctx, [&] {
-    B200W_CHECK(arch != nullptr && max_batch >= 1 && max_batch <= 128, "bad arch / max_batch (1..128)");
-    B200W_CHECK(ctx_infer_slot(ctx) == nullptr, "inference model already initialised");
-    B200W_CHECK(arch->family == B200W_FAMILY_LLAMA || arch->family == B200W_FAMILY_FALCON ||
-                    arch->family == B200W_FAMILY_OPT, "unknown family");
-    B200W_CHECK(arch->head_dim == 64 || arch->head_dim == 128, "head_dim must be 64 or 128");
-    B200W_CHECK(arch->num_heads % arch->num_kv_heads == 0, "heads must be a multiple of kv heads");
-    B200W_CHECK(arch->hidden_size % 8 == 0 && arch->intermediate_size % 8 == 0 && arch->vocab_size % 8 == 0,
-                "sizes must be multiples of 8");
-    B200W_CHECK(arch->hidden_size <= 256 * 8 * LN_MAXP, "hidden_size too large for the decode LayerNorm");
-    B200W_CHECK(arch->max_ctx >= 1 && arch->max_ctx <= 8192, "max_ctx must be in 1..8192");
-    if (arch->family == B200W_FAMILY_OPT)
-      B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
-    auto m = std::make_unique<Infer>();
-    m->a = *arch;
-    m->max_batch = max_batch;
-    if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
-    m->lt.resize(arch->num_layers);   // all-null when the tiled copies are disabled
-    build(m.get());
-    const auto& a = m->a;
-    const size_t B = max_batch, d = a.hidden_size, f = a.intermediate_size;
-    const size_t qd = m->qd, kd = m->kd;
-    m->w = m->alloc<bf16>(m->n_elems);
-    m->h = m->alloc<bf16>(B * d);
-    m->h2 = m->alloc<bf16>(B * d);
-    m->nrm = m->alloc<bf16>(B * d);
-    m->qkv = m->alloc<bf16>(B * (qd + 2 * kd));
-    m->cat = m->alloc<bf16>(B * m->ld_cat);
-    const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
-    m->mid = m->alloc<bf16>(B * fmid);
-    m->act = m->alloc<bf16>(B * f);
-    m->logits = m->alloc<bf16>(B * a.vocab_size);
-    const size_t cache = static_cast<size_t>(a.num_layers) * B * a.max_ctx * kd;
-    m->kc = m->alloc<bf16>(cache);
-    m->vc = m->alloc<bf16>(cache);
-    // zero: the tensor-core decode attention multiplies P = 0 by whatever the rows beyond a slot's length hold
-    B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
-    B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
-    m->nsplit = (a.max_ctx + TC_KB - 1) / TC_KB;
-    if (a.num_heads / a.num_kv_heads >= 4) {
-      m->part_o = m->alloc<float>(B * a.num_heads * m->nsplit * a.head_dim);
-      m->part_ml = m->alloc<float2>(B * a.num_heads * m->nsplit);
-    }
-    m->tok = m->alloc<int32_t>(B);
-    m->pos = m->alloc<int32_t>(B);
-    m->slot = m->alloc<int32_t>(B);
-    m->next = m->alloc<int32_t>(B);
-    m->pf_len = m->alloc<int32_t>(B);
-    m->pf_slot = m->alloc<int32_t>(B);
-    m->pf_last = m->alloc<int32_t>(B);
-    B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin), 4 * B * sizeof(int32_t)));
-    m->inv_freq = m->alloc<float>(a.head_dim / 2);
-    const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + qd + 2 * kd, d});
-    m->ws = m->alloc<float>(B * max_n);
-    m->counters = m->alloc<unsigned>((max_n + 127) / 128);
-    B200W_CUDA(cudaMemset(m->ws, 0, B * max_n * sizeof(float)));
-    B200W_CUDA(cudaMemset(m->counters, 0, ((max_n + 127) / 128) * sizeof(unsigned)));
-    std::vector<float> inv(a.head_dim / 2);
-    for (int i = 0; i < a.head_dim / 2; ++i)
-      inv[i] = static_cast<float>(1.0 / pow(static_cast<double>(a.rope_theta > 0 ? a.rope_theta : 10000.0),
-                                            2.0 * i / a.head_dim));
-    B200W_CUDA(cudaMemcpy(m->inv_freq, inv.data(), inv.size() * 4, cudaMemcpyHostToDevice));
-    ctx_set_infer(ctx, m.release(), infer_destroy);
+    B200W_CHECK(n_pages >= 1, "n_pages must be >= 1");
+    init_infer(ctx, arch, max_batch, n_pages, prefill_tokens);
   });
+}
+
+int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens) {
+  bool short_of_pages = false;
+  const int st = iguard(ctx, [&] {
+    Infer* m = paged_model(ctx);
+    B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
+    B200W_CHECK(n_tokens >= 1 && n_tokens <= m->a.max_ctx, "n_tokens must be in 1..max_ctx");
+    const size_t need = cdiv(n_tokens, KV_PAGE);
+    if (need > m->free_pages.size() + m->held[slot].size()) {
+      ctx_set_error(ctx, ("KV page pool exhausted: " + std::to_string(need) + " pages needed, " +
+                          std::to_string(m->free_pages.size()) + " free").c_str());
+      short_of_pages = true;
+      return;
+    }
+    release_pages(m, slot);
+    auto& h = m->held[slot];
+    for (size_t i = 0; i < need; ++i) {
+      h.push_back(m->free_pages.back());
+      m->free_pages.pop_back();
+    }
+    // the row goes to the device on the library stream, so it lands before the next step or prefill; the
+    // table's address never changes, so the captured decode graphs read the new row
+    int32_t* row = m->table_pin + static_cast<size_t>(slot) * m->tpages;
+    std::copy(h.begin(), h.end(), row);
+    std::fill(row + h.size(), row + m->tpages, 0);
+    B200W_CUDA(cudaMemcpyAsync(m->table + static_cast<size_t>(slot) * m->tpages, row, m->tpages * sizeof(int32_t),
+                               cudaMemcpyHostToDevice, ctx_stream(ctx)));
+  });
+  return st == B200W_OK && short_of_pages ? B200W_ERR_OOM : st;
+}
+
+int b200w_infer_release(b200w_ctx* ctx, int slot) {
+  return iguard(ctx, [&] {
+    Infer* m = paged_model(ctx);
+    B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
+    release_pages(m, slot);   // the device row is left as it was: steps and prefills of the slot are refused
+  });
+}
+
+int b200w_infer_kv_pages(b200w_ctx* ctx, int64_t* total, int64_t* free_pages) {
+  return iguard(ctx, [&] {
+    Infer* m = paged_model(ctx);
+    if (total) *total = m->n_pages;
+    if (free_pages) *free_pages = static_cast<int64_t>(m->free_pages.size());
+  });
+}
+
+int b200w_infer_slot_pages(b200w_ctx* ctx, int slot, int32_t* out, int cap) {
+  int n = 0;
+  const int st = iguard(ctx, [&] {
+    Infer* m = paged_model(ctx);
+    B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
+    const auto& h = m->held[slot];
+    n = static_cast<int>(h.size());
+    if (out) std::copy(h.begin(), h.begin() + std::min(n, std::max(cap, 0)), out);
+  });
+  return st == B200W_OK ? n : st;
 }
 
 int b200w_infer_param_count(b200w_ctx* ctx, int64_t* n_tensors, int64_t* n_elements) {
@@ -1166,6 +1343,7 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
       B200W_CHECK(positions[i] >= 0 && positions[i] < a.max_ctx, "position outside the KV cache");
       B200W_CHECK(slots[i] >= 0 && slots[i] < m->max_batch, "bad cache slot");
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
+      check_paged_slot(m, slots[i], positions[i] + 1LL);
     }
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
@@ -1236,20 +1414,16 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     for (int b = 0; b < n_seqs; ++b) {
       B200W_CHECK(lengths[b] >= 1 && lengths[b] <= S && lengths[b] <= a.max_ctx, "bad prompt length");
       B200W_CHECK(slots[b] >= 0 && slots[b] < m->max_batch, "bad cache slot");
+      check_paged_slot(m, slots[b], lengths[b]);
     }
+    if (m->n_pages) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
     for (size_t i = 0; i < T; ++i)
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
     if (a.family == B200W_FAMILY_OPT) B200W_CHECK(S <= a.max_positions, "OPT: padded_len exceeds the position table");
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
     ensure_prefill(m, T);
-    const size_t need = T + 3 * static_cast<size_t>(m->max_batch);
-    if (m->pf_pin_cap < need) {
-      if (m->pf_pin) cudaFreeHost(m->pf_pin);
-      m->pf_pin = nullptr;
-      B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pf_pin), need * sizeof(int32_t)));
-      m->pf_pin_cap = need;
-    }
+    ensure_prefill_pin(m, T);
     const int B = m->max_batch;
     int32_t* pin = m->pf_pin;
     memcpy(pin, tokens, T * 4);
@@ -1270,7 +1444,8 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     const int dhp = 128, HT = H + 2 * Hkv;
     const bool padded = dh != dhp;
     const float scale = 1.f / sqrtf(static_cast<float>(dh));
-    const size_t layer_cache = static_cast<size_t>(B) * a.max_ctx * m->kd;
+    const size_t layer_cache = m->layer_rows() * m->kd;
+    auto scatter = m->n_pages ? prefill_rope_scatter_kernel<true> : prefill_rope_scatter_kernel<false>;
     const int Ti = static_cast<int>(T);
     auto G = [&](const void* A, int lda, size_t woff, int ldw, void* D, const void* C, int ldd, int N, int K,
                  const void* bias = nullptr, int act = 0) {
@@ -1295,9 +1470,8 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
       bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
       const int ld_in = padded ? HT * dhp : qkvd;
       const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
-      prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq, m->pf_len,
-                                                                m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dhp, a.max_ctx,
-                                                                opt ? 0 : 1); ++nl;
+      scatter<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq, m->pf_len, m->pf_slot, kc, vc,
+                                            Ti, S, H, Hkv, dh, dhp, a.max_ctx, opt ? 0 : 1, m->table, m->tpages); ++nl;
       B200W_CUDA(cudaGetLastError());
       bf16* att_out = padded ? m->pf_attp : m->pf_cat;
       const int ld_out = padded ? H * dhp : ldc;

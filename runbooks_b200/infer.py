@@ -71,13 +71,61 @@ class ServeArch:
         raise ValueError(f"unsupported model_type {mt!r} (falcon, llama, opt)")
 
 
+KV_PAGE = 128   # positions per page of the paged KV cache (one key block of the decode attention)
+
+
+def kv_page_bytes(arch: ServeArch) -> int:
+    """Device bytes of one page: K and V, every layer, 128 positions of num_kv_heads * head_dim bf16."""
+    return 2 * arch.num_layers * KV_PAGE * arch.num_kv_heads * arch.head_dim * 2
+
+
+def pages_for(n_tokens: int) -> int:
+    return (n_tokens + KV_PAGE - 1) // KV_PAGE
+
+
+class CacheFull(RuntimeError):
+    """The paged KV cache has too few free pages for a request right now (it fits the pool once others end)."""
+
+
 class InferEngine(Engine):
-    def init_infer(self, arch: ServeArch, max_batch: int = 32):
+    kv_pages: Optional[int] = None   # pages in the pool; None: the contiguous max_batch x max_ctx cache
+
+    def init_infer(self, arch: ServeArch, max_batch: int = 32, kv_pages: Optional[int] = None,
+                   prefill_tokens: Optional[int] = None):
+        """kv_pages: serve from a pool of that many 128-position pages shared by all slots (b200w_infer_init_paged)
+        instead of reserving max_ctx positions per slot; arch.max_ctx is then the longest single request.
+        prefill_tokens: the most tokens (n_seqs * padded length) one prefill call takes in paged mode."""
         ca = _CArch(FAMILY[arch.family], arch.vocab_size, arch.hidden_size, arch.intermediate_size,
                     arch.num_layers, arch.num_heads, arch.num_kv_heads, arch.head_dim, arch.max_ctx,
                     arch.norm_eps, arch.rope_theta, 1 if arch.tie_embeddings else 0, arch.max_positions)
-        self._check(self._lib.b200w_infer_init(self._h, C.byref(ca), max_batch))
+        if kv_pages is None:
+            self._check(self._lib.b200w_infer_init(self._h, C.byref(ca), max_batch))
+        else:
+            if prefill_tokens is None:
+                prefill_tokens = max(16384, pages_for(arch.max_ctx) * KV_PAGE)
+            self._check(self._lib.b200w_infer_init_paged(self._h, C.byref(ca), max_batch, kv_pages, prefill_tokens))
+            self.kv_pages, self.prefill_tokens = kv_pages, prefill_tokens
         self.serve_arch, self.max_batch = arch, max_batch
+
+    def reserve(self, slot: int, n_tokens: int):
+        """Give `slot` the pages for positions [0, n_tokens) (releasing what it held); B200WError with status
+        B200W_ERR_OOM (-5) when too few pages are free."""
+        self._check(self._lib.b200w_infer_reserve(self._h, slot, n_tokens))
+
+    def release(self, slot: int):
+        self._check(self._lib.b200w_infer_release(self._h, slot))
+
+    def kv_pages_free(self) -> int:
+        free = C.c_int64()
+        self._check(self._lib.b200w_infer_kv_pages(self._h, None, C.byref(free)))
+        return free.value
+
+    def slot_pages(self, slot: int) -> List[int]:
+        out = np.empty(self.kv_pages, dtype=np.int32)
+        n = self._lib.b200w_infer_slot_pages(self._h, slot, out.ctypes.data, out.size)
+        if n < 0:
+            self._check(n)
+        return out[:n].tolist()
 
     def infer_params(self) -> Iterable[Tuple[str, Tuple[int, ...]]]:
         n = C.c_int64()
@@ -181,6 +229,8 @@ class Generator:
         self.active: List[_Req] = []
         self.use_prefill = use_prefill and hasattr(engine, "prefill")
         self._deferred: List[_Req] = []
+        # paged KV cache: a request holds pages for len(prompt) + max_tokens positions from admission to its end
+        self.kv_pages = getattr(engine, "kv_pages", None)
 
     def add(self, prompt: List[int], max_tokens: int, temperature: float = 0.0, top_p: float = 1.0,
             seed: Optional[int] = None, defer_prefill: bool = False) -> _Req:
@@ -195,8 +245,15 @@ class Generator:
             raise ValueError(f"token id {bad[0]} outside the model vocabulary ({V})")
         if len(prompt) + max_tokens > self.e.serve_arch.max_ctx:
             raise ValueError("prompt + max_tokens exceeds the KV cache length")
+        if self.kv_pages is not None and pages_for(len(prompt) + max_tokens) > self.kv_pages:
+            raise ValueError(f"prompt + max_tokens needs {pages_for(len(prompt) + max_tokens)} KV pages, "
+                             f"the cache holds {self.kv_pages}")
         if not self.free:
             raise RuntimeError("no free cache slot")
+        if self.kv_pages is not None:
+            if pages_for(len(prompt) + max_tokens) > self.e.kv_pages_free():
+                raise CacheFull("KV cache full: too few free pages for this request now")
+            self.e.reserve(self.free[-1], len(prompt) + max_tokens)
         r = _Req(list(prompt), max_tokens, [], 0, self.free.pop(), False, float(temperature), float(top_p),
                  np.random.default_rng(seed) if temperature > 0 else None)
         self.active.append(r)
@@ -212,7 +269,12 @@ class Generator:
         groups: Dict[int, List[_Req]] = {}
         for r in pend:
             groups.setdefault((len(r.prompt) + 127) // 128, []).append(r)
-        for _, rs in sorted(groups.items()):
+        calls = []
+        for blocks, rs in sorted(groups.items()):
+            # paged: a call's n_seqs * padded_len stays within the prefill workspace the engine allocated
+            per_call = max(1, self.e.prefill_tokens // (blocks * 128)) if self.kv_pages is not None else len(rs)
+            calls += [rs[i:i + per_call] for i in range(0, len(rs), per_call)]
+        for rs in calls:
             need_logits = any(not r.greedy for r in rs)
             nxt, lg = self.e.prefill([r.prompt for r in rs], [r.slot for r in rs], want_logits=need_logits)
             if need_logits and lg is None:
@@ -232,12 +294,17 @@ class Generator:
         if r in self.active:
             r.done = True
             self.active.remove(r)
-            self.free.append(r.slot)
+            self._free_slot(r)
+
+    def _free_slot(self, r: _Req):
+        self.free.append(r.slot)
+        if self.kv_pages is not None:
+            self.e.release(r.slot)
 
     def _retire(self):
         for r in [r for r in self.active if r.done]:
             self.active.remove(r)
-            self.free.append(r.slot)
+            self._free_slot(r)
 
     def step(self):
         """One engine step for every active request."""

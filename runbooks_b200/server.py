@@ -90,29 +90,38 @@ class Scheduler(threading.Thread):
 
     def run(self):
         from ._lib import B200WError
+        from .infer import CacheFull
         self.ready.set()
         pending = {}
+        held = None     # paged KV cache: the head of the line, waiting for pages that running requests hold
         try:
             while True:
                 # admit as many queued requests as there are free slots; their prompts are then ingested together
                 # (one prefill call per padded length) before the next decode step
-                block = not self.gen.active
+                block = not self.gen.active and held is None
                 admitted = []
                 while self.gen.free:
-                    try:
-                        item = self.q.get(timeout=0.5 if block else 0)
-                    except queue.Empty:
-                        break
+                    if held is not None:
+                        item, held = held, None
+                    else:
+                        try:
+                            item = self.q.get(timeout=0.5 if block else 0)
+                        except queue.Empty:
+                            break
                     block = False
                     if item["cancelled"]:
                         continue
                     try:
-                        ids = self.tok.encode(item["prompt"])
-                        if self.tok.bos_id is not None:
-                            ids = [self.tok.bos_id] + ids
+                        if "ids" not in item:
+                            ids = self.tok.encode(item["prompt"])
+                            item["ids"] = [self.tok.bos_id] + ids if self.tok.bos_id is not None else ids
+                        ids = item["ids"]
                         req = self.gen.add(ids, item["max_tokens"], item["temperature"], item["top_p"], item["seed"],
                                            defer_prefill=True)
                         admitted.append((req, item, len(ids)))
+                    except CacheFull:       # fits the pool, not now: keep its place, retry after the next step
+                        held = item
+                        break
                     except Exception as e:  # noqa: BLE001 — per-request failure, the server lives on
                         item["events"].put(("error", str(e)))
                 if admitted:
@@ -310,13 +319,48 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
     return H
 
 
-def load_engine(model_dir: str, max_batch: int, max_ctx: int | None):
+def server_params(content: str, max_batch: int | None = None, kv_cache_gb: float | None = None,
+                  environ=None) -> tuple:
+    """(max_batch, kv_cache_gb) of the Server. A command-line value wins; otherwise the container contract's
+    params (/content/params.json, PARAM_<UPPER> overriding it, merged by contract.load_params); otherwise 32 slots
+    and the contiguous cache (kv_cache_gb None)."""
+    extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
+
+    def pick(cli, key, typ):
+        if cli is not None or key not in extra:
+            return cli
+        try:
+            return contract._coerce(extra[key], typ)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"param {key!r}: cannot read {extra[key]!r} as {typ.__name__}") from e
+    max_batch = pick(max_batch, "max_batch", int)
+    max_batch = 32 if max_batch is None else max_batch
+    kv_cache_gb = pick(kv_cache_gb, "kv_cache_gb", float)
+    if not 1 <= max_batch <= 128:
+        raise ValueError(f"max_batch must be in 1..128, got {max_batch}")
+    if kv_cache_gb is not None and not (kv_cache_gb > 0 and kv_cache_gb < float("inf")):
+        raise ValueError(f"kv_cache_gb must be a positive number of GB, got {kv_cache_gb}")
+    return max_batch, kv_cache_gb
+
+
+def kv_pages_for_gb(arch, kv_cache_gb: float) -> int:
+    """Pages of a paged KV cache of kv_cache_gb * 10^9 bytes; ValueError when that cannot hold one max_ctx request."""
+    from .infer import kv_page_bytes, pages_for
+    pages = int(kv_cache_gb * 1e9 // kv_page_bytes(arch))
+    if pages < pages_for(arch.max_ctx):
+        raise ValueError(f"kv_cache_gb {kv_cache_gb} holds {pages} pages of {kv_page_bytes(arch) / 1e6:.1f} MB; one "
+                         f"request of max_ctx {arch.max_ctx} needs {pages_for(arch.max_ctx)}")
+    return pages
+
+
+def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None):
     from .infer import InferEngine, ServeArch
 
     cfg = contract.read_hf_config(model_dir)
     arch = ServeArch.from_hf_config(cfg, max_ctx)
+    kv_pages = None if kv_cache_gb is None else kv_pages_for_gb(arch, kv_cache_gb)
     e = InferEngine(int(os.environ.get("B200W_DEVICE", "0")))
-    e.init_infer(arch, max_batch=max_batch)
+    e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages)
     wanted = {n for n, _ in e.infer_params()}
     seen, unused = set(), []
     for name, arr in contract.iter_safetensors(model_dir):
@@ -333,17 +377,22 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None):
     return e, cfg
 
 
-def serve(content: str, port: int, max_batch: int, max_ctx: int | None):
+def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None):
+    max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
     model_dir = os.path.join(content, "model")
     t0 = time.time()
-    engine, cfg = load_engine(model_dir, max_batch, max_ctx)
+    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb)
     tok = contract.Tokenizer(model_dir)
     sched = Scheduler(engine, tok)
     sched.start()
     name = cfg.get("_name_or_path") or cfg.get("model_type", "model")
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
-    print(json.dumps({"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
-                      "max_batch": max_batch}), flush=True)
+    ready = {"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
+             "max_batch": max_batch}
+    if engine.kv_pages is not None:
+        from .infer import kv_page_bytes
+        ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch) / 1e6, 2))
+    print(json.dumps(ready), flush=True)
     httpd.serve_forever()
 
 
@@ -351,11 +400,14 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="runbooks_b200.server")
     ap.add_argument("--content", default=contract.CONTENT)
     ap.add_argument("--port", type=int, default=8080)       # server_controller.go:156-161
-    ap.add_argument("--max-batch", type=int, default=32)
+    ap.add_argument("--max-batch", type=int, default=None, help="cache slots (default: param max_batch, else 32)")
     ap.add_argument("--max-ctx", type=int, default=None)
+    ap.add_argument("--kv-cache-gb", type=float, default=None,
+                    help="serve from a paged KV cache of this many GB (default: param kv_cache_gb, else a "
+                         "contiguous max_batch x max_ctx cache)")
     a = ap.parse_args(argv)
     try:
-        serve(a.content, a.port, a.max_batch, a.max_ctx)
+        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()

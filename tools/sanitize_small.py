@@ -80,3 +80,14 @@ ie.infer_init_random(0, 0.05)
 out = Generator(ie).generate([[1, 2, 3, 4, 5, 6, 7], [9, 8, 7]], 4)
 print("falcon serve ok:", out, flush=True)
 ie.close()
+# paged KV cache: reused pages out of order, both decode attention kernels (MQA: tensor cores; MHA: CUDA cores)
+for kv in (1, 4):
+    ie = InferEngine(0)
+    ie.init_infer(ServeArch("falcon", 512, 256, 1024, 2, 4, kv, 64, 256, 1e-5, 10000.0, True), max_batch=2, kv_pages=4,
+                  prefill_tokens=256)
+    ie.infer_init_random(0, 0.05)
+    g = Generator(ie)
+    first = g.generate([list(range(1, 140)), [9, 8, 7]], 3)
+    out = g.generate([list(range(3, 200))], 8)
+    print(f"paged serve (kv heads {kv}) ok:", first, out, flush=True)
+    ie.close()
