@@ -153,26 +153,24 @@ __global__ void gelu_strided_kernel(bf16* x, int T, int N, int ld) {
   *reinterpret_cast<uint4*>(x + t * ld + c) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// KV-cache layouts. Contiguous: a layer's cache is [max_batch][max_ctx] rows of kd elements. Paged
-// (b200w_infer_init_paged): a layer's cache is a pool of pages of KV_PAGE rows, and position p of a slot
-// lives in row table[slot][p / KV_PAGE] * KV_PAGE + p % KV_PAGE. A page is one 128-key block of the
-// tensor-core decode attention, so a block is always one TMA box inside one page.
+// KV-cache layout: a layer's cache is rows of kd elements, and the table [max_batch][nsplit] holds the first
+// cache row of each block of KV_PAGE positions of a slot, so position p of a slot lives in row
+// table[slot][p / KV_PAGE] + p % KV_PAGE. Contiguous (b200w_infer_init): [max_batch][max_ctx] rows and a table
+// fixed at init, entry j of slot s = s * max_ctx + j * KV_PAGE. Paged (b200w_infer_init_paged): a pool of pages
+// of KV_PAGE rows, entry j = KV_PAGE * (the slot's j-th page). A block is one 128-key block of the tensor-core
+// decode attention, so each block is one TMA box.
 constexpr int KV_PAGE = 128;
-template <bool PAGED>
-__device__ __forceinline__ size_t cache_row(int slot, int p, int max_ctx, const int32_t* __restrict__ table,
-                                            int tpages) {
-  if constexpr (PAGED) return static_cast<size_t>(table[slot * tpages + p / KV_PAGE]) * KV_PAGE + p % KV_PAGE;
-  else return static_cast<size_t>(slot) * max_ctx + p;
+// cache row of position p of the slot whose table row is `row` (a row index is below 2^31: 32-bit arithmetic)
+__device__ __forceinline__ size_t cache_row(const int32_t* __restrict__ row, unsigned p) {
+  return static_cast<unsigned>(row[p / KV_PAGE]) + p % KV_PAGE;
 }
 
 // Decode: rotate_half RoPE on the q heads (in place) and on k (rope != 0; OPT has none); k and v are
 // written into the cache at [slot][pos]. One thread per (row, head, pair index).
-template <bool PAGED>
 __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* __restrict__ inv_freq,
                                    const int32_t* __restrict__ pos, const int32_t* __restrict__ slot,
                                    bf16* __restrict__ kcache, bf16* __restrict__ vcache, int n, int H,
-                                   int Hkv, int dh, int max_ctx, int rope, const int32_t* __restrict__ table,
-                                   int tpages) {
+                                   int Hkv, int dh, int rope, const int32_t* __restrict__ table, int nsplit) {
   pdl_trigger();
   pdl_wait();
   const int half = dh / 2;
@@ -196,7 +194,7 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* 
     }
   } else {
     const int hk = h - H;
-    const size_t off = (cache_row<PAGED>(slot[r], p, max_ctx, table, tpages) * Hkv + hk) * dh;
+    const size_t off = (cache_row(table + slot[r] * nsplit, p) * Hkv + hk) * dh;
     kcache[off + i] = o1;
     kcache[off + i + half] = o2;
     const bf16* vsrc = qkv + static_cast<size_t>(r) * ld + (H + Hkv + hk) * dh;
@@ -208,13 +206,12 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* 
 // Prefill: token t = b * S + p of sequence b. q / k (rotated when rope != 0) and v go to the attention
 // input `dst` [T, (H + 2 Hkv) * dhp] (heads at stride dhp >= dh; the padding columns are zero from
 // allocation and never written) and, for real positions p < len[b], k / v also into cache slot[b].
-template <bool PAGED>
 __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
                                             int ld_dst, const float* __restrict__ inv_freq,
                                             const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
                                             bf16* __restrict__ kcache, bf16* __restrict__ vcache, int T, int S,
-                                            int H, int Hkv, int dh, int dhp, int max_ctx, int rope,
-                                            const int32_t* __restrict__ table, int tpages) {
+                                            int H, int Hkv, int dh, int dhp, int rope,
+                                            const int32_t* __restrict__ table, int nsplit) {
   const int half = dh / 2, HT = H + 2 * Hkv;
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(T) * HT * half;
@@ -238,7 +235,7 @@ __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld
   if (h >= H && p < lens[b]) {
     const bool is_k = h < H + Hkv;
     const int hk = is_k ? h - H : h - H - Hkv;
-    const size_t off = (cache_row<PAGED>(slot[b], p, max_ctx, table, tpages) * Hkv + hk) * dh;
+    const size_t off = (cache_row(table + slot[b] * nsplit, p) * Hkv + hk) * dh;
     bf16* c = is_k ? kcache : vcache;
     c[off + i] = o1;
     c[off + i + half] = o2;
@@ -271,12 +268,12 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* 
 // group of GT query heads that share that kv head): every K/V row is read once per block.
 constexpr int ATT_GT = 8;
 constexpr int ATT_THREADS = 256;
-template <int DH, bool PAGED>
+template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS)
 decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache,
                    const bf16* __restrict__ vcache, const int32_t* __restrict__ pos,
                    const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
-                   int max_ctx, int sc_stride, float scale, const int32_t* __restrict__ table, int tpages) {
+                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit) {
   extern __shared__ float sm[];
   pdl_trigger();
   pdl_wait();
@@ -293,15 +290,10 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
     sq[g * DH + c] = __bfloat162float(qkv[static_cast<size_t>(r) * ld + (hk * G + g0 + g) * DH + c]) * scale;
   }
   __syncthreads();
-  const size_t cbase = static_cast<size_t>(slot[r]) * max_ctx;   // contiguous
-  const int32_t* prow = table + slot[r] * tpages;                 // paged: the slot's page-table row
-  auto crow = [&](int t) -> size_t {                              // cache row of key position t
-    if constexpr (PAGED) return static_cast<size_t>(prow[t / KV_PAGE]) * KV_PAGE + t % KV_PAGE;
-    else return cbase + t;
-  };
+  const int32_t* prow = table + slot[r] * nsplit;   // the slot's table row
   // scores: one key position per thread, the K row lives in registers for all ng heads
   for (int t = tid; t < len; t += ATT_THREADS) {
-    const uint4* krow = reinterpret_cast<const uint4*>(kcache + (crow(t) * Hkv + hk) * DH);
+    const uint4* krow = reinterpret_cast<const uint4*>(kcache + (cache_row(prow, t) * Hkv + hk) * DH);
     float acc[ATT_GT];
 #pragma unroll
     for (int g = 0; g < ATT_GT; ++g) acc[g] = 0.f;
@@ -352,7 +344,7 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int t = t0 + u * SLICES;
-      vv[u] = t < len ? *reinterpret_cast<const uint4*>(vcache + (crow(t) * Hkv + hk) * DH + dg * 8)
+      vv[u] = t < len ? *reinterpret_cast<const uint4*>(vcache + (cache_row(prow, t) * Hkv + hk) * DH + dg * 8)
                       : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
@@ -417,13 +409,12 @@ __device__ __forceinline__ float ex2f(float x) {
 }
 
 static_assert(TC_KB == KV_PAGE, "a key block of the tensor-core decode attention is one cache page");
-template <int DH, bool PAGED>
+template <int DH>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                       const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
                       const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
-                      int H, int Hkv, int max_ctx, int nsplit, float scale_log2, const int32_t* __restrict__ table,
-                      int tpages) {
+                      int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table) {
   constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
   const int split = blockIdx.x, hk = blockIdx.y, r = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31;
@@ -450,8 +441,7 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
   }
   __syncthreads();
   if (tid == 0) {
-    // first cache row of this block (paged: the first row of page `split` of the slot)
-    const int row0 = PAGED ? table[slot[r] * tpages + split] * KV_PAGE : slot[r] * max_ctx + k0;
+    const int row0 = table[slot[r] * nsplit + split];   // first cache row of this block
     mbar_arrive_expect_tx(bar_kv, 2 * NA * TC_ATOM);
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
@@ -662,10 +652,10 @@ struct Infer {
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
   bf16 *kc = nullptr, *vc = nullptr;  // [L][layer_rows()][Hkv*dh], zero-initialised
-  // paged layout (n_pages > 0): page table [max_batch][tpages] on the device, written from pinned staging by
-  // b200w_infer_reserve; `held` is its host mirror (the pages a slot owns, in table order), `free_pages` a
-  // LIFO stack of the others
-  int n_pages = 0, tpages = 0;
+  // the table [max_batch][nsplit] of first cache rows (KV_PAGE above) on the device, written from pinned staging:
+  // once at init when contiguous, by b200w_infer_reserve when paged (n_pages > 0). Paged: `held` mirrors it on the
+  // host (the pages a slot owns, in table order), `free_pages` is a LIFO stack of the others
+  int n_pages = 0;
   int32_t* table = nullptr;
   int32_t* table_pin = nullptr;
   std::vector<int32_t> free_pages;
@@ -882,13 +872,27 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
   m->tiled_valid = true;
 }
 
+// the tensor-core decode attention and the merge of its blocks -> out [n, ldo]
+template <int DH>
+void decode_attention_tc(Infer* m, cudaStream_t s, int n, const CUtensorMap& tk, const CUtensorMap& tv,
+                         float scale_log2, bf16* out, int ldo) {
+  const int H = m->a.num_heads, Hkv = m->a.num_kv_heads;
+  static PerDeviceOnce once;
+  once.run([&] {
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<DH>()));
+  });
+  launch_pdl(decode_attn_tc_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), tc_smem_bytes<DH>(), s, tk, tv,
+             m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table);
+  launch_pdl(decode_attn_merge_kernel<DH>, dim3(cdiv(H, 256 / DH), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
+             out, ldo, H, m->nsplit);
+}
+
 // attention of the n new tokens over their cache slots -> out [n, ldo]
 void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int ldo, int64_t& nl) {
   const auto& a = m->a;
   const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, G = H / Hkv;
   const float scale = 1.f / sqrtf(static_cast<float>(dh));
   const uint64_t rows = m->layer_rows();
-  const bool paged = m->n_pages > 0;
   bf16* kc = m->kc + layer * rows * m->kd;
   bf16* vc = m->vc + layer * rows * m->kd;
   if (G >= 4) {
@@ -896,30 +900,8 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
     CUtensorMap tk = make_tmap_bf16_2d(kc, rows, m->kd, m->kd, TC_KB, 64);
     CUtensorMap tv = make_tmap_bf16_2d(vc, rows, m->kd, m->kd, TC_KB, 64);
     const float scale_log2 = scale * 1.4426950408889634f;
-    const dim3 grid(m->nsplit, Hkv, n);
-    if (dh == 64) {
-      static PerDeviceOnce once;
-      once.run([&] {
-        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<64>()));
-        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<64>()));
-      });
-      launch_pdl(paged ? decode_attn_tc_kernel<64, true> : decode_attn_tc_kernel<64, false>, grid, dim3(TC_THREADS),
-                 tc_smem_bytes<64>(), s, tk, tv, m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv,
-                 a.max_ctx, m->nsplit, scale_log2, m->table, m->tpages);
-      launch_pdl(decode_attn_merge_kernel<64>, dim3(cdiv(H, 4), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
-                 out, ldo, H, m->nsplit);
-    } else {
-      static PerDeviceOnce once;
-      once.run([&] {
-        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<128>()));
-        B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<128>()));
-      });
-      launch_pdl(paged ? decode_attn_tc_kernel<128, true> : decode_attn_tc_kernel<128, false>, grid, dim3(TC_THREADS),
-                 tc_smem_bytes<128>(), s, tk, tv, m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv,
-                 a.max_ctx, m->nsplit, scale_log2, m->table, m->tpages);
-      launch_pdl(decode_attn_merge_kernel<128>, dim3(cdiv(H, 2), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
-                 out, ldo, H, m->nsplit);
-    }
+    if (dh == 64) decode_attention_tc<64>(m, s, n, tk, tv, scale_log2, out, ldo);
+    else decode_attention_tc<128>(m, s, n, tk, tv, scale_log2, out, ldo);
     nl += 2;
     return;
   }
@@ -930,15 +912,11 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
   B200W_CHECK(att_smem <= 200 * 1024, "max_ctx too large for the decode attention kernel");
   static PerDeviceOnce once;
   once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   });
-  auto kern = dh == 64 ? (paged ? decode_attn_kernel<64, true> : decode_attn_kernel<64, false>)
-                       : (paged ? decode_attn_kernel<128, true> : decode_attn_kernel<128, false>);
-  launch_pdl(kern, agrid, dim3(ATT_THREADS), att_smem, s, m->qkv, m->qkvd, kc, vc, m->pos, m->slot, out, ldo, H, Hkv,
-             a.max_ctx, sc_stride, scale, m->table, m->tpages);
+  launch_pdl(dh == 64 ? decode_attn_kernel<64> : decode_attn_kernel<128>, agrid, dim3(ATT_THREADS), att_smem, s,
+             m->qkv, m->qkvd, kc, vc, m->pos, m->slot, out, ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit);
   ++nl;
 }
 
@@ -955,7 +933,6 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   const int qd = m->qd, qkvd = m->qkvd;
   const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
   const size_t layer_cache = m->layer_rows() * m->kd;
-  auto rope_append = m->n_pages ? rope_append_kernel<true> : rope_append_kernel<false>;
   B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin + B, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin + 2 * B, n * 4, cudaMemcpyHostToDevice, s));
@@ -978,8 +955,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       o1.out2 = m->cat + qd; o1.ldo2 = m->ld_cat; o1.n_split = qkvd;
       o1.act = 1; o1.act_from = qkvd;   // exact GeLU on the MLP half only
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd + f, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1, m->table, m->tpages); ++nl;
+      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, 1, m->table, m->nsplit); ++nl;
       decode_attention(m, s, n, l, m->cat, m->ld_cat, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -990,8 +967,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd; o1.bias = m->w + p.bqkv;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 0, m->table, m->tpages); ++nl;
+      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, 0, m->table, m->nsplit); ++nl;
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d; o2.bias = m->w + p.bo;
@@ -1008,8 +985,8 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, a.max_ctx, 1, m->table, m->tpages); ++nl;
+      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
+                 kc, vc, n, H, Hkv, dh, 1, m->table, m->nsplit); ++nl;
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -1112,8 +1089,9 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   if (arch->family == B200W_FAMILY_OPT)
     B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
   const int64_t ctx_rounded = cdiv(arch->max_ctx, KV_PAGE) * static_cast<int64_t>(KV_PAGE);
+  // a table entry is an int32 TMA row coordinate: at most (2^24 - 1) * 128 paged, below 128 * 8192 contiguous
+  // (max_batch <= 128, max_ctx <= 8192)
   if (n_pages) {
-    // a page index times KV_PAGE is an int32 TMA row coordinate
     B200W_CHECK(n_pages >= 1 && n_pages <= (1 << 24), "n_pages must be in 1..2^24");
     B200W_CHECK(prefill_tokens >= ctx_rounded && prefill_tokens <= (1 << 20),
                 "prefill_tokens must be in [max_ctx rounded up to 128, 2^20]");
@@ -1146,13 +1124,17 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
   B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
   m->nsplit = (a.max_ctx + TC_KB - 1) / TC_KB;
+  const size_t tab = B * m->nsplit;
+  m->table = m->alloc<int32_t>(tab);
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->table_pin), tab * sizeof(int32_t)));
+  // contiguous: block j of slot s starts at row s * max_ctx + j * KV_PAGE for the context's life (when max_ctx is
+  // not a multiple of KV_PAGE, a slot's last block runs into the next slot's rows, or past the end of the cache
+  // where TMA fills zeros; the attention weights those keys by 0). Paged: no slot holds a page yet, entries 0.
+  for (size_t s = 0; s < B; ++s)
+    for (int j = 0; j < m->nsplit; ++j)
+      m->table_pin[s * m->nsplit + j] = n_pages ? 0 : static_cast<int32_t>(s * a.max_ctx + j * KV_PAGE);
+  B200W_CUDA(cudaMemcpy(m->table, m->table_pin, tab * sizeof(int32_t), cudaMemcpyHostToDevice));
   if (n_pages) {
-    m->tpages = m->nsplit;
-    const size_t tab = B * m->tpages;
-    m->table = m->alloc<int32_t>(tab);
-    B200W_CUDA(cudaMemset(m->table, 0, tab * sizeof(int32_t)));
-    B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->table_pin), tab * sizeof(int32_t)));
-    memset(m->table_pin, 0, tab * sizeof(int32_t));
     for (int p = n_pages - 1; p >= 0; --p) m->free_pages.push_back(p);   // page 0 is handed out first
     m->held.assign(B, {});
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
@@ -1223,10 +1205,10 @@ int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens) {
     }
     // the row goes to the device on the library stream, so it lands before the next step or prefill; the
     // table's address never changes, so the captured decode graphs read the new row
-    int32_t* row = m->table_pin + static_cast<size_t>(slot) * m->tpages;
-    std::copy(h.begin(), h.end(), row);
-    std::fill(row + h.size(), row + m->tpages, 0);
-    B200W_CUDA(cudaMemcpyAsync(m->table + static_cast<size_t>(slot) * m->tpages, row, m->tpages * sizeof(int32_t),
+    int32_t* row = m->table_pin + static_cast<size_t>(slot) * m->nsplit;
+    std::transform(h.begin(), h.end(), row, [](int32_t page) { return page * KV_PAGE; });
+    std::fill(row + h.size(), row + m->nsplit, 0);
+    B200W_CUDA(cudaMemcpyAsync(m->table + static_cast<size_t>(slot) * m->nsplit, row, m->nsplit * sizeof(int32_t),
                                cudaMemcpyHostToDevice, ctx_stream(ctx)));
   });
   return st == B200W_OK && short_of_pages ? B200W_ERR_OOM : st;
@@ -1445,8 +1427,7 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     const bool padded = dh != dhp;
     const float scale = 1.f / sqrtf(static_cast<float>(dh));
     const size_t layer_cache = m->layer_rows() * m->kd;
-    auto scatter = m->n_pages ? prefill_rope_scatter_kernel<true> : prefill_rope_scatter_kernel<false>;
-    const int Ti = static_cast<int>(T);
+      const int Ti = static_cast<int>(T);
     auto G = [&](const void* A, int lda, size_t woff, int ldw, void* D, const void* C, int ldd, int N, int K,
                  const void* bias = nullptr, int act = 0) {
       gemm_bf16_ex(A, false, lda, m->w + woff, false, ldw, D, C, false, ldd, Ti, N, K, 0, bias, act, s); ++nl;
@@ -1470,8 +1451,9 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
       bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
       const int ld_in = padded ? HT * dhp : qkvd;
       const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
-      scatter<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq, m->pf_len, m->pf_slot, kc, vc,
-                                            Ti, S, H, Hkv, dh, dhp, a.max_ctx, opt ? 0 : 1, m->table, m->tpages); ++nl;
+      prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq, m->pf_len,
+                                                                m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dhp, opt ? 0 : 1,
+                                                                m->table, m->nsplit); ++nl;
       B200W_CUDA(cudaGetLastError());
       bf16* att_out = padded ? m->pf_attp : m->pf_cat;
       const int ld_out = padded ? H * dhp : ldc;

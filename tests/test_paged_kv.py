@@ -65,9 +65,12 @@ class Pair:
         return a
 
 
-@pytest.mark.parametrize("name", list(MODELS))
-def test_paged_equals_contiguous_bit_for_bit(name):
-    arch = _arch(name)
+# max_ctx 500: a contiguous slot's blocks of 128 positions start off a multiple of 128, and its last block runs into
+# the next slot's rows (the last slot's past the end of the cache)
+@pytest.mark.parametrize("name,max_ctx", [pytest.param(n, c, id=n if c == 512 else f"{n}-max_ctx{c}")
+                                          for c in (512, 500) for n in MODELS])
+def test_paged_equals_contiguous_bit_for_bit(name, max_ctx):
+    arch = _arch(name, max_ctx)
     rng = np.random.default_rng(11)
     V = arch.vocab_size
     x = Pair(arch, kv_pages=12)          # 12 pages; the contiguous cache holds 4 x 4
@@ -91,7 +94,7 @@ def test_paged_equals_contiguous_bit_for_bit(name):
         pos = [p + 1 for p in pos]
     reused = x.p.slot_pages(1)
     earlier = set(first_owners[1]) | set(first_owners[2])
-    print(f"{name}: {x.checked} calls bit-identical; slot 1 pages {first_owners[1]} -> {reused}, "
+    print(f"{name}, max_ctx {max_ctx}: {x.checked} calls bit-identical; slot 1 pages {first_owners[1]} -> {reused}, "
           f"free {x.p.kv_pages_free()} of 12")
     assert reused != sorted(reused) and set(reused) & earlier
     x.c.close()
