@@ -246,6 +246,30 @@ B200W_API int b200w_infer_kv_pages(b200w_ctx* ctx, int64_t* total, int64_t* free
 /* Test aid: the pages `slot` holds, in position order, into out[0 .. cap). Returns their count (>= 0) or a
  * negative B200W_ERR_*. */
 B200W_API int b200w_infer_slot_pages(b200w_ctx* ctx, int slot, int32_t* out, int cap);
+/* Prefix sharing on the paged cache. A page holds one reference per slot whose table names it, plus those the host
+ * index retains; it returns to the free list when its count reaches 0 (b200w_infer_kv_pages counts those).
+ * reserve_shared: releases what `slot` holds, then its first n_shared table entries become shared_pages[0 ..
+ * n_shared) (each gains a reference and must keep at least one besides the slot's own: a free page is
+ * B200W_ERR_INVALID) and the other ceil(n_tokens / 128) - n_shared come from the free list. B200W_ERR_OOM when too
+ * few pages are free; nothing changes then. The slot's write floor becomes n_shared * 128: a step or a prefill that
+ * writes K/V below it is B200W_ERR_INVALID, so a shared page is never written through a slot that borrowed it.
+ * b200w_infer_reserve is this call with n_shared = 0. */
+B200W_API int b200w_infer_reserve_shared(b200w_ctx* ctx, int slot, int n_tokens, const int32_t* shared_pages,
+                                         int n_shared);
+/* The host index's references: delta +1 retains pages[0 .. n) (each must already hold a reference), -1 drops
+ * references retained before. Anything else is B200W_ERR_INVALID and changes nothing. While any page is retained,
+ * b200w_infer_load_tensor and b200w_infer_init_random return B200W_ERR_STATE: cached K/V belong to the weights that
+ * computed them. reserve_shared and retain_pages return B200W_ERR_STATE on a contiguous cache. */
+B200W_API int b200w_infer_retain_pages(b200w_ctx* ctx, const int32_t* pages, int n, int delta);
+/* b200w_infer_prefill after a cached prefix: row b of tokens [n_seqs, padded_len] holds the prompt's positions
+ * starts[b] .. lengths[b] - 1, whose K/V this call writes; the K/V of positions [0, starts[b]) are already in the
+ * slot's pages. starts[b] is a multiple of 128 with 0 < starts[b] < lengths[b], lengths[b] - starts[b] <=
+ * padded_len; otherwise as b200w_infer_prefill (same outputs, same prefill_tokens limit). Paged cache only
+ * (B200W_ERR_STATE on a contiguous one). The suffix attends through the page table with a dedicated sm_90a flash
+ * attention kernel. */
+B200W_API int b200w_infer_prefill_cached(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts,
+                                         const int32_t* lengths, const int32_t* slots, int n_seqs, int padded_len,
+                                         int32_t* next_tokens, float* logits_out);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.
@@ -301,6 +325,16 @@ B200W_API int b200w_op_ce(b200w_ctx* ctx, void* logits, const int32_t* labels, f
 B200W_API int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            void* out, int ld_out, float* lse2, int B, int S, int H, int Hkv,
                            float scale);
+/* The attention of b200w_infer_prefill_cached on its own. q [n_seqs * S, ld_q]: sequence b's rows are its positions
+ * starts[b] + p, head h at column h * q_head_stride (its first dh columns used). kcache / vcache [cache_rows,
+ * Hkv * dh] hold position t of sequence b at row table[slots[b] * nsplit + t / 128] + t % 128. out [n_seqs * S,
+ * ld_out], head h at column h * dh. slots, starts, lengths: DEVICE int32 [n_seqs]; starts[b] a multiple of 128 below
+ * lengths[b]; the table rows of positions [0, lengths[b]) must lie inside the cache (not validated). dh 64 or 128. */
+B200W_API int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride,
+                                            const void* kcache, const void* vcache, int64_t cache_rows,
+                                            const int32_t* table, int nsplit, const int32_t* slots,
+                                            const int32_t* starts, const int32_t* lengths, void* out, int ld_out,
+                                            int n_seqs, int S, int H, int Hkv, int dh, float scale);
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);

@@ -92,6 +92,9 @@ PROTOTYPES = {
     "b200w_infer_release": (C.c_int, [c_ctx, C.c_int]),
     "b200w_infer_kv_pages": (C.c_int, [c_ctx, i64p, i64p]),
     "b200w_infer_slot_pages": (C.c_int, [c_ctx, C.c_int, vp, C.c_int]),
+    "b200w_infer_reserve_shared": (C.c_int, [c_ctx, C.c_int, C.c_int, vp, C.c_int]),
+    "b200w_infer_retain_pages": (C.c_int, [c_ctx, vp, C.c_int, C.c_int]),
+    "b200w_infer_prefill_cached": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
@@ -118,6 +121,9 @@ PROTOTYPES = {
     "b200w_op_ce": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp,
                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
+    "b200w_op_attention_fwd_cached": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
+                                                vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                C.c_float]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,

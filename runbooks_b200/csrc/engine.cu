@@ -1921,6 +1921,13 @@ int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_of
                            float scale) {
   HOOK(attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx->stream));
 }
+int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
+                                  const void* vcache, int64_t cache_rows, const int32_t* table, int nsplit,
+                                  const int32_t* slots, const int32_t* starts, const int32_t* lengths, void* out,
+                                  int ld_out, int n_seqs, int S, int H, int Hkv, int dh, float scale) {
+  HOOK(attention_fwd_cached(q, ld_q, q_head_stride, kcache, vcache, cache_rows, table, nsplit, slots, starts, lengths,
+                            out, ld_out, n_seqs, S, H, Hkv, dh, scale, ctx->stream));
+}
 int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {

@@ -203,15 +203,17 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* 
   }
 }
 
-// Prefill: token t = b * S + p of sequence b. q / k (rotated when rope != 0) and v go to the attention
-// input `dst` [T, (H + 2 Hkv) * dhp] (heads at stride dhp >= dh; the padding columns are zero from
-// allocation and never written) and, for real positions p < len[b], k / v also into cache slot[b].
+// Prefill: token t = b * S + p of sequence b, at position p + start[b] (start == nullptr: p). q / k (rotated when
+// rope != 0) and v go to the attention input `dst` [T, (H + 2 Hkv) * dhp] (heads at stride dhp >= dh; the padding
+// columns are zero from allocation and never written) and, for real positions < len[b], k / v also into cache
+// slot[b].
 __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
                                             int ld_dst, const float* __restrict__ inv_freq,
                                             const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
                                             bf16* __restrict__ kcache, bf16* __restrict__ vcache, int T, int S,
                                             int H, int Hkv, int dh, int dhp, int rope,
-                                            const int32_t* __restrict__ table, int nsplit) {
+                                            const int32_t* __restrict__ table, int nsplit,
+                                            const int32_t* __restrict__ start) {
   const int half = dh / 2, HT = H + 2 * Hkv;
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(T) * HT * half;
@@ -219,7 +221,7 @@ __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld
   const int i = static_cast<int>(idx % half);
   const int h = static_cast<int>((idx / half) % HT);
   const int t = static_cast<int>(idx / (static_cast<long long>(half) * HT));
-  const int b = t / S, p = t % S;
+  const int b = t / S, p = t % S + (start ? start[b] : 0);
   const bf16* x = src + static_cast<size_t>(t) * ld_src + h * dh;
   const float x1 = __bfloat162float(x[i]), x2 = __bfloat162float(x[i + half]);
   bf16 o1 = x[i], o2 = x[i + half];
@@ -579,6 +581,246 @@ __global__ void decode_attn_merge_kernel(const float* __restrict__ part_o, const
   out[static_cast<size_t>(r) * ldo + h * DH + d] = __float2bfloat16_rn(num / den);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Prefill after a cached prefix (b200w_infer_prefill_cached): causal flash attention whose queries are the suffix
+// rows of each sequence and whose keys and values all come from the paged cache (the suffix K/V were scattered
+// there earlier in the same layer). CTA = (128-query tile, query head, sequence), the structure of attn_fwd_kernel
+// (attention.cu): warpgroup 2 is the TMA producer (setmaxnreg.dec), warpgroups 0 and 1 own 64 query rows each.
+// Key block j is page j of the slot: one TMA box of K and one of V at row table[slot][j], in a ring of CA_STAGES
+// buffers with full / free mbarriers. start is a multiple of 128, so query tile i is exactly page start / 128 + i
+// and only a tile's last block needs the causal mask.
+//   S[64, 128] = Q K^T  (m64n128, both K-major from shared memory)
+//   P = 2^(S * scale_log2 - m) (exact online softmax), O = O * alpha + P V  (P from registers, V MN-major)
+// Block j's score product is issued ahead of block j - 1's P V, as in attn_fwd_kernel. A tile whose rows are all
+// padding walks the slot's pages up to ceil(len / 128) unmasked: finite values (the pool is zeroed at init) that
+// nothing reads.
+// ------------------------------------------------------------------------------------------------
+constexpr int CA_THREADS = 384, CA_STAGES = 2, CA_CONSUMER_WARPS = 8;
+constexpr int CA_PRODUCER_REGS = 24, CA_CONSUMER_REGS = 240;
+static_assert(128 * CA_PRODUCER_REGS + 256 * CA_CONSUMER_REGS <= 65536, "register budget of one CTA per SM");
+template <int DH>
+constexpr int ca_smem_bytes() { return (1 + 2 * CA_STAGES) * (DH / 64) * TC_ATOM + 1024 + 256; }
+
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+__device__ __forceinline__ void warp_release(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+
+template <int DH>
+__global__ void __launch_bounds__(CA_THREADS, 1)
+attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                       const __grid_constant__ CUtensorMap tm_v, int q_head_stride, bf16* __restrict__ out,
+                       int ld_out, const int32_t* __restrict__ table, int nsplit, const int32_t* __restrict__ slots,
+                       const int32_t* __restrict__ starts, const int32_t* __restrict__ lens, int n_seqs, int S,
+                       int H, int Hkv, float scale_log2) {
+  constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* sQ = smem;                            // NA atoms [128 query rows x 128 B]
+  uint8_t* sK = sQ + NA * TC_ATOM;               // CA_STAGES buffers x NA atoms [128 keys x 128 B]
+  uint8_t* sV = sK + CA_STAGES * NA * TC_ATOM;   // the same, read MN-major (N = dh)
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + CA_STAGES * NA * TC_ATOM);
+  uint64_t* bar_k = bar_q + 1;                   // [CA_STAGES]
+  uint64_t* bar_v = bar_k + CA_STAGES;           // [CA_STAGES]
+  uint64_t* bar_kfree = bar_v + CA_STAGES;       // [CA_STAGES] the S products that read K buffer b retired
+  uint64_t* bar_vfree = bar_kfree + CA_STAGES;   // [CA_STAGES] the P V products that read V buffer b retired
+
+  const int nbh = n_seqs * H;
+  const int qi = S / 128 - 1 - static_cast<int>(blockIdx.x) / nbh;   // longest tiles (most pages) first
+  const int h = static_cast<int>(blockIdx.x) % nbh % H, b = static_cast<int>(blockIdx.x) % nbh / H;
+  const int hk = h / (H / Hkv);
+  const int len = lens[b];
+  const int tile_page = starts[b] / KV_PAGE + qi;        // the page that holds this tile's query positions
+  const int npages = (len + KV_PAGE - 1) / KV_PAGE;
+  const bool diag = tile_page < npages;                   // the tile holds real rows: its last block is masked
+  const int nkb = diag ? tile_page + 1 : npages;          // key blocks (pages) [0, nkb)
+  const int32_t* prow = table + static_cast<size_t>(slots[b]) * nsplit;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm_q);
+    tma_prefetch_desc(&tm_k);
+    tma_prefetch_desc(&tm_v);
+    mbar_init(bar_q, 1);
+    for (int i = 0; i < CA_STAGES; ++i) {
+      mbar_init(&bar_k[i], 1);
+      mbar_init(&bar_v[i], 1);
+      mbar_init(&bar_kfree[i], CA_CONSUMER_WARPS);
+      mbar_init(&bar_vfree[i], CA_CONSUMER_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >> 2 == 2) {
+    setmaxnreg_dec<CA_PRODUCER_REGS>();
+    if (tid == 256) {
+      mbar_arrive_expect_tx(bar_q, NA * TC_ATOM);
+#pragma unroll
+      for (int a = 0; a < NA; ++a)
+        tma_load_2d(sQ + a * TC_ATOM, &tm_q, bar_q, h * q_head_stride + a * 64, b * S + qi * 128);
+      for (int j = 0; j < nkb; ++j) {
+        const int buf = j % CA_STAGES;
+        const uint32_t free_par = (j / CA_STAGES - 1) & 1;
+        const int row0 = prow[j];
+        if (j >= CA_STAGES) mbar_wait(&bar_kfree[buf], free_par);
+        mbar_arrive_expect_tx(&bar_k[buf], NA * TC_ATOM);
+#pragma unroll
+        for (int a = 0; a < NA; ++a)
+          tma_load_2d(sK + (buf * NA + a) * TC_ATOM, &tm_k, &bar_k[buf], hk * DH + a * 64, row0);
+        if (j >= CA_STAGES) mbar_wait(&bar_vfree[buf], free_par);
+        mbar_arrive_expect_tx(&bar_v[buf], NA * TC_ATOM);
+#pragma unroll
+        for (int a = 0; a < NA; ++a)
+          tma_load_2d(sV + (buf * NA + a) * TC_ATOM, &tm_v, &bar_v[buf], hk * DH + a * 64, row0);
+      }
+    }
+    return;
+  }
+
+  // =============================== consumers ===============================
+  // A page is taken in SUB sub-blocks of KB keys: at dh 128 the whole page's scores (64 registers), their bf16
+  // fragments and O do not fit the 168 registers ptxas gives a 384-thread CTA, so the scores are two m64n64 halves.
+  // Sub-block u is keys [KB (u % SUB), KB (u % SUB + 1)) of page u / SUB.
+  constexpr int KB = DH == 64 ? KV_PAGE : KV_PAGE / 2, SUB = KV_PAGE / KB;
+  setmaxnreg_inc<CA_CONSUMER_REGS>();
+  const int wg = warp >> 2, wi = warp & 3;
+  const int r0 = wg * 64 + wi * 16 + (lane >> 2), r1 = r0 + 8;   // this thread's rows inside the tile
+  const int c0 = 2 * (lane & 3);
+  const uint64_t dq = wg_desc(smem_u32(sQ) + wg * 64 * 128, 16);
+  float o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f, alpha0, alpha1;
+  float s[KB / 2];
+  uint32_t pa[KB / 16][4];
+  auto issue_scores = [&](int u) {
+    const uint64_t dk = wg_desc(smem_u32(sK + (u / SUB) % CA_STAGES * NA * TC_ATOM) + (u % SUB) * KB * 128, 16);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < DH / 16; ++kk)  // over dh: 32 B steps inside an atom row, then the next atom
+      Wgmma<KB>::template ss<0, 0>(s, desc_add(dq, (kk / 4) * TC_ATOM + (kk % 4) * 32),
+                                   desc_add(dk, (kk / 4) * TC_ATOM + (kk % 4) * 32), kk != 0);
+    wg_commit();
+  };
+  auto issue_pv = [&](int u) {
+    const uint64_t dv =
+        wg_desc(smem_u32(sV + (u / SUB) % CA_STAGES * NA * TC_ATOM) + (u % SUB) * KB * 128, TC_ATOM);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < KB / 16; ++kk)  // over the keys: 16 key rows = 2048 B
+      Wgmma<DH>::template rs<1>(o, pa[kk], desc_add(dv, kk * 2048), 1u);
+    wg_commit();
+  };
+  // online softmax of sub-block u's scores in s: P in s, O's rescale in alpha
+  auto softmax = [&](int u) {
+    if (diag && u / SUB == nkb - 1) {   // the tile's own page: key column c is visible to row r iff c <= r
+      const int cb = (u % SUB) * KB + c0;
+#pragma unroll
+      for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = cb + 8 * jj + e;
+          if (col > r0) s[4 * jj + e] = -INFINITY;
+          if (col > r1) s[4 * jj + 2 + e] = -INFINITY;
+        }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < KB / 8; ++jj) {
+      mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+      mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
+    }
+    // scale > 0 commutes with max; key 0 of block 0 is visible to every row, so m is finite from block 0 on
+    const float mn0 = fmaxf(m0, quad_max(mx0) * scale_log2), mn1 = fmaxf(m1, quad_max(mx1) * scale_log2);
+    alpha0 = ex2f(m0 - mn0);
+    alpha1 = ex2f(m1 - mn1);
+    m0 = mn0;
+    m1 = mn1;
+    float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < KB / 8; ++jj) {
+      s[4 * jj] = ex2f(fmaf(s[4 * jj], scale_log2, -m0));
+      s[4 * jj + 1] = ex2f(fmaf(s[4 * jj + 1], scale_log2, -m0));
+      s[4 * jj + 2] = ex2f(fmaf(s[4 * jj + 2], scale_log2, -m1));
+      s[4 * jj + 3] = ex2f(fmaf(s[4 * jj + 3], scale_log2, -m1));
+      ps0 += s[4 * jj] + s[4 * jj + 1];
+      ps1 += s[4 * jj + 2] + s[4 * jj + 3];
+    }
+    l0 = l0 * alpha0 + ps0;  // this thread's part of the row sums
+    l1 = l1 * alpha1 + ps1;
+  };
+  auto to_pa = [&] {  // fp32 P columns [16 kk, 16 kk + 16) -> the bf16 A fragment of the kk-th K = 16 slice
+#pragma unroll
+    for (int kk = 0; kk < KB / 16; ++kk)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) pa[kk][q] = pack_bf16x2(s[8 * kk + 2 * q], s[8 * kk + 2 * q + 1]);
+  };
+  // the full barrier of sub-block u's page (waiting again on a completed phase returns at once: the buffer is not
+  // refilled before every sub-block of its page released it)
+  auto wait_full = [&](uint64_t* bars, int u) {
+    mbar_wait(&bars[(u / SUB) % CA_STAGES], (u / SUB / CA_STAGES) & 1);
+  };
+  // after sub-block u's product that reads `frees`' buffer retired: the page's last sub-block releases it
+  auto release = [&](uint64_t* frees, int u) {
+    if (u % SUB == SUB - 1) warp_release(&frees[(u / SUB) % CA_STAGES]);
+  };
+
+  const int nsub = nkb * SUB;
+  mbar_wait(bar_q, 0);
+  wait_full(bar_k, 0);
+  issue_scores(0);
+  wg_wait<0>();
+  wg_fence_regs(s);
+  release(bar_kfree, 0);
+  softmax(0);  // O is still 0: its rescale is a no-op
+  to_pa();
+  for (int u = 1; u < nsub; ++u) {
+    wait_full(bar_k, u);
+    issue_scores(u);
+    wait_full(bar_v, u - 1);
+    issue_pv(u - 1);
+    wg_wait<1>();  // S(u) retired; PV(u - 1) may still run
+    wg_fence_regs(s);
+    release(bar_kfree, u);
+    softmax(u);
+    wg_wait<0>();  // PV(u - 1) retired: O may be rescaled, pa rewritten and V(u - 1) released
+    wg_fence_regs(o);
+    release(bar_vfree, u - 1);
+    to_pa();
+#pragma unroll
+    for (int jj = 0; jj < DH / 8; ++jj) {
+      o[4 * jj] *= alpha0;
+      o[4 * jj + 1] *= alpha0;
+      o[4 * jj + 2] *= alpha1;
+      o[4 * jj + 3] *= alpha1;
+    }
+  }
+  wait_full(bar_v, nsub - 1);
+  issue_pv(nsub - 1);
+  wg_wait<0>();
+  wg_fence_regs(o);
+  release(bar_vfree, nsub - 1);
+
+  const float inv0 = 1.f / quad_sum(l0), inv1 = 1.f / quad_sum(l1);
+  bf16* orow0 = out + static_cast<size_t>(b * S + qi * 128 + r0) * ld_out + h * DH + c0;
+  bf16* orow1 = orow0 + static_cast<size_t>(8) * ld_out;
+#pragma unroll
+  for (int jj = 0; jj < DH / 8; ++jj) {
+    *reinterpret_cast<uint32_t*>(orow0 + 8 * jj) = pack_bf16x2(o[4 * jj] * inv0, o[4 * jj + 1] * inv0);
+    *reinterpret_cast<uint32_t*>(orow1 + 8 * jj) = pack_bf16x2(o[4 * jj + 2] * inv1, o[4 * jj + 3] * inv1);
+  }
+}
+
 // greedy token: first index of the row maximum (torch.argmax tie-breaking)
 __global__ void argmax_kernel(const bf16* __restrict__ logits, int V, int32_t* __restrict__ out) {
   __shared__ float sv[32];
@@ -660,6 +902,11 @@ struct Infer {
   int32_t* table_pin = nullptr;
   std::vector<int32_t> free_pages;
   std::vector<std::vector<int32_t>> held;
+  // paged: references of each page (one per table entry of a slot that holds it, plus the host index's, which
+  // index_refs counts; `retained` is their sum); a page is on the free list iff refs == 0. floor[slot]: the first
+  // position the slot may write, n_shared * KV_PAGE (b200w_infer_reserve_shared)
+  std::vector<int32_t> refs, index_refs, floor;
+  int64_t retained = 0;
   size_t pf_limit = 0;  // paged: tokens of the preallocated prefill workspace, the most one prefill call takes
   size_t layer_rows() const {
     return n_pages ? static_cast<size_t>(n_pages) * KV_PAGE : static_cast<size_t>(max_batch) * a.max_ctx;
@@ -679,7 +926,8 @@ struct Infer {
   bf16 *pf_h = nullptr, *pf_h2 = nullptr, *pf_nrm = nullptr, *pf_qkv = nullptr, *pf_qkvp = nullptr,
        *pf_attp = nullptr, *pf_cat = nullptr, *pf_mid = nullptr, *pf_act = nullptr;
   float* pf_lse = nullptr;
-  int32_t *pf_tok = nullptr, *pf_len = nullptr, *pf_slot = nullptr, *pf_last = nullptr;
+  int32_t *pf_tok = nullptr, *pf_len = nullptr, *pf_slot = nullptr, *pf_last = nullptr, *pf_start = nullptr;
+  int32_t* pf_pos = nullptr;   // OPT after a cached prefix: the learned-position row of every token
   int32_t* pf_pin = nullptr;
   size_t pf_pin_cap = 0;
   std::vector<void*> allocs;
@@ -1022,7 +1270,7 @@ void ensure_prefill(Infer* m, size_t T) {
   for (void* p : {static_cast<void*>(m->pf_h), static_cast<void*>(m->pf_h2), static_cast<void*>(m->pf_nrm),
                   static_cast<void*>(m->pf_qkv), static_cast<void*>(m->pf_qkvp), static_cast<void*>(m->pf_attp),
                   static_cast<void*>(m->pf_cat), static_cast<void*>(m->pf_mid), static_cast<void*>(m->pf_act),
-                  static_cast<void*>(m->pf_lse), static_cast<void*>(m->pf_tok)})
+                  static_cast<void*>(m->pf_lse), static_cast<void*>(m->pf_tok), static_cast<void*>(m->pf_pos)})
     if (p) m->release(p);
   m->pf_h = m->alloc<bf16>(T * d);
   m->pf_h2 = m->alloc<bf16>(T * d);
@@ -1041,12 +1289,14 @@ void ensure_prefill(Infer* m, size_t T) {
   m->pf_act = a.family == B200W_FAMILY_LLAMA ? m->alloc<bf16>(T * f) : nullptr;
   m->pf_lse = m->alloc<float>(H * T);
   m->pf_tok = m->alloc<int32_t>(T);
+  m->pf_pos = m->alloc<int32_t>(T);
   m->pf_cap = T;
 }
 
-// pinned staging of one prefill call: tokens [T] | lengths | slots | last rows [max_batch each]
+// pinned staging of one prefill call: tokens [T] | lengths | slots | last rows | starts [max_batch each] |
+// positions [T]
 void ensure_prefill_pin(Infer* m, size_t T) {
-  const size_t need = T + 3 * static_cast<size_t>(m->max_batch);
+  const size_t need = 2 * T + 4 * static_cast<size_t>(m->max_batch);
   if (m->pf_pin_cap >= need) return;
   if (m->pf_pin) cudaFreeHost(m->pf_pin);
   m->pf_pin = nullptr;
@@ -1060,18 +1310,27 @@ Infer* paged_model(b200w_ctx* ctx) {
   return m;
 }
 
-// Paged mode: positions [0, n_tokens) of `slot` must lie in pages the slot holds (the host mirror of the table).
-void check_paged_slot(const Infer* m, int slot, long long n_tokens) {
+// Paged mode: positions [0, n_tokens) of `slot` must lie in pages the slot holds (the host mirror of the table), and
+// the call writes K/V from position `first_write` on, which must not lie in a page the slot shares.
+void check_paged_slot(const Infer* m, int slot, long long n_tokens, long long first_write) {
   if (m->n_pages == 0) return;
   const size_t held = m->held[slot].size();
   B200W_CHECK(held > 0, "cache slot holds no KV pages (b200w_infer_reserve)");
   B200W_CHECK(n_tokens <= static_cast<long long>(held) * KV_PAGE, "position beyond the KV pages the slot holds");
+  B200W_CHECK(first_write >= m->floor[slot], "K/V write below the slot's write floor (into a shared page)");
 }
 
+// drops the slot's reference to each page it holds; a page nobody references returns to the free list, in table order
 void release_pages(Infer* m, int slot) {
   auto& h = m->held[slot];
-  m->free_pages.insert(m->free_pages.end(), h.begin(), h.end());
+  for (const int32_t p : h)
+    if (--m->refs[p] == 0) m->free_pages.push_back(p);
   h.clear();
+  m->floor[slot] = 0;
+}
+
+void check_weights_unshared(const Infer* m) {
+  if (m->retained) throw StateError("KV pages are retained: cached K/V belong to the weights that computed them");
 }
 
 // b200w_infer_init (n_pages == 0) and b200w_infer_init_paged
@@ -1137,6 +1396,9 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   if (n_pages) {
     for (int p = n_pages - 1; p >= 0; --p) m->free_pages.push_back(p);   // page 0 is handed out first
     m->held.assign(B, {});
+    m->floor.assign(B, 0);
+    m->refs.assign(n_pages, 0);
+    m->index_refs.assign(n_pages, 0);
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
     m->pf_limit = static_cast<size_t>(prefill_tokens);
     ensure_prefill(m.get(), m->pf_limit);
@@ -1153,6 +1415,7 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->pf_len = m->alloc<int32_t>(B);
   m->pf_slot = m->alloc<int32_t>(B);
   m->pf_last = m->alloc<int32_t>(B);
+  m->pf_start = m->alloc<int32_t>(B);
   B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin), 4 * B * sizeof(int32_t)));
   m->inv_freq = m->alloc<float>(a.head_dim / 2);
   const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + qd + 2 * kd, d});
@@ -1170,6 +1433,40 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
 
 }  // namespace
 
+void b200w::attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
+                                 int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
+                                 const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs,
+                                 int S, int H, int Hkv, int dh, float scale, cudaStream_t s) {
+  B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
+  B200W_CHECK(n_seqs >= 1 && S >= 128 && S % 128 == 0, "padded length must be a positive multiple of 128");
+  B200W_CHECK(H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad head configuration");
+  B200W_CHECK(q_head_stride >= dh && ld_q >= H * q_head_stride && ld_out >= H * dh && ld_out % 8 == 0,
+              "bad query / output strides");
+  B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1, "bad KV cache");
+  const int kd = Hkv * dh;
+  const CUtensorMap tq = make_tmap_bf16_2d(q, static_cast<uint64_t>(n_seqs) * S, ld_q, ld_q, 128, 64);
+  const CUtensorMap tk = make_tmap_bf16_2d(kcache, cache_rows, kd, kd, KV_PAGE, 64);
+  const CUtensorMap tv = make_tmap_bf16_2d(vcache, cache_rows, kd, kd, KV_PAGE, 64);
+  static PerDeviceOnce once;
+  once.run([&] {
+    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    ca_smem_bytes<64>()));
+    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    ca_smem_bytes<128>()));
+  });
+  const dim3 grid((S / 128) * n_seqs * H);
+  const float scale_log2 = scale * 1.4426950408889634f;
+  if (dh == 64)
+    attn_fwd_cached_kernel<64><<<grid, CA_THREADS, ca_smem_bytes<64>(), s>>>(
+        tq, tk, tv, q_head_stride, static_cast<bf16*>(out), ld_out, table, nsplit, slots, starts, lengths, n_seqs, S,
+        H, Hkv, scale_log2);
+  else
+    attn_fwd_cached_kernel<128><<<grid, CA_THREADS, ca_smem_bytes<128>(), s>>>(
+        tq, tk, tv, q_head_stride, static_cast<bf16*>(out), ld_out, table, nsplit, slots, starts, lengths, n_seqs, S,
+        H, Hkv, scale_log2);
+  B200W_CUDA(cudaGetLastError());
+}
+
 extern "C" {
 
 int b200w_infer_init(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch) {
@@ -1184,25 +1481,45 @@ int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max
   });
 }
 
-int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens) {
+int b200w_infer_reserve_shared(b200w_ctx* ctx, int slot, int n_tokens, const int32_t* shared_pages, int n_shared) {
   bool short_of_pages = false;
   const int st = iguard(ctx, [&] {
     Infer* m = paged_model(ctx);
     B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
     B200W_CHECK(n_tokens >= 1 && n_tokens <= m->a.max_ctx, "n_tokens must be in 1..max_ctx");
     const size_t need = cdiv(n_tokens, KV_PAGE);
-    if (need > m->free_pages.size() + m->held[slot].size()) {
-      ctx_set_error(ctx, ("KV page pool exhausted: " + std::to_string(need) + " pages needed, " +
+    B200W_CHECK(n_shared >= 0 && static_cast<size_t>(n_shared) <= need && (n_shared == 0 || shared_pages),
+                "n_shared must be in 0..ceil(n_tokens / 128)");
+    auto& h = m->held[slot];
+    // the references left once the slot has let go of what it holds: its pages with none return to the free list,
+    // and a shared page must keep one (a free page holds nothing to share)
+    auto after_release = [&](int32_t p) {
+      return m->refs[p] - static_cast<int32_t>(std::count(h.begin(), h.end(), p));
+    };
+    for (int i = 0; i < n_shared; ++i)
+      B200W_CHECK(shared_pages[i] >= 0 && shared_pages[i] < m->n_pages && after_release(shared_pages[i]) >= 1,
+                  "a shared page must be held by a slot or retained");
+    size_t returning = 0;
+    for (size_t i = 0; i < h.size(); ++i)
+      if (std::find(h.begin(), h.begin() + i, h[i]) == h.begin() + i && after_release(h[i]) == 0) ++returning;
+    const size_t fresh = need - n_shared;
+    if (fresh > m->free_pages.size() + returning) {
+      ctx_set_error(ctx, ("KV page pool exhausted: " + std::to_string(fresh) + " pages needed, " +
                           std::to_string(m->free_pages.size()) + " free").c_str());
       short_of_pages = true;
       return;
     }
     release_pages(m, slot);
-    auto& h = m->held[slot];
-    for (size_t i = 0; i < need; ++i) {
+    for (int i = 0; i < n_shared; ++i) {
+      h.push_back(shared_pages[i]);
+      ++m->refs[shared_pages[i]];
+    }
+    for (size_t i = 0; i < fresh; ++i) {
       h.push_back(m->free_pages.back());
+      m->refs[m->free_pages.back()] = 1;
       m->free_pages.pop_back();
     }
+    m->floor[slot] = n_shared * KV_PAGE;
     // the row goes to the device on the library stream, so it lands before the next step or prefill; the
     // table's address never changes, so the captured decode graphs read the new row
     int32_t* row = m->table_pin + static_cast<size_t>(slot) * m->nsplit;
@@ -1214,11 +1531,39 @@ int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens) {
   return st == B200W_OK && short_of_pages ? B200W_ERR_OOM : st;
 }
 
+int b200w_infer_reserve(b200w_ctx* ctx, int slot, int n_tokens) {
+  return b200w_infer_reserve_shared(ctx, slot, n_tokens, nullptr, 0);
+}
+
 int b200w_infer_release(b200w_ctx* ctx, int slot) {
   return iguard(ctx, [&] {
     Infer* m = paged_model(ctx);
     B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
     release_pages(m, slot);   // the device row is left as it was: steps and prefills of the slot are refused
+  });
+}
+
+int b200w_infer_retain_pages(b200w_ctx* ctx, const int32_t* pages, int n, int delta) {
+  return iguard(ctx, [&] {
+    Infer* m = paged_model(ctx);
+    B200W_CHECK(delta == 1 || delta == -1, "delta must be +1 or -1");
+    B200W_CHECK(n >= 0 && (n == 0 || pages), "bad page list");
+    std::unordered_map<int32_t, int32_t> count;   // every page is checked before any reference changes
+    for (int i = 0; i < n; ++i) {
+      B200W_CHECK(pages[i] >= 0 && pages[i] < m->n_pages, "page outside the pool");
+      ++count[pages[i]];
+    }
+    for (const auto& pc : count) {
+      if (delta > 0) B200W_CHECK(m->refs[pc.first] >= 1, "retaining a page that holds no reference (a free page)");
+      else B200W_CHECK(m->index_refs[pc.first] >= pc.second, "dropping a retained reference that does not exist");
+    }
+    for (int i = 0; i < n; ++i) {
+      const int32_t p = pages[i];
+      m->refs[p] += delta;
+      m->index_refs[p] += delta;
+      m->retained += delta;
+      if (m->refs[p] == 0) m->free_pages.push_back(p);
+    }
   });
 }
 
@@ -1275,6 +1620,7 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     const IParam& p = m->params[it->second];
     B200W_CHECK(n_elements == p.rows * p.cols, "element count does not match the parameter shape");
     B200W_CHECK(dtype == B200W_BF16 || dtype == B200W_F32, "dtype must be bf16 or f32");
+    check_weights_unshared(m);
     cudaStream_t s = ctx_stream(ctx);
     const size_t n = static_cast<size_t>(n_elements);
     m->tiled_valid = false;
@@ -1305,6 +1651,7 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
 int b200w_infer_init_random(b200w_ctx* ctx, uint64_t seed, float std) {
   return iguard(ctx, [&] {
     Infer* m = model(ctx);
+    check_weights_unshared(m);
     // one device-side fill of the whole flat space (the fused matrices included), then the 1-D parameters
     m->tiled_valid = false;
     ctx_fill_normal(ctx, m->w, m->n_elems, seed, std);
@@ -1325,7 +1672,7 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
       B200W_CHECK(positions[i] >= 0 && positions[i] < a.max_ctx, "position outside the KV cache");
       B200W_CHECK(slots[i] >= 0 && slots[i] < m->max_batch, "bad cache slot");
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
-      check_paged_slot(m, slots[i], positions[i] + 1LL);
+      check_paged_slot(m, slots[i], positions[i] + 1LL, positions[i]);
     }
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
@@ -1382,11 +1729,13 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
 // forward (causal within each sequence), K/V of the real positions written to the cache slots, and the
 // greedy token after each prompt. Padding tokens sit AFTER the real ones, so causality keeps them
 // from influencing any real position.
-int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const int32_t* slots,
-                        int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out) {
+// b200w_infer_prefill (starts == nullptr) and b200w_infer_prefill_cached: row b of `tokens` holds positions
+// [start_b, lengths[b]) of its prompt, start_b = starts ? starts[b] : 0.
+static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
+                        const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out) {
   return iguard(ctx, [&] {
     NvtxRange nvtx_range("b200w prefill");
-    Infer* m = model(ctx);
+    Infer* m = starts ? paged_model(ctx) : model(ctx);
     const auto& a = m->a;
     B200W_CHECK(tokens && lengths && slots && n_seqs >= 1 && n_seqs <= m->max_batch, "bad prefill batch");
     B200W_CHECK(padded_len >= 128 && padded_len % 128 == 0, "padded_len must be a positive multiple of 128");
@@ -1394,14 +1743,19 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     const size_t T = static_cast<size_t>(n_seqs) * S;
     B200W_CHECK(T <= (1u << 20), "prefill batch too large");
     for (int b = 0; b < n_seqs; ++b) {
-      B200W_CHECK(lengths[b] >= 1 && lengths[b] <= S && lengths[b] <= a.max_ctx, "bad prompt length");
+      const int start = starts ? starts[b] : 0;
+      if (starts)
+        B200W_CHECK(start > 0 && start % KV_PAGE == 0 && start < lengths[b],
+                    "a cached prefix must be a positive multiple of 128 below the prompt length");
+      B200W_CHECK(lengths[b] >= 1 && lengths[b] - start <= S && lengths[b] <= a.max_ctx, "bad prompt length");
       B200W_CHECK(slots[b] >= 0 && slots[b] < m->max_batch, "bad cache slot");
-      check_paged_slot(m, slots[b], lengths[b]);
+      check_paged_slot(m, slots[b], lengths[b], start);
     }
     if (m->n_pages) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
     for (size_t i = 0; i < T; ++i)
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
-    if (a.family == B200W_FAMILY_OPT) B200W_CHECK(S <= a.max_positions, "OPT: padded_len exceeds the position table");
+    if (a.family == B200W_FAMILY_OPT && !starts)
+      B200W_CHECK(S <= a.max_positions, "OPT: padded_len exceeds the position table");
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
     ensure_prefill(m, T);
@@ -1410,14 +1764,26 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     int32_t* pin = m->pf_pin;
     memcpy(pin, tokens, T * 4);
     for (int b = 0; b < n_seqs; ++b) {
+      const int start = starts ? starts[b] : 0;
       pin[T + b] = lengths[b];
       pin[T + B + b] = slots[b];
-      pin[T + 2 * B + b] = b * S + lengths[b] - 1;   // row of the last real token
+      pin[T + 2 * B + b] = b * S + lengths[b] - start - 1;   // row of the last real token
+      pin[T + 3 * B + b] = start;
+      // OPT after a cached prefix: the learned position of each row; padding rows repeat the last real one, so that
+      // they stay inside the position table
+      if (starts && a.family == B200W_FAMILY_OPT)
+        for (int p = 0; p < S; ++p)
+          pin[T + 4 * B + static_cast<size_t>(b) * S + p] = std::min(start + p, lengths[b] - 1);
     }
     B200W_CUDA(cudaMemcpyAsync(m->pf_tok, pin, T * 4, cudaMemcpyHostToDevice, s));
     B200W_CUDA(cudaMemcpyAsync(m->pf_len, pin + T, n_seqs * 4, cudaMemcpyHostToDevice, s));
     B200W_CUDA(cudaMemcpyAsync(m->pf_slot, pin + T + B, n_seqs * 4, cudaMemcpyHostToDevice, s));
     B200W_CUDA(cudaMemcpyAsync(m->pf_last, pin + T + 2 * B, n_seqs * 4, cudaMemcpyHostToDevice, s));
+    if (starts) {
+      B200W_CUDA(cudaMemcpyAsync(m->pf_start, pin + T + 3 * B, n_seqs * 4, cudaMemcpyHostToDevice, s));
+      if (a.family == B200W_FAMILY_OPT)
+        B200W_CUDA(cudaMemcpyAsync(m->pf_pos, pin + T + 4 * B, T * 4, cudaMemcpyHostToDevice, s));
+    }
 
     const int d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim,
               V = a.vocab_size;
@@ -1434,7 +1800,11 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
     };
     bf16* h = m->pf_h;
     bf16* h2 = m->pf_h2;
-    embed_fwd(m->pf_tok, m->w + m->p_embed, opt ? m->w + m->p_pos : nullptr, h, Ti, d, V, S, opt ? 2 : 0, s); ++nl;
+    if (opt && starts)
+      infer_embed_pos_kernel<<<Ti, 128, 0, s>>>(m->pf_tok, m->pf_pos, m->w + m->p_embed, m->w + m->p_pos, h, d, 2);
+    else
+      embed_fwd(m->pf_tok, m->w + m->p_embed, opt ? m->w + m->p_pos : nullptr, h, Ti, d, V, S, opt ? 2 : 0, s);
+    ++nl;
     for (int l = 0; l < a.num_layers; ++l) {
       const auto& p = m->lp[l];
       bf16* kc = m->kc + l * layer_cache;
@@ -1448,19 +1818,31 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
         const long long ge = static_cast<long long>(Ti) * (f / 8);
         gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, s>>>(m->pf_cat + qd, Ti, f, ldc); ++nl;
       }
-      bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
-      const int ld_in = padded ? HT * dhp : qkvd;
       const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
-      prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq, m->pf_len,
-                                                                m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dhp, opt ? 0 : 1,
-                                                                m->table, m->nsplit); ++nl;
-      B200W_CUDA(cudaGetLastError());
-      bf16* att_out = padded ? m->pf_attp : m->pf_cat;
-      const int ld_out = padded ? H * dhp : ldc;
-      attention_fwd(att_in, ld_in, H * dhp, (H + Hkv) * dhp, att_out, ld_out, m->pf_lse, n_seqs, S, H, Hkv, scale, s); ++nl;
-      if (padded) {
-        const long long ue = static_cast<long long>(Ti) * H * (dh / 8);
-        unpad_heads_kernel<<<cdiv(ue, 256), 256, 0, s>>>(m->pf_attp, H * dhp, m->pf_cat, ldc, Ti, H, dh, dhp); ++nl;
+      if (starts) {
+        // after a cached prefix: q / k rotated in place at their positions, the suffix K/V into the slot's pages, then
+        // the paged attention reads the queries at their own width and writes the o-projection's input directly
+        prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, m->pf_qkv, qkvd, m->inv_freq,
+                                                                  m->pf_len, m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dh,
+                                                                  opt ? 0 : 1, m->table, m->nsplit, m->pf_start); ++nl;
+        B200W_CUDA(cudaGetLastError());
+        attention_fwd_cached(m->pf_qkv, qkvd, dh, kc, vc, m->layer_rows(), m->table, m->nsplit, m->pf_slot, m->pf_start,
+                             m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv, dh, scale, s); ++nl;
+      } else {
+        bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
+        const int ld_in = padded ? HT * dhp : qkvd;
+        prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq,
+                                                                  m->pf_len, m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dhp,
+                                                                  opt ? 0 : 1, m->table, m->nsplit, nullptr); ++nl;
+        B200W_CUDA(cudaGetLastError());
+        bf16* att_out = padded ? m->pf_attp : m->pf_cat;
+        const int ld_out = padded ? H * dhp : ldc;
+        attention_fwd(att_in, ld_in, H * dhp, (H + Hkv) * dhp, att_out, ld_out, m->pf_lse, n_seqs, S, H, Hkv, scale, s);
+        ++nl;
+        if (padded) {
+          const long long ue = static_cast<long long>(Ti) * H * (dh / 8);
+          unpad_heads_kernel<<<cdiv(ue, 256), 256, 0, s>>>(m->pf_attp, H * dhp, m->pf_cat, ldc, Ti, H, dh, dhp); ++nl;
+        }
       }
       if (falcon) {
         G(m->pf_cat, ldc, p.wo, ldc, h2, h, d, d, ldc);   // h' = h + [attn | gelu(h_to_4h)] [dense | 4h_to_h]^T
@@ -1500,6 +1882,18 @@ int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* le
       cudaFree(tmp);
     }
   });
+}
+
+int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const int32_t* slots,
+                        int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out) {
+  return prefill_impl(ctx, tokens, nullptr, lengths, slots, n_seqs, padded_len, next_tokens, logits_out);
+}
+
+int b200w_infer_prefill_cached(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
+                               const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
+                               float* logits_out) {
+  if (!starts) return B200W_ERR_INVALID;
+  return prefill_impl(ctx, tokens, starts, lengths, slots, n_seqs, padded_len, next_tokens, logits_out);
 }
 
 int64_t b200w_infer_device_bytes(b200w_ctx* ctx) {

@@ -76,6 +76,20 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
                    const void* dout, int ld_out, const float* lse2, float* delta, void* dqkv, int B,
                    int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs = nullptr);
 
+// ---- infer.cu ------------------------------------------------------------------------------
+// Causal attention of prompt suffixes after a cached prefix (infer.cu attn_fwd_cached_kernel). Sequence b's rows
+// [b * S, b * S + S) of q [n_seqs * S, ld_q] (head h at column h * q_head_stride, its first dh columns used) are its
+// positions starts[b] + p; they attend to positions [0, position] of cache slot slots[b], whose K and V are rows
+// table[slot * nsplit + position / 128] + position % 128 of kcache / vcache [cache_rows, Hkv * dh]. starts[b] is a
+// multiple of 128 below lengths[b]; the pages of positions [0, lengths[b]) are the caller's to have filled and
+// entered in the table. out [n_seqs * S, ld_out]: head h at column h * dh. slots / starts / lengths: DEVICE int32
+// [n_seqs]. Rows at positions >= lengths[b] get finite values that mean nothing.
+void attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
+                          int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
+                          const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
+                          int H, int Hkv, int dh, float scale, cudaStream_t s);
+
+
 // ---- ops.cu --------------------------------------------------------------------------------
 // out[t] = table[ids[t]] (+ pos_table[t % S + pos_offset] when pos_table != nullptr: OPT's learned
 // positions). embed_bwd: dtable[ids[t]] += dout[t] unless ids[t] == pad_id (nn.Embedding padding_idx;

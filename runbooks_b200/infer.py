@@ -4,7 +4,7 @@ slot per step — prompt ingestion and generation are the same step)."""
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Dict, Iterable, List, Optional, Tuple
 
 import numpy as np
@@ -112,6 +112,18 @@ class InferEngine(Engine):
         B200W_ERR_OOM (-5) when too few pages are free."""
         self._check(self._lib.b200w_infer_reserve(self._h, slot, n_tokens))
 
+    def reserve_shared(self, slot: int, n_tokens: int, shared_pages: List[int]):
+        """reserve, with the slot's first len(shared_pages) pages being those (already referenced) pages; the slot
+        may then write K/V only from position 128 * len(shared_pages) on (b200w_infer_reserve_shared)."""
+        sp = np.ascontiguousarray(shared_pages, dtype=np.int32)
+        self._check(self._lib.b200w_infer_reserve_shared(self._h, slot, n_tokens, sp.ctypes.data if sp.size else None,
+                                                         sp.size))
+
+    def retain_pages(self, pages: List[int], delta: int):
+        """The host prefix index's references: +1 retains pages that hold a reference, -1 drops retained ones."""
+        pg = np.ascontiguousarray(pages, dtype=np.int32)
+        self._check(self._lib.b200w_infer_retain_pages(self._h, pg.ctypes.data if pg.size else None, pg.size, delta))
+
     def release(self, slot: int):
         self._check(self._lib.b200w_infer_release(self._h, slot))
 
@@ -183,6 +195,24 @@ class InferEngine(Engine):
                                                   nxt.ctypes.data, logits.ctypes.data if want_logits else None))
         return nxt, logits
 
+    def prefill_cached(self, prompts: List[List[int]], starts: List[int], slots: List[int], want_logits: bool = False):
+        """prefill of whole prompts whose positions [0, starts[i]) already have their K/V in the slot's (shared)
+        pages: only prompts[i][starts[i]:] is computed (b200w_infer_prefill_cached)."""
+        n = len(prompts)
+        S = ((max(len(p) - s for p, s in zip(prompts, starts)) + 127) // 128) * 128
+        tok = np.zeros((n, S), dtype=np.int32)
+        for i, (p, s) in enumerate(zip(prompts, starts)):
+            tok[i, :len(p) - s] = p[s:]
+        st = np.ascontiguousarray(starts, dtype=np.int32)
+        lens = np.array([len(p) for p in prompts], dtype=np.int32)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        nxt = np.empty(n, dtype=np.int32)
+        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
+        self._check(self._lib.b200w_infer_prefill_cached(self._h, tok.ctypes.data, st.ctypes.data, lens.ctypes.data,
+                                                         sl.ctypes.data, n, S, nxt.ctypes.data,
+                                                         logits.ctypes.data if want_logits else None))
+        return nxt, logits
+
 
 def sample_token(logits: np.ndarray, temperature: float, top_p: float, rng: np.random.Generator) -> int:
     """Host-side sampling of one row (the engine itself is greedy): softmax(logits / T) restricted to the
@@ -212,10 +242,25 @@ class _Req:
     temperature: float = 0.0
     top_p: float = 1.0
     rng: Optional[np.random.Generator] = None
+    cached_tokens: int = 0                                    # prompt positions whose K/V came from the prefix index
+    nodes: List["_Node"] = field(default_factory=list)        # index nodes whose page the slot holds
+    entered: List["_Node"] = field(default_factory=list)      # of those, the ones this request's prefill fills
 
     @property
     def greedy(self) -> bool:
         return self.temperature <= 0.0
+
+
+class _Node:
+    """A full prompt page in the prefix index: the K/V of the KV_PAGE tokens `key` that follow the tokens of its
+    ancestors. A page's K/V depend on every token before it, and the path from the root spells exactly those."""
+    __slots__ = ("parent", "key", "page", "children", "users", "last_use")
+
+    def __init__(self, parent: Optional["_Node"], key: Tuple[int, ...], page: int):
+        self.parent, self.key, self.page = parent, key, page
+        self.children: Dict[Tuple[int, ...], "_Node"] = {}
+        self.users = 0          # active requests whose slot holds the page
+        self.last_use = 0
 
 
 class Generator:
@@ -223,7 +268,11 @@ class Generator:
     pass when it is admitted (engines without `prefill`, i.e. the CPU test stubs, feed it one token per
     step through the decode path); from then on every active request advances one token per step."""
 
-    def __init__(self, engine: InferEngine, eos_id: Optional[int] = None, use_prefill: bool = True):
+    def __init__(self, engine: InferEngine, eos_id: Optional[int] = None, use_prefill: bool = True,
+                 prefix_cache: bool = False):
+        """prefix_cache (paged KV cache only): requests whose prompts share leading full pages share those pages and
+        prefill only the rest. An index of the prompt pages served keeps them (one retained reference each) until
+        pages run short, then gives back the least recently used ones."""
         self.e, self.eos = engine, eos_id
         self.free = list(range(engine.max_batch))
         self.active: List[_Req] = []
@@ -231,6 +280,12 @@ class Generator:
         self._deferred: List[_Req] = []
         # paged KV cache: a request holds pages for len(prompt) + max_tokens positions from admission to its end
         self.kv_pages = getattr(engine, "kv_pages", None)
+        self.prefix_cache = prefix_cache
+        if prefix_cache and (self.kv_pages is None or not self.use_prefill):
+            raise ValueError("prefix caching needs the paged KV cache and an engine that prefills")
+        self._root = _Node(None, (), -1)
+        self._nodes: Dict[_Node, None] = {}     # every node of the index, in insertion order
+        self._tick = 0
 
     def add(self, prompt: List[int], max_tokens: int, temperature: float = 0.0, top_p: float = 1.0,
             seed: Optional[int] = None, defer_prefill: bool = False) -> _Req:
@@ -250,12 +305,16 @@ class Generator:
                              f"the cache holds {self.kv_pages}")
         if not self.free:
             raise RuntimeError("no free cache slot")
-        if self.kv_pages is not None:
+        matched, entered = [], []
+        if self.prefix_cache:
+            matched, entered = self._admit(list(prompt), len(prompt) + max_tokens, self.free[-1])
+        elif self.kv_pages is not None:
             if pages_for(len(prompt) + max_tokens) > self.e.kv_pages_free():
                 raise CacheFull("KV cache full: too few free pages for this request now")
             self.e.reserve(self.free[-1], len(prompt) + max_tokens)
         r = _Req(list(prompt), max_tokens, [], 0, self.free.pop(), False, float(temperature), float(top_p),
-                 np.random.default_rng(seed) if temperature > 0 else None)
+                 np.random.default_rng(seed) if temperature > 0 else None,
+                 len(matched) * KV_PAGE, matched + entered, entered)
         self.active.append(r)
         if self.use_prefill and len(prompt) > 1:
             self._deferred.append(r)
@@ -263,20 +322,95 @@ class Generator:
                 self.flush_prefill()
         return r
 
+    def _admit(self, prompt: List[int], n_tokens: int, slot: int):
+        """Prefix cache admission into `slot`: the longest chain of indexed pages that prefixes the prompt (at most
+        (len - 1) // 128, so that at least one prompt token is computed for the next-token logits) is shared; the
+        request's own full prompt pages beyond it enter the index at once, so that requests admitted later in the
+        same round share them too. -> (matched nodes, entered nodes)."""
+        matched: List[_Node] = []
+        node = self._root
+        for k in range((len(prompt) - 1) // KV_PAGE):
+            node = node.children.get(tuple(prompt[k * KV_PAGE:(k + 1) * KV_PAGE]))
+            if node is None:
+                break
+            matched.append(node)
+        short = pages_for(n_tokens) - len(matched) - self.e.kv_pages_free()
+        if short > 0:
+            keep = set(matched)
+            if short > sum(1 for n in self._nodes if n.users == 0 and n not in keep):
+                raise CacheFull("KV cache full: too few free or evictable pages for this request now")
+            for _ in range(short):   # least recently used leaves that no request holds (each frees its page)
+                self._drop(min((n for n in self._nodes if not n.children and n.users == 0 and n not in keep),
+                               key=lambda n: n.last_use))
+        self.e.reserve_shared(slot, n_tokens, [n.page for n in matched])
+        self._tick += 1
+        for n in matched:
+            n.users += 1
+            n.last_use = self._tick
+        entered: List[_Node] = []
+        parent = matched[-1] if matched else self._root
+        if len(prompt) // KV_PAGE > len(matched):
+            pages = self.e.slot_pages(slot)
+            for k in range(len(matched), len(prompt) // KV_PAGE):
+                key = tuple(prompt[k * KV_PAGE:(k + 1) * KV_PAGE])
+                if key in parent.children:   # the last page of an indexed prompt of the same length (the cap above)
+                    break
+                node = _Node(parent, key, pages[k])
+                node.users, node.last_use = 1, self._tick
+                parent.children[key] = node
+                self._nodes[node] = None
+                entered.append(node)
+                parent = node
+            if entered:
+                self.e.retain_pages([n.page for n in entered], +1)
+        return matched, entered
+
+    def _drop(self, node: _Node):
+        """Takes `node` and everything below it out of the prefix index, with the index's references."""
+        gone, stack = [], [node]
+        while stack:
+            n = stack.pop()
+            gone.append(n)
+            stack.extend(n.children.values())
+        del node.parent.children[node.key]
+        for n in gone:
+            del self._nodes[n]
+        self.e.retain_pages([n.page for n in gone], -1)
+
+    def clear_prefix_cache(self):
+        """Drops every index entry; a page returns to the free list once no request holds it either."""
+        for n in list(self._root.children.values()):
+            self._drop(n)
+
     def flush_prefill(self):
-        """One prefill call per group of deferred prompts that pad to the same multiple of 128 tokens."""
+        """One prefill call per group of deferred prompts with the same cached prefix that pad to the same multiple of
+        128 tokens. Cold prompts (no cached prefix) go first, then the others in ascending prefix length: a request
+        shares only pages that a request with a shorter prefix fills, so those are written by an earlier call."""
         pend, self._deferred = self._deferred, []
-        groups: Dict[int, List[_Req]] = {}
+        groups: Dict[Tuple[int, int], List[_Req]] = {}
         for r in pend:
-            groups.setdefault((len(r.prompt) + 127) // 128, []).append(r)
+            groups.setdefault((r.cached_tokens, pages_for(len(r.prompt) - r.cached_tokens)), []).append(r)
         calls = []
-        for blocks, rs in sorted(groups.items()):
+        for (start, blocks), rs in sorted(groups.items()):
             # paged: a call's n_seqs * padded_len stays within the prefill workspace the engine allocated
             per_call = max(1, self.e.prefill_tokens // (blocks * 128)) if self.kv_pages is not None else len(rs)
-            calls += [rs[i:i + per_call] for i in range(0, len(rs), per_call)]
-        for rs in calls:
+            calls += [(start, rs[i:i + per_call]) for i in range(0, len(rs), per_call)]
+        for ci, (start, rs) in enumerate(calls):
             need_logits = any(not r.greedy for r in rs)
-            nxt, lg = self.e.prefill([r.prompt for r in rs], [r.slot for r in rs], want_logits=need_logits)
+            try:
+                if start:
+                    nxt, lg = self.e.prefill_cached([r.prompt for r in rs], [start] * len(rs), [r.slot for r in rs],
+                                                    want_logits=need_logits)
+                else:
+                    nxt, lg = self.e.prefill([r.prompt for r in rs], [r.slot for r in rs], want_logits=need_logits)
+            except Exception:
+                # the pages this call and the calls after it were to fill hold no K/V: out of the index
+                for _, later in calls[ci:]:
+                    for r in later:
+                        for n in r.entered:
+                            if n in self._nodes:
+                                self._drop(n)
+                raise
             if need_logits and lg is None:
                 raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
             for i, r in enumerate(rs):
@@ -298,6 +432,10 @@ class Generator:
 
     def _free_slot(self, r: _Req):
         self.free.append(r.slot)
+        self._tick += 1
+        for n in r.nodes:
+            n.users -= 1
+            n.last_use = self._tick
         if self.kv_pages is not None:
             self.e.release(r.slot)
 

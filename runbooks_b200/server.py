@@ -37,10 +37,10 @@ class Scheduler(threading.Thread):
     advances every active request by one token per engine step, and feeds each request's event queue
     (text deltas for streaming clients, one final record for everybody)."""
 
-    def __init__(self, engine, tokenizer, max_queue: int = 0):
+    def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False):
         super().__init__(daemon=True)
         from .infer import Generator
-        self.gen = Generator(engine, eos_id=tokenizer.eos_id)
+        self.gen = Generator(engine, eos_id=tokenizer.eos_id, prefix_cache=prefix_cache)
         self.tok, self.q = tokenizer, queue.Queue()
         self.max_queue = max_queue or 4 * engine.max_batch
         self.ready = threading.Event()
@@ -84,7 +84,7 @@ class Scheduler(threading.Thread):
             if not req.done:            # stopped by a stop string: free the slot now
                 self.gen.cancel(req)
             item["events"].put(("done", {"text": text, "prompt_tokens": n_prompt, "completion_tokens": len(out),
-                                         "finish_reason": finish}))
+                                         "cached_tokens": req.cached_tokens, "finish_reason": finish}))
             return True
         return False
 
@@ -257,7 +257,7 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             deadline = time.time() + request_timeout_s
             if r["stream"]:
                 return self._stream(items[0], r, cid, created, deadline)
-            choices, usage_p, usage_c = [], 0, 0
+            choices, usage_p, usage_c, cached = [], 0, 0, 0
             for i, it in enumerate(items):
                 final = None
                 while final is None:
@@ -276,10 +276,13 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
                 text = (r["prompt"] if r["echo"] else "") + final["text"]
                 choices.append({"index": i, "text": text, "logprobs": None, "finish_reason": final["finish_reason"]})
                 usage_p, usage_c = final["prompt_tokens"], usage_c + final["completion_tokens"]
+                # the prompt is counted once, as prompt_tokens is: its tokens that the best-served copy found cached
+                cached = max(cached, final["cached_tokens"])
+            usage = {"prompt_tokens": usage_p, "completion_tokens": usage_c, "total_tokens": usage_p + usage_c}
+            if sched.gen.prefix_cache:
+                usage["prompt_tokens_details"] = {"cached_tokens": cached}
             self._send(200, {"id": cid, "object": "text_completion", "created": created, "model": model_name,
-                             "choices": choices,
-                             "usage": {"prompt_tokens": usage_p, "completion_tokens": usage_c,
-                                       "total_tokens": usage_p + usage_c}})
+                             "choices": choices, "usage": usage})
 
         def _stream(self, item, r, cid, created, deadline):
             """Server-sent events, the OpenAI / basaran streaming shape: one `data: {json}` per text delta,
@@ -343,6 +346,20 @@ def server_params(content: str, max_batch: int | None = None, kv_cache_gb: float
     return max_batch, kv_cache_gb
 
 
+def prefix_cache_param(content: str, prefix_cache: bool | None = None, environ=None) -> bool:
+    """Whether the Server shares the K/V pages of repeated prompt prefixes: --prefix-cache, else the params'
+    prefix_cache (params.json, PARAM_PREFIX_CACHE over it: true / false, 1 / 0, yes / no), else off."""
+    if prefix_cache is not None:
+        return bool(prefix_cache)
+    extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
+    v = extra.get("prefix_cache", False)
+    if isinstance(v, bool) or v in (0, 1):
+        return bool(v)
+    if isinstance(v, str) and v.strip().lower() in ("true", "1", "yes", "false", "0", "no"):
+        return v.strip().lower() in ("true", "1", "yes")
+    raise ValueError(f"param 'prefix_cache': cannot read {v!r} as a boolean")
+
+
 def kv_pages_for_gb(arch, kv_cache_gb: float) -> int:
     """Pages of a paged KV cache of kv_cache_gb * 10^9 bytes; ValueError when that cannot hold one max_ctx request."""
     from .infer import kv_page_bytes, pages_for
@@ -377,13 +394,17 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
     return e, cfg
 
 
-def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None):
+def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
+          prefix_cache: bool | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
+    prefix_cache = prefix_cache_param(content, prefix_cache)
+    if prefix_cache and kv_cache_gb is None:
+        raise ValueError("prefix_cache shares pages of the paged KV cache: it needs kv_cache_gb")
     model_dir = os.path.join(content, "model")
     t0 = time.time()
     engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb)
     tok = contract.Tokenizer(model_dir)
-    sched = Scheduler(engine, tok)
+    sched = Scheduler(engine, tok, prefix_cache=prefix_cache)
     sched.start()
     name = cfg.get("_name_or_path") or cfg.get("model_type", "model")
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
@@ -391,7 +412,8 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
              "max_batch": max_batch}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
-        ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch) / 1e6, 2))
+        ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch) / 1e6, 2),
+                     prefix_cache=prefix_cache)
     print(json.dumps(ready), flush=True)
     httpd.serve_forever()
 
@@ -405,9 +427,12 @@ def main(argv=None) -> int:
     ap.add_argument("--kv-cache-gb", type=float, default=None,
                     help="serve from a paged KV cache of this many GB (default: param kv_cache_gb, else a "
                          "contiguous max_batch x max_ctx cache)")
+    ap.add_argument("--prefix-cache", action="store_true", default=None,
+                    help="share the KV pages of repeated prompt prefixes (needs the paged cache; default: param "
+                         "prefix_cache, else off)")
     a = ap.parse_args(argv)
     try:
-        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb)
+        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()
