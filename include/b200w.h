@@ -280,6 +280,10 @@ B200W_API int b200w_op_gemm(b200w_ctx* ctx, const void* A, int a_mn, int lda, co
  * in the GEMM epilogue, fp32 until the single rounding (OPT family). bias: DEVICE bf16, 16-byte aligned. */
 B200W_API int b200w_op_gemm_bias(b200w_ctx* ctx, const void* A, int lda, const void* B, int ldb, void* D,
                        const void* C, int ldd, int M, int N, int K, const void* bias, int act, int block_n);
+/* b200w_op_gemm with an fp32 D (C may be NULL or alias D) that also writes d2 (bf16, row stride ldd), the
+ * bf16-rounded copy of D that the last micro-step's weight gradient hands to the gradient exchange. */
+B200W_API int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb,
+                                 float* D, const float* C, int ldd, int M, int N, int K, int block_n, void* d2);
 /* out[M,N] = X[M,K] W[N,K]^T (+C), M <= 128: the decode-time projection (swap-AB, split-K). */
 B200W_API int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k);

@@ -99,6 +99,8 @@ PROTOTYPES = {
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
                                      C.c_int, C.c_int]),
+    "b200w_op_gemm_wire": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
+                                     C.c_int, C.c_int, C.c_int, vp]),
     "b200w_op_gemm_decode": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_fwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_bwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,

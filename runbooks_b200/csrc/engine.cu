@@ -1791,6 +1791,11 @@ int b200w_op_gemm_bias(b200w_ctx* ctx, const void* A, int lda, const void* B, in
                        int M, int N, int K, const void* bias, int act, int block_n) {
   HOOK(gemm_bf16_ex(A, false, lda, B, false, ldb, D, C, false, ldd, M, N, K, block_n, bias, act, ctx->stream));
 }
+int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb, float* D,
+                       const float* C, int ldd, int M, int N, int K, int block_n, void* d2) {
+  HOOK(gemm_bf16_ex(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, true, ldd, M, N, K, block_n, nullptr, 0, ctx->stream,
+                    d2));
+}
 int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k) {
   return guarded(ctx, [&] {

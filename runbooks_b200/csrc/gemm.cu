@@ -15,6 +15,7 @@
 // The producer runs ahead across tile boundaries, so the next tile's operands stream in while the
 // consumers write the previous tile out.
 #include <mutex>
+#include <type_traits>
 
 #include "host_common.h"
 #include "ops.h"
@@ -62,66 +63,72 @@ constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr int A_HALF_BYTES = 64 * 128;
 constexpr int PAIR_N = 256;    // tile width of the 2-CTA cluster kernel (block_n = 512)
 
+// Epilogue staging: each consumer warpgroup owns EPI_SLOTS boxes of 64 rows x 128 B (8 KB, the SWIZZLE_128B layout
+// TMA reads and writes). A tile's 64 x BLOCK_N rows of a warpgroup are `chunks` of one box width (64 bf16 or 32
+// fp32 columns; 32 columns for the 32-wide tile), handled EPI_SLOTS chunks per pass.
+constexpr int EPI_SLOT_BYTES = 64 * 128;
+
 template <int BLOCK_N>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // 4 x 48 KB, 6 x 32 KB, 8 x 24 KB, 9 x 20 KB of the 227 KB a block may use: the narrow tiles exist for
-  // small M, where the job is to keep every SM streaming weights, not to feed the tensor pipe
+  // 4 x 48 KB, 6 x 32 KB, 8 x 24 KB, 9 x 20 KB of the 227 KB a block may use, plus 32 / 32 / 16 / 16 KB of staging:
+  // a whole bf16 tile for the narrower ones, half of it for 128 x 256. The narrow tiles exist for small M, where the
+  // job is to keep every SM streaming weights, not to feed the tensor pipe.
   static constexpr int STAGES = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128) ? 6 : (BLOCK_N == 64) ? 8 : 9;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int EPI_SLOTS = BLOCK_N >= 128 ? 2 : 1;  // per consumer warpgroup
+  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
+  // the tile's bias columns (bf16, at most 256), one copy per warpgroup
+  static constexpr int BIAS_OFFSET = EPI_OFFSET + 2 * EPI_SLOTS * EPI_SLOT_BYTES;
+  static constexpr int BIAS_BYTES = 256 * 2;
+  static constexpr int BAR_OFFSET = BIAS_OFFSET + 2 * BIAS_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFFSET + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 };
 
-// Epilogue extras of the bf16-output GEMM (nn.Linear(bias=True) + activation of the OPT family): v + bias[col]
-// (+ C) -> act. bias: [N] bf16; act: 0 none, 1 ReLU.
-// d2 (fp32-output GEMMs only): a second, bf16-rounded copy of the output with the same row stride -- the
-// last accumulation micro-step's wgrad writes the gradient's NCCL wire copy from the registers that hold the
-// fp32 sum, instead of a separate cast pass re-reading the fp32 gradient (engine.cu exchange_one).
+// Epilogue extras: v (+ bias[col]) (+ C) -> act -> D. bias: [N] bf16 (nn.Linear(bias=True) of the OPT family,
+// bf16 outputs only); act: 0 none, 1 ReLU. c: C is added (its tensor map is the kernel's tmC).
+// d2 (fp32-output GEMMs only): a second, bf16-rounded copy of the output with the same row stride -- the last
+// accumulation micro-step's wgrad writes the gradient's NCCL wire copy from the registers that hold the fp32 sum,
+// instead of a separate cast pass re-reading the fp32 gradient (engine.cu exchange_one). The kernel writes it
+// through the tensor map tmD2 and uses the pointer only as the flag.
 struct EpiExtra {
   const __nv_bfloat16* bias;
   int act;
   __nv_bfloat16* d2;
+  bool c;
 };
 
-// one output row's columns (col, col + 1); `two`: col + 1 < N. col is even and rows are 16-byte aligned, so
-// the pair is one 4-byte (bf16) or 8-byte (fp32) access.
-__device__ __forceinline__ void store_pair(__nv_bfloat16* d, const __nv_bfloat16* c, float v0, float v1, bool two,
-                                           const __nv_bfloat16* bias, int act, __nv_bfloat16* /*d2: fp32 only*/) {
-  if (two) {
-    if (bias) {
-      const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(bias));
-      v0 += b.x;
-      v1 += b.y;
-    }
-    if (c) {
-      const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(c));
-      v0 += f.x;
-      v1 += f.y;
-    }
-    if (act == 1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-    *reinterpret_cast<uint32_t*>(d) = pack_bf16x2(v0, v1);
-  } else {
-    if (bias) v0 += __bfloat162float(bias[0]);
-    if (c) v0 += __bfloat162float(c[0]);
-    if (act == 1) v0 = fmaxf(v0, 0.f);
-    d[0] = __float2bfloat16_rn(v0);
+// byte offset of byte `lin` of a box whose rows are stored back to back, after the SWIZZLE_128B permutation (the
+// 16-byte unit index within each 128 bytes XOR the 128-byte row index mod 8), for a 1024-byte aligned box
+__device__ __forceinline__ uint32_t sw128(uint32_t lin) { return lin ^ ((lin >> 3) & 0x70u); }
+
+// one output row's columns (col, col + 1) at `p` in the staging: the same fp32 operations as a direct store --
+// v + bias, + C (read from `p`, where the producer put it), ReLU -- then one round-to-nearest conversion for bf16
+// (the columns past N are computed too and left out by the store). bias: shared address of the pair's bias.
+template <bool ADD_C, bool BIAS>
+__device__ __forceinline__ void epi_pair(uint32_t p, float& v0, float& v1, uint32_t bias, bool relu, __nv_bfloat16) {
+  if constexpr (BIAS) {
+    const float2 b = unpack_bf16x2(ld_shared_b32(bias));
+    v0 += b.x;
+    v1 += b.y;
   }
+  if constexpr (ADD_C) {
+    const float2 f = unpack_bf16x2(ld_shared_b32(p));
+    v0 += f.x;
+    v1 += f.y;
+  }
+  if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+  st_shared_b32(p, pack_bf16x2(v0, v1));
 }
-__device__ __forceinline__ void store_pair(float* d, const float* c, float v0, float v1, bool two,
-                                           const __nv_bfloat16* /*bias*/, int /*act*/, __nv_bfloat16* d2) {
-  if (two) {
-    if (c) {
-      const float2 f = *reinterpret_cast<const float2*>(c);
-      v0 += f.x;
-      v1 += f.y;
-    }
-    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
-    if (d2) *reinterpret_cast<uint32_t*>(d2) = pack_bf16x2(v0, v1);
-  } else {
-    if (c) v0 += c[0];
-    d[0] = v0;
-    if (d2) d2[0] = __float2bfloat16_rn(v0);
+template <bool ADD_C, bool BIAS>
+__device__ __forceinline__ void epi_pair(uint32_t p, float& v0, float& v1, uint32_t, bool, float) {
+  if constexpr (ADD_C) {
+    const float2 f = ld_shared_v2f32(p);
+    v0 += f.x;
+    v1 += f.y;
   }
+  st_shared_v2f32(p, v0, v1);
 }
 
 // PAIR: the CTA is one of a 2-CTA cluster that computes a 256 x 256 tile (the CTA of cluster rank r owns rows
@@ -137,28 +144,60 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, uint32_t rank) {
   if constexpr (PAIR) mbar_arrive_cluster(bar, rank ^ 1);
 }
 
+// Epilogue geometry of a tile for output type OutT: a chunk is one staging box (64 rows x CW columns, ROW_BYTES per
+// row), CHUNKS per warpgroup tile, PER_PASS of them staged at once, PASSES passes.
+template <int BLOCK_N, typename OutT>
+struct Epi {
+  static constexpr int CW = (128 / sizeof(OutT)) < BLOCK_N ? (128 / sizeof(OutT)) : BLOCK_N;
+  static constexpr int ROW_BYTES = CW * sizeof(OutT);
+  static constexpr int BOX_BYTES = 64 * ROW_BYTES;
+  // 128-byte rows use the SWIZZLE_128B layout (conflict-free for the accumulator pattern); the 64-byte rows of the
+  // 32-wide tile are stored plain
+  static constexpr bool SWIZZLE = ROW_BYTES == 128;
+  static __device__ __forceinline__ uint32_t at(uint32_t lin) { return SWIZZLE ? sw128(lin) : lin; }
+  static constexpr int CHUNKS = BLOCK_N / CW;
+  static constexpr int PER_PASS = Cfg<BLOCK_N>::EPI_SLOTS < CHUNKS ? Cfg<BLOCK_N>::EPI_SLOTS : CHUNKS;
+  static constexpr int PASSES = CHUNKS / PER_PASS;
+  static_assert(CHUNKS % PER_PASS == 0, "whole passes");
+};
+
 template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR>
-__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB, OutT* D, const OutT* C, int M,
-                                          int N, int K, int ldd, int n_fast, const EpiExtra& ex) {
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmD,
+                                          const CUtensorMap* tmC, const CUtensorMap* tmD2, const CUtensorMap* tmBias,
+                                          int M, int N, int K, int n_fast, const EpiExtra& ex) {
   using cfg = Cfg<BLOCK_N>;
+  using epi = Epi<BLOCK_N, OutT>;
   constexpr int STAGES = cfg::STAGES;
   constexpr int TILE_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * cfg::STAGE_BYTES);
+  uint8_t* staging = smem + cfg::EPI_OFFSET;  // warpgroup wg's boxes: staging + (wg * EPI_SLOTS + q) * EPI_SLOT_BYTES
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + cfg::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
+  // per consumer warpgroup: c_full = the tile's addend C has landed in its staging; c_free = the staging's previous
+  // TMA stores have read it, so the producer may load the next tile's C there
+  uint64_t* c_full = empty_bar + STAGES;
+  uint64_t* c_free = c_full + 2;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+  // the producer TMA-loads the tile's addend C and bias into shared memory ahead of the epilogue
+  const bool bias = sizeof(OutT) == 2 && ex.bias != nullptr;
+  const bool addend = ex.c || bias;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(tmA);
     tma_prefetch_desc(tmB);
+    tma_prefetch_desc(tmD);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], PAIR ? 16 : 8);  // one arrival per consumer warp (of both CTAs)
+    }
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&c_full[w], 1);
+      mbar_init(&c_free[w], 1);
     }
     fence_barrier_init();
   }
@@ -176,7 +215,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
-      uint32_t phase = 0;
+      uint32_t phase = 0, c_phase = 0;
+      // the addend's first pass (and the tile's bias) is loaded once the tile's first min(num_kb, STAGES) k-blocks are in flight: the ring
+      // is full then, and the consumers free the staging at their first k-block of the tile
+      const int c_at = (num_kb < STAGES ? num_kb : STAGES) - 1;
       for (int tile = first; tile < num_tiles; tile += stride) {
         int mi, ni;
         tile_coords(tile, num_m, num_n, n_fast, mi, ni);
@@ -214,6 +256,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
               tma_load_2d(sb + a * (BLOCK_K * 128), tmB, &full_bar[stage], n0 + a * 64, k0);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (addend && kb == c_at) {
+            for (int w = 0; w < 2; ++w) {
+              mbar_wait(&c_free[w], c_phase);
+              mbar_arrive_expect_tx(&c_full[w], (ex.c ? epi::PER_PASS * epi::BOX_BYTES : 0) + (bias ? BLOCK_N * 2 : 0));
+              if (ex.c)
+                for (int q = 0; q < epi::PER_PASS; ++q)
+                  tma_load_2d(staging + (w * cfg::EPI_SLOTS + q) * EPI_SLOT_BYTES, tmC, &c_full[w], n0 + q * epi::CW,
+                              m0 + w * 64);
+              if (bias) tma_load_2d(smem + cfg::BIAS_OFFSET + w * cfg::BIAS_BYTES, tmBias, &c_full[w], n0, 0);
+            }
+            c_phase ^= 1;
+          }
         }
       }
     }
@@ -224,13 +278,16 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
     constexpr uint32_t b_kstep = B_MN ? (WG_K * 128) : (WG_K * 2);
     constexpr uint32_t a_lbo = A_MN ? (BLOCK_K * 128) : 16;
     constexpr uint32_t b_lbo = B_MN ? (BLOCK_K * 128) : 16;
+    // one elected thread per warpgroup issues the staging's TMA stores and waits for them; the named barrier
+    // (1 + wg) covers that warpgroup's 128 threads only
+    const bool elected = (threadIdx.x & 127) == 0;
+    uint8_t* stg = staging + wg * cfg::EPI_SLOTS * EPI_SLOT_BYTES;
+    const uint32_t stg_s = smem_u32(stg);
+    const uint32_t bias_s = smem_u32(smem + cfg::BIAS_OFFSET) + wg * cfg::BIAS_BYTES;
     float acc[BLOCK_N / 2];
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, c_phase = 0;
     for (int tile = first; tile < num_tiles; tile += stride) {
-      int mi, ni;
-      tile_coords(tile, num_m, num_n, n_fast, mi, ni);
-      const int m0 = mi * TILE_M + rank * BLOCK_M, n0 = ni * BLOCK_N;
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -242,6 +299,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           Wgmma<BLOCK_N>::template ss<A_MN, B_MN>(acc, desc_add(da, k * a_kstep), desc_add(db, k * b_kstep),
                                                   (kb | k) != 0);
         wg_commit();
+        // with the first k-block's MMAs running, hand the staging to the producer for this tile's C once the
+        // previous tile's stores have read it
+        if (addend && kb == 0 && elected) {
+          bulk_wait_read<0>();
+          mbar_arrive(&c_free[wg]);
+        }
         // the previous k-block's MMAs have retired once at most this one is in flight: free its stage
         wg_wait<1>();
         if (prev >= 0 && lane == 0) release_stage<PAIR>(&empty_bar[prev], rank);
@@ -252,24 +315,93 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
       wg_fence_regs(acc);
       if (lane == 0) release_stage<PAIR>(&empty_bar[prev], rank);
 
-      // epilogue: registers -> global (the producer is already loading the next tile)
-      const int r0 = m0 + wg * 64 + wi * 16 + (lane >> 2);
-      const int c0 = n0 + 2 * (lane & 3);
+      // epilogue: registers (+ C from the staging) -> staging -> TMA store; the producer is already loading the
+      // next tile, and the stores drain while the next tile's MMAs run. acc[4 j + 2 h + e] is row
+      // 16 wi + lane / 4 + 8 h of the warpgroup's 64, column 8 j + 2 (lane % 4) + e of the tile.
+      int mi, ni;  // (derived here, not kept in registers through the k-loop)
+      tile_coords(tile, num_m, num_n, n_fast, mi, ni);
+      const int n0 = ni * BLOCK_N;
+      const int mw = mi * TILE_M + rank * BLOCK_M + wg * 64;
+      const int row_lo = wi * 16 + (lane >> 2);
 #pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int col = c0 + 8 * j;
-        if (col >= N) continue;
-        const bool two = col + 1 < N;
+      for (int p = 0; p < epi::PASSES; ++p) {
+        if (ex.c) {
+          if (p > 0 && elected) {  // the previous pass's stores have read the staging: load this pass's C
+            bulk_wait_read<0>();
+            mbar_arrive_expect_tx(&c_full[wg], epi::PER_PASS * epi::BOX_BYTES);
+            for (int q = 0; q < epi::PER_PASS; ++q)
+              tma_load_2d(stg + q * EPI_SLOT_BYTES, tmC, &c_full[wg], n0 + (p * epi::PER_PASS + q) * epi::CW, mw);
+          }
+          mbar_wait(&c_full[wg], c_phase);
+          c_phase ^= 1;
+        } else if (bias && p == 0) {  // the bias has landed (and, as for C, the previous stores have read the staging)
+          mbar_wait(&c_full[wg], c_phase);
+          c_phase ^= 1;
+        } else {
+          if (elected) bulk_wait_read<0>();
+          named_bar_sync(1 + wg, 128);
+        }
+        // the flags are uniform: one straight-line body per combination
+        auto combine = [&](auto add_c, auto bias) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          if (row >= M) continue;
-          const size_t off = static_cast<size_t>(row) * ldd + col;
-          store_pair(D + off, C ? C + off : nullptr, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], two,
-                     ex.bias ? ex.bias + col : nullptr, ex.act, ex.d2 ? ex.d2 + off : nullptr);
+          for (int q = 0; q < epi::PER_PASS; ++q) {
+#pragma unroll
+            for (int jj = 0; jj < epi::CW / 8; ++jj) {
+              const int j = (p * epi::PER_PASS + q) * (epi::CW / 8) + jj;
+              const int cb = 8 * jj + 2 * (lane & 3);  // column within the chunk
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t at = stg_s + q * EPI_SLOT_BYTES +
+                                    epi::at((row_lo + 8 * h) * epi::ROW_BYTES + cb * static_cast<int>(sizeof(OutT)));
+                epi_pair<decltype(add_c)::value, decltype(bias)::value>(
+                    at, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bias_s + 2 * (8 * j + 2 * (lane & 3)),
+                    ex.act == 1, OutT{});
+              }
+            }
+          }
+        };
+        using yes = std::true_type;
+        using no = std::false_type;
+        if (bias) {
+          if (ex.c) combine(yes{}, yes{});
+          else combine(no{}, yes{});
+        } else {
+          if (ex.c) combine(yes{}, no{});
+          else combine(no{}, no{});
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + wg, 128);
+        if (elected) {
+          for (int q = 0; q < epi::PER_PASS; ++q)
+            tma_store_2d(tmD, stg + q * EPI_SLOT_BYTES, n0 + (p * epi::PER_PASS + q) * epi::CW, mw);
+          bulk_commit();
+        }
+        // (fp32 outputs run on tiles >= 128 wide, whose passes are whole 64-column bf16 boxes)
+        if constexpr (sizeof(OutT) == 4 && epi::PER_PASS * epi::CW % 64 == 0) {
+          if (ex.d2) {  // the pass's columns once more, rounded to bf16: 64-column boxes over the same staging
+            if (elected) bulk_wait_read<0>();
+            named_bar_sync(1 + wg, 128);
+#pragma unroll
+            for (int jp = 0; jp < epi::PER_PASS * epi::CW / 8; ++jp) {
+              const int j = p * epi::PER_PASS * epi::CW / 8 + jp;
+              const int cp = 8 * jp + 2 * (lane & 3);  // column within the pass
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                st_shared_b32(stg_s + (cp / 64) * EPI_SLOT_BYTES + sw128((row_lo + 8 * h) * 128 + (cp % 64) * 2),
+                              pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+            }
+            fence_proxy_async_smem();
+            named_bar_sync(1 + wg, 128);
+            if (elected) {
+              for (int b = 0; b < epi::PER_PASS * epi::CW / 64; ++b)
+                tma_store_2d(tmD2, stg + b * EPI_SLOT_BYTES, n0 + p * epi::PER_PASS * epi::CW + b * 64, mw);
+              bulk_commit();
+            }
+          }
         }
       }
     }
+    if (elected) bulk_wait<0>();  // the last stores have completed before the CTA's shared memory goes away
   }
   if constexpr (PAIR) {
     __syncwarp();
@@ -280,16 +412,20 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 OutT* D, const OutT* C, int M, int N, int K, int ldd, int n_fast, EpiExtra ex) {
-  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(&tmA, &tmB, D, C, M, N, K, ldd, n_fast, ex);
+                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmC,
+                 const __grid_constant__ CUtensorMap tmD2, const __grid_constant__ CUtensorMap tmBias, int M, int N,
+                 int K, int n_fast, EpiExtra ex) {
+  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(&tmA, &tmB, &tmD, &tmC, &tmD2, &tmBias, M, N, K, n_fast, ex);
 }
 
 // 256 x 256 tiles on a 2-CTA cluster with the B operand multicast (block_n = 512)
 template <bool A_MN, bool B_MN, typename OutT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      OutT* D, const OutT* C, int M, int N, int K, int ldd, int n_fast, EpiExtra ex) {
-  gemm_body<PAIR_N, A_MN, B_MN, OutT, true>(&tmA, &tmB, D, C, M, N, K, ldd, n_fast, ex);
+                      const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmC,
+                      const __grid_constant__ CUtensorMap tmD2, const __grid_constant__ CUtensorMap tmBias, int M,
+                      int N, int K, int n_fast, EpiExtra ex) {
+  gemm_body<PAIR_N, A_MN, B_MN, OutT, true>(&tmA, &tmB, &tmD, &tmC, &tmD2, &tmBias, M, N, K, n_fast, ex);
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR = false>
@@ -302,7 +438,21 @@ void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, 
                          : make_tmap_bf16_2d(A, M, K, lda, BLOCK_M, BLOCK_K);
   CUtensorMap tmB = B_MN ? make_tmap_bf16_2d(B, K, N, ldb, BLOCK_K, 64)
                          : make_tmap_bf16_2d(B, N, K, ldb, PAIR ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
-  void (*kern)(CUtensorMap, CUtensorMap, OutT*, const OutT*, int, int, int, int, int, EpiExtra);
+  // D and C: [M rows, N cols] with row stride ldd in boxes of 64 rows (one consumer warpgroup) x one staging chunk;
+  // TMA leaves out what lies past M, N
+  using epi = Epi<BLOCK_N, OutT>;
+  auto out_map = [&](const void* p) {
+    return sizeof(OutT) == 4 ? make_tmap_f32_2d(p, M, N, ldd, 64, epi::CW)
+                             : make_tmap_bf16_2d(p, M, N, ldd, 64, epi::CW, epi::SWIZZLE);
+  };
+  const CUtensorMap tmD = out_map(D);
+  const CUtensorMap tmC = C ? out_map(C) : tmD;
+  const CUtensorMap tmD2 = ex.d2 ? make_tmap_bf16_2d(ex.d2, M, N, ldd, 64, 64) : tmD;
+  // bias: one row of N columns in boxes of the tile's width, stored plain (columns past N arrive as zeros)
+  const CUtensorMap tmBias = ex.bias ? make_tmap_bf16_2d(ex.bias, 1, N, (N + 7) / 8 * 8, 1, BLOCK_N, false) : tmD;
+  ex.c = C != nullptr;
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, int,
+               EpiExtra);
   if constexpr (PAIR) kern = gemm_bf16_pair_kernel<A_MN, B_MN, OutT>;
   else kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, OutT>;
   static PerDeviceOnce once;  // per template instantiation
@@ -313,7 +463,7 @@ void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, 
   const int num_tiles = ((M + TILE_M - 1) / TILE_M) * ((N + BLOCK_N - 1) / BLOCK_N);
   const int slots = (sm_count() - gemm_sm_reserve()) / (PAIR ? 2 : 1);
   const int grid = (num_tiles < slots ? num_tiles : slots) * (PAIR ? 2 : 1);
-  kern<<<grid, GEMM_THREADS, cfg::SMEM_BYTES, stream>>>(tmA, tmB, D, C, M, N, K, ldd,
+  kern<<<grid, GEMM_THREADS, cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmC, tmD2, tmBias, M, N, K,
                                                         pick_raster(M, N, K, TILE_M, BLOCK_N), ex);
   B200W_CUDA(cudaGetLastError());
 }
@@ -756,12 +906,12 @@ void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, i
   B200W_CHECK((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bias must be 16-byte aligned");
   B200W_CHECK(!d2_bf16 || (out_fp32 && ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(d2_bf16) & 15) == 0),
               "the bf16 copy exists for fp32 outputs with 16-byte aligned bf16 rows");
-  const EpiExtra ex{static_cast<const __nv_bfloat16*>(bias), act, static_cast<__nv_bfloat16*>(d2_bf16)};
+  const EpiExtra ex{static_cast<const __nv_bfloat16*>(bias), act, static_cast<__nv_bfloat16*>(d2_bf16), false};
   B200W_CHECK(M > 0 && N > 0 && K > 0, "empty GEMM");
   B200W_CHECK(lda % 8 == 0 && ldb % 8 == 0, "TMA needs 16-byte aligned row strides");
   B200W_CHECK(ldd % (out_fp32 ? 4 : 8) == 0, "output rows must be 16-byte aligned");
   B200W_CHECK((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(D) & 15) == 0,
+                  (reinterpret_cast<uintptr_t>(D) & 15) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0,
               "operands must be 16-byte aligned");
   if (block_n == 0) {
     // widest tile that still gives every SM a tile; K-major-only narrow tiles when M fits one tile

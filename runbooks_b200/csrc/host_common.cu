@@ -25,24 +25,34 @@ EncodeTiledFn encode_fn() {
   });
   return fn;
 }
-}  // namespace
 
-CUtensorMap make_tmap_bf16_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                              uint32_t box_rows, uint32_t box_cols) {
-  B200W_CHECK(box_cols * 2 <= 128 && box_rows <= 256, "box exceeds SWIZZLE_128B / TMA limits");
-  B200W_CHECK((ld * 2) % 16 == 0, "row stride must be a multiple of 16 bytes");
+CUtensorMap make_tmap_2d(CUtensorMapDataType type, uint32_t elem_bytes, const void* base, uint64_t rows,
+                         uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols, bool swizzle) {
+  B200W_CHECK((!swizzle || box_cols * elem_bytes <= 128) && box_cols <= 256 && box_rows <= 256,
+              "box exceeds SWIZZLE_128B / TMA limits");
+  B200W_CHECK((ld * elem_bytes) % 16 == 0, "row stride must be a multiple of 16 bytes");
   CUtensorMap m;
   cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {ld * 2};
+  cuuint64_t gstride[1] = {ld * elem_bytes};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estride[2] = {1, 1};
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim,
+  CUresult r = encode_fn()(&m, type, 2, const_cast<void*>(base), gdim,
                            gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     throw Error("cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
   return m;
+}
+}  // namespace
+
+CUtensorMap make_tmap_bf16_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                              uint32_t box_rows, uint32_t box_cols, bool swizzle) {
+  return make_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, rows, cols, ld, box_rows, box_cols, swizzle);
+}
+CUtensorMap make_tmap_f32_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                             uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, rows, cols, ld, box_rows, box_cols, true);
 }
 
 int sm_count() {

@@ -33,10 +33,14 @@ struct Error : std::runtime_error {
   } while (0)
 
 // 2-D bf16 row-major tensor [rows, cols] with leading dimension ld (elements).
-// Box = [box_rows, box_cols]; box_cols * 2 bytes must be <= 128 (SWIZZLE_128B span).
+// Box = [box_rows, box_cols], each at most 256; box_cols * 2 bytes must be <= 128 (SWIZZLE_128B span) when swizzled.
 // Out-of-bounds elements are zero-filled by the hardware (used for K / M / N tails).
+// swizzle = false: the box is stored in shared memory as plain rows (no SWIZZLE_128B permutation).
 CUtensorMap make_tmap_bf16_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                              uint32_t box_rows, uint32_t box_cols);
+                              uint32_t box_rows, uint32_t box_cols, bool swizzle = true);
+// The same for fp32 elements (box_cols * 4 bytes <= 128).
+CUtensorMap make_tmap_f32_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                             uint32_t box_rows, uint32_t box_cols);
 
 // SM count of the CURRENT device (cached per device: a process may hold contexts on several GPUs)
 int sm_count();

@@ -140,6 +140,48 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_sr
       : "memory");
 }
 
+// 2-D tiled store shared -> global into the issuing thread's current bulk async-group. Parts of the box outside the
+// tensor map's extent are not written. The source must be made visible to the async proxy first
+// (fence_proxy_async_smem) and stays in use until bulk_wait_read says it has been read.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk async-groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's bulk async-groups are incomplete (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// barrier over `threads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// shared-memory accesses by 32-bit shared address
+__device__ __forceinline__ void st_shared_b32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_v2f32(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_v2f32(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
+
 // ------------------------------------------------------------------------------------------
 // register reallocation between warpgroups: every warp of a warpgroup executes the same one. A producer warpgroup
 // gives registers back (dec) so that the consumer warpgroups can take them (inc); the block's total must stay

@@ -631,6 +631,143 @@ def wg_gemm_kernel(num_items, rng, stages=4, ctas=1, **kw):
     return wg_ring_kernel(num_items, stages, rng, ctas=ctas, lag=1, **kw)
 
 
+def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, threads=2, addend=True,
+                            free_after_read=True, later_pass_waits_read=True):
+    """gemm_bf16_kernel's epilogue: each of two consumer warpgroups (`threads` threads, thread 0 elected) writes a
+    tile into its shared-memory staging in `passes` passes and the elected thread TMA-stores each pass. With an addend
+    (C and / or bias) the producer loads the first pass's C into the staging on c_full once the tile's first
+    min(num_kb, stages) k-blocks are issued, after waiting on c_free, which the elected thread arrives on at its first
+    k-block once its previous stores have read the staging (`free_after_read`); later passes' C is loaded by the
+    elected thread after the previous pass's store has read the staging (`later_pass_waits_read`). Without an addend
+    the elected thread waits for that read and the warpgroup meets at its named barrier before writing. TMA copies in
+    flight (operand and C loads landing, stores reading the staging) complete in any order."""
+    W = 2
+    copies = []                                           # async copies in flight
+    full = [Mbar(1) for _ in range(stages)]
+    empty = [Mbar(W * threads) for _ in range(stages)]    # one arrival per consumer warp
+    slot = [None] * stages
+    c_full = [Mbar(1) for _ in range(W)]
+    c_free = [Mbar(1) for _ in range(W)]
+    stg = [[None] * threads for _ in range(W)]            # what each thread's part of a warpgroup's staging holds
+    reading = [0] * W                                     # a warpgroup's stores that have not read the staging yet
+    barr = [[0, 0] for _ in range(W)]                     # named barrier: arrivals, generation
+    state = dict(live=1 + W * threads, stored=[])
+
+    def load_c(w, t, p):
+        def land():
+            if reading[w]:
+                raise Violation(f"C of tile {t} pass {p} landed in warpgroup {w}'s staging before its store had read it")
+            stg[w] = [("C", t, p)] * threads
+            c_full[w].arrive()
+        copies.append(land)
+
+    def store(w, t, p):
+        def read():
+            if stg[w] != [("D", t, p)] * threads:
+                raise Violation(f"store of tile {t} pass {p} read warpgroup {w}'s staging holding {stg[w]}")
+            reading[w] -= 1
+            state["stored"].append((w, t, p))
+        reading[w] += 1
+        copies.append(read)
+
+    def barrier(w):
+        g = barr[w][1]
+        barr[w][0] += 1
+        if barr[w][0] == threads:
+            barr[w][0], barr[w][1] = 0, g + 1
+        yield (lambda: barr[w][1] != g)
+
+    def producer():
+        stage = phase = cph = 0
+        c_at = min(num_kb, stages) - 1
+        for t in range(num_tiles):
+            for kb in range(num_kb):
+                ph = phase
+                yield (lambda s=stage, ph=ph: empty[s].passed(ph ^ 1))
+
+                def land(s=stage, tag=(t, kb)):
+                    slot[s] = tag
+                    full[s].arrive()
+                copies.append(land)
+                stage += 1
+                if stage == stages:
+                    stage, phase = 0, phase ^ 1
+                if addend and kb == c_at:
+                    for w in range(W):
+                        c = cph
+                        yield (lambda w=w, c=c: c_free[w].passed(c))
+                        load_c(w, t, 0)
+                    cph ^= 1
+                yield None
+        state["live"] -= 1
+
+    def consumer(w, i):
+        elected = i == 0
+        stage = phase = cph = 0
+        for t in range(num_tiles):
+            prev = None
+            for kb in range(num_kb):
+                ph = phase
+                yield (lambda s=stage, ph=ph: full[s].passed(ph))
+                if slot[stage] != (t, kb):
+                    raise Violation(f"consumer {(w, i)} found k-block {slot[stage]} for {(t, kb)}")
+                if addend and kb == 0 and elected:
+                    if free_after_read:
+                        yield (lambda: reading[w] == 0)
+                    c_free[w].arrive()
+                if prev is not None:
+                    empty[prev].arrive()
+                prev = stage
+                stage += 1
+                if stage == stages:
+                    stage, phase = 0, phase ^ 1
+                yield None
+            empty[prev].arrive()
+            for p in range(passes):
+                if addend:
+                    if p > 0 and elected:
+                        if later_pass_waits_read:
+                            yield (lambda: reading[w] == 0)
+                        load_c(w, t, p)
+                    c = cph
+                    yield (lambda c=c: c_full[w].passed(c))
+                    cph ^= 1
+                    if stg[w][i] != ("C", t, p):
+                        raise Violation(f"thread {(w, i)} read C {stg[w][i]} for tile {t} pass {p}")
+                else:
+                    if elected:
+                        yield (lambda: reading[w] == 0)
+                    yield from barrier(w)
+                stg[w][i] = ("D", t, p)
+                yield from barrier(w)
+                if elected:
+                    store(w, t, p)
+                yield None
+        if elected:
+            yield (lambda: reading[w] == 0)
+        state["live"] -= 1
+
+    def engine():
+        while True:
+            if copies:
+                copies.pop(rng.randrange(len(copies)))()
+                yield None
+            elif state["live"] == 0:
+                return
+            else:
+                yield (lambda: bool(copies) or state["live"] == 0)
+
+    agents = {"tma": producer(), "copies": engine()}
+    for w in range(W):
+        for i in range(threads):
+            agents[f"c{w}{i}"] = consumer(w, i)
+    res = run(agents, rng)
+    if res == "ok" and sorted(state["stored"]) != sorted((w, t, p) for w in range(W) for t in range(num_tiles)
+                                                         for p in range(passes)):
+        raise Violation(f"stores {sorted(state['stored'])}")
+    return res
+
+
 def explore(kernel, trials, seed=0, **kw):
     """-> (#ok, first violation or None, other outcomes)"""
     ok, first, other = 0, None, {}
