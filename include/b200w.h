@@ -237,6 +237,19 @@ B200W_API int64_t b200w_infer_device_bytes(b200w_ctx* ctx);
  * n_seqs * padded_len > prefill_tokens is B200W_ERR_INVALID. */
 B200W_API int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
                                      int64_t prefill_tokens);
+/* Element type of the paged KV cache. B200W_KV_FP8_E4M3: K and V are stored as e4m3 bytes with one fp32 scale per
+ * (position, kv head), scale = amax / 448 over the head's values (DESIGN §3.5): a page costs
+ * 2 * num_layers * 128 * (Hkv * dh + 4 * Hkv) bytes instead of 2 * num_layers * 128 * Hkv * dh * 2. */
+typedef enum { B200W_KV_BF16 = 0, B200W_KV_FP8_E4M3 = 1 } b200w_kv_dtype;
+/* b200w_infer_init_paged with the cache's element type; an unknown kv_dtype is B200W_ERR_INVALID.
+ * b200w_infer_init_paged is this call with B200W_KV_BF16. */
+B200W_API int b200w_infer_init_paged_kv(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
+                                        int64_t prefill_tokens, int kv_dtype /* a b200w_kv_dtype value */);
+/* Test aid: the raw cache rows of positions [pos0, pos0 + n) of `slot` in `layer`, read through the page table into
+ * HOST buffers: k_out / v_out [n, Hkv * dh] bf16, or e4m3 bytes on an fp8 cache with k_scale_out / v_scale_out
+ * [n, Hkv] fp32 (ignored, and may be NULL, on a bf16 cache). Paged: the positions must lie in pages the slot holds. */
+B200W_API int b200w_infer_kv_read(b200w_ctx* ctx, int layer, int slot, int pos0, int n, void* k_out, void* v_out,
+                                  float* k_scale_out, float* v_scale_out);
 /* Releases what `slot` holds, then gives it ceil(n_tokens / 128) pages (n_tokens in 1..max_ctx) from a LIFO
  * free list. B200W_ERR_OOM when too few pages are free; nothing changes then. The page table reaches the
  * device before the next step or prefill. The four page calls return B200W_ERR_STATE on a contiguous cache. */
@@ -339,6 +352,24 @@ B200W_API int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int l
                                             const int32_t* table, int nsplit, const int32_t* slots,
                                             const int32_t* starts, const int32_t* lengths, void* out, int ld_out,
                                             int n_seqs, int S, int H, int Hkv, int dh, float scale);
+/* The same over an fp8 (e4m3) cache: kcache / vcache bytes [cache_rows, Hkv * dh], kscale / vscale fp32
+ * [cache_rows, Hkv] (b200w_infer_init_paged_kv). */
+B200W_API int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride,
+                                                const void* kcache, const void* vcache, const float* kscale,
+                                                const float* vscale, int64_t cache_rows, const int32_t* table,
+                                                int nsplit, const int32_t* slots, const int32_t* starts,
+                                                const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
+                                                int H, int Hkv, int dh, float scale);
+/* The decode step's attention over an fp8 pool on its own (the engine's kernels: CUDA cores when H / Hkv < 4,
+ * tensor cores otherwise). q [n, ld_q] (ld_q >= (H + 2 Hkv) dh, the step's QKV rows): row r's query head h at column
+ * h * dh, at position positions[r] of cache slot slots[r]; it attends to positions [0, positions[r]] through
+ * table [*, nsplit] (nsplit * 128 <= 8192). kcache / vcache / kscale / vscale as in
+ * b200w_op_attention_fwd_cached_fp8. out [n, ld_out], head h at column h * dh. scale must be 1 / sqrt(dh). */
+B200W_API int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache,
+                                            const void* vcache, const float* kscale, const float* vscale,
+                                            int64_t cache_rows, const int32_t* table, int nsplit,
+                                            const int32_t* positions, const int32_t* slots, void* out, int ld_out,
+                                            int n, int H, int Hkv, int dh, float scale);
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);

@@ -88,6 +88,8 @@ PROTOTYPES = {
     "b200w_infer_prefill": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "b200w_infer_device_bytes": (C.c_int64, [c_ctx]),
     "b200w_infer_init_paged": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int, C.c_int, C.c_int64]),
+    "b200w_infer_init_paged_kv": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "b200w_infer_kv_read": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
     "b200w_infer_reserve": (C.c_int, [c_ctx, C.c_int, C.c_int]),
     "b200w_infer_release": (C.c_int, [c_ctx, C.c_int]),
     "b200w_infer_kv_pages": (C.c_int, [c_ctx, i64p, i64p]),
@@ -126,6 +128,11 @@ PROTOTYPES = {
     "b200w_op_attention_fwd_cached": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
                                                 vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                                 C.c_float]),
+    "b200w_op_attention_fwd_cached_fp8": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp,
+                                                    C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                    C.c_int, C.c_int, C.c_float]),
+    "b200w_op_decode_attention_fp8": (C.c_int, [c_ctx, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
+                                                vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,

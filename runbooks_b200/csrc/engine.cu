@@ -1933,6 +1933,23 @@ int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q
   HOOK(attention_fwd_cached(q, ld_q, q_head_stride, kcache, vcache, cache_rows, table, nsplit, slots, starts, lengths,
                             out, ld_out, n_seqs, S, H, Hkv, dh, scale, ctx->stream));
 }
+int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
+                                      const void* vcache, const float* kscale, const float* vscale, int64_t cache_rows,
+                                      const int32_t* table, int nsplit, const int32_t* slots, const int32_t* starts,
+                                      const int32_t* lengths, void* out, int ld_out, int n_seqs, int S, int H, int Hkv,
+                                      int dh, float scale) {
+  if (!kscale || !vscale) return B200W_ERR_INVALID;
+  HOOK(attention_fwd_cached(q, ld_q, q_head_stride, kcache, vcache, cache_rows, table, nsplit, slots, starts, lengths,
+                            out, ld_out, n_seqs, S, H, Hkv, dh, scale, ctx->stream, kscale, vscale));
+}
+int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
+                                  const float* kscale, const float* vscale, int64_t cache_rows, const int32_t* table,
+                                  int nsplit, const int32_t* positions, const int32_t* slots, void* out, int ld_out,
+                                  int n, int H, int Hkv, int dh, float scale) {
+  if (!(scale > 0.f) || fabsf(scale * sqrtf(static_cast<float>(dh)) - 1.f) > 1e-6f) return B200W_ERR_INVALID;
+  HOOK(decode_attention_fp8(q, ld_q, kcache, vcache, kscale, vscale, cache_rows, table, nsplit, positions, slots, out,
+                            ld_out, n, H, Hkv, dh, scale, ctx->stream));
+}
 int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {

@@ -54,6 +54,10 @@ CUtensorMap make_tmap_f32_2d(const void* base, uint64_t rows, uint64_t cols, uin
                              uint32_t box_rows, uint32_t box_cols) {
   return make_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, rows, cols, ld, box_rows, box_cols, true);
 }
+CUtensorMap make_tmap_u8_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                            uint32_t box_cols) {
+  return make_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, base, rows, cols, ld, box_rows, box_cols, false);
+}
 
 int sm_count() {
   static int cache[64] = {0};

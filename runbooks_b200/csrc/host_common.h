@@ -42,6 +42,10 @@ CUtensorMap make_tmap_bf16_2d(const void* base, uint64_t rows, uint64_t cols, ui
 CUtensorMap make_tmap_f32_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                              uint32_t box_rows, uint32_t box_cols);
 
+// 2-D byte tensor (e4m3 KV cache) [rows, cols], stored in shared memory as plain rows (box_cols a multiple of 16).
+CUtensorMap make_tmap_u8_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                            uint32_t box_cols);
+
 // SM count of the CURRENT device (cached per device: a process may hold contexts on several GPUs)
 int sm_count();
 

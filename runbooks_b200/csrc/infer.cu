@@ -19,9 +19,13 @@
 //   * MQA/GQA decode attention ON THE TENSOR CORES (decode_attn_tc_kernel): the query heads that share a
 //     kv head are the M dimension of a wgmma tile (Falcon-7B: 71 of 128 rows), S = Q K^T and O = P V
 //     per 128-key block, partial (max, sum, O) per block merged by a second kernel.
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <math.h>
 #include <math.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include <algorithm>
 #include <memory>
@@ -244,6 +248,142 @@ __global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld
   }
 }
 
+// ---- the fp8 (e4m3) pool (b200w_infer_init_paged_kv, DESIGN §3.5) ----
+// A layer's K and V are e4m3 bytes [rows, kd] with one fp32 scale per (row, kv head) in [rows, Hkv]. A head's dh
+// values x (rotated and rounded to bf16, what the bf16 pool would store) are stored as q = e4m3_rn_satfinite(x /
+// scale), scale = amax|x| / 448, both divisions IEEE; amax = 0 stores scale 0 and q = 0. Every e4m3 value is exact
+// in bf16, and the readers apply the scales in fp32.
+__device__ __forceinline__ uint8_t e4m3_rn(float x) {
+  return static_cast<uint8_t>(__nv_cvt_float_to_fp8(x, __NV_SATFINITE, __NV_E4M3));
+}
+// two e4m3 bytes (low byte first) -> two floats, exact
+__device__ __forceinline__ float2 e4m3x2_to_float2(uint32_t two) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two), __NV_E4M3);
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// 8 e4m3 bytes -> 4 bf16x2 words, exact
+__device__ __forceinline__ void e4m3x8_to_bf16(uint2 u, uint32_t* w) {
+  const uint32_t b[2] = {u.x, u.y};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = e4m3x2_to_float2(b[j / 2] >> (16 * (j % 2)));
+    w[j] = pack_bf16x2(f.x, f.y);
+  }
+}
+// One warp stores one head: lane l holds the pairs (x[i], x[i + dh / 2]) of i = l + 32 j, j < np (entries with
+// i >= dh / 2 hold 0 and are not stored).
+__device__ __forceinline__ void quant_head_warp(const float (&lo)[2], const float (&hi)[2], int half,
+                                                uint8_t* __restrict__ dst, float* __restrict__ scale_dst) {
+  const int lane = threadIdx.x & 31;
+  float amax = 0.f;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) amax = fmaxf(amax, fmaxf(fabsf(lo[j]), fabsf(hi[j])));
+  amax = warp_max_f(amax);
+  const float scale = __fdiv_rn(amax, 448.f);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = lane + 32 * j;
+    if (i < half) {
+      dst[i] = amax > 0.f ? e4m3_rn(__fdiv_rn(lo[j], scale)) : 0;
+      dst[i + half] = amax > 0.f ? e4m3_rn(__fdiv_rn(hi[j], scale)) : 0;
+    }
+  }
+  if (lane == 0) *scale_dst = scale;
+}
+// lo / hi of quant_head_warp from a bf16 head at x
+__device__ __forceinline__ void load_head_pairs(const bf16* __restrict__ x, int half, float (&lo)[2], float (&hi)[2]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = lane + 32 * j;
+    lo[j] = i < half ? __bfloat162float(x[i]) : 0.f;
+    hi[j] = i < half ? __bfloat162float(x[i + half]) : 0.f;
+  }
+}
+// rotate_half RoPE of the pairs at position p, rounded to bf16 as the bf16 pool stores them
+__device__ __forceinline__ void rope_pairs(const float* __restrict__ inv_freq, int p, int half, float (&lo)[2],
+                                           float (&hi)[2]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = lane + 32 * j;
+    if (i < half) {
+      float sn, cs;
+      sincosf(static_cast<float>(p) * inv_freq[i], &sn, &cs);
+      const float x1 = lo[j], x2 = hi[j];
+      lo[j] = __bfloat162float(__float2bfloat16_rn(x1 * cs - x2 * sn));
+      hi[j] = __bfloat162float(__float2bfloat16_rn(x2 * cs + x1 * sn));
+    }
+  }
+}
+__device__ __forceinline__ void store_head_pairs(bf16* __restrict__ y, int half, const float (&lo)[2],
+                                                 const float (&hi)[2]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = lane + 32 * j;
+    if (i < half) {
+      y[i] = __float2bfloat16_rn(lo[j]);
+      y[i + half] = __float2bfloat16_rn(hi[j]);
+    }
+  }
+}
+
+// rope_append_kernel for the fp8 pool: one warp per (row, head), the scale being a reduction over the head
+__global__ void rope_append_fp8_kernel(bf16* __restrict__ qkv, int ld, const float* __restrict__ inv_freq,
+                                       const int32_t* __restrict__ pos, const int32_t* __restrict__ slot,
+                                       uint8_t* __restrict__ kcache, uint8_t* __restrict__ vcache,
+                                       float* __restrict__ kscale, float* __restrict__ vscale, int n, int H, int Hkv,
+                                       int dh, int rope, const int32_t* __restrict__ table, int nsplit) {
+  pdl_trigger();
+  pdl_wait();
+  const int half = dh / 2;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (w >= static_cast<long long>(n) * (H + Hkv)) return;   // warp-uniform
+  const int h = static_cast<int>(w % (H + Hkv)), r = static_cast<int>(w / (H + Hkv));
+  const int p = pos[r];
+  bf16* src = qkv + static_cast<size_t>(r) * ld + h * dh;
+  float lo[2], hi[2];
+  load_head_pairs(src, half, lo, hi);
+  if (rope) rope_pairs(inv_freq, p, half, lo, hi);
+  if (h < H) {
+    if (rope) store_head_pairs(src, half, lo, hi);
+    return;
+  }
+  const int hk = h - H;
+  const size_t row = cache_row(table + slot[r] * nsplit, p);
+  quant_head_warp(lo, hi, half, kcache + (row * Hkv + hk) * dh, kscale + row * Hkv + hk);
+  load_head_pairs(qkv + static_cast<size_t>(r) * ld + (H + Hkv + hk) * dh, half, lo, hi);
+  quant_head_warp(lo, hi, half, vcache + (row * Hkv + hk) * dh, vscale + row * Hkv + hk);
+}
+
+// prefill_rope_scatter_kernel for the fp8 pool: one warp per (token, head)
+__global__ void prefill_rope_scatter_fp8_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
+                                                int ld_dst, const float* __restrict__ inv_freq,
+                                                const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
+                                                uint8_t* __restrict__ kcache, uint8_t* __restrict__ vcache,
+                                                float* __restrict__ kscale, float* __restrict__ vscale, int T, int S,
+                                                int H, int Hkv, int dh, int dhp, int rope,
+                                                const int32_t* __restrict__ table, int nsplit,
+                                                const int32_t* __restrict__ start) {
+  const int half = dh / 2, HT = H + 2 * Hkv;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (w >= static_cast<long long>(T) * HT) return;   // warp-uniform
+  const int h = static_cast<int>(w % HT), t = static_cast<int>(w / HT);
+  const int b = t / S, p = t % S + (start ? start[b] : 0);
+  float lo[2], hi[2];
+  load_head_pairs(src + static_cast<size_t>(t) * ld_src + h * dh, half, lo, hi);
+  if (rope && h < H + Hkv) rope_pairs(inv_freq, p, half, lo, hi);
+  store_head_pairs(dst + static_cast<size_t>(t) * ld_dst + h * dhp, half, lo, hi);
+  if (h >= H && p < lens[b]) {
+    const bool is_k = h < H + Hkv;
+    const int hk = is_k ? h - H : h - H - Hkv;
+    const size_t row = cache_row(table + slot[b] * nsplit, p);
+    quant_head_warp(lo, hi, half, (is_k ? kcache : vcache) + (row * Hkv + hk) * dh,
+                    (is_k ? kscale : vscale) + row * Hkv + hk);
+  }
+}
+
 // dst[t, h*dh + c] = src[t, h*dhp + c] for c < dh: drops the head padding after the prefill attention
 __global__ void unpad_heads_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst, int ld_dst,
                                    int T, int H, int dh, int dhp) {
@@ -268,6 +408,11 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* 
 
 // Attention of one new query token per row over its slot's cache [0, pos]. Block = (row, kv head,
 // group of GT query heads that share that kv head): every K/V row is read once per block.
+// decode_attn_fp8_kernel (below) is the same kernel over the e4m3 pool: 8 bytes per 8 dims, a key's K scale
+// (kscale [rows, Hkv]) multiplies its score and its V scale its probability in P V, the row sum running over the
+// unscaled probabilities. It is a copy rather than a second instance of one template body: sharing the body changed
+// the code ptxas makes for the bf16 kernel.
+using fp8 = __nv_fp8_e4m3;
 constexpr int ATT_GT = 8;
 constexpr int ATT_THREADS = 256;
 template <int DH>
@@ -387,6 +532,129 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
   }
 }
 
+
+template <int DH>
+__global__ void __launch_bounds__(ATT_THREADS)
+decode_attn_fp8_kernel(const bf16* __restrict__ qkv, int ld, const fp8* __restrict__ kcache,
+                   const fp8* __restrict__ vcache, const int32_t* __restrict__ pos,
+                   const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
+                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
+                   const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  extern __shared__ float sm[];
+  pdl_trigger();
+  pdl_wait();
+  const int r = blockIdx.x, hk = blockIdx.y, G = H / Hkv;
+  const int g0 = blockIdx.z * ATT_GT;
+  const int ng = min(ATT_GT, G - g0);
+  const int len = pos[r] + 1;
+  float* sq = sm;                       // [ATT_GT][DH]
+  float* sc = sq + ATT_GT * DH;         // [ATT_GT][sc_stride]; reused to combine output slices
+  float* red = sc + ATT_GT * sc_stride; // [32]
+  const int tid = threadIdx.x;
+  for (int i = tid; i < ng * DH; i += ATT_THREADS) {
+    const int g = i / DH, c = i % DH;
+    sq[g * DH + c] = __bfloat162float(qkv[static_cast<size_t>(r) * ld + (hk * G + g0 + g) * DH + c]) * scale;
+  }
+  __syncthreads();
+  const int32_t* prow = table + slot[r] * nsplit;   // the slot's table row
+  // scores: one key position per thread, the K row lives in registers for all ng heads
+  for (int t = tid; t < len; t += ATT_THREADS) {
+    float acc[ATT_GT];
+#pragma unroll
+    for (int g = 0; g < ATT_GT; ++g) acc[g] = 0.f;
+    const size_t row = cache_row(prow, t) * Hkv + hk;
+    const uint2* krow = reinterpret_cast<const uint2*>(kcache + row * DH);
+#pragma unroll
+    for (int c8 = 0; c8 < DH / 8; ++c8) {   // 8 bytes per 8 dims
+      const uint2 u = krow[c8];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 kf = e4m3x2_to_float2((j < 2 ? u.x : u.y) >> (16 * (j % 2)));
+#pragma unroll
+        for (int g = 0; g < ATT_GT; ++g)
+          acc[g] += kf.x * sq[g * DH + c8 * 8 + 2 * j] + kf.y * sq[g * DH + c8 * 8 + 2 * j + 1];
+      }
+    }
+    const float ks = kscale[row];
+#pragma unroll
+    for (int g = 0; g < ATT_GT; ++g) acc[g] *= ks;
+#pragma unroll
+    for (int g = 0; g < ATT_GT; ++g)
+      if (g < ng) sc[g * sc_stride + t] = acc[g];
+  }
+  __syncthreads();
+  // softmax per head
+  float inv_sum[ATT_GT];
+  for (int g = 0; g < ng; ++g) {
+    float m = -INFINITY;
+    for (int t = tid; t < len; t += ATT_THREADS) m = fmaxf(m, sc[g * sc_stride + t]);
+    m = block_reduce(m, red, true);
+    float s = 0.f;
+    for (int t = tid; t < len; t += ATT_THREADS) {
+      const float e = __expf(sc[g * sc_stride + t] - m);
+      sc[g * sc_stride + t] = e;   // the V scale joins in P V, once per key for all heads
+      s += e;
+    }
+    inv_sum[g] = 1.f / block_reduce(s, red, false);
+  }
+  __syncthreads();
+  // output: thread = (8 dims via one 16-byte load, position slice); 4 independent positions in
+  // flight per thread; V read once for all ng heads
+  constexpr int DG = DH / 8;                 // 16-byte groups per row
+  constexpr int SLICES = ATT_THREADS / DG;   // 32 (dh 64) or 16 (dh 128) position slices
+  const int dg = tid % DG, sl = tid / DG;
+  float o[ATT_GT][8];
+#pragma unroll
+  for (int g = 0; g < ATT_GT; ++g)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[g][e] = 0.f;
+  for (int t0 = sl; t0 < len; t0 += 4 * SLICES) {
+    uint2 vv[4];   // 8 bytes per 8 dims
+    float vsc[4];  // their V scales
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = t0 + u * SLICES;
+      const size_t row = t < len ? cache_row(prow, t) * Hkv + hk : 0;
+      vv[u] = t < len ? *reinterpret_cast<const uint2*>(vcache + row * DH + dg * 8) : make_uint2(0, 0);
+      vsc[u] = t < len ? vscale[row] : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = t0 + u * SLICES;
+      if (t < len) {
+        float vf[8];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = e4m3x2_to_float2((j < 2 ? vv[u].x : vv[u].y) >> (16 * (j % 2)));
+          vf[2 * j] = f.x;
+          vf[2 * j + 1] = f.y;
+        }
+#pragma unroll
+        for (int g = 0; g < ATT_GT; ++g) {
+          const float p = sc[g * sc_stride + t] * vsc[u];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[g][e] += p * vf[e];
+        }
+      }
+    }
+  }
+  __syncthreads();  // scores are dead: reuse their space to combine the slices
+  float* so = sc;   // [SLICES][ATT_GT][DH]: sc_stride >= SLICES * dh (decode_attention)
+#pragma unroll
+  for (int g = 0; g < ATT_GT; ++g)
+    if (g < ng) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) so[(sl * ATT_GT + g) * DH + dg * 8 + e] = o[g][e];
+    }
+  __syncthreads();
+  for (int i = tid; i < ng * DH; i += ATT_THREADS) {
+    const int g = i / DH, dim = i % DH;
+    float a = 0.f;
+    for (int s2 = 0; s2 < SLICES; ++s2) a += so[(s2 * ATT_GT + g) * DH + dim];
+    out[static_cast<size_t>(r) * ldo + (hk * G + g0 + g) * DH + dim] = __float2bfloat16_rn(a * inv_sum[g]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Decode attention on the tensor cores (wgmma) for grouped / multi-query models. CTA = (128-key block,
 // kv head, row). The G = H / Hkv query heads of the group are rows of a 128-row tile (zero rows above G),
@@ -410,13 +678,37 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-static_assert(TC_KB == KV_PAGE, "a key block of the tensor-core decode attention is one cache page");
+// fp8 pool: the block's K and V arrive as one e4m3 box each ([128 keys x DH] bytes, unswizzled) in the space of sV,
+// and the CTA widens them into the bf16 SWIZZLE_128B tiles the wgmma reads (V last, once every thread holds its part
+// of the staging); the block's 128 K and 128 V scales follow the barrier, in TC_SCALE_BYTES more shared memory.
+constexpr int TC_SCALE_BYTES = 2 * TC_KB * 4;
+
+// Widening of a [128 x DH] e4m3 box (row-major bytes) into bf16 SWIZZLE_128B atoms: item i is the box's 16 bytes
+// i * 16, two 16-byte chunks of the tile. u: the item's bytes.
 template <int DH>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
-                      const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
+__device__ __forceinline__ void widen_e4m3_item(uint4 u, uint8_t* __restrict__ dst, int i) {
+  const int row = i / (DH / 16), c = 2 * (i % (DH / 16));   // c: the item's first bf16 chunk along the row
+  uint32_t w[8];
+  e4m3x8_to_bf16(make_uint2(u.x, u.y), w);
+  e4m3x8_to_bf16(make_uint2(u.z, u.w), w + 4);
+  *reinterpret_cast<uint4*>(dst + (c / 8) * TC_ATOM + sw128_offset(row, c % 8)) = make_uint4(w[0], w[1], w[2], w[3]);
+  *reinterpret_cast<uint4*>(dst + (c / 8) * TC_ATOM + sw128_offset(row, c % 8 + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
+}
+// items i0, i0 + step, ... of the box at src
+template <int DH>
+__device__ __forceinline__ void widen_e4m3_box(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int i0,
+                                               int step) {
+  for (int i = i0; i < 8 * DH; i += step) widen_e4m3_item<DH>(reinterpret_cast<const uint4*>(src)[i], dst, i);
+}
+
+static_assert(TC_KB == KV_PAGE, "a key block of the tensor-core decode attention is one cache page");
+template <int DH, typename KV>
+__device__ __forceinline__ void
+decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
                       const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
-                      int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table) {
+                      int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table,
+                      const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
   constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
   const int split = blockIdx.x, hk = blockIdx.y, r = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31;
@@ -442,7 +734,16 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
     fence_barrier_init();
   }
   __syncthreads();
-  if (tid == 0) {
+  float* sS = reinterpret_cast<float*>(sV + NA * TC_ATOM + 64);   // fp8: [K scales | V scales] of the block's keys
+  if constexpr (F8) {
+    const int row0 = table[slot[r] * nsplit + split];
+    if (tid == 0) {
+      mbar_arrive_expect_tx(bar_kv, 2 * TC_KB * DH);
+      tma_load_2d(sV, &tm_k, bar_kv, hk * DH, row0);
+      tma_load_2d(sV + TC_KB * DH, &tm_v, bar_kv, hk * DH, row0);
+    }
+    sS[tid] = (tid < TC_KB ? kscale : vscale)[static_cast<size_t>(row0 + tid % TC_KB) * Hkv + hk];
+  } else if (tid == 0) {
     const int row0 = table[slot[r] * nsplit + split];   // first cache row of this block
     mbar_arrive_expect_tx(bar_kv, 2 * NA * TC_ATOM);
 #pragma unroll
@@ -458,11 +759,22 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
                           : make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4*>(sQ + (c / 8) * TC_ATOM + sw128_offset(g, c % 8)) = v;
   }
+  if constexpr (F8) {
+    mbar_wait(bar_kv, 0);
+    constexpr int NV = 8 * DH / TC_THREADS;   // 16-byte items of the V box per thread
+    uint4 vst[NV];
+#pragma unroll
+    for (int j = 0; j < NV; ++j) vst[j] = reinterpret_cast<const uint4*>(sV + TC_KB * DH)[tid + j * TC_THREADS];
+    widen_e4m3_box<DH>(sV, sK, tid, TC_THREADS);
+    __syncthreads();   // the staging in sV is read: V's bf16 tile may overwrite it
+#pragma unroll
+    for (int j = 0; j < NV; ++j) widen_e4m3_item<DH>(vst[j], sV, tid + j * TC_THREADS);
+  }
   fence_proxy_async_smem();
   __syncthreads();
   const int wg = tid >> 7, wi = (tid >> 5) & 3;
   if (wg * 64 >= G) return;  // warpgroup-uniform: every row of this warpgroup is padding
-  mbar_wait(bar_kv, 0);
+  if constexpr (!F8) mbar_wait(bar_kv, 0);
 
   float s[TC_KB / 2];
   {
@@ -478,6 +790,12 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
   }
   const int valid = min(TC_KB, len - k0);
   const int c0 = 2 * (lane & 3);
+  if constexpr (F8) {   // key column c of the scores times its K scale
+#pragma unroll
+    for (int jj = 0; jj < TC_KB / 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) s[4 * jj + e] *= sS[8 * jj + c0 + (e & 1)];
+  }
   float m[2] = {-INFINITY, -INFINITY};
 #pragma unroll
   for (int jj = 0; jj < TC_KB / 8; ++jj)
@@ -503,6 +821,11 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
       float p1 = ex2f(fmaf(s[4 * jj + 2 * h + 1], scale_log2, -m[h]));
       if (8 * jj + c0 >= valid) p0 = 0.f;
       if (8 * jj + c0 + 1 >= valid) p1 = 0.f;
+      if constexpr (F8) {   // the row sum over the unscaled probabilities, P V over the V-scaled ones
+        l[h] += p0 + p1;
+        pa[jj / 2][(jj & 1) * 2 + h] = pack_bf16x2(p0 * sS[TC_KB + 8 * jj + c0], p1 * sS[TC_KB + 8 * jj + c0 + 1]);
+        continue;
+      }
       // the row sum runs over the bf16-rounded values the PV product will see
       const uint32_t pk = pack_bf16x2(p0, p1);
       const float2 pr = unpack_bf16x2(pk);
@@ -536,6 +859,26 @@ decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_con
     for (int jj = 0; jj < DH / 8; ++jj)
       *reinterpret_cast<float2*>(po + 8 * jj) = make_float2(o[4 * jj + 2 * h], o[4 * jj + 2 * h + 1]);
   }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+                      const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
+                      const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
+                      int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table) {
+  decode_attn_tc<DH, bf16>(tm_k, tm_v, qkv, ld, pos, slot, part_o, part_ml, H, Hkv, nsplit, scale_log2, table, nullptr,
+                           nullptr);
+}
+template <int DH>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+decode_attn_tc_fp8_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+                          const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
+                          const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
+                          int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table,
+                          const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  decode_attn_tc<DH, fp8>(tm_k, tm_v, qkv, ld, pos, slot, part_o, part_ml, H, Hkv, nsplit, scale_log2, table, kscale,
+                          vscale);
 }
 
 // out[r, h*DH + d] = sum_s 2^(m_s - M) O_s[d] / sum_s 2^(m_s - M) l_s over the ceil(len / 128) blocks of row r
@@ -600,6 +943,10 @@ constexpr int CA_PRODUCER_REGS = 24, CA_CONSUMER_REGS = 240;
 static_assert(128 * CA_PRODUCER_REGS + 256 * CA_CONSUMER_REGS <= 65536, "register budget of one CTA per SM");
 template <int DH>
 constexpr int ca_smem_bytes() { return (1 + 2 * CA_STAGES) * (DH / 64) * TC_ATOM + 1024 + 256; }
+// fp8 pool: after the barriers, one staging buffer for a page's e4m3 K and V boxes and a scale ring [CA_STAGES]
+// x [K scales | V scales] of 128 keys each. The producer warpgroup widens the staging into the bf16 ring.
+template <int DH>
+constexpr int ca_fp8_extra_bytes() { return 2 * KV_PAGE * DH + CA_STAGES * 2 * KV_PAGE * 4; }
 
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
@@ -614,13 +961,19 @@ __device__ __forceinline__ void warp_release(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-template <int DH>
-__global__ void __launch_bounds__(CA_THREADS, 1)
-attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                       const __grid_constant__ CUtensorMap tm_v, int q_head_stride, bf16* __restrict__ out,
+// The fp8 instance (KV = fp8): the producer warpgroup loads page j's e4m3 K and V boxes into the staging buffer
+// (bar_st), widens K into K buffer j % CA_STAGES once its free barrier says so and writes the page's K and V scales
+// into scale slot j % CA_STAGES, then arrives on the K full barrier (all 128 threads); the same for V on the V
+// barriers; then a named barrier over the warpgroup before the staging is loaded again. A consumer applies the K and
+// V scales of a sub-block in its softmax and releases the K buffer (and with it the scale slot) only after that.
+template <int DH, typename KV>
+__device__ __forceinline__ void
+attn_fwd_cached(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v, int q_head_stride, bf16* __restrict__ out,
                        int ld_out, const int32_t* __restrict__ table, int nsplit, const int32_t* __restrict__ slots,
                        const int32_t* __restrict__ starts, const int32_t* __restrict__ lens, int n_seqs, int S,
-                       int H, int Hkv, float scale_log2) {
+                       int H, int Hkv, float scale_log2, const float* __restrict__ kscale,
+                       const float* __restrict__ vscale) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
   constexpr int NA = DH / 64;  // 64-element atoms along the head dimension
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -633,6 +986,9 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
   uint64_t* bar_v = bar_k + CA_STAGES;           // [CA_STAGES]
   uint64_t* bar_kfree = bar_v + CA_STAGES;       // [CA_STAGES] the S products that read K buffer b retired
   uint64_t* bar_vfree = bar_kfree + CA_STAGES;   // [CA_STAGES] the P V products that read V buffer b retired
+  uint64_t* bar_st = bar_vfree + CA_STAGES;      // fp8: the staging buffer holds page j's boxes
+  uint8_t* st8 = reinterpret_cast<uint8_t*>(bar_q) + 256;                      // fp8: [K box | V box]
+  float* sS = reinterpret_cast<float*>(st8 + 2 * KV_PAGE * DH);                // fp8: [CA_STAGES][2][128] scales
 
   const int nbh = n_seqs * H;
   const int qi = S / 128 - 1 - static_cast<int>(blockIdx.x) / nbh;   // longest tiles (most pages) first
@@ -652,16 +1008,51 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     tma_prefetch_desc(&tm_v);
     mbar_init(bar_q, 1);
     for (int i = 0; i < CA_STAGES; ++i) {
-      mbar_init(&bar_k[i], 1);
-      mbar_init(&bar_v[i], 1);
+      mbar_init(&bar_k[i], F8 ? 128 : 1);
+      mbar_init(&bar_v[i], F8 ? 128 : 1);
       mbar_init(&bar_kfree[i], CA_CONSUMER_WARPS);
       mbar_init(&bar_vfree[i], CA_CONSUMER_WARPS);
     }
+    if constexpr (F8) mbar_init(bar_st, 1);
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp >> 2 == 2) {
+  if constexpr (F8) {
+    if (warp >> 2 == 2) {
+      setmaxnreg_dec<CA_PRODUCER_REGS>();
+      const int pt = tid - 256;
+      if (pt == 0) {
+        mbar_arrive_expect_tx(bar_q, NA * TC_ATOM);
+#pragma unroll
+        for (int a = 0; a < NA; ++a)
+          tma_load_2d(sQ + a * TC_ATOM, &tm_q, bar_q, h * q_head_stride + a * 64, b * S + qi * 128);
+      }
+      for (int j = 0; j < nkb; ++j) {
+        const int buf = j % CA_STAGES;
+        const uint32_t free_par = (j / CA_STAGES - 1) & 1;
+        const int row0 = prow[j];
+        if (pt == 0) {
+          mbar_arrive_expect_tx(bar_st, 2 * KV_PAGE * DH);
+          tma_load_2d(st8, &tm_k, bar_st, hk * DH, row0);
+          tma_load_2d(st8 + KV_PAGE * DH, &tm_v, bar_st, hk * DH, row0);
+        }
+        mbar_wait(bar_st, j & 1);
+        if (j >= CA_STAGES) mbar_wait(&bar_kfree[buf], free_par);   // also frees scale slot buf
+        widen_e4m3_box<DH>(st8, sK + buf * NA * TC_ATOM, pt, 128);
+        sS[(buf * 2) * KV_PAGE + pt] = kscale[static_cast<size_t>(row0 + pt) * Hkv + hk];
+        sS[(buf * 2 + 1) * KV_PAGE + pt] = vscale[static_cast<size_t>(row0 + pt) * Hkv + hk];
+        fence_proxy_async_smem();
+        mbar_arrive(&bar_k[buf]);
+        if (j >= CA_STAGES) mbar_wait(&bar_vfree[buf], free_par);
+        widen_e4m3_box<DH>(st8 + KV_PAGE * DH, sV + buf * NA * TC_ATOM, pt, 128);
+        fence_proxy_async_smem();
+        mbar_arrive(&bar_v[buf]);
+        named_bar_sync(1, 128);   // every producer thread has read the staging: it may be loaded again
+      }
+      return;
+    }
+  } else if (warp >> 2 == 2) {
     setmaxnreg_dec<CA_PRODUCER_REGS>();
     if (tid == 256) {
       mbar_arrive_expect_tx(bar_q, NA * TC_ATOM);
@@ -758,6 +1149,23 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     }
     l0 = l0 * alpha0 + ps0;  // this thread's part of the row sums
     l1 = l1 * alpha1 + ps1;
+    if constexpr (F8) {   // P V over the V-scaled probabilities
+      const float* vs = sS + ((u / SUB) % CA_STAGES * 2 + 1) * KV_PAGE + (u % SUB) * KB + c0;
+#pragma unroll
+      for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) s[4 * jj + e] *= vs[8 * jj + (e & 1)];
+    }
+  };
+  // fp8: key column c of sub-block u's scores times its K scale (before the causal mask and the maximum)
+  auto scale_k = [&](int u) {
+    if constexpr (F8) {
+      const float* ks = sS + ((u / SUB) % CA_STAGES * 2) * KV_PAGE + (u % SUB) * KB + c0;
+#pragma unroll
+      for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) s[4 * jj + e] *= ks[8 * jj + (e & 1)];
+    }
   };
   auto to_pa = [&] {  // fp32 P columns [16 kk, 16 kk + 16) -> the bf16 A fragment of the kk-th K = 16 slice
 #pragma unroll
@@ -781,8 +1189,14 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
   issue_scores(0);
   wg_wait<0>();
   wg_fence_regs(s);
-  release(bar_kfree, 0);
-  softmax(0);  // O is still 0: its rescale is a no-op
+  if constexpr (F8) {   // the scale slot is released with the K buffer: after the softmax read it
+    scale_k(0);
+    softmax(0);
+    release(bar_kfree, 0);
+  } else {
+    release(bar_kfree, 0);
+    softmax(0);  // O is still 0: its rescale is a no-op
+  }
   to_pa();
   for (int u = 1; u < nsub; ++u) {
     wait_full(bar_k, u);
@@ -791,8 +1205,14 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     issue_pv(u - 1);
     wg_wait<1>();  // S(u) retired; PV(u - 1) may still run
     wg_fence_regs(s);
-    release(bar_kfree, u);
-    softmax(u);
+    if constexpr (F8) {
+      scale_k(u);
+      softmax(u);
+      release(bar_kfree, u);
+    } else {
+      release(bar_kfree, u);
+      softmax(u);
+    }
     wg_wait<0>();  // PV(u - 1) retired: O may be rescaled, pa rewritten and V(u - 1) released
     wg_fence_regs(o);
     release(bar_vfree, u - 1);
@@ -819,6 +1239,28 @@ attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     *reinterpret_cast<uint32_t*>(orow0 + 8 * jj) = pack_bf16x2(o[4 * jj] * inv0, o[4 * jj + 1] * inv0);
     *reinterpret_cast<uint32_t*>(orow1 + 8 * jj) = pack_bf16x2(o[4 * jj + 2] * inv1, o[4 * jj + 3] * inv1);
   }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(CA_THREADS, 1)
+attn_fwd_cached_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                       const __grid_constant__ CUtensorMap tm_v, int q_head_stride, bf16* __restrict__ out,
+                       int ld_out, const int32_t* __restrict__ table, int nsplit, const int32_t* __restrict__ slots,
+                       const int32_t* __restrict__ starts, const int32_t* __restrict__ lens, int n_seqs, int S,
+                       int H, int Hkv, float scale_log2) {
+  attn_fwd_cached<DH, bf16>(tm_q, tm_k, tm_v, q_head_stride, out, ld_out, table, nsplit, slots, starts, lens, n_seqs, S,
+                            H, Hkv, scale_log2, nullptr, nullptr);
+}
+template <int DH>
+__global__ void __launch_bounds__(CA_THREADS, 1)
+attn_fwd_cached_fp8_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                           const __grid_constant__ CUtensorMap tm_v, int q_head_stride, bf16* __restrict__ out,
+                           int ld_out, const int32_t* __restrict__ table, int nsplit,
+                           const int32_t* __restrict__ slots, const int32_t* __restrict__ starts,
+                           const int32_t* __restrict__ lens, int n_seqs, int S, int H, int Hkv, float scale_log2,
+                           const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  attn_fwd_cached<DH, fp8>(tm_q, tm_k, tm_v, q_head_stride, out, ld_out, table, nsplit, slots, starts, lens, n_seqs, S,
+                           H, Hkv, scale_log2, kscale, vscale);
 }
 
 // greedy token: first index of the row maximum (torch.argmax tie-breaking)
@@ -894,6 +1336,20 @@ struct Infer {
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
   bf16 *kc = nullptr, *vc = nullptr;  // [L][layer_rows()][Hkv*dh], zero-initialised
+  // B200W_KV_FP8_E4M3 (paged only): kc / vc are null, K and V are e4m3 bytes [L][layer_rows()][Hkv*dh] with fp32
+  // scales [L][layer_rows()][Hkv] (DESIGN §3.5), all zero-initialised
+  int kv_dtype = B200W_KV_BF16;
+  uint8_t *kq = nullptr, *vq = nullptr;
+  float *ks = nullptr, *vs = nullptr;
+  bool fp8() const { return kv_dtype == B200W_KV_FP8_E4M3; }
+  // layer l's K / V pools and scales: {k, v, k scales, v scales} (scales null for bf16)
+  struct KVLayer { void *k, *v; float *ks, *vs; };
+  KVLayer kv_layer(int l) const {
+    const size_t rows = layer_rows();
+    if (!fp8()) return {kc + l * rows * kd, vc + l * rows * kd, nullptr, nullptr};
+    const size_t n = rows * a.num_kv_heads;
+    return {kq + l * rows * kd, vq + l * rows * kd, ks + l * n, vs + l * n};
+  }
   // the table [max_batch][nsplit] of first cache rows (KV_PAGE above) on the device, written from pinned staging:
   // once at init when contiguous, by b200w_infer_reserve when paged (n_pages > 0). Paged: `held` mirrors it on the
   // host (the pages a slot owns, in table order), `free_pages` is a LIFO stack of the others
@@ -1121,16 +1577,25 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
 }
 
 // the tensor-core decode attention and the merge of its blocks -> out [n, ldo]
-template <int DH>
+template <int DH, typename KV>
 void decode_attention_tc(Infer* m, cudaStream_t s, int n, const CUtensorMap& tk, const CUtensorMap& tv,
-                         float scale_log2, bf16* out, int ldo) {
+                         float scale_log2, bf16* out, int ldo, const float* kscale, const float* vscale) {
   const int H = m->a.num_heads, Hkv = m->a.num_kv_heads;
+  const int smem = tc_smem_bytes<DH>() + (std::is_same<KV, fp8>::value ? TC_SCALE_BYTES : 0);
   static PerDeviceOnce once;
-  once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes<DH>()));
-  });
-  launch_pdl(decode_attn_tc_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), tc_smem_bytes<DH>(), s, tk, tv,
-             m->qkv, m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table);
+  if constexpr (std::is_same<KV, fp8>::value) {
+    once.run([&] {
+      B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_fp8_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    });
+    launch_pdl(decode_attn_tc_fp8_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tk, tv, m->qkv,
+               m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table, kscale, vscale);
+  } else {
+    once.run([&] {
+      B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    });
+    launch_pdl(decode_attn_tc_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tk, tv, m->qkv, m->qkvd,
+               m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table);
+  }
   launch_pdl(decode_attn_merge_kernel<DH>, dim3(cdiv(H, 256 / DH), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
              out, ldo, H, m->nsplit);
 }
@@ -1141,15 +1606,21 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
   const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, G = H / Hkv;
   const float scale = 1.f / sqrtf(static_cast<float>(dh));
   const uint64_t rows = m->layer_rows();
-  bf16* kc = m->kc + layer * rows * m->kd;
-  bf16* vc = m->vc + layer * rows * m->kd;
+  const Infer::KVLayer c = m->kv_layer(layer);
   if (G >= 4) {
     // grouped / multi-query: the group is the M dimension of a tensor-core tile
-    CUtensorMap tk = make_tmap_bf16_2d(kc, rows, m->kd, m->kd, TC_KB, 64);
-    CUtensorMap tv = make_tmap_bf16_2d(vc, rows, m->kd, m->kd, TC_KB, 64);
     const float scale_log2 = scale * 1.4426950408889634f;
-    if (dh == 64) decode_attention_tc<64>(m, s, n, tk, tv, scale_log2, out, ldo);
-    else decode_attention_tc<128>(m, s, n, tk, tv, scale_log2, out, ldo);
+    if (m->fp8()) {   // one unswizzled [128 keys x dh] byte box each
+      CUtensorMap tk = make_tmap_u8_2d(c.k, rows, m->kd, m->kd, TC_KB, dh);
+      CUtensorMap tv = make_tmap_u8_2d(c.v, rows, m->kd, m->kd, TC_KB, dh);
+      if (dh == 64) decode_attention_tc<64, fp8>(m, s, n, tk, tv, scale_log2, out, ldo, c.ks, c.vs);
+      else decode_attention_tc<128, fp8>(m, s, n, tk, tv, scale_log2, out, ldo, c.ks, c.vs);
+    } else {
+      CUtensorMap tk = make_tmap_bf16_2d(c.k, rows, m->kd, m->kd, TC_KB, 64);
+      CUtensorMap tv = make_tmap_bf16_2d(c.v, rows, m->kd, m->kd, TC_KB, 64);
+      if (dh == 64) decode_attention_tc<64, bf16>(m, s, n, tk, tv, scale_log2, out, ldo, nullptr, nullptr);
+      else decode_attention_tc<128, bf16>(m, s, n, tk, tv, scale_log2, out, ldo, nullptr, nullptr);
+    }
     nl += 2;
     return;
   }
@@ -1162,9 +1633,35 @@ void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int
   once.run([&] {
     B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_fp8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_fp8_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   });
-  launch_pdl(dh == 64 ? decode_attn_kernel<64> : decode_attn_kernel<128>, agrid, dim3(ATT_THREADS), att_smem, s,
-             m->qkv, m->qkvd, kc, vc, m->pos, m->slot, out, ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit);
+  if (m->fp8())
+    launch_pdl(dh == 64 ? decode_attn_fp8_kernel<64> : decode_attn_fp8_kernel<128>, agrid, dim3(ATT_THREADS), att_smem,
+               s, m->qkv, m->qkvd, static_cast<const fp8*>(c.k), static_cast<const fp8*>(c.v), m->pos, m->slot, out,
+               ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit, static_cast<const float*>(c.ks),
+               static_cast<const float*>(c.vs));
+  else
+    launch_pdl(dh == 64 ? decode_attn_kernel<64> : decode_attn_kernel<128>, agrid, dim3(ATT_THREADS), att_smem, s,
+               m->qkv, m->qkvd, static_cast<const bf16*>(c.k), static_cast<const bf16*>(c.v), m->pos, m->slot, out,
+               ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit);
+  ++nl;
+}
+
+// the K/V append of a decode step: rotate q and k (rope != 0), k and v into the slot's cache rows
+void append_kv(Infer* m, cudaStream_t s, int n, int layer, int rope, int64_t& nl) {
+  const auto& a = m->a;
+  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
+  const Infer::KVLayer c = m->kv_layer(layer);
+  if (m->fp8()) {   // a warp per (row, head)
+    launch_pdl(rope_append_fp8_kernel, dim3(cdiv(static_cast<long long>(n) * (H + Hkv) * 32, 256)), dim3(256), 0, s,
+               m->qkv, m->qkvd, m->inv_freq, m->pos, m->slot, static_cast<uint8_t*>(c.k), static_cast<uint8_t*>(c.v),
+               c.ks, c.vs, n, H, Hkv, dh, rope, m->table, m->nsplit);
+  } else {
+    const long long rp = static_cast<long long>(n) * (H + Hkv) * (dh / 2);
+    launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, m->qkvd, m->inv_freq, m->pos, m->slot,
+               static_cast<bf16*>(c.k), static_cast<bf16*>(c.v), n, H, Hkv, dh, rope, m->table, m->nsplit);
+  }
   ++nl;
 }
 
@@ -1176,11 +1673,9 @@ void launch_ln(cudaStream_t s, int rows, const bf16* x, const bf16* w, const bf1
 void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   const auto& a = m->a;
   const int B = m->max_batch;
-  const int d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim,
-            V = a.vocab_size;
+  const int d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size;
   const int qd = m->qd, qkvd = m->qkvd;
   const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
-  const size_t layer_cache = m->layer_rows() * m->kd;
   B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin + B, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin + 2 * B, n * 4, cudaMemcpyHostToDevice, s));
@@ -1192,9 +1687,6 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   B200W_CUDA(cudaGetLastError());
   for (int l = 0; l < a.num_layers; ++l) {
     const auto& p = m->lp[l];
-    bf16* kc = m->kc + l * layer_cache;
-    bf16* vc = m->vc + l * layer_cache;
-    const long long rp = static_cast<long long>(n) * (H + Hkv) * (dh / 2);
     if (falcon) {
       // parallel residual: h' = h + dense(attn(ln)) + W2 gelu(W1 ln)   (modeling_falcon.py FalconDecoderLayer)
       launch_ln(s, n, h, m->w + p.ln1_w, m->w + p.ln1_b, m->nrm, d, a.norm_eps); ++nl;
@@ -1203,8 +1695,7 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       o1.out2 = m->cat + qd; o1.ldo2 = m->ld_cat; o1.n_split = qkvd;
       o1.act = 1; o1.act_from = qkvd;   // exact GeLU on the MLP half only
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd + f, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, 1, m->table, m->nsplit); ++nl;
+      append_kv(m, s, n, l, 1, nl);
       decode_attention(m, s, n, l, m->cat, m->ld_cat, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -1215,8 +1706,7 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd; o1.bias = m->w + p.bqkv;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, 0, m->table, m->nsplit); ++nl;
+      append_kv(m, s, n, l, 0, nl);
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d; o2.bias = m->w + p.bo;
@@ -1233,8 +1723,7 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, qkvd, m->inv_freq, m->pos, m->slot,
-                 kc, vc, n, H, Hkv, dh, 1, m->table, m->nsplit); ++nl;
+      append_kv(m, s, n, l, 1, nl);
       decode_attention(m, s, n, l, m->cat, qd, nl);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
@@ -1333,9 +1822,12 @@ void check_weights_unshared(const Infer* m) {
   if (m->retained) throw StateError("KV pages are retained: cached K/V belong to the weights that computed them");
 }
 
-// b200w_infer_init (n_pages == 0) and b200w_infer_init_paged
-void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages, int64_t prefill_tokens) {
+// b200w_infer_init (n_pages == 0) and b200w_infer_init_paged_kv
+void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages, int64_t prefill_tokens,
+                int kv_dtype = B200W_KV_BF16) {
   B200W_CHECK(arch != nullptr && max_batch >= 1 && max_batch <= 128, "bad arch / max_batch (1..128)");
+  B200W_CHECK(kv_dtype == B200W_KV_BF16 || kv_dtype == B200W_KV_FP8_E4M3, "unknown KV cache dtype");
+  B200W_CHECK(kv_dtype == B200W_KV_BF16 || n_pages > 0, "an fp8 KV cache must be paged");
   B200W_CHECK(ctx_infer_slot(ctx) == nullptr, "inference model already initialised");
   B200W_CHECK(arch->family == B200W_FAMILY_LLAMA || arch->family == B200W_FAMILY_FALCON ||
                   arch->family == B200W_FAMILY_OPT, "unknown family");
@@ -1359,6 +1851,7 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->a = *arch;
   m->max_batch = max_batch;
   m->n_pages = n_pages;
+  m->kv_dtype = kv_dtype;
   if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
   m->lt.resize(arch->num_layers);   // all-null when the tiled copies are disabled
   build(m.get());
@@ -1376,12 +1869,25 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->act = m->alloc<bf16>(B * f);
   m->logits = m->alloc<bf16>(B * a.vocab_size);
   const size_t cache = static_cast<size_t>(a.num_layers) * m->layer_rows() * kd;
-  m->kc = m->alloc<bf16>(cache);
-  m->vc = m->alloc<bf16>(cache);
   // zero: the tensor-core decode attention multiplies P = 0 by whatever the rows beyond a slot's length hold
-  // (a page handed out again holds zeros or K/V an earlier request wrote: finite either way)
-  B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
-  B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
+  // (a page handed out again holds zeros or K/V an earlier request wrote: finite either way; the fp8 writer never
+  // stores a NaN byte)
+  if (m->fp8()) {
+    const size_t scales = static_cast<size_t>(a.num_layers) * m->layer_rows() * a.num_kv_heads;
+    m->kq = m->alloc<uint8_t>(cache);
+    m->vq = m->alloc<uint8_t>(cache);
+    m->ks = m->alloc<float>(scales);
+    m->vs = m->alloc<float>(scales);
+    B200W_CUDA(cudaMemset(m->kq, 0, cache));
+    B200W_CUDA(cudaMemset(m->vq, 0, cache));
+    B200W_CUDA(cudaMemset(m->ks, 0, scales * sizeof(float)));
+    B200W_CUDA(cudaMemset(m->vs, 0, scales * sizeof(float)));
+  } else {
+    m->kc = m->alloc<bf16>(cache);
+    m->vc = m->alloc<bf16>(cache);
+    B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
+    B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
+  }
   m->nsplit = (a.max_ctx + TC_KB - 1) / TC_KB;
   const size_t tab = B * m->nsplit;
   m->table = m->alloc<int32_t>(tab);
@@ -1436,35 +1942,90 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
 void b200w::attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
                                  int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
                                  const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs,
-                                 int S, int H, int Hkv, int dh, float scale, cudaStream_t s) {
+                                 int S, int H, int Hkv, int dh, float scale, cudaStream_t s, const float* kscale,
+                                 const float* vscale) {
   B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
   B200W_CHECK(n_seqs >= 1 && S >= 128 && S % 128 == 0, "padded length must be a positive multiple of 128");
   B200W_CHECK(H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad head configuration");
   B200W_CHECK(q_head_stride >= dh && ld_q >= H * q_head_stride && ld_out >= H * dh && ld_out % 8 == 0,
               "bad query / output strides");
   B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1, "bad KV cache");
+  const bool f8 = kscale != nullptr;
+  B200W_CHECK(f8 == (vscale != nullptr), "an fp8 cache needs both scale arrays");
   const int kd = Hkv * dh;
   const CUtensorMap tq = make_tmap_bf16_2d(q, static_cast<uint64_t>(n_seqs) * S, ld_q, ld_q, 128, 64);
-  const CUtensorMap tk = make_tmap_bf16_2d(kcache, cache_rows, kd, kd, KV_PAGE, 64);
-  const CUtensorMap tv = make_tmap_bf16_2d(vcache, cache_rows, kd, kd, KV_PAGE, 64);
+  const CUtensorMap tk = f8 ? make_tmap_u8_2d(kcache, cache_rows, kd, kd, KV_PAGE, dh)
+                            : make_tmap_bf16_2d(kcache, cache_rows, kd, kd, KV_PAGE, 64);
+  const CUtensorMap tv = f8 ? make_tmap_u8_2d(vcache, cache_rows, kd, kd, KV_PAGE, dh)
+                            : make_tmap_bf16_2d(vcache, cache_rows, kd, kd, KV_PAGE, 64);
   static PerDeviceOnce once;
   once.run([&] {
     B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     ca_smem_bytes<64>()));
     B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     ca_smem_bytes<128>()));
+    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_fp8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    ca_smem_bytes<64>() + ca_fp8_extra_bytes<64>()));
+    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_fp8_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    ca_smem_bytes<128>() + ca_fp8_extra_bytes<128>()));
   });
   const dim3 grid((S / 128) * n_seqs * H);
   const float scale_log2 = scale * 1.4426950408889634f;
-  if (dh == 64)
+  bf16* o = static_cast<bf16*>(out);
+  if (f8 && dh == 64)
+    attn_fwd_cached_fp8_kernel<64><<<grid, CA_THREADS, ca_smem_bytes<64>() + ca_fp8_extra_bytes<64>(), s>>>(
+        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2,
+        kscale, vscale);
+  else if (f8)
+    attn_fwd_cached_fp8_kernel<128><<<grid, CA_THREADS, ca_smem_bytes<128>() + ca_fp8_extra_bytes<128>(), s>>>(
+        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2,
+        kscale, vscale);
+  else if (dh == 64)
     attn_fwd_cached_kernel<64><<<grid, CA_THREADS, ca_smem_bytes<64>(), s>>>(
-        tq, tk, tv, q_head_stride, static_cast<bf16*>(out), ld_out, table, nsplit, slots, starts, lengths, n_seqs, S,
-        H, Hkv, scale_log2);
+        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2);
   else
     attn_fwd_cached_kernel<128><<<grid, CA_THREADS, ca_smem_bytes<128>(), s>>>(
-        tq, tk, tv, q_head_stride, static_cast<bf16*>(out), ld_out, table, nsplit, slots, starts, lengths, n_seqs, S,
-        H, Hkv, scale_log2);
+        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2);
   B200W_CUDA(cudaGetLastError());
+}
+
+void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, const void* vcache, const float* kscale,
+                                 const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
+                                 const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H,
+                                 int Hkv, int dh, float /*scale: 1 / sqrt(dh), as the engine uses*/, cudaStream_t s) {
+  B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
+  B200W_CHECK(n >= 1 && H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad batch / head configuration");
+  B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1 && nsplit * KV_PAGE <= 8192,
+              "bad KV cache");
+  B200W_CHECK(ld_q >= (H + 2 * Hkv) * dh && ld_out >= H * dh && kscale && vscale, "bad strides / scales");
+  // the engine's decode attention on one layer of a pool the caller owns: a model that allocates only the
+  // tensor-core partials and borrows everything else
+  Infer m;
+  m.a.num_heads = H;
+  m.a.num_kv_heads = Hkv;
+  m.a.head_dim = dh;
+  m.a.max_ctx = nsplit * KV_PAGE;
+  m.kd = Hkv * dh;
+  m.qkvd = ld_q;
+  m.n_pages = static_cast<int>(cache_rows / KV_PAGE);
+  m.nsplit = nsplit;
+  m.kv_dtype = B200W_KV_FP8_E4M3;
+  m.kq = static_cast<uint8_t*>(const_cast<void*>(kcache));
+  m.vq = static_cast<uint8_t*>(const_cast<void*>(vcache));
+  m.ks = const_cast<float*>(kscale);
+  m.vs = const_cast<float*>(vscale);
+  m.qkv = static_cast<bf16*>(const_cast<void*>(q));
+  m.pos = const_cast<int32_t*>(positions);
+  m.slot = const_cast<int32_t*>(slots);
+  m.table = const_cast<int32_t*>(table);
+  if (H / Hkv >= 4) {
+    m.part_o = m.alloc<float>(static_cast<size_t>(n) * H * nsplit * dh);
+    m.part_ml = m.alloc<float2>(static_cast<size_t>(n) * H * nsplit);
+  }
+  int64_t nl = 0;
+  decode_attention(&m, s, n, 0, static_cast<bf16*>(out), ld_out, nl);
+  B200W_CUDA(cudaGetLastError());
+  B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed with m
 }
 
 extern "C" {
@@ -1473,11 +2034,48 @@ int b200w_infer_init(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch
   return iguard(ctx, [&] { init_infer(ctx, arch, max_batch, 0, 0); });
 }
 
-int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
-                           int64_t prefill_tokens) {
+int b200w_infer_init_paged_kv(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
+                              int64_t prefill_tokens, int kv_dtype) {
   return iguard(ctx, [&] {
     B200W_CHECK(n_pages >= 1, "n_pages must be >= 1");
-    init_infer(ctx, arch, max_batch, n_pages, prefill_tokens);
+    init_infer(ctx, arch, max_batch, n_pages, prefill_tokens, kv_dtype);
+  });
+}
+
+int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages,
+                           int64_t prefill_tokens) {
+  return b200w_infer_init_paged_kv(ctx, arch, max_batch, n_pages, prefill_tokens, B200W_KV_BF16);
+}
+
+int b200w_infer_kv_read(b200w_ctx* ctx, int layer, int slot, int pos0, int n, void* k_out, void* v_out,
+                        float* k_scale_out, float* v_scale_out) {
+  return iguard(ctx, [&] {
+    Infer* m = model(ctx);
+    B200W_CHECK(layer >= 0 && layer < m->a.num_layers && slot >= 0 && slot < m->max_batch, "bad layer / slot");
+    B200W_CHECK(pos0 >= 0 && n >= 0 && pos0 + static_cast<int64_t>(n) <= m->a.max_ctx && (n == 0 || (k_out && v_out)),
+                "bad positions / outputs");
+    if (m->n_pages)
+      B200W_CHECK(pos0 + static_cast<int64_t>(n) <= static_cast<int64_t>(m->held[slot].size()) * KV_PAGE,
+                  "position beyond the KV pages the slot holds");
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+    const Infer::KVLayer c = m->kv_layer(layer);
+    const int Hkv = m->a.num_kv_heads;
+    const size_t row_bytes = static_cast<size_t>(m->kd) * (m->fp8() ? 1 : sizeof(bf16));
+    for (int i = 0; i < n; ++i) {   // through the host copy of the table
+      const int p = pos0 + i;
+      const size_t row = static_cast<size_t>(m->table_pin[static_cast<size_t>(slot) * m->nsplit + p / KV_PAGE]) +
+                         p % KV_PAGE;
+      B200W_CUDA(cudaMemcpy(static_cast<uint8_t*>(k_out) + i * row_bytes, static_cast<uint8_t*>(c.k) + row * row_bytes,
+                            row_bytes, cudaMemcpyDeviceToHost));
+      B200W_CUDA(cudaMemcpy(static_cast<uint8_t*>(v_out) + i * row_bytes, static_cast<uint8_t*>(c.v) + row * row_bytes,
+                            row_bytes, cudaMemcpyDeviceToHost));
+      if (m->fp8() && k_scale_out)
+        B200W_CUDA(cudaMemcpy(k_scale_out + static_cast<size_t>(i) * Hkv, c.ks + row * Hkv, Hkv * sizeof(float),
+                              cudaMemcpyDeviceToHost));
+      if (m->fp8() && v_scale_out)
+        B200W_CUDA(cudaMemcpy(v_scale_out + static_cast<size_t>(i) * Hkv, c.vs + row * Hkv, Hkv * sizeof(float),
+                              cudaMemcpyDeviceToHost));
+    }
   });
 }
 
@@ -1792,7 +2390,6 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     const int dhp = 128, HT = H + 2 * Hkv;
     const bool padded = dh != dhp;
     const float scale = 1.f / sqrtf(static_cast<float>(dh));
-    const size_t layer_cache = m->layer_rows() * m->kd;
       const int Ti = static_cast<int>(T);
     auto G = [&](const void* A, int lda, size_t woff, int ldw, void* D, const void* C, int ldd, int N, int K,
                  const void* bias = nullptr, int act = 0) {
@@ -1807,8 +2404,25 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     ++nl;
     for (int l = 0; l < a.num_layers; ++l) {
       const auto& p = m->lp[l];
-      bf16* kc = m->kc + l * layer_cache;
-      bf16* vc = m->vc + l * layer_cache;
+      const Infer::KVLayer c = m->kv_layer(l);
+      // q / k rotated (rope != 0) into dst [T, *] at head stride dh_dst, the real positions' K/V into the cache
+      auto scatter = [&](bf16* dst, int ld_dst, int dh_dst, const int32_t* start) {
+        if (m->fp8()) {   // a warp per (token, head)
+          const long long warps = static_cast<long long>(Ti) * HT;
+          prefill_rope_scatter_fp8_kernel<<<cdiv(warps * 32, 256), 256, 0, s>>>(
+              m->pf_qkv, qkvd, dst, ld_dst, m->inv_freq, m->pf_len, m->pf_slot, static_cast<uint8_t*>(c.k),
+              static_cast<uint8_t*>(c.v), c.ks, c.vs, Ti, S, H, Hkv, dh, dh_dst, opt ? 0 : 1, m->table, m->nsplit,
+              start);
+        } else {
+          const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
+          prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, dst, ld_dst, m->inv_freq, m->pf_len,
+                                                                    m->pf_slot, static_cast<bf16*>(c.k),
+                                                                    static_cast<bf16*>(c.v), Ti, S, H, Hkv, dh, dh_dst,
+                                                                    opt ? 0 : 1, m->table, m->nsplit, start);
+        }
+        ++nl;
+        B200W_CUDA(cudaGetLastError());
+      };
       if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + p.ln1_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s);
       else layernorm_kernel<<<Ti, 256, 0, s>>>(h, m->w + p.ln1_w, m->w + p.ln1_b, m->pf_nrm, d, a.norm_eps);
       ++nl;
@@ -1818,23 +2432,18 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
         const long long ge = static_cast<long long>(Ti) * (f / 8);
         gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, s>>>(m->pf_cat + qd, Ti, f, ldc); ++nl;
       }
-      const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
       if (starts) {
         // after a cached prefix: q / k rotated in place at their positions, the suffix K/V into the slot's pages, then
         // the paged attention reads the queries at their own width and writes the o-projection's input directly
-        prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, m->pf_qkv, qkvd, m->inv_freq,
-                                                                  m->pf_len, m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dh,
-                                                                  opt ? 0 : 1, m->table, m->nsplit, m->pf_start); ++nl;
-        B200W_CUDA(cudaGetLastError());
-        attention_fwd_cached(m->pf_qkv, qkvd, dh, kc, vc, m->layer_rows(), m->table, m->nsplit, m->pf_slot, m->pf_start,
-                             m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv, dh, scale, s); ++nl;
+        // (on the fp8 pool every key it reads, the suffix's own included, is the quantized one)
+        scatter(m->pf_qkv, qkvd, dh, m->pf_start);
+        attention_fwd_cached(m->pf_qkv, qkvd, dh, c.k, c.v, m->layer_rows(), m->table, m->nsplit, m->pf_slot, m->pf_start,
+                             m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv, dh, scale, s, c.ks, c.vs); ++nl;
       } else {
+        // a cold prefill attends over the bf16 activations, on either pool
         bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
         const int ld_in = padded ? HT * dhp : qkvd;
-        prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, att_in, ld_in, m->inv_freq,
-                                                                  m->pf_len, m->pf_slot, kc, vc, Ti, S, H, Hkv, dh, dhp,
-                                                                  opt ? 0 : 1, m->table, m->nsplit, nullptr); ++nl;
-        B200W_CUDA(cudaGetLastError());
+        scatter(att_in, ld_in, dhp, nullptr);
         bf16* att_out = padded ? m->pf_attp : m->pf_cat;
         const int ld_out = padded ? H * dhp : ldc;
         attention_fwd(att_in, ld_in, H * dhp, (H + Hkv) * dhp, att_out, ld_out, m->pf_lse, n_seqs, S, H, Hkv, scale, s);

@@ -84,10 +84,18 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
 // multiple of 128 below lengths[b]; the pages of positions [0, lengths[b]) are the caller's to have filled and
 // entered in the table. out [n_seqs * S, ld_out]: head h at column h * dh. slots / starts / lengths: DEVICE int32
 // [n_seqs]. Rows at positions >= lengths[b] get finite values that mean nothing.
+// The decode step's attention over one layer of an fp8 pool (the engine's kernels: CUDA cores when H / Hkv < 4,
+// tensor cores otherwise). q [n, ld_q]: row r's query heads at columns h * dh; positions / slots DEVICE int32 [n].
+void decode_attention_fp8(const void* q, int ld_q, const void* kcache, const void* vcache, const float* kscale,
+                          const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
+                          const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H, int Hkv,
+                          int dh, float scale, cudaStream_t s);
+// kscale / vscale [cache_rows, Hkv] non-null: kcache / vcache hold e4m3 bytes (DESIGN §3.5)
 void attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
                           int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
                           const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
-                          int H, int Hkv, int dh, float scale, cudaStream_t s);
+                          int H, int Hkv, int dh, float scale, cudaStream_t s, const float* kscale = nullptr,
+                          const float* vscale = nullptr);
 
 
 // ---- ops.cu --------------------------------------------------------------------------------

@@ -74,9 +74,17 @@ class ServeArch:
 KV_PAGE = 128   # positions per page of the paged KV cache (one key block of the decode attention)
 
 
-def kv_page_bytes(arch: ServeArch) -> int:
-    """Device bytes of one page: K and V, every layer, 128 positions of num_kv_heads * head_dim bf16."""
-    return 2 * arch.num_layers * KV_PAGE * arch.num_kv_heads * arch.head_dim * 2
+KV_DTYPES = {"bf16": 0, "fp8": 1}   # b200w_kv_dtype: bf16, or e4m3 with one fp32 scale per (position, kv head)
+
+
+def kv_page_bytes(arch: ServeArch, kv_dtype: str = "bf16") -> int:
+    """Device bytes of one page: K and V, every layer, 128 positions of num_kv_heads * head_dim bf16 values, or of
+    as many e4m3 bytes plus one fp32 scale per kv head (kv_dtype "fp8")."""
+    if kv_dtype not in KV_DTYPES:
+        raise ValueError(f"kv_dtype must be one of {sorted(KV_DTYPES)}, got {kv_dtype!r}")
+    kd = arch.num_kv_heads * arch.head_dim
+    row = 2 * kd if kv_dtype == "bf16" else kd + 4 * arch.num_kv_heads
+    return 2 * arch.num_layers * KV_PAGE * row
 
 
 def pages_for(n_tokens: int) -> int:
@@ -89,12 +97,19 @@ class CacheFull(RuntimeError):
 
 class InferEngine(Engine):
     kv_pages: Optional[int] = None   # pages in the pool; None: the contiguous max_batch x max_ctx cache
+    kv_dtype: str = "bf16"
 
     def init_infer(self, arch: ServeArch, max_batch: int = 32, kv_pages: Optional[int] = None,
-                   prefill_tokens: Optional[int] = None):
+                   prefill_tokens: Optional[int] = None, kv_dtype: str = "bf16"):
         """kv_pages: serve from a pool of that many 128-position pages shared by all slots (b200w_infer_init_paged)
         instead of reserving max_ctx positions per slot; arch.max_ctx is then the longest single request.
-        prefill_tokens: the most tokens (n_seqs * padded length) one prefill call takes in paged mode."""
+        prefill_tokens: the most tokens (n_seqs * padded length) one prefill call takes in paged mode.
+        kv_dtype: "bf16", or "fp8" (paged only): K/V stored as e4m3 with per-(position, kv head) scales, about half
+        the bytes per page (DESIGN §3.5)."""
+        if kv_dtype not in KV_DTYPES:
+            raise ValueError(f"kv_dtype must be one of {sorted(KV_DTYPES)}, got {kv_dtype!r}")
+        if kv_dtype != "bf16" and kv_pages is None:
+            raise ValueError("an fp8 KV cache must be paged (kv_pages)")
         ca = _CArch(FAMILY[arch.family], arch.vocab_size, arch.hidden_size, arch.intermediate_size,
                     arch.num_layers, arch.num_heads, arch.num_kv_heads, arch.head_dim, arch.max_ctx,
                     arch.norm_eps, arch.rope_theta, 1 if arch.tie_embeddings else 0, arch.max_positions)
@@ -103,9 +118,23 @@ class InferEngine(Engine):
         else:
             if prefill_tokens is None:
                 prefill_tokens = max(16384, pages_for(arch.max_ctx) * KV_PAGE)
-            self._check(self._lib.b200w_infer_init_paged(self._h, C.byref(ca), max_batch, kv_pages, prefill_tokens))
+            self._check(self._lib.b200w_infer_init_paged_kv(self._h, C.byref(ca), max_batch, kv_pages, prefill_tokens,
+                                                            KV_DTYPES[kv_dtype]))
             self.kv_pages, self.prefill_tokens = kv_pages, prefill_tokens
-        self.serve_arch, self.max_batch = arch, max_batch
+        self.serve_arch, self.max_batch, self.kv_dtype = arch, max_batch, kv_dtype
+
+    def kv_read(self, layer: int, slot: int, pos0: int, n: int):
+        """The raw cache rows of positions [pos0, pos0 + n) of `slot` (b200w_infer_kv_read): (k, v) as bf16 bit
+        patterns (uint16 [n, Hkv * dh]), or on an fp8 cache (k, v, k_scale, v_scale) with e4m3 bytes (uint8) and
+        fp32 scales [n, Hkv]."""
+        a = self.serve_arch
+        kd = a.num_kv_heads * a.head_dim
+        dt = np.uint8 if self.kv_dtype == "fp8" else np.uint16
+        k, v = np.empty((n, kd), dtype=dt), np.empty((n, kd), dtype=dt)
+        ks, vs = (np.empty((n, a.num_kv_heads), dtype=np.float32) for _ in range(2))
+        self._check(self._lib.b200w_infer_kv_read(self._h, layer, slot, pos0, n, k.ctypes.data, v.ctypes.data,
+                                                  ks.ctypes.data, vs.ctypes.data))
+        return (k, v, ks, vs) if self.kv_dtype == "fp8" else (k, v)
 
     def reserve(self, slot: int, n_tokens: int):
         """Give `slot` the pages for positions [0, n_tokens) (releasing what it held); B200WError with status

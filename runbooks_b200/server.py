@@ -360,24 +360,41 @@ def prefix_cache_param(content: str, prefix_cache: bool | None = None, environ=N
     raise ValueError(f"param 'prefix_cache': cannot read {v!r} as a boolean")
 
 
-def kv_pages_for_gb(arch, kv_cache_gb: float) -> int:
+KV_CACHE_DTYPES = {"auto": "bf16", "bf16": "bf16", "fp8": "fp8", "fp8_e4m3": "fp8"}
+
+
+def kv_cache_dtype_param(content: str, kv_cache_dtype: str | None = None, environ=None) -> str:
+    """The element type of the paged KV cache, "bf16" or "fp8": --kv-cache-dtype, else the params' kv_cache_dtype
+    (params.json, PARAM_KV_CACHE_DTYPE over it), else bf16. auto / bf16 and fp8 / fp8_e4m3 are accepted."""
+    if kv_cache_dtype is None:
+        extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
+        kv_cache_dtype = extra.get("kv_cache_dtype", "auto")
+    v = kv_cache_dtype.strip().lower() if isinstance(kv_cache_dtype, str) else kv_cache_dtype
+    if v not in KV_CACHE_DTYPES:
+        raise ValueError(f"param 'kv_cache_dtype' must be one of {sorted(KV_CACHE_DTYPES)}, got {kv_cache_dtype!r}")
+    return KV_CACHE_DTYPES[v]
+
+
+def kv_pages_for_gb(arch, kv_cache_gb: float, kv_dtype: str = "bf16") -> int:
     """Pages of a paged KV cache of kv_cache_gb * 10^9 bytes; ValueError when that cannot hold one max_ctx request."""
     from .infer import kv_page_bytes, pages_for
-    pages = int(kv_cache_gb * 1e9 // kv_page_bytes(arch))
+    page = kv_page_bytes(arch, kv_dtype)
+    pages = int(kv_cache_gb * 1e9 // page)
     if pages < pages_for(arch.max_ctx):
-        raise ValueError(f"kv_cache_gb {kv_cache_gb} holds {pages} pages of {kv_page_bytes(arch) / 1e6:.1f} MB; one "
+        raise ValueError(f"kv_cache_gb {kv_cache_gb} holds {pages} pages of {page / 1e6:.1f} MB; one "
                          f"request of max_ctx {arch.max_ctx} needs {pages_for(arch.max_ctx)}")
     return pages
 
 
-def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None):
+def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None,
+                kv_dtype: str = "bf16"):
     from .infer import InferEngine, ServeArch
 
     cfg = contract.read_hf_config(model_dir)
     arch = ServeArch.from_hf_config(cfg, max_ctx)
-    kv_pages = None if kv_cache_gb is None else kv_pages_for_gb(arch, kv_cache_gb)
+    kv_pages = None if kv_cache_gb is None else kv_pages_for_gb(arch, kv_cache_gb, kv_dtype)
     e = InferEngine(int(os.environ.get("B200W_DEVICE", "0")))
-    e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages)
+    e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages, kv_dtype=kv_dtype)
     wanted = {n for n, _ in e.infer_params()}
     seen, unused = set(), []
     for name, arr in contract.iter_safetensors(model_dir):
@@ -395,14 +412,17 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
-          prefix_cache: bool | None = None):
+          prefix_cache: bool | None = None, kv_cache_dtype: str | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
     prefix_cache = prefix_cache_param(content, prefix_cache)
+    kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
     if prefix_cache and kv_cache_gb is None:
         raise ValueError("prefix_cache shares pages of the paged KV cache: it needs kv_cache_gb")
+    if kv_dtype != "bf16" and kv_cache_gb is None:
+        raise ValueError("an fp8 KV cache is paged: kv_cache_dtype fp8 needs kv_cache_gb")
     model_dir = os.path.join(content, "model")
     t0 = time.time()
-    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb)
+    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype)
     tok = contract.Tokenizer(model_dir)
     sched = Scheduler(engine, tok, prefix_cache=prefix_cache)
     sched.start()
@@ -412,8 +432,8 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
              "max_batch": max_batch}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
-        ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch) / 1e6, 2),
-                     prefix_cache=prefix_cache)
+        ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch, kv_dtype) / 1e6, 2),
+                     kv_cache_dtype=kv_dtype, prefix_cache=prefix_cache)
     print(json.dumps(ready), flush=True)
     httpd.serve_forever()
 
@@ -430,9 +450,12 @@ def main(argv=None) -> int:
     ap.add_argument("--prefix-cache", action="store_true", default=None,
                     help="share the KV pages of repeated prompt prefixes (needs the paged cache; default: param "
                          "prefix_cache, else off)")
+    ap.add_argument("--kv-cache-dtype", default=None,
+                    help="element type of the paged KV cache: auto / bf16, or fp8 / fp8_e4m3 (needs kv_cache_gb; "
+                         "default: param kv_cache_dtype, else bf16)")
     a = ap.parse_args(argv)
     try:
-        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache)
+        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()

@@ -768,6 +768,95 @@ def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, thread
     return res
 
 
+def wg_cached_fp8_kernel(npages, rng, threads=2, warps=2, release_after_softmax=True, staging_barrier=True):
+    """attn_fwd_cached_kernel<DH, fp8>'s producer warpgroup (`threads` threads, thread 0 elected): thread 0 TMA-loads
+    page j's e4m3 K and V boxes into ONE staging buffer (bar_st); every thread waits for them, waits on K buffer
+    j % 2's free barrier, widens its part of K into it and writes its part of the page's K and V scales into scale
+    slot j % 2, arrives on the K full barrier (count `threads`), then the same for V (V free / V full); a named
+    barrier over the warpgroup precedes the next load of the staging (`staging_barrier`). Consumer warps wait on K
+    full, run the score product, read both scales in the softmax and arrive on K free (`release_after_softmax`;
+    before the softmax, the slot's scales may be overwritten by page j + 2), then wait on V full, run P V and arrive
+    on V free."""
+    S = 2
+    copies = []
+    bar_st = Mbar(1)
+    kfull, vfull = [Mbar(threads) for _ in range(S)], [Mbar(threads) for _ in range(S)]
+    kfree, vfree = [Mbar(warps) for _ in range(S)], [Mbar(warps) for _ in range(S)]
+    staging = [None]
+    ring_k, ring_v, scales = ([[None] * threads for _ in range(S)] for _ in range(3))
+    barr = [0, 0]
+    state = dict(done=0)
+
+    def engine():
+        while state["done"] < threads + warps:
+            if copies:
+                copies.pop(rng.randrange(len(copies)))()
+                yield None
+            else:
+                yield (lambda: bool(copies) or state["done"] >= threads + warps)
+
+    def read_staging(i, j):
+        if staging[0] != j:
+            raise Violation(f"producer thread {i} widened page {j} from a staging buffer holding {staging[0]}")
+
+    def producer(i):
+        for j in range(npages):
+            b, fp = j % S, ((j // S) - 1) & 1
+            if i == 0:
+                def land(j=j):
+                    staging[0] = j
+                    bar_st.arrive()
+                copies.append(land)
+            yield (lambda j=j: bar_st.passed(j & 1))
+            if j >= S:
+                yield (lambda b=b, fp=fp: kfree[b].passed(fp))
+            read_staging(i, j)
+            ring_k[b][i] = scales[b][i] = j
+            yield None
+            kfull[b].arrive()
+            if j >= S:
+                yield (lambda b=b, fp=fp: vfree[b].passed(fp))
+            read_staging(i, j)
+            ring_v[b][i] = j
+            yield None
+            vfull[b].arrive()
+            if staging_barrier:
+                g = barr[1]
+                barr[0] += 1
+                if barr[0] == threads:
+                    barr[0], barr[1] = 0, g + 1
+                yield (lambda g=g: barr[1] != g)
+        state["done"] += 1
+
+    def consumer(w):
+        for u in range(npages):
+            b, ph = u % S, (u // S) & 1
+            yield (lambda b=b, ph=ph: kfull[b].passed(ph))
+            if ring_k[b] != [u] * threads:
+                raise Violation(f"warp {w}'s score product of page {u} read K buffer {b} holding {ring_k[b]}")
+            yield None
+            if not release_after_softmax:
+                kfree[b].arrive()
+                yield None
+            if scales[b] != [u] * threads:
+                raise Violation(f"warp {w}'s softmax of page {u} read scale slot {b} holding {scales[b]}")
+            if release_after_softmax:
+                kfree[b].arrive()
+            yield (lambda b=b, ph=ph: vfull[b].passed(ph))
+            if ring_v[b] != [u] * threads:
+                raise Violation(f"warp {w}'s P V of page {u} read V buffer {b} holding {ring_v[b]}")
+            yield None
+            vfree[b].arrive()
+        state["done"] += 1
+
+    agents = {"copies": engine()}
+    for i in range(threads):
+        agents[f"p{i}"] = producer(i)
+    for w in range(warps):
+        agents[f"c{w}"] = consumer(w)
+    return run(agents, rng)
+
+
 def explore(kernel, trials, seed=0, **kw):
     """-> (#ok, first violation or None, other outcomes)"""
     ok, first, other = 0, None, {}
@@ -801,6 +890,9 @@ if __name__ == "__main__":
                          ("sm_90a dQ", wg_dq_kernel, dict(njb=8)),
                          ("sm_90a dK/dV", wg_dkdv_kernel, dict(n_iter=9)),
                          ("sm_90a cluster GEMM", wg_gemm_kernel, dict(num_items=13, ctas=2)),
+                         ("cached-prefix fp8 widening", wg_cached_fp8_kernel, dict(npages=6)),
+                         ("fp8, K freed before the softmax", wg_cached_fp8_kernel,
+                          dict(npages=6, release_after_softmax=False)),
                          ("sm_90a cluster GEMM, local release", wg_gemm_kernel, dict(num_items=13, ctas=2, remote_release=False))]:
         ok, first, other = explore(fn, 2000, **kw)
         print(f"{name:36s} ok {ok:4d}/2000   first violation: {first}   other: {other}")
