@@ -283,6 +283,38 @@ B200W_API int b200w_infer_retain_pages(b200w_ctx* ctx, const int32_t* pages, int
 B200W_API int b200w_infer_prefill_cached(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts,
                                          const int32_t* lengths, const int32_t* slots, int n_seqs, int padded_len,
                                          int32_t* next_tokens, float* logits_out);
+/* Token log-probabilities (DESIGN §3.5). The numbers are the log-softmax of the bf16 logits the engine computed, at
+ * temperature 1 and without nucleus truncation, in fp32: lse = max + log(sum(exp(x - max))), a token's
+ * log-probability is x - lse. They do not depend on how a caller samples. The top entries are the top_k largest
+ * logits, by value descending with ties to the smaller id (argmax's rule), so top_ids[row * top_k] is the greedy
+ * token. A call with top_k outside 0..B200W_MAX_TOP_LOGPROBS or a non-zero reserved is B200W_ERR_INVALID before any
+ * GPU work. */
+#define B200W_MAX_TOP_LOGPROBS 5 /* the OpenAI completions limit */
+typedef struct {
+  int32_t top_k;     /* 0 .. B200W_MAX_TOP_LOGPROBS                                               */
+  int32_t reserved;  /* zero                                                                      */
+  float* lse;        /* HOST [rows] or NULL: log-sum-exp of each next-token logits row            */
+  float* token_lp;   /* HOST [rows] or NULL: log-probability of next_tokens[row] (the greedy one) */
+  int32_t* top_ids;  /* HOST [rows, top_k]: descending logit, ties to the smaller id              */
+  float* top_lp;     /* HOST [rows, top_k]                                                        */
+} b200w_logprobs;
+/* b200w_infer_step, and `next` (NULL: none) filled for its n rows. The step's captured graph is the same; the
+ * log-softmax runs after it on the step's logits. */
+B200W_API int b200w_infer_step_logprobs(b200w_ctx* ctx, const int32_t* tokens, const int32_t* positions,
+                                        const int32_t* slots, int n, int32_t* next_tokens, float* logits_out,
+                                        const b200w_logprobs* next);
+/* b200w_infer_prefill (a cold prefill: no cached prefix), `next` (NULL: none) filled for the token after each prompt,
+ * and the prompt scored position by position. prompt_lp HOST [n_seqs, padded_len] or NULL: prompt_lp[b][p] =
+ * log P(tokens[b][p] | tokens[b][< p]) for 1 <= p < lengths[b], 0 elsewhere. prompt_top_ids / prompt_top_lp HOST
+ * [n_seqs, padded_len, next->top_k] or NULL: the top entries of the distribution over position p, for the same p
+ * (ids -1 and 0 elsewhere). The next-token outputs come from the same last-row computation as b200w_infer_prefill
+ * and are bit-identical to it. Scoring runs the final norm and lm_head over every prompt row, in chunks of up to
+ * 1024 rows through a bf16 [chunk, vocab] buffer that the first scoring call allocates and the context keeps;
+ * B200W_ERR_OOM if that allocation fails (the context stays usable). */
+B200W_API int b200w_infer_prefill_logprobs(b200w_ctx* ctx, const int32_t* tokens, const int32_t* lengths,
+                                           const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
+                                           float* logits_out, const b200w_logprobs* next, float* prompt_lp,
+                                           int32_t* prompt_top_ids, float* prompt_top_lp);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.
@@ -370,6 +402,12 @@ B200W_API int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int l
                                             int64_t cache_rows, const int32_t* table, int nsplit,
                                             const int32_t* positions, const int32_t* slots, void* out, int ld_out,
                                             int n, int H, int Hkv, int dh, float scale);
+/* The log-softmax of the token log-probability calls on bf16 logits [rows, ld] (vocab V % 8 == 0, ld % 8 == 0):
+ * lse, target_lp (log-probability of targets[r]; targets NULL or an id outside [0, V): 0), token_lp (of the row
+ * maximum) [rows] and top_ids / top_lp [rows, top_k], each nullable. DEVICE pointers. */
+B200W_API int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets,
+                                int top_k, float* lse, float* target_lp, float* token_lp, int32_t* top_ids,
+                                float* top_lp);
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);

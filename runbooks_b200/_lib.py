@@ -42,6 +42,15 @@ class InferArch(C.Structure):
     ]
 
 
+MAX_TOP_LOGPROBS = 5  # include/b200w.h B200W_MAX_TOP_LOGPROBS
+
+
+class Logprobs(C.Structure):
+    """b200w_logprobs: HOST output arrays of the token log-probability calls."""
+    _fields_ = [("top_k", C.c_int32), ("reserved", C.c_int32), ("lse", vp), ("token_lp", vp), ("top_ids", vp),
+                ("top_lp", vp)]
+
+
 class HParams(C.Structure):
     _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
                 ("weight_decay", C.c_float), ("max_grad_norm", C.c_float)]
@@ -97,6 +106,8 @@ PROTOTYPES = {
     "b200w_infer_reserve_shared": (C.c_int, [c_ctx, C.c_int, C.c_int, vp, C.c_int]),
     "b200w_infer_retain_pages": (C.c_int, [c_ctx, vp, C.c_int, C.c_int]),
     "b200w_infer_prefill_cached": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
+    "b200w_infer_step_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp, vp]),
+    "b200w_infer_prefill_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
@@ -133,6 +144,7 @@ PROTOTYPES = {
                                                     C.c_int, C.c_int, C.c_float]),
     "b200w_op_decode_attention_fp8": (C.c_int, [c_ctx, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
                                                 vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
+    "b200w_op_logprobs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,

@@ -1950,6 +1950,11 @@ int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const
   HOOK(decode_attention_fp8(q, ld_q, kcache, vcache, kscale, vscale, cache_rows, table, nsplit, positions, slots, out,
                             ld_out, n, H, Hkv, dh, scale, ctx->stream));
 }
+int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets, int top_k,
+                      float* lse, float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp) {
+  if (top_k < 0 || top_k > B200W_MAX_TOP_LOGPROBS) return B200W_ERR_INVALID;
+  HOOK(logprobs(logits, ld, rows, V, targets, top_k, lse, target_lp, token_lp, top_ids, top_lp, ctx->stream));
+}
 int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {

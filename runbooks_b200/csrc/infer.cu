@@ -1306,6 +1306,129 @@ __global__ void argmax_kernel(const bf16* __restrict__ logits, int V, int32_t* _
   }
 }
 
+// ---- token log-probabilities (b200w_infer_step_logprobs, b200w_infer_prefill_logprobs, b200w_op_logprobs) ----
+// The log-softmax of the bf16 logits the engine computed (temperature 1, no truncation), per row: lse, the
+// log-probability of a target id and of the row maximum, and the B200W_MAX_TOP_LOGPROBS largest logits ordered by
+// value descending with ties to the smaller id (argmax_kernel's and torch.argmax's rule, so top-1 is the greedy
+// token). Every thread keeps an online (max, sum) and a sorted top list in registers; both are reduced across the
+// CTA in a fixed tree, so a re-run is bit-identical. Log-probabilities are (x - max) - log(sum): x - max is exact in
+// fp32 for bf16 inputs, which keeps them accurate where |lse| is large.
+constexpr int LP_THREADS = 512;
+constexpr int LP_K = B200W_MAX_TOP_LOGPROBS;
+
+// (v, i) ranks before (w, j): larger value, or equal value and smaller id
+__device__ __forceinline__ bool lp_before(float v, int i, float w, int j) { return v > w || (v == w && i < j); }
+
+// inserts (v, i) into the sorted list (tv, ti) when it ranks before the last entry
+__device__ __forceinline__ void lp_insert(float (&tv)[LP_K], int (&ti)[LP_K], float v, int i) {
+  if (!lp_before(v, i, tv[LP_K - 1], ti[LP_K - 1])) return;
+  tv[LP_K - 1] = v;
+  ti[LP_K - 1] = i;
+#pragma unroll
+  for (int j = LP_K - 1; j > 0; --j)
+    if (lp_before(tv[j], ti[j], tv[j - 1], ti[j - 1])) {
+      const float fv = tv[j]; tv[j] = tv[j - 1]; tv[j - 1] = fv;
+      const int fi = ti[j]; ti[j] = ti[j - 1]; ti[j - 1] = fi;
+    }
+}
+
+// (m, s) <- the online-softmax merge with (om, os); m == -inf on both sides keeps s
+__device__ __forceinline__ void lp_merge(float& m, float& s, float om, float os) {
+  const float nm = fmaxf(m, om);
+  s = (m == nm ? s : s * expf(m - nm)) + (om == nm ? os : os * expf(om - nm));
+  m = nm;
+}
+
+// butterfly over the warp: every lane ends with the warp's (m, s) and top list
+__device__ __forceinline__ void lp_warp_reduce(float& m, float& s, float (&tv)[LP_K], int (&ti)[LP_K]) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const float os = __shfl_xor_sync(0xffffffffu, s, o);
+    lp_merge(m, s, om, os);
+    float pv[LP_K];
+    int pi[LP_K];
+#pragma unroll
+    for (int j = 0; j < LP_K; ++j) {
+      pv[j] = __shfl_xor_sync(0xffffffffu, tv[j], o);
+      pi[j] = __shfl_xor_sync(0xffffffffu, ti[j], o);
+    }
+#pragma unroll
+    for (int j = 0; j < LP_K; ++j) lp_insert(tv, ti, pv[j], pi[j]);
+  }
+}
+
+// one CTA per row of logits [rows, ld]; V % 8 == 0, ld % 8 == 0. targets (nullable): a target outside [0, V) gives
+// target_lp 0. Every output is nullable; top_ids / top_lp are [rows, k].
+__global__ void __launch_bounds__(LP_THREADS)
+logprobs_kernel(const bf16* __restrict__ logits, int ld, int V, const int32_t* __restrict__ targets, int k,
+                float* __restrict__ lse, float* __restrict__ target_lp, float* __restrict__ token_lp,
+                int32_t* __restrict__ top_ids, float* __restrict__ top_lp) {
+  __shared__ float sm[LP_THREADS / 32], ss[LP_THREADS / 32], sv[LP_THREADS / 32][LP_K];
+  __shared__ int si[LP_THREADS / 32][LP_K];
+  const bf16* row = logits + static_cast<size_t>(blockIdx.x) * ld;
+  float m = -INFINITY, s = 0.f;
+  float tv[LP_K];
+  int ti[LP_K];
+#pragma unroll
+  for (int j = 0; j < LP_K; ++j) { tv[j] = -INFINITY; ti[j] = 0x7fffffff; }
+  for (int i = threadIdx.x * 8; i < V; i += LP_THREADS * 8) {
+    const uint4 u = *reinterpret_cast<const uint4*>(row + i);
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    float x[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = unpack_bf16x2(w[j]);
+      x[2 * j] = f.x;
+      x[2 * j + 1] = f.y;
+    }
+    float cm = x[0];
+#pragma unroll
+    for (int j = 1; j < 8; ++j) cm = fmaxf(cm, x[j]);
+    const float nm = fmaxf(m, cm);
+    if (nm != m) { s = s == 0.f ? 0.f : s * expf(m - nm); m = nm; }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      s += __expf(x[j] - m);   // ex2.approx of the exact difference: a few ulp, far inside the 2e-5 bar
+      lp_insert(tv, ti, x[j], i + j);
+    }
+  }
+  lp_warp_reduce(m, s, tv, ti);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+    sm[warp] = m;
+    ss[warp] = s;
+#pragma unroll
+    for (int j = 0; j < LP_K; ++j) { sv[warp][j] = tv[j]; si[warp][j] = ti[j]; }
+  }
+  __syncthreads();
+  if (warp != 0) return;
+  const bool have = lane < LP_THREADS / 32;
+  m = have ? sm[lane] : -INFINITY;
+  s = have ? ss[lane] : 0.f;
+#pragma unroll
+  for (int j = 0; j < LP_K; ++j) {
+    tv[j] = have ? sv[lane][j] : -INFINITY;
+    ti[j] = have ? si[lane][j] : 0x7fffffff;
+  }
+  lp_warp_reduce(m, s, tv, ti);
+  if (lane != 0) return;
+  const float ls = logf(s);
+  const int r = blockIdx.x;
+  if (lse) lse[r] = m + ls;
+  if (token_lp) token_lp[r] = -ls;
+  if (target_lp) {
+    const int t = targets ? targets[r] : -1;
+    target_lp[r] = t >= 0 && t < V ? (__bfloat162float(row[t]) - m) - ls : 0.f;
+  }
+#pragma unroll
+  for (int j = 0; j < LP_K; ++j)
+    if (j < k) {
+      if (top_ids) top_ids[static_cast<size_t>(r) * k + j] = ti[j];
+      if (top_lp) top_lp[static_cast<size_t>(r) * k + j] = (tv[j] - m) - ls;
+    }
+}
+
 struct IParam {
   std::string name;
   int64_t rows, cols;
@@ -1386,6 +1509,15 @@ struct Infer {
   int32_t* pf_pos = nullptr;   // OPT after a cached prefix: the learned-position row of every token
   int32_t* pf_pin = nullptr;
   size_t pf_pin_cap = 0;
+  // token log-probabilities, allocated by the first call that asks for them: the next-token rows [max_batch]
+  // (lse, token_lp, top ids / top log-probabilities [max_batch, B200W_MAX_TOP_LOGPROBS]); for prompt scoring a bf16
+  // chunk of lm_head outputs [lp_chunk_rows, V] and per-row outputs for lp_cap prefill rows
+  float *nx_lse = nullptr, *nx_tok = nullptr, *nx_top = nullptr;
+  int32_t* nx_ids = nullptr;
+  bf16* lp_chunk = nullptr;
+  size_t lp_chunk_rows = 0, lp_cap = 0;
+  float *lp_tgt = nullptr, *lp_top = nullptr;
+  int32_t *lp_ids = nullptr, *lp_targets = nullptr;
   std::vector<void*> allocs;
   int64_t bytes = 0;
   template <typename T>
@@ -1793,6 +1925,61 @@ void ensure_prefill_pin(Infer* m, size_t T) {
   m->pf_pin_cap = need;
 }
 
+constexpr int LP_CHUNK = 1024;   // prompt rows per lm_head GEMM of prompt scoring
+
+// a b200w_logprobs from the caller, checked before any GPU work; -> its top_k (0 for NULL)
+int check_logprobs(const b200w_logprobs* lp) {
+  if (!lp) return 0;
+  B200W_CHECK(lp->top_k >= 0 && lp->top_k <= B200W_MAX_TOP_LOGPROBS && lp->reserved == 0,
+              "b200w_logprobs: top_k must be in 0..B200W_MAX_TOP_LOGPROBS and reserved zero");
+  return lp->top_k;
+}
+
+void ensure_next_logprobs(Infer* m) {
+  if (m->nx_lse) return;
+  const size_t B = m->max_batch, K = B200W_MAX_TOP_LOGPROBS;
+  float* p = m->alloc<float>(B * (2 + 2 * K));
+  m->nx_lse = p;
+  m->nx_tok = p + B;
+  m->nx_top = p + 2 * B;
+  m->nx_ids = reinterpret_cast<int32_t*>(p + (2 + K) * B);
+}
+
+// the next-token log-probabilities of rows [0, n) of m->logits into the caller's host arrays
+void next_logprobs(Infer* m, cudaStream_t s, int n, const b200w_logprobs* lp, int64_t& nl) {
+  const int V = m->a.vocab_size, k = lp->top_k;
+  logprobs(m->logits, V, n, V, nullptr, k, m->nx_lse, nullptr, m->nx_tok, m->nx_ids, m->nx_top, s); ++nl;
+  if (lp->lse) B200W_CUDA(cudaMemcpyAsync(lp->lse, m->nx_lse, n * 4, cudaMemcpyDeviceToHost, s));
+  if (lp->token_lp) B200W_CUDA(cudaMemcpyAsync(lp->token_lp, m->nx_tok, n * 4, cudaMemcpyDeviceToHost, s));
+  if (lp->top_ids && k) B200W_CUDA(cudaMemcpyAsync(lp->top_ids, m->nx_ids, n * k * 4, cudaMemcpyDeviceToHost, s));
+  if (lp->top_lp && k) B200W_CUDA(cudaMemcpyAsync(lp->top_lp, m->nx_top, n * k * 4, cudaMemcpyDeviceToHost, s));
+}
+
+// prompt scoring buffers for T prefill rows; a failed allocation leaves none of them behind (B200W_ERR_OOM)
+void ensure_scoring(Infer* m, size_t T) {
+  const size_t rows = std::min<size_t>(T, LP_CHUNK);
+  if (rows > m->lp_chunk_rows) {
+    if (m->lp_chunk) m->release(m->lp_chunk);
+    m->lp_chunk = nullptr;
+    m->lp_chunk_rows = 0;
+    m->lp_chunk = m->alloc<bf16>(rows * m->a.vocab_size);
+    m->lp_chunk_rows = rows;
+  }
+  if (T > m->lp_cap) {
+    for (void* p : {static_cast<void*>(m->lp_tgt), static_cast<void*>(m->lp_top), static_cast<void*>(m->lp_ids),
+                    static_cast<void*>(m->lp_targets)})
+      if (p) m->release(p);
+    m->lp_tgt = m->lp_top = nullptr;
+    m->lp_ids = m->lp_targets = nullptr;
+    m->lp_cap = 0;
+    m->lp_tgt = m->alloc<float>(T);
+    m->lp_top = m->alloc<float>(T * B200W_MAX_TOP_LOGPROBS);
+    m->lp_ids = m->alloc<int32_t>(T * B200W_MAX_TOP_LOGPROBS);
+    m->lp_targets = m->alloc<int32_t>(T);
+    m->lp_cap = T;
+  }
+}
+
 Infer* paged_model(b200w_ctx* ctx) {
   Infer* m = model(ctx);
   if (m->n_pages == 0) throw StateError("the KV cache is not paged (b200w_infer_init_paged)");
@@ -2028,6 +2215,17 @@ void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, co
   B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed with m
 }
 
+void b200w::logprobs(const void* logits, int ld, int rows, int V, const int32_t* targets, int k, float* lse,
+                     float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp, cudaStream_t s) {
+  B200W_CHECK(logits && rows >= 1 && V >= 8 && V % 8 == 0 && ld >= V && ld % 8 == 0 &&
+                  (reinterpret_cast<uintptr_t>(logits) & 15) == 0,
+              "logits must be 16-byte aligned rows of a multiple of 8 entries");
+  B200W_CHECK(k >= 0 && k <= B200W_MAX_TOP_LOGPROBS, "top_k must be in 0..B200W_MAX_TOP_LOGPROBS");
+  logprobs_kernel<<<rows, LP_THREADS, 0, s>>>(static_cast<const bf16*>(logits), ld, V, targets, k, lse, target_lp,
+                                              token_lp, top_ids, top_lp);
+  B200W_CUDA(cudaGetLastError());
+}
+
 extern "C" {
 
 int b200w_infer_init(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch) {
@@ -2259,12 +2457,14 @@ int b200w_infer_init_random(b200w_ctx* ctx, uint64_t seed, float std) {
   });
 }
 
-int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* positions,
-                     const int32_t* slots, int n, int32_t* next_tokens, float* logits_out) {
+// b200w_infer_step and, when next != nullptr, b200w_infer_step_logprobs
+static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* positions, const int32_t* slots, int n,
+                     int32_t* next_tokens, float* logits_out, const b200w_logprobs* next) {
   return iguard(ctx, [&] {
     NvtxRange nvtx_range("b200w decode step");
     Infer* m = model(ctx);
     const auto& a = m->a;
+    check_logprobs(next);
     B200W_CHECK(tokens && positions && slots && n >= 1 && n <= m->max_batch, "bad batch");
     for (int i = 0; i < n; ++i) {
       B200W_CHECK(positions[i] >= 0 && positions[i] < a.max_ctx, "position outside the KV cache");
@@ -2278,6 +2478,7 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     memcpy(m->pin, tokens, n * 4);
     memcpy(m->pin + B, positions, n * 4);
     memcpy(m->pin + 2 * B, slots, n * 4);
+    if (next) ensure_next_logprobs(m);
     ensure_tiled(m, s);   // no-op unless the weights changed since the last step
     int64_t step_launches = 0;
     // Run eagerly the first time a row count is seen (first-use attribute calls), captured into a
@@ -2308,6 +2509,8 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
       m->warm[n] = static_cast<int>(step_launches);
     }
     nl += step_launches;
+    // outside the graph, on the logits it left: the captured step is the same with and without log-probabilities
+    if (next) next_logprobs(m, s, n, next, nl);
     B200W_CUDA(cudaStreamSynchronize(s));
     if (next_tokens) memcpy(next_tokens, m->pin + 3 * B, n * 4);
     if (logits_out) {
@@ -2322,6 +2525,16 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
   });
 }
 
+int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* positions, const int32_t* slots, int n,
+                     int32_t* next_tokens, float* logits_out) {
+  return step_impl(ctx, tokens, positions, slots, n, next_tokens, logits_out, nullptr);
+}
+
+int b200w_infer_step_logprobs(b200w_ctx* ctx, const int32_t* tokens, const int32_t* positions, const int32_t* slots,
+                              int n, int32_t* next_tokens, float* logits_out, const b200w_logprobs* next) {
+  return step_impl(ctx, tokens, positions, slots, n, next_tokens, logits_out, next);
+}
+
 // Prompt ingestion in ONE pass (round 1 fed prompts through b200w_infer_step one token per weight
 // sweep): big-M wgmma GEMMs over all n_seqs * padded_len tokens, the training flash-attention
 // forward (causal within each sequence), K/V of the real positions written to the cache slots, and the
@@ -2329,12 +2542,17 @@ int b200w_infer_step(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
 // from influencing any real position.
 // b200w_infer_prefill (starts == nullptr) and b200w_infer_prefill_cached: row b of `tokens` holds positions
 // [start_b, lengths[b]) of its prompt, start_b = starts ? starts[b] : 0.
+// b200w_infer_prefill_logprobs (cold only): `next` and the prompt outputs as that call documents.
 static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
-                        const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out) {
+                        const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out,
+                        const b200w_logprobs* next = nullptr, float* prompt_lp = nullptr,
+                        int32_t* prompt_top_ids = nullptr, float* prompt_top_lp = nullptr) {
   return iguard(ctx, [&] {
     NvtxRange nvtx_range("b200w prefill");
     Infer* m = starts ? paged_model(ctx) : model(ctx);
     const auto& a = m->a;
+    const int top_k = check_logprobs(next);
+    const bool score = prompt_lp || (top_k && (prompt_top_ids || prompt_top_lp));
     B200W_CHECK(tokens && lengths && slots && n_seqs >= 1 && n_seqs <= m->max_batch, "bad prefill batch");
     B200W_CHECK(padded_len >= 128 && padded_len % 128 == 0, "padded_len must be a positive multiple of 128");
     const int S = padded_len;
@@ -2358,6 +2576,8 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     int64_t& nl = ctx_launches(ctx);
     ensure_prefill(m, T);
     ensure_prefill_pin(m, T);
+    if (next) ensure_next_logprobs(m);
+    if (score) ensure_scoring(m, T);
     const int B = m->max_batch;
     int32_t* pin = m->pf_pin;
     memcpy(pin, tokens, T * 4);
@@ -2372,6 +2592,12 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
       if (starts && a.family == B200W_FAMILY_OPT)
         for (int p = 0; p < S; ++p)
           pin[T + 4 * B + static_cast<size_t>(b) * S + p] = std::min(start + p, lengths[b] - 1);
+      // scoring (cold prefills only, so the positions' staging is free): row p predicts token p + 1
+      if (score)
+        for (int p = 0; p < S; ++p) {
+          const size_t r = static_cast<size_t>(b) * S + p;
+          pin[T + 4 * B + r] = p + 1 < lengths[b] ? tokens[r + 1] : -1;
+        }
     }
     B200W_CUDA(cudaMemcpyAsync(m->pf_tok, pin, T * 4, cudaMemcpyHostToDevice, s));
     B200W_CUDA(cudaMemcpyAsync(m->pf_len, pin + T, n_seqs * 4, cudaMemcpyHostToDevice, s));
@@ -2382,6 +2608,7 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
       if (a.family == B200W_FAMILY_OPT)
         B200W_CUDA(cudaMemcpyAsync(m->pf_pos, pin + T + 4 * B, T * 4, cudaMemcpyHostToDevice, s));
     }
+    if (score) B200W_CUDA(cudaMemcpyAsync(m->lp_targets, pin + T + 4 * B, T * 4, cudaMemcpyHostToDevice, s));
 
     const int d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim,
               V = a.vocab_size;
@@ -2480,7 +2707,48 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     argmax_kernel<<<n_seqs, 1024, 0, s>>>(m->logits, V, m->next); ++nl;
     B200W_CUDA(cudaGetLastError());
     B200W_CUDA(cudaMemcpyAsync(m->pin + 3 * B, m->next, n_seqs * 4, cudaMemcpyDeviceToHost, s));
+    if (next) next_logprobs(m, s, n_seqs, next, nl);
+    std::vector<float> row_lp, row_top;
+    std::vector<int32_t> row_ids;
+    if (score) {
+      // the final norm over every row into pf_nrm (dead since the last layer), then lm_head and the log-softmax in
+      // chunks of rows through lp_chunk: the rows [0, lengths[b] - 1) of each sequence, whose next token is known
+      if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + m->p_lnf_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s);
+      else layernorm_kernel<<<Ti, 256, 0, s>>>(h, m->w + m->p_lnf_w, m->w + m->p_lnf_b, m->pf_nrm, d, a.norm_eps);
+      ++nl;
+      const int C = static_cast<int>(m->lp_chunk_rows);
+      for (int b = 0; b < n_seqs; ++b)
+        for (int p0 = 0; p0 < lengths[b] - 1; p0 += C) {
+          const int rows = std::min(C, lengths[b] - 1 - p0);
+          const size_t r0 = static_cast<size_t>(b) * S + p0;
+          gemm_bf16_ex(m->pf_nrm + r0 * d, false, d, m->w + m->p_lm, false, d, m->lp_chunk, nullptr, false, V, rows, V,
+                       d, 0, nullptr, 0, s); ++nl;
+          logprobs(m->lp_chunk, V, rows, V, m->lp_targets + r0, top_k, nullptr, m->lp_tgt + r0, nullptr,
+                   m->lp_ids + r0 * top_k, m->lp_top + r0 * top_k, s); ++nl;
+        }
+      row_lp.resize(T);
+      row_ids.resize(T * top_k);
+      row_top.resize(T * top_k);
+      B200W_CUDA(cudaMemcpyAsync(row_lp.data(), m->lp_tgt, T * 4, cudaMemcpyDeviceToHost, s));
+      if (top_k) {
+        B200W_CUDA(cudaMemcpyAsync(row_ids.data(), m->lp_ids, T * top_k * 4, cudaMemcpyDeviceToHost, s));
+        B200W_CUDA(cudaMemcpyAsync(row_top.data(), m->lp_top, T * top_k * 4, cudaMemcpyDeviceToHost, s));
+      }
+    }
     B200W_CUDA(cudaStreamSynchronize(s));
+    if (score) {
+      // row p - 1's distribution is position p's; positions 0 and >= lengths[b] have none
+      for (int b = 0; b < n_seqs; ++b)
+        for (int p = 0; p < S; ++p) {
+          const size_t r = static_cast<size_t>(b) * S + p;
+          const bool has = p >= 1 && p < lengths[b];
+          if (prompt_lp) prompt_lp[r] = has ? row_lp[r - 1] : 0.f;
+          for (int j = 0; j < top_k; ++j) {
+            if (prompt_top_ids) prompt_top_ids[r * top_k + j] = has ? row_ids[(r - 1) * top_k + j] : -1;
+            if (prompt_top_lp) prompt_top_lp[r * top_k + j] = has ? row_top[(r - 1) * top_k + j] : 0.f;
+          }
+        }
+    }
     if (next_tokens) memcpy(next_tokens, m->pin + 3 * B, n_seqs * 4);
     if (logits_out) {
       void* tmp = nullptr;
@@ -2503,6 +2771,14 @@ int b200w_infer_prefill_cached(b200w_ctx* ctx, const int32_t* tokens, const int3
                                float* logits_out) {
   if (!starts) return B200W_ERR_INVALID;
   return prefill_impl(ctx, tokens, starts, lengths, slots, n_seqs, padded_len, next_tokens, logits_out);
+}
+
+int b200w_infer_prefill_logprobs(b200w_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const int32_t* slots,
+                                 int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out,
+                                 const b200w_logprobs* next, float* prompt_lp, int32_t* prompt_top_ids,
+                                 float* prompt_top_lp) {
+  return prefill_impl(ctx, tokens, nullptr, lengths, slots, n_seqs, padded_len, next_tokens, logits_out, next,
+                      prompt_lp, prompt_top_ids, prompt_top_lp);
 }
 
 int64_t b200w_infer_device_bytes(b200w_ctx* ctx) {

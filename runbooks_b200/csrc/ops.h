@@ -96,6 +96,12 @@ void attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void
                           const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
                           int H, int Hkv, int dh, float scale, cudaStream_t s, const float* kscale = nullptr,
                           const float* vscale = nullptr);
+// Row-wise log-softmax of bf16 logits [rows, ld] (V % 8 == 0, ld % 8 == 0; infer.cu logprobs_kernel): lse, the
+// log-probability of targets[r] (nullable; an id outside [0, V) gives 0) and of the row maximum, and the k
+// (<= B200W_MAX_TOP_LOGPROBS) largest logits as ids and log-probabilities [rows, k], by value descending with ties
+// to the smaller id. Every output is nullable.
+void logprobs(const void* logits, int ld, int rows, int V, const int32_t* targets, int k, float* lse,
+              float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp, cudaStream_t s);
 
 
 // ---- ops.cu --------------------------------------------------------------------------------

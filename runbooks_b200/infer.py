@@ -242,6 +242,68 @@ class InferEngine(Engine):
                                                          logits.ctypes.data if want_logits else None))
         return nxt, logits
 
+    def step_logprobs(self, tokens, positions, slots, top_k: int, want_logits: bool = False):
+        """step, plus the log-probabilities of each row's next-token distribution (b200w_infer_step_logprobs):
+        -> (next tokens, logits or None, TokenLogprobs)."""
+        tok = np.ascontiguousarray(tokens, dtype=np.int32)
+        pos = np.ascontiguousarray(positions, dtype=np.int32)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        n = tok.size
+        nxt = np.empty(n, dtype=np.int32)
+        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
+        lp, s = TokenLogprobs.alloc(n, top_k)
+        self._check(self._lib.b200w_infer_step_logprobs(self._h, tok.ctypes.data, pos.ctypes.data, sl.ctypes.data, n,
+                                                        nxt.ctypes.data, logits.ctypes.data if want_logits else None,
+                                                        C.byref(s)))
+        return nxt, logits, lp
+
+    def prefill_logprobs(self, prompts: List[List[int]], slots: List[int], top_k: int, want_logits: bool = False,
+                         score_prompts: bool = True):
+        """prefill (cold), plus the next-token log-probabilities and, with score_prompts, every prompt position's
+        (b200w_infer_prefill_logprobs): -> (next tokens, logits or None, TokenLogprobs, prompt) where prompt[i] is
+        None or (lp [len], top_ids [len, top_k], top_lp [len, top_k]) of prompts[i]; lp[p] = log P(prompt[p] |
+        prompt[:p]) and position 0 has none (0, ids -1)."""
+        n = len(prompts)
+        S = ((max(len(p) for p in prompts) + 127) // 128) * 128
+        tok = np.zeros((n, S), dtype=np.int32)
+        for i, p in enumerate(prompts):
+            tok[i, :len(p)] = p
+        lens = np.array([len(p) for p in prompts], dtype=np.int32)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        nxt = np.empty(n, dtype=np.int32)
+        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
+        lp, s = TokenLogprobs.alloc(n, top_k)
+        if score_prompts:
+            plp = np.empty((n, S), dtype=np.float32)
+            pids = np.empty((n, S, top_k), dtype=np.int32)
+            ptop = np.empty((n, S, top_k), dtype=np.float32)
+        self._check(self._lib.b200w_infer_prefill_logprobs(
+            self._h, tok.ctypes.data, lens.ctypes.data, sl.ctypes.data, n, S, nxt.ctypes.data,
+            logits.ctypes.data if want_logits else None, C.byref(s), plp.ctypes.data if score_prompts else None,
+            pids.ctypes.data if score_prompts and top_k else None, ptop.ctypes.data if score_prompts and top_k else None))
+        prompt = [(plp[i, :len(p)], pids[i, :len(p)], ptop[i, :len(p)]) if score_prompts else None
+                  for i, p in enumerate(prompts)]
+        return nxt, logits, lp, prompt
+
+
+@dataclass
+class TokenLogprobs:
+    """Host arrays of a b200w_logprobs: per row the log-sum-exp of the next-token logits, the log-probability of the
+    greedy token and the top_k largest logits' ids and log-probabilities (descending, ties to the smaller id)."""
+    lse: np.ndarray
+    token_lp: np.ndarray
+    top_ids: np.ndarray
+    top_lp: np.ndarray
+
+    @classmethod
+    def alloc(cls, n: int, top_k: int):
+        if not 0 <= top_k <= _lib.MAX_TOP_LOGPROBS:
+            raise ValueError(f"top_k must be in 0..{_lib.MAX_TOP_LOGPROBS}, got {top_k}")
+        lp = cls(np.empty(n, np.float32), np.empty(n, np.float32), np.empty((n, top_k), np.int32),
+                 np.empty((n, top_k), np.float32))
+        return lp, _lib.Logprobs(top_k, 0, lp.lse.ctypes.data, lp.token_lp.ctypes.data, lp.top_ids.ctypes.data,
+                                 lp.top_lp.ctypes.data)
+
 
 def sample_token(logits: np.ndarray, temperature: float, top_p: float, rng: np.random.Generator) -> int:
     """Host-side sampling of one row (the engine itself is greedy): softmax(logits / T) restricted to the
@@ -274,10 +336,20 @@ class _Req:
     cached_tokens: int = 0                                    # prompt positions whose K/V came from the prefix index
     nodes: List["_Node"] = field(default_factory=list)        # index nodes whose page the slot holds
     entered: List["_Node"] = field(default_factory=list)      # of those, the ones this request's prefill fills
+    # log-probabilities: `logprobs` top entries per token (None: not asked). out_lp[i] = (log-probability of out[i],
+    # [(id, log-probability)] of the top entries); prompt_lp the same per prompt position, None at position 0
+    logprobs: Optional[int] = None
+    prompt_logprobs: bool = False
+    out_lp: List[Tuple[float, List[Tuple[int, float]]]] = field(default_factory=list)
+    prompt_lp: Optional[List[Optional[Tuple[float, List[Tuple[int, float]]]]]] = None
 
     @property
     def greedy(self) -> bool:
         return self.temperature <= 0.0
+
+    @property
+    def scores_prompt(self) -> bool:
+        return self.prompt_logprobs and len(self.prompt) > 1
 
 
 class _Node:
@@ -317,12 +389,23 @@ class Generator:
         self._tick = 0
 
     def add(self, prompt: List[int], max_tokens: int, temperature: float = 0.0, top_p: float = 1.0,
-            seed: Optional[int] = None, defer_prefill: bool = False) -> _Req:
+            seed: Optional[int] = None, defer_prefill: bool = False, logprobs: Optional[int] = None,
+            prompt_logprobs: bool = False) -> _Req:
         """defer_prefill: only register the request; flush_prefill() then ingests every deferred prompt of the
         same padded length in ONE prefill call (what the scheduler does when several requests are admitted in
-        the same round)."""
+        the same round).
+        logprobs (0..5): record the log-probability of every generated token and its `logprobs` top entries
+        (req.out_lp); prompt_logprobs: the same for every prompt position after the first (req.prompt_lp), computed
+        by the prefill. Both are the engine's raw log-softmax (temperature 1, no top_p), and a request that asks for
+        either borrows no prefix-cache pages: their hidden states are needed and were never computed."""
         if not prompt:
             raise ValueError("empty prompt")
+        if logprobs is not None and not (isinstance(logprobs, int) and 0 <= logprobs <= _lib.MAX_TOP_LOGPROBS):
+            raise ValueError(f"logprobs must be in 0..{_lib.MAX_TOP_LOGPROBS}, got {logprobs!r}")
+        if logprobs is not None and not hasattr(self.e, "step_logprobs"):
+            raise ValueError("log-probabilities need an engine that computes them")
+        if prompt_logprobs and not (self.use_prefill and hasattr(self.e, "prefill_logprobs")):
+            raise ValueError("prompt log-probabilities need an engine that prefills")
         V = self.e.serve_arch.vocab_size
         bad = [t for t in prompt if not 0 <= int(t) < V]
         if bad:   # a per-request error (HTTP 400), never an engine failure that would take the server down
@@ -336,14 +419,17 @@ class Generator:
             raise RuntimeError("no free cache slot")
         matched, entered = [], []
         if self.prefix_cache:
-            matched, entered = self._admit(list(prompt), len(prompt) + max_tokens, self.free[-1])
+            matched, entered = self._admit(list(prompt), len(prompt) + max_tokens, self.free[-1],
+                                           borrow=logprobs is None and not prompt_logprobs)
         elif self.kv_pages is not None:
             if pages_for(len(prompt) + max_tokens) > self.e.kv_pages_free():
                 raise CacheFull("KV cache full: too few free pages for this request now")
             self.e.reserve(self.free[-1], len(prompt) + max_tokens)
         r = _Req(list(prompt), max_tokens, [], 0, self.free.pop(), False, float(temperature), float(top_p),
                  np.random.default_rng(seed) if temperature > 0 else None,
-                 len(matched) * KV_PAGE, matched + entered, entered)
+                 len(matched) * KV_PAGE, matched + entered, entered, logprobs, bool(prompt_logprobs))
+        if r.prompt_logprobs and not r.scores_prompt:
+            r.prompt_lp = [None]          # one token: nothing to score
         self.active.append(r)
         if self.use_prefill and len(prompt) > 1:
             self._deferred.append(r)
@@ -351,14 +437,15 @@ class Generator:
                 self.flush_prefill()
         return r
 
-    def _admit(self, prompt: List[int], n_tokens: int, slot: int):
+    def _admit(self, prompt: List[int], n_tokens: int, slot: int, borrow: bool = True):
         """Prefix cache admission into `slot`: the longest chain of indexed pages that prefixes the prompt (at most
         (len - 1) // 128, so that at least one prompt token is computed for the next-token logits) is shared; the
         request's own full prompt pages beyond it enter the index at once, so that requests admitted later in the
-        same round share them too. -> (matched nodes, entered nodes)."""
+        same round share them too. borrow=False shares nothing (a request whose every position is computed).
+        -> (matched nodes, entered nodes)."""
         matched: List[_Node] = []
         node = self._root
-        for k in range((len(prompt) - 1) // KV_PAGE):
+        for k in range((len(prompt) - 1) // KV_PAGE if borrow else 0):
             node = node.children.get(tuple(prompt[k * KV_PAGE:(k + 1) * KV_PAGE]))
             if node is None:
                 break
@@ -416,25 +503,32 @@ class Generator:
         128 tokens. Cold prompts (no cached prefix) go first, then the others in ascending prefix length: a request
         shares only pages that a request with a shorter prefix fills, so those are written by an earlier call."""
         pend, self._deferred = self._deferred, []
-        groups: Dict[Tuple[int, int], List[_Req]] = {}
-        for r in pend:
-            groups.setdefault((r.cached_tokens, pages_for(len(r.prompt) - r.cached_tokens)), []).append(r)
+        groups: Dict[Tuple[int, int, bool], List[_Req]] = {}
+        for r in pend:   # prompts to score go through their own calls: a plain prompt never pays for scoring
+            groups.setdefault((r.cached_tokens, pages_for(len(r.prompt) - r.cached_tokens), r.scores_prompt),
+                              []).append(r)
         calls = []
-        for (start, blocks), rs in sorted(groups.items()):
+        for (start, blocks, score), rs in sorted(groups.items()):
             # paged: a call's n_seqs * padded_len stays within the prefill workspace the engine allocated
             per_call = max(1, self.e.prefill_tokens // (blocks * 128)) if self.kv_pages is not None else len(rs)
-            calls += [(start, rs[i:i + per_call]) for i in range(0, len(rs), per_call)]
-        for ci, (start, rs) in enumerate(calls):
+            calls += [(start, score, rs[i:i + per_call]) for i in range(0, len(rs), per_call)]
+        for ci, (start, score, rs) in enumerate(calls):
             need_logits = any(not r.greedy for r in rs)
+            top_k = max((r.logprobs for r in rs if r.logprobs is not None), default=None)
+            lp = prompt = None
             try:
                 if start:
                     nxt, lg = self.e.prefill_cached([r.prompt for r in rs], [start] * len(rs), [r.slot for r in rs],
                                                     want_logits=need_logits)
+                elif score or top_k is not None:
+                    nxt, lg, lp, prompt = self.e.prefill_logprobs([r.prompt for r in rs], [r.slot for r in rs],
+                                                                  top_k or 0, want_logits=need_logits,
+                                                                  score_prompts=score)
                 else:
                     nxt, lg = self.e.prefill([r.prompt for r in rs], [r.slot for r in rs], want_logits=need_logits)
             except Exception:
                 # the pages this call and the calls after it were to fill hold no K/V: out of the index
-                for _, later in calls[ci:]:
+                for _, _, later in calls[ci:]:
                     for r in later:
                         for n in r.entered:
                             if n in self._nodes:
@@ -444,8 +538,23 @@ class Generator:
                 raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
             for i, r in enumerate(rs):
                 r.fed = len(r.prompt)
-                self._emit(r, int(nxt[i]) if r.greedy else sample_token(lg[i], r.temperature, r.top_p, r.rng))
+                if score:
+                    plp, pids, ptop = prompt[i]
+                    k = r.logprobs or 0
+                    r.prompt_lp = [None] + [(float(plp[p]), list(zip(pids[p, :k].tolist(), ptop[p, :k].tolist())))
+                                            for p in range(1, len(r.prompt))]
+                self._emit_token(r, i, nxt, lg, lp)
         self._retire()
+
+    def _emit_token(self, r: _Req, i: int, nxt, lg, lp: Optional[TokenLogprobs]):
+        """Emits row i's token for r: the greedy one, or one sampled from its logits; with its log-probability when
+        r asks for it (the greedy token's from the engine, a sampled one's from its logit and the row's lse)."""
+        t = int(nxt[i]) if r.greedy else sample_token(lg[i], r.temperature, r.top_p, r.rng)
+        if r.logprobs is not None:
+            x = lp.token_lp[i] if r.greedy else np.float32(lg[i][t]) - lp.lse[i]
+            k = r.logprobs
+            r.out_lp.append((float(x), list(zip(lp.top_ids[i, :k].tolist(), lp.top_lp[i, :k].tolist()))))
+        self._emit(r, t)
 
     def _emit(self, r: _Req, t: int):
         r.out.append(t)
@@ -479,14 +588,20 @@ class Generator:
             return
         toks = [(r.prompt[r.fed] if r.fed < len(r.prompt) else r.out[-1]) for r in self.active]
         need_logits = any(not r.greedy for r in self.active)
-        nxt, lg = self.e.step(toks, [r.fed for r in self.active], [r.slot for r in self.active],
-                              want_logits=need_logits)
+        top_k = max((r.logprobs for r in self.active if r.logprobs is not None), default=None)
+        lp = None
+        if top_k is None:
+            nxt, lg = self.e.step(toks, [r.fed for r in self.active], [r.slot for r in self.active],
+                                  want_logits=need_logits)
+        else:
+            nxt, lg, lp = self.e.step_logprobs(toks, [r.fed for r in self.active], [r.slot for r in self.active],
+                                               top_k, want_logits=need_logits)
         if need_logits and lg is None:
             raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
-        for i, (r, t) in enumerate(zip(self.active, nxt)):
+        for i, r in enumerate(self.active):
             r.fed += 1
             if r.fed >= len(r.prompt):        # the token just fed was the last known one
-                self._emit(r, int(t) if r.greedy else sample_token(lg[i], r.temperature, r.top_p, r.rng))
+                self._emit_token(r, i, nxt, lg, lp)
         self._retire()
 
     def generate(self, prompts: List[List[int]], max_tokens: int) -> List[List[int]]:

@@ -8,8 +8,9 @@ Contract (docs/container-contract.md:50-55; server_controller.go:156-173): liste
 test/system.sh:73-78 and the basaran image speak — `POST /v1/completions {"prompt", "max_tokens"}`
 returns an OpenAI-style completion; `"stream": true` answers with server-sent events (one `data:` JSON
 chunk per text delta, then `data: [DONE]`), as basaran does. Accepted and honoured: temperature / top_p
-(host-side nucleus sampling over the engine's logits; default 0 = greedy), stop, n, echo, seed; anything
-else that would change the result (logprobs, penalties, best_of) is a 400. Prompts are ingested in one
+(host-side nucleus sampling over the engine's logits; default 0 = greedy), stop, n, echo, seed, a prompt of
+token ids, and logprobs up to the server's max_logprobs (0 by default: logprobs > 0 is then a 400); anything
+else that would change the result (penalties, best_of) is a 400. Prompts are ingested in one
 prefill pass; continuous batching over the engine's cache slots (one scheduler thread owns the GPU,
 HTTP handler threads only queue requests); a full admission queue answers 503 + Retry-After.
 """
@@ -37,24 +38,73 @@ class Scheduler(threading.Thread):
     advances every active request by one token per engine step, and feeds each request's event queue
     (text deltas for streaming clients, one final record for everybody)."""
 
-    def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False):
+    def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False, max_logprobs: int = 0):
+        """max_logprobs (0..5): the most top entries a request may ask for with `logprobs`; 0 refuses them."""
         super().__init__(daemon=True)
         from .infer import Generator
         self.gen = Generator(engine, eos_id=tokenizer.eos_id, prefix_cache=prefix_cache)
         self.tok, self.q = tokenizer, queue.Queue()
         self.max_queue = max_queue or 4 * engine.max_batch
+        self.max_logprobs = max_logprobs
         self.ready = threading.Event()
         self.failed: str | None = None
 
-    def submit(self, prompt: str, max_tokens: int, temperature: float = 0.0, top_p: float = 1.0, stop=(),
-               seed=None):
-        """-> item (dict) or None when the admission queue is full (the caller answers 503)."""
+    def submit(self, prompt, max_tokens: int, temperature: float = 0.0, top_p: float = 1.0, stop=(),
+               seed=None, logprobs=None, echo: bool = False):
+        """prompt: text, or token ids fed as given. logprobs (None: not asked): log-probabilities of the completion
+        tokens with that many top entries, and with echo of the prompt tokens too.
+        -> item (dict) or None when the admission queue is full (the caller answers 503)."""
         if self.q.qsize() >= self.max_queue:
             return None
         item = {"prompt": prompt, "max_tokens": max_tokens, "temperature": temperature, "top_p": top_p,
-                "stop": tuple(stop), "seed": seed, "events": queue.Queue(), "cancelled": False}
+                "stop": tuple(stop), "seed": seed, "events": queue.Queue(), "cancelled": False,
+                "logprobs": logprobs, "echo": echo}
+        if isinstance(prompt, list):
+            item["ids"] = list(prompt)
         self.q.put(item)
         return item
+
+    # ---- log-probabilities in the OpenAI completions shape (scheduler thread only) ----
+    def _detok(self, ids, st):
+        """Extends st["strs"] to one string per id by incremental decoding: a token's string is the text it completes
+        given the tokens before it ("" while it only starts a character, e.g. part of a UTF-8 sequence)."""
+        strs = st.setdefault("strs", [])
+        for i in range(len(strs), len(ids)):
+            p, r = st.get("p", 0), st.get("r", 0)
+            prev = self.tok.decode(ids[p:r])
+            new = self.tok.decode(ids[p:i + 1])
+            if len(new) > len(prev) and not new.endswith("\ufffd"):
+                strs.append(new[len(prev):])
+                st["p"], st["r"] = r, i + 1
+            else:
+                strs.append("")
+        return strs
+
+    def _lp_entries(self, strs, lps, base, first, last, offset0):
+        """{"tokens", "token_logprobs", "top_logprobs", "text_offset"} of tokens [first, last): offset0 is the text
+        offset of token `first`; lps[i] is (log-probability, [(id, log-probability)]) or None (no distribution)."""
+        e = {"tokens": [], "token_logprobs": [], "top_logprobs": [], "text_offset": []}
+        off = offset0
+        for i in range(first, last):
+            e["tokens"].append(strs[i])
+            e["text_offset"].append(base + off)
+            off += len(strs[i])
+            if lps[i] is None:
+                e["token_logprobs"].append(None)
+                e["top_logprobs"].append(None)
+                continue
+            lp, top = lps[i]
+            d = {self.tok.decode([t]): v for t, v in top}
+            d[strs[i]] = lp          # the chosen token is always listed
+            e["token_logprobs"].append(lp)
+            e["top_logprobs"].append(d)
+        return e
+
+    def _prompt_entries(self, req):
+        """The echoed prompt's text and entries: every prompt token as the engine saw it, the first without a
+        log-probability."""
+        strs = self._detok(req.prompt, {})
+        return "".join(strs), self._lp_entries(strs, req.prompt_lp, 0, 0, len(strs), 0)
 
     # ---- per-request bookkeeping (scheduler thread only) ----
     def _progress(self, req, item, n_prompt, state):
@@ -62,11 +112,11 @@ class Scheduler(threading.Thread):
         out = req.out
         eos_hit = self.tok.eos_id is not None and out and out[-1] == self.tok.eos_id
         text = self.tok.decode(out[:-1] if eos_hit else out)
-        finish = None
+        finish, cut = None, False
         for st in item["stop"]:
             k = text.find(st)
             if k >= 0:
-                text, finish = text[:k], "stop"
+                text, finish, cut = text[:k], "stop", True
                 break
         if finish is None and req.done:
             finish = "stop" if eos_hit else "length"
@@ -77,14 +127,32 @@ class Scheduler(threading.Thread):
             safe = max(state["sent"], len(text) - hold)
             if text.endswith("\ufffd"):
                 safe = min(safe, len(text) - 1)
+        if item["logprobs"] is not None:
+            # the entries of the tokens whose text starts in the text sent so far (EOS adds none and is not listed);
+            # at the end every token, or after a stop string those that start before the cut
+            strs = self._detok(out[:-1] if eos_hit else out, state["detok"])
+            i0 = i = state["lp_n"]
+            off = state["lp_off"]
+            while i < len(strs) and (off < safe or (finish is not None and not cut)):
+                off += len(strs[i])
+                i += 1
+            if i > i0:
+                e = self._lp_entries(strs, req.out_lp, state["base"], i0, i, state["lp_off"])
+                for key, vals in e.items():
+                    state["lp"][key] += vals
+                item["events"].put(("logprobs", e))
+                state["lp_n"], state["lp_off"] = i, off
         if safe > state["sent"]:
             item["events"].put(("delta", text[state["sent"]:safe]))
             state["sent"] = safe
         if finish is not None:
             if not req.done:            # stopped by a stop string: free the slot now
                 self.gen.cancel(req)
-            item["events"].put(("done", {"text": text, "prompt_tokens": n_prompt, "completion_tokens": len(out),
-                                         "cached_tokens": req.cached_tokens, "finish_reason": finish}))
+            done = {"text": text, "prompt_tokens": n_prompt, "completion_tokens": len(out),
+                    "cached_tokens": req.cached_tokens, "finish_reason": finish}
+            if item["logprobs"] is not None:
+                done["logprobs"] = state["lp"]
+            item["events"].put(("done", done))
             return True
         return False
 
@@ -117,7 +185,8 @@ class Scheduler(threading.Thread):
                             item["ids"] = [self.tok.bos_id] + ids if self.tok.bos_id is not None else ids
                         ids = item["ids"]
                         req = self.gen.add(ids, item["max_tokens"], item["temperature"], item["top_p"], item["seed"],
-                                           defer_prefill=True)
+                                           defer_prefill=True, logprobs=item["logprobs"],
+                                           prompt_logprobs=item["echo"] and item["logprobs"] is not None)
                         admitted.append((req, item, len(ids)))
                     except CacheFull:       # fits the pool, not now: keep its place, retry after the next step
                         held = item
@@ -136,6 +205,14 @@ class Scheduler(threading.Thread):
                         admitted = []
                     for req, item, n_ids in admitted:
                         state = {"sent": 0}
+                        if item["logprobs"] is not None:
+                            state.update(detok={}, lp_n=0, lp_off=0, base=0,
+                                         lp={"tokens": [], "token_logprobs": [], "top_logprobs": [], "text_offset": []})
+                            if item["echo"]:   # completion offsets count from the start of the echoed prompt
+                                echo, state["lp"] = self._prompt_entries(req)
+                                state["base"] = len(echo)
+                                item["events"].put(("prompt", (echo, state["lp"])))
+                                state["lp"] = {k: list(v) for k, v in state["lp"].items()}
                         if not self._progress(req, item, n_ids, state):
                             pending[id(req)] = (req, item, n_ids, state)
                 try:
@@ -163,16 +240,22 @@ class Scheduler(threading.Thread):
             os._exit(1)
 
 
-def parse_completion_request(req: dict) -> dict:
+def _is_token_ids(x) -> bool:
+    return isinstance(x, list) and len(x) > 0 and all(isinstance(t, int) and not isinstance(t, bool) for t in x)
+
+
+def parse_completion_request(req: dict, max_logprobs: int = 0) -> dict:
     """The OpenAI / basaran `/v1/completions` fields. Everything that is accepted is honoured; a value this
-    server does not implement is a 400, never a silent fallback to something else."""
+    server does not implement is a 400, never a silent fallback to something else.
+    prompt: a string, a list of token ids (fed as given, no BOS added), or a list holding one of either.
+    logprobs: refused above 0 unless the server was started with max_logprobs >= 1; then 0..max_logprobs."""
     prompt = req["prompt"]
-    if isinstance(prompt, list):
+    if isinstance(prompt, list) and not _is_token_ids(prompt):
         if len(prompt) != 1:
             raise ValueError("exactly one prompt per request")
         prompt = prompt[0]
-    if not isinstance(prompt, str):
-        raise ValueError("prompt must be a string")
+    if not (isinstance(prompt, str) or _is_token_ids(prompt)):
+        raise ValueError("prompt must be a string or a list of token ids")
     max_tokens = int(req.get("max_tokens", 16))
     if max_tokens < 1:
         raise ValueError("max_tokens must be >= 1")
@@ -194,7 +277,15 @@ def parse_completion_request(req: dict) -> dict:
     stream = bool(req.get("stream", False))
     if stream and n != 1:
         raise ValueError("stream with n > 1 is not implemented")
+    logprobs = req.get("logprobs")
+    if max_logprobs >= 1 and logprobs is not None:
+        if isinstance(logprobs, bool) or not isinstance(logprobs, int) or not 0 <= logprobs <= max_logprobs:
+            raise ValueError(f"logprobs must be an integer in 0..{max_logprobs}")
+    else:
+        logprobs = None
     for key, default in (("logprobs", None), ("best_of", None), ("suffix", None), ("logit_bias", None)):
+        if key == "logprobs" and max_logprobs >= 1:
+            continue
         if req.get(key, default) not in (default, 0 if key == "logprobs" else default, 1 if key == "best_of" else default):
             raise ValueError(f"{key} is not implemented")
     for key in ("presence_penalty", "frequency_penalty"):
@@ -202,7 +293,8 @@ def parse_completion_request(req: dict) -> dict:
             raise ValueError(f"{key} is not implemented")
     seed = req.get("seed")
     return dict(prompt=prompt, max_tokens=max_tokens, temperature=temperature, top_p=top_p, n=n, stop=stop,
-                stream=stream, echo=bool(req.get("echo", False)), seed=None if seed is None else int(seed))
+                stream=stream, echo=bool(req.get("echo", False)), seed=None if seed is None else int(seed),
+                logprobs=logprobs)
 
 
 def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 600.0):
@@ -231,22 +323,25 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             else:
                 self._send(404, {"error": "not found"})
 
-        def _chunk(self, cid, created, text, finish):
+        def _chunk(self, cid, created, text, finish, logprobs=None):
             return {"id": cid, "object": "text_completion", "created": created, "model": model_name,
-                    "choices": [{"index": 0, "text": text, "logprobs": None, "finish_reason": finish}]}
+                    "choices": [{"index": 0, "text": text, "logprobs": logprobs, "finish_reason": finish}]}
 
         def do_POST(self):
             if self.path != "/v1/completions":
                 return self._send(404, {"error": "not found"})
             try:
                 n = int(self.headers.get("Content-Length", "0"))
-                r = parse_completion_request(json.loads(self.rfile.read(n) or b"{}"))
+                r = parse_completion_request(json.loads(self.rfile.read(n) or b"{}"), sched.max_logprobs)
             except Exception as e:  # noqa: BLE001
                 return self._send(400, {"error": f"bad request: {e}"})
+            # the echoed prompt: a token-id prompt's decoding; with log-probabilities, the prompt tokens' strings
+            echo = r["prompt"] if isinstance(r["prompt"], str) else sched.tok.decode(r["prompt"])
             items = []
             for i in range(r["n"]):
                 seed = None if r["seed"] is None else r["seed"] + i
-                it = sched.submit(r["prompt"], r["max_tokens"], r["temperature"], r["top_p"], r["stop"], seed)
+                it = sched.submit(r["prompt"], r["max_tokens"], r["temperature"], r["top_p"], r["stop"], seed,
+                                  r["logprobs"], r["echo"])
                 if it is None:          # back-pressure: every slot busy and the admission queue full
                     for x in items:
                         x["cancelled"] = True
@@ -256,7 +351,7 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             cid, created = "cmpl-" + uuid.uuid4().hex[:24], int(time.time())
             deadline = time.time() + request_timeout_s
             if r["stream"]:
-                return self._stream(items[0], r, cid, created, deadline)
+                return self._stream(items[0], r, echo, cid, created, deadline)
             choices, usage_p, usage_c, cached = [], 0, 0, 0
             for i, it in enumerate(items):
                 final = None
@@ -271,10 +366,13 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
                         for x in items:
                             x["cancelled"] = True
                         return self._send(400, {"error": val})
+                    if kind == "prompt":
+                        echo = val[0]
                     if kind == "done":
                         final = val
-                text = (r["prompt"] if r["echo"] else "") + final["text"]
-                choices.append({"index": i, "text": text, "logprobs": None, "finish_reason": final["finish_reason"]})
+                text = (echo if r["echo"] else "") + final["text"]
+                choices.append({"index": i, "text": text, "logprobs": final.get("logprobs"),
+                                "finish_reason": final["finish_reason"]})
                 usage_p, usage_c = final["prompt_tokens"], usage_c + final["completion_tokens"]
                 # the prompt is counted once, as prompt_tokens is: its tokens that the best-served copy found cached
                 cached = max(cached, final["cached_tokens"])
@@ -284,9 +382,10 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             self._send(200, {"id": cid, "object": "text_completion", "created": created, "model": model_name,
                              "choices": choices, "usage": usage})
 
-        def _stream(self, item, r, cid, created, deadline):
+        def _stream(self, item, r, echo, cid, created, deadline):
             """Server-sent events, the OpenAI / basaran streaming shape: one `data: {json}` per text delta,
-            a final chunk carrying finish_reason, then `data: [DONE]`."""
+            a final chunk carrying finish_reason, then `data: [DONE]`. With logprobs, each chunk carries the entries of
+            the tokens whose text starts in it (the echo chunk the prompt's), and the final chunk any left."""
             self.send_response(200)
             self.send_header("Content-Type", "text/event-stream")
             self.send_header("Cache-Control", "no-cache")
@@ -297,9 +396,12 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             def emit(obj):
                 self.wfile.write(b"data: " + (obj if isinstance(obj, bytes) else json.dumps(obj).encode()) + b"\n\n")
                 self.wfile.flush()
+            lp = r["logprobs"] is not None
+            empty = {"tokens": [], "token_logprobs": [], "top_logprobs": [], "text_offset": []}
             try:
-                if r["echo"]:
-                    emit(self._chunk(cid, created, r["prompt"], None))
+                if r["echo"] and not lp:
+                    emit(self._chunk(cid, created, echo, None))
+                entries = empty
                 while True:
                     try:
                         kind, val = item["events"].get(timeout=max(0.0, deadline - time.time()))
@@ -307,13 +409,18 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
                         item["cancelled"] = True
                         emit({"error": "request timed out"})
                         break
-                    if kind == "delta":
-                        emit(self._chunk(cid, created, val, None))
+                    if kind == "prompt":
+                        emit(self._chunk(cid, created, val[0], None, val[1]))
+                    elif kind == "logprobs":
+                        entries = {k: entries[k] + val[k] for k in empty}
+                    elif kind == "delta":
+                        emit(self._chunk(cid, created, val, None, entries if lp else None))
+                        entries = empty
                     elif kind == "error":
                         emit({"error": val})
                         break
                     else:
-                        emit(self._chunk(cid, created, "", val["finish_reason"]))
+                        emit(self._chunk(cid, created, "", val["finish_reason"], entries if lp else None))
                         break
                 emit(b"[DONE]")
             except (BrokenPipeError, ConnectionResetError):
@@ -358,6 +465,22 @@ def prefix_cache_param(content: str, prefix_cache: bool | None = None, environ=N
     if isinstance(v, str) and v.strip().lower() in ("true", "1", "yes", "false", "0", "no"):
         return v.strip().lower() in ("true", "1", "yes")
     raise ValueError(f"param 'prefix_cache': cannot read {v!r} as a boolean")
+
+
+def max_logprobs_param(content: str, max_logprobs: int | None = None, environ=None) -> int:
+    """The most top entries a request may ask for with `logprobs` (vLLM's max_logprobs), 0..5: --max-logprobs, else
+    the params' max_logprobs (params.json, PARAM_MAX_LOGPROBS over it), else 0, which refuses logprobs > 0."""
+    if max_logprobs is None:
+        extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
+        v = max_logprobs = extra.get("max_logprobs", 0)
+        if isinstance(v, str):
+            try:
+                max_logprobs = int(v.strip())
+            except ValueError as e:
+                raise ValueError(f"param 'max_logprobs': cannot read {v!r} as an integer") from e
+    if isinstance(max_logprobs, bool) or not isinstance(max_logprobs, int) or not 0 <= max_logprobs <= 5:
+        raise ValueError(f"max_logprobs must be an integer in 0..5, got {max_logprobs!r}")
+    return max_logprobs
 
 
 KV_CACHE_DTYPES = {"auto": "bf16", "bf16": "bf16", "fp8": "fp8", "fp8_e4m3": "fp8"}
@@ -412,10 +535,11 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
-          prefix_cache: bool | None = None, kv_cache_dtype: str | None = None):
+          prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
     prefix_cache = prefix_cache_param(content, prefix_cache)
     kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
+    max_logprobs = max_logprobs_param(content, max_logprobs)
     if prefix_cache and kv_cache_gb is None:
         raise ValueError("prefix_cache shares pages of the paged KV cache: it needs kv_cache_gb")
     if kv_dtype != "bf16" and kv_cache_gb is None:
@@ -424,12 +548,12 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
     t0 = time.time()
     engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype)
     tok = contract.Tokenizer(model_dir)
-    sched = Scheduler(engine, tok, prefix_cache=prefix_cache)
+    sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs)
     sched.start()
     name = cfg.get("_name_or_path") or cfg.get("model_type", "model")
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
     ready = {"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
-             "max_batch": max_batch}
+             "max_batch": max_batch, "max_logprobs": max_logprobs}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
         ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch, kv_dtype) / 1e6, 2),
@@ -453,9 +577,13 @@ def main(argv=None) -> int:
     ap.add_argument("--kv-cache-dtype", default=None,
                     help="element type of the paged KV cache: auto / bf16, or fp8 / fp8_e4m3 (needs kv_cache_gb; "
                          "default: param kv_cache_dtype, else bf16)")
+    ap.add_argument("--max-logprobs", type=int, default=None,
+                    help="the most top entries a request may ask for with logprobs, 0..5 (default: param "
+                         "max_logprobs, else 0: logprobs > 0 is refused)")
     a = ap.parse_args(argv)
     try:
-        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype)
+        serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype,
+              a.max_logprobs)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()
