@@ -315,6 +315,30 @@ B200W_API int b200w_infer_prefill_logprobs(b200w_ctx* ctx, const int32_t* tokens
                                            const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
                                            float* logits_out, const b200w_logprobs* next, float* prompt_lp,
                                            int32_t* prompt_top_ids, float* prompt_top_lp);
+/* Sampling on the device (DESIGN §3.5). Per row: order the tokens by logit descending, ties to the smaller id;
+ * weights w = exp((x - max) / T); top_k keeps the first k tokens of that order; top_p keeps, of those, the shortest
+ * prefix of the order whose weight reaches top_p of theirs (top_k first, then top_p); the token is the smallest id
+ * i of the kept set with sum of w over kept ids <= i above u * (weight of the kept set). u in [0, 1) is word 0 of
+ * Philox4x32-10 with key (seed low word, seed high word) and counter (draw low, draw high, 0, 0), shifted right by 8
+ * and scaled by 2^-24: a request's stream depends on its seed and on how many tokens it has drawn, not on its row,
+ * its slot or the rest of the batch. A row with temperature <= 0 gets the greedy token of the step calls.
+ * NULL arrays, a non-zero reserved, a NaN or infinite temperature, top_p outside (0, 1] or top_k outside 0..vocab
+ * are B200W_ERR_INVALID before any GPU work. */
+typedef struct b200w_sampling {
+  int32_t reserved;            /* zero                                                      */
+  const float* temperature;    /* HOST [n]; <= 0: the row is greedy                         */
+  const float* top_p;          /* HOST [n], (0, 1]; 1 = off                                 */
+  const int32_t* top_k;        /* HOST [n], 0 = off, else 1..vocab                          */
+  const uint64_t* seed;        /* HOST [n]                                                  */
+  const uint64_t* draw;        /* HOST [n]: index of this draw within the request           */
+} b200w_sampling;
+/* Samples rows [0, n) of the logits that the immediately preceding successful b200w_infer_step* /
+ * b200w_infer_prefill* call left on the device; n must equal that call's row count. After any other b200w_infer_*
+ * call (a weight load, a page reservation, a failed step), or with another n, B200W_ERR_STATE; a sample call itself
+ * may be repeated. tokens_out HOST [n]; token_logit_out HOST [n] or NULL: the sampled token's logit as fp32 (its
+ * log-probability is that minus the row's lse). The staging buffers are allocated by the first call and kept. */
+B200W_API int b200w_infer_sample(b200w_ctx* ctx, int n, const b200w_sampling* sampling, int32_t* tokens_out,
+                                 float* token_logit_out);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.
@@ -408,6 +432,12 @@ B200W_API int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int l
 B200W_API int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets,
                                 int top_k, float* lse, float* target_lp, float* token_lp, int32_t* top_ids,
                                 float* top_lp);
+/* The kernel of b200w_infer_sample on bf16 DEVICE logits [rows, ld] (vocab V % 8 == 0, ld % 8 == 0). sampling, u,
+ * tokens_out and token_logit_out (nullable) are HOST arrays [rows]; u NULL: Philox from seed / draw, else the
+ * uniform numbers to use. */
+B200W_API int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V,
+                              const b200w_sampling* sampling, const float* u, int32_t* tokens_out,
+                              float* token_logit_out);
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);

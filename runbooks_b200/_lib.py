@@ -51,6 +51,12 @@ class Logprobs(C.Structure):
                 ("top_lp", vp)]
 
 
+class Sampling(C.Structure):
+    """b200w_sampling: HOST per-row parameter arrays of b200w_infer_sample / b200w_op_sample."""
+    _fields_ = [("reserved", C.c_int32), ("temperature", vp), ("top_p", vp), ("top_k", vp), ("seed", vp),
+                ("draw", vp)]
+
+
 class HParams(C.Structure):
     _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
                 ("weight_decay", C.c_float), ("max_grad_norm", C.c_float)]
@@ -108,6 +114,7 @@ PROTOTYPES = {
     "b200w_infer_prefill_cached": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "b200w_infer_step_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp, vp]),
     "b200w_infer_prefill_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
+    "b200w_infer_sample": (C.c_int, [c_ctx, C.c_int, vp, vp, vp]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
@@ -145,6 +152,7 @@ PROTOTYPES = {
     "b200w_op_decode_attention_fp8": (C.c_int, [c_ctx, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
                                                 vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_logprobs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
+    "b200w_op_sample": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,

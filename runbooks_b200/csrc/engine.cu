@@ -1955,6 +1955,23 @@ int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int 
   if (top_k < 0 || top_k > B200W_MAX_TOP_LOGPROBS) return B200W_ERR_INVALID;
   HOOK(logprobs(logits, ld, rows, V, targets, top_k, lse, target_lp, token_lp, top_ids, top_lp, ctx->stream));
 }
+int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_sampling* sp,
+                    const float* u, int32_t* tokens_out, float* token_logit_out) {
+  return guarded(ctx, [&] {
+    check_sampling(sp, rows, V, tokens_out);
+    std::vector<uint8_t> host(sample_bytes(rows));
+    void* dev = nullptr;
+    B200W_CUDA(cudaMalloc(&dev, host.size()));
+    try {
+      sample(logits, ld, rows, V, sp, u, tokens_out, token_logit_out, host.data(), dev, rows, ctx->stream);
+    } catch (...) {
+      cudaFree(dev);
+      throw;
+    }
+    cudaFree(dev);
+    ++ctx->launches;
+  });
+}
 int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {

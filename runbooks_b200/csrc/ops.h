@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+struct b200w_sampling;   // include/b200w.h
+
 namespace b200w {
 
 // ---- gemm.cu -------------------------------------------------------------------------------
@@ -102,6 +104,14 @@ void attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void
 // to the smaller id. Every output is nullable.
 void logprobs(const void* logits, int ld, int rows, int V, const int32_t* targets, int k, float* lse,
               float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp, cudaStream_t s);
+// One sampled token per row of bf16 logits [rows, ld] (infer.cu sample_kernel; b200w.h b200w_infer_sample has the
+// definition). sp, u (nullable: Philox from seed / draw), tokens_out and token_logit_out (nullable) are HOST arrays;
+// they travel through `host` (pinned or not) and `dev`, sample_bytes(cap) bytes each, rows <= cap. check_sampling
+// throws on a bad argument; sample calls it before any GPU work and returns after the stream has drained.
+size_t sample_bytes(int cap);
+void check_sampling(const b200w_sampling* sp, int n, int V, const int32_t* tokens_out);
+void sample(const void* logits, int ld, int rows, int V, const b200w_sampling* sp, const float* u,
+            int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s);
 
 
 // ---- ops.cu --------------------------------------------------------------------------------

@@ -1,9 +1,10 @@
 """Host side of the Server decode path: `InferEngine` wraps the b200w_infer_* C ABI; `Generator`
-turns it into a continuously-batched greedy generator (one cache slot per request, one token per
-slot per step — prompt ingestion and generation are the same step)."""
+turns it into a continuously-batched generator (one cache slot per request, one token per slot per step —
+prompt ingestion and generation are the same step), greedy or sampled on the device (`InferEngine.sample`)."""
 from __future__ import annotations
 
 import ctypes as C
+import os
 from dataclasses import dataclass, field
 from typing import Dict, Iterable, List, Optional, Tuple
 
@@ -285,6 +286,25 @@ class InferEngine(Engine):
                   for i, p in enumerate(prompts)]
         return nxt, logits, lp, prompt
 
+    def sample(self, n: int, temperature, top_p, top_k, seeds, draws, want_logit: bool = False):
+        """One token per row of the logits the step / prefill call just before left on the device
+        (b200w_infer_sample; n is that call's row count): softmax(logits / temperature) cut by top_k (0: off), then
+        top_p, drawn with the uniform number Philox4x32-10 gives for (seeds[i], draws[i]). Rows with temperature <= 0
+        get the greedy token. -> (tokens, the tokens' logits as fp32 or None)."""
+        t = np.ascontiguousarray(temperature, dtype=np.float32)
+        p = np.ascontiguousarray(top_p, dtype=np.float32)
+        k = np.ascontiguousarray(top_k, dtype=np.int32)
+        sd = np.ascontiguousarray(seeds, dtype=np.uint64)
+        dr = np.ascontiguousarray(draws, dtype=np.uint64)
+        if not t.size == p.size == k.size == sd.size == dr.size == n:
+            raise ValueError("sample: one temperature, top_p, top_k, seed and draw index per row")
+        s = _lib.Sampling(0, t.ctypes.data, p.ctypes.data, k.ctypes.data, sd.ctypes.data, dr.ctypes.data)
+        tok = np.empty(n, dtype=np.int32)
+        lg = np.empty(n, dtype=np.float32) if want_logit else None
+        self._check(self._lib.b200w_infer_sample(self._h, n, C.byref(s), tok.ctypes.data,
+                                                 lg.ctypes.data if want_logit else None))
+        return tok, lg
+
 
 @dataclass
 class TokenLogprobs:
@@ -306,7 +326,7 @@ class TokenLogprobs:
 
 
 def sample_token(logits: np.ndarray, temperature: float, top_p: float, rng: np.random.Generator) -> int:
-    """Host-side sampling of one row (the engine itself is greedy): softmax(logits / T) restricted to the
+    """Host-side sampling of one row, for engines without `sample`: softmax(logits / T) restricted to the
     smallest prefix of the sorted distribution whose mass reaches top_p (nucleus sampling)."""
     z = logits.astype(np.float64) / max(temperature, 1e-6)
     z -= z.max()
@@ -332,7 +352,7 @@ class _Req:
     done: bool = False
     temperature: float = 0.0
     top_p: float = 1.0
-    rng: Optional[np.random.Generator] = None
+    rng: Optional[np.random.Generator] = None                 # host sampling only (an engine without `sample`)
     cached_tokens: int = 0                                    # prompt positions whose K/V came from the prefix index
     nodes: List["_Node"] = field(default_factory=list)        # index nodes whose page the slot holds
     entered: List["_Node"] = field(default_factory=list)      # of those, the ones this request's prefill fills
@@ -342,6 +362,9 @@ class _Req:
     prompt_logprobs: bool = False
     out_lp: List[Tuple[float, List[Tuple[int, float]]]] = field(default_factory=list)
     prompt_lp: Optional[List[Optional[Tuple[float, List[Tuple[int, float]]]]]] = None
+    # sampling on the device: draw i of the request uses the uniform number of (seed, i), i = len(out)
+    top_k: int = 0
+    seed: int = 0
 
     @property
     def greedy(self) -> bool:
@@ -387,19 +410,27 @@ class Generator:
         self._root = _Node(None, (), -1)
         self._nodes: Dict[_Node, None] = {}     # every node of the index, in insertion order
         self._tick = 0
+        self.device_sampling = hasattr(engine, "sample")   # else the logits come to the host (sample_token)
 
     def add(self, prompt: List[int], max_tokens: int, temperature: float = 0.0, top_p: float = 1.0,
             seed: Optional[int] = None, defer_prefill: bool = False, logprobs: Optional[int] = None,
-            prompt_logprobs: bool = False) -> _Req:
+            prompt_logprobs: bool = False, top_k: int = 0) -> _Req:
         """defer_prefill: only register the request; flush_prefill() then ingests every deferred prompt of the
         same padded length in ONE prefill call (what the scheduler does when several requests are admitted in
         the same round).
         logprobs (0..5): record the log-probability of every generated token and its `logprobs` top entries
         (req.out_lp); prompt_logprobs: the same for every prompt position after the first (req.prompt_lp), computed
         by the prefill. Both are the engine's raw log-softmax (temperature 1, no top_p), and a request that asks for
-        either borrows no prefix-cache pages: their hidden states are needed and were never computed."""
+        either borrows no prefix-cache pages: their hidden states are needed and were never computed.
+        top_k (0: off; at or above the vocabulary size keeps everything): sample among the top_k largest logits only,
+        before top_p; needs an engine that samples on the device. seed (None: from OS entropy): with it the
+        request's tokens are a function of its logits alone."""
         if not prompt:
             raise ValueError("empty prompt")
+        if not (isinstance(top_k, int) and top_k >= 0):
+            raise ValueError(f"top_k must be 0 (off) or a positive integer, got {top_k!r}")
+        if top_k and not self.device_sampling:
+            raise ValueError("top_k needs an engine that samples on the device")
         if logprobs is not None and not (isinstance(logprobs, int) and 0 <= logprobs <= _lib.MAX_TOP_LOGPROBS):
             raise ValueError(f"logprobs must be in 0..{_lib.MAX_TOP_LOGPROBS}, got {logprobs!r}")
         if logprobs is not None and not hasattr(self.e, "step_logprobs"):
@@ -426,8 +457,11 @@ class Generator:
                 raise CacheFull("KV cache full: too few free pages for this request now")
             self.e.reserve(self.free[-1], len(prompt) + max_tokens)
         r = _Req(list(prompt), max_tokens, [], 0, self.free.pop(), False, float(temperature), float(top_p),
-                 np.random.default_rng(seed) if temperature > 0 else None,
+                 np.random.default_rng(seed) if temperature > 0 and not self.device_sampling else None,
                  len(matched) * KV_PAGE, matched + entered, entered, logprobs, bool(prompt_logprobs))
+        if self.device_sampling and not r.greedy:
+            r.top_k = 0 if top_k >= V else top_k
+            r.seed = (int(seed) if seed is not None else int.from_bytes(os.urandom(8), "little")) % 2 ** 64
         if r.prompt_logprobs and not r.scores_prompt:
             r.prompt_lp = [None]          # one token: nothing to score
         self.active.append(r)
@@ -513,7 +547,7 @@ class Generator:
             per_call = max(1, self.e.prefill_tokens // (blocks * 128)) if self.kv_pages is not None else len(rs)
             calls += [(start, score, rs[i:i + per_call]) for i in range(0, len(rs), per_call)]
         for ci, (start, score, rs) in enumerate(calls):
-            need_logits = any(not r.greedy for r in rs)
+            need_logits = not self.device_sampling and any(not r.greedy for r in rs)
             top_k = max((r.logprobs for r in rs if r.logprobs is not None), default=None)
             lp = prompt = None
             try:
@@ -536,6 +570,7 @@ class Generator:
                 raise
             if need_logits and lg is None:
                 raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
+            drawn = self._sample(rs, [True] * len(rs))
             for i, r in enumerate(rs):
                 r.fed = len(r.prompt)
                 if score:
@@ -543,15 +578,31 @@ class Generator:
                     k = r.logprobs or 0
                     r.prompt_lp = [None] + [(float(plp[p]), list(zip(pids[p, :k].tolist(), ptop[p, :k].tolist())))
                                             for p in range(1, len(r.prompt))]
-                self._emit_token(r, i, nxt, lg, lp)
+                self._emit_token(r, i, nxt, lg, lp, drawn)
         self._retire()
 
-    def _emit_token(self, r: _Req, i: int, nxt, lg, lp: Optional[TokenLogprobs]):
-        """Emits row i's token for r: the greedy one, or one sampled from its logits; with its log-probability when
-        r asks for it (the greedy token's from the engine, a sampled one's from its logit and the row's lse)."""
-        t = int(nxt[i]) if r.greedy else sample_token(lg[i], r.temperature, r.top_p, r.rng)
+    def _sample(self, rs: List[_Req], emits: List[bool]):
+        """Right after the step / prefill call over the rows `rs`: one engine.sample call for them when a row that
+        emits a token samples (the others go as greedy rows) -> (tokens, their logits or None), or None."""
+        on = [e and not r.greedy for r, e in zip(rs, emits)]
+        if not (self.device_sampling and any(on)):
+            return None
+        return self.e.sample(len(rs), [r.temperature if s else 0.0 for r, s in zip(rs, on)], [r.top_p for r in rs],
+                             [r.top_k for r in rs], [r.seed for r in rs], [len(r.out) for r in rs],
+                             want_logit=any(s and r.logprobs is not None for r, s in zip(rs, on)))
+
+    def _emit_token(self, r: _Req, i: int, nxt, lg, lp: Optional[TokenLogprobs], drawn=None):
+        """Emits row i's token for r: the greedy one, or one sampled from its logits (`drawn`, what _sample returned,
+        or on the host from lg); with its log-probability when r asks for it (the greedy token's from the engine, a
+        sampled one's from its logit and the row's lse)."""
+        if r.greedy:
+            t = int(nxt[i])
+        elif drawn is not None:
+            t = int(drawn[0][i])
+        else:
+            t = sample_token(lg[i], r.temperature, r.top_p, r.rng)
         if r.logprobs is not None:
-            x = lp.token_lp[i] if r.greedy else np.float32(lg[i][t]) - lp.lse[i]
+            x = lp.token_lp[i] if r.greedy else (drawn[1][i] if drawn is not None else np.float32(lg[i][t])) - lp.lse[i]
             k = r.logprobs
             r.out_lp.append((float(x), list(zip(lp.top_ids[i, :k].tolist(), lp.top_lp[i, :k].tolist()))))
         self._emit(r, t)
@@ -587,7 +638,7 @@ class Generator:
         if not self.active:
             return
         toks = [(r.prompt[r.fed] if r.fed < len(r.prompt) else r.out[-1]) for r in self.active]
-        need_logits = any(not r.greedy for r in self.active)
+        need_logits = not self.device_sampling and any(not r.greedy for r in self.active)
         top_k = max((r.logprobs for r in self.active if r.logprobs is not None), default=None)
         lp = None
         if top_k is None:
@@ -598,10 +649,11 @@ class Generator:
                                                top_k, want_logits=need_logits)
         if need_logits and lg is None:
             raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
+        drawn = self._sample(self.active, [r.fed + 1 >= len(r.prompt) for r in self.active])
         for i, r in enumerate(self.active):
             r.fed += 1
             if r.fed >= len(r.prompt):        # the token just fed was the last known one
-                self._emit_token(r, i, nxt, lg, lp)
+                self._emit_token(r, i, nxt, lg, lp, drawn)
         self._retire()
 
     def generate(self, prompts: List[List[int]], max_tokens: int) -> List[List[int]]:

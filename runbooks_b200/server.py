@@ -7,8 +7,8 @@ Contract (docs/container-contract.md:50-55; server_controller.go:156-173): liste
 `GET /` answers 200 once the model in /content/model is loaded (readiness probe), and — what
 test/system.sh:73-78 and the basaran image speak — `POST /v1/completions {"prompt", "max_tokens"}`
 returns an OpenAI-style completion; `"stream": true` answers with server-sent events (one `data:` JSON
-chunk per text delta, then `data: [DONE]`), as basaran does. Accepted and honoured: temperature / top_p
-(host-side nucleus sampling over the engine's logits; default 0 = greedy), stop, n, echo, seed, a prompt of
+chunk per text delta, then `data: [DONE]`), as basaran does. Accepted and honoured: temperature / top_p /
+top_k (sampled on the GPU from the step's logits; default temperature 0 = greedy), stop, n, echo, seed, a prompt of
 token ids, and logprobs up to the server's max_logprobs (0 by default: logprobs > 0 is then a 400); anything
 else that would change the result (penalties, best_of) is a 400. Prompts are ingested in one
 prefill pass; continuous batching over the engine's cache slots (one scheduler thread owns the GPU,
@@ -50,7 +50,7 @@ class Scheduler(threading.Thread):
         self.failed: str | None = None
 
     def submit(self, prompt, max_tokens: int, temperature: float = 0.0, top_p: float = 1.0, stop=(),
-               seed=None, logprobs=None, echo: bool = False):
+               seed=None, logprobs=None, echo: bool = False, top_k: int = 0):
         """prompt: text, or token ids fed as given. logprobs (None: not asked): log-probabilities of the completion
         tokens with that many top entries, and with echo of the prompt tokens too.
         -> item (dict) or None when the admission queue is full (the caller answers 503)."""
@@ -58,7 +58,7 @@ class Scheduler(threading.Thread):
             return None
         item = {"prompt": prompt, "max_tokens": max_tokens, "temperature": temperature, "top_p": top_p,
                 "stop": tuple(stop), "seed": seed, "events": queue.Queue(), "cancelled": False,
-                "logprobs": logprobs, "echo": echo}
+                "logprobs": logprobs, "echo": echo, "top_k": top_k}
         if isinstance(prompt, list):
             item["ids"] = list(prompt)
         self.q.put(item)
@@ -186,7 +186,8 @@ class Scheduler(threading.Thread):
                         ids = item["ids"]
                         req = self.gen.add(ids, item["max_tokens"], item["temperature"], item["top_p"], item["seed"],
                                            defer_prefill=True, logprobs=item["logprobs"],
-                                           prompt_logprobs=item["echo"] and item["logprobs"] is not None)
+                                           prompt_logprobs=item["echo"] and item["logprobs"] is not None,
+                                           top_k=item["top_k"])
                         admitted.append((req, item, len(ids)))
                     except CacheFull:       # fits the pool, not now: keep its place, retry after the next step
                         held = item
@@ -266,6 +267,11 @@ def parse_completion_request(req: dict, max_logprobs: int = 0) -> dict:
     top_p = num("top_p", 1.0)
     if temperature < 0 or not 0 < top_p <= 1:
         raise ValueError("temperature must be >= 0 and top_p in (0, 1]")
+    top_k = req.get("top_k")       # absent, null, 0 or -1: off (the vLLM convention)
+    if top_k in (None, -1):
+        top_k = 0
+    if isinstance(top_k, bool) or not isinstance(top_k, int) or top_k < 0:
+        raise ValueError("top_k must be a positive integer, or 0 / -1 / null for off")
     n = int(num("n", 1))
     if n < 1 or n > 8:
         raise ValueError("n must be in 1..8")
@@ -294,7 +300,7 @@ def parse_completion_request(req: dict, max_logprobs: int = 0) -> dict:
     seed = req.get("seed")
     return dict(prompt=prompt, max_tokens=max_tokens, temperature=temperature, top_p=top_p, n=n, stop=stop,
                 stream=stream, echo=bool(req.get("echo", False)), seed=None if seed is None else int(seed),
-                logprobs=logprobs)
+                logprobs=logprobs, top_k=top_k)
 
 
 def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 600.0):
@@ -341,7 +347,7 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             for i in range(r["n"]):
                 seed = None if r["seed"] is None else r["seed"] + i
                 it = sched.submit(r["prompt"], r["max_tokens"], r["temperature"], r["top_p"], r["stop"], seed,
-                                  r["logprobs"], r["echo"])
+                                  r["logprobs"], r["echo"], r["top_k"])
                 if it is None:          # back-pressure: every slot busy and the admission queue full
                     for x in items:
                         x["cancelled"] = True
