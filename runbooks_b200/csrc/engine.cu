@@ -1930,8 +1930,14 @@ int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q
                                   const void* vcache, int64_t cache_rows, const int32_t* table, int nsplit,
                                   const int32_t* slots, const int32_t* starts, const int32_t* lengths, void* out,
                                   int ld_out, int n_seqs, int S, int H, int Hkv, int dh, float scale) {
-  HOOK(attention_fwd_cached(q, ld_q, q_head_stride, kcache, vcache, cache_rows, table, nsplit, slots, starts, lengths,
-                            out, ld_out, n_seqs, S, H, Hkv, dh, scale, ctx->stream));
+  KVLayer c;
+  c.k = const_cast<void*>(kcache);
+  c.v = const_cast<void*>(vcache);
+  c.rows = cache_rows;
+  c.table = table;
+  c.nsplit = nsplit;
+  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
+                            ctx->stream));
 }
 int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
                                       const void* vcache, const float* kscale, const float* vscale, int64_t cache_rows,
@@ -1939,8 +1945,17 @@ int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, i
                                       const int32_t* lengths, void* out, int ld_out, int n_seqs, int S, int H, int Hkv,
                                       int dh, float scale) {
   if (!kscale || !vscale) return B200W_ERR_INVALID;
-  HOOK(attention_fwd_cached(q, ld_q, q_head_stride, kcache, vcache, cache_rows, table, nsplit, slots, starts, lengths,
-                            out, ld_out, n_seqs, S, H, Hkv, dh, scale, ctx->stream, kscale, vscale));
+  KVLayer c;
+  c.k = const_cast<void*>(kcache);
+  c.v = const_cast<void*>(vcache);
+  c.kscale = const_cast<float*>(kscale);
+  c.vscale = const_cast<float*>(vscale);
+  c.rows = cache_rows;
+  c.table = table;
+  c.nsplit = nsplit;
+  c.dtype = B200W_KV_FP8_E4M3;
+  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
+                            ctx->stream));
 }
 int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
                                   const float* kscale, const float* vscale, int64_t cache_rows, const int32_t* table,

@@ -37,6 +37,7 @@
 #include "../../include/b200w.h"
 #include "ctx_access.h"
 #include "host_common.h"
+#include "kv_cache.h"
 #include "ops.h"
 #include "ptx.cuh"
 
@@ -157,105 +158,8 @@ __global__ void gelu_strided_kernel(bf16* x, int T, int N, int ld) {
   *reinterpret_cast<uint4*>(x + t * ld + c) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// KV-cache layout: a layer's cache is rows of kd elements, and the table [max_batch][nsplit] holds the first
-// cache row of each block of KV_PAGE positions of a slot, so position p of a slot lives in row
-// table[slot][p / KV_PAGE] + p % KV_PAGE. Contiguous (b200w_infer_init): [max_batch][max_ctx] rows and a table
-// fixed at init, entry j of slot s = s * max_ctx + j * KV_PAGE. Paged (b200w_infer_init_paged): a pool of pages
-// of KV_PAGE rows, entry j = KV_PAGE * (the slot's j-th page). A block is one 128-key block of the tensor-core
-// decode attention, so each block is one TMA box.
-constexpr int KV_PAGE = 128;
-// cache row of position p of the slot whose table row is `row` (a row index is below 2^31: 32-bit arithmetic)
-__device__ __forceinline__ size_t cache_row(const int32_t* __restrict__ row, unsigned p) {
-  return static_cast<unsigned>(row[p / KV_PAGE]) + p % KV_PAGE;
-}
-
-// Decode: rotate_half RoPE on the q heads (in place) and on k (rope != 0; OPT has none); k and v are
-// written into the cache at [slot][pos]. One thread per (row, head, pair index).
-__global__ void rope_append_kernel(bf16* __restrict__ qkv, int ld, const float* __restrict__ inv_freq,
-                                   const int32_t* __restrict__ pos, const int32_t* __restrict__ slot,
-                                   bf16* __restrict__ kcache, bf16* __restrict__ vcache, int n, int H,
-                                   int Hkv, int dh, int rope, const int32_t* __restrict__ table, int nsplit) {
-  pdl_trigger();
-  pdl_wait();
-  const int half = dh / 2;
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long total = static_cast<long long>(n) * (H + Hkv) * half;
-  if (idx >= total) return;
-  const int i = static_cast<int>(idx % half);
-  const int h = static_cast<int>((idx / half) % (H + Hkv));
-  const int r = static_cast<int>(idx / (static_cast<long long>(half) * (H + Hkv)));
-  const int p = pos[r];
-  float sn = 0.f, cs = 1.f;
-  if (rope) sincosf(static_cast<float>(p) * inv_freq[i], &sn, &cs);
-  bf16* src = qkv + static_cast<size_t>(r) * ld + h * dh;
-  const float x1 = __bfloat162float(src[i]), x2 = __bfloat162float(src[i + half]);
-  const bf16 o1 = rope ? __float2bfloat16_rn(x1 * cs - x2 * sn) : src[i];
-  const bf16 o2 = rope ? __float2bfloat16_rn(x2 * cs + x1 * sn) : src[i + half];
-  if (h < H) {
-    if (rope) {
-      src[i] = o1;
-      src[i + half] = o2;
-    }
-  } else {
-    const int hk = h - H;
-    const size_t off = (cache_row(table + slot[r] * nsplit, p) * Hkv + hk) * dh;
-    kcache[off + i] = o1;
-    kcache[off + i + half] = o2;
-    const bf16* vsrc = qkv + static_cast<size_t>(r) * ld + (H + Hkv + hk) * dh;
-    vcache[off + i] = vsrc[i];
-    vcache[off + i + half] = vsrc[i + half];
-  }
-}
-
-// Prefill: token t = b * S + p of sequence b, at position p + start[b] (start == nullptr: p). q / k (rotated when
-// rope != 0) and v go to the attention input `dst` [T, (H + 2 Hkv) * dhp] (heads at stride dhp >= dh; the padding
-// columns are zero from allocation and never written) and, for real positions < len[b], k / v also into cache
-// slot[b].
-__global__ void prefill_rope_scatter_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
-                                            int ld_dst, const float* __restrict__ inv_freq,
-                                            const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
-                                            bf16* __restrict__ kcache, bf16* __restrict__ vcache, int T, int S,
-                                            int H, int Hkv, int dh, int dhp, int rope,
-                                            const int32_t* __restrict__ table, int nsplit,
-                                            const int32_t* __restrict__ start) {
-  const int half = dh / 2, HT = H + 2 * Hkv;
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long total = static_cast<long long>(T) * HT * half;
-  if (idx >= total) return;
-  const int i = static_cast<int>(idx % half);
-  const int h = static_cast<int>((idx / half) % HT);
-  const int t = static_cast<int>(idx / (static_cast<long long>(half) * HT));
-  const int b = t / S, p = t % S + (start ? start[b] : 0);
-  const bf16* x = src + static_cast<size_t>(t) * ld_src + h * dh;
-  const float x1 = __bfloat162float(x[i]), x2 = __bfloat162float(x[i + half]);
-  bf16 o1 = x[i], o2 = x[i + half];
-  if (rope && h < H + Hkv) {
-    float sn, cs;
-    sincosf(static_cast<float>(p) * inv_freq[i], &sn, &cs);
-    o1 = __float2bfloat16_rn(x1 * cs - x2 * sn);
-    o2 = __float2bfloat16_rn(x2 * cs + x1 * sn);
-  }
-  bf16* y = dst + static_cast<size_t>(t) * ld_dst + h * dhp;
-  y[i] = o1;
-  y[i + half] = o2;
-  if (h >= H && p < lens[b]) {
-    const bool is_k = h < H + Hkv;
-    const int hk = is_k ? h - H : h - H - Hkv;
-    const size_t off = (cache_row(table + slot[b] * nsplit, p) * Hkv + hk) * dh;
-    bf16* c = is_k ? kcache : vcache;
-    c[off + i] = o1;
-    c[off + i + half] = o2;
-  }
-}
-
-// ---- the fp8 (e4m3) pool (b200w_infer_init_paged_kv, DESIGN §3.5) ----
-// A layer's K and V are e4m3 bytes [rows, kd] with one fp32 scale per (row, kv head) in [rows, Hkv]. A head's dh
-// values x (rotated and rounded to bf16, what the bf16 pool would store) are stored as q = e4m3_rn_satfinite(x /
-// scale), scale = amax|x| / 448, both divisions IEEE; amax = 0 stores scale 0 and q = 0. Every e4m3 value is exact
-// in bf16, and the readers apply the scales in fp32.
-__device__ __forceinline__ uint8_t e4m3_rn(float x) {
-  return static_cast<uint8_t>(__nv_cvt_float_to_fp8(x, __NV_SATFINITE, __NV_E4M3));
-}
+// e4m3 pool readers (DESIGN §3.5): the bytes are exact in bf16, and the scales are applied in fp32
+using fp8 = __nv_fp8_e4m3;
 // two e4m3 bytes (low byte first) -> two floats, exact
 __device__ __forceinline__ float2 e4m3x2_to_float2(uint32_t two) {
   const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two), __NV_E4M3);
@@ -270,120 +174,6 @@ __device__ __forceinline__ void e4m3x8_to_bf16(uint2 u, uint32_t* w) {
     w[j] = pack_bf16x2(f.x, f.y);
   }
 }
-// One warp stores one head: lane l holds the pairs (x[i], x[i + dh / 2]) of i = l + 32 j, j < np (entries with
-// i >= dh / 2 hold 0 and are not stored).
-__device__ __forceinline__ void quant_head_warp(const float (&lo)[2], const float (&hi)[2], int half,
-                                                uint8_t* __restrict__ dst, float* __restrict__ scale_dst) {
-  const int lane = threadIdx.x & 31;
-  float amax = 0.f;
-#pragma unroll
-  for (int j = 0; j < 2; ++j) amax = fmaxf(amax, fmaxf(fabsf(lo[j]), fabsf(hi[j])));
-  amax = warp_max_f(amax);
-  const float scale = __fdiv_rn(amax, 448.f);
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int i = lane + 32 * j;
-    if (i < half) {
-      dst[i] = amax > 0.f ? e4m3_rn(__fdiv_rn(lo[j], scale)) : 0;
-      dst[i + half] = amax > 0.f ? e4m3_rn(__fdiv_rn(hi[j], scale)) : 0;
-    }
-  }
-  if (lane == 0) *scale_dst = scale;
-}
-// lo / hi of quant_head_warp from a bf16 head at x
-__device__ __forceinline__ void load_head_pairs(const bf16* __restrict__ x, int half, float (&lo)[2], float (&hi)[2]) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int i = lane + 32 * j;
-    lo[j] = i < half ? __bfloat162float(x[i]) : 0.f;
-    hi[j] = i < half ? __bfloat162float(x[i + half]) : 0.f;
-  }
-}
-// rotate_half RoPE of the pairs at position p, rounded to bf16 as the bf16 pool stores them
-__device__ __forceinline__ void rope_pairs(const float* __restrict__ inv_freq, int p, int half, float (&lo)[2],
-                                           float (&hi)[2]) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int i = lane + 32 * j;
-    if (i < half) {
-      float sn, cs;
-      sincosf(static_cast<float>(p) * inv_freq[i], &sn, &cs);
-      const float x1 = lo[j], x2 = hi[j];
-      lo[j] = __bfloat162float(__float2bfloat16_rn(x1 * cs - x2 * sn));
-      hi[j] = __bfloat162float(__float2bfloat16_rn(x2 * cs + x1 * sn));
-    }
-  }
-}
-__device__ __forceinline__ void store_head_pairs(bf16* __restrict__ y, int half, const float (&lo)[2],
-                                                 const float (&hi)[2]) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int i = lane + 32 * j;
-    if (i < half) {
-      y[i] = __float2bfloat16_rn(lo[j]);
-      y[i + half] = __float2bfloat16_rn(hi[j]);
-    }
-  }
-}
-
-// rope_append_kernel for the fp8 pool: one warp per (row, head), the scale being a reduction over the head
-__global__ void rope_append_fp8_kernel(bf16* __restrict__ qkv, int ld, const float* __restrict__ inv_freq,
-                                       const int32_t* __restrict__ pos, const int32_t* __restrict__ slot,
-                                       uint8_t* __restrict__ kcache, uint8_t* __restrict__ vcache,
-                                       float* __restrict__ kscale, float* __restrict__ vscale, int n, int H, int Hkv,
-                                       int dh, int rope, const int32_t* __restrict__ table, int nsplit) {
-  pdl_trigger();
-  pdl_wait();
-  const int half = dh / 2;
-  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-  if (w >= static_cast<long long>(n) * (H + Hkv)) return;   // warp-uniform
-  const int h = static_cast<int>(w % (H + Hkv)), r = static_cast<int>(w / (H + Hkv));
-  const int p = pos[r];
-  bf16* src = qkv + static_cast<size_t>(r) * ld + h * dh;
-  float lo[2], hi[2];
-  load_head_pairs(src, half, lo, hi);
-  if (rope) rope_pairs(inv_freq, p, half, lo, hi);
-  if (h < H) {
-    if (rope) store_head_pairs(src, half, lo, hi);
-    return;
-  }
-  const int hk = h - H;
-  const size_t row = cache_row(table + slot[r] * nsplit, p);
-  quant_head_warp(lo, hi, half, kcache + (row * Hkv + hk) * dh, kscale + row * Hkv + hk);
-  load_head_pairs(qkv + static_cast<size_t>(r) * ld + (H + Hkv + hk) * dh, half, lo, hi);
-  quant_head_warp(lo, hi, half, vcache + (row * Hkv + hk) * dh, vscale + row * Hkv + hk);
-}
-
-// prefill_rope_scatter_kernel for the fp8 pool: one warp per (token, head)
-__global__ void prefill_rope_scatter_fp8_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst,
-                                                int ld_dst, const float* __restrict__ inv_freq,
-                                                const int32_t* __restrict__ lens, const int32_t* __restrict__ slot,
-                                                uint8_t* __restrict__ kcache, uint8_t* __restrict__ vcache,
-                                                float* __restrict__ kscale, float* __restrict__ vscale, int T, int S,
-                                                int H, int Hkv, int dh, int dhp, int rope,
-                                                const int32_t* __restrict__ table, int nsplit,
-                                                const int32_t* __restrict__ start) {
-  const int half = dh / 2, HT = H + 2 * Hkv;
-  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-  if (w >= static_cast<long long>(T) * HT) return;   // warp-uniform
-  const int h = static_cast<int>(w % HT), t = static_cast<int>(w / HT);
-  const int b = t / S, p = t % S + (start ? start[b] : 0);
-  float lo[2], hi[2];
-  load_head_pairs(src + static_cast<size_t>(t) * ld_src + h * dh, half, lo, hi);
-  if (rope && h < H + Hkv) rope_pairs(inv_freq, p, half, lo, hi);
-  store_head_pairs(dst + static_cast<size_t>(t) * ld_dst + h * dhp, half, lo, hi);
-  if (h >= H && p < lens[b]) {
-    const bool is_k = h < H + Hkv;
-    const int hk = is_k ? h - H : h - H - Hkv;
-    const size_t row = cache_row(table + slot[b] * nsplit, p);
-    quant_head_warp(lo, hi, half, (is_k ? kcache : vcache) + (row * Hkv + hk) * dh,
-                    (is_k ? kscale : vscale) + row * Hkv + hk);
-  }
-}
-
 // dst[t, h*dh + c] = src[t, h*dhp + c] for c < dh: drops the head padding after the prefill attention
 __global__ void unpad_heads_kernel(const bf16* __restrict__ src, int ld_src, bf16* __restrict__ dst, int ld_dst,
                                    int T, int H, int dh, int dhp) {
@@ -408,19 +198,35 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* 
 
 // Attention of one new query token per row over its slot's cache [0, pos]. Block = (row, kv head,
 // group of GT query heads that share that kv head): every K/V row is read once per block.
-// decode_attn_fp8_kernel (below) is the same kernel over the e4m3 pool: 8 bytes per 8 dims, a key's K scale
-// (kscale [rows, Hkv]) multiplies its score and its V scale its probability in P V, the row sum running over the
-// unscaled probabilities. It is a copy rather than a second instance of one template body: sharing the body changed
-// the code ptxas makes for the bf16 kernel.
-using fp8 = __nv_fp8_e4m3;
+// KV = fp8 reads the e4m3 pool: 8 bytes per 8 dims, a key's K scale (kscale [rows, Hkv]) multiplies its score and
+// its V scale its probability in P V, the row sum running over the unscaled probabilities (bf16: kscale / vscale
+// are not read).
 constexpr int ATT_GT = 8;
 constexpr int ATT_THREADS = 256;
-template <int DH>
+// 8 consecutive dims of a K or V row: 16 bytes of bf16 or 8 of e4m3
+template <typename KV>
+using Dims8 = typename std::conditional<std::is_same<KV, fp8>::value, uint2, uint4>::type;
+// dims 2 j and 2 j + 1 of the 8
+template <typename KV>
+__device__ __forceinline__ float2 dims8_pair(Dims8<KV> u, int j) {
+  if constexpr (std::is_same<KV, fp8>::value) return e4m3x2_to_float2((j < 2 ? u.x : u.y) >> (16 * (j % 2)));
+  else return unpack_bf16x2(j == 0 ? u.x : j == 1 ? u.y : j == 2 ? u.z : u.w);
+}
+// a key's K or V scale (e4m3; bf16 has none: 1)
+template <typename KV>
+__device__ __forceinline__ float row_scale(const float* __restrict__ scale, size_t row) {
+  if constexpr (std::is_same<KV, fp8>::value) return scale[row];
+  else return 1.f;
+}
+
+template <int DH, typename KV>
 __global__ void __launch_bounds__(ATT_THREADS)
-decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache,
-                   const bf16* __restrict__ vcache, const int32_t* __restrict__ pos,
+decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ kcache,
+                   const KV* __restrict__ vcache, const int32_t* __restrict__ pos,
                    const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
-                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit) {
+                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
+                   const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
   extern __shared__ float sm[];
   pdl_trigger();
   pdl_wait();
@@ -440,28 +246,33 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
   const int32_t* prow = table + slot[r] * nsplit;   // the slot's table row
   // scores: one key position per thread, the K row lives in registers for all ng heads
   for (int t = tid; t < len; t += ATT_THREADS) {
-    const uint4* krow = reinterpret_cast<const uint4*>(kcache + (cache_row(prow, t) * Hkv + hk) * DH);
+    const size_t row = cache_row(prow, t) * Hkv + hk;
+    const Dims8<KV>* krow = reinterpret_cast<const Dims8<KV>*>(kcache + row * DH);
     float acc[ATT_GT];
 #pragma unroll
     for (int g = 0; g < ATT_GT; ++g) acc[g] = 0.f;
 #pragma unroll
     for (int c8 = 0; c8 < DH / 8; ++c8) {
-      const uint4 u = krow[c8];
-      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+      const Dims8<KV> u = krow[c8];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float2 kf = unpack_bf16x2(w[j]);
+        const float2 kf = dims8_pair<KV>(u, j);
 #pragma unroll
         for (int g = 0; g < ATT_GT; ++g)
           acc[g] += kf.x * sq[g * DH + c8 * 8 + 2 * j] + kf.y * sq[g * DH + c8 * 8 + 2 * j + 1];
       }
+    }
+    if constexpr (F8) {
+      const float ks = row_scale<KV>(kscale, row);
+#pragma unroll
+      for (int g = 0; g < ATT_GT; ++g) acc[g] *= ks;
     }
 #pragma unroll
     for (int g = 0; g < ATT_GT; ++g)
       if (g < ng) sc[g * sc_stride + t] = acc[g];
   }
   __syncthreads();
-  // softmax per head
+  // softmax per head (the V scale joins in P V, once per key for all heads)
   float inv_sum[ATT_GT];
   for (int g = 0; g < ng; ++g) {
     float m = -INFINITY;
@@ -476,9 +287,9 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
     inv_sum[g] = 1.f / block_reduce(s, red, false);
   }
   __syncthreads();
-  // output: thread = (8 dims via one 16-byte load, position slice); 4 independent positions in
+  // output: thread = (8 dims via one load, position slice); 4 independent positions in
   // flight per thread; V read once for all ng heads
-  constexpr int DG = DH / 8;                 // 16-byte groups per row
+  constexpr int DG = DH / 8;                 // 8-dim groups per row
   constexpr int SLICES = ATT_THREADS / DG;   // 32 (dh 64) or 16 (dh 128) position slices
   const int dg = tid % DG, sl = tid / DG;
   float o[ATT_GT][8];
@@ -487,136 +298,14 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict_
 #pragma unroll
     for (int e = 0; e < 8; ++e) o[g][e] = 0.f;
   for (int t0 = sl; t0 < len; t0 += 4 * SLICES) {
-    uint4 vv[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int t = t0 + u * SLICES;
-      vv[u] = t < len ? *reinterpret_cast<const uint4*>(vcache + (cache_row(prow, t) * Hkv + hk) * DH + dg * 8)
-                      : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int t = t0 + u * SLICES;
-      if (t < len) {
-        const uint32_t w[4] = {vv[u].x, vv[u].y, vv[u].z, vv[u].w};
-        float vf[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = unpack_bf16x2(w[j]);
-          vf[2 * j] = f.x;
-          vf[2 * j + 1] = f.y;
-        }
-#pragma unroll
-        for (int g = 0; g < ATT_GT; ++g) {
-          const float p = sc[g * sc_stride + t];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o[g][e] += p * vf[e];
-        }
-      }
-    }
-  }
-  __syncthreads();  // scores are dead: reuse their space to combine the slices
-  float* so = sc;   // [SLICES][ATT_GT][DH]  (sc_stride >= SLICES * DH / ... checked on the host)
-#pragma unroll
-  for (int g = 0; g < ATT_GT; ++g)
-    if (g < ng) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) so[(sl * ATT_GT + g) * DH + dg * 8 + e] = o[g][e];
-    }
-  __syncthreads();
-  for (int i = tid; i < ng * DH; i += ATT_THREADS) {
-    const int g = i / DH, dim = i % DH;
-    float a = 0.f;
-    for (int s2 = 0; s2 < SLICES; ++s2) a += so[(s2 * ATT_GT + g) * DH + dim];
-    out[static_cast<size_t>(r) * ldo + (hk * G + g0 + g) * DH + dim] = __float2bfloat16_rn(a * inv_sum[g]);
-  }
-}
-
-
-template <int DH>
-__global__ void __launch_bounds__(ATT_THREADS)
-decode_attn_fp8_kernel(const bf16* __restrict__ qkv, int ld, const fp8* __restrict__ kcache,
-                   const fp8* __restrict__ vcache, const int32_t* __restrict__ pos,
-                   const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
-                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
-                   const float* __restrict__ kscale, const float* __restrict__ vscale) {
-  extern __shared__ float sm[];
-  pdl_trigger();
-  pdl_wait();
-  const int r = blockIdx.x, hk = blockIdx.y, G = H / Hkv;
-  const int g0 = blockIdx.z * ATT_GT;
-  const int ng = min(ATT_GT, G - g0);
-  const int len = pos[r] + 1;
-  float* sq = sm;                       // [ATT_GT][DH]
-  float* sc = sq + ATT_GT * DH;         // [ATT_GT][sc_stride]; reused to combine output slices
-  float* red = sc + ATT_GT * sc_stride; // [32]
-  const int tid = threadIdx.x;
-  for (int i = tid; i < ng * DH; i += ATT_THREADS) {
-    const int g = i / DH, c = i % DH;
-    sq[g * DH + c] = __bfloat162float(qkv[static_cast<size_t>(r) * ld + (hk * G + g0 + g) * DH + c]) * scale;
-  }
-  __syncthreads();
-  const int32_t* prow = table + slot[r] * nsplit;   // the slot's table row
-  // scores: one key position per thread, the K row lives in registers for all ng heads
-  for (int t = tid; t < len; t += ATT_THREADS) {
-    float acc[ATT_GT];
-#pragma unroll
-    for (int g = 0; g < ATT_GT; ++g) acc[g] = 0.f;
-    const size_t row = cache_row(prow, t) * Hkv + hk;
-    const uint2* krow = reinterpret_cast<const uint2*>(kcache + row * DH);
-#pragma unroll
-    for (int c8 = 0; c8 < DH / 8; ++c8) {   // 8 bytes per 8 dims
-      const uint2 u = krow[c8];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 kf = e4m3x2_to_float2((j < 2 ? u.x : u.y) >> (16 * (j % 2)));
-#pragma unroll
-        for (int g = 0; g < ATT_GT; ++g)
-          acc[g] += kf.x * sq[g * DH + c8 * 8 + 2 * j] + kf.y * sq[g * DH + c8 * 8 + 2 * j + 1];
-      }
-    }
-    const float ks = kscale[row];
-#pragma unroll
-    for (int g = 0; g < ATT_GT; ++g) acc[g] *= ks;
-#pragma unroll
-    for (int g = 0; g < ATT_GT; ++g)
-      if (g < ng) sc[g * sc_stride + t] = acc[g];
-  }
-  __syncthreads();
-  // softmax per head
-  float inv_sum[ATT_GT];
-  for (int g = 0; g < ng; ++g) {
-    float m = -INFINITY;
-    for (int t = tid; t < len; t += ATT_THREADS) m = fmaxf(m, sc[g * sc_stride + t]);
-    m = block_reduce(m, red, true);
-    float s = 0.f;
-    for (int t = tid; t < len; t += ATT_THREADS) {
-      const float e = __expf(sc[g * sc_stride + t] - m);
-      sc[g * sc_stride + t] = e;   // the V scale joins in P V, once per key for all heads
-      s += e;
-    }
-    inv_sum[g] = 1.f / block_reduce(s, red, false);
-  }
-  __syncthreads();
-  // output: thread = (8 dims via one 16-byte load, position slice); 4 independent positions in
-  // flight per thread; V read once for all ng heads
-  constexpr int DG = DH / 8;                 // 16-byte groups per row
-  constexpr int SLICES = ATT_THREADS / DG;   // 32 (dh 64) or 16 (dh 128) position slices
-  const int dg = tid % DG, sl = tid / DG;
-  float o[ATT_GT][8];
-#pragma unroll
-  for (int g = 0; g < ATT_GT; ++g)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o[g][e] = 0.f;
-  for (int t0 = sl; t0 < len; t0 += 4 * SLICES) {
-    uint2 vv[4];   // 8 bytes per 8 dims
+    Dims8<KV> vv[4];
     float vsc[4];  // their V scales
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int t = t0 + u * SLICES;
-      const size_t row = t < len ? cache_row(prow, t) * Hkv + hk : 0;
-      vv[u] = t < len ? *reinterpret_cast<const uint2*>(vcache + row * DH + dg * 8) : make_uint2(0, 0);
-      vsc[u] = t < len ? vscale[row] : 0.f;
+      vv[u] = t < len ? *reinterpret_cast<const Dims8<KV>*>(vcache + (cache_row(prow, t) * Hkv + hk) * DH + dg * 8)
+                      : Dims8<KV>{};
+      vsc[u] = t < len ? row_scale<KV>(vscale, cache_row(prow, t) * Hkv + hk) : 0.f;
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -625,13 +314,14 @@ decode_attn_fp8_kernel(const bf16* __restrict__ qkv, int ld, const fp8* __restri
         float vf[8];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 f = e4m3x2_to_float2((j < 2 ? vv[u].x : vv[u].y) >> (16 * (j % 2)));
+          const float2 f = dims8_pair<KV>(vv[u], j);
           vf[2 * j] = f.x;
           vf[2 * j + 1] = f.y;
         }
 #pragma unroll
         for (int g = 0; g < ATT_GT; ++g) {
-          const float p = sc[g * sc_stride + t] * vsc[u];
+          float p = sc[g * sc_stride + t];
+          if constexpr (F8) p *= vsc[u];
 #pragma unroll
           for (int e = 0; e < 8; ++e) o[g][e] += p * vf[e];
         }
@@ -1747,44 +1437,13 @@ struct Infer {
   // decode activations [max_batch, *]
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
-  bf16 *kc = nullptr, *vc = nullptr;  // [L][layer_rows()][Hkv*dh], zero-initialised
-  // B200W_KV_FP8_E4M3 (paged only): kc / vc are null, K and V are e4m3 bytes [L][layer_rows()][Hkv*dh] with fp32
-  // scales [L][layer_rows()][Hkv] (DESIGN §3.5), all zero-initialised
-  int kv_dtype = B200W_KV_BF16;
-  uint8_t *kq = nullptr, *vq = nullptr;
-  float *ks = nullptr, *vs = nullptr;
-  bool fp8() const { return kv_dtype == B200W_KV_FP8_E4M3; }
-  // layer l's K / V pools and scales: {k, v, k scales, v scales} (scales null for bf16)
-  struct KVLayer { void *k, *v; float *ks, *vs; };
-  KVLayer kv_layer(int l) const {
-    const size_t rows = layer_rows();
-    if (!fp8()) return {kc + l * rows * kd, vc + l * rows * kd, nullptr, nullptr};
-    const size_t n = rows * a.num_kv_heads;
-    return {kq + l * rows * kd, vq + l * rows * kd, ks + l * n, vs + l * n};
-  }
-  // the table [max_batch][nsplit] of first cache rows (KV_PAGE above) on the device, written from pinned staging:
-  // once at init when contiguous, by b200w_infer_reserve when paged (n_pages > 0). Paged: `held` mirrors it on the
-  // host (the pages a slot owns, in table order), `free_pages` is a LIFO stack of the others
-  int n_pages = 0;
-  int32_t* table = nullptr;
-  int32_t* table_pin = nullptr;
-  std::vector<int32_t> free_pages;
-  std::vector<std::vector<int32_t>> held;
-  // paged: references of each page (one per table entry of a slot that holds it, plus the host index's, which
-  // index_refs counts; `retained` is their sum); a page is on the free list iff refs == 0. floor[slot]: the first
-  // position the slot may write, n_shared * KV_PAGE (b200w_infer_reserve_shared)
-  std::vector<int32_t> refs, index_refs, floor;
-  int64_t retained = 0;
+  KVCache kv;
   size_t pf_limit = 0;  // paged: tokens of the preallocated prefill workspace, the most one prefill call takes
-  size_t layer_rows() const {
-    return n_pages ? static_cast<size_t>(n_pages) * KV_PAGE : static_cast<size_t>(max_batch) * a.max_ctx;
-  }
   float* inv_freq = nullptr;
   float* ws = nullptr;          // split-K workspace [max_batch, max N] (kept zeroed)
   unsigned* counters = nullptr;
   float* part_o = nullptr;      // tensor-core decode attention partials [max_batch, H, nsplit, dh]
   float2* part_ml = nullptr;    // [max_batch, H, nsplit] (max, sum)
-  int nsplit = 0;
   int32_t *tok = nullptr, *pos = nullptr, *slot = nullptr, *next = nullptr;
   int32_t* pin = nullptr;  // pinned host staging: tok | pos | slot | next, max_batch each
   std::unordered_map<int, cudaGraphExec_t> graphs;  // whole decode step per row count
@@ -1838,7 +1497,6 @@ struct Infer {
     if (pin) cudaFreeHost(pin);
     if (pf_pin) cudaFreeHost(pf_pin);
     if (sp_pin) cudaFreeHost(sp_pin);
-    if (table_pin) cudaFreeHost(table_pin);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -2006,91 +1664,66 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
 
 // the tensor-core decode attention and the merge of its blocks -> out [n, ldo]
 template <int DH, typename KV>
-void decode_attention_tc(Infer* m, cudaStream_t s, int n, const CUtensorMap& tk, const CUtensorMap& tv,
-                         float scale_log2, bf16* out, int ldo, const float* kscale, const float* vscale) {
-  const int H = m->a.num_heads, Hkv = m->a.num_kv_heads;
-  const int smem = tc_smem_bytes<DH>() + (std::is_same<KV, fp8>::value ? TC_SCALE_BYTES : 0);
+void decode_attention_tc(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n,
+                         int H, int Hkv, float scale_log2, float* part_o, float2* part_ml, bf16* out, int ldo,
+                         cudaStream_t s) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
+  const int smem = tc_smem_bytes<DH>() + (F8 ? TC_SCALE_BYTES : 0);
+  const KVTmaps tm = kv_tmaps(c, Hkv, DH);
   static PerDeviceOnce once;
-  if constexpr (std::is_same<KV, fp8>::value) {
+  if constexpr (F8) {
     once.run([&] {
       B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_fp8_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     });
-    launch_pdl(decode_attn_tc_fp8_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tk, tv, m->qkv,
-               m->qkvd, m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table, kscale, vscale);
+    launch_pdl(decode_attn_tc_fp8_kernel<DH>, dim3(c.nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tm.k, tm.v, q, ld_q,
+               pos, slot, part_o, part_ml, H, Hkv, c.nsplit, scale_log2, c.table, c.kscale, c.vscale);
   } else {
     once.run([&] {
       B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     });
-    launch_pdl(decode_attn_tc_kernel<DH>, dim3(m->nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tk, tv, m->qkv, m->qkvd,
-               m->pos, m->slot, m->part_o, m->part_ml, H, Hkv, m->nsplit, scale_log2, m->table);
+    launch_pdl(decode_attn_tc_kernel<DH>, dim3(c.nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tm.k, tm.v, q, ld_q, pos,
+               slot, part_o, part_ml, H, Hkv, c.nsplit, scale_log2, c.table);
   }
-  launch_pdl(decode_attn_merge_kernel<DH>, dim3(cdiv(H, 256 / DH), n), dim3(256), 0, s, m->part_o, m->part_ml, m->pos,
-             out, ldo, H, m->nsplit);
+  launch_pdl(decode_attn_merge_kernel<DH>, dim3(cdiv(H, 256 / DH), n), dim3(256), 0, s, part_o, part_ml, pos, out, ldo,
+             H, c.nsplit);
 }
 
-// attention of the n new tokens over their cache slots -> out [n, ldo]
-void decode_attention(Infer* m, cudaStream_t s, int n, int layer, bf16* out, int ldo, int64_t& nl) {
-  const auto& a = m->a;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, G = H / Hkv;
-  const float scale = 1.f / sqrtf(static_cast<float>(dh));
-  const uint64_t rows = m->layer_rows();
-  const Infer::KVLayer c = m->kv_layer(layer);
-  if (G >= 4) {
-    // grouped / multi-query: the group is the M dimension of a tensor-core tile
-    const float scale_log2 = scale * 1.4426950408889634f;
-    if (m->fp8()) {   // one unswizzled [128 keys x dh] byte box each
-      CUtensorMap tk = make_tmap_u8_2d(c.k, rows, m->kd, m->kd, TC_KB, dh);
-      CUtensorMap tv = make_tmap_u8_2d(c.v, rows, m->kd, m->kd, TC_KB, dh);
-      if (dh == 64) decode_attention_tc<64, fp8>(m, s, n, tk, tv, scale_log2, out, ldo, c.ks, c.vs);
-      else decode_attention_tc<128, fp8>(m, s, n, tk, tv, scale_log2, out, ldo, c.ks, c.vs);
-    } else {
-      CUtensorMap tk = make_tmap_bf16_2d(c.k, rows, m->kd, m->kd, TC_KB, 64);
-      CUtensorMap tv = make_tmap_bf16_2d(c.v, rows, m->kd, m->kd, TC_KB, 64);
-      if (dh == 64) decode_attention_tc<64, bf16>(m, s, n, tk, tv, scale_log2, out, ldo, nullptr, nullptr);
-      else decode_attention_tc<128, bf16>(m, s, n, tk, tv, scale_log2, out, ldo, nullptr, nullptr);
-    }
-    nl += 2;
-    return;
-  }
-  const dim3 agrid(n, Hkv, (G + ATT_GT - 1) / ATT_GT);
-  const int slices = ATT_THREADS / (dh / 8);   // staging area: slices * ATT_GT * dh floats
-  const int sc_stride = std::max(a.max_ctx, slices * dh);
-  const size_t att_smem = (static_cast<size_t>(ATT_GT) * dh + static_cast<size_t>(ATT_GT) * sc_stride + 32) * 4;
+// the CUDA-core decode attention -> out [n, ldo]
+template <int DH, typename KV>
+void decode_attention_cc(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n,
+                         int H, int Hkv, int max_ctx, bf16* out, int ldo, cudaStream_t s) {
+  const int slices = ATT_THREADS / (DH / 8);   // staging area: slices * ATT_GT * dh floats
+  const int sc_stride = std::max(max_ctx, slices * DH);
+  const size_t att_smem = (static_cast<size_t>(ATT_GT) * DH + static_cast<size_t>(ATT_GT) * sc_stride + 32) * 4;
   B200W_CHECK(att_smem <= 200 * 1024, "max_ctx too large for the decode attention kernel");
   static PerDeviceOnce once;
   once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_fp8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_fp8_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<DH, KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   });
-  if (m->fp8())
-    launch_pdl(dh == 64 ? decode_attn_fp8_kernel<64> : decode_attn_fp8_kernel<128>, agrid, dim3(ATT_THREADS), att_smem,
-               s, m->qkv, m->qkvd, static_cast<const fp8*>(c.k), static_cast<const fp8*>(c.v), m->pos, m->slot, out,
-               ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit, static_cast<const float*>(c.ks),
-               static_cast<const float*>(c.vs));
-  else
-    launch_pdl(dh == 64 ? decode_attn_kernel<64> : decode_attn_kernel<128>, agrid, dim3(ATT_THREADS), att_smem, s,
-               m->qkv, m->qkvd, static_cast<const bf16*>(c.k), static_cast<const bf16*>(c.v), m->pos, m->slot, out,
-               ldo, H, Hkv, sc_stride, scale, m->table, m->nsplit);
-  ++nl;
+  launch_pdl(decode_attn_kernel<DH, KV>, dim3(n, Hkv, (H / Hkv + ATT_GT - 1) / ATT_GT), dim3(ATT_THREADS), att_smem, s,
+             q, ld_q, static_cast<const KV*>(c.k), static_cast<const KV*>(c.v), pos, slot, out, ldo, H, Hkv, sc_stride,
+             1.f / sqrtf(static_cast<float>(DH)), c.table, c.nsplit, static_cast<const float*>(c.kscale),
+             static_cast<const float*>(c.vscale));
 }
 
-// the K/V append of a decode step: rotate q and k (rope != 0), k and v into the slot's cache rows
-void append_kv(Infer* m, cudaStream_t s, int n, int layer, int rope, int64_t& nl) {
-  const auto& a = m->a;
-  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
-  const Infer::KVLayer c = m->kv_layer(layer);
-  if (m->fp8()) {   // a warp per (row, head)
-    launch_pdl(rope_append_fp8_kernel, dim3(cdiv(static_cast<long long>(n) * (H + Hkv) * 32, 256)), dim3(256), 0, s,
-               m->qkv, m->qkvd, m->inv_freq, m->pos, m->slot, static_cast<uint8_t*>(c.k), static_cast<uint8_t*>(c.v),
-               c.ks, c.vs, n, H, Hkv, dh, rope, m->table, m->nsplit);
-  } else {
-    const long long rp = static_cast<long long>(n) * (H + Hkv) * (dh / 2);
-    launch_pdl(rope_append_kernel, dim3(cdiv(rp, 256)), dim3(256), 0, s, m->qkv, m->qkvd, m->inv_freq, m->pos, m->slot,
-               static_cast<bf16*>(c.k), static_cast<bf16*>(c.v), n, H, Hkv, dh, rope, m->table, m->nsplit);
+// Attention of the n new tokens (queries q [n, ld_q], head h at column h * dh; pos / slot DEVICE [n]) over their cache
+// slots -> out [n, ldo]: on the tensor cores when H / Hkv >= 4 (partials part_o [n, H, nsplit, dh] and part_ml
+// [n, H, nsplit]), else on the CUDA cores (max_ctx sizes the score staging). Returns the launches.
+int decode_attention(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n, int H,
+                     int Hkv, int dh, int max_ctx, float* part_o, float2* part_ml, bf16* out, int ldo, cudaStream_t s) {
+  const bool f8 = c.dtype == B200W_KV_FP8_E4M3;
+  if (H / Hkv >= 4) {
+    // grouped / multi-query: the group is the M dimension of a tensor-core tile
+    const float scale_log2 = 1.f / sqrtf(static_cast<float>(dh)) * 1.4426950408889634f;
+    auto tc = dh == 64 ? (f8 ? decode_attention_tc<64, fp8> : decode_attention_tc<64, bf16>)
+                       : (f8 ? decode_attention_tc<128, fp8> : decode_attention_tc<128, bf16>);
+    tc(c, q, ld_q, pos, slot, n, H, Hkv, scale_log2, part_o, part_ml, out, ldo, s);
+    return 2;
   }
-  ++nl;
+  auto cc = dh == 64 ? (f8 ? decode_attention_cc<64, fp8> : decode_attention_cc<64, bf16>)
+                     : (f8 ? decode_attention_cc<128, fp8> : decode_attention_cc<128, bf16>);
+  cc(c, q, ld_q, pos, slot, n, H, Hkv, max_ctx, out, ldo, s);
+  return 1;
 }
 
 void launch_ln(cudaStream_t s, int rows, const bf16* x, const bf16* w, const bf16* b, bf16* y, int d, float eps) {
@@ -2102,7 +1735,7 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   const auto& a = m->a;
   const int B = m->max_batch;
   const int d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size;
-  const int qd = m->qd, qkvd = m->qkvd;
+  const int qd = m->qd, qkvd = m->qkvd, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
   const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
   B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin + B, n * 4, cudaMemcpyHostToDevice, s));
@@ -2123,8 +1756,9 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       o1.out2 = m->cat + qd; o1.ldo2 = m->ld_cat; o1.n_split = qkvd;
       o1.act = 1; o1.act_from = qkvd;   // exact GeLU on the MLP half only
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd + f, d, o1, m->lt[l].qkv); ++nl;
-      append_kv(m, s, n, l, 1, nl);
-      decode_attention(m, s, n, l, m->cat, m->ld_cat, nl);
+      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 1, s); ++nl;
+      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
+                             m->part_ml, m->cat, m->ld_cat, s);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
       dgemm(m, s, n, m->cat, m->ld_cat, p.wo, m->ld_cat, d, m->ld_cat, o2, m->lt[l].o); ++nl;
@@ -2134,8 +1768,9 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd; o1.bias = m->w + p.bqkv;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      append_kv(m, s, n, l, 0, nl);
-      decode_attention(m, s, n, l, m->cat, qd, nl);
+      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 0, s); ++nl;
+      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
+                             m->part_ml, m->cat, qd, s);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d; o2.bias = m->w + p.bo;
       dgemm(m, s, n, m->cat, qd, p.wo, qd, d, qd, o2, m->lt[l].o); ++nl;
@@ -2151,8 +1786,9 @@ void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
       GemmDecodeOut o1;
       o1.out = m->qkv; o1.ldo = qkvd;
       dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      append_kv(m, s, n, l, 1, nl);
-      decode_attention(m, s, n, l, m->cat, qd, nl);
+      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 1, s); ++nl;
+      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
+                             m->part_ml, m->cat, qd, s);
       GemmDecodeOut o2;
       o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
       dgemm(m, s, n, m->cat, qd, p.wo, qd, d, qd, o2, m->lt[l].o); ++nl;
@@ -2278,34 +1914,15 @@ void ensure_scoring(Infer* m, size_t T) {
 
 Infer* paged_model(b200w_ctx* ctx) {
   Infer* m = model(ctx);
-  if (m->n_pages == 0) throw StateError("the KV cache is not paged (b200w_infer_init_paged)");
+  if (!m->kv.paged) throw StateError("the KV cache is not paged (b200w_infer_init_paged)");
   return m;
 }
 
-// Paged mode: positions [0, n_tokens) of `slot` must lie in pages the slot holds (the host mirror of the table), and
-// the call writes K/V from position `first_write` on, which must not lie in a page the slot shares.
-void check_paged_slot(const Infer* m, int slot, long long n_tokens, long long first_write) {
-  if (m->n_pages == 0) return;
-  const size_t held = m->held[slot].size();
-  B200W_CHECK(held > 0, "cache slot holds no KV pages (b200w_infer_reserve)");
-  B200W_CHECK(n_tokens <= static_cast<long long>(held) * KV_PAGE, "position beyond the KV pages the slot holds");
-  B200W_CHECK(first_write >= m->floor[slot], "K/V write below the slot's write floor (into a shared page)");
-}
-
-// drops the slot's reference to each page it holds; a page nobody references returns to the free list, in table order
-void release_pages(Infer* m, int slot) {
-  auto& h = m->held[slot];
-  for (const int32_t p : h)
-    if (--m->refs[p] == 0) m->free_pages.push_back(p);
-  h.clear();
-  m->floor[slot] = 0;
-}
-
 void check_weights_unshared(const Infer* m) {
-  if (m->retained) throw StateError("KV pages are retained: cached K/V belong to the weights that computed them");
+  if (m->kv.retained) throw StateError("KV pages are retained: cached K/V belong to the weights that computed them");
 }
 
-// b200w_infer_init (n_pages == 0) and b200w_infer_init_paged_kv
+// b200w_infer_init (n_pages 0: the contiguous cache) and b200w_infer_init_paged_kv
 void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages, int64_t prefill_tokens,
                 int kv_dtype = B200W_KV_BF16) {
   B200W_CHECK(arch != nullptr && max_batch >= 1 && max_batch <= 128, "bad arch / max_batch (1..128)");
@@ -2333,8 +1950,6 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   auto m = std::make_unique<Infer>();
   m->a = *arch;
   m->max_batch = max_batch;
-  m->n_pages = n_pages;
-  m->kv_dtype = kv_dtype;
   if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
   m->lt.resize(arch->num_layers);   // all-null when the tiled copies are disabled
   build(m.get());
@@ -2351,51 +1966,17 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->mid = m->alloc<bf16>(B * fmid);
   m->act = m->alloc<bf16>(B * f);
   m->logits = m->alloc<bf16>(B * a.vocab_size);
-  const size_t cache = static_cast<size_t>(a.num_layers) * m->layer_rows() * kd;
-  // zero: the tensor-core decode attention multiplies P = 0 by whatever the rows beyond a slot's length hold
-  // (a page handed out again holds zeros or K/V an earlier request wrote: finite either way; the fp8 writer never
-  // stores a NaN byte)
-  if (m->fp8()) {
-    const size_t scales = static_cast<size_t>(a.num_layers) * m->layer_rows() * a.num_kv_heads;
-    m->kq = m->alloc<uint8_t>(cache);
-    m->vq = m->alloc<uint8_t>(cache);
-    m->ks = m->alloc<float>(scales);
-    m->vs = m->alloc<float>(scales);
-    B200W_CUDA(cudaMemset(m->kq, 0, cache));
-    B200W_CUDA(cudaMemset(m->vq, 0, cache));
-    B200W_CUDA(cudaMemset(m->ks, 0, scales * sizeof(float)));
-    B200W_CUDA(cudaMemset(m->vs, 0, scales * sizeof(float)));
-  } else {
-    m->kc = m->alloc<bf16>(cache);
-    m->vc = m->alloc<bf16>(cache);
-    B200W_CUDA(cudaMemset(m->kc, 0, cache * sizeof(bf16)));
-    B200W_CUDA(cudaMemset(m->vc, 0, cache * sizeof(bf16)));
-  }
-  m->nsplit = (a.max_ctx + TC_KB - 1) / TC_KB;
-  const size_t tab = B * m->nsplit;
-  m->table = m->alloc<int32_t>(tab);
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->table_pin), tab * sizeof(int32_t)));
-  // contiguous: block j of slot s starts at row s * max_ctx + j * KV_PAGE for the context's life (when max_ctx is
-  // not a multiple of KV_PAGE, a slot's last block runs into the next slot's rows, or past the end of the cache
-  // where TMA fills zeros; the attention weights those keys by 0). Paged: no slot holds a page yet, entries 0.
-  for (size_t s = 0; s < B; ++s)
-    for (int j = 0; j < m->nsplit; ++j)
-      m->table_pin[s * m->nsplit + j] = n_pages ? 0 : static_cast<int32_t>(s * a.max_ctx + j * KV_PAGE);
-  B200W_CUDA(cudaMemcpy(m->table, m->table_pin, tab * sizeof(int32_t), cudaMemcpyHostToDevice));
-  if (n_pages) {
-    for (int p = n_pages - 1; p >= 0; --p) m->free_pages.push_back(p);   // page 0 is handed out first
-    m->held.assign(B, {});
-    m->floor.assign(B, 0);
-    m->refs.assign(n_pages, 0);
-    m->index_refs.assign(n_pages, 0);
+  m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim,
+             [&](size_t bytes) { return static_cast<void*>(m->alloc<uint8_t>(bytes)); });
+  if (m->kv.paged) {
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
     m->pf_limit = static_cast<size_t>(prefill_tokens);
     ensure_prefill(m.get(), m->pf_limit);
     ensure_prefill_pin(m.get(), m->pf_limit);
   }
   if (a.num_heads / a.num_kv_heads >= 4) {
-    m->part_o = m->alloc<float>(B * a.num_heads * m->nsplit * a.head_dim);
-    m->part_ml = m->alloc<float2>(B * a.num_heads * m->nsplit);
+    m->part_o = m->alloc<float>(B * a.num_heads * m->kv.nsplit * a.head_dim);
+    m->part_ml = m->alloc<float2>(B * a.num_heads * m->kv.nsplit);
   }
   m->tok = m->alloc<int32_t>(B);
   m->pos = m->alloc<int32_t>(B);
@@ -2420,55 +2001,51 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   ctx_set_infer(ctx, m.release(), infer_destroy);
 }
 
+
+template <int DH, typename KV>
+void attention_fwd_cached_launch(const KVLayer& c, const CUtensorMap& tq, int q_head_stride, bf16* out, int ld_out,
+                                 const int32_t* slots, const int32_t* starts, const int32_t* lengths, int n_seqs, int S,
+                                 int H, int Hkv, float scale_log2, cudaStream_t s) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
+  const int smem = ca_smem_bytes<DH>() + (F8 ? ca_fp8_extra_bytes<DH>() : 0);
+  const KVTmaps tm = kv_tmaps(c, Hkv, DH);
+  const dim3 grid((S / 128) * n_seqs * H);
+  static PerDeviceOnce once;
+  if constexpr (F8) {
+    once.run([&] {
+      B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_fp8_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    });
+    attn_fwd_cached_fp8_kernel<DH><<<grid, CA_THREADS, smem, s>>>(tq, tm.k, tm.v, q_head_stride, out, ld_out, c.table,
+                                                                 c.nsplit, slots, starts, lengths, n_seqs, S, H, Hkv,
+                                                                 scale_log2, c.kscale, c.vscale);
+  } else {
+    once.run([&] {
+      B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    });
+    attn_fwd_cached_kernel<DH><<<grid, CA_THREADS, smem, s>>>(tq, tm.k, tm.v, q_head_stride, out, ld_out, c.table,
+                                                             c.nsplit, slots, starts, lengths, n_seqs, S, H, Hkv,
+                                                             scale_log2);
+  }
+}
+
 }  // namespace
 
-void b200w::attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
-                                 int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
+void b200w::attention_fwd_cached(const KVLayer& c, const void* q, int ld_q, int q_head_stride, const int32_t* slots,
                                  const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs,
-                                 int S, int H, int Hkv, int dh, float scale, cudaStream_t s, const float* kscale,
-                                 const float* vscale) {
+                                 int S, int H, int Hkv, int dh, float scale, cudaStream_t s) {
   B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
   B200W_CHECK(n_seqs >= 1 && S >= 128 && S % 128 == 0, "padded length must be a positive multiple of 128");
   B200W_CHECK(H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad head configuration");
   B200W_CHECK(q_head_stride >= dh && ld_q >= H * q_head_stride && ld_out >= H * dh && ld_out % 8 == 0,
               "bad query / output strides");
-  B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1, "bad KV cache");
-  const bool f8 = kscale != nullptr;
-  B200W_CHECK(f8 == (vscale != nullptr), "an fp8 cache needs both scale arrays");
-  const int kd = Hkv * dh;
+  B200W_CHECK(c.rows >= KV_PAGE && c.rows % KV_PAGE == 0 && c.nsplit >= 1, "bad KV cache");
+  const bool f8 = c.dtype == B200W_KV_FP8_E4M3;
+  B200W_CHECK(!f8 || (c.kscale && c.vscale), "an fp8 cache needs both scale arrays");
   const CUtensorMap tq = make_tmap_bf16_2d(q, static_cast<uint64_t>(n_seqs) * S, ld_q, ld_q, 128, 64);
-  const CUtensorMap tk = f8 ? make_tmap_u8_2d(kcache, cache_rows, kd, kd, KV_PAGE, dh)
-                            : make_tmap_bf16_2d(kcache, cache_rows, kd, kd, KV_PAGE, 64);
-  const CUtensorMap tv = f8 ? make_tmap_u8_2d(vcache, cache_rows, kd, kd, KV_PAGE, dh)
-                            : make_tmap_bf16_2d(vcache, cache_rows, kd, kd, KV_PAGE, 64);
-  static PerDeviceOnce once;
-  once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ca_smem_bytes<64>()));
-    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ca_smem_bytes<128>()));
-    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_fp8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ca_smem_bytes<64>() + ca_fp8_extra_bytes<64>()));
-    B200W_CUDA(cudaFuncSetAttribute(attn_fwd_cached_fp8_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ca_smem_bytes<128>() + ca_fp8_extra_bytes<128>()));
-  });
-  const dim3 grid((S / 128) * n_seqs * H);
-  const float scale_log2 = scale * 1.4426950408889634f;
-  bf16* o = static_cast<bf16*>(out);
-  if (f8 && dh == 64)
-    attn_fwd_cached_fp8_kernel<64><<<grid, CA_THREADS, ca_smem_bytes<64>() + ca_fp8_extra_bytes<64>(), s>>>(
-        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2,
-        kscale, vscale);
-  else if (f8)
-    attn_fwd_cached_fp8_kernel<128><<<grid, CA_THREADS, ca_smem_bytes<128>() + ca_fp8_extra_bytes<128>(), s>>>(
-        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2,
-        kscale, vscale);
-  else if (dh == 64)
-    attn_fwd_cached_kernel<64><<<grid, CA_THREADS, ca_smem_bytes<64>(), s>>>(
-        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2);
-  else
-    attn_fwd_cached_kernel<128><<<grid, CA_THREADS, ca_smem_bytes<128>(), s>>>(
-        tq, tk, tv, q_head_stride, o, ld_out, table, nsplit, slots, starts, lengths, n_seqs, S, H, Hkv, scale_log2);
+  auto launch = dh == 64 ? (f8 ? attention_fwd_cached_launch<64, fp8> : attention_fwd_cached_launch<64, bf16>)
+                         : (f8 ? attention_fwd_cached_launch<128, fp8> : attention_fwd_cached_launch<128, bf16>);
+  launch(c, tq, q_head_stride, static_cast<bf16*>(out), ld_out, slots, starts, lengths, n_seqs, S, H, Hkv,
+         scale * 1.4426950408889634f, s);
   B200W_CUDA(cudaGetLastError());
 }
 
@@ -2481,34 +2058,25 @@ void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, co
   B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1 && nsplit * KV_PAGE <= 8192,
               "bad KV cache");
   B200W_CHECK(ld_q >= (H + 2 * Hkv) * dh && ld_out >= H * dh && kscale && vscale, "bad strides / scales");
-  // the engine's decode attention on one layer of a pool the caller owns: a model that allocates only the
-  // tensor-core partials and borrows everything else
-  Infer m;
-  m.a.num_heads = H;
-  m.a.num_kv_heads = Hkv;
-  m.a.head_dim = dh;
-  m.a.max_ctx = nsplit * KV_PAGE;
-  m.kd = Hkv * dh;
-  m.qkvd = ld_q;
-  m.n_pages = static_cast<int>(cache_rows / KV_PAGE);
-  m.nsplit = nsplit;
-  m.kv_dtype = B200W_KV_FP8_E4M3;
-  m.kq = static_cast<uint8_t*>(const_cast<void*>(kcache));
-  m.vq = static_cast<uint8_t*>(const_cast<void*>(vcache));
-  m.ks = const_cast<float*>(kscale);
-  m.vs = const_cast<float*>(vscale);
-  m.qkv = static_cast<bf16*>(const_cast<void*>(q));
-  m.pos = const_cast<int32_t*>(positions);
-  m.slot = const_cast<int32_t*>(slots);
-  m.table = const_cast<int32_t*>(table);
-  if (H / Hkv >= 4) {
-    m.part_o = m.alloc<float>(static_cast<size_t>(n) * H * nsplit * dh);
-    m.part_ml = m.alloc<float2>(static_cast<size_t>(n) * H * nsplit);
-  }
-  int64_t nl = 0;
-  decode_attention(&m, s, n, 0, static_cast<bf16*>(out), ld_out, nl);
+  // the engine's decode attention on one layer of a pool the caller owns; only the tensor-core partials are allocated
+  KVLayer c;
+  c.k = const_cast<void*>(kcache);
+  c.v = const_cast<void*>(vcache);
+  c.kscale = const_cast<float*>(kscale);
+  c.vscale = const_cast<float*>(vscale);
+  c.rows = cache_rows;
+  c.table = table;
+  c.nsplit = nsplit;
+  c.dtype = B200W_KV_FP8_E4M3;
+  const size_t n_part = H / Hkv >= 4 ? static_cast<size_t>(n) * H * nsplit : 0;   // [n, H, nsplit]
+  void* part = nullptr;
+  if (n_part) B200W_CUDA(cudaMalloc(&part, n_part * (dh * sizeof(float) + sizeof(float2))));
+  std::unique_ptr<void, cudaError_t (*)(void*)> owner(part, cudaFree);
+  float* part_o = static_cast<float*>(part);
+  decode_attention(c, static_cast<const bf16*>(q), ld_q, positions, slots, n, H, Hkv, dh, nsplit * KV_PAGE, part_o,
+                   reinterpret_cast<float2*>(part_o + n_part * dh), static_cast<bf16*>(out), ld_out, s);
   B200W_CUDA(cudaGetLastError());
-  B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed with m
+  B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed on return
 }
 
 void b200w::logprobs(const void* logits, int ld, int rows, int V, const int32_t* targets, int k, float* lse,
@@ -2598,28 +2166,8 @@ int b200w_infer_kv_read(b200w_ctx* ctx, int layer, int slot, int pos0, int n, vo
     B200W_CHECK(layer >= 0 && layer < m->a.num_layers && slot >= 0 && slot < m->max_batch, "bad layer / slot");
     B200W_CHECK(pos0 >= 0 && n >= 0 && pos0 + static_cast<int64_t>(n) <= m->a.max_ctx && (n == 0 || (k_out && v_out)),
                 "bad positions / outputs");
-    if (m->n_pages)
-      B200W_CHECK(pos0 + static_cast<int64_t>(n) <= static_cast<int64_t>(m->held[slot].size()) * KV_PAGE,
-                  "position beyond the KV pages the slot holds");
     B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
-    const Infer::KVLayer c = m->kv_layer(layer);
-    const int Hkv = m->a.num_kv_heads;
-    const size_t row_bytes = static_cast<size_t>(m->kd) * (m->fp8() ? 1 : sizeof(bf16));
-    for (int i = 0; i < n; ++i) {   // through the host copy of the table
-      const int p = pos0 + i;
-      const size_t row = static_cast<size_t>(m->table_pin[static_cast<size_t>(slot) * m->nsplit + p / KV_PAGE]) +
-                         p % KV_PAGE;
-      B200W_CUDA(cudaMemcpy(static_cast<uint8_t*>(k_out) + i * row_bytes, static_cast<uint8_t*>(c.k) + row * row_bytes,
-                            row_bytes, cudaMemcpyDeviceToHost));
-      B200W_CUDA(cudaMemcpy(static_cast<uint8_t*>(v_out) + i * row_bytes, static_cast<uint8_t*>(c.v) + row * row_bytes,
-                            row_bytes, cudaMemcpyDeviceToHost));
-      if (m->fp8() && k_scale_out)
-        B200W_CUDA(cudaMemcpy(k_scale_out + static_cast<size_t>(i) * Hkv, c.ks + row * Hkv, Hkv * sizeof(float),
-                              cudaMemcpyDeviceToHost));
-      if (m->fp8() && v_scale_out)
-        B200W_CUDA(cudaMemcpy(v_scale_out + static_cast<size_t>(i) * Hkv, c.vs + row * Hkv, Hkv * sizeof(float),
-                              cudaMemcpyDeviceToHost));
-    }
+    m->kv.read_rows(layer, slot, pos0, n, k_out, v_out, k_scale_out, v_scale_out);
   });
 }
 
@@ -2632,43 +2180,11 @@ int b200w_infer_reserve_shared(b200w_ctx* ctx, int slot, int n_tokens, const int
     const size_t need = cdiv(n_tokens, KV_PAGE);
     B200W_CHECK(n_shared >= 0 && static_cast<size_t>(n_shared) <= need && (n_shared == 0 || shared_pages),
                 "n_shared must be in 0..ceil(n_tokens / 128)");
-    auto& h = m->held[slot];
-    // the references left once the slot has let go of what it holds: its pages with none return to the free list,
-    // and a shared page must keep one (a free page holds nothing to share)
-    auto after_release = [&](int32_t p) {
-      return m->refs[p] - static_cast<int32_t>(std::count(h.begin(), h.end(), p));
-    };
-    for (int i = 0; i < n_shared; ++i)
-      B200W_CHECK(shared_pages[i] >= 0 && shared_pages[i] < m->n_pages && after_release(shared_pages[i]) >= 1,
-                  "a shared page must be held by a slot or retained");
-    size_t returning = 0;
-    for (size_t i = 0; i < h.size(); ++i)
-      if (std::find(h.begin(), h.begin() + i, h[i]) == h.begin() + i && after_release(h[i]) == 0) ++returning;
-    const size_t fresh = need - n_shared;
-    if (fresh > m->free_pages.size() + returning) {
-      ctx_set_error(ctx, ("KV page pool exhausted: " + std::to_string(fresh) + " pages needed, " +
-                          std::to_string(m->free_pages.size()) + " free").c_str());
+    std::string err;
+    if (!m->kv.reserve_shared(slot, need, shared_pages, n_shared, ctx_stream(ctx), err)) {
+      ctx_set_error(ctx, err.c_str());
       short_of_pages = true;
-      return;
     }
-    release_pages(m, slot);
-    for (int i = 0; i < n_shared; ++i) {
-      h.push_back(shared_pages[i]);
-      ++m->refs[shared_pages[i]];
-    }
-    for (size_t i = 0; i < fresh; ++i) {
-      h.push_back(m->free_pages.back());
-      m->refs[m->free_pages.back()] = 1;
-      m->free_pages.pop_back();
-    }
-    m->floor[slot] = n_shared * KV_PAGE;
-    // the row goes to the device on the library stream, so it lands before the next step or prefill; the
-    // table's address never changes, so the captured decode graphs read the new row
-    int32_t* row = m->table_pin + static_cast<size_t>(slot) * m->nsplit;
-    std::transform(h.begin(), h.end(), row, [](int32_t page) { return page * KV_PAGE; });
-    std::fill(row + h.size(), row + m->nsplit, 0);
-    B200W_CUDA(cudaMemcpyAsync(m->table + static_cast<size_t>(slot) * m->nsplit, row, m->nsplit * sizeof(int32_t),
-                               cudaMemcpyHostToDevice, ctx_stream(ctx)));
   });
   return st == B200W_OK && short_of_pages ? B200W_ERR_OOM : st;
 }
@@ -2681,7 +2197,7 @@ int b200w_infer_release(b200w_ctx* ctx, int slot) {
   return iguard(ctx, [&] {
     Infer* m = paged_model(ctx);
     B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
-    release_pages(m, slot);   // the device row is left as it was: steps and prefills of the slot are refused
+    m->kv.release(slot);   // the device row is left as it was: steps and prefills of the slot are refused
   });
 }
 
@@ -2690,30 +2206,15 @@ int b200w_infer_retain_pages(b200w_ctx* ctx, const int32_t* pages, int n, int de
     Infer* m = paged_model(ctx);
     B200W_CHECK(delta == 1 || delta == -1, "delta must be +1 or -1");
     B200W_CHECK(n >= 0 && (n == 0 || pages), "bad page list");
-    std::unordered_map<int32_t, int32_t> count;   // every page is checked before any reference changes
-    for (int i = 0; i < n; ++i) {
-      B200W_CHECK(pages[i] >= 0 && pages[i] < m->n_pages, "page outside the pool");
-      ++count[pages[i]];
-    }
-    for (const auto& pc : count) {
-      if (delta > 0) B200W_CHECK(m->refs[pc.first] >= 1, "retaining a page that holds no reference (a free page)");
-      else B200W_CHECK(m->index_refs[pc.first] >= pc.second, "dropping a retained reference that does not exist");
-    }
-    for (int i = 0; i < n; ++i) {
-      const int32_t p = pages[i];
-      m->refs[p] += delta;
-      m->index_refs[p] += delta;
-      m->retained += delta;
-      if (m->refs[p] == 0) m->free_pages.push_back(p);
-    }
+    m->kv.retain(pages, n, delta);
   });
 }
 
 int b200w_infer_kv_pages(b200w_ctx* ctx, int64_t* total, int64_t* free_pages) {
   return iguard(ctx, [&] {
     Infer* m = paged_model(ctx);
-    if (total) *total = m->n_pages;
-    if (free_pages) *free_pages = static_cast<int64_t>(m->free_pages.size());
+    if (total) *total = m->kv.n_pages;
+    if (free_pages) *free_pages = static_cast<int64_t>(m->kv.free_pages.size());
   });
 }
 
@@ -2722,7 +2223,7 @@ int b200w_infer_slot_pages(b200w_ctx* ctx, int slot, int32_t* out, int cap) {
   const int st = iguard(ctx, [&] {
     Infer* m = paged_model(ctx);
     B200W_CHECK(slot >= 0 && slot < m->max_batch, "bad cache slot");
-    const auto& h = m->held[slot];
+    const auto& h = m->kv.held[slot];
     n = static_cast<int>(h.size());
     if (out) std::copy(h.begin(), h.begin() + std::min(n, std::max(cap, 0)), out);
   });
@@ -2816,7 +2317,7 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
       B200W_CHECK(positions[i] >= 0 && positions[i] < a.max_ctx, "position outside the KV cache");
       B200W_CHECK(slots[i] >= 0 && slots[i] < m->max_batch, "bad cache slot");
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
-      check_paged_slot(m, slots[i], positions[i] + 1LL, positions[i]);
+      m->kv.check_slot(slots[i], positions[i] + 1LL, positions[i]);
     }
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
@@ -2912,9 +2413,9 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
                     "a cached prefix must be a positive multiple of 128 below the prompt length");
       B200W_CHECK(lengths[b] >= 1 && lengths[b] - start <= S && lengths[b] <= a.max_ctx, "bad prompt length");
       B200W_CHECK(slots[b] >= 0 && slots[b] < m->max_batch, "bad cache slot");
-      check_paged_slot(m, slots[b], lengths[b], start);
+      m->kv.check_slot(slots[b], lengths[b], start);
     }
-    if (m->n_pages) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
+    if (m->kv.paged) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
     for (size_t i = 0; i < T; ++i)
       B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
     if (a.family == B200W_FAMILY_OPT && !starts)
@@ -2978,24 +2479,11 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     ++nl;
     for (int l = 0; l < a.num_layers; ++l) {
       const auto& p = m->lp[l];
-      const Infer::KVLayer c = m->kv_layer(l);
-      // q / k rotated (rope != 0) into dst [T, *] at head stride dh_dst, the real positions' K/V into the cache
+      const KVLayer c = m->kv.layer(l);
       auto scatter = [&](bf16* dst, int ld_dst, int dh_dst, const int32_t* start) {
-        if (m->fp8()) {   // a warp per (token, head)
-          const long long warps = static_cast<long long>(Ti) * HT;
-          prefill_rope_scatter_fp8_kernel<<<cdiv(warps * 32, 256), 256, 0, s>>>(
-              m->pf_qkv, qkvd, dst, ld_dst, m->inv_freq, m->pf_len, m->pf_slot, static_cast<uint8_t*>(c.k),
-              static_cast<uint8_t*>(c.v), c.ks, c.vs, Ti, S, H, Hkv, dh, dh_dst, opt ? 0 : 1, m->table, m->nsplit,
-              start);
-        } else {
-          const long long rp = static_cast<long long>(Ti) * HT * (dh / 2);
-          prefill_rope_scatter_kernel<<<cdiv(rp, 256), 256, 0, s>>>(m->pf_qkv, qkvd, dst, ld_dst, m->inv_freq, m->pf_len,
-                                                                    m->pf_slot, static_cast<bf16*>(c.k),
-                                                                    static_cast<bf16*>(c.v), Ti, S, H, Hkv, dh, dh_dst,
-                                                                    opt ? 0 : 1, m->table, m->nsplit, start);
-        }
+        m->kv.scatter(l, m->pf_qkv, qkvd, dst, ld_dst, dh_dst, m->inv_freq, m->pf_len, m->pf_slot, Ti, S, H, dh,
+                      opt ? 0 : 1, start, s);
         ++nl;
-        B200W_CUDA(cudaGetLastError());
       };
       if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + p.ln1_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s);
       else layernorm_kernel<<<Ti, 256, 0, s>>>(h, m->w + p.ln1_w, m->w + p.ln1_b, m->pf_nrm, d, a.norm_eps);
@@ -3011,8 +2499,8 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
         // the paged attention reads the queries at their own width and writes the o-projection's input directly
         // (on the fp8 pool every key it reads, the suffix's own included, is the quantized one)
         scatter(m->pf_qkv, qkvd, dh, m->pf_start);
-        attention_fwd_cached(m->pf_qkv, qkvd, dh, c.k, c.v, m->layer_rows(), m->table, m->nsplit, m->pf_slot, m->pf_start,
-                             m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv, dh, scale, s, c.ks, c.vs); ++nl;
+        attention_fwd_cached(c, m->pf_qkv, qkvd, dh, m->pf_slot, m->pf_start, m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv,
+                             dh, scale, s); ++nl;
       } else {
         // a cold prefill attends over the bf16 activations, on either pool
         bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;

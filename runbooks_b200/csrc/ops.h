@@ -79,25 +79,32 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
                    int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs = nullptr);
 
 // ---- infer.cu ------------------------------------------------------------------------------
+// One layer of a KV cache as its writers and readers see it (DESIGN §3.5). Position p of cache slot `slot` is row
+// table[slot * nsplit + p / 128] + p % 128 of k / v [rows, Hkv * dh]: bf16, or e4m3 bytes (dtype B200W_KV_FP8_E4M3)
+// with one fp32 scale per (row, kv head) in kscale / vscale [rows, Hkv]. rows is a multiple of 128.
+struct KVLayer {
+  void *k = nullptr, *v = nullptr;
+  float *kscale = nullptr, *vscale = nullptr;
+  int64_t rows = 0;
+  const int32_t* table = nullptr;
+  int nsplit = 0;
+  int dtype = 0;   // B200W_KV_BF16 (0) or B200W_KV_FP8_E4M3
+};
 // Causal attention of prompt suffixes after a cached prefix (infer.cu attn_fwd_cached_kernel). Sequence b's rows
 // [b * S, b * S + S) of q [n_seqs * S, ld_q] (head h at column h * q_head_stride, its first dh columns used) are its
-// positions starts[b] + p; they attend to positions [0, position] of cache slot slots[b], whose K and V are rows
-// table[slot * nsplit + position / 128] + position % 128 of kcache / vcache [cache_rows, Hkv * dh]. starts[b] is a
+// positions starts[b] + p; they attend to positions [0, position] of cache slot slots[b] of c. starts[b] is a
 // multiple of 128 below lengths[b]; the pages of positions [0, lengths[b]) are the caller's to have filled and
 // entered in the table. out [n_seqs * S, ld_out]: head h at column h * dh. slots / starts / lengths: DEVICE int32
 // [n_seqs]. Rows at positions >= lengths[b] get finite values that mean nothing.
+void attention_fwd_cached(const KVLayer& c, const void* q, int ld_q, int q_head_stride, const int32_t* slots,
+                          const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
+                          int H, int Hkv, int dh, float scale, cudaStream_t s);
 // The decode step's attention over one layer of an fp8 pool (the engine's kernels: CUDA cores when H / Hkv < 4,
 // tensor cores otherwise). q [n, ld_q]: row r's query heads at columns h * dh; positions / slots DEVICE int32 [n].
 void decode_attention_fp8(const void* q, int ld_q, const void* kcache, const void* vcache, const float* kscale,
                           const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
                           const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H, int Hkv,
                           int dh, float scale, cudaStream_t s);
-// kscale / vscale [cache_rows, Hkv] non-null: kcache / vcache hold e4m3 bytes (DESIGN §3.5)
-void attention_fwd_cached(const void* q, int ld_q, int q_head_stride, const void* kcache, const void* vcache,
-                          int64_t cache_rows, const int32_t* table, int nsplit, const int32_t* slots,
-                          const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
-                          int H, int Hkv, int dh, float scale, cudaStream_t s, const float* kscale = nullptr,
-                          const float* vscale = nullptr);
 // Row-wise log-softmax of bf16 logits [rows, ld] (V % 8 == 0, ld % 8 == 0; infer.cu logprobs_kernel): lse, the
 // log-probability of targets[r] (nullable; an id outside [0, V) gives 0) and of the row maximum, and the k
 // (<= B200W_MAX_TOP_LOGPROBS) largest logits as ids and log-probabilities [rows, k], by value descending with ties

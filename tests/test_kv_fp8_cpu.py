@@ -51,23 +51,31 @@ def test_fp8_without_a_paged_cache_fails_at_startup(tmp_path):
     assert server.main(["--content", str(tmp_path), "--port", "0", "--kv-cache-dtype", "e5m2"]) == 1
 
 
-def test_fp8_kernel_instances_neither_spill_nor_serialize(tmp_path):
+def test_kv_writer_and_reader_instances_neither_spill_nor_serialize(tmp_path):
     nvcc = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.exists("/usr/local/cuda/bin/nvcc") else None)
     if nvcc is None:
         pytest.skip("nvcc is not installed")
     from runbooks_b200.build import NVCC_FLAGS
-    r = subprocess.run([nvcc, *NVCC_FLAGS, "-Xptxas=-v", "-c", os.path.join(ROOT, "runbooks_b200", "csrc", "infer.cu"),
-                        "-o", str(tmp_path / "infer.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    log = r.stdout + r.stderr
+    log = ""
+    for src in ("kv_cache.cu", "infer.cu"):   # the writers, and the readers
+        r = subprocess.run([nvcc, *NVCC_FLAGS, "-Xptxas=-v", "-c", os.path.join(ROOT, "runbooks_b200", "csrc", src),
+                            "-o", str(tmp_path / src.replace(".cu", ".o"))], capture_output=True, text=True)
+        assert r.returncode == 0, r.stderr
+        log += r.stdout + r.stderr
     assert not [ln for ln in log.splitlines() if re.search(r"C751[45]|serialized", ln)]
     props = re.findall(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
                        r"(\d+) bytes spill loads", log)
-    fp8 = {fn: (int(st), int(ld)) for fn, _, st, ld in props if "fp8" in fn}
-    writers = [fn for fn in fp8 if re.search(r"(rope_append|prefill_rope_scatter)_fp8_kernel", fn)]
-    attn = [fn for fn in fp8 if re.search(r"(decode_attn|decode_attn_tc|attn_fwd_cached)_fp8_kernelILi(64|128)EE", fn)]
+    spills = {fn: (int(st), int(ld)) for fn, _, st, ld in props}
+    fp8 = {fn: v for fn, v in spills.items() if "fp8" in fn}
+    writers = [fn for fn in fp8 if re.search(r"(rope_append|prefill_rope_scatter)_kernelI13__nv_fp8_e4m3", fn)]
+    attn = [fn for fn in fp8 if re.search(r"decode_attn_kernelILi(64|128)E13__nv_fp8_e4m3|"
+                                          r"(decode_attn_tc|attn_fwd_cached)_fp8_kernelILi(64|128)EE", fn)]
     assert len(writers) == 2 and len(attn) == 6, sorted(fp8)   # 2 CUDA-core, 2 tensor-core, 2 cached-prefix
     assert all(v == (0, 0) for v in fp8.values()), fp8
+    # the bf16 instances of the same writers
+    bf16_writers = {fn: v for fn, v in spills.items()
+                    if re.search(r"(rope_append|prefill_rope_scatter)_kernelI13__nv_bfloat16", fn)}
+    assert len(bf16_writers) == 2 and all(v == (0, 0) for v in bf16_writers.values()), bf16_writers
 
 
 # ---- the cached-prefix kernel's fp8 hand-off (tools/protocol_model.py) ----

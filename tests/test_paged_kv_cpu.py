@@ -265,7 +265,7 @@ def test_bad_command_line_values_fail_at_startup(tmp_path):
 
 
 # ---- the decode attention kernels as compiled ----
-def test_decode_attention_neither_spills_nor_serializes(tmp_path):
+def test_decode_attention_instances_neither_spill_nor_serialize(tmp_path):
     nvcc = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.exists("/usr/local/cuda/bin/nvcc") else None)
     if nvcc is None:
         pytest.skip("nvcc is not installed")
@@ -278,6 +278,7 @@ def test_decode_attention_neither_spills_nor_serializes(tmp_path):
     props = re.findall(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
                        r"(\d+) bytes spill loads", log)
     attn = {fn: (int(st), int(ld)) for fn, _, st, ld in props if "decode_attn" in fn}
-    kernels = [fn for fn in attn if re.search(r"decode_attn(_tc)?_kernelILi(64|128)EE", fn)]
+    kernels = [fn for fn in attn if re.search(r"decode_attn_kernelILi(64|128)E13__nv_bfloat16EE|"
+                                              r"decode_attn_tc_kernelILi(64|128)EE", fn)]
     assert len(kernels) == 4, sorted(attn)      # CUDA-core and tensor-core, one instance per head width
     assert all(v == (0, 0) for v in attn.values()), attn
