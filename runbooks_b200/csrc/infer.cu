@@ -1423,14 +1423,15 @@ struct Infer {
   std::unordered_map<std::string, int> index;
   size_t n_elems = 0;
   bf16* w = nullptr;
-  // per layer: norm parameters, the projections (offsets of their (0,0) element) and biases (OPT)
-  struct L { size_t ln1_w, ln1_b, ln2_w, ln2_b, wqkv, bqkv, wo, bo, w1, b1, w2, b2; };
+  // per layer: norm parameters, the projections (offsets of their (0,0) element), biases (OPT), and the decode-time
+  // copy of each projection as consecutive 16 KB swizzled tile images (gemm.cu retile_weights): a decode GEMM CTA
+  // streams one contiguous HBM region instead of 128-byte row segments (null until ensure_tiled makes them)
+  struct L {
+    size_t ln1_w, ln1_b, ln2_w, ln2_b, wqkv, bqkv, wo, bo, w1, b1, w2, b2;
+    uint8_t *t_qkv, *t_o, *t_w1, *t_w2;
+  };
   std::vector<L> lp;
   size_t p_embed = 0, p_pos = 0, p_lnf_w = 0, p_lnf_b = 0, p_lm = 0;
-  // decode-time copy of every projection as consecutive 16 KB swizzled tile images (gemm.cu retile_weights):
-  // a decode GEMM CTA streams one contiguous HBM region instead of 128-byte row segments
-  struct LT { uint8_t *qkv = nullptr, *o = nullptr, *w1 = nullptr, *w2 = nullptr; };
-  std::vector<LT> lt;
   uint8_t* t_lm = nullptr;
   bool tiled_valid = false, use_tiled = true;
   int qd = 0, kd = 0, qkvd = 0, ld_cat = 0;  // Falcon: ld_cat = qd + f, the [attention | mlp hidden] operand
@@ -1445,7 +1446,8 @@ struct Infer {
   float* part_o = nullptr;      // tensor-core decode attention partials [max_batch, H, nsplit, dh]
   float2* part_ml = nullptr;    // [max_batch, H, nsplit] (max, sum)
   int32_t *tok = nullptr, *pos = nullptr, *slot = nullptr, *next = nullptr;
-  int32_t* pin = nullptr;  // pinned host staging: tok | pos | slot | next, max_batch each
+  // pinned host staging, max_batch each, one allocation: a step's tokens, positions, slots; any call's next tokens
+  int32_t *pin_tok = nullptr, *pin_pos = nullptr, *pin_slot = nullptr, *pin_next = nullptr;
   std::unordered_map<int, cudaGraphExec_t> graphs;  // whole decode step per row count
   std::unordered_map<int, int> warm;
   // prefill buffers, grown on demand to the largest n_seqs * padded_len seen
@@ -1455,8 +1457,7 @@ struct Infer {
   float* pf_lse = nullptr;
   int32_t *pf_tok = nullptr, *pf_len = nullptr, *pf_slot = nullptr, *pf_last = nullptr, *pf_start = nullptr;
   int32_t* pf_pos = nullptr;   // OPT after a cached prefix: the learned-position row of every token
-  int32_t* pf_pin = nullptr;
-  size_t pf_pin_cap = 0;
+  int32_t* pf_pin = nullptr;   // pinned staging of a prefill call of up to pf_cap rows (stage_prefill)
   // token log-probabilities, allocated by the first call that asks for them: the next-token rows [max_batch]
   // (lse, token_lp, top ids / top log-probabilities [max_batch, B200W_MAX_TOP_LOGPROBS]); for prompt scoring a bf16
   // chunk of lm_head outputs [lp_chunk_rows, V] and per-row outputs for lp_cap prefill rows
@@ -1494,7 +1495,7 @@ struct Infer {
   }
   ~Infer() {
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
-    if (pin) cudaFreeHost(pin);
+    if (pin_tok) cudaFreeHost(pin_tok);
     if (pf_pin) cudaFreeHost(pf_pin);
     if (sp_pin) cudaFreeHost(sp_pin);
     for (void* p : allocs) cudaFree(p);
@@ -1644,18 +1645,16 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
     if (!dst) dst = m->alloc<uint8_t>(retiled_bytes(N, K));
     retile_weights(m->w + woff, ldw, dst, N, K, s);
   };
-  m->lt.resize(a.num_layers);
   for (int l = 0; l < a.num_layers; ++l) {
-    const auto& p = m->lp[l];
-    auto& t = m->lt[l];
+    auto& p = m->lp[l];
     if (falcon) {
-      make(t.qkv, p.wqkv, d, qkvd + f, d);                 // [q k v | dense_h_to_4h]
-      make(t.o, p.wo, m->ld_cat, d, m->ld_cat);            // [dense | dense_4h_to_h]
+      make(p.t_qkv, p.wqkv, d, qkvd + f, d);               // [q k v | dense_h_to_4h]
+      make(p.t_o, p.wo, m->ld_cat, d, m->ld_cat);          // [dense | dense_4h_to_h]
     } else {
-      make(t.qkv, p.wqkv, d, qkvd, d);
-      make(t.o, p.wo, qd, d, qd);
-      make(t.w1, p.w1, d, llama ? 2 * f : f, d);
-      make(t.w2, p.w2, f, d, f);
+      make(p.t_qkv, p.wqkv, d, qkvd, d);
+      make(p.t_o, p.wo, qd, d, qd);
+      make(p.t_w1, p.w1, d, llama ? 2 * f : f, d);
+      make(p.t_w2, p.w2, f, d, f);
     }
   }
   make(m->t_lm, m->p_lm, d, V, d);
@@ -1726,93 +1725,187 @@ int decode_attention(const KVLayer& c, const bf16* q, int ld_q, const int32_t* p
   return 1;
 }
 
-void launch_ln(cudaStream_t s, int rows, const bf16* x, const bf16* w, const bf16* b, bf16* y, int d, float eps) {
-  launch_pdl(layernorm_kernel, dim3(rows), dim3(256), 0, s, x, w, b, y, d, eps);
+// One forward pass over `rows` token rows, a decode step or a prefill (n_seqs * S rows), as the layer functions see it.
+// What differs between the two sits behind gemm (the decode GEMM on the tile-major weights, or the wgmma GEMM),
+// attend (the decode attention, or the prefill's) and launch (programmatic dependent launch in the step only).
+struct Pass {
+  Infer* m;
+  bool decode;
+  int rows;
+  bf16 *h, *h2, *nrm, *qkv, *cat, *mid, *act;   // activations [rows, *]; Falcon swaps h and h2 every layer
+  cudaStream_t s;
+  int64_t& nl;                                   // launches
+  int n_seqs = 0, S = 0;                         // prefill only
+  const int32_t* start = nullptr;                // prefill after a cached prefix: DEVICE [n_seqs], else null
+};
+
+enum class Act { none, relu };
+
+template <typename... KArgs, typename... Args>
+void launch(Pass& p, void (*kern)(KArgs...), dim3 grid, dim3 block, Args&&... args) {
+  if (p.decode) launch_pdl(kern, grid, block, 0, p.s, std::forward<Args>(args)...);
+  else kern<<<grid, block, 0, p.s>>>(std::forward<Args>(args)...);
 }
 
-// Everything of one decode step between the H2D of the index vectors and the D2H of the argmax.
+// out [rows, N] (row stride ldo) = act(X W^T + bias) (+ C, same stride); tiled: the step's tile-major copy of W
+void gemm(Pass& p, const bf16* X, int ldx, size_t w, int ldw, int N, int K, bf16* out, int ldo, const uint8_t* tiled,
+          const bf16* C = nullptr, const bf16* bias = nullptr, Act act = Act::none) {
+  if (p.decode) {
+    GemmDecodeOut o;
+    o.out = out; o.ldo = ldo; o.bias = bias; o.act = act == Act::relu ? 2 : 0;
+    if (C) { o.C = C; o.ldc = ldo; }
+    dgemm(p.m, p.s, p.rows, X, ldx, w, ldw, N, K, o, tiled);
+  } else {
+    gemm_bf16_ex(X, false, ldx, p.m->w + w, false, ldw, out, C, false, ldo, p.rows, N, K, 0, bias,
+                 act == Act::relu ? 1 : 0, p.s);
+  }
+  ++p.nl;
+}
+
+// the family's norm of x [rows, d] -> y: RMSNorm (Llama, weight w) or LayerNorm (weight w, bias b)
+void norm(Pass& p, int rows, const bf16* x, size_t w, size_t b, bf16* y) {
+  const Infer* m = p.m;
+  const auto& a = m->a;
+  if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(x, m->w + w, y, nullptr, rows, a.hidden_size, a.norm_eps, p.s);
+  else launch(p, layernorm_kernel, dim3(rows), dim3(256), x, m->w + w, m->w + b, y, a.hidden_size, a.norm_eps);
+  ++p.nl;
+}
+
+// attention of layer l: q / k / v of p.qkv (K / V into the cache) -> p.cat [rows, ld_cat]
+void attend(Pass& p, int l) {
+  Infer* m = p.m;
+  const auto& a = m->a;
+  const int H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim, qkvd = m->qkvd, ldc = m->ld_cat;
+  const int rope = a.family == B200W_FAMILY_OPT ? 0 : 1;
+  if (p.decode) {
+    m->kv.append(l, p.qkv, qkvd, m->inv_freq, m->pos, m->slot, p.rows, H, dh, rope, p.s); ++p.nl;
+    p.nl += decode_attention(m->kv.layer(l), p.qkv, qkvd, m->pos, m->slot, p.rows, H, Hkv, dh, a.max_ctx, m->part_o,
+                             m->part_ml, p.cat, ldc, p.s);
+    return;
+  }
+  // q / k rotated and K / V into the cache; a cold prefill attends over the bf16 activations, on either pool, with
+  // 64-wide heads zero-padded to the 128 attention_fwd takes. After a cached prefix the paged attention reads the
+  // queries in place (on the fp8 pool every key it reads, the suffix's own included, is the quantized one).
+  const bool padded = !p.start && dh != 128;
+  const int dhp = padded ? 128 : dh;
+  bf16* in = padded ? m->pf_qkvp : p.qkv;
+  const int ld_in = padded ? (H + 2 * Hkv) * dhp : qkvd;
+  m->kv.scatter(l, p.qkv, qkvd, in, ld_in, dhp, m->inv_freq, m->pf_len, m->pf_slot, p.rows, p.S, H, dh, rope, p.start,
+                p.s); ++p.nl;
+  const float scale = 1.f / sqrtf(static_cast<float>(dh));
+  if (p.start)
+    attention_fwd_cached(m->kv.layer(l), p.qkv, qkvd, dh, m->pf_slot, p.start, m->pf_len, p.cat, ldc, p.n_seqs, p.S,
+                         H, Hkv, dh, scale, p.s);
+  else
+    attention_fwd(in, ld_in, H * dhp, (H + Hkv) * dhp, padded ? m->pf_attp : p.cat, padded ? H * dhp : ldc, m->pf_lse,
+                  p.n_seqs, p.S, H, Hkv, scale, p.s);
+  ++p.nl;
+  if (padded) {
+    const long long ue = static_cast<long long>(p.rows) * H * (dh / 8);
+    unpad_heads_kernel<<<cdiv(ue, 256), 256, 0, p.s>>>(m->pf_attp, H * dhp, p.cat, ldc, p.rows, H, dh, dhp); ++p.nl;
+  }
+}
+
+void layer_llama(Pass& p, int l) {
+  const auto& w = p.m->lp[l];
+  const int d = p.m->a.hidden_size, f = p.m->a.intermediate_size, qkvd = p.m->qkvd, ldc = p.m->ld_cat;
+  norm(p, p.rows, p.h, w.ln1_w, 0, p.nrm);
+  gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, w.t_qkv);
+  attend(p, l);
+  gemm(p, p.cat, ldc, w.wo, ldc, d, ldc, p.h2, d, w.t_o, p.h);
+  norm(p, p.rows, p.h2, w.ln2_w, 0, p.nrm);
+  gemm(p, p.nrm, d, w.w1, d, 2 * f, d, p.mid, 2 * f, w.t_w1);   // [gate | up]
+  swiglu_fwd(p.mid, p.act, p.rows, f, p.s); ++p.nl;
+  gemm(p, p.act, f, w.w2, f, d, f, p.h, d, w.t_w2, p.h2);
+}
+
+void layer_opt(Pass& p, int l) {
+  const Infer* m = p.m;
+  const auto& w = m->lp[l];
+  const int d = m->a.hidden_size, f = m->a.intermediate_size, qkvd = m->qkvd, ldc = m->ld_cat;
+  norm(p, p.rows, p.h, w.ln1_w, w.ln1_b, p.nrm);
+  gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, w.t_qkv, nullptr, m->w + w.bqkv);
+  attend(p, l);
+  gemm(p, p.cat, ldc, w.wo, ldc, d, ldc, p.h2, d, w.t_o, p.h, m->w + w.bo);
+  norm(p, p.rows, p.h2, w.ln2_w, w.ln2_b, p.nrm);
+  gemm(p, p.nrm, d, w.w1, d, f, d, p.mid, f, w.t_w1, nullptr, m->w + w.b1, Act::relu);
+  gemm(p, p.mid, f, w.w2, f, d, f, p.h, d, w.t_w2, p.h2, m->w + w.b2);
+}
+
+// parallel residual: h' = h + dense(attn(ln)) + W2 gelu(W1 ln)   (modeling_falcon.py FalconDecoderLayer)
+void layer_falcon(Pass& p, int l) {
+  const auto& w = p.m->lp[l];
+  const int d = p.m->a.hidden_size, f = p.m->a.intermediate_size, qd = p.m->qd, qkvd = p.m->qkvd, ldc = p.m->ld_cat;
+  norm(p, p.rows, p.h, w.ln1_w, w.ln1_b, p.nrm);
+  if (p.decode) {
+    // one launch for [q k v | dense_h_to_4h]: the MLP half goes to cat's second window, exact GeLU on it only
+    GemmDecodeOut o;
+    o.out = p.qkv; o.ldo = qkvd;
+    o.out2 = p.cat + qd; o.ldo2 = ldc; o.n_split = qkvd;
+    o.act = 1; o.act_from = qkvd;
+    dgemm(p.m, p.s, p.rows, p.nrm, d, w.wqkv, d, qkvd + f, d, o, w.t_qkv); ++p.nl;
+  } else {
+    gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, nullptr);
+    gemm(p, p.nrm, d, w.w1, d, f, d, p.cat + qd, ldc, nullptr);
+    const long long ge = static_cast<long long>(p.rows) * (f / 8);
+    gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, p.s>>>(p.cat + qd, p.rows, f, ldc); ++p.nl;
+  }
+  attend(p, l);
+  gemm(p, p.cat, ldc, w.wo, ldc, d, ldc, p.h2, d, w.t_o, p.h);   // h' = h + [attn | gelu(h_to_4h)] [dense | 4h_to_h]^T
+  std::swap(p.h, p.h2);
+}
+
+void layers(Pass& p) {
+  const int fam = p.m->a.family;
+  const auto layer = fam == B200W_FAMILY_FALCON ? layer_falcon : fam == B200W_FAMILY_OPT ? layer_opt : layer_llama;
+  for (int l = 0; l < p.m->a.num_layers; ++l) layer(p, l);
+}
+
+// the next token of n rows x [n, d] into the pinned staging: final norm, lm_head (tile-major in the step only), argmax
+void head(Pass& p, const bf16* x, int n) {
+  Infer* m = p.m;
+  const int d = m->a.hidden_size, V = m->a.vocab_size;
+  norm(p, n, x, m->p_lnf_w, m->p_lnf_b, m->nrm);
+  GemmDecodeOut o;
+  o.out = m->logits; o.ldo = V;
+  dgemm(m, p.s, n, m->nrm, d, m->p_lm, d, V, d, o, p.decode ? m->t_lm : nullptr); ++p.nl;
+  launch(p, argmax_kernel, dim3(n), dim3(1024), m->logits, V, m->next); ++p.nl;
+  B200W_CUDA(cudaGetLastError());
+  B200W_CUDA(cudaMemcpyAsync(m->pin_next, m->next, n * 4, cudaMemcpyDeviceToHost, p.s));
+}
+
+// After a step or prefill of n rows has synchronized: the next tokens and the fp32 logits into the caller's host
+// arrays (either may be null). Those rows of m->logits are what b200w_infer_sample draws from next.
+void read_outputs(Infer* m, cudaStream_t s, int n, int32_t* next_tokens, float* logits_out) {
+  if (next_tokens) memcpy(next_tokens, m->pin_next, n * 4);
+  if (logits_out) {
+    const size_t count = static_cast<size_t>(n) * m->a.vocab_size;
+    void* tmp = nullptr;
+    B200W_CUDA(cudaMalloc(&tmp, count * 4));
+    cast_bf16_to_f32(m->logits, static_cast<float*>(tmp), count, s);
+    B200W_CUDA(cudaStreamSynchronize(s));
+    B200W_CUDA(cudaMemcpy(logits_out, tmp, count * 4, cudaMemcpyDeviceToHost));
+    cudaFree(tmp);
+  }
+  m->logits_rows = n;
+}
+
+// Everything of one decode step between the H2D of the index vectors and the D2H of the next tokens. Nothing is
+// carried from one step to the next in h or h2: each step starts again from the embedding.
 void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   const auto& a = m->a;
-  const int B = m->max_batch;
-  const int d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size;
-  const int qd = m->qd, qkvd = m->qkvd, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim;
-  const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
-  B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin, n * 4, cudaMemcpyHostToDevice, s));
-  B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin + B, n * 4, cudaMemcpyHostToDevice, s));
-  B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin + 2 * B, n * 4, cudaMemcpyHostToDevice, s));
-  bf16* h = m->h;
-  bf16* h2 = m->h2;
-  if (opt) infer_embed_pos_kernel<<<n, 128, 0, s>>>(m->tok, m->pos, m->w + m->p_embed, m->w + m->p_pos, h, d, 2);
-  else embed_fwd(m->tok, m->w + m->p_embed, nullptr, h, n, d, V, 1, 0, s);
+  B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin_tok, n * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin_pos, n * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin_slot, n * 4, cudaMemcpyHostToDevice, s));
+  Pass p{m, true, n, m->h, m->h2, m->nrm, m->qkv, m->cat, m->mid, m->act, s, nl};
+  if (a.family == B200W_FAMILY_OPT)
+    infer_embed_pos_kernel<<<n, 128, 0, s>>>(m->tok, m->pos, m->w + m->p_embed, m->w + m->p_pos, p.h, a.hidden_size, 2);
+  else
+    embed_fwd(m->tok, m->w + m->p_embed, nullptr, p.h, n, a.hidden_size, a.vocab_size, 1, 0, s);
   ++nl;
   B200W_CUDA(cudaGetLastError());
-  for (int l = 0; l < a.num_layers; ++l) {
-    const auto& p = m->lp[l];
-    if (falcon) {
-      // parallel residual: h' = h + dense(attn(ln)) + W2 gelu(W1 ln)   (modeling_falcon.py FalconDecoderLayer)
-      launch_ln(s, n, h, m->w + p.ln1_w, m->w + p.ln1_b, m->nrm, d, a.norm_eps); ++nl;
-      GemmDecodeOut o1;
-      o1.out = m->qkv; o1.ldo = qkvd;
-      o1.out2 = m->cat + qd; o1.ldo2 = m->ld_cat; o1.n_split = qkvd;
-      o1.act = 1; o1.act_from = qkvd;   // exact GeLU on the MLP half only
-      dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd + f, d, o1, m->lt[l].qkv); ++nl;
-      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 1, s); ++nl;
-      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
-                             m->part_ml, m->cat, m->ld_cat, s);
-      GemmDecodeOut o2;
-      o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
-      dgemm(m, s, n, m->cat, m->ld_cat, p.wo, m->ld_cat, d, m->ld_cat, o2, m->lt[l].o); ++nl;
-      std::swap(h, h2);
-    } else if (opt) {
-      launch_ln(s, n, h, m->w + p.ln1_w, m->w + p.ln1_b, m->nrm, d, a.norm_eps); ++nl;
-      GemmDecodeOut o1;
-      o1.out = m->qkv; o1.ldo = qkvd; o1.bias = m->w + p.bqkv;
-      dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 0, s); ++nl;
-      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
-                             m->part_ml, m->cat, qd, s);
-      GemmDecodeOut o2;
-      o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d; o2.bias = m->w + p.bo;
-      dgemm(m, s, n, m->cat, qd, p.wo, qd, d, qd, o2, m->lt[l].o); ++nl;
-      launch_ln(s, n, h2, m->w + p.ln2_w, m->w + p.ln2_b, m->nrm, d, a.norm_eps); ++nl;
-      GemmDecodeOut o3;
-      o3.out = m->mid; o3.ldo = f; o3.bias = m->w + p.b1; o3.act = 2;
-      dgemm(m, s, n, m->nrm, d, p.w1, d, f, d, o3, m->lt[l].w1); ++nl;
-      GemmDecodeOut o4;
-      o4.out = h; o4.ldo = d; o4.C = h2; o4.ldc = d; o4.bias = m->w + p.b2;
-      dgemm(m, s, n, m->mid, f, p.w2, f, d, f, o4, m->lt[l].w2); ++nl;
-    } else {
-      rmsnorm_fwd(h, m->w + p.ln1_w, m->nrm, nullptr, n, d, a.norm_eps, s); ++nl;
-      GemmDecodeOut o1;
-      o1.out = m->qkv; o1.ldo = qkvd;
-      dgemm(m, s, n, m->nrm, d, p.wqkv, d, qkvd, d, o1, m->lt[l].qkv); ++nl;
-      m->kv.append(l, m->qkv, qkvd, m->inv_freq, m->pos, m->slot, n, H, dh, 1, s); ++nl;
-      nl += decode_attention(m->kv.layer(l), m->qkv, qkvd, m->pos, m->slot, n, H, Hkv, dh, a.max_ctx, m->part_o,
-                             m->part_ml, m->cat, qd, s);
-      GemmDecodeOut o2;
-      o2.out = h2; o2.ldo = d; o2.C = h; o2.ldc = d;
-      dgemm(m, s, n, m->cat, qd, p.wo, qd, d, qd, o2, m->lt[l].o); ++nl;
-      rmsnorm_fwd(h2, m->w + p.ln2_w, m->nrm, nullptr, n, d, a.norm_eps, s); ++nl;
-      GemmDecodeOut o3;
-      o3.out = m->mid; o3.ldo = 2 * f;
-      dgemm(m, s, n, m->nrm, d, p.w1, d, 2 * f, d, o3, m->lt[l].w1); ++nl;
-      swiglu_fwd(m->mid, m->act, n, f, s); ++nl;
-      GemmDecodeOut o4;
-      o4.out = h; o4.ldo = d; o4.C = h2; o4.ldc = d;
-      dgemm(m, s, n, m->act, f, p.w2, f, d, f, o4, m->lt[l].w2); ++nl;
-    }
-  }
-  if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + m->p_lnf_w, m->nrm, nullptr, n, d, a.norm_eps, s);
-  else launch_ln(s, n, h, m->w + m->p_lnf_w, m->w + m->p_lnf_b, m->nrm, d, a.norm_eps);
-  ++nl;
-  GemmDecodeOut ol;
-  ol.out = m->logits; ol.ldo = V;
-  dgemm(m, s, n, m->nrm, d, m->p_lm, d, V, d, ol, m->t_lm); ++nl;
-  launch_pdl(argmax_kernel, dim3(n), dim3(1024), 0, s, m->logits, V, m->next); ++nl;
-  B200W_CUDA(cudaGetLastError());
-  B200W_CUDA(cudaMemcpyAsync(m->pin + 3 * B, m->next, n * 4, cudaMemcpyDeviceToHost, s));
-  // (h / h2 swap per Falcon layer: with an odd layer count the stream ends in m->h2 -- nothing is carried
-  // from one step to the next in either buffer, the next step starts again from the embedding)
+  layers(p);
+  head(p, p.h, n);
 }
 
 void ensure_prefill(Infer* m, size_t T) {
@@ -1820,11 +1913,9 @@ void ensure_prefill(Infer* m, size_t T) {
   const auto& a = m->a;
   const size_t d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads;
   const size_t dhp = 128, HT = H + 2 * Hkv;
-  for (void* p : {static_cast<void*>(m->pf_h), static_cast<void*>(m->pf_h2), static_cast<void*>(m->pf_nrm),
-                  static_cast<void*>(m->pf_qkv), static_cast<void*>(m->pf_qkvp), static_cast<void*>(m->pf_attp),
-                  static_cast<void*>(m->pf_cat), static_cast<void*>(m->pf_mid), static_cast<void*>(m->pf_act),
-                  static_cast<void*>(m->pf_lse), static_cast<void*>(m->pf_tok), static_cast<void*>(m->pf_pos)})
-    if (p) m->release(p);
+  for (void* p : std::initializer_list<void*>{m->pf_h, m->pf_h2, m->pf_nrm, m->pf_qkv, m->pf_qkvp, m->pf_attp,
+                                              m->pf_cat, m->pf_mid, m->pf_act, m->pf_lse, m->pf_tok, m->pf_pos})
+    m->release(p);
   m->pf_h = m->alloc<bf16>(T * d);
   m->pf_h2 = m->alloc<bf16>(T * d);
   m->pf_nrm = m->alloc<bf16>(T * d);
@@ -1843,18 +1934,10 @@ void ensure_prefill(Infer* m, size_t T) {
   m->pf_lse = m->alloc<float>(H * T);
   m->pf_tok = m->alloc<int32_t>(T);
   m->pf_pos = m->alloc<int32_t>(T);
-  m->pf_cap = T;
-}
-
-// pinned staging of one prefill call: tokens [T] | lengths | slots | last rows | starts [max_batch each] |
-// positions [T]
-void ensure_prefill_pin(Infer* m, size_t T) {
-  const size_t need = 2 * T + 4 * static_cast<size_t>(m->max_batch);
-  if (m->pf_pin_cap >= need) return;
   if (m->pf_pin) cudaFreeHost(m->pf_pin);
   m->pf_pin = nullptr;
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pf_pin), need * sizeof(int32_t)));
-  m->pf_pin_cap = need;
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pf_pin), (2 * T + 4 * m->max_batch) * sizeof(int32_t)));
+  m->pf_cap = T;
 }
 
 constexpr int LP_CHUNK = 1024;   // prompt rows per lm_head GEMM of prompt scoring
@@ -1898,9 +1981,7 @@ void ensure_scoring(Infer* m, size_t T) {
     m->lp_chunk_rows = rows;
   }
   if (T > m->lp_cap) {
-    for (void* p : {static_cast<void*>(m->lp_tgt), static_cast<void*>(m->lp_top), static_cast<void*>(m->lp_ids),
-                    static_cast<void*>(m->lp_targets)})
-      if (p) m->release(p);
+    for (void* p : std::initializer_list<void*>{m->lp_tgt, m->lp_top, m->lp_ids, m->lp_targets}) m->release(p);
     m->lp_tgt = m->lp_top = nullptr;
     m->lp_ids = m->lp_targets = nullptr;
     m->lp_cap = 0;
@@ -1910,6 +1991,105 @@ void ensure_scoring(Infer* m, size_t T) {
     m->lp_targets = m->alloc<int32_t>(T);
     m->lp_cap = T;
   }
+}
+
+// The arguments of a prefill call, checked before any GPU work. Row b of `tokens` [n_seqs, S] holds positions
+// [start_b, lengths[b]) of its prompt, start_b = starts ? starts[b] : 0.
+void check_prefill(Infer* m, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
+                   const int32_t* slots, int n_seqs, int S) {
+  const auto& a = m->a;
+  B200W_CHECK(tokens && lengths && slots && n_seqs >= 1 && n_seqs <= m->max_batch, "bad prefill batch");
+  B200W_CHECK(S >= 128 && S % 128 == 0, "padded_len must be a positive multiple of 128");
+  const size_t T = static_cast<size_t>(n_seqs) * S;
+  B200W_CHECK(T <= (1u << 20), "prefill batch too large");
+  for (int b = 0; b < n_seqs; ++b) {
+    const int start = starts ? starts[b] : 0;
+    if (starts)
+      B200W_CHECK(start > 0 && start % KV_PAGE == 0 && start < lengths[b],
+                  "a cached prefix must be a positive multiple of 128 below the prompt length");
+    B200W_CHECK(lengths[b] >= 1 && lengths[b] - start <= S && lengths[b] <= a.max_ctx, "bad prompt length");
+    B200W_CHECK(slots[b] >= 0 && slots[b] < m->max_batch, "bad cache slot");
+    m->kv.check_slot(slots[b], lengths[b], start);
+  }
+  if (m->kv.paged) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
+  for (size_t i = 0; i < T; ++i)
+    B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
+  if (a.family == B200W_FAMILY_OPT && !starts)
+    B200W_CHECK(S <= a.max_positions, "OPT: padded_len exceeds the position table");
+}
+
+// A prefill call's index vectors through the pinned staging to the device.
+void stage_prefill(Infer* m, cudaStream_t s, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
+                   const int32_t* slots, int n_seqs, int S, bool score) {
+  const size_t T = static_cast<size_t>(n_seqs) * S;
+  const bool opt = m->a.family == B200W_FAMILY_OPT;
+  // the staging's regions: tokens [T] | lengths | slots | last rows | starts [max_batch each] | one value per row [T],
+  // OPT's learned position after a cached prefix or the target a cold prefill scores
+  const int B = m->max_batch;
+  int32_t *pin_tok = m->pf_pin, *pin_len = pin_tok + T, *pin_slot = pin_len + B, *pin_last = pin_slot + B,
+          *pin_start = pin_last + B, *pin_row = pin_start + B;
+  memcpy(pin_tok, tokens, T * 4);
+  for (int b = 0; b < n_seqs; ++b) {
+    const int start = starts ? starts[b] : 0;
+    const size_t r0 = static_cast<size_t>(b) * S;
+    pin_len[b] = lengths[b];
+    pin_slot[b] = slots[b];
+    pin_last[b] = b * S + lengths[b] - start - 1;   // row of the last real token
+    pin_start[b] = start;
+    // OPT after a cached prefix: the learned position of each row; padding rows repeat the last real one, so that
+    // they stay inside the position table
+    if (starts && opt)
+      for (int p = 0; p < S; ++p) pin_row[r0 + p] = std::min(start + p, lengths[b] - 1);
+    // scoring (cold prefills only, so the positions' region is free): row p predicts token p + 1
+    if (score)
+      for (int p = 0; p < S; ++p) pin_row[r0 + p] = p + 1 < lengths[b] ? tokens[r0 + p + 1] : -1;
+  }
+  B200W_CUDA(cudaMemcpyAsync(m->pf_tok, pin_tok, T * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->pf_len, pin_len, n_seqs * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->pf_slot, pin_slot, n_seqs * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->pf_last, pin_last, n_seqs * 4, cudaMemcpyHostToDevice, s));
+  if (starts) {
+    B200W_CUDA(cudaMemcpyAsync(m->pf_start, pin_start, n_seqs * 4, cudaMemcpyHostToDevice, s));
+    if (opt) B200W_CUDA(cudaMemcpyAsync(m->pf_pos, pin_row, T * 4, cudaMemcpyHostToDevice, s));
+  }
+  if (score) B200W_CUDA(cudaMemcpyAsync(m->lp_targets, pin_row, T * 4, cudaMemcpyHostToDevice, s));
+}
+
+// Prompt scoring after the layers of a cold prefill, into b200w_infer_prefill_logprobs' prompt outputs [n_seqs, S
+// (, top_k)]: the final norm over every row into p.nrm (dead since the last layer), then lm_head and the log-softmax
+// in chunks of rows through lp_chunk -- the rows [0, lengths[b] - 1) of each sequence, whose next token is known.
+// Row p - 1's distribution is position p's, so the rows go one position on; positions 0 and >= lengths[b] have none.
+void score_prompts(Pass& p, const int32_t* lengths, int top_k, float* prompt_lp, int32_t* prompt_top_ids,
+                   float* prompt_top_lp) {
+  const Infer* m = p.m;
+  const int d = m->a.hidden_size, V = m->a.vocab_size;
+  norm(p, p.rows, p.h, m->p_lnf_w, m->p_lnf_b, p.nrm);
+  const int C = static_cast<int>(m->lp_chunk_rows);
+  for (int b = 0; b < p.n_seqs; ++b)
+    for (int p0 = 0; p0 < lengths[b] - 1; p0 += C) {
+      const int rows = std::min(C, lengths[b] - 1 - p0);
+      const size_t r0 = static_cast<size_t>(b) * p.S + p0;
+      gemm_bf16_ex(p.nrm + r0 * d, false, d, m->w + m->p_lm, false, d, m->lp_chunk, nullptr, false, V, rows, V, d, 0,
+                   nullptr, 0, p.s); ++p.nl;
+      logprobs(m->lp_chunk, V, rows, V, m->lp_targets + r0, top_k, nullptr, m->lp_tgt + r0, nullptr,
+               m->lp_ids + r0 * top_k, m->lp_top + r0 * top_k, p.s); ++p.nl;
+    }
+  B200W_CUDA(cudaStreamSynchronize(p.s));
+  const size_t T = p.rows, k = top_k;
+  if (prompt_lp) B200W_CUDA(cudaMemcpy(prompt_lp + 1, m->lp_tgt, (T - 1) * 4, cudaMemcpyDeviceToHost));
+  if (prompt_top_ids && k)
+    B200W_CUDA(cudaMemcpy(prompt_top_ids + k, m->lp_ids, (T - 1) * k * 4, cudaMemcpyDeviceToHost));
+  if (prompt_top_lp && k) B200W_CUDA(cudaMemcpy(prompt_top_lp + k, m->lp_top, (T - 1) * k * 4, cudaMemcpyDeviceToHost));
+  for (int b = 0; b < p.n_seqs; ++b)
+    for (int i = 0; i < p.S; ++i) {
+      if (i >= 1 && i < lengths[b]) continue;
+      const size_t r = static_cast<size_t>(b) * p.S + i;
+      if (prompt_lp) prompt_lp[r] = 0.f;
+      for (size_t j = 0; j < k; ++j) {
+        if (prompt_top_ids) prompt_top_ids[r * k + j] = -1;
+        if (prompt_top_lp) prompt_top_lp[r * k + j] = 0.f;
+      }
+    }
 }
 
 Infer* paged_model(b200w_ctx* ctx) {
@@ -1951,7 +2131,6 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->a = *arch;
   m->max_batch = max_batch;
   if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
-  m->lt.resize(arch->num_layers);   // all-null when the tiled copies are disabled
   build(m.get());
   const auto& a = m->a;
   const size_t B = max_batch, d = a.hidden_size, f = a.intermediate_size;
@@ -1972,7 +2151,6 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
     m->pf_limit = static_cast<size_t>(prefill_tokens);
     ensure_prefill(m.get(), m->pf_limit);
-    ensure_prefill_pin(m.get(), m->pf_limit);
   }
   if (a.num_heads / a.num_kv_heads >= 4) {
     m->part_o = m->alloc<float>(B * a.num_heads * m->kv.nsplit * a.head_dim);
@@ -1986,7 +2164,10 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   m->pf_slot = m->alloc<int32_t>(B);
   m->pf_last = m->alloc<int32_t>(B);
   m->pf_start = m->alloc<int32_t>(B);
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin), 4 * B * sizeof(int32_t)));
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin_tok), 4 * B * sizeof(int32_t)));
+  m->pin_pos = m->pin_tok + B;
+  m->pin_slot = m->pin_tok + 2 * B;
+  m->pin_next = m->pin_tok + 3 * B;
   m->inv_freq = m->alloc<float>(a.head_dim / 2);
   const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + qd + 2 * kd, d});
   m->ws = m->alloc<float>(B * max_n);
@@ -2321,10 +2502,9 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     }
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
-    const int B = m->max_batch, V = a.vocab_size;
-    memcpy(m->pin, tokens, n * 4);
-    memcpy(m->pin + B, positions, n * 4);
-    memcpy(m->pin + 2 * B, slots, n * 4);
+    memcpy(m->pin_tok, tokens, n * 4);
+    memcpy(m->pin_pos, positions, n * 4);
+    memcpy(m->pin_slot, slots, n * 4);
     if (next) ensure_next_logprobs(m);
     ensure_tiled(m, s);   // no-op unless the weights changed since the last step
     int64_t step_launches = 0;
@@ -2359,17 +2539,7 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     // outside the graph, on the logits it left: the captured step is the same with and without log-probabilities
     if (next) next_logprobs(m, s, n, next, nl);
     B200W_CUDA(cudaStreamSynchronize(s));
-    if (next_tokens) memcpy(next_tokens, m->pin + 3 * B, n * 4);
-    if (logits_out) {
-      void* tmp = nullptr;
-      B200W_CUDA(cudaMalloc(&tmp, static_cast<size_t>(n) * V * 4));
-      cast_bf16_to_f32(m->logits, static_cast<float*>(tmp), static_cast<size_t>(n) * V, s);
-      B200W_CUDA(cudaStreamSynchronize(s));
-      B200W_CUDA(cudaMemcpy(logits_out, tmp, static_cast<size_t>(n) * V * 4, cudaMemcpyDeviceToHost));
-      cudaFree(tmp);
-    }
-    B200W_CUDA(cudaStreamSynchronize(s));
-    m->logits_rows = n;
+    read_outputs(m, s, n, next_tokens, logits_out);
   });
 }
 
@@ -2383,16 +2553,13 @@ int b200w_infer_step_logprobs(b200w_ctx* ctx, const int32_t* tokens, const int32
   return step_impl(ctx, tokens, positions, slots, n, next_tokens, logits_out, next);
 }
 
-// Prompt ingestion in ONE pass (round 1 fed prompts through b200w_infer_step one token per weight
-// sweep): big-M wgmma GEMMs over all n_seqs * padded_len tokens, the training flash-attention
-// forward (causal within each sequence), K/V of the real positions written to the cache slots, and the
-// greedy token after each prompt. Padding tokens sit AFTER the real ones, so causality keeps them
-// from influencing any real position.
-// b200w_infer_prefill (starts == nullptr) and b200w_infer_prefill_cached: row b of `tokens` holds positions
-// [start_b, lengths[b]) of its prompt, start_b = starts ? starts[b] : 0.
+// Prompt ingestion in one pass: big-M wgmma GEMMs over all n_seqs * padded_len tokens, the training
+// flash-attention forward (causal within each sequence), K/V of the real positions written to the cache slots, and
+// the greedy token after each prompt. Padding tokens sit AFTER the real ones, so causality keeps them from
+// influencing any real position. b200w_infer_prefill (starts == nullptr), b200w_infer_prefill_cached, and
 // b200w_infer_prefill_logprobs (cold only): `next` and the prompt outputs as that call documents.
 static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* starts, const int32_t* lengths,
-                        const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens, float* logits_out,
+                        const int32_t* slots, int n_seqs, int S, int32_t* next_tokens, float* logits_out,
                         const b200w_logprobs* next = nullptr, float* prompt_lp = nullptr,
                         int32_t* prompt_top_ids = nullptr, float* prompt_top_lp = nullptr) {
   return iguard(ctx, [&] {
@@ -2401,199 +2568,31 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     const auto& a = m->a;
     const int top_k = check_logprobs(next);
     const bool score = prompt_lp || (top_k && (prompt_top_ids || prompt_top_lp));
-    B200W_CHECK(tokens && lengths && slots && n_seqs >= 1 && n_seqs <= m->max_batch, "bad prefill batch");
-    B200W_CHECK(padded_len >= 128 && padded_len % 128 == 0, "padded_len must be a positive multiple of 128");
-    const int S = padded_len;
+    check_prefill(m, tokens, starts, lengths, slots, n_seqs, S);
     const size_t T = static_cast<size_t>(n_seqs) * S;
-    B200W_CHECK(T <= (1u << 20), "prefill batch too large");
-    for (int b = 0; b < n_seqs; ++b) {
-      const int start = starts ? starts[b] : 0;
-      if (starts)
-        B200W_CHECK(start > 0 && start % KV_PAGE == 0 && start < lengths[b],
-                    "a cached prefix must be a positive multiple of 128 below the prompt length");
-      B200W_CHECK(lengths[b] >= 1 && lengths[b] - start <= S && lengths[b] <= a.max_ctx, "bad prompt length");
-      B200W_CHECK(slots[b] >= 0 && slots[b] < m->max_batch, "bad cache slot");
-      m->kv.check_slot(slots[b], lengths[b], start);
-    }
-    if (m->kv.paged) B200W_CHECK(T <= m->pf_limit, "n_seqs * padded_len exceeds the prefill workspace (prefill_tokens)");
-    for (size_t i = 0; i < T; ++i)
-      B200W_CHECK(tokens[i] >= 0 && tokens[i] < a.vocab_size, "token id outside the vocabulary");
-    if (a.family == B200W_FAMILY_OPT && !starts)
-      B200W_CHECK(S <= a.max_positions, "OPT: padded_len exceeds the position table");
     cudaStream_t s = ctx_stream(ctx);
-    int64_t& nl = ctx_launches(ctx);
     ensure_prefill(m, T);
-    ensure_prefill_pin(m, T);
     if (next) ensure_next_logprobs(m);
     if (score) ensure_scoring(m, T);
-    const int B = m->max_batch;
-    int32_t* pin = m->pf_pin;
-    memcpy(pin, tokens, T * 4);
-    for (int b = 0; b < n_seqs; ++b) {
-      const int start = starts ? starts[b] : 0;
-      pin[T + b] = lengths[b];
-      pin[T + B + b] = slots[b];
-      pin[T + 2 * B + b] = b * S + lengths[b] - start - 1;   // row of the last real token
-      pin[T + 3 * B + b] = start;
-      // OPT after a cached prefix: the learned position of each row; padding rows repeat the last real one, so that
-      // they stay inside the position table
-      if (starts && a.family == B200W_FAMILY_OPT)
-        for (int p = 0; p < S; ++p)
-          pin[T + 4 * B + static_cast<size_t>(b) * S + p] = std::min(start + p, lengths[b] - 1);
-      // scoring (cold prefills only, so the positions' staging is free): row p predicts token p + 1
-      if (score)
-        for (int p = 0; p < S; ++p) {
-          const size_t r = static_cast<size_t>(b) * S + p;
-          pin[T + 4 * B + r] = p + 1 < lengths[b] ? tokens[r + 1] : -1;
-        }
-    }
-    B200W_CUDA(cudaMemcpyAsync(m->pf_tok, pin, T * 4, cudaMemcpyHostToDevice, s));
-    B200W_CUDA(cudaMemcpyAsync(m->pf_len, pin + T, n_seqs * 4, cudaMemcpyHostToDevice, s));
-    B200W_CUDA(cudaMemcpyAsync(m->pf_slot, pin + T + B, n_seqs * 4, cudaMemcpyHostToDevice, s));
-    B200W_CUDA(cudaMemcpyAsync(m->pf_last, pin + T + 2 * B, n_seqs * 4, cudaMemcpyHostToDevice, s));
-    if (starts) {
-      B200W_CUDA(cudaMemcpyAsync(m->pf_start, pin + T + 3 * B, n_seqs * 4, cudaMemcpyHostToDevice, s));
-      if (a.family == B200W_FAMILY_OPT)
-        B200W_CUDA(cudaMemcpyAsync(m->pf_pos, pin + T + 4 * B, T * 4, cudaMemcpyHostToDevice, s));
-    }
-    if (score) B200W_CUDA(cudaMemcpyAsync(m->lp_targets, pin + T + 4 * B, T * 4, cudaMemcpyHostToDevice, s));
-
-    const int d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads, dh = a.head_dim,
-              V = a.vocab_size;
-    const int qd = m->qd, qkvd = m->qkvd, ldc = m->ld_cat;
-    const bool falcon = a.family == B200W_FAMILY_FALCON, opt = a.family == B200W_FAMILY_OPT;
-    const int dhp = 128, HT = H + 2 * Hkv;
-    const bool padded = dh != dhp;
-    const float scale = 1.f / sqrtf(static_cast<float>(dh));
-      const int Ti = static_cast<int>(T);
-    auto G = [&](const void* A, int lda, size_t woff, int ldw, void* D, const void* C, int ldd, int N, int K,
-                 const void* bias = nullptr, int act = 0) {
-      gemm_bf16_ex(A, false, lda, m->w + woff, false, ldw, D, C, false, ldd, Ti, N, K, 0, bias, act, s); ++nl;
-    };
-    bf16* h = m->pf_h;
-    bf16* h2 = m->pf_h2;
+    stage_prefill(m, s, tokens, starts, lengths, slots, n_seqs, S, score);
+    Pass p{m, false, static_cast<int>(T), m->pf_h, m->pf_h2, m->pf_nrm, m->pf_qkv, m->pf_cat, m->pf_mid, m->pf_act, s,
+           ctx_launches(ctx), n_seqs, S, starts ? m->pf_start : nullptr};
+    const bool opt = a.family == B200W_FAMILY_OPT;
     if (opt && starts)
-      infer_embed_pos_kernel<<<Ti, 128, 0, s>>>(m->pf_tok, m->pf_pos, m->w + m->p_embed, m->w + m->p_pos, h, d, 2);
+      infer_embed_pos_kernel<<<p.rows, 128, 0, s>>>(m->pf_tok, m->pf_pos, m->w + m->p_embed, m->w + m->p_pos, p.h,
+                                                    a.hidden_size, 2);
     else
-      embed_fwd(m->pf_tok, m->w + m->p_embed, opt ? m->w + m->p_pos : nullptr, h, Ti, d, V, S, opt ? 2 : 0, s);
-    ++nl;
-    for (int l = 0; l < a.num_layers; ++l) {
-      const auto& p = m->lp[l];
-      const KVLayer c = m->kv.layer(l);
-      auto scatter = [&](bf16* dst, int ld_dst, int dh_dst, const int32_t* start) {
-        m->kv.scatter(l, m->pf_qkv, qkvd, dst, ld_dst, dh_dst, m->inv_freq, m->pf_len, m->pf_slot, Ti, S, H, dh,
-                      opt ? 0 : 1, start, s);
-        ++nl;
-      };
-      if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + p.ln1_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s);
-      else layernorm_kernel<<<Ti, 256, 0, s>>>(h, m->w + p.ln1_w, m->w + p.ln1_b, m->pf_nrm, d, a.norm_eps);
-      ++nl;
-      G(m->pf_nrm, d, p.wqkv, d, m->pf_qkv, nullptr, qkvd, qkvd, d, opt ? m->w + p.bqkv : nullptr, 0);
-      if (falcon) {  // the MLP half of the parallel block reads the same LayerNorm output
-        G(m->pf_nrm, d, p.w1, d, m->pf_cat + qd, nullptr, ldc, f, d);
-        const long long ge = static_cast<long long>(Ti) * (f / 8);
-        gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, s>>>(m->pf_cat + qd, Ti, f, ldc); ++nl;
-      }
-      if (starts) {
-        // after a cached prefix: q / k rotated in place at their positions, the suffix K/V into the slot's pages, then
-        // the paged attention reads the queries at their own width and writes the o-projection's input directly
-        // (on the fp8 pool every key it reads, the suffix's own included, is the quantized one)
-        scatter(m->pf_qkv, qkvd, dh, m->pf_start);
-        attention_fwd_cached(c, m->pf_qkv, qkvd, dh, m->pf_slot, m->pf_start, m->pf_len, m->pf_cat, ldc, n_seqs, S, H, Hkv,
-                             dh, scale, s); ++nl;
-      } else {
-        // a cold prefill attends over the bf16 activations, on either pool
-        bf16* att_in = padded ? m->pf_qkvp : m->pf_qkv;
-        const int ld_in = padded ? HT * dhp : qkvd;
-        scatter(att_in, ld_in, dhp, nullptr);
-        bf16* att_out = padded ? m->pf_attp : m->pf_cat;
-        const int ld_out = padded ? H * dhp : ldc;
-        attention_fwd(att_in, ld_in, H * dhp, (H + Hkv) * dhp, att_out, ld_out, m->pf_lse, n_seqs, S, H, Hkv, scale, s);
-        ++nl;
-        if (padded) {
-          const long long ue = static_cast<long long>(Ti) * H * (dh / 8);
-          unpad_heads_kernel<<<cdiv(ue, 256), 256, 0, s>>>(m->pf_attp, H * dhp, m->pf_cat, ldc, Ti, H, dh, dhp); ++nl;
-        }
-      }
-      if (falcon) {
-        G(m->pf_cat, ldc, p.wo, ldc, h2, h, d, d, ldc);   // h' = h + [attn | gelu(h_to_4h)] [dense | 4h_to_h]^T
-        std::swap(h, h2);
-      } else if (opt) {
-        G(m->pf_cat, qd, p.wo, qd, h2, h, d, d, qd, m->w + p.bo, 0);
-        layernorm_kernel<<<Ti, 256, 0, s>>>(h2, m->w + p.ln2_w, m->w + p.ln2_b, m->pf_nrm, d, a.norm_eps); ++nl;
-        G(m->pf_nrm, d, p.w1, d, m->pf_mid, nullptr, f, f, d, m->w + p.b1, 1);   // bias + ReLU in the epilogue
-        G(m->pf_mid, f, p.w2, f, h, h2, d, d, f, m->w + p.b2, 0);
-      } else {
-        G(m->pf_cat, qd, p.wo, qd, h2, h, d, d, qd);
-        rmsnorm_fwd(h2, m->w + p.ln2_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s); ++nl;
-        G(m->pf_nrm, d, p.w1, d, m->pf_mid, nullptr, 2 * f, 2 * f, d);
-        swiglu_fwd(m->pf_mid, m->pf_act, Ti, f, s); ++nl;
-        G(m->pf_act, f, p.w2, f, h, h2, d, d, f);
-      }
-    }
-    // the token after each prompt: final norm + lm_head on the last real row of every sequence
-    gather_rows_kernel<<<n_seqs, 128, 0, s>>>(h, m->pf_last, m->h2, d); ++nl;
-    if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(m->h2, m->w + m->p_lnf_w, m->nrm, nullptr, n_seqs, d, a.norm_eps, s);
-    else layernorm_kernel<<<n_seqs, 256, 0, s>>>(m->h2, m->w + m->p_lnf_w, m->w + m->p_lnf_b, m->nrm, d, a.norm_eps);
-    ++nl;
-    GemmDecodeOut ol;
-    ol.out = m->logits; ol.ldo = V;
-    gemm_decode_ex(m->nrm, d, m->w + m->p_lm, d, ol, m->ws, m->counters, n_seqs, V, d, s); ++nl;
-    argmax_kernel<<<n_seqs, 1024, 0, s>>>(m->logits, V, m->next); ++nl;
-    B200W_CUDA(cudaGetLastError());
-    B200W_CUDA(cudaMemcpyAsync(m->pin + 3 * B, m->next, n_seqs * 4, cudaMemcpyDeviceToHost, s));
-    if (next) next_logprobs(m, s, n_seqs, next, nl);
-    std::vector<float> row_lp, row_top;
-    std::vector<int32_t> row_ids;
-    if (score) {
-      // the final norm over every row into pf_nrm (dead since the last layer), then lm_head and the log-softmax in
-      // chunks of rows through lp_chunk: the rows [0, lengths[b] - 1) of each sequence, whose next token is known
-      if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(h, m->w + m->p_lnf_w, m->pf_nrm, nullptr, Ti, d, a.norm_eps, s);
-      else layernorm_kernel<<<Ti, 256, 0, s>>>(h, m->w + m->p_lnf_w, m->w + m->p_lnf_b, m->pf_nrm, d, a.norm_eps);
-      ++nl;
-      const int C = static_cast<int>(m->lp_chunk_rows);
-      for (int b = 0; b < n_seqs; ++b)
-        for (int p0 = 0; p0 < lengths[b] - 1; p0 += C) {
-          const int rows = std::min(C, lengths[b] - 1 - p0);
-          const size_t r0 = static_cast<size_t>(b) * S + p0;
-          gemm_bf16_ex(m->pf_nrm + r0 * d, false, d, m->w + m->p_lm, false, d, m->lp_chunk, nullptr, false, V, rows, V,
-                       d, 0, nullptr, 0, s); ++nl;
-          logprobs(m->lp_chunk, V, rows, V, m->lp_targets + r0, top_k, nullptr, m->lp_tgt + r0, nullptr,
-                   m->lp_ids + r0 * top_k, m->lp_top + r0 * top_k, s); ++nl;
-        }
-      row_lp.resize(T);
-      row_ids.resize(T * top_k);
-      row_top.resize(T * top_k);
-      B200W_CUDA(cudaMemcpyAsync(row_lp.data(), m->lp_tgt, T * 4, cudaMemcpyDeviceToHost, s));
-      if (top_k) {
-        B200W_CUDA(cudaMemcpyAsync(row_ids.data(), m->lp_ids, T * top_k * 4, cudaMemcpyDeviceToHost, s));
-        B200W_CUDA(cudaMemcpyAsync(row_top.data(), m->lp_top, T * top_k * 4, cudaMemcpyDeviceToHost, s));
-      }
-    }
+      embed_fwd(m->pf_tok, m->w + m->p_embed, opt ? m->w + m->p_pos : nullptr, p.h, p.rows, a.hidden_size,
+                a.vocab_size, S, opt ? 2 : 0, s);
+    ++p.nl;
+    layers(p);
+    // the token after each prompt: the head on the last real row of every sequence
+    gather_rows_kernel<<<n_seqs, 128, 0, s>>>(p.h, m->pf_last, m->h2, a.hidden_size); ++p.nl;
+    head(p, m->h2, n_seqs);
+    if (next) next_logprobs(m, s, n_seqs, next, p.nl);
+    if (score) score_prompts(p, lengths, top_k, prompt_lp, prompt_top_ids, prompt_top_lp);
     B200W_CUDA(cudaStreamSynchronize(s));
-    if (score) {
-      // row p - 1's distribution is position p's; positions 0 and >= lengths[b] have none
-      for (int b = 0; b < n_seqs; ++b)
-        for (int p = 0; p < S; ++p) {
-          const size_t r = static_cast<size_t>(b) * S + p;
-          const bool has = p >= 1 && p < lengths[b];
-          if (prompt_lp) prompt_lp[r] = has ? row_lp[r - 1] : 0.f;
-          for (int j = 0; j < top_k; ++j) {
-            if (prompt_top_ids) prompt_top_ids[r * top_k + j] = has ? row_ids[(r - 1) * top_k + j] : -1;
-            if (prompt_top_lp) prompt_top_lp[r * top_k + j] = has ? row_top[(r - 1) * top_k + j] : 0.f;
-          }
-        }
-    }
-    if (next_tokens) memcpy(next_tokens, m->pin + 3 * B, n_seqs * 4);
-    if (logits_out) {
-      void* tmp = nullptr;
-      B200W_CUDA(cudaMalloc(&tmp, static_cast<size_t>(n_seqs) * V * 4));
-      cast_bf16_to_f32(m->logits, static_cast<float*>(tmp), static_cast<size_t>(n_seqs) * V, s);
-      B200W_CUDA(cudaStreamSynchronize(s));
-      B200W_CUDA(cudaMemcpy(logits_out, tmp, static_cast<size_t>(n_seqs) * V * 4, cudaMemcpyDeviceToHost));
-      cudaFree(tmp);
-    }
-    m->logits_rows = n_seqs;
+    read_outputs(m, s, n_seqs, next_tokens, logits_out);
   });
 }
 

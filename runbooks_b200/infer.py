@@ -196,66 +196,65 @@ class InferEngine(Engine):
     def infer_init_random(self, seed: int = 0, std: float = 0.02):
         self._check(self._lib.b200w_infer_init_random(self._h, seed, std))
 
+    def _outputs(self, n: int, want_logits: bool):
+        """The next tokens [n] and, with want_logits, fp32 logits [n, V] a step or prefill call writes."""
+        return (np.empty(n, dtype=np.int32),
+                np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None)
+
+    def _step_args(self, tokens, positions, slots, want_logits: bool):
+        """-> the int32 arguments of a step call (tokens, positions, slots) and its outputs (next tokens, logits)."""
+        tok, pos, sl = (np.ascontiguousarray(x, dtype=np.int32) for x in (tokens, positions, slots))
+        return (tok, pos, sl) + self._outputs(tok.size, want_logits)
+
+    @staticmethod
+    def _padded(prompts, starts=None):
+        """The prompts, or their suffixes prompts[i][starts[i]:], zero-padded into [n, S] int32 with S the longest
+        rounded up to a multiple of 128 -> (that array, the int32 lengths of the whole prompts)."""
+        if starts is None:
+            starts = [0] * len(prompts)
+        S = ((max(len(p) - s for p, s in zip(prompts, starts)) + 127) // 128) * 128
+        tok = np.zeros((len(prompts), S), dtype=np.int32)
+        for i, (p, s) in enumerate(zip(prompts, starts)):
+            tok[i, :len(p) - s] = p[s:]
+        return tok, np.array([len(p) for p in prompts], dtype=np.int32)
+
     def step(self, tokens, positions, slots, want_logits: bool = False):
-        tok = np.ascontiguousarray(tokens, dtype=np.int32)
-        pos = np.ascontiguousarray(positions, dtype=np.int32)
-        sl = np.ascontiguousarray(slots, dtype=np.int32)
-        n = tok.size
-        nxt = np.empty(n, dtype=np.int32)
-        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
-        self._check(self._lib.b200w_infer_step(self._h, tok.ctypes.data, pos.ctypes.data, sl.ctypes.data, n,
+        tok, pos, sl, nxt, logits = self._step_args(tokens, positions, slots, want_logits)
+        self._check(self._lib.b200w_infer_step(self._h, tok.ctypes.data, pos.ctypes.data, sl.ctypes.data, tok.size,
                                                nxt.ctypes.data, logits.ctypes.data if want_logits else None))
         return nxt, logits
-
 
     def prefill(self, prompts: List[List[int]], slots: List[int], want_logits: bool = False):
         """One pass over whole prompts (b200w_infer_prefill): K/V of every prompt position goes to its
         cache slot; returns (greedy token after each prompt, logits [n, V] or None)."""
-        n = len(prompts)
-        longest = max(len(p) for p in prompts)
-        S = ((longest + 127) // 128) * 128
-        tok = np.zeros((n, S), dtype=np.int32)
-        for i, p in enumerate(prompts):
-            tok[i, :len(p)] = p
-        lens = np.array([len(p) for p in prompts], dtype=np.int32)
+        tok, lens = self._padded(prompts)
         sl = np.ascontiguousarray(slots, dtype=np.int32)
-        nxt = np.empty(n, dtype=np.int32)
-        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
-        self._check(self._lib.b200w_infer_prefill(self._h, tok.ctypes.data, lens.ctypes.data, sl.ctypes.data, n, S,
-                                                  nxt.ctypes.data, logits.ctypes.data if want_logits else None))
+        nxt, logits = self._outputs(len(prompts), want_logits)
+        self._check(self._lib.b200w_infer_prefill(self._h, tok.ctypes.data, lens.ctypes.data, sl.ctypes.data,
+                                                  *tok.shape, nxt.ctypes.data,
+                                                  logits.ctypes.data if want_logits else None))
         return nxt, logits
 
     def prefill_cached(self, prompts: List[List[int]], starts: List[int], slots: List[int], want_logits: bool = False):
         """prefill of whole prompts whose positions [0, starts[i]) already have their K/V in the slot's (shared)
         pages: only prompts[i][starts[i]:] is computed (b200w_infer_prefill_cached)."""
-        n = len(prompts)
-        S = ((max(len(p) - s for p, s in zip(prompts, starts)) + 127) // 128) * 128
-        tok = np.zeros((n, S), dtype=np.int32)
-        for i, (p, s) in enumerate(zip(prompts, starts)):
-            tok[i, :len(p) - s] = p[s:]
+        tok, lens = self._padded(prompts, starts)
         st = np.ascontiguousarray(starts, dtype=np.int32)
-        lens = np.array([len(p) for p in prompts], dtype=np.int32)
         sl = np.ascontiguousarray(slots, dtype=np.int32)
-        nxt = np.empty(n, dtype=np.int32)
-        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
+        nxt, logits = self._outputs(len(prompts), want_logits)
         self._check(self._lib.b200w_infer_prefill_cached(self._h, tok.ctypes.data, st.ctypes.data, lens.ctypes.data,
-                                                         sl.ctypes.data, n, S, nxt.ctypes.data,
+                                                         sl.ctypes.data, *tok.shape, nxt.ctypes.data,
                                                          logits.ctypes.data if want_logits else None))
         return nxt, logits
 
     def step_logprobs(self, tokens, positions, slots, top_k: int, want_logits: bool = False):
         """step, plus the log-probabilities of each row's next-token distribution (b200w_infer_step_logprobs):
         -> (next tokens, logits or None, TokenLogprobs)."""
-        tok = np.ascontiguousarray(tokens, dtype=np.int32)
-        pos = np.ascontiguousarray(positions, dtype=np.int32)
-        sl = np.ascontiguousarray(slots, dtype=np.int32)
-        n = tok.size
-        nxt = np.empty(n, dtype=np.int32)
-        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
-        lp, s = TokenLogprobs.alloc(n, top_k)
-        self._check(self._lib.b200w_infer_step_logprobs(self._h, tok.ctypes.data, pos.ctypes.data, sl.ctypes.data, n,
-                                                        nxt.ctypes.data, logits.ctypes.data if want_logits else None,
-                                                        C.byref(s)))
+        tok, pos, sl, nxt, logits = self._step_args(tokens, positions, slots, want_logits)
+        lp, s = TokenLogprobs.alloc(tok.size, top_k)
+        self._check(self._lib.b200w_infer_step_logprobs(self._h, tok.ctypes.data, pos.ctypes.data, sl.ctypes.data,
+                                                        tok.size, nxt.ctypes.data,
+                                                        logits.ctypes.data if want_logits else None, C.byref(s)))
         return nxt, logits, lp
 
     def prefill_logprobs(self, prompts: List[List[int]], slots: List[int], top_k: int, want_logits: bool = False,
@@ -264,15 +263,10 @@ class InferEngine(Engine):
         (b200w_infer_prefill_logprobs): -> (next tokens, logits or None, TokenLogprobs, prompt) where prompt[i] is
         None or (lp [len], top_ids [len, top_k], top_lp [len, top_k]) of prompts[i]; lp[p] = log P(prompt[p] |
         prompt[:p]) and position 0 has none (0, ids -1)."""
-        n = len(prompts)
-        S = ((max(len(p) for p in prompts) + 127) // 128) * 128
-        tok = np.zeros((n, S), dtype=np.int32)
-        for i, p in enumerate(prompts):
-            tok[i, :len(p)] = p
-        lens = np.array([len(p) for p in prompts], dtype=np.int32)
+        tok, lens = self._padded(prompts)
+        n, S = tok.shape
         sl = np.ascontiguousarray(slots, dtype=np.int32)
-        nxt = np.empty(n, dtype=np.int32)
-        logits = np.empty((n, self.serve_arch.vocab_size), dtype=np.float32) if want_logits else None
+        nxt, logits = self._outputs(n, want_logits)
         lp, s = TokenLogprobs.alloc(n, top_k)
         if score_prompts:
             plp = np.empty((n, S), dtype=np.float32)
