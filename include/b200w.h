@@ -339,6 +339,35 @@ typedef struct b200w_sampling {
  * log-probability is that minus the row's lse). The staging buffers are allocated by the first call and kept. */
 B200W_API int b200w_infer_sample(b200w_ctx* ctx, int n, const b200w_sampling* sampling, int32_t* tokens_out,
                                  float* token_logit_out);
+/* Presence, frequency and repetition penalties and logit bias (DESIGN §3.5), applied on the device before the draw.
+ * Row i's entries are [offsets[i], offsets[i + 1]): for each, with x the raw logit of ids[j], c = out_count[j]
+ * (times the token occurs in the request's output so far) and in fp32, one rounded operation at a time:
+ *   x += bias[j];  if (in_prompt[j] || c > 0) x = x > 0 ? x / repetition : x * repetition;
+ *   x -= frequency * c (the product rounded first);  if (c > 0) x -= presence;
+ *   x = min(max(x, -BF16_MAX), BF16_MAX) (fmaxf / fminf: a NaN goes to -BF16_MAX);  then x is rounded to bf16 (RNE).
+ * So a finite logit stays finite. Tokens without an entry, or whose raw logit is +-inf, keep their logit. The draw (or, at temperature <= 0, the argmax with ties
+ * to the smaller id) is b200w_infer_sample's on the penalized rows. A row with no entries samples as it would
+ * without penalties. NULL arrays (ids .. bias may be NULL when there are no entries), a non-zero reserved, offsets
+ * not starting at 0 or decreasing, an id outside 0..vocab-1 or twice in a row, a negative count, in_prompt other
+ * than 0 / 1, a non-finite value or repetition <= 0 are B200W_ERR_INVALID before any GPU work. */
+typedef struct b200w_penalties {
+  int32_t reserved;            /* zero                                                                 */
+  const float* presence;       /* HOST [n]                                                             */
+  const float* frequency;      /* HOST [n]                                                             */
+  const float* repetition;     /* HOST [n], > 0; 1 = off                                               */
+  const int32_t* offsets;      /* HOST [n + 1]: row i's entries are [offsets[i], offsets[i + 1])       */
+  const int32_t* ids;          /* HOST [offsets[n]], distinct within a row, 0..vocab-1                 */
+  const int32_t* out_count;    /* HOST [offsets[n]], >= 0                                              */
+  const int32_t* in_prompt;    /* HOST [offsets[n]], 0 / 1                                             */
+  const float* bias;           /* HOST [offsets[n]], finite; 0 = none                                  */
+} b200w_penalties;
+/* b200w_infer_sample on the rows penalized by `penalties` (NULL: b200w_infer_sample itself), with its state rule.
+ * token_logit_out holds the drawn tokens' raw logits: a token's log-probability stays raw logit - lse. The first
+ * penalized call allocates a bf16 [max_batch, vocab] buffer for the penalized rows (counted in
+ * b200w_infer_device_bytes) and the entry staging, which grows to the largest call's; the context keeps both. */
+B200W_API int b200w_infer_sample_penalized(b200w_ctx* ctx, int n, const b200w_sampling* sampling,
+                                           const b200w_penalties* penalties, int32_t* tokens_out,
+                                           float* token_logit_out);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.
@@ -438,6 +467,10 @@ B200W_API int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int 
 B200W_API int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V,
                               const b200w_sampling* sampling, const float* u, int32_t* tokens_out,
                               float* token_logit_out);
+/* The penalty kernel of b200w_infer_sample_penalized on bf16 DEVICE logits [rows, ld] (V % 8 == 0, ld % 8 == 0):
+ * out DEVICE bf16 [rows, V] (16-byte aligned) <- the penalized rows; penalties as there (HOST arrays). */
+B200W_API int b200w_op_penalize(b200w_ctx* ctx, const void* logits, int ld, int rows, int V,
+                                const b200w_penalties* penalties, void* out);
 B200W_API int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale);

@@ -57,6 +57,13 @@ class Sampling(C.Structure):
                 ("draw", vp)]
 
 
+class Penalties(C.Structure):
+    """b200w_penalties: HOST per-row penalties and CSR entry arrays of b200w_infer_sample_penalized /
+    b200w_op_penalize."""
+    _fields_ = [("reserved", C.c_int32), ("presence", vp), ("frequency", vp), ("repetition", vp), ("offsets", vp),
+                ("ids", vp), ("out_count", vp), ("in_prompt", vp), ("bias", vp)]
+
+
 class HParams(C.Structure):
     _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
                 ("weight_decay", C.c_float), ("max_grad_norm", C.c_float)]
@@ -115,6 +122,7 @@ PROTOTYPES = {
     "b200w_infer_step_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp, vp]),
     "b200w_infer_prefill_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "b200w_infer_sample": (C.c_int, [c_ctx, C.c_int, vp, vp, vp]),
+    "b200w_infer_sample_penalized": (C.c_int, [c_ctx, C.c_int, vp, vp, vp, vp]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
@@ -153,6 +161,7 @@ PROTOTYPES = {
                                                 vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_logprobs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
     "b200w_op_sample": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
+    "b200w_op_penalize": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp]),
     "b200w_op_attention_bwd": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp,
                                          vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "b200w_op_attention_fwd_docs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp,

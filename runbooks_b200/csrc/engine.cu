@@ -1987,6 +1987,25 @@ int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V,
     ++ctx->launches;
   });
 }
+int b200w_op_penalize(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_penalties* pen,
+                      void* out) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(V >= 8, "bad vocabulary size");
+    const int64_t entries = check_penalties(pen, rows, V);
+    std::vector<uint8_t> host(penalty_bytes(rows, entries));
+    void* dev = nullptr;
+    B200W_CUDA(cudaMalloc(&dev, host.size()));
+    try {
+      penalize(logits, ld, rows, V, pen, out, host.data(), dev, ctx->stream);
+      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
+    } catch (...) {
+      cudaFree(dev);
+      throw;
+    }
+    cudaFree(dev);
+    ++ctx->launches;
+  });
+}
 int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
                            const void* out, const void* dout, int ld_out, const float* lse2,
                            float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {

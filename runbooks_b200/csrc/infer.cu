@@ -1408,6 +1408,52 @@ sample_kernel(const bf16* __restrict__ logits, int ld, int V, SampleArgs p, int3
   }
 }
 
+// ---- penalties (b200w_infer_sample_penalized, b200w_op_penalize) ----
+// Row r of `out` [rows, V] <- row r of the logits with the row's entries penalized (DESIGN §3.5 has the definition),
+// in fp32 one rounded operation at a time (the __f*_rn intrinsics keep nvcc from contracting them into an FMA), then
+// rounded to bf16 for sample_kernel. Ids are distinct within a row, so the entries' stores after the copy never meet.
+struct PenaltyArgs {   // DEVICE
+  const float *presence, *frequency, *repetition;           // [rows]
+  const int32_t *offsets, *ids, *out_count, *in_prompt;      // [rows + 1], then [entries] each
+  const float* bias;                                         // [entries]
+};
+
+constexpr float PEN_BF16_MAX = 0x1.FEp127f;   // the largest finite bf16, 3.3895e38
+
+// one CTA per row, sample_kernel's shape; V % 8 == 0, ld % 8 == 0
+__global__ void __launch_bounds__(SP_THREADS)
+penalize_kernel(const bf16* __restrict__ logits, int ld, int V, PenaltyArgs p, bf16* __restrict__ out) {
+  const int r = blockIdx.x;
+  const bf16* row = logits + static_cast<size_t>(r) * ld;
+  bf16* dst = out + static_cast<size_t>(r) * V;
+  for (int i = threadIdx.x * 8; i < V; i += SP_THREADS * 8)
+    *reinterpret_cast<uint4*>(dst + i) = *reinterpret_cast<const uint4*>(row + i);
+  const int lo = p.offsets[r], hi = p.offsets[r + 1];
+  if (lo == hi) return;
+  __syncthreads();   // the copy of an entry's position lands before its penalized value
+  const float presence = p.presence[r], frequency = p.frequency[r], repetition = p.repetition[r];
+  for (int j = lo + threadIdx.x; j < hi; j += SP_THREADS) {
+    const int t = p.ids[j], c = p.out_count[j];
+    const float raw = __bfloat162float(row[t]);
+    if (!isfinite(raw)) continue;   // ±inf stay as the copy left them
+    float x = __fadd_rn(raw, p.bias[j]);
+    if (p.in_prompt[j] || c > 0) x = x > 0.f ? __fdiv_rn(x, repetition) : __fmul_rn(x, repetition);
+    x = __fsub_rn(x, __fmul_rn(frequency, static_cast<float>(c)));
+    if (c > 0) x = __fsub_rn(x, presence);
+    // a finite logit stays finite: saturated at the largest bf16 magnitude (fmaxf maps a NaN to the lower bound)
+    dst[t] = __float2bfloat16_rn(fminf(fmaxf(x, -PEN_BF16_MAX), PEN_BF16_MAX));
+  }
+}
+
+// token_logit[r] <- the raw logit of tokens[r] (0 for a negative token): a penalized row's log-probability stays raw
+__global__ void raw_logit_kernel(const bf16* __restrict__ logits, int ld, int rows, const int32_t* __restrict__ tokens,
+                                 float* __restrict__ token_logit) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const int t = tokens[r];
+  token_logit[r] = t >= 0 ? __bfloat162float(logits[static_cast<size_t>(r) * ld + t]) : 0.f;
+}
+
 struct IParam {
   std::string name;
   int64_t rows, cols;
@@ -1471,6 +1517,12 @@ struct Infer {
   // the per-row parameters and results of a call (sample_bytes), on the device and pinned, from the first such call
   int logits_rows = 0;
   uint8_t *sp_dev = nullptr, *sp_pin = nullptr;
+  // penalties, from the first b200w_infer_sample_penalized call: the penalized rows [max_batch, V] sample_kernel then
+  // reads, and the entry staging (penalty_bytes), on the device and pinned, grown to the largest call's
+  bf16* pen_rows = nullptr;
+  uint8_t *pen_dev = nullptr, *pen_pin = nullptr;
+  size_t pen_cap = 0;          // bytes of both stagings (0 until both exist)
+  int64_t pen_dev_bytes = 0;   // what pen_dev adds to `bytes`, taken off again when it is replaced
   std::vector<void*> allocs;
   int64_t bytes = 0;
   template <typename T>
@@ -1498,6 +1550,7 @@ struct Infer {
     if (pin_tok) cudaFreeHost(pin_tok);
     if (pf_pin) cudaFreeHost(pf_pin);
     if (sp_pin) cudaFreeHost(sp_pin);
+    if (pen_pin) cudaFreeHost(pen_pin);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -2287,11 +2340,91 @@ void b200w::check_sampling(const b200w_sampling* sp, int n, int V, const int32_t
   }
 }
 
-void b200w::sample(const void* logits, int ld, int rows, int V, const b200w_sampling* sp, const float* u,
-                   int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s) {
+static void check_logit_rows(const void* logits, int ld, int V) {
   B200W_CHECK(logits && V >= 8 && V % 8 == 0 && ld >= V && ld % 8 == 0 &&
                   (reinterpret_cast<uintptr_t>(logits) & 15) == 0,
               "logits must be 16-byte aligned rows of a multiple of 8 entries");
+}
+
+// per call: offsets [rows + 1] | presence | frequency | repetition [rows] | ids | out_count | in_prompt | bias [entries]
+size_t b200w::penalty_bytes(int rows, int64_t entries) {
+  return 4 * (4 * static_cast<size_t>(rows) + 1) + 16 * static_cast<size_t>(entries);
+}
+
+int64_t b200w::check_penalties(const b200w_penalties* pen, int n, int V) {
+  B200W_CHECK(pen && n >= 1 && pen->reserved == 0 && pen->presence && pen->frequency && pen->repetition &&
+                  pen->offsets && pen->offsets[0] == 0,
+              "b200w_penalties: presence, frequency, repetition and offsets must be given, offsets[0] 0, reserved 0");
+  for (int i = 0; i < n; ++i) {
+    B200W_CHECK(pen->offsets[i + 1] >= pen->offsets[i], "offsets must not decrease");
+    B200W_CHECK(std::isfinite(pen->presence[i]) && std::isfinite(pen->frequency[i]),
+                "presence and frequency must be finite");
+    B200W_CHECK(std::isfinite(pen->repetition[i]) && pen->repetition[i] > 0.f, "repetition must be finite and > 0");
+  }
+  const int64_t entries = pen->offsets[n];
+  if (entries == 0) return 0;
+  B200W_CHECK(pen->ids && pen->out_count && pen->in_prompt && pen->bias,
+              "b200w_penalties: ids, out_count, in_prompt and bias must be given when there are entries");
+  // distinct ids within a row: the row's stamp in a per-thread table of the vocabulary
+  thread_local std::vector<uint32_t> seen;
+  thread_local uint32_t stamp = 0;
+  if (seen.size() < static_cast<size_t>(V)) seen.assign(V, 0);
+  for (int i = 0; i < n; ++i) {
+    if (++stamp == 0) {
+      std::fill(seen.begin(), seen.end(), 0u);
+      stamp = 1;
+    }
+    for (int64_t j = pen->offsets[i]; j < pen->offsets[i + 1]; ++j) {
+      const int32_t t = pen->ids[j];
+      B200W_CHECK(t >= 0 && t < V, "penalty id outside the vocabulary");
+      B200W_CHECK(seen[t] != stamp, "penalty ids must be distinct within a row");
+      seen[t] = stamp;
+      B200W_CHECK(pen->out_count[j] >= 0, "out_count must be >= 0");
+      B200W_CHECK(pen->in_prompt[j] == 0 || pen->in_prompt[j] == 1, "in_prompt must be 0 or 1");
+      B200W_CHECK(std::isfinite(pen->bias[j]), "bias must be finite");
+    }
+  }
+  return entries;
+}
+
+void b200w::penalize(const void* logits, int ld, int rows, int V, const b200w_penalties* pen, void* out, void* host,
+                     void* dev, cudaStream_t s) {
+  check_logit_rows(logits, ld, V);
+  B200W_CHECK(out && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "out must be 16-byte aligned");
+  const int64_t e = pen->offsets[rows];
+  const size_t n = rows;
+  uint8_t* h = static_cast<uint8_t*>(host);
+  uint8_t* d = static_cast<uint8_t*>(dev);
+  const size_t o_pre = 4 * (n + 1), o_freq = o_pre + 4 * n, o_rep = o_freq + 4 * n, o_ids = o_rep + 4 * n,
+               o_cnt = o_ids + 4 * e, o_inp = o_cnt + 4 * e, o_bias = o_inp + 4 * e;
+  memcpy(h, pen->offsets, 4 * (n + 1));
+  memcpy(h + o_pre, pen->presence, 4 * n);
+  memcpy(h + o_freq, pen->frequency, 4 * n);
+  memcpy(h + o_rep, pen->repetition, 4 * n);
+  if (e) {
+    memcpy(h + o_ids, pen->ids, 4 * e);
+    memcpy(h + o_cnt, pen->out_count, 4 * e);
+    memcpy(h + o_inp, pen->in_prompt, 4 * e);
+    memcpy(h + o_bias, pen->bias, 4 * e);
+  }
+  B200W_CUDA(cudaMemcpyAsync(d, h, penalty_bytes(rows, e), cudaMemcpyHostToDevice, s));
+  PenaltyArgs a;
+  a.offsets = reinterpret_cast<const int32_t*>(d);
+  a.presence = reinterpret_cast<const float*>(d + o_pre);
+  a.frequency = reinterpret_cast<const float*>(d + o_freq);
+  a.repetition = reinterpret_cast<const float*>(d + o_rep);
+  a.ids = reinterpret_cast<const int32_t*>(d + o_ids);
+  a.out_count = reinterpret_cast<const int32_t*>(d + o_cnt);
+  a.in_prompt = reinterpret_cast<const int32_t*>(d + o_inp);
+  a.bias = reinterpret_cast<const float*>(d + o_bias);
+  penalize_kernel<<<rows, SP_THREADS, 0, s>>>(static_cast<const bf16*>(logits), ld, V, a, static_cast<bf16*>(out));
+  B200W_CUDA(cudaGetLastError());
+}
+
+void b200w::sample(const void* logits, int ld, int rows, int V, const b200w_sampling* sp, const float* u,
+                   int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s,
+                   const b200w_penalties* pen, const PenaltyBuffers* pb) {
+  check_logit_rows(logits, ld, V);
   check_sampling(sp, rows, V, tokens_out);
   B200W_CHECK(rows <= cap, "more rows than the staging holds");
   const size_t c = cap, n = rows;
@@ -2311,9 +2444,17 @@ void b200w::sample(const void* logits, int ld, int rows, int V, const b200w_samp
   a.top_p = reinterpret_cast<const float*>(d + 20 * c);
   a.top_k = reinterpret_cast<const int32_t*>(d + 24 * c);
   a.u = u ? reinterpret_cast<const float*>(d + 28 * c) : nullptr;
-  sample_kernel<<<rows, SP_THREADS, 0, s>>>(static_cast<const bf16*>(logits), ld, V, a,
-                                            reinterpret_cast<int32_t*>(d + 32 * c),
-                                            reinterpret_cast<float*>(d + 36 * c));
+  int32_t* tok_d = reinterpret_cast<int32_t*>(d + 32 * c);
+  float* logit_d = reinterpret_cast<float*>(d + 36 * c);
+  if (pen) {   // sample from the penalized rows; the tokens' logits come from the raw ones
+    penalize(logits, ld, rows, V, pen, pb->rows, pb->host, pb->dev, s);
+    sample_kernel<<<rows, SP_THREADS, 0, s>>>(static_cast<const bf16*>(pb->rows), V, V, a, tok_d, nullptr);
+    B200W_CUDA(cudaGetLastError());
+    if (token_logit_out)
+      raw_logit_kernel<<<cdiv(rows, 128), 128, 0, s>>>(static_cast<const bf16*>(logits), ld, rows, tok_d, logit_d);
+  } else {
+    sample_kernel<<<rows, SP_THREADS, 0, s>>>(static_cast<const bf16*>(logits), ld, V, a, tok_d, logit_d);
+  }
   B200W_CUDA(cudaGetLastError());
   B200W_CUDA(cudaMemcpyAsync(h + 32 * c, d + 32 * c, c * SP_OUT_BYTES, cudaMemcpyDeviceToHost, s));
   B200W_CUDA(cudaStreamSynchronize(s));
@@ -2616,24 +2757,57 @@ int b200w_infer_prefill_logprobs(b200w_ctx* ctx, const int32_t* tokens, const in
                       prompt_lp, prompt_top_ids, prompt_top_lp);
 }
 
-int b200w_infer_sample(b200w_ctx* ctx, int n, const b200w_sampling* sp, int32_t* tokens_out, float* token_logit_out) {
+// b200w_infer_sample and, when pen != nullptr, b200w_infer_sample_penalized
+static int sample_impl(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b200w_penalties* pen,
+                       int32_t* tokens_out, float* token_logit_out) {
   Infer* m = ctx ? static_cast<Infer*>(ctx_infer_slot(ctx)) : nullptr;
   const int have = m ? m->logits_rows : 0;
   const int st = iguard(ctx, [&] {
     model(ctx);
     const int V = m->a.vocab_size;
     check_sampling(sp, n, V, tokens_out);
+    const int64_t entries = pen ? check_penalties(pen, n, V) : 0;
     if (n != have) throw StateError("b200w_infer_sample must follow the step or prefill call whose rows it samples");
     if (!m->sp_dev) {
       m->sp_dev = m->alloc<uint8_t>(sample_bytes(m->max_batch));
       B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->sp_pin), sample_bytes(m->max_batch)));
     }
+    PenaltyBuffers pb{};
+    if (pen) {
+      if (!m->pen_rows) m->pen_rows = m->alloc<bf16>(static_cast<size_t>(m->max_batch) * V);
+      const size_t need = penalty_bytes(n, entries);
+      if (need > m->pen_cap) {   // grown geometrically: a request's entries grow by one token a step
+        const size_t cap = std::max(need, 2 * m->pen_cap);
+        if (m->pen_dev) {   // the count keeps what the context holds: the old staging leaves it
+          m->release(m->pen_dev);
+          m->bytes -= m->pen_dev_bytes;
+        }
+        if (m->pen_pin) cudaFreeHost(m->pen_pin);
+        m->pen_dev = m->pen_pin = nullptr;
+        m->pen_cap = 0;
+        const int64_t before = m->bytes;
+        m->pen_dev = m->alloc<uint8_t>(cap);
+        m->pen_dev_bytes = m->bytes - before;
+        B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pen_pin), cap));
+        m->pen_cap = cap;
+      }
+      pb = PenaltyBuffers{m->pen_rows, m->pen_pin, m->pen_dev};
+    }
     sample(m->logits, V, n, V, sp, nullptr, tokens_out, token_logit_out, m->sp_pin, m->sp_dev, m->max_batch,
-           ctx_stream(ctx));
-    ++ctx_launches(ctx);
+           ctx_stream(ctx), pen, pen ? &pb : nullptr);
+    ctx_launches(ctx) += pen ? (token_logit_out ? 3 : 2) : 1;
   });
   if (m) m->logits_rows = have;   // the logits are as they were: the call may be repeated
   return st;
+}
+
+int b200w_infer_sample(b200w_ctx* ctx, int n, const b200w_sampling* sp, int32_t* tokens_out, float* token_logit_out) {
+  return sample_impl(ctx, n, sp, nullptr, tokens_out, token_logit_out);
+}
+
+int b200w_infer_sample_penalized(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b200w_penalties* pen,
+                                 int32_t* tokens_out, float* token_logit_out) {
+  return sample_impl(ctx, n, sp, pen, tokens_out, token_logit_out);
 }
 
 int64_t b200w_infer_device_bytes(b200w_ctx* ctx) {

@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 struct b200w_sampling;   // include/b200w.h
+struct b200w_penalties;  // include/b200w.h
 
 namespace b200w {
 
@@ -115,10 +116,24 @@ void logprobs(const void* logits, int ld, int rows, int V, const int32_t* target
 // definition). sp, u (nullable: Philox from seed / draw), tokens_out and token_logit_out (nullable) are HOST arrays;
 // they travel through `host` (pinned or not) and `dev`, sample_bytes(cap) bytes each, rows <= cap. check_sampling
 // throws on a bad argument; sample calls it before any GPU work and returns after the stream has drained.
+// With pen (b200w.h b200w_penalties, checked by check_penalties), the rows are penalized into pb->rows [rows, V]
+// first (penalize), sample_kernel draws from those, and token_logit_out holds the drawn tokens' raw logits.
+struct PenaltyBuffers {
+  void* rows;         // DEVICE bf16 [rows, V]
+  void *host, *dev;   // penalty_bytes(rows, entries) each; host pinned or not
+};
 size_t sample_bytes(int cap);
 void check_sampling(const b200w_sampling* sp, int n, int V, const int32_t* tokens_out);
 void sample(const void* logits, int ld, int rows, int V, const b200w_sampling* sp, const float* u,
-            int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s);
+            int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s,
+            const b200w_penalties* pen = nullptr, const PenaltyBuffers* pb = nullptr);
+// Penalties (infer.cu penalize_kernel; b200w.h b200w_penalties has the definition). check_penalties throws on a bad
+// argument and returns the number of entries; penalize (after it) stages the entries through `host` and `dev`,
+// penalty_bytes(rows, entries) bytes each, and writes out [rows, V] (16-byte aligned) on stream s.
+size_t penalty_bytes(int rows, int64_t entries);
+int64_t check_penalties(const b200w_penalties* pen, int n, int V);
+void penalize(const void* logits, int ld, int rows, int V, const b200w_penalties* pen, void* out, void* host,
+              void* dev, cudaStream_t s);
 
 
 // ---- ops.cu --------------------------------------------------------------------------------

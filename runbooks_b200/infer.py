@@ -1,6 +1,7 @@
 """Host side of the Server decode path: `InferEngine` wraps the b200w_infer_* C ABI; `Generator`
 turns it into a continuously-batched generator (one cache slot per request, one token per slot per step —
-prompt ingestion and generation are the same step), greedy or sampled on the device (`InferEngine.sample`)."""
+prompt ingestion and generation are the same step), greedy or sampled on the device (`InferEngine.sample`), with
+penalties and logit bias applied on the device before the draw (`InferEngine.sample_penalized`)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -299,6 +300,98 @@ class InferEngine(Engine):
                                                  lg.ctypes.data if want_logit else None))
         return tok, lg
 
+    def sample_penalized(self, n: int, temperature, top_p, top_k, seeds, draws, penalties: "Penalties",
+                         want_logit: bool = False):
+        """sample on the rows after their presence, frequency and repetition penalties and logit bias
+        (b200w_infer_sample_penalized; DESIGN §3.5). Rows with temperature <= 0 get the argmax of the penalized row.
+        -> (tokens, the tokens' raw logits as fp32 or None)."""
+        t = np.ascontiguousarray(temperature, dtype=np.float32)
+        p = np.ascontiguousarray(top_p, dtype=np.float32)
+        k = np.ascontiguousarray(top_k, dtype=np.int32)
+        sd = np.ascontiguousarray(seeds, dtype=np.uint64)
+        dr = np.ascontiguousarray(draws, dtype=np.uint64)
+        if not t.size == p.size == k.size == sd.size == dr.size == penalties.presence.size == n:
+            raise ValueError("sample_penalized: one temperature, top_p, top_k, seed, draw index and penalty per row")
+        s = _lib.Sampling(0, t.ctypes.data, p.ctypes.data, k.ctypes.data, sd.ctypes.data, dr.ctypes.data)
+        pen = penalties.c_struct()
+        tok = np.empty(n, dtype=np.int32)
+        lg = np.empty(n, dtype=np.float32) if want_logit else None
+        self._check(self._lib.b200w_infer_sample_penalized(self._h, n, C.byref(s), C.byref(pen), tok.ctypes.data,
+                                                           lg.ctypes.data if want_logit else None))
+        return tok, lg
+
+
+@dataclass
+class Penalties:
+    """The b200w_penalties of one call: per row presence, frequency and repetition, and the rows' entries in CSR form
+    (row i's are [offsets[i], offsets[i + 1])): distinct ids, how often each occurs in the request's output, whether
+    it occurs in its prompt, and its logit bias."""
+    presence: np.ndarray     # float32 [n]
+    frequency: np.ndarray    # float32 [n]
+    repetition: np.ndarray   # float32 [n]
+    offsets: np.ndarray      # int32 [n + 1]
+    ids: np.ndarray          # int32 [entries]
+    out_count: np.ndarray    # int32 [entries]
+    in_prompt: np.ndarray    # int32 [entries]
+    bias: np.ndarray         # float32 [entries]
+
+    @classmethod
+    def pack(cls, rows: List[Optional["RequestPenalties"]]) -> "Penalties":
+        """One call's arrays from each row's RequestPenalties (None: a row without penalties)."""
+        live = [r for r in rows if r is not None]
+        counts = [r.n if r is not None else 0 for r in rows]
+        offsets = np.zeros(len(rows) + 1, np.int32)
+        np.cumsum(counts, out=offsets[1:])
+
+        def cat(field, dt):
+            return np.concatenate([getattr(r, field)[:r.n] for r in live]) if live else np.zeros(0, dt)
+        return cls(np.array([r.presence if r else 0.0 for r in rows], np.float32),
+                   np.array([r.frequency if r else 0.0 for r in rows], np.float32),
+                   np.array([r.repetition if r else 1.0 for r in rows], np.float32), offsets,
+                   cat("ids", np.int32), cat("out_count", np.int32), cat("in_prompt", np.int32),
+                   cat("bias", np.float32))
+
+    def c_struct(self) -> _lib.Penalties:
+        arrs = [np.ascontiguousarray(getattr(self, f), dtype=dt) for f, dt in (
+            ("presence", np.float32), ("frequency", np.float32), ("repetition", np.float32), ("offsets", np.int32),
+            ("ids", np.int32), ("out_count", np.int32), ("in_prompt", np.int32), ("bias", np.float32))]
+        s = _lib.Penalties(0, *(a.ctypes.data for a in arrs))
+        s._keep = arrs   # the struct holds raw pointers: keep the arrays alive with it
+        return s
+
+
+class RequestPenalties:
+    """A request's penalties and its entries, kept as it generates: the distinct ids of its prompt (only when
+    repetition != 1: they matter to nothing else), of its logit_bias and of its output so far, with the output counts,
+    the prompt flags and the biases. emit() counts a generated token; a step packs these arrays as they stand."""
+
+    def __init__(self, prompt: List[int], presence: float, frequency: float, repetition: float,
+                 logit_bias: Dict[int, float]):
+        self.presence, self.frequency, self.repetition = float(presence), float(frequency), float(repetition)
+        ids = list(dict.fromkeys((list(prompt) if self.repetition != 1.0 else []) + list(logit_bias)))
+        self.pos = {t: i for i, t in enumerate(ids)}
+        self.n = len(ids)
+        cap = max(16, 2 * self.n)
+        self.ids, self.out_count, self.in_prompt = (np.zeros(cap, np.int32) for _ in range(3))
+        self.bias = np.zeros(cap, np.float32)
+        self.ids[:self.n] = ids
+        if self.repetition != 1.0:
+            self.in_prompt[[self.pos[t] for t in set(prompt)]] = 1
+        for t, b in logit_bias.items():
+            self.bias[self.pos[t]] = b
+
+    def emit(self, t: int):
+        i = self.pos.get(t)
+        if i is None:
+            if self.n == self.ids.size:
+                for f in ("ids", "out_count", "in_prompt", "bias"):
+                    a = getattr(self, f)
+                    setattr(self, f, np.concatenate([a, np.zeros_like(a)]))
+            i = self.pos[t] = self.n
+            self.ids[i] = t
+            self.n += 1
+        self.out_count[i] += 1
+
 
 @dataclass
 class TokenLogprobs:
@@ -359,10 +452,17 @@ class _Req:
     # sampling on the device: draw i of the request uses the uniform number of (seed, i), i = len(out)
     top_k: int = 0
     seed: int = 0
+    pen: Optional[RequestPenalties] = None                    # None: no penalty and no logit_bias
+    error: Optional[str] = None                               # set when the request failed on its own (done too)
 
     @property
     def greedy(self) -> bool:
         return self.temperature <= 0.0
+
+    @property
+    def step_token(self) -> bool:
+        """Whether the token it emits is the step's own greedy token (not drawn, and nothing to penalize)."""
+        return self.greedy and self.pen is None
 
     @property
     def scores_prompt(self) -> bool:
@@ -408,7 +508,9 @@ class Generator:
 
     def add(self, prompt: List[int], max_tokens: int, temperature: float = 0.0, top_p: float = 1.0,
             seed: Optional[int] = None, defer_prefill: bool = False, logprobs: Optional[int] = None,
-            prompt_logprobs: bool = False, top_k: int = 0) -> _Req:
+            prompt_logprobs: bool = False, top_k: int = 0, presence_penalty: float = 0.0,
+            frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
+            logit_bias: Optional[Dict[int, float]] = None) -> _Req:
         """defer_prefill: only register the request; flush_prefill() then ingests every deferred prompt of the
         same padded length in ONE prefill call (what the scheduler does when several requests are admitted in
         the same round).
@@ -418,9 +520,14 @@ class Generator:
         either borrows no prefix-cache pages: their hidden states are needed and were never computed.
         top_k (0: off; at or above the vocabulary size keeps everything): sample among the top_k largest logits only,
         before top_p; needs an engine that samples on the device. seed (None: from OS entropy): with it the
-        request's tokens are a function of its logits alone."""
+        request's tokens are a function of its logits alone.
+        presence_penalty, frequency_penalty, repetition_penalty (> 0; 1 is off) and logit_bias ({token id: bias}):
+        applied to the logits on the device before the draw, greedy rows included (DESIGN §3.5), with the counts of
+        this request's own output; needs an engine that samples on the device. Log-probabilities stay raw."""
         if not prompt:
             raise ValueError("empty prompt")
+        V = self.e.serve_arch.vocab_size
+        pen = self._penalties(prompt, presence_penalty, frequency_penalty, repetition_penalty, logit_bias, V)
         if not (isinstance(top_k, int) and top_k >= 0):
             raise ValueError(f"top_k must be 0 (off) or a positive integer, got {top_k!r}")
         if top_k and not self.device_sampling:
@@ -431,7 +538,6 @@ class Generator:
             raise ValueError("log-probabilities need an engine that computes them")
         if prompt_logprobs and not (self.use_prefill and hasattr(self.e, "prefill_logprobs")):
             raise ValueError("prompt log-probabilities need an engine that prefills")
-        V = self.e.serve_arch.vocab_size
         bad = [t for t in prompt if not 0 <= int(t) < V]
         if bad:   # a per-request error (HTTP 400), never an engine failure that would take the server down
             raise ValueError(f"token id {bad[0]} outside the model vocabulary ({V})")
@@ -456,6 +562,7 @@ class Generator:
         if self.device_sampling and not r.greedy:
             r.top_k = 0 if top_k >= V else top_k
             r.seed = (int(seed) if seed is not None else int.from_bytes(os.urandom(8), "little")) % 2 ** 64
+        r.pen = pen
         if r.prompt_logprobs and not r.scores_prompt:
             r.prompt_lp = [None]          # one token: nothing to score
         self.active.append(r)
@@ -464,6 +571,29 @@ class Generator:
             if not defer_prefill:
                 self.flush_prefill()
         return r
+
+    def _penalties(self, prompt, presence, frequency, repetition, logit_bias, V) -> Optional[RequestPenalties]:
+        """A request's RequestPenalties, None when every penalty is neutral; ValueError on a value out of range. The
+        values are checked as the float32 the engine receives: one the engine would refuse fails this request alone,
+        never a whole step's batch."""
+        with np.errstate(over="ignore", under="ignore"):
+            presence, frequency, repetition = (float(np.float32(x)) for x in (presence, frequency, repetition))
+            if not all(np.isfinite(x) for x in (presence, frequency, repetition)) or not repetition > 0:
+                raise ValueError("presence_penalty and frequency_penalty must be finite, repetition_penalty finite and "
+                                 "> 0 (as float32)")
+            bias = {}
+            for t, b in (logit_bias or {}).items():
+                if isinstance(t, bool) or not isinstance(t, (int, np.integer)) or not 0 <= t < V:
+                    raise ValueError(f"logit_bias token id {t!r} outside the model vocabulary ({V})")
+                if not np.isfinite(np.float32(b)):
+                    raise ValueError(f"logit_bias of token {t} must be finite (as float32)")
+                bias[int(t)] = float(np.float32(b))
+        if presence == 0 and frequency == 0 and repetition == 1 and not bias:
+            return None
+        if not hasattr(self.e, "sample_penalized"):
+            raise ValueError("presence, frequency and repetition penalties and logit_bias need an engine that samples "
+                             "on the device")
+        return RequestPenalties(prompt, presence, frequency, repetition, bias)
 
     def _admit(self, prompt: List[int], n_tokens: int, slot: int, borrow: bool = True):
         """Prefix cache admission into `slot`: the longest chain of indexed pages that prefixes the prompt (at most
@@ -577,32 +707,45 @@ class Generator:
 
     def _sample(self, rs: List[_Req], emits: List[bool]):
         """Right after the step / prefill call over the rows `rs`: one engine.sample call for them when a row that
-        emits a token samples (the others go as greedy rows) -> (tokens, their logits or None), or None."""
+        emits a token samples (the others go as greedy rows), or one engine.sample_penalized call when such a row
+        is penalized (the others go without entries) -> (tokens, their raw logits or None), or None."""
         on = [e and not r.greedy for r, e in zip(rs, emits)]
-        if not (self.device_sampling and any(on)):
+        pen = [e and r.pen is not None for r, e in zip(rs, emits)]
+        if not (self.device_sampling and (any(on) or any(pen))):
             return None
-        return self.e.sample(len(rs), [r.temperature if s else 0.0 for r, s in zip(rs, on)], [r.top_p for r in rs],
-                             [r.top_k for r in rs], [r.seed for r in rs], [len(r.out) for r in rs],
-                             want_logit=any(s and r.logprobs is not None for r, s in zip(rs, on)))
+        args = (len(rs), [r.temperature if s else 0.0 for r, s in zip(rs, on)], [r.top_p for r in rs],
+                [r.top_k for r in rs], [r.seed for r in rs], [len(r.out) for r in rs])
+        want_logit = any((s or p) and r.logprobs is not None for r, s, p in zip(rs, on, pen))
+        if any(pen):
+            return self.e.sample_penalized(*args, Penalties.pack([r.pen if p else None for r, p in zip(rs, pen)]),
+                                           want_logit=want_logit)
+        return self.e.sample(*args, want_logit=want_logit)
 
     def _emit_token(self, r: _Req, i: int, nxt, lg, lp: Optional[TokenLogprobs], drawn=None):
-        """Emits row i's token for r: the greedy one, or one sampled from its logits (`drawn`, what _sample returned,
-        or on the host from lg); with its log-probability when r asks for it (the greedy token's from the engine, a
-        sampled one's from its logit and the row's lse)."""
-        if r.greedy:
+        """Emits row i's token for r: the greedy one, or one drawn from its (penalized) logits (`drawn`, what _sample
+        returned, or on the host from lg); with its log-probability when r asks for it (the greedy token's from the
+        engine, any other's from its raw logit and the row's lse)."""
+        if r.step_token:
             t = int(nxt[i])
         elif drawn is not None:
             t = int(drawn[0][i])
         else:
             t = sample_token(lg[i], r.temperature, r.top_p, r.rng)
+        if not 0 <= t < self.e.serve_arch.vocab_size:   # e.g. a row of infinite logits: fail r, not the batch
+            r.error = f"no token could be drawn from this request's logits (got id {t})"
+            r.done = True
+            return
         if r.logprobs is not None:
-            x = lp.token_lp[i] if r.greedy else (drawn[1][i] if drawn is not None else np.float32(lg[i][t])) - lp.lse[i]
+            x = (lp.token_lp[i] if r.step_token
+                 else (drawn[1][i] if drawn is not None else np.float32(lg[i][t])) - lp.lse[i])
             k = r.logprobs
             r.out_lp.append((float(x), list(zip(lp.top_ids[i, :k].tolist(), lp.top_lp[i, :k].tolist()))))
         self._emit(r, t)
 
     def _emit(self, r: _Req, t: int):
         r.out.append(t)
+        if r.pen is not None:
+            r.pen.emit(t)
         if len(r.out) >= r.max_tokens or (self.eos is not None and t == self.eos):
             r.done = True
 

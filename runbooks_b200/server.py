@@ -9,8 +9,11 @@ test/system.sh:73-78 and the basaran image speak — `POST /v1/completions {"pro
 returns an OpenAI-style completion; `"stream": true` answers with server-sent events (one `data:` JSON
 chunk per text delta, then `data: [DONE]`), as basaran does. Accepted and honoured: temperature / top_p /
 top_k (sampled on the GPU from the step's logits; default temperature 0 = greedy), stop, n, echo, seed, a prompt of
-token ids, and logprobs up to the server's max_logprobs (0 by default: logprobs > 0 is then a 400); anything
-else that would change the result (penalties, best_of) is a 400. Prompts are ingested in one
+token ids, logprobs up to the server's max_logprobs (0 by default: logprobs > 0 is then a 400), and, when the
+server runs with penalties on (off by default: they are then a 400, a repetition_penalty other than 1 included),
+presence_penalty / frequency_penalty /
+repetition_penalty / logit_bias (applied on the GPU before the draw, greedy requests included); anything else
+that would change the result (best_of, suffix) is a 400. Prompts are ingested in one
 prefill pass; continuous batching over the engine's cache slots (one scheduler thread owns the GPU,
 HTTP handler threads only queue requests); a full admission queue answers 503 + Retry-After.
 """
@@ -38,27 +41,31 @@ class Scheduler(threading.Thread):
     advances every active request by one token per engine step, and feeds each request's event queue
     (text deltas for streaming clients, one final record for everybody)."""
 
-    def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False, max_logprobs: int = 0):
-        """max_logprobs (0..5): the most top entries a request may ask for with `logprobs`; 0 refuses them."""
+    def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False, max_logprobs: int = 0,
+                 penalties: bool = False):
+        """max_logprobs (0..5): the most top entries a request may ask for with `logprobs`; 0 refuses them.
+        penalties: accept presence_penalty, frequency_penalty, repetition_penalty and logit_bias (else a 400)."""
         super().__init__(daemon=True)
         from .infer import Generator
         self.gen = Generator(engine, eos_id=tokenizer.eos_id, prefix_cache=prefix_cache)
         self.tok, self.q = tokenizer, queue.Queue()
         self.max_queue = max_queue or 4 * engine.max_batch
         self.max_logprobs = max_logprobs
+        self.penalties = penalties
         self.ready = threading.Event()
         self.failed: str | None = None
 
     def submit(self, prompt, max_tokens: int, temperature: float = 0.0, top_p: float = 1.0, stop=(),
-               seed=None, logprobs=None, echo: bool = False, top_k: int = 0):
+               seed=None, logprobs=None, echo: bool = False, top_k: int = 0, penalties=None):
         """prompt: text, or token ids fed as given. logprobs (None: not asked): log-probabilities of the completion
-        tokens with that many top entries, and with echo of the prompt tokens too.
+        tokens with that many top entries, and with echo of the prompt tokens too. penalties (None: none): the
+        presence_penalty, frequency_penalty, repetition_penalty and logit_bias arguments of Generator.add.
         -> item (dict) or None when the admission queue is full (the caller answers 503)."""
         if self.q.qsize() >= self.max_queue:
             return None
         item = {"prompt": prompt, "max_tokens": max_tokens, "temperature": temperature, "top_p": top_p,
                 "stop": tuple(stop), "seed": seed, "events": queue.Queue(), "cancelled": False,
-                "logprobs": logprobs, "echo": echo, "top_k": top_k}
+                "logprobs": logprobs, "echo": echo, "top_k": top_k, "penalties": dict(penalties or {})}
         if isinstance(prompt, list):
             item["ids"] = list(prompt)
         self.q.put(item)
@@ -108,7 +115,11 @@ class Scheduler(threading.Thread):
 
     # ---- per-request bookkeeping (scheduler thread only) ----
     def _progress(self, req, item, n_prompt, state):
-        """Push the text produced since the last call; finish the request on EOS / length / stop string."""
+        """Push the text produced since the last call; finish the request on EOS / length / stop string, or with an
+        error when the Generator failed it on its own."""
+        if getattr(req, "error", None):
+            item["events"].put(("error", req.error))
+            return True
         out = req.out
         eos_hit = self.tok.eos_id is not None and out and out[-1] == self.tok.eos_id
         text = self.tok.decode(out[:-1] if eos_hit else out)
@@ -187,7 +198,7 @@ class Scheduler(threading.Thread):
                         req = self.gen.add(ids, item["max_tokens"], item["temperature"], item["top_p"], item["seed"],
                                            defer_prefill=True, logprobs=item["logprobs"],
                                            prompt_logprobs=item["echo"] and item["logprobs"] is not None,
-                                           top_k=item["top_k"])
+                                           top_k=item["top_k"], **(item.get("penalties") or {}))
                         admitted.append((req, item, len(ids)))
                     except CacheFull:       # fits the pool, not now: keep its place, retry after the next step
                         held = item
@@ -245,11 +256,50 @@ def _is_token_ids(x) -> bool:
     return isinstance(x, list) and len(x) > 0 and all(isinstance(t, int) and not isinstance(t, bool) for t in x)
 
 
-def parse_completion_request(req: dict, max_logprobs: int = 0) -> dict:
+MAX_LOGIT_BIAS = 300   # entries per request, OpenAI's limit
+REPETITION_RANGE = (0.01, 100.0)   # far beyond what clients use (1 to 2), and exact enough as float32
+
+
+def _parse_penalties(req: dict) -> dict:
+    """presence_penalty and frequency_penalty in [-2, 2], repetition_penalty in [0.01, 100] (absent or null: 1) and
+    logit_bias (up to 300 entries, token ids as strings or integers, biases in [-100, 100]) -> Generator.add's
+    arguments."""
+    def num(key, default):
+        v = req.get(key)
+        if v is None:
+            return default
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise ValueError(f"{key} must be a number")
+        return float(v)
+    presence, frequency = num("presence_penalty", 0.0), num("frequency_penalty", 0.0)
+    repetition = num("repetition_penalty", 1.0)
+    if not (-2 <= presence <= 2 and -2 <= frequency <= 2):
+        raise ValueError("presence_penalty and frequency_penalty must be in [-2, 2]")
+    if not REPETITION_RANGE[0] <= repetition <= REPETITION_RANGE[1]:
+        raise ValueError(f"repetition_penalty must be in [{REPETITION_RANGE[0]}, {REPETITION_RANGE[1]:g}]")
+    raw = req.get("logit_bias") or {}
+    if not isinstance(raw, dict) or len(raw) > MAX_LOGIT_BIAS:
+        raise ValueError(f"logit_bias must map up to {MAX_LOGIT_BIAS} token ids to biases")
+    bias = {}
+    for k, v in raw.items():
+        if isinstance(k, str) and k.strip().lstrip("-").isdigit():
+            k = int(k)
+        if isinstance(k, bool) or not isinstance(k, int) or k < 0:
+            raise ValueError(f"logit_bias key {k!r} is not a token id")
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not -100 <= v <= 100:
+            raise ValueError(f"logit_bias of token {k} must be a number in [-100, 100]")
+        bias[k] = float(v)
+    return dict(presence_penalty=presence, frequency_penalty=frequency, repetition_penalty=repetition,
+                logit_bias=bias)
+
+
+def parse_completion_request(req: dict, max_logprobs: int = 0, penalties: bool = False) -> dict:
     """The OpenAI / basaran `/v1/completions` fields. Everything that is accepted is honoured; a value this
     server does not implement is a 400, never a silent fallback to something else.
     prompt: a string, a list of token ids (fed as given, no BOS added), or a list holding one of either.
-    logprobs: refused above 0 unless the server was started with max_logprobs >= 1; then 0..max_logprobs."""
+    logprobs: refused above 0 unless the server was started with max_logprobs >= 1; then 0..max_logprobs.
+    presence_penalty, frequency_penalty, repetition_penalty, logit_bias: refused unless the server was started with
+    penalties on; then in the ranges of _parse_penalties."""
     prompt = req["prompt"]
     if isinstance(prompt, list) and not _is_token_ids(prompt):
         if len(prompt) != 1:
@@ -290,17 +340,23 @@ def parse_completion_request(req: dict, max_logprobs: int = 0) -> dict:
     else:
         logprobs = None
     for key, default in (("logprobs", None), ("best_of", None), ("suffix", None), ("logit_bias", None)):
-        if key == "logprobs" and max_logprobs >= 1:
+        if (key == "logprobs" and max_logprobs >= 1) or (key == "logit_bias" and penalties):
             continue
         if req.get(key, default) not in (default, 0 if key == "logprobs" else default, 1 if key == "best_of" else default):
             raise ValueError(f"{key} is not implemented")
-    for key in ("presence_penalty", "frequency_penalty"):
-        if float(req.get(key, 0) or 0) != 0:
-            raise ValueError(f"{key} is not implemented")
+    if penalties:
+        pen = _parse_penalties(req)
+    else:
+        for key in ("presence_penalty", "frequency_penalty"):
+            if float(req.get(key, 0) or 0) != 0:
+                raise ValueError(f"{key} is not implemented")
+        if req.get("repetition_penalty") not in (None, 1):
+            raise ValueError("repetition_penalty is not implemented")
+        pen = {}
     seed = req.get("seed")
     return dict(prompt=prompt, max_tokens=max_tokens, temperature=temperature, top_p=top_p, n=n, stop=stop,
                 stream=stream, echo=bool(req.get("echo", False)), seed=None if seed is None else int(seed),
-                logprobs=logprobs, top_k=top_k)
+                logprobs=logprobs, top_k=top_k, penalties=pen)
 
 
 def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 600.0):
@@ -338,7 +394,8 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
                 return self._send(404, {"error": "not found"})
             try:
                 n = int(self.headers.get("Content-Length", "0"))
-                r = parse_completion_request(json.loads(self.rfile.read(n) or b"{}"), sched.max_logprobs)
+                r = parse_completion_request(json.loads(self.rfile.read(n) or b"{}"), sched.max_logprobs,
+                                             sched.penalties)
             except Exception as e:  # noqa: BLE001
                 return self._send(400, {"error": f"bad request: {e}"})
             # the echoed prompt: a token-id prompt's decoding; with log-probabilities, the prompt tokens' strings
@@ -347,7 +404,7 @@ def make_handler(sched: Scheduler, model_name: str, request_timeout_s: float = 6
             for i in range(r["n"]):
                 seed = None if r["seed"] is None else r["seed"] + i
                 it = sched.submit(r["prompt"], r["max_tokens"], r["temperature"], r["top_p"], r["stop"], seed,
-                                  r["logprobs"], r["echo"], r["top_k"])
+                                  r["logprobs"], r["echo"], r["top_k"], r["penalties"])
                 if it is None:          # back-pressure: every slot busy and the admission queue full
                     for x in items:
                         x["cancelled"] = True
@@ -462,15 +519,26 @@ def server_params(content: str, max_batch: int | None = None, kv_cache_gb: float
 def prefix_cache_param(content: str, prefix_cache: bool | None = None, environ=None) -> bool:
     """Whether the Server shares the K/V pages of repeated prompt prefixes: --prefix-cache, else the params'
     prefix_cache (params.json, PARAM_PREFIX_CACHE over it: true / false, 1 / 0, yes / no), else off."""
-    if prefix_cache is not None:
-        return bool(prefix_cache)
+    return _bool_param(content, "prefix_cache", prefix_cache, environ)
+
+
+def penalties_param(content: str, penalties: bool | None = None, environ=None) -> bool:
+    """Whether the Server accepts presence_penalty, frequency_penalty, repetition_penalty and logit_bias: --penalties,
+    else the params' penalties (params.json, PARAM_PENALTIES over it: true / false, 1 / 0, yes / no), else off (they
+    are then a 400)."""
+    return _bool_param(content, "penalties", penalties, environ)
+
+
+def _bool_param(content: str, key: str, cli: bool | None, environ) -> bool:
+    if cli is not None:
+        return bool(cli)
     extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
-    v = extra.get("prefix_cache", False)
+    v = extra.get(key, False)
     if isinstance(v, bool) or v in (0, 1):
         return bool(v)
     if isinstance(v, str) and v.strip().lower() in ("true", "1", "yes", "false", "0", "no"):
         return v.strip().lower() in ("true", "1", "yes")
-    raise ValueError(f"param 'prefix_cache': cannot read {v!r} as a boolean")
+    raise ValueError(f"param {key!r}: cannot read {v!r} as a boolean")
 
 
 def max_logprobs_param(content: str, max_logprobs: int | None = None, environ=None) -> int:
@@ -541,11 +609,13 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
-          prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None):
+          prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None,
+          penalties: bool | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
     prefix_cache = prefix_cache_param(content, prefix_cache)
     kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
     max_logprobs = max_logprobs_param(content, max_logprobs)
+    penalties = penalties_param(content, penalties)
     if prefix_cache and kv_cache_gb is None:
         raise ValueError("prefix_cache shares pages of the paged KV cache: it needs kv_cache_gb")
     if kv_dtype != "bf16" and kv_cache_gb is None:
@@ -554,12 +624,12 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
     t0 = time.time()
     engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype)
     tok = contract.Tokenizer(model_dir)
-    sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs)
+    sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs, penalties=penalties)
     sched.start()
     name = cfg.get("_name_or_path") or cfg.get("model_type", "model")
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
     ready = {"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
-             "max_batch": max_batch, "max_logprobs": max_logprobs}
+             "max_batch": max_batch, "max_logprobs": max_logprobs, "penalties": penalties}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
         ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch, kv_dtype) / 1e6, 2),
@@ -586,10 +656,13 @@ def main(argv=None) -> int:
     ap.add_argument("--max-logprobs", type=int, default=None,
                     help="the most top entries a request may ask for with logprobs, 0..5 (default: param "
                          "max_logprobs, else 0: logprobs > 0 is refused)")
+    ap.add_argument("--penalties", action="store_true", default=None,
+                    help="accept presence_penalty, frequency_penalty, repetition_penalty and logit_bias (default: "
+                         "param penalties, else off: they are refused)")
     a = ap.parse_args(argv)
     try:
         serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype,
-              a.max_logprobs)
+              a.max_logprobs, a.penalties)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()
