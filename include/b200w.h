@@ -368,6 +368,15 @@ typedef struct b200w_penalties {
 B200W_API int b200w_infer_sample_penalized(b200w_ctx* ctx, int n, const b200w_sampling* sampling,
                                            const b200w_penalties* penalties, int32_t* tokens_out,
                                            float* token_logit_out);
+/* Rows per step beyond max_batch, for steps that hold several rows of one slot at consecutive positions (speculative
+ * decoding: a slot's last token and the tokens drafted after it, verified in one step). Sizes every per-row buffer for
+ * max_rows rows (max_batch <= max_rows <= 128, the decode GEMM's row limit; B200W_ERR_INVALID otherwise): the
+ * activations, the index staging, the split-K and attention workspaces, the logits, and the log-probability, sampling
+ * and penalty buffers when they are allocated later; b200w_infer_device_bytes counts them. b200w_infer_step,
+ * b200w_infer_step_logprobs, b200w_infer_sample and b200w_infer_sample_penalized then take up to max_rows rows.
+ * Only between init and the first step or prefill (B200W_ERR_STATE after); it may be repeated until then. A context
+ * that never calls it holds max_batch rows. B200W_ERR_OOM leaves the previous size in place. */
+B200W_API int b200w_infer_set_step_rows(b200w_ctx* ctx, int max_rows);
 
 /* ---- per-kernel hooks for the parity tests (DEVICE pointers, bf16 unless noted) ------------ */
 /* D[M,N] = opA[M,K] opB[N,K]^T (+C). a_mn / b_mn: operand stored [K,M] / [K,N] row-major.

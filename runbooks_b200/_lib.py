@@ -123,6 +123,7 @@ PROTOTYPES = {
     "b200w_infer_prefill_logprobs": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "b200w_infer_sample": (C.c_int, [c_ctx, C.c_int, vp, vp, vp]),
     "b200w_infer_sample_penalized": (C.c_int, [c_ctx, C.c_int, vp, vp, vp, vp]),
+    "b200w_infer_set_step_rows": (C.c_int, [c_ctx, C.c_int]),
     "b200w_op_gemm": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_gemm_bias": (C.c_int, [c_ctx, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,

@@ -196,8 +196,34 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* 
   for (int i = threadIdx.x; i < d / 8; i += blockDim.x) d4[i] = s4[i];
 }
 
-// Attention of one new query token per row over its slot's cache [0, pos]. Block = (row, kv head,
-// group of GT query heads that share that kv head): every K/V row is read once per block.
+// Row groups of a decode step (speculative decoding verifies a slot's last token and its drafts in one step): a group
+// is a maximal run of consecutive rows of one slot at consecutive positions p, p + 1, ..., cut every DECODE_GROUP
+// rows. Both decode attention kernels read a group's K/V once for all its rows; a group of one row is the plain step.
+// Each row attends to its own positions [0, pos], so its output does not depend on the grouping.
+constexpr int DECODE_GROUP = 8;
+// the rows of row r's group, and r's place t in it (the group's first row is r - t)
+__device__ __forceinline__ int group_span(const int32_t* __restrict__ pos, const int32_t* __restrict__ slot, int n,
+                                          int r, int& t) {
+  const int sr = slot[r], pr = pos[r];
+  int s = r;   // the first row of r's run
+  while (s > 0 && slot[s - 1] == sr && pos[s - 1] + (r - s) + 1 == pr) --s;
+  t = (r - s) % DECODE_GROUP;
+  int k = t + 1;
+  while (k < DECODE_GROUP && r - t + k < n && slot[r - t + k] == sr && pos[r - t + k] == pr - t + k) ++k;
+  return k;
+}
+// rows in the group that row r leads, 0 when r does not lead one (it belongs to the group of an earlier row)
+__device__ __forceinline__ int group_rows(const int32_t* __restrict__ pos, const int32_t* __restrict__ slot, int n,
+                                          int r) {
+  int t;
+  const int k = group_span(pos, slot, n, r, t);
+  return t ? 0 : k;
+}
+
+// Attention of the new query tokens over their slot's cache [0, pos]. Block = (group of rows, kv head, ATT_GT of the
+// group's (row, query head) pairs, rows outer, over the heads that share that kv head): every K/V row is read once
+// per block, and each pair keeps its own length pos + 1. GROUPED = false (a step with no two rows of one slot at
+// consecutive positions) makes every row its own group without looking at its neighbours.
 // KV = fp8 reads the e4m3 pool: 8 bytes per 8 dims, a key's K scale (kscale [rows, Hkv]) multiplies its score and
 // its V scale its probability in P V, the row sum running over the unscaled probabilities (bf16: kscale / vscale
 // are not read).
@@ -219,32 +245,36 @@ __device__ __forceinline__ float row_scale(const float* __restrict__ scale, size
   else return 1.f;
 }
 
-template <int DH, typename KV>
-__global__ void __launch_bounds__(ATT_THREADS)
-decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ kcache,
-                   const KV* __restrict__ vcache, const int32_t* __restrict__ pos,
-                   const int32_t* __restrict__ slot, bf16* __restrict__ out, int ldo, int H, int Hkv,
-                   int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
-                   const float* __restrict__ kscale, const float* __restrict__ vscale) {
+template <int DH, typename KV, bool GROUPED>
+__device__ __forceinline__ void
+decode_attn(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ kcache, const KV* __restrict__ vcache,
+            const int32_t* __restrict__ pos, const int32_t* __restrict__ slot, int n, bf16* __restrict__ out, int ldo,
+            int H, int Hkv, int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
+            const float* __restrict__ kscale, const float* __restrict__ vscale) {
   constexpr bool F8 = std::is_same<KV, fp8>::value;
   extern __shared__ float sm[];
   pdl_trigger();
   pdl_wait();
   const int r = blockIdx.x, hk = blockIdx.y, G = H / Hkv;
-  const int g0 = blockIdx.z * ATT_GT;
-  const int ng = min(ATT_GT, G - g0);
-  const int len = pos[r] + 1;
+  const int g0 = blockIdx.z * ATT_GT;               // first (row, head) pair of this block: row r + pair / G
+  const int ng = min(ATT_GT, (GROUPED ? group_rows(pos, slot, n, r) : 1) * G - g0);
+  if (ng <= 0) return;                              // CTA-uniform
+  // pair g0 + g of the block: row r + pair_row(g), query head hk * G + pair_head(g)
+  auto pair_row = [&](int g) { return GROUPED ? (g0 + g) / G : 0; };
+  auto pair_head = [&](int g) { return GROUPED ? (g0 + g) % G : g0 + g; };
+  const int len = pos[r + pair_row(ng - 1)] + 1;   // the longest of the block's rows: its last
   float* sq = sm;                       // [ATT_GT][DH]
   float* sc = sq + ATT_GT * DH;         // [ATT_GT][sc_stride]; reused to combine output slices
   float* red = sc + ATT_GT * sc_stride; // [32]
   const int tid = threadIdx.x;
   for (int i = tid; i < ng * DH; i += ATT_THREADS) {
     const int g = i / DH, c = i % DH;
-    sq[g * DH + c] = __bfloat162float(qkv[static_cast<size_t>(r) * ld + (hk * G + g0 + g) * DH + c]) * scale;
+    sq[g * DH + c] =
+        __bfloat162float(qkv[static_cast<size_t>(r + pair_row(g)) * ld + (hk * G + pair_head(g)) * DH + c]) * scale;
   }
   __syncthreads();
   const int32_t* prow = table + slot[r] * nsplit;   // the slot's table row
-  // scores: one key position per thread, the K row lives in registers for all ng heads
+  // scores: one key position per thread, the K row lives in registers for all ng pairs
   for (int t = tid; t < len; t += ATT_THREADS) {
     const size_t row = cache_row(prow, t) * Hkv + hk;
     const Dims8<KV>* krow = reinterpret_cast<const Dims8<KV>*>(kcache + row * DH);
@@ -272,18 +302,22 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ 
       if (g < ng) sc[g * sc_stride + t] = acc[g];
   }
   __syncthreads();
-  // softmax per head (the V scale joins in P V, once per key for all heads)
+  // softmax per pair over its own positions (the V scale joins in P V, once per key for all pairs); a pair's weights
+  // of the later positions its block reads for longer rows are 0
   float inv_sum[ATT_GT];
   for (int g = 0; g < ng; ++g) {
+    const int lg = GROUPED ? pos[r + pair_row(g)] + 1 : len;
     float m = -INFINITY;
-    for (int t = tid; t < len; t += ATT_THREADS) m = fmaxf(m, sc[g * sc_stride + t]);
+    for (int t = tid; t < lg; t += ATT_THREADS) m = fmaxf(m, sc[g * sc_stride + t]);
     m = block_reduce(m, red, true);
     float s = 0.f;
-    for (int t = tid; t < len; t += ATT_THREADS) {
+    for (int t = tid; t < lg; t += ATT_THREADS) {
       const float e = __expf(sc[g * sc_stride + t] - m);
       sc[g * sc_stride + t] = e;
       s += e;
     }
+    if (GROUPED)
+      for (int t = lg + tid; t < len; t += ATT_THREADS) sc[g * sc_stride + t] = 0.f;
     inv_sum[g] = 1.f / block_reduce(s, red, false);
   }
   __syncthreads();
@@ -341,14 +375,40 @@ decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ 
     const int g = i / DH, dim = i % DH;
     float a = 0.f;
     for (int s2 = 0; s2 < SLICES; ++s2) a += so[(s2 * ATT_GT + g) * DH + dim];
-    out[static_cast<size_t>(r) * ldo + (hk * G + g0 + g) * DH + dim] = __float2bfloat16_rn(a * inv_sum[g]);
+    out[static_cast<size_t>(r + pair_row(g)) * ldo + (hk * G + pair_head(g)) * DH + dim] =
+        __float2bfloat16_rn(a * inv_sum[g]);
   }
+}
+
+// the per-row kernel (a plain step) and the grouped one
+template <int DH, typename KV>
+__global__ void __launch_bounds__(ATT_THREADS)
+decode_attn_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ kcache, const KV* __restrict__ vcache,
+                   const int32_t* __restrict__ pos, const int32_t* __restrict__ slot, int n, bf16* __restrict__ out,
+                   int ldo, int H, int Hkv, int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
+                   const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  decode_attn<DH, KV, false>(qkv, ld, kcache, vcache, pos, slot, n, out, ldo, H, Hkv, sc_stride, scale, table, nsplit,
+                             kscale, vscale);
+}
+template <int DH, typename KV>
+__global__ void __launch_bounds__(ATT_THREADS)
+decode_attn_grouped_kernel(const bf16* __restrict__ qkv, int ld, const KV* __restrict__ kcache,
+                           const KV* __restrict__ vcache, const int32_t* __restrict__ pos,
+                           const int32_t* __restrict__ slot, int n, bf16* __restrict__ out, int ldo, int H, int Hkv,
+                           int sc_stride, float scale, const int32_t* __restrict__ table, int nsplit,
+                           const float* __restrict__ kscale, const float* __restrict__ vscale) {
+  decode_attn<DH, KV, true>(qkv, ld, kcache, vcache, pos, slot, n, out, ldo, H, Hkv, sc_stride, scale, table, nsplit,
+                            kscale, vscale);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Decode attention on the tensor cores (wgmma) for grouped / multi-query models. CTA = (128-key block,
-// kv head, row). The G = H / Hkv query heads of the group are rows of a 128-row tile (zero rows above G),
-// warpgroup wg owning rows [64 wg, 64 wg + 64) (a warpgroup whose rows are all padding has nothing to do):
+// kv head, row). The (row, query head) pairs of a group of rows, rows outer over the G = H / Hkv query heads of the
+// kv head, are the rows of 128-row tiles (zero rows after the last pair); the CTA of the group's row t serves tile t
+// (a group of one row: its G heads, zero rows above G), so a group's K/V block is read once per tile instead of once
+// per row. Warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile (a warpgroup whose rows are all padding has nothing
+// to do), and each pair masks the keys beyond its own row's length. GROUPED = false (no two rows of one slot at
+// consecutive positions): every row is its own group, without looking at its neighbours:
 //   S[64, 128 keys] = Q K^T   (A = Q K-major from smem, B = K block K-major, TMA from the cache)
 //   P = 2^(S * scale_log2 - m) per head row, keys >= len masked to 0, bf16 in registers
 //   O[64, DH] = P V           (A = P from registers, B = V block MN-major)
@@ -392,10 +452,32 @@ __device__ __forceinline__ void widen_e4m3_box(const uint8_t* __restrict__ src, 
 }
 
 static_assert(TC_KB == KV_PAGE, "a key block of the tensor-core decode attention is one cache page");
-template <int DH, typename KV>
+
+// Tile rows [0, 128) <- the queries of pairs b .. b + 127 of group row r (pair p: row r + p / G, head hk * G + p % G),
+// zero after the last pair P - 1, into the K-major A tile sQ (not GROUPED: row r alone, pair p is head hk * G + p)
+template <int DH, bool GROUPED>
+__device__ __forceinline__ void load_q_tile(uint8_t* sQ, const bf16* __restrict__ qkv, int ld, int r, int hk, int G,
+                                            int P, int b, int tid) {
+  for (int i = tid; i < 128 * (DH / 8); i += TC_THREADS) {
+    const int g = i / (DH / 8), c = i % (DH / 8), p = b + g;
+    const uint4 v = p < P ? reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(r + (GROUPED ? p / G : 0)) * ld +
+                                                           (hk * G + (GROUPED ? p % G : p)) * DH)[c]
+                          : make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4*>(sQ + (c / 8) * TC_ATOM + sw128_offset(g, c % 8)) = v;
+  }
+}
+
+template <int DH, typename KV, bool GROUPED>
+__device__ __forceinline__ void
+decode_attn_tc_tile(const uint8_t* sQ, const uint8_t* sK, const uint8_t* sV, const float* sS,
+                    const int32_t* __restrict__ pos, int r, int b, int G, int P, int k0, float scale_log2,
+                    float* __restrict__ part_o, float2* __restrict__ part_ml, int H, int hk, int nsplit, int split,
+                    int wg, int wi, int lane);
+
+template <int DH, typename KV, bool GROUPED>
 __device__ __forceinline__ void
 decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
-                      const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
+                      const int32_t* __restrict__ slot, int n, float* __restrict__ part_o, float2* __restrict__ part_ml,
                       int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table,
                       const float* __restrict__ kscale, const float* __restrict__ vscale) {
   constexpr bool F8 = std::is_same<KV, fp8>::value;
@@ -404,10 +486,18 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
   const int tid = threadIdx.x, lane = tid & 31;
   if (tid == 0) pdl_trigger();
   pdl_wait();  // q / cache rows / pos come from the kernels before this one
-  const int len = pos[r] + 1;
+  int t = 0;                                        // row r's place in its group: the CTA serves tile t
+  const int nr = GROUPED ? group_span(pos, slot, n, r, t) : 1;
+  const int r0 = r - t, b = 128 * t;                // the group's first row, the tile's first pair
+  int len = pos[r] + 1;                             // the tile's longest row: the row of its last pair
+  if constexpr (GROUPED) {
+    const int pairs = nr * (H / Hkv);
+    if (b >= pairs) return;                         // CTA-uniform: the group has fewer tiles than rows
+    len = pos[r0 + (min(pairs, b + 128) - 1) / (H / Hkv)] + 1;
+  }
   const int k0 = split * TC_KB;
-  if (k0 >= len) return;  // CTA-uniform: this block holds no key of the row (the merge knows from len)
-  const int G = H / Hkv;
+  if (k0 >= len) return;  // CTA-uniform: this block holds no key of the tile's rows (the merge knows from len)
+  const int G = H / Hkv, P = nr * G;                // P: the group's pairs
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -442,13 +532,8 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
       tma_load_2d(sV + a * TC_ATOM, &tm_v, bar_kv, hk * DH + a * 64, row0);
     }
   }
-  // the group's query rows (zero above G) -> the K-major A tile
-  for (int i = tid; i < 128 * (DH / 8); i += TC_THREADS) {
-    const int g = i / (DH / 8), c = i % (DH / 8);
-    const uint4 v = g < G ? reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(r) * ld + (hk * G + g) * DH)[c]
-                          : make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4*>(sQ + (c / 8) * TC_ATOM + sw128_offset(g, c % 8)) = v;
-  }
+  // the tile's query rows (zero after the last pair) -> the K-major A tile
+  load_q_tile<DH, GROUPED>(sQ, qkv, ld, r0, hk, G, P, b, tid);
   if constexpr (F8) {
     mbar_wait(bar_kv, 0);
     constexpr int NV = 8 * DH / TC_THREADS;   // 16-byte items of the V box per thread
@@ -463,9 +548,21 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
   fence_proxy_async_smem();
   __syncthreads();
   const int wg = tid >> 7, wi = (tid >> 5) & 3;
-  if (wg * 64 >= G) return;  // warpgroup-uniform: every row of this warpgroup is padding
+  if (b + wg * 64 >= P) return;  // warpgroup-uniform: every row of this warpgroup is padding
   if constexpr (!F8) mbar_wait(bar_kv, 0);
+  decode_attn_tc_tile<DH, KV, GROUPED>(sQ, sK, sV, sS, pos, r0, b, G, P, k0, scale_log2, part_o, part_ml, H, hk, nsplit,
+                                       split, wg, wi, lane);
+}
 
+// The tile of pairs [b, b + 128) of the group that starts at row r: S = Q K^T, the masked softmax of the block,
+// O = P V, and the partials of its pairs.
+template <int DH, typename KV, bool GROUPED>
+__device__ __forceinline__ void
+decode_attn_tc_tile(const uint8_t* sQ, const uint8_t* sK, const uint8_t* sV, const float* sS,
+                    const int32_t* __restrict__ pos, int r, int b, int G, int P, int k0, float scale_log2,
+                    float* __restrict__ part_o, float2* __restrict__ part_ml, int H, int hk, int nsplit, int split,
+                    int wg, int wi, int lane) {
+  constexpr bool F8 = std::is_same<KV, fp8>::value;
   float s[TC_KB / 2];
   {
     const uint64_t da = wg_desc(smem_u32(sQ) + wg * 64 * 128, 16), db = wg_desc(smem_u32(sK), 16);
@@ -478,7 +575,15 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
     wg_wait<0>();
     wg_fence_regs(s);
   }
-  const int valid = min(TC_KB, len - k0);
+  // this thread's two pairs (tile rows wg * 64 + wi * 16 + lane / 4 + 8 h) and their keys in the block (not GROUPED:
+  // those of row r for both, the padding rows' included, whose results are not stored)
+  int pair[2], valid[2];
+  const int valid_r = min(TC_KB, pos[r] + 1 - k0);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    pair[h] = b + wg * 64 + wi * 16 + (lane >> 2) + 8 * h;
+    valid[h] = !GROUPED ? valid_r : pair[h] < P ? min(TC_KB, pos[r + pair[h] / G] + 1 - k0) : 0;
+  }
   const int c0 = 2 * (lane & 3);
   if constexpr (F8) {   // key column c of the scores times its K scale
 #pragma unroll
@@ -490,17 +595,21 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
 #pragma unroll
   for (int jj = 0; jj < TC_KB / 8; ++jj)
 #pragma unroll
-    for (int e = 0; e < 2; ++e)
-      if (8 * jj + c0 + e < valid) {
+    for (int e = 0; e < 2; ++e) {
+      if constexpr (GROUPED) {
+        if (8 * jj + c0 + e < valid[0]) m[0] = fmaxf(m[0], s[4 * jj + e]);
+        if (8 * jj + c0 + e < valid[1]) m[1] = fmaxf(m[1], s[4 * jj + 2 + e]);
+      } else if (8 * jj + c0 + e < valid[0]) {   // one row: one mask for both
         m[0] = fmaxf(m[0], s[4 * jj + e]);
         m[1] = fmaxf(m[1], s[4 * jj + 2 + e]);
       }
+    }
   float l[2] = {0.f, 0.f};
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
     m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
-    m[h] *= scale_log2;  // scale > 0 commutes with max; key 0 of the block is always valid, so m is finite
+    m[h] *= scale_log2;  // scale > 0 commutes with max; finite unless the block holds no key of the pair (valid <= 0)
   }
   uint32_t pa[TC_KB / 16][4];
 #pragma unroll
@@ -509,8 +618,8 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
     for (int h = 0; h < 2; ++h) {
       float p0 = ex2f(fmaf(s[4 * jj + 2 * h], scale_log2, -m[h]));
       float p1 = ex2f(fmaf(s[4 * jj + 2 * h + 1], scale_log2, -m[h]));
-      if (8 * jj + c0 >= valid) p0 = 0.f;
-      if (8 * jj + c0 + 1 >= valid) p1 = 0.f;
+      if (8 * jj + c0 >= valid[h]) p0 = 0.f;
+      if (8 * jj + c0 + 1 >= valid[h]) p1 = 0.f;
       if constexpr (F8) {   // the row sum over the unscaled probabilities, P V over the V-scaled ones
         l[h] += p0 + p1;
         pa[jj / 2][(jj & 1) * 2 + h] = pack_bf16x2(p0 * sS[TC_KB + 8 * jj + c0], p1 * sS[TC_KB + 8 * jj + c0 + 1]);
@@ -540,9 +649,9 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int g = wg * 64 + wi * 16 + (lane >> 2) + 8 * h;
-    if (g >= G) continue;
-    const size_t pidx = (static_cast<size_t>(r) * H + hk * G + g) * nsplit + split;
+    if (pair[h] >= P || valid[h] <= 0) continue;   // padding, or the block lies beyond this pair's row
+    const size_t pidx = GROUPED ? (static_cast<size_t>(r + pair[h] / G) * H + hk * G + pair[h] % G) * nsplit + split
+                                : (static_cast<size_t>(r) * H + hk * G + pair[h]) * nsplit + split;
     if ((lane & 3) == 0) part_ml[pidx] = make_float2(m[h], l[h]);
     float* po = part_o + pidx * DH + c0;
 #pragma unroll
@@ -551,25 +660,22 @@ decode_attn_tc(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const bf16* __r
   }
 }
 
-template <int DH>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-decode_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
-                      const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
-                      const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
-                      int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table) {
-  decode_attn_tc<DH, bf16>(tm_k, tm_v, qkv, ld, pos, slot, part_o, part_ml, H, Hkv, nsplit, scale_log2, table, nullptr,
-                           nullptr);
-}
-template <int DH>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-decode_attn_tc_fp8_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
-                          const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos,
-                          const int32_t* __restrict__ slot, float* __restrict__ part_o, float2* __restrict__ part_ml,
-                          int H, int Hkv, int nsplit, float scale_log2, const int32_t* __restrict__ table,
-                          const float* __restrict__ kscale, const float* __restrict__ vscale) {
-  decode_attn_tc<DH, fp8>(tm_k, tm_v, qkv, ld, pos, slot, part_o, part_ml, H, Hkv, nsplit, scale_log2, table, kscale,
-                          vscale);
-}
+// bf16 and fp8 pools, each per row (a plain step) and grouped
+#define DECODE_ATTN_TC_KERNEL(NAME, KV, GROUPED)                                                                     \
+  template <int DH>                                                                                                  \
+  __global__ void __launch_bounds__(TC_THREADS, 1)                                                                   \
+  NAME(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,                           \
+       const bf16* __restrict__ qkv, int ld, const int32_t* __restrict__ pos, const int32_t* __restrict__ slot, int n, \
+       float* __restrict__ part_o, float2* __restrict__ part_ml, int H, int Hkv, int nsplit, float scale_log2,        \
+       const int32_t* __restrict__ table, const float* __restrict__ kscale, const float* __restrict__ vscale) {      \
+    decode_attn_tc<DH, KV, GROUPED>(tm_k, tm_v, qkv, ld, pos, slot, n, part_o, part_ml, H, Hkv, nsplit, scale_log2,  \
+                                    table, kscale, vscale);                                                          \
+  }
+DECODE_ATTN_TC_KERNEL(decode_attn_tc_kernel, bf16, false)
+DECODE_ATTN_TC_KERNEL(decode_attn_tc_grouped_kernel, bf16, true)
+DECODE_ATTN_TC_KERNEL(decode_attn_tc_fp8_kernel, fp8, false)
+DECODE_ATTN_TC_KERNEL(decode_attn_tc_fp8_grouped_kernel, fp8, true)
+#undef DECODE_ATTN_TC_KERNEL
 
 // out[r, h*DH + d] = sum_s 2^(m_s - M) O_s[d] / sum_s 2^(m_s - M) l_s over the ceil(len / 128) blocks of row r
 template <int DH>
@@ -1465,6 +1571,9 @@ struct IParam {
 struct Infer {
   b200w_infer_arch a{};
   int max_batch = 0;
+  int max_rows = 0;     // rows a step may hold (b200w_infer_set_step_rows; max_batch unless set)
+  bool used = false;    // a step or prefill has run: the per-row buffers are fixed from then on
+  bool grouped = false; // the step being enqueued has rows of one slot at consecutive positions (decode_attention)
   std::vector<IParam> params;
   std::unordered_map<std::string, int> index;
   size_t n_elems = 0;
@@ -1481,20 +1590,21 @@ struct Infer {
   uint8_t* t_lm = nullptr;
   bool tiled_valid = false, use_tiled = true;
   int qd = 0, kd = 0, qkvd = 0, ld_cat = 0;  // Falcon: ld_cat = qd + f, the [attention | mlp hidden] operand
-  // decode activations [max_batch, *]
+  // decode activations [max_rows, *]
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
   KVCache kv;
   size_t pf_limit = 0;  // paged: tokens of the preallocated prefill workspace, the most one prefill call takes
   float* inv_freq = nullptr;
-  float* ws = nullptr;          // split-K workspace [max_batch, max N] (kept zeroed)
+  float* ws = nullptr;          // split-K workspace [max_batch, max N] (kept zeroed; the decode GEMM splits K only
+                                // when it is set and reads nothing from it, so it does not grow with max_rows)
   unsigned* counters = nullptr;
-  float* part_o = nullptr;      // tensor-core decode attention partials [max_batch, H, nsplit, dh]
-  float2* part_ml = nullptr;    // [max_batch, H, nsplit] (max, sum)
+  float* part_o = nullptr;      // tensor-core decode attention partials [max_rows, H, nsplit, dh]
+  float2* part_ml = nullptr;    // [max_rows, H, nsplit] (max, sum)
   int32_t *tok = nullptr, *pos = nullptr, *slot = nullptr, *next = nullptr;
-  // pinned host staging, max_batch each, one allocation: a step's tokens, positions, slots; any call's next tokens
+  // pinned host staging, max_rows each, one allocation: a step's tokens, positions, slots; any call's next tokens
   int32_t *pin_tok = nullptr, *pin_pos = nullptr, *pin_slot = nullptr, *pin_next = nullptr;
-  std::unordered_map<int, cudaGraphExec_t> graphs;  // whole decode step per row count
+  std::unordered_map<int, cudaGraphExec_t> graphs;  // whole decode step per row count and grouping (graph_key)
   std::unordered_map<int, int> warm;
   // prefill buffers, grown on demand to the largest n_seqs * padded_len seen
   size_t pf_cap = 0;
@@ -1504,8 +1614,8 @@ struct Infer {
   int32_t *pf_tok = nullptr, *pf_len = nullptr, *pf_slot = nullptr, *pf_last = nullptr, *pf_start = nullptr;
   int32_t* pf_pos = nullptr;   // OPT after a cached prefix: the learned-position row of every token
   int32_t* pf_pin = nullptr;   // pinned staging of a prefill call of up to pf_cap rows (stage_prefill)
-  // token log-probabilities, allocated by the first call that asks for them: the next-token rows [max_batch]
-  // (lse, token_lp, top ids / top log-probabilities [max_batch, B200W_MAX_TOP_LOGPROBS]); for prompt scoring a bf16
+  // token log-probabilities, allocated by the first call that asks for them: the next-token rows [max_rows]
+  // (lse, token_lp, top ids / top log-probabilities [max_rows, B200W_MAX_TOP_LOGPROBS]); for prompt scoring a bf16
   // chunk of lm_head outputs [lp_chunk_rows, V] and per-row outputs for lp_cap prefill rows
   float *nx_lse = nullptr, *nx_tok = nullptr, *nx_top = nullptr;
   int32_t* nx_ids = nullptr;
@@ -1517,7 +1627,7 @@ struct Infer {
   // the per-row parameters and results of a call (sample_bytes), on the device and pinned, from the first such call
   int logits_rows = 0;
   uint8_t *sp_dev = nullptr, *sp_pin = nullptr;
-  // penalties, from the first b200w_infer_sample_penalized call: the penalized rows [max_batch, V] sample_kernel then
+  // penalties, from the first b200w_infer_sample_penalized call: the penalized rows [max_rows, V] sample_kernel then
   // reads, and the entry staging (penalty_bytes), on the device and pinned, grown to the largest call's
   bf16* pen_rows = nullptr;
   uint8_t *pen_dev = nullptr, *pen_pin = nullptr;
@@ -1544,6 +1654,14 @@ struct Infer {
         allocs.erase(allocs.begin() + i);
         return;
       }
+  }
+  // release, and the count drops the n * sizeof(T) bytes alloc<T>(n) added for p
+  template <typename T>
+  void release_counted(T*& p, size_t n) {
+    if (!p) return;
+    release(p);
+    bytes -= static_cast<int64_t>(((n * sizeof(T) + 255) / 256) * 256);
+    p = nullptr;
   }
   ~Infer() {
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
@@ -1715,7 +1833,7 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
 }
 
 // the tensor-core decode attention and the merge of its blocks -> out [n, ldo]
-template <int DH, typename KV>
+template <int DH, typename KV, bool GROUPED>
 void decode_attention_tc(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n,
                          int H, int Hkv, float scale_log2, float* part_o, float2* part_ml, bf16* out, int ldo,
                          cudaStream_t s) {
@@ -1723,25 +1841,17 @@ void decode_attention_tc(const KVLayer& c, const bf16* q, int ld_q, const int32_
   const int smem = tc_smem_bytes<DH>() + (F8 ? TC_SCALE_BYTES : 0);
   const KVTmaps tm = kv_tmaps(c, Hkv, DH);
   static PerDeviceOnce once;
-  if constexpr (F8) {
-    once.run([&] {
-      B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_fp8_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    });
-    launch_pdl(decode_attn_tc_fp8_kernel<DH>, dim3(c.nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tm.k, tm.v, q, ld_q,
-               pos, slot, part_o, part_ml, H, Hkv, c.nsplit, scale_log2, c.table, c.kscale, c.vscale);
-  } else {
-    once.run([&] {
-      B200W_CUDA(cudaFuncSetAttribute(decode_attn_tc_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    });
-    launch_pdl(decode_attn_tc_kernel<DH>, dim3(c.nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tm.k, tm.v, q, ld_q, pos,
-               slot, part_o, part_ml, H, Hkv, c.nsplit, scale_log2, c.table);
-  }
+  auto kern = F8 ? (GROUPED ? decode_attn_tc_fp8_grouped_kernel<DH> : decode_attn_tc_fp8_kernel<DH>)
+                 : (GROUPED ? decode_attn_tc_grouped_kernel<DH> : decode_attn_tc_kernel<DH>);
+  once.run([&] { B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); });
+  launch_pdl(kern, dim3(c.nsplit, Hkv, n), dim3(TC_THREADS), smem, s, tm.k, tm.v, q, ld_q, pos, slot, n, part_o,
+             part_ml, H, Hkv, c.nsplit, scale_log2, c.table, c.kscale, c.vscale);
   launch_pdl(decode_attn_merge_kernel<DH>, dim3(cdiv(H, 256 / DH), n), dim3(256), 0, s, part_o, part_ml, pos, out, ldo,
              H, c.nsplit);
 }
 
 // the CUDA-core decode attention -> out [n, ldo]
-template <int DH, typename KV>
+template <int DH, typename KV, bool GROUPED>
 void decode_attention_cc(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n,
                          int H, int Hkv, int max_ctx, bf16* out, int ldo, cudaStream_t s) {
   const int slices = ATT_THREADS / (DH / 8);   // staging area: slices * ATT_GT * dh floats
@@ -1749,31 +1859,40 @@ void decode_attention_cc(const KVLayer& c, const bf16* q, int ld_q, const int32_
   const size_t att_smem = (static_cast<size_t>(ATT_GT) * DH + static_cast<size_t>(ATT_GT) * sc_stride + 32) * 4;
   B200W_CHECK(att_smem <= 200 * 1024, "max_ctx too large for the decode attention kernel");
   static PerDeviceOnce once;
-  once.run([&] {
-    B200W_CUDA(cudaFuncSetAttribute(decode_attn_kernel<DH, KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  });
-  launch_pdl(decode_attn_kernel<DH, KV>, dim3(n, Hkv, (H / Hkv + ATT_GT - 1) / ATT_GT), dim3(ATT_THREADS), att_smem, s,
-             q, ld_q, static_cast<const KV*>(c.k), static_cast<const KV*>(c.v), pos, slot, out, ldo, H, Hkv, sc_stride,
-             1.f / sqrtf(static_cast<float>(DH)), c.table, c.nsplit, static_cast<const float*>(c.kscale),
+  auto kern = GROUPED ? decode_attn_grouped_kernel<DH, KV> : decode_attn_kernel<DH, KV>;
+  once.run([&] { B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); });
+  // z: the (row, head) pairs of a full group, ATT_GT per block; blocks past a group's pairs return at once
+  launch_pdl(kern, dim3(n, Hkv, cdiv((GROUPED ? DECODE_GROUP : 1) * (H / Hkv), ATT_GT)), dim3(ATT_THREADS), att_smem,
+             s, q, ld_q, static_cast<const KV*>(c.k), static_cast<const KV*>(c.v), pos, slot, n, out, ldo, H, Hkv,
+             sc_stride, 1.f / sqrtf(static_cast<float>(DH)), c.table, c.nsplit, static_cast<const float*>(c.kscale),
              static_cast<const float*>(c.vscale));
 }
 
 // Attention of the n new tokens (queries q [n, ld_q], head h at column h * dh; pos / slot DEVICE [n]) over their cache
 // slots -> out [n, ldo]: on the tensor cores when H / Hkv >= 4 (partials part_o [n, H, nsplit, dh] and part_ml
-// [n, H, nsplit]), else on the CUDA cores (max_ctx sizes the score staging). Returns the launches.
+// [n, H, nsplit]), else on the CUDA cores (max_ctx sizes the score staging). grouped: some rows share a slot at
+// consecutive positions (their K/V is then read once per group; the kernels without it treat each row alone, which
+// is what the plain step does). Returns the launches.
 int decode_attention(const KVLayer& c, const bf16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n, int H,
-                     int Hkv, int dh, int max_ctx, float* part_o, float2* part_ml, bf16* out, int ldo, cudaStream_t s) {
+                     int Hkv, int dh, int max_ctx, float* part_o, float2* part_ml, bf16* out, int ldo, cudaStream_t s,
+                     bool grouped) {
   const bool f8 = c.dtype == B200W_KV_FP8_E4M3;
   if (H / Hkv >= 4) {
-    // grouped / multi-query: the group is the M dimension of a tensor-core tile
+    // grouped / multi-query: the group is the M dimension of a tensor-core tile. Row groups pay here only when two
+    // rows' heads share a tile; with more than 64 heads per kv head (Falcon-7B: 71) every row of a group still needs
+    // a tile of its own, and the grouped kernel measured no faster than the per-row one (DESIGN §3.5).
     const float scale_log2 = 1.f / sqrtf(static_cast<float>(dh)) * 1.4426950408889634f;
-    auto tc = dh == 64 ? (f8 ? decode_attention_tc<64, fp8> : decode_attention_tc<64, bf16>)
-                       : (f8 ? decode_attention_tc<128, fp8> : decode_attention_tc<128, bf16>);
+    auto tc = grouped && 2 * (H / Hkv) <= 128 ? (dh == 64 ? (f8 ? decode_attention_tc<64, fp8, true> : decode_attention_tc<64, bf16, true>)
+                                  : (f8 ? decode_attention_tc<128, fp8, true> : decode_attention_tc<128, bf16, true>))
+                      : (dh == 64 ? (f8 ? decode_attention_tc<64, fp8, false> : decode_attention_tc<64, bf16, false>)
+                                  : (f8 ? decode_attention_tc<128, fp8, false> : decode_attention_tc<128, bf16, false>));
     tc(c, q, ld_q, pos, slot, n, H, Hkv, scale_log2, part_o, part_ml, out, ldo, s);
     return 2;
   }
-  auto cc = dh == 64 ? (f8 ? decode_attention_cc<64, fp8> : decode_attention_cc<64, bf16>)
-                     : (f8 ? decode_attention_cc<128, fp8> : decode_attention_cc<128, bf16>);
+  auto cc = grouped ? (dh == 64 ? (f8 ? decode_attention_cc<64, fp8, true> : decode_attention_cc<64, bf16, true>)
+                                : (f8 ? decode_attention_cc<128, fp8, true> : decode_attention_cc<128, bf16, true>))
+                    : (dh == 64 ? (f8 ? decode_attention_cc<64, fp8, false> : decode_attention_cc<64, bf16, false>)
+                                : (f8 ? decode_attention_cc<128, fp8, false> : decode_attention_cc<128, bf16, false>));
   cc(c, q, ld_q, pos, slot, n, H, Hkv, max_ctx, out, ldo, s);
   return 1;
 }
@@ -1833,7 +1952,7 @@ void attend(Pass& p, int l) {
   if (p.decode) {
     m->kv.append(l, p.qkv, qkvd, m->inv_freq, m->pos, m->slot, p.rows, H, dh, rope, p.s); ++p.nl;
     p.nl += decode_attention(m->kv.layer(l), p.qkv, qkvd, m->pos, m->slot, p.rows, H, Hkv, dh, a.max_ctx, m->part_o,
-                             m->part_ml, p.cat, ldc, p.s);
+                             m->part_ml, p.cat, ldc, p.s, m->grouped);
     return;
   }
   // q / k rotated and K / V into the cache; a cold prefill attends over the bf16 activations, on either pool, with
@@ -2005,7 +2124,7 @@ int check_logprobs(const b200w_logprobs* lp) {
 
 void ensure_next_logprobs(Infer* m) {
   if (m->nx_lse) return;
-  const size_t B = m->max_batch, K = B200W_MAX_TOP_LOGPROBS;
+  const size_t B = m->max_rows, K = B200W_MAX_TOP_LOGPROBS;
   float* p = m->alloc<float>(B * (2 + 2 * K));
   m->nx_lse = p;
   m->nx_tok = p + B;
@@ -2155,6 +2274,70 @@ void check_weights_unshared(const Infer* m) {
   if (m->kv.retained) throw StateError("KV pages are retained: cached K/V belong to the weights that computed them");
 }
 
+// The buffers of the decode step that hold one entry per row: the activations, the attention partials, the index
+// vectors and their pinned staging. free_rows releases those of B rows that exist.
+void free_rows(Infer* m, size_t B) {
+  const auto& a = m->a;
+  const size_t d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size;
+  const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
+  const size_t part = static_cast<size_t>(a.num_heads) * m->kv.nsplit;
+  for (bf16** p : {&m->h, &m->h2, &m->nrm}) m->release_counted(*p, B * d);
+  m->release_counted(m->qkv, B * m->qkvd);
+  m->release_counted(m->cat, B * m->ld_cat);
+  m->release_counted(m->mid, B * fmid);
+  m->release_counted(m->act, B * f);
+  m->release_counted(m->logits, B * V);
+  m->release_counted(m->part_o, B * part * a.head_dim);
+  m->release_counted(m->part_ml, B * part);
+  for (int32_t** p : {&m->tok, &m->pos, &m->slot, &m->next}) m->release_counted(*p, B);
+  if (m->pin_tok) cudaFreeHost(m->pin_tok);
+  m->pin_tok = m->pin_pos = m->pin_slot = m->pin_next = nullptr;
+  m->max_rows = 0;
+}
+
+void alloc_rows(Infer* m, size_t B) {
+  const auto& a = m->a;
+  const size_t d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size, qkvd = m->qkvd, ldc = m->ld_cat;
+  const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
+  const bool tc = a.num_heads / a.num_kv_heads >= 4;
+  const size_t part = static_cast<size_t>(a.num_heads) * m->kv.nsplit;
+  m->h = m->alloc<bf16>(B * d);
+  m->h2 = m->alloc<bf16>(B * d);
+  m->nrm = m->alloc<bf16>(B * d);
+  m->qkv = m->alloc<bf16>(B * qkvd);
+  m->cat = m->alloc<bf16>(B * ldc);
+  m->mid = m->alloc<bf16>(B * fmid);
+  m->act = m->alloc<bf16>(B * f);
+  m->logits = m->alloc<bf16>(B * V);
+  if (tc) {
+    m->part_o = m->alloc<float>(B * part * a.head_dim);
+    m->part_ml = m->alloc<float2>(B * part);
+  }
+  m->tok = m->alloc<int32_t>(B);
+  m->pos = m->alloc<int32_t>(B);
+  m->slot = m->alloc<int32_t>(B);
+  m->next = m->alloc<int32_t>(B);
+  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin_tok), 4 * B * sizeof(int32_t)));
+  m->pin_pos = m->pin_tok + B;
+  m->pin_slot = m->pin_tok + 2 * B;
+  m->pin_next = m->pin_tok + 3 * B;
+  m->max_rows = static_cast<int>(B);
+}
+
+// Sizes the per-row buffers of the decode step for R rows. If that fails, the buffers for the rows held before are
+// allocated again (they were just freed) and the error goes on to the caller: the context stays usable.
+void step_rows(Infer* m, int R) {
+  const int old = m->max_rows;
+  free_rows(m, old);
+  try {
+    alloc_rows(m, R);
+  } catch (...) {
+    free_rows(m, R);
+    if (old) alloc_rows(m, old);
+    throw;
+  }
+}
+
 // b200w_infer_init (n_pages 0: the contiguous cache) and b200w_infer_init_paged_kv
 void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int n_pages, int64_t prefill_tokens,
                 int kv_dtype = B200W_KV_BF16) {
@@ -2186,18 +2369,8 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
   build(m.get());
   const auto& a = m->a;
-  const size_t B = max_batch, d = a.hidden_size, f = a.intermediate_size;
-  const size_t qd = m->qd, kd = m->kd;
+  const size_t B = max_batch;
   m->w = m->alloc<bf16>(m->n_elems);
-  m->h = m->alloc<bf16>(B * d);
-  m->h2 = m->alloc<bf16>(B * d);
-  m->nrm = m->alloc<bf16>(B * d);
-  m->qkv = m->alloc<bf16>(B * (qd + 2 * kd));
-  m->cat = m->alloc<bf16>(B * m->ld_cat);
-  const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
-  m->mid = m->alloc<bf16>(B * fmid);
-  m->act = m->alloc<bf16>(B * f);
-  m->logits = m->alloc<bf16>(B * a.vocab_size);
   m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim,
              [&](size_t bytes) { return static_cast<void*>(m->alloc<uint8_t>(bytes)); });
   if (m->kv.paged) {
@@ -2205,24 +2378,15 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
     m->pf_limit = static_cast<size_t>(prefill_tokens);
     ensure_prefill(m.get(), m->pf_limit);
   }
-  if (a.num_heads / a.num_kv_heads >= 4) {
-    m->part_o = m->alloc<float>(B * a.num_heads * m->kv.nsplit * a.head_dim);
-    m->part_ml = m->alloc<float2>(B * a.num_heads * m->kv.nsplit);
-  }
-  m->tok = m->alloc<int32_t>(B);
-  m->pos = m->alloc<int32_t>(B);
-  m->slot = m->alloc<int32_t>(B);
-  m->next = m->alloc<int32_t>(B);
+  step_rows(m.get(), max_batch);
   m->pf_len = m->alloc<int32_t>(B);
   m->pf_slot = m->alloc<int32_t>(B);
   m->pf_last = m->alloc<int32_t>(B);
   m->pf_start = m->alloc<int32_t>(B);
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin_tok), 4 * B * sizeof(int32_t)));
-  m->pin_pos = m->pin_tok + B;
-  m->pin_slot = m->pin_tok + 2 * B;
-  m->pin_next = m->pin_tok + 3 * B;
   m->inv_freq = m->alloc<float>(a.head_dim / 2);
-  const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + qd + 2 * kd, d});
+  const size_t f = a.intermediate_size, fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
+  const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + m->qkvd,
+                                         static_cast<size_t>(a.hidden_size)});
   m->ws = m->alloc<float>(B * max_n);
   m->counters = m->alloc<unsigned>((max_n + 127) / 128);
   B200W_CUDA(cudaMemset(m->ws, 0, B * max_n * sizeof(float)));
@@ -2308,7 +2472,7 @@ void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, co
   std::unique_ptr<void, cudaError_t (*)(void*)> owner(part, cudaFree);
   float* part_o = static_cast<float*>(part);
   decode_attention(c, static_cast<const bf16*>(q), ld_q, positions, slots, n, H, Hkv, dh, nsplit * KV_PAGE, part_o,
-                   reinterpret_cast<float2*>(part_o + n_part * dh), static_cast<bf16*>(out), ld_out, s);
+                   reinterpret_cast<float2*>(part_o + n_part * dh), static_cast<bf16*>(out), ld_out, s, false);
   B200W_CUDA(cudaGetLastError());
   B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed on return
 }
@@ -2481,6 +2645,15 @@ int b200w_infer_init_paged(b200w_ctx* ctx, const b200w_infer_arch* arch, int max
   return b200w_infer_init_paged_kv(ctx, arch, max_batch, n_pages, prefill_tokens, B200W_KV_BF16);
 }
 
+int b200w_infer_set_step_rows(b200w_ctx* ctx, int max_rows) {
+  return iguard(ctx, [&] {
+    Infer* m = model(ctx);
+    B200W_CHECK(max_rows >= m->max_batch && max_rows <= 128, "max_rows must be in max_batch..128");
+    if (m->used) throw StateError("the step's rows are fixed once a step or prefill has run");
+    step_rows(m, max_rows);
+  });
+}
+
 int b200w_infer_kv_read(b200w_ctx* ctx, int layer, int slot, int pos0, int n, void* k_out, void* v_out,
                         float* k_scale_out, float* v_scale_out) {
   return iguard(ctx, [&] {
@@ -2634,7 +2807,7 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     Infer* m = model(ctx);
     const auto& a = m->a;
     check_logprobs(next);
-    B200W_CHECK(tokens && positions && slots && n >= 1 && n <= m->max_batch, "bad batch");
+    B200W_CHECK(tokens && positions && slots && n >= 1 && n <= m->max_rows, "bad batch (1..max_rows rows)");
     for (int i = 0; i < n; ++i) {
       B200W_CHECK(positions[i] >= 0 && positions[i] < a.max_ctx, "position outside the KV cache");
       B200W_CHECK(slots[i] >= 0 && slots[i] < m->max_batch, "bad cache slot");
@@ -2643,20 +2816,24 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     }
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
+    m->used = true;
     memcpy(m->pin_tok, tokens, n * 4);
     memcpy(m->pin_pos, positions, n * 4);
     memcpy(m->pin_slot, slots, n * 4);
+    m->grouped = false;
+    for (int i = 1; i < n; ++i) m->grouped |= slots[i] == slots[i - 1] && positions[i] == positions[i - 1] + 1;
+    const int key = 2 * n + (m->grouped ? 1 : 0);   // one graph per row count and kernel kind: it reads pos / slot
     if (next) ensure_next_logprobs(m);
     ensure_tiled(m, s);   // no-op unless the weights changed since the last step
     int64_t step_launches = 0;
     // Run eagerly the first time a row count is seen (first-use attribute calls), captured into a
     // CUDA graph the second time, replayed from then on: ~200 launches (and their programmatic
     // dependencies) become one.
-    auto git = m->graphs.find(n);
+    auto git = m->graphs.find(key);
     if (git != m->graphs.end()) {
       B200W_CUDA(cudaGraphLaunch(git->second, s));
-      step_launches = m->warm[n];
-    } else if (m->warm.count(n)) {
+      step_launches = m->warm[key];
+    } else if (m->warm.count(key)) {
       cudaGraph_t graph = nullptr;
       B200W_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
       try {
@@ -2670,11 +2847,11 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
       cudaGraphExec_t exec = nullptr;
       B200W_CUDA(cudaGraphInstantiate(&exec, graph, 0));
       cudaGraphDestroy(graph);
-      m->graphs[n] = exec;
+      m->graphs[key] = exec;
       B200W_CUDA(cudaGraphLaunch(exec, s));
     } else {
       enqueue_decode(m, s, n, step_launches);
-      m->warm[n] = static_cast<int>(step_launches);
+      m->warm[key] = static_cast<int>(step_launches);
     }
     nl += step_launches;
     // outside the graph, on the logits it left: the captured step is the same with and without log-probabilities
@@ -2712,6 +2889,7 @@ static int prefill_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* st
     check_prefill(m, tokens, starts, lengths, slots, n_seqs, S);
     const size_t T = static_cast<size_t>(n_seqs) * S;
     cudaStream_t s = ctx_stream(ctx);
+    m->used = true;
     ensure_prefill(m, T);
     if (next) ensure_next_logprobs(m);
     if (score) ensure_scoring(m, T);
@@ -2769,12 +2947,12 @@ static int sample_impl(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b2
     const int64_t entries = pen ? check_penalties(pen, n, V) : 0;
     if (n != have) throw StateError("b200w_infer_sample must follow the step or prefill call whose rows it samples");
     if (!m->sp_dev) {
-      m->sp_dev = m->alloc<uint8_t>(sample_bytes(m->max_batch));
-      B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->sp_pin), sample_bytes(m->max_batch)));
+      m->sp_dev = m->alloc<uint8_t>(sample_bytes(m->max_rows));
+      B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->sp_pin), sample_bytes(m->max_rows)));
     }
     PenaltyBuffers pb{};
     if (pen) {
-      if (!m->pen_rows) m->pen_rows = m->alloc<bf16>(static_cast<size_t>(m->max_batch) * V);
+      if (!m->pen_rows) m->pen_rows = m->alloc<bf16>(static_cast<size_t>(m->max_rows) * V);
       const size_t need = penalty_bytes(n, entries);
       if (need > m->pen_cap) {   // grown geometrically: a request's entries grow by one token a step
         const size_t cap = std::max(need, 2 * m->pen_cap);
@@ -2793,7 +2971,7 @@ static int sample_impl(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b2
       }
       pb = PenaltyBuffers{m->pen_rows, m->pen_pin, m->pen_dev};
     }
-    sample(m->logits, V, n, V, sp, nullptr, tokens_out, token_logit_out, m->sp_pin, m->sp_dev, m->max_batch,
+    sample(m->logits, V, n, V, sp, nullptr, tokens_out, token_logit_out, m->sp_pin, m->sp_dev, m->max_rows,
            ctx_stream(ctx), pen, pen ? &pb : nullptr);
     ctx_launches(ctx) += pen ? (token_logit_out ? 3 : 2) : 1;
   });

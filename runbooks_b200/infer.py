@@ -102,12 +102,14 @@ class InferEngine(Engine):
     kv_dtype: str = "bf16"
 
     def init_infer(self, arch: ServeArch, max_batch: int = 32, kv_pages: Optional[int] = None,
-                   prefill_tokens: Optional[int] = None, kv_dtype: str = "bf16"):
+                   prefill_tokens: Optional[int] = None, kv_dtype: str = "bf16", max_rows: Optional[int] = None):
         """kv_pages: serve from a pool of that many 128-position pages shared by all slots (b200w_infer_init_paged)
         instead of reserving max_ctx positions per slot; arch.max_ctx is then the longest single request.
         prefill_tokens: the most tokens (n_seqs * padded length) one prefill call takes in paged mode.
         kv_dtype: "bf16", or "fp8" (paged only): K/V stored as e4m3 with per-(position, kv head) scales, about half
-        the bytes per page (DESIGN §3.5)."""
+        the bytes per page (DESIGN §3.5).
+        max_rows (max_batch..128; None: max_batch): rows one step may hold, for steps that verify drafted tokens
+        (b200w_infer_set_step_rows)."""
         if kv_dtype not in KV_DTYPES:
             raise ValueError(f"kv_dtype must be one of {sorted(KV_DTYPES)}, got {kv_dtype!r}")
         if kv_dtype != "bf16" and kv_pages is None:
@@ -123,7 +125,10 @@ class InferEngine(Engine):
             self._check(self._lib.b200w_infer_init_paged_kv(self._h, C.byref(ca), max_batch, kv_pages, prefill_tokens,
                                                             KV_DTYPES[kv_dtype]))
             self.kv_pages, self.prefill_tokens = kv_pages, prefill_tokens
+        if max_rows is not None:
+            self._check(self._lib.b200w_infer_set_step_rows(self._h, max_rows))
         self.serve_arch, self.max_batch, self.kv_dtype = arch, max_batch, kv_dtype
+        self.max_rows = max_batch if max_rows is None else max_rows
 
     def kv_read(self, layer: int, slot: int, pos0: int, n: int):
         """The raw cache rows of positions [pos0, pos0 + n) of `slot` (b200w_infer_kv_read): (k, v) as bf16 bit
@@ -380,6 +385,17 @@ class RequestPenalties:
         for t, b in logit_bias.items():
             self.bias[self.pos[t]] = b
 
+    def after(self, tokens: List[int]) -> "RequestPenalties":
+        """A copy with `tokens` counted as emitted: the entries of a step row that follows drafted tokens."""
+        c = RequestPenalties.__new__(RequestPenalties)
+        c.presence, c.frequency, c.repetition, c.n = self.presence, self.frequency, self.repetition, self.n
+        c.pos = dict(self.pos)
+        c.ids, c.out_count, c.in_prompt, c.bias = (a.copy() for a in (self.ids, self.out_count, self.in_prompt,
+                                                                       self.bias))
+        for t in tokens:
+            c.emit(t)
+        return c
+
     def emit(self, t: int):
         i = self.pos.get(t)
         if i is None:
@@ -429,6 +445,45 @@ def sample_token(logits: np.ndarray, temperature: float, top_p: float, rng: np.r
     return int(rng.choice(len(p), p=p))
 
 
+class NgramProposer:
+    """Prompt lookup (HF generate(prompt_lookup_num_tokens=...), vLLM's ngram speculation) over a request's ids, the
+    prompt as fed and then its output: the draft is what followed the latest earlier occurrence of the ids' last n
+    tokens, n = 3, then 2, then 1. An index from each n-gram to the end of its latest occurrence is built over the
+    prompt when the request is admitted and grows as ids are appended, so a step's proposal costs O(n + d) however
+    long the request is."""
+    N = 3
+
+    def __init__(self, ids: Iterable[int] = ()):
+        self.ids: List[int] = list(ids)
+        self.latest: List[Dict[Tuple[int, ...], int]] = [{} for _ in range(self.N + 1)]
+        self.indexed = 0     # n-grams that end at positions <= indexed are in the index
+        self._index()
+
+    def append(self, t: int):
+        self.ids.append(t)
+
+    def _index(self):
+        """Every n-gram that ends before the last id (the suffix a proposal looks up ends there) into the index."""
+        ids, L = self.ids, len(self.ids)
+        for e in range(self.indexed + 1, L):
+            for n in range(1, min(self.N, e) + 1):
+                self.latest[n][tuple(ids[e - n:e])] = e
+        self.indexed = max(self.indexed, L - 1)
+
+    def propose(self, d: int) -> List[int]:
+        """At most d tokens: ids[e : e + d] for the end e < len(ids) of the latest earlier occurrence of the longest
+        suffix n-gram that has one; [] when none has."""
+        self._index()
+        ids, L = self.ids, len(self.ids)
+        if d <= 0:
+            return []
+        for n in range(min(self.N, L - 1), 0, -1):
+            e = self.latest[n].get(tuple(ids[L - n:]))
+            if e is not None:
+                return ids[e:e + d]
+        return []
+
+
 @dataclass
 class _Req:
     prompt: List[int]
@@ -454,6 +509,7 @@ class _Req:
     seed: int = 0
     pen: Optional[RequestPenalties] = None                    # None: no penalty and no logit_bias
     error: Optional[str] = None                               # set when the request failed on its own (done too)
+    lookup: Optional[NgramProposer] = None                    # speculation: the n-gram index of prompt + output
 
     @property
     def greedy(self) -> bool:
@@ -484,13 +540,23 @@ class _Node:
 class Generator:
     """Continuous batching over the engine's cache slots. A request's prompt is ingested in one prefill
     pass when it is admitted (engines without `prefill`, i.e. the CPU test stubs, feed it one token per
-    step through the decode path); from then on every active request advances one token per step."""
+    step through the decode path); from then on every active request advances one token per step, or with
+    speculation up to 1 + speculative_tokens."""
 
     def __init__(self, engine: InferEngine, eos_id: Optional[int] = None, use_prefill: bool = True,
-                 prefix_cache: bool = False):
+                 prefix_cache: bool = False, speculative_tokens: int = 0):
         """prefix_cache (paged KV cache only): requests whose prompts share leading full pages share those pages and
         prefill only the rest. An index of the prompt pages served keeps them (one retained reference each) until
-        pages run short, then gives back the least recently used ones."""
+        pages run short, then gives back the least recently used ones.
+        speculative_tokens (0..7; 0: off): a request past its prompt feeds its last token and up to that many drafted
+        tokens (`propose`, prompt lookup by default) at consecutive positions in one step, and emits the step's
+        tokens while they match the drafts (DESIGN §3.5). Its tokens are the same as without speculation; the step's
+        rows stay within the engine's max_rows."""
+        if isinstance(speculative_tokens, bool) or not isinstance(speculative_tokens, int) or \
+                not 0 <= speculative_tokens <= 7:
+            raise ValueError(f"speculative_tokens must be an integer in 0..7, got {speculative_tokens!r}")
+        self.spec = speculative_tokens
+        self.max_rows = getattr(engine, "max_rows", engine.max_batch)
         self.e, self.eos = engine, eos_id
         self.free = list(range(engine.max_batch))
         self.active: List[_Req] = []
@@ -563,6 +629,8 @@ class Generator:
             r.top_k = 0 if top_k >= V else top_k
             r.seed = (int(seed) if seed is not None else int.from_bytes(os.urandom(8), "little")) % 2 ** 64
         r.pen = pen
+        if self.spec:
+            r.lookup = NgramProposer(r.prompt)
         if r.prompt_logprobs and not r.scores_prompt:
             r.prompt_lp = [None]          # one token: nothing to score
         self.active.append(r)
@@ -705,19 +773,23 @@ class Generator:
                 self._emit_token(r, i, nxt, lg, lp, drawn)
         self._retire()
 
-    def _sample(self, rs: List[_Req], emits: List[bool]):
+    def _sample(self, rs: List[_Req], emits: List[bool], ahead: Optional[List[List[int]]] = None):
         """Right after the step / prefill call over the rows `rs`: one engine.sample call for them when a row that
         emits a token samples (the others go as greedy rows), or one engine.sample_penalized call when such a row
-        is penalized (the others go without entries) -> (tokens, their raw logits or None), or None."""
+        is penalized (the others go without entries) -> (tokens, their raw logits or None), or None.
+        ahead[i] (speculation): the drafted tokens row i follows; its draw is len(out) + len(ahead[i]), and its
+        penalties count them as emitted."""
+        ahead = ahead or [[]] * len(rs)
         on = [e and not r.greedy for r, e in zip(rs, emits)]
         pen = [e and r.pen is not None for r, e in zip(rs, emits)]
         if not (self.device_sampling and (any(on) or any(pen))):
             return None
         args = (len(rs), [r.temperature if s else 0.0 for r, s in zip(rs, on)], [r.top_p for r in rs],
-                [r.top_k for r in rs], [r.seed for r in rs], [len(r.out) for r in rs])
+                [r.top_k for r in rs], [r.seed for r in rs], [len(r.out) + len(a) for r, a in zip(rs, ahead)])
         want_logit = any((s or p) and r.logprobs is not None for r, s, p in zip(rs, on, pen))
         if any(pen):
-            return self.e.sample_penalized(*args, Penalties.pack([r.pen if p else None for r, p in zip(rs, pen)]),
+            return self.e.sample_penalized(*args, Penalties.pack([(r.pen.after(a) if a else r.pen) if p else None
+                                                                  for r, p, a in zip(rs, pen, ahead)]),
                                            want_logit=want_logit)
         return self.e.sample(*args, want_logit=want_logit)
 
@@ -746,6 +818,8 @@ class Generator:
         r.out.append(t)
         if r.pen is not None:
             r.pen.emit(t)
+        if r.lookup is not None:
+            r.lookup.append(t)
         if len(r.out) >= r.max_tokens or (self.eos is not None and t == self.eos):
             r.done = True
 
@@ -770,27 +844,62 @@ class Generator:
             self.active.remove(r)
             self._free_slot(r)
 
+    def propose(self, r: _Req, d: int) -> List[int]:
+        """Up to d drafted tokens to follow r's ids (prompt lookup); a test may replace this."""
+        return r.lookup.propose(d)
+
+    def _drafts(self) -> List[List[int]]:
+        """Each active request's drafts for this step. Only a request past its prompt drafts, at most
+        min(speculative_tokens, max_tokens - len(out) - 1) tokens (its last position stays inside what admission
+        reserved), and the step's rows stay within max_rows: requests take the spare rows in the order they are
+        active. A request sampled on the host drafts nothing (its generator has state)."""
+        spare = self.max_rows - len(self.active)
+        drafts = []
+        for r in self.active:
+            d = min(self.spec, r.max_tokens - len(r.out) - 1, spare)
+            if r.fed < len(r.prompt) or (r.rng is not None) or d <= 0:
+                drafts.append([])
+                continue
+            dr = [int(t) for t in self.propose(r, d)[:d]]
+            spare -= len(dr)
+            drafts.append(dr)
+        return drafts
+
     def step(self):
-        """One engine step for every active request."""
+        """One engine step for every active request: its next token's row, then one row per drafted token."""
         if not self.active:
             return
-        toks = [(r.prompt[r.fed] if r.fed < len(r.prompt) else r.out[-1]) for r in self.active]
+        drafts = self._drafts() if self.spec else [[] for _ in self.active]
+        rs, toks, pos, ahead = [], [], [], []
+        for r, dr in zip(self.active, drafts):
+            for j, t in enumerate([r.prompt[r.fed] if r.fed < len(r.prompt) else r.out[-1]] + dr):
+                rs.append(r)
+                toks.append(t)
+                pos.append(r.fed + j)
+                ahead.append(dr[:j])
+        slots = [r.slot for r in rs]
         need_logits = not self.device_sampling and any(not r.greedy for r in self.active)
         top_k = max((r.logprobs for r in self.active if r.logprobs is not None), default=None)
         lp = None
         if top_k is None:
-            nxt, lg = self.e.step(toks, [r.fed for r in self.active], [r.slot for r in self.active],
-                                  want_logits=need_logits)
+            nxt, lg = self.e.step(toks, pos, slots, want_logits=need_logits)
         else:
-            nxt, lg, lp = self.e.step_logprobs(toks, [r.fed for r in self.active], [r.slot for r in self.active],
-                                               top_k, want_logits=need_logits)
+            nxt, lg, lp = self.e.step_logprobs(toks, pos, slots, top_k, want_logits=need_logits)
         if need_logits and lg is None:
             raise ValueError("sampling (temperature > 0) needs an engine that returns logits")
-        drawn = self._sample(self.active, [r.fed + 1 >= len(r.prompt) for r in self.active])
-        for i, r in enumerate(self.active):
+        drawn = self._sample(rs, [r.fed + 1 + len(a) >= len(r.prompt) for r, a in zip(rs, ahead)],
+                             ahead if self.spec else None)
+        i = 0
+        for r, dr in zip(self.active, drafts):
             r.fed += 1
             if r.fed >= len(r.prompt):        # the token just fed was the last known one
-                self._emit_token(r, i, nxt, lg, lp, drawn)
+                # row j's token is right while every draft before it was: emit until the first mismatch
+                for j in range(len(dr) + 1):
+                    self._emit_token(r, i + j, nxt, lg, lp, drawn)
+                    if r.done or j == len(dr) or r.out[-1] != dr[j]:
+                        break
+                    r.fed += 1
+            i += 1 + len(dr)
         self._retire()
 
     def generate(self, prompts: List[List[int]], max_tokens: int) -> List[List[int]]:

@@ -42,12 +42,14 @@ class Scheduler(threading.Thread):
     (text deltas for streaming clients, one final record for everybody)."""
 
     def __init__(self, engine, tokenizer, max_queue: int = 0, prefix_cache: bool = False, max_logprobs: int = 0,
-                 penalties: bool = False):
+                 penalties: bool = False, speculative_tokens: int = 0):
         """max_logprobs (0..5): the most top entries a request may ask for with `logprobs`; 0 refuses them.
-        penalties: accept presence_penalty, frequency_penalty, repetition_penalty and logit_bias (else a 400)."""
+        penalties: accept presence_penalty, frequency_penalty, repetition_penalty and logit_bias (else a 400).
+        speculative_tokens (0..7): tokens drafted by prompt lookup and verified per request and step (Generator)."""
         super().__init__(daemon=True)
         from .infer import Generator
-        self.gen = Generator(engine, eos_id=tokenizer.eos_id, prefix_cache=prefix_cache)
+        self.gen = Generator(engine, eos_id=tokenizer.eos_id, prefix_cache=prefix_cache,
+                             speculative_tokens=speculative_tokens)
         self.tok, self.q = tokenizer, queue.Queue()
         self.max_queue = max_queue or 4 * engine.max_batch
         self.max_logprobs = max_logprobs
@@ -116,11 +118,22 @@ class Scheduler(threading.Thread):
     # ---- per-request bookkeeping (scheduler thread only) ----
     def _progress(self, req, item, n_prompt, state):
         """Push the text produced since the last call; finish the request on EOS / length / stop string, or with an
-        error when the Generator failed it on its own."""
+        error when the Generator failed it on its own. A step that emitted several tokens (speculation) is taken one
+        token at a time, so that a stop string ends the request at the token that completed it."""
         if getattr(req, "error", None):
             item["events"].put(("error", req.error))
             return True
-        out = req.out
+        n0 = state.get("n", 0)
+        for n in range(min(n0 + 1, len(req.out)), len(req.out) + 1):
+            state["n"] = n
+            if self._progress_upto(req, item, n_prompt, state, n):
+                return True
+        return False
+
+    def _progress_upto(self, req, item, n_prompt, state, n):
+        """_progress as it stands after the request's first n tokens."""
+        out = req.out[:n]
+        done = req.done and n == len(req.out)
         eos_hit = self.tok.eos_id is not None and out and out[-1] == self.tok.eos_id
         text = self.tok.decode(out[:-1] if eos_hit else out)
         finish, cut = None, False
@@ -129,7 +142,7 @@ class Scheduler(threading.Thread):
             if k >= 0:
                 text, finish, cut = text[:k], "stop", True
                 break
-        if finish is None and req.done:
+        if finish is None and done:
             finish = "stop" if eos_hit else "length"
         # hold back a tail that could still turn into a stop string or an incomplete UTF-8 sequence
         safe = len(text)
@@ -541,6 +554,23 @@ def _bool_param(content: str, key: str, cli: bool | None, environ) -> bool:
     raise ValueError(f"param {key!r}: cannot read {v!r} as a boolean")
 
 
+def speculative_tokens_param(content: str, speculative_tokens: int | None = None, environ=None) -> int:
+    """Tokens drafted (prompt lookup) and verified per request and step, 0..7: --speculative-tokens, else the params'
+    speculative_tokens (params.json, PARAM_SPECULATIVE_TOKENS over it), else 0 (off)."""
+    if speculative_tokens is None:
+        extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
+        v = speculative_tokens = extra.get("speculative_tokens", 0)
+        if isinstance(v, str):
+            try:
+                speculative_tokens = int(v.strip())
+            except ValueError as e:
+                raise ValueError(f"param 'speculative_tokens': cannot read {v!r} as an integer") from e
+    if isinstance(speculative_tokens, bool) or not isinstance(speculative_tokens, int) or \
+            not 0 <= speculative_tokens <= 7:
+        raise ValueError(f"speculative_tokens must be an integer in 0..7, got {speculative_tokens!r}")
+    return speculative_tokens
+
+
 def max_logprobs_param(content: str, max_logprobs: int | None = None, environ=None) -> int:
     """The most top entries a request may ask for with `logprobs` (vLLM's max_logprobs), 0..5: --max-logprobs, else
     the params' max_logprobs (params.json, PARAM_MAX_LOGPROBS over it), else 0, which refuses logprobs > 0."""
@@ -584,14 +614,16 @@ def kv_pages_for_gb(arch, kv_cache_gb: float, kv_dtype: str = "bf16") -> int:
 
 
 def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None,
-                kv_dtype: str = "bf16"):
+                kv_dtype: str = "bf16", speculative_tokens: int = 0):
+    """speculative_tokens > 0: a step holds up to min(128, max_batch * (1 + speculative_tokens)) rows."""
     from .infer import InferEngine, ServeArch
 
     cfg = contract.read_hf_config(model_dir)
     arch = ServeArch.from_hf_config(cfg, max_ctx)
     kv_pages = None if kv_cache_gb is None else kv_pages_for_gb(arch, kv_cache_gb, kv_dtype)
     e = InferEngine(int(os.environ.get("B200W_DEVICE", "0")))
-    e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages, kv_dtype=kv_dtype)
+    e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages, kv_dtype=kv_dtype,
+                 max_rows=min(128, max_batch * (1 + speculative_tokens)) if speculative_tokens else None)
     wanted = {n for n, _ in e.infer_params()}
     seen, unused = set(), []
     for name, arr in contract.iter_safetensors(model_dir):
@@ -610,8 +642,9 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
           prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None,
-          penalties: bool | None = None):
+          penalties: bool | None = None, speculative_tokens: int | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
+    speculative_tokens = speculative_tokens_param(content, speculative_tokens)
     prefix_cache = prefix_cache_param(content, prefix_cache)
     kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
     max_logprobs = max_logprobs_param(content, max_logprobs)
@@ -622,14 +655,16 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
         raise ValueError("an fp8 KV cache is paged: kv_cache_dtype fp8 needs kv_cache_gb")
     model_dir = os.path.join(content, "model")
     t0 = time.time()
-    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype)
+    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype, speculative_tokens)
     tok = contract.Tokenizer(model_dir)
-    sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs, penalties=penalties)
+    sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs, penalties=penalties,
+                      speculative_tokens=speculative_tokens)
     sched.start()
     name = cfg.get("_name_or_path") or cfg.get("model_type", "model")
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
     ready = {"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
-             "max_batch": max_batch, "max_logprobs": max_logprobs, "penalties": penalties}
+             "max_batch": max_batch, "max_logprobs": max_logprobs, "penalties": penalties,
+             "speculative_tokens": speculative_tokens}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
         ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch, kv_dtype) / 1e6, 2),
@@ -659,10 +694,13 @@ def main(argv=None) -> int:
     ap.add_argument("--penalties", action="store_true", default=None,
                     help="accept presence_penalty, frequency_penalty, repetition_penalty and logit_bias (default: "
                          "param penalties, else off: they are refused)")
+    ap.add_argument("--speculative-tokens", type=int, default=None,
+                    help="tokens drafted by prompt lookup and verified per request and step, 0..7 (default: param "
+                         "speculative_tokens, else 0: off)")
     a = ap.parse_args(argv)
     try:
         serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype,
-              a.max_logprobs, a.penalties)
+              a.max_logprobs, a.penalties, a.speculative_tokens)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()
