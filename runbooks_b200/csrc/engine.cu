@@ -179,8 +179,7 @@ struct b200w_ctx {
   cudaStream_t stream = nullptr, comm_stream = nullptr;
   std::string err;
   int64_t launches = 0;
-  int64_t dev_bytes = 0;
-  std::vector<void*> allocs;
+  DeviceMemory mem;
 
   // ---- model ----
   bool has_model = false, training = false;
@@ -221,7 +220,7 @@ struct b200w_ctx {
   float *rstdf = nullptr, *meanf = nullptr, *nll = nullptr;
   int32_t *ids_dev = nullptr, *labels_dev = nullptr, *targets = nullptr;
   size_t ids_cap = 0;
-  int32_t* pinned = nullptr;
+  PinnedBuffer<int32_t> pinned;
   size_t pinned_cap = 0;
   // per-document attention (the _docs calls): the batch's positions and the DocBounds derived from them
   int32_t *pos_dev = nullptr, *doc_start = nullptr, *doc_end = nullptr;
@@ -233,7 +232,7 @@ struct b200w_ctx {
   float* inv_n = nullptr;   // 1 / (global) target count of the running step
   long long* cnt_dev = nullptr;  // target count, summed over the ranks (HF num_items_in_batch)
   double* sumsq = nullptr;
-  float* host_scal = nullptr;  // pinned [8]
+  PinnedBuffer<float> host_scal;  // [8]
   float* hook_scal = nullptr;
 
   // ---- timing / profiling (bench.py) ----
@@ -253,33 +252,6 @@ struct b200w_ctx {
   int ar_sm_reserve = 0;  // SMs the GEMMs leave to NCCL while the all-reduce overlaps the backward
   bool poisoned = false;  // a CUDA / NCCL call failed: the context (and any collective) is dead
   cudaEvent_t ev_grad = nullptr, ev_comm = nullptr;
-
-  template <typename T>
-  T* alloc(size_t n) {
-    void* p = nullptr;
-    const size_t bytes = ((n * sizeof(T) + 255) / 256) * 256;
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      throw std::bad_alloc();
-    }
-    allocs.push_back(p);
-    dev_bytes += static_cast<int64_t>(bytes);
-    return static_cast<T*>(p);
-  }
-  void release(void* p) {
-    for (size_t i = 0; i < allocs.size(); ++i)
-      if (allocs[i] == p) {
-        cudaFree(p);
-        allocs.erase(allocs.begin() + i);
-        return;
-      }
-  }
-  void free_all() {
-    for (void* p : allocs) cudaFree(p);
-    allocs.clear();
-    dev_bytes = 0;
-  }
 };
 
 namespace {
@@ -298,7 +270,7 @@ constexpr int OPT_POS_OFFSET = 2;  // HF models/opt/modeling_opt.py:53
 
 // device scalar scratch for the per-kernel hooks (exists without a model)
 float* ctx_scal(b200w_ctx* c) {
-  if (!c->hook_scal) c->hook_scal = c->alloc<float>(8);
+  if (!c->hook_scal) c->hook_scal = c->mem.alloc<float>(8);
   return c->hook_scal;
 }
 
@@ -485,44 +457,44 @@ void alloc_activations(b200w_ctx* c) {
   for (int l = 0; l < L; ++l) {
     if (l < Lsave) {
       auto& x = c->la[l];
-      x.h_in = c->alloc<bf16>(T * d);
-      x.n1 = c->alloc<bf16>(T * d);
-      x.qkv = c->alloc<bf16>(T * qkvd);
-      x.attn = c->alloc<bf16>(T * qd);
-      x.h_mid = c->alloc<bf16>(T * d);
-      x.n2 = c->alloc<bf16>(T * d);
-      x.gu = opt ? nullptr : c->alloc<bf16>(T * (falcon ? 1 : 2) * f);  // Falcon: the pre-GeLU activation
-      x.act = c->alloc<bf16>(T * f);
-      x.rstd1 = c->alloc<float>(T);
-      x.rstd2 = c->alloc<float>(T);
-      x.mean1 = ln ? c->alloc<float>(T) : nullptr;
-      x.mean2 = opt ? c->alloc<float>(T) : nullptr;
-      x.lse = c->alloc<float>(H * T);
+      x.h_in = c->mem.alloc<bf16>(T * d);
+      x.n1 = c->mem.alloc<bf16>(T * d);
+      x.qkv = c->mem.alloc<bf16>(T * qkvd);
+      x.attn = c->mem.alloc<bf16>(T * qd);
+      x.h_mid = c->mem.alloc<bf16>(T * d);
+      x.n2 = c->mem.alloc<bf16>(T * d);
+      x.gu = opt ? nullptr : c->mem.alloc<bf16>(T * (falcon ? 1 : 2) * f);  // Falcon: the pre-GeLU activation
+      x.act = c->mem.alloc<bf16>(T * f);
+      x.rstd1 = c->mem.alloc<float>(T);
+      x.rstd2 = c->mem.alloc<float>(T);
+      x.mean1 = ln ? c->mem.alloc<float>(T) : nullptr;
+      x.mean2 = opt ? c->mem.alloc<float>(T) : nullptr;
+      x.lse = c->mem.alloc<float>(H * T);
     } else {
       c->la[l] = c->la[0];
-      if (c->training && c->recompute) c->la[l].h_in = c->alloc<bf16>(T * d);
+      if (c->training && c->recompute) c->la[l].h_in = c->mem.alloc<bf16>(T * d);
     }
   }
-  c->h_final = c->alloc<bf16>(T * d);
-  c->nf = c->alloc<bf16>(T * d);
-  c->rstdf = c->alloc<float>(T);
-  if (ln) c->meanf = c->alloc<float>(T);
-  c->logits = c->alloc<bf16>(T * a.vocab_size);
-  c->nll = c->alloc<float>(T);
-  c->targets = c->alloc<int32_t>(T);
-  c->scal = c->alloc<float>(8);
-  c->inv_n = c->alloc<float>(1);
-  c->cnt_dev = c->alloc<long long>(1);
-  c->sumsq = c->alloc<double>(1);
+  c->h_final = c->mem.alloc<bf16>(T * d);
+  c->nf = c->mem.alloc<bf16>(T * d);
+  c->rstdf = c->mem.alloc<float>(T);
+  if (ln) c->meanf = c->mem.alloc<float>(T);
+  c->logits = c->mem.alloc<bf16>(T * a.vocab_size);
+  c->nll = c->mem.alloc<float>(T);
+  c->targets = c->mem.alloc<int32_t>(T);
+  c->scal = c->mem.alloc<float>(8);
+  c->inv_n = c->mem.alloc<float>(1);
+  c->cnt_dev = c->mem.alloc<long long>(1);
+  c->sumsq = c->mem.alloc<double>(1);
   if (c->training) {
-    c->dh_a = c->alloc<bf16>(T * d);
-    c->dh_b = c->alloc<bf16>(T * d);
-    c->dn = c->alloc<bf16>(T * d);
-    c->dact = c->alloc<bf16>(T * f);
-    if (!ln) c->dgu = c->alloc<bf16>(T * 2 * f);
-    c->dattn = c->alloc<bf16>(T * qd);
-    c->dqkv = c->alloc<bf16>(T * qkvd);
-    c->delta = c->alloc<float>(H * T);
+    c->dh_a = c->mem.alloc<bf16>(T * d);
+    c->dh_b = c->mem.alloc<bf16>(T * d);
+    c->dn = c->mem.alloc<bf16>(T * d);
+    c->dact = c->mem.alloc<bf16>(T * f);
+    if (!ln) c->dgu = c->mem.alloc<bf16>(T * 2 * f);
+    c->dattn = c->mem.alloc<bf16>(T * qd);
+    c->dqkv = c->mem.alloc<bf16>(T * qkvd);
+    c->delta = c->mem.alloc<float>(H * T);
     // norm backward partials [blocks, d] (RMSNorm) or [blocks, 2 d] (LayerNorm); bias column sums
     // [colsum_blocks, widest projection]
     size_t part = static_cast<size_t>(rmsnorm_bwd_blocks(static_cast<int>(T))) * d * (ln ? 2 : 1);
@@ -530,10 +502,10 @@ void alloc_activations(b200w_ctx* c) {
       const size_t widest = std::max<size_t>({qkvd, f, d});
       part = std::max(part, static_cast<size_t>(colsum_blocks(static_cast<int>(T))) * widest);
     }
-    c->dw_partial = c->alloc<float>(part);
+    c->dw_partial = c->mem.alloc<float>(part);
   }
   if (!opt) {  // the table is over the real head_dim; padded heads rotate their first head_dim columns
-    c->rope_tab = c->alloc<float2>(static_cast<size_t>(a.max_seq_len) * (a.head_dim / 2));
+    c->rope_tab = c->mem.alloc<float2>(static_cast<size_t>(a.max_seq_len) * (a.head_dim / 2));
     rope_table(c->rope_tab, a.max_seq_len, a.head_dim, a.rope_theta, c->stream);
   }
 }
@@ -689,7 +661,7 @@ ArMode ar_mode() {
 }
 
 void ensure_wire(b200w_ctx* c) {
-  if (!c->gw) c->gw = c->alloc<bf16>(c->n_elems);
+  if (!c->gw) c->gw = c->mem.alloc<bf16>(c->n_elems);
 }
 
 // Gradient exchange of the flat range [off, off + count): the fp32 accumulation buffer is rounded to
@@ -892,20 +864,21 @@ void ensure_ids(b200w_ctx* c, size_t n_tok) {
   if (c->ids_cap < n_tok) {
     if (c->ids_dev) {  // every kernel that read the old buffers was enqueued before this point
       B200W_CUDA(cudaStreamSynchronize(c->stream));
-      c->release(c->ids_dev);
-      c->release(c->labels_dev);
+      c->mem.release(c->ids_dev);
+      c->mem.release(c->labels_dev);
+      c->ids_cap = 0;
     }
-    c->ids_dev = c->alloc<int32_t>(n_tok);
-    c->labels_dev = c->alloc<int32_t>(n_tok);
+    c->ids_dev = c->mem.alloc<int32_t>(n_tok);
+    c->labels_dev = c->mem.alloc<int32_t>(n_tok);
     c->ids_cap = n_tok;
   }
   if (c->pinned_cap < 2 * n_tok) {
     if (c->pinned) {
       B200W_CUDA(cudaStreamSynchronize(c->stream));
-      cudaFreeHost(c->pinned);
-      c->pinned = nullptr;
+      c->pinned.reset();
+      c->pinned_cap = 0;
     }
-    B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&c->pinned), 2 * n_tok * sizeof(int32_t)));
+    c->pinned = pinned_buffer<int32_t>(2 * n_tok);
     c->pinned_cap = 2 * n_tok;
   }
 }
@@ -931,11 +904,11 @@ void upload_batch(b200w_ctx* c, const int32_t* ids, const int32_t* labels, size_
       throw Error("check failed: label outside the vocabulary (use -100 to ignore)");
   }
   ensure_ids(c, n_tok);
-  memcpy(c->pinned, ids, n_tok * sizeof(int32_t));
-  memcpy(c->pinned + n_tok, labels, n_tok * sizeof(int32_t));
-  B200W_CUDA(cudaMemcpyAsync(c->ids_dev, c->pinned, n_tok * sizeof(int32_t), cudaMemcpyHostToDevice,
+  memcpy(c->pinned.get(), ids, n_tok * sizeof(int32_t));
+  memcpy(c->pinned.get() + n_tok, labels, n_tok * sizeof(int32_t));
+  B200W_CUDA(cudaMemcpyAsync(c->ids_dev, c->pinned.get(), n_tok * sizeof(int32_t), cudaMemcpyHostToDevice,
                              c->stream));
-  B200W_CUDA(cudaMemcpyAsync(c->labels_dev, c->pinned + n_tok, n_tok * sizeof(int32_t),
+  B200W_CUDA(cudaMemcpyAsync(c->labels_dev, c->pinned.get() + n_tok, n_tok * sizeof(int32_t),
                              cudaMemcpyHostToDevice, c->stream));
 }
 
@@ -963,13 +936,14 @@ void upload_positions(b200w_ctx* c, const int32_t* positions, int n_seqs) {
   if (c->docs_cap < n) {
     if (c->pos_dev) {  // every kernel that read the old buffers was enqueued before this point
       B200W_CUDA(cudaStreamSynchronize(c->stream));
-      c->release(c->pos_dev);
-      c->release(c->doc_start);
-      c->release(c->doc_end);
+      c->mem.release(c->pos_dev);
+      c->mem.release(c->doc_start);
+      c->mem.release(c->doc_end);
+      c->docs_cap = 0;
     }
-    c->pos_dev = c->alloc<int32_t>(n);
-    c->doc_start = c->alloc<int32_t>(n);
-    c->doc_end = c->alloc<int32_t>(n);
+    c->pos_dev = c->mem.alloc<int32_t>(n);
+    c->doc_start = c->mem.alloc<int32_t>(n);
+    c->doc_end = c->mem.alloc<int32_t>(n);
     c->docs_cap = n;
   }
   // pageable source: the call returns once the bytes are staged, so the caller's array may go
@@ -1152,7 +1126,7 @@ bool owned_part(const b200w_ctx* c, const Param& p, OwnedPart* out) {
 
 // loss and grad-norm (each nullable) from the device scalars, once the main stream has drained
 void read_scalars(b200w_ctx* ctx, float* loss_out, float* gnorm_out) {
-  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal, ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  B200W_CUDA(cudaMemcpyAsync(ctx->host_scal.get(), ctx->scal, 4 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   if (loss_out) *loss_out = ctx->host_scal[0];
   if (gnorm_out) *gnorm_out = ctx->host_scal[2];
@@ -1194,12 +1168,10 @@ void forward_call(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels, con
   }
   forward_micro(ctx, ctx->ids_dev, n_seqs, positions ? &db : nullptr);
   if (logits_out) {
-    void* scratch = nullptr;
-    B200W_CUDA(cudaMalloc(&scratch, T * V * 4));
-    cast_bf16_to_f32(ctx->logits, static_cast<float*>(scratch), T * V, ctx->stream);
+    auto scratch = device_scratch<float>(T * V);
+    cast_bf16_to_f32(ctx->logits, scratch.get(), T * V, ctx->stream);
     B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    B200W_CUDA(cudaMemcpy(logits_out, scratch, T * V * 4, cudaMemcpyDeviceToHost));
-    cudaFree(scratch);
+    B200W_CUDA(cudaMemcpy(logits_out, scratch.get(), T * V * 4, cudaMemcpyDeviceToHost));
   }
   if (labels && (nll_out || loss_out)) {
     set_count(ctx, count_valid(labels, n_seqs, S));
@@ -1268,7 +1240,7 @@ int b200w_create(int device, b200w_ctx** out) {
     B200W_CUDA(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
     B200W_CUDA(cudaEventCreateWithFlags(&c->ev_grad, cudaEventDisableTiming));
     B200W_CUDA(cudaEventCreateWithFlags(&c->ev_comm, cudaEventDisableTiming));
-    B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&c->host_scal), 8 * sizeof(float)));
+    c->host_scal = pinned_buffer<float>(8);
     *out = c.release();
     return B200W_OK;
   } catch (const std::exception& e) {
@@ -1291,9 +1263,6 @@ void b200w_destroy(b200w_ctx* ctx) {
     else if (nccl().CommAbort) nccl().CommAbort(ctx->comm);
   }
   if (ctx->infer && ctx->infer_destroy) ctx->infer_destroy(ctx->infer);
-  ctx->free_all();
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
-  if (ctx->host_scal) cudaFreeHost(ctx->host_scal);
   if (ctx->ev_grad) cudaEventDestroy(ctx->ev_grad);
   if (ctx->ev_comm) cudaEventDestroy(ctx->ev_comm);
   if (ctx->ev_t0) cudaEventDestroy(ctx->ev_t0);
@@ -1301,7 +1270,7 @@ void b200w_destroy(b200w_ctx* ctx) {
   for (cudaEvent_t e : ctx->prof_events) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->comm_stream) cudaStreamDestroy(ctx->comm_stream);
-  delete ctx;
+  delete ctx;   // and with it the device and pinned memory the context holds
 }
 
 const char* b200w_last_error(const b200w_ctx* ctx) {
@@ -1388,15 +1357,15 @@ int b200w_model_init(b200w_ctx* ctx, const b200w_arch* arch, const b200w_hparams
       }
       B200W_CHECK(covered == ctx->n_elems, "internal: exchange ranges do not cover the parameter space");
     }
-    ctx->w = ctx->alloc<bf16>(ctx->n_elems);
+    ctx->w = ctx->mem.alloc<bf16>(ctx->n_elems);
     B200W_CUDA(cudaMemsetAsync(ctx->w, 0, ctx->n_elems * sizeof(bf16), ctx->stream));  // head padding = 0
     if (ctx->training) {
       // replicated: fp32 master + Adam moments for every parameter; sharded: for this rank's 1/nranks only
       const size_t n_state = ctx->shard ? ctx->n_elems / ctx->nranks : ctx->n_elems;
-      ctx->master = ctx->alloc<float>(n_state);
-      ctx->m = ctx->alloc<float>(n_state);
-      ctx->v = ctx->alloc<float>(n_state);
-      ctx->g = ctx->alloc<float>(ctx->n_elems);
+      ctx->master = ctx->mem.alloc<float>(n_state);
+      ctx->m = ctx->mem.alloc<float>(n_state);
+      ctx->v = ctx->mem.alloc<float>(n_state);
+      ctx->g = ctx->mem.alloc<float>(ctx->n_elems);
       B200W_CUDA(cudaMemsetAsync(ctx->master, 0, n_state * sizeof(float), ctx->stream));
       B200W_CUDA(cudaMemsetAsync(ctx->m, 0, n_state * sizeof(float), ctx->stream));
       B200W_CUDA(cudaMemsetAsync(ctx->v, 0, n_state * sizeof(float), ctx->stream));
@@ -1451,35 +1420,32 @@ int b200w_load_tensor(b200w_ctx* ctx, const char* name, const void* host, b200w_
     if (ctx->shard) {
       // every rank holds the whole bf16 compute copy; the fp32 master exists for the owned slice only and
       // receives the exact fp32 values of an fp32 checkpoint there
-      float* dense = nullptr;
-      void* raw = nullptr;
-      B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&dense), n * 4));
-      try {
-        if (dtype == B200W_F32) {
-          B200W_CUDA(cudaMemcpyAsync(dense, host, n * 4, cudaMemcpyHostToDevice, s));
-          cast_f32_to_bf16(dense, ctx->w + p.off, n, s);
-        } else {
-          B200W_CUDA(cudaMemcpyAsync(ctx->w + p.off, host, n * 2, cudaMemcpyHostToDevice, s));
-          cast_bf16_to_f32(ctx->w + p.off, dense, n, s);
-        }
-        OwnedPart op;
-        if (owned_part(ctx, p, &op))
-          B200W_CUDA(cudaMemcpyAsync(ctx->master + op.compact, dense + (op.lo - p.off), op.n * 4,
-                                     cudaMemcpyDeviceToDevice, s));
-        B200W_CUDA(cudaStreamSynchronize(s));
-      } catch (...) { cudaFree(dense); cudaFree(raw); throw; }
-      cudaFree(dense);
+      auto dense = device_scratch<float>(n);
+      if (dtype == B200W_F32) {
+        B200W_CUDA(cudaMemcpyAsync(dense.get(), host, n * 4, cudaMemcpyHostToDevice, s));
+        cast_f32_to_bf16(dense.get(), ctx->w + p.off, n, s);
+      } else {
+        B200W_CUDA(cudaMemcpyAsync(ctx->w + p.off, host, n * 2, cudaMemcpyHostToDevice, s));
+        cast_bf16_to_f32(ctx->w + p.off, dense.get(), n, s);
+      }
+      OwnedPart op;
+      if (owned_part(ctx, p, &op))
+        B200W_CUDA(cudaMemcpyAsync(ctx->master + op.compact, dense.get() + (op.lo - p.off), op.n * 4,
+                                   cudaMemcpyDeviceToDevice, s));
+      B200W_CUDA(cudaStreamSynchronize(s));
       return;
     }
     if (p.pad == 0) {
       if (dtype == B200W_F32) {
+        DeviceScratch<float> scratch;
         float* tmp = ctx->training ? ctx->master + p.off : nullptr;
-        void* scratch = nullptr;
-        if (!tmp) { B200W_CUDA(cudaMalloc(&scratch, n * 4)); tmp = static_cast<float*>(scratch); }
+        if (!tmp) {
+          scratch = device_scratch<float>(n);
+          tmp = scratch.get();
+        }
         B200W_CUDA(cudaMemcpyAsync(tmp, host, n * 4, cudaMemcpyHostToDevice, s));
         cast_f32_to_bf16(tmp, ctx->w + p.off, n, s);
         B200W_CUDA(cudaStreamSynchronize(s));
-        if (scratch) cudaFree(scratch);
       } else {
         B200W_CUDA(cudaMemcpyAsync(ctx->w + p.off, host, n * 2, cudaMemcpyHostToDevice, s));
         if (ctx->training) cast_bf16_to_f32(ctx->w + p.off, ctx->master + p.off, n, s);
@@ -1488,25 +1454,20 @@ int b200w_load_tensor(b200w_ctx* ctx, const char* name, const void* host, b200w_
       return;
     }
     // head-padded parameter: stage dense fp32 on the device, scatter into the padded rows / columns
-    float* dense = nullptr;
-    void* raw = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&dense), n * 4));
-    try {
-      if (dtype == B200W_F32) {
-        B200W_CUDA(cudaMemcpyAsync(dense, host, n * 4, cudaMemcpyHostToDevice, s));
-      } else {
-        B200W_CUDA(cudaMalloc(&raw, n * 2));
-        B200W_CUDA(cudaMemcpyAsync(raw, host, n * 2, cudaMemcpyHostToDevice, s));
-        cast_bf16_to_f32(raw, dense, n, s);
-      }
-      pad_scatter_kernel<<<sm_count() * 4, 256, 0, s>>>(dense, ctx->training ? ctx->master + p.off : nullptr,
-                                                        ctx->w + p.off, p.rows, p.cols, p.icols, p.pad,
-                                                        ctx->arch.head_dim, ctx->dhp);
-      B200W_CUDA(cudaGetLastError());
-      B200W_CUDA(cudaStreamSynchronize(s));
-    } catch (...) { cudaFree(dense); cudaFree(raw); throw; }
-    cudaFree(dense);
-    cudaFree(raw);
+    auto dense = device_scratch<float>(n);
+    DeviceScratch<bf16> raw;
+    if (dtype == B200W_F32) {
+      B200W_CUDA(cudaMemcpyAsync(dense.get(), host, n * 4, cudaMemcpyHostToDevice, s));
+    } else {
+      raw = device_scratch<bf16>(n);
+      B200W_CUDA(cudaMemcpyAsync(raw.get(), host, n * 2, cudaMemcpyHostToDevice, s));
+      cast_bf16_to_f32(raw.get(), dense.get(), n, s);
+    }
+    pad_scatter_kernel<<<sm_count() * 4, 256, 0, s>>>(dense.get(), ctx->training ? ctx->master + p.off : nullptr,
+                                                      ctx->w + p.off, p.rows, p.cols, p.icols, p.pad,
+                                                      ctx->arch.head_dim, ctx->dhp);
+    B200W_CUDA(cudaGetLastError());
+    B200W_CUDA(cudaStreamSynchronize(s));
   });
 }
 
@@ -1521,17 +1482,13 @@ void read_dense(b200w_ctx* ctx, const Param& p, const float* srcf, const bf16* s
     B200W_CUDA(cudaMemcpy(host, srcf + p.off, n * 4, cudaMemcpyDeviceToHost));
     return;
   }
-  float* dense = nullptr;
-  B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&dense), n * 4));
-  try {
-    pad_gather_kernel<<<sm_count() * 4, 256, 0, s>>>(srcf ? srcf + p.off : nullptr, srcb ? srcb + p.off : nullptr,
-                                                     dense, p.rows, p.cols, p.icols, p.pad, ctx->arch.head_dim,
-                                                     ctx->dhp);
-    B200W_CUDA(cudaGetLastError());
-    B200W_CUDA(cudaStreamSynchronize(s));
-    B200W_CUDA(cudaMemcpy(host, dense, n * 4, cudaMemcpyDeviceToHost));
-  } catch (...) { cudaFree(dense); throw; }
-  cudaFree(dense);
+  auto dense = device_scratch<float>(n);
+  pad_gather_kernel<<<sm_count() * 4, 256, 0, s>>>(srcf ? srcf + p.off : nullptr, srcb ? srcb + p.off : nullptr,
+                                                   dense.get(), p.rows, p.cols, p.icols, p.pad, ctx->arch.head_dim,
+                                                   ctx->dhp);
+  B200W_CUDA(cudaGetLastError());
+  B200W_CUDA(cudaStreamSynchronize(s));
+  B200W_CUDA(cudaMemcpy(host, dense.get(), n * 4, cudaMemcpyDeviceToHost));
 }
 }  // namespace
 
@@ -1659,20 +1616,14 @@ int b200w_comm_init(b200w_ctx* ctx, int rank, int nranks, const void* id128) {
     // GPU, instead of in the middle of the first backward.
     {
       const size_t n_big = size_t(64) << 20;  // 128 MB of bf16: same protocol/algorithm class as a matrix gradient
-      bf16* scratch = nullptr;
-      B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&scratch), n_big * sizeof(bf16)));
+      auto buf = device_scratch<bf16>(n_big);
+      bf16* scratch = buf.get();
       cudaStream_t cs = ctx->comm_stream;
-      try {
-        B200W_CUDA(cudaMemsetAsync(scratch, 0, n_big * sizeof(bf16), cs));
-        B200W_NCCL(nccl().AllReduce(scratch, scratch, n_big, kNcclBfloat16, kNcclSum, ctx->comm, cs));
-        B200W_NCCL(nccl().AllReduce(scratch, scratch, 1, kNcclFloat32, kNcclSum, ctx->comm, cs));
-        B200W_NCCL(nccl().AllReduce(scratch, scratch, 1, kNcclInt64, kNcclSum, ctx->comm, cs));
-        B200W_CUDA(cudaStreamSynchronize(cs));
-      } catch (...) {
-        cudaFree(scratch);
-        throw;
-      }
-      B200W_CUDA(cudaFree(scratch));
+      B200W_CUDA(cudaMemsetAsync(scratch, 0, n_big * sizeof(bf16), cs));
+      B200W_NCCL(nccl().AllReduce(scratch, scratch, n_big, kNcclBfloat16, kNcclSum, ctx->comm, cs));
+      B200W_NCCL(nccl().AllReduce(scratch, scratch, 1, kNcclFloat32, kNcclSum, ctx->comm, cs));
+      B200W_NCCL(nccl().AllReduce(scratch, scratch, 1, kNcclInt64, kNcclSum, ctx->comm, cs));
+      B200W_CUDA(cudaStreamSynchronize(cs));
     }
   });
 }
@@ -1772,7 +1723,7 @@ int b200w_forward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels
 }
 
 int64_t b200w_launch_count(const b200w_ctx* ctx) { return ctx ? ctx->launches : 0; }
-int64_t b200w_device_bytes(const b200w_ctx* ctx) { return ctx ? ctx->dev_bytes : 0; }
+int64_t b200w_device_bytes(const b200w_ctx* ctx) { return ctx ? ctx->mem.bytes() : 0; }
 
 // ---- per-kernel hooks ---------------------------------------------------------------------
 #define HOOK(body)                                              \
@@ -1799,22 +1750,19 @@ int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const v
 int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k) {
   return guarded(ctx, [&] {
-    float* ws = nullptr;
-    unsigned* cnt = nullptr;
+    DeviceScratch<float> ws;
+    DeviceScratch<unsigned> cnt;
     if (split_k) {
-      B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&ws), static_cast<size_t>(M) * N * 4));
-      B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&cnt), ((N + 127) / 128) * 4));
-      B200W_CUDA(cudaMemsetAsync(ws, 0, static_cast<size_t>(M) * N * 4, ctx->stream));
-      B200W_CUDA(cudaMemsetAsync(cnt, 0, ((N + 127) / 128) * 4, ctx->stream));
+      ws = device_scratch<float>(static_cast<size_t>(M) * N);
+      cnt = device_scratch<unsigned>((N + 127) / 128);
+      B200W_CUDA(cudaMemsetAsync(ws.get(), 0, static_cast<size_t>(M) * N * 4, ctx->stream));
+      B200W_CUDA(cudaMemsetAsync(cnt.get(), 0, ((N + 127) / 128) * 4, ctx->stream));
     }
-    try {
-      gemm_decode(X, W, out, C, ws, cnt, M, N, K, N, 0, ctx->stream);
-      gemm_decode(X, W, out, C, ws, cnt, M, N, K, N, 0, ctx->stream);  // twice: the scratch must come back clean
-      ctx->launches += 2;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(ws); cudaFree(cnt); throw; }
-    cudaFree(ws);
-    cudaFree(cnt);
+    // twice: the scratch must come back clean
+    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx->stream);
+    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx->stream);
+    ctx->launches += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_embed_fwd(b200w_ctx* ctx, const int32_t* ids, const void* table, const void* pos_table,
@@ -1833,15 +1781,10 @@ int b200w_op_layernorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const 
                            const float* rstd, const void* dresid, void* dx, float* dw, float* db, int T,
                            int d) {
   return guarded(ctx, [&] {
-    float* part = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&part),
-                          static_cast<size_t>(rmsnorm_bwd_blocks(T)) * 2 * d * sizeof(float)));
-    try {
-      layernorm_bwd(dy, x, w, mean, rstd, dresid, dx, dw, db, part, T, d, ctx->stream);
-      ctx->launches += 3;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(part); throw; }
-    cudaFree(part);
+    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * 2 * d);
+    layernorm_bwd(dy, x, w, mean, rstd, dresid, dx, dw, db, part.get(), T, d, ctx->stream);
+    ctx->launches += 3;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_bias_act(b200w_ctx* ctx, void* x, const void* bias, int T, int N, int ld, int act) {
@@ -1858,14 +1801,10 @@ int b200w_op_gelu_bwd(b200w_ctx* ctx, const void* dy, const void* x, void* dx, i
 }
 int b200w_op_colsum(b200w_ctx* ctx, const void* dy, float* db, int T, int N, int ld) {
   return guarded(ctx, [&] {
-    float* part = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&part), static_cast<size_t>(colsum_blocks(T)) * N * sizeof(float)));
-    try {
-      colsum_add(dy, db, part, T, N, ld, ctx->stream);
-      ctx->launches += 2;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(part); throw; }
-    cudaFree(part);
+    auto part = device_scratch<float>(static_cast<size_t>(colsum_blocks(T)) * N);
+    colsum_add(dy, db, part.get(), T, N, ld, ctx->stream);
+    ctx->launches += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_rmsnorm_fwd(b200w_ctx* ctx, const void* x, const void* w, void* y, float* rstd, int T,
@@ -1875,29 +1814,20 @@ int b200w_op_rmsnorm_fwd(b200w_ctx* ctx, const void* x, const void* w, void* y, 
 int b200w_op_rmsnorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const void* w,
                          const float* rstd, const void* dresid, void* dx, float* dw, int T, int d) {
   return guarded(ctx, [&] {
-    float* part = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&part),
-                          static_cast<size_t>(rmsnorm_bwd_blocks(T)) * d * sizeof(float)));
-    try {
-      rmsnorm_bwd(dy, x, w, rstd, dresid, dx, dw, part, T, d, ctx->stream);
-      ctx->launches += 2;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(part); throw; }
-    cudaFree(part);
+    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * d);
+    rmsnorm_bwd(dy, x, w, rstd, dresid, dx, dw, part.get(), T, d, ctx->stream);
+    ctx->launches += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_rope(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
                   int inverse) {
   return guarded(ctx, [&] {
-    float2* tab = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&tab), static_cast<size_t>(S) * (dh / 2) * sizeof(float2)));
-    try {
-      rope_table(tab, S, dh, theta, ctx->stream);
-      rope_apply(buf, ld, tab, T, S, nheads, dh, inverse != 0, ctx->stream);
-      ++ctx->launches;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(tab); throw; }
-    cudaFree(tab);
+    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
+    rope_table(tab.get(), S, dh, theta, ctx->stream);
+    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx->stream);
+    ++ctx->launches;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_swiglu_fwd(b200w_ctx* ctx, const void* gu, void* h, int T, int f) {
@@ -1909,16 +1839,12 @@ int b200w_op_swiglu_bwd(b200w_ctx* ctx, const void* dh, const void* gu, void* dg
 int b200w_op_ce(b200w_ctx* ctx, void* logits, const int32_t* labels, float* nll, int T, int S, int V,
                 float inv_n) {
   return guarded(ctx, [&] {
-    int32_t* tg = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&tg), static_cast<size_t>(T) * 4));
-    try {
-      B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx) + 4, &inv_n, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-      ce_shift_targets(labels, tg, T, S, ctx->stream);
-      ce_loss_fwd_bwd(logits, tg, nll, T, V, ctx_scal(ctx) + 4, ctx->stream);
-      ctx->launches += 2;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(tg); throw; }
-    cudaFree(tg);
+    auto tg = device_scratch<int32_t>(T);
+    B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx) + 4, &inv_n, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    ce_shift_targets(labels, tg.get(), T, S, ctx->stream);
+    ce_loss_fwd_bwd(logits, tg.get(), nll, T, V, ctx_scal(ctx) + 4, ctx->stream);
+    ctx->launches += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
@@ -1975,15 +1901,8 @@ int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V,
   return guarded(ctx, [&] {
     check_sampling(sp, rows, V, tokens_out);
     std::vector<uint8_t> host(sample_bytes(rows));
-    void* dev = nullptr;
-    B200W_CUDA(cudaMalloc(&dev, host.size()));
-    try {
-      sample(logits, ld, rows, V, sp, u, tokens_out, token_logit_out, host.data(), dev, rows, ctx->stream);
-    } catch (...) {
-      cudaFree(dev);
-      throw;
-    }
-    cudaFree(dev);
+    auto dev = device_scratch<uint8_t>(host.size());
+    sample(logits, ld, rows, V, sp, u, tokens_out, token_logit_out, host.data(), dev.get(), rows, ctx->stream);
     ++ctx->launches;
   });
 }
@@ -1993,16 +1912,9 @@ int b200w_op_penalize(b200w_ctx* ctx, const void* logits, int ld, int rows, int 
     B200W_CHECK(V >= 8, "bad vocabulary size");
     const int64_t entries = check_penalties(pen, rows, V);
     std::vector<uint8_t> host(penalty_bytes(rows, entries));
-    void* dev = nullptr;
-    B200W_CUDA(cudaMalloc(&dev, host.size()));
-    try {
-      penalize(logits, ld, rows, V, pen, out, host.data(), dev, ctx->stream);
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) {
-      cudaFree(dev);
-      throw;
-    }
-    cudaFree(dev);
+    auto dev = device_scratch<uint8_t>(host.size());
+    penalize(logits, ld, rows, V, pen, out, host.data(), dev.get(), ctx->stream);
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
     ++ctx->launches;
   });
 }
@@ -2020,16 +1932,13 @@ template <typename F>
 void with_doc_bounds(b200w_ctx* ctx, const int32_t* positions, int B, int S, F&& f) {
   B200W_CHECK(positions, "NULL positions");
   const size_t T = static_cast<size_t>(B) * S;
-  int32_t* se = nullptr;
-  B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&se), 2 * T * sizeof(int32_t)));
-  try {
-    doc_bounds(positions, se, se + T, static_cast<int>(T), S, ctx->stream);
-    ++ctx->launches;
-    const DocBounds db{positions, se, se + T};
-    f(db);
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  } catch (...) { cudaFree(se); throw; }
-  cudaFree(se);
+  auto buf = device_scratch<int32_t>(2 * T);
+  int32_t* se = buf.get();
+  doc_bounds(positions, se, se + T, static_cast<int>(T), S, ctx->stream);
+  ++ctx->launches;
+  const DocBounds db{positions, se, se + T};
+  f(db);
+  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
 }
 }  // namespace
 
@@ -2060,15 +1969,11 @@ int b200w_op_rope_positions(b200w_ctx* ctx, void* buf, int ld, int T, int S, int
                             int inverse, const int32_t* positions) {
   return guarded(ctx, [&] {
     B200W_CHECK(positions, "NULL positions");
-    float2* tab = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&tab), static_cast<size_t>(S) * (dh / 2) * sizeof(float2)));
-    try {
-      rope_table(tab, S, dh, theta, ctx->stream);
-      rope_apply(buf, ld, tab, T, S, nheads, dh, inverse != 0, ctx->stream, 0, positions);
-      ++ctx->launches;
-      B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    } catch (...) { cudaFree(tab); throw; }
-    cudaFree(tab);
+    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
+    rope_table(tab.get(), S, dh, theta, ctx->stream);
+    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx->stream, 0, positions);
+    ++ctx->launches;
+    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
   });
 }
 int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, const void* g, int g_bf16,
@@ -2097,15 +2002,13 @@ int b200w_op_poison_onchip(b200w_ctx* ctx, uint32_t pattern) {
 
 int b200w_op_grad_norm(b200w_ctx* ctx, const void* g, int g_bf16, int64_t n, float* norm_out) {
   return guarded(ctx, [&] {
-    double* ss = nullptr;
-    B200W_CUDA(cudaMalloc(reinterpret_cast<void**>(&ss), sizeof(double)));
-    B200W_CUDA(cudaMemsetAsync(ss, 0, sizeof(double), ctx->stream));
-    grad_sumsq(g, g_bf16 != 0, static_cast<size_t>(n), ss, ctx->stream);
+    auto ss = device_scratch<double>(1);
+    B200W_CUDA(cudaMemsetAsync(ss.get(), 0, sizeof(double), ctx->stream));
+    grad_sumsq(g, g_bf16 != 0, static_cast<size_t>(n), ss.get(), ctx->stream);
     ++ctx->launches;
     double h = 0;
-    B200W_CUDA(cudaMemcpyAsync(&h, ss, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    B200W_CUDA(cudaMemcpyAsync(&h, ss.get(), sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ss);
     if (norm_out) *norm_out = static_cast<float>(sqrt(h));
   });
 }

@@ -4,6 +4,32 @@
 
 namespace b200w {
 
+void* DeviceMemory::alloc_bytes(size_t n) {
+  const size_t bytes = (n + 255) / 256 * 256;
+  void* p = nullptr;
+  if (cudaMalloc(&p, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    throw std::bad_alloc();
+  }
+  held_.emplace_back(p, bytes);
+  bytes_ += static_cast<int64_t>(bytes);
+  return p;
+}
+
+void DeviceMemory::free_held(void* p) {
+  for (auto it = held_.begin(); it != held_.end(); ++it)
+    if (it->first == p) {
+      cudaFree(p);
+      bytes_ -= static_cast<int64_t>(it->second);
+      held_.erase(it);
+      return;
+    }
+}
+
+DeviceMemory::~DeviceMemory() {
+  for (const auto& h : held_) cudaFree(h.first);
+}
+
 namespace {
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                    const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,

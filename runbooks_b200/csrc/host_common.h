@@ -1,13 +1,15 @@
-// Host-side plumbing shared by the kernel launchers: error capture and TMA tensor-map creation.
+// Host-side plumbing shared by the kernel launchers: error capture, memory ownership and TMA tensor-map creation.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include <nvtx3/nvToolsExt.h>
 
@@ -31,6 +33,65 @@ struct Error : std::runtime_error {
       throw ::b200w::Error(std::string("check failed: " #cond " — ") + (msg) +             \
                            " (" __FILE__ ":" + std::to_string(__LINE__) + ")");            \
   } while (0)
+
+// The device memory a context holds: each allocation is cudaMalloc'd in whole 256-byte units, and bytes() is the sum
+// of the units currently held. release and the destructor free with cudaFree, which waits for the device, so a
+// buffer that enqueued work still reads may be released.
+class DeviceMemory {
+ public:
+  DeviceMemory() = default;
+  DeviceMemory(const DeviceMemory&) = delete;
+  DeviceMemory& operator=(const DeviceMemory&) = delete;
+  ~DeviceMemory();
+  // n elements of T; std::bad_alloc, with the CUDA error cleared, when the device has no room
+  template <typename T>
+  T* alloc(size_t n) {
+    return static_cast<T*>(alloc_bytes(n * sizeof(T)));
+  }
+  // frees p, takes its bytes off the count and sets p to nullptr; a pointer alloc did not return (nullptr
+  // included) is only cleared
+  template <typename T>
+  void release(T*& p) {
+    free_held(p);
+    p = nullptr;
+  }
+  int64_t bytes() const { return bytes_; }
+
+ private:
+  void* alloc_bytes(size_t n);
+  void free_held(void* p);
+  std::vector<std::pair<void*, size_t>> held_;
+  int64_t bytes_ = 0;
+};
+
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+
+// Device scratch for the length of one call, counted by no DeviceMemory: n elements of T, freed with cudaFree when
+// it goes out of scope. A failed cudaMalloc throws Error, as every failed CUDA call does.
+template <typename T>
+using DeviceScratch = std::unique_ptr<T[], CudaFree>;
+template <typename T>
+DeviceScratch<T> device_scratch(size_t n) {
+  void* p = nullptr;
+  B200W_CUDA(cudaMalloc(&p, n * sizeof(T)));
+  return DeviceScratch<T>(static_cast<T*>(p));
+}
+
+// Pinned host memory: n elements of T from cudaMallocHost, freed with cudaFreeHost. To regrow one, reset() it before
+// allocating the new one, so that the two are never held at once.
+template <typename T>
+using PinnedBuffer = std::unique_ptr<T[], CudaFreeHost>;
+template <typename T>
+PinnedBuffer<T> pinned_buffer(size_t n) {
+  void* p = nullptr;
+  B200W_CUDA(cudaMallocHost(&p, n * sizeof(T)));
+  return PinnedBuffer<T>(static_cast<T*>(p));
+}
 
 // 2-D bf16 row-major tensor [rows, cols] with leading dimension ld (elements).
 // Box = [box_rows, box_cols], each at most 256; box_cols * 2 bytes must be <= 128 (SWIZZLE_128B span) when swizzled.

@@ -1577,6 +1577,7 @@ struct Infer {
   std::vector<IParam> params;
   std::unordered_map<std::string, int> index;
   size_t n_elems = 0;
+  DeviceMemory mem;   // the device buffers below, the KV cache's included (b200w_infer_device_bytes)
   bf16* w = nullptr;
   // per layer: norm parameters, the projections (offsets of their (0,0) element), biases (OPT), and the decode-time
   // copy of each projection as consecutive 16 KB swizzled tile images (gemm.cu retile_weights): a decode GEMM CTA
@@ -1603,7 +1604,8 @@ struct Infer {
   float2* part_ml = nullptr;    // [max_rows, H, nsplit] (max, sum)
   int32_t *tok = nullptr, *pos = nullptr, *slot = nullptr, *next = nullptr;
   // pinned host staging, max_rows each, one allocation: a step's tokens, positions, slots; any call's next tokens
-  int32_t *pin_tok = nullptr, *pin_pos = nullptr, *pin_slot = nullptr, *pin_next = nullptr;
+  PinnedBuffer<int32_t> pin_tok;
+  int32_t *pin_pos = nullptr, *pin_slot = nullptr, *pin_next = nullptr;
   std::unordered_map<int, cudaGraphExec_t> graphs;  // whole decode step per row count and grouping (graph_key)
   std::unordered_map<int, int> warm;
   // prefill buffers, grown on demand to the largest n_seqs * padded_len seen
@@ -1613,7 +1615,7 @@ struct Infer {
   float* pf_lse = nullptr;
   int32_t *pf_tok = nullptr, *pf_len = nullptr, *pf_slot = nullptr, *pf_last = nullptr, *pf_start = nullptr;
   int32_t* pf_pos = nullptr;   // OPT after a cached prefix: the learned-position row of every token
-  int32_t* pf_pin = nullptr;   // pinned staging of a prefill call of up to pf_cap rows (stage_prefill)
+  PinnedBuffer<int32_t> pf_pin;   // staging of a prefill call of up to pf_cap rows (stage_prefill)
   // token log-probabilities, allocated by the first call that asks for them: the next-token rows [max_rows]
   // (lse, token_lp, top ids / top log-probabilities [max_rows, B200W_MAX_TOP_LOGPROBS]); for prompt scoring a bf16
   // chunk of lm_head outputs [lp_chunk_rows, V] and per-row outputs for lp_cap prefill rows
@@ -1626,50 +1628,17 @@ struct Infer {
   // sampling: rows of m->logits a b200w_infer_sample call may draw from (0: none; every other call clears it), and
   // the per-row parameters and results of a call (sample_bytes), on the device and pinned, from the first such call
   int logits_rows = 0;
-  uint8_t *sp_dev = nullptr, *sp_pin = nullptr;
+  uint8_t* sp_dev = nullptr;
+  PinnedBuffer<uint8_t> sp_pin;
   // penalties, from the first b200w_infer_sample_penalized call: the penalized rows [max_rows, V] sample_kernel then
   // reads, and the entry staging (penalty_bytes), on the device and pinned, grown to the largest call's
   bf16* pen_rows = nullptr;
-  uint8_t *pen_dev = nullptr, *pen_pin = nullptr;
+  uint8_t* pen_dev = nullptr;
+  PinnedBuffer<uint8_t> pen_pin;
   size_t pen_cap = 0;          // bytes of both stagings (0 until both exist)
-  int64_t pen_dev_bytes = 0;   // what pen_dev adds to `bytes`, taken off again when it is replaced
-  std::vector<void*> allocs;
-  int64_t bytes = 0;
-  template <typename T>
-  T* alloc(size_t n) {
-    void* p = nullptr;
-    const size_t b = ((n * sizeof(T) + 255) / 256) * 256;
-    if (cudaMalloc(&p, b) != cudaSuccess) {
-      cudaGetLastError();
-      throw std::bad_alloc();
-    }
-    allocs.push_back(p);
-    bytes += b;
-    return static_cast<T*>(p);
-  }
-  void release(void* p) {
-    for (size_t i = 0; i < allocs.size(); ++i)
-      if (allocs[i] == p) {
-        cudaFree(p);
-        allocs.erase(allocs.begin() + i);
-        return;
-      }
-  }
-  // release, and the count drops the n * sizeof(T) bytes alloc<T>(n) added for p
-  template <typename T>
-  void release_counted(T*& p, size_t n) {
-    if (!p) return;
-    release(p);
-    bytes -= static_cast<int64_t>(((n * sizeof(T) + 255) / 256) * 256);
-    p = nullptr;
-  }
+  // the graphs are destroyed here, before the members that hold the memory they read
   ~Infer() {
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
-    if (pin_tok) cudaFreeHost(pin_tok);
-    if (pf_pin) cudaFreeHost(pf_pin);
-    if (sp_pin) cudaFreeHost(sp_pin);
-    if (pen_pin) cudaFreeHost(pen_pin);
-    for (void* p : allocs) cudaFree(p);
   }
 };
 
@@ -1813,7 +1782,7 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
   const int d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size, qd = m->qd, qkvd = m->qkvd;
   const bool falcon = a.family == B200W_FAMILY_FALCON, llama = a.family == B200W_FAMILY_LLAMA;
   auto make = [&](uint8_t*& dst, size_t woff, int ldw, int N, int K) {
-    if (!dst) dst = m->alloc<uint8_t>(retiled_bytes(N, K));
+    if (!dst) dst = m->mem.alloc<uint8_t>(retiled_bytes(N, K));
     retile_weights(m->w + woff, ldw, dst, N, K, s);
   };
   for (int l = 0; l < a.num_layers; ++l) {
@@ -2052,12 +2021,10 @@ void read_outputs(Infer* m, cudaStream_t s, int n, int32_t* next_tokens, float* 
   if (next_tokens) memcpy(next_tokens, m->pin_next, n * 4);
   if (logits_out) {
     const size_t count = static_cast<size_t>(n) * m->a.vocab_size;
-    void* tmp = nullptr;
-    B200W_CUDA(cudaMalloc(&tmp, count * 4));
-    cast_bf16_to_f32(m->logits, static_cast<float*>(tmp), count, s);
+    auto tmp = device_scratch<float>(count);
+    cast_bf16_to_f32(m->logits, tmp.get(), count, s);
     B200W_CUDA(cudaStreamSynchronize(s));
-    B200W_CUDA(cudaMemcpy(logits_out, tmp, count * 4, cudaMemcpyDeviceToHost));
-    cudaFree(tmp);
+    B200W_CUDA(cudaMemcpy(logits_out, tmp.get(), count * 4, cudaMemcpyDeviceToHost));
   }
   m->logits_rows = n;
 }
@@ -2066,7 +2033,7 @@ void read_outputs(Infer* m, cudaStream_t s, int n, int32_t* next_tokens, float* 
 // carried from one step to the next in h or h2: each step starts again from the embedding.
 void enqueue_decode(Infer* m, cudaStream_t s, int n, int64_t& nl) {
   const auto& a = m->a;
-  B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin_tok, n * 4, cudaMemcpyHostToDevice, s));
+  B200W_CUDA(cudaMemcpyAsync(m->tok, m->pin_tok.get(), n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->pos, m->pin_pos, n * 4, cudaMemcpyHostToDevice, s));
   B200W_CUDA(cudaMemcpyAsync(m->slot, m->pin_slot, n * 4, cudaMemcpyHostToDevice, s));
   Pass p{m, true, n, m->h, m->h2, m->nrm, m->qkv, m->cat, m->mid, m->act, s, nl};
@@ -2085,30 +2052,31 @@ void ensure_prefill(Infer* m, size_t T) {
   const auto& a = m->a;
   const size_t d = a.hidden_size, f = a.intermediate_size, H = a.num_heads, Hkv = a.num_kv_heads;
   const size_t dhp = 128, HT = H + 2 * Hkv;
-  for (void* p : std::initializer_list<void*>{m->pf_h, m->pf_h2, m->pf_nrm, m->pf_qkv, m->pf_qkvp, m->pf_attp,
-                                              m->pf_cat, m->pf_mid, m->pf_act, m->pf_lse, m->pf_tok, m->pf_pos})
-    m->release(p);
-  m->pf_h = m->alloc<bf16>(T * d);
-  m->pf_h2 = m->alloc<bf16>(T * d);
-  m->pf_nrm = m->alloc<bf16>(T * d);
-  m->pf_qkv = m->alloc<bf16>(T * m->qkvd);
-  m->pf_qkvp = nullptr;
-  m->pf_attp = nullptr;
+  for (bf16** p : {&m->pf_h, &m->pf_h2, &m->pf_nrm, &m->pf_qkv, &m->pf_qkvp, &m->pf_attp, &m->pf_cat, &m->pf_mid,
+                   &m->pf_act})
+    m->mem.release(*p);
+  m->mem.release(m->pf_lse);
+  m->mem.release(m->pf_tok);
+  m->mem.release(m->pf_pos);
+  m->pf_cap = 0;
+  m->pf_h = m->mem.alloc<bf16>(T * d);
+  m->pf_h2 = m->mem.alloc<bf16>(T * d);
+  m->pf_nrm = m->mem.alloc<bf16>(T * d);
+  m->pf_qkv = m->mem.alloc<bf16>(T * m->qkvd);
   if (a.head_dim != static_cast<int>(dhp)) {   // 64-wide heads are zero-padded to the 128 the attention kernels take
-    m->pf_qkvp = m->alloc<bf16>(T * HT * dhp);
-    m->pf_attp = m->alloc<bf16>(T * H * dhp);
+    m->pf_qkvp = m->mem.alloc<bf16>(T * HT * dhp);
+    m->pf_attp = m->mem.alloc<bf16>(T * H * dhp);
     B200W_CUDA(cudaMemset(m->pf_qkvp, 0, T * HT * dhp * sizeof(bf16)));
   }
-  m->pf_cat = m->alloc<bf16>(T * m->ld_cat);
+  m->pf_cat = m->mem.alloc<bf16>(T * m->ld_cat);
   const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
-  m->pf_mid = a.family == B200W_FAMILY_FALCON ? nullptr : m->alloc<bf16>(T * fmid);
-  m->pf_act = a.family == B200W_FAMILY_LLAMA ? m->alloc<bf16>(T * f) : nullptr;
-  m->pf_lse = m->alloc<float>(H * T);
-  m->pf_tok = m->alloc<int32_t>(T);
-  m->pf_pos = m->alloc<int32_t>(T);
-  if (m->pf_pin) cudaFreeHost(m->pf_pin);
-  m->pf_pin = nullptr;
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pf_pin), (2 * T + 4 * m->max_batch) * sizeof(int32_t)));
+  m->pf_mid = a.family == B200W_FAMILY_FALCON ? nullptr : m->mem.alloc<bf16>(T * fmid);
+  m->pf_act = a.family == B200W_FAMILY_LLAMA ? m->mem.alloc<bf16>(T * f) : nullptr;
+  m->pf_lse = m->mem.alloc<float>(H * T);
+  m->pf_tok = m->mem.alloc<int32_t>(T);
+  m->pf_pos = m->mem.alloc<int32_t>(T);
+  m->pf_pin.reset();
+  m->pf_pin = pinned_buffer<int32_t>(2 * T + 4 * m->max_batch);
   m->pf_cap = T;
 }
 
@@ -2125,7 +2093,7 @@ int check_logprobs(const b200w_logprobs* lp) {
 void ensure_next_logprobs(Infer* m) {
   if (m->nx_lse) return;
   const size_t B = m->max_rows, K = B200W_MAX_TOP_LOGPROBS;
-  float* p = m->alloc<float>(B * (2 + 2 * K));
+  float* p = m->mem.alloc<float>(B * (2 + 2 * K));
   m->nx_lse = p;
   m->nx_tok = p + B;
   m->nx_top = p + 2 * B;
@@ -2146,21 +2114,21 @@ void next_logprobs(Infer* m, cudaStream_t s, int n, const b200w_logprobs* lp, in
 void ensure_scoring(Infer* m, size_t T) {
   const size_t rows = std::min<size_t>(T, LP_CHUNK);
   if (rows > m->lp_chunk_rows) {
-    if (m->lp_chunk) m->release(m->lp_chunk);
-    m->lp_chunk = nullptr;
+    m->mem.release(m->lp_chunk);
     m->lp_chunk_rows = 0;
-    m->lp_chunk = m->alloc<bf16>(rows * m->a.vocab_size);
+    m->lp_chunk = m->mem.alloc<bf16>(rows * m->a.vocab_size);
     m->lp_chunk_rows = rows;
   }
   if (T > m->lp_cap) {
-    for (void* p : std::initializer_list<void*>{m->lp_tgt, m->lp_top, m->lp_ids, m->lp_targets}) m->release(p);
-    m->lp_tgt = m->lp_top = nullptr;
-    m->lp_ids = m->lp_targets = nullptr;
+    m->mem.release(m->lp_tgt);
+    m->mem.release(m->lp_top);
+    m->mem.release(m->lp_ids);
+    m->mem.release(m->lp_targets);
     m->lp_cap = 0;
-    m->lp_tgt = m->alloc<float>(T);
-    m->lp_top = m->alloc<float>(T * B200W_MAX_TOP_LOGPROBS);
-    m->lp_ids = m->alloc<int32_t>(T * B200W_MAX_TOP_LOGPROBS);
-    m->lp_targets = m->alloc<int32_t>(T);
+    m->lp_tgt = m->mem.alloc<float>(T);
+    m->lp_top = m->mem.alloc<float>(T * B200W_MAX_TOP_LOGPROBS);
+    m->lp_ids = m->mem.alloc<int32_t>(T * B200W_MAX_TOP_LOGPROBS);
+    m->lp_targets = m->mem.alloc<int32_t>(T);
     m->lp_cap = T;
   }
 }
@@ -2198,7 +2166,7 @@ void stage_prefill(Infer* m, cudaStream_t s, const int32_t* tokens, const int32_
   // the staging's regions: tokens [T] | lengths | slots | last rows | starts [max_batch each] | one value per row [T],
   // OPT's learned position after a cached prefix or the target a cold prefill scores
   const int B = m->max_batch;
-  int32_t *pin_tok = m->pf_pin, *pin_len = pin_tok + T, *pin_slot = pin_len + B, *pin_last = pin_slot + B,
+  int32_t *pin_tok = m->pf_pin.get(), *pin_len = pin_tok + T, *pin_slot = pin_len + B, *pin_last = pin_slot + B,
           *pin_start = pin_last + B, *pin_row = pin_start + B;
   memcpy(pin_tok, tokens, T * 4);
   for (int b = 0; b < n_seqs; ++b) {
@@ -2275,23 +2243,14 @@ void check_weights_unshared(const Infer* m) {
 }
 
 // The buffers of the decode step that hold one entry per row: the activations, the attention partials, the index
-// vectors and their pinned staging. free_rows releases those of B rows that exist.
-void free_rows(Infer* m, size_t B) {
-  const auto& a = m->a;
-  const size_t d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size;
-  const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
-  const size_t part = static_cast<size_t>(a.num_heads) * m->kv.nsplit;
-  for (bf16** p : {&m->h, &m->h2, &m->nrm}) m->release_counted(*p, B * d);
-  m->release_counted(m->qkv, B * m->qkvd);
-  m->release_counted(m->cat, B * m->ld_cat);
-  m->release_counted(m->mid, B * fmid);
-  m->release_counted(m->act, B * f);
-  m->release_counted(m->logits, B * V);
-  m->release_counted(m->part_o, B * part * a.head_dim);
-  m->release_counted(m->part_ml, B * part);
-  for (int32_t** p : {&m->tok, &m->pos, &m->slot, &m->next}) m->release_counted(*p, B);
-  if (m->pin_tok) cudaFreeHost(m->pin_tok);
-  m->pin_tok = m->pin_pos = m->pin_slot = m->pin_next = nullptr;
+// vectors and their pinned staging. free_rows releases those that exist.
+void free_rows(Infer* m) {
+  for (bf16** p : {&m->h, &m->h2, &m->nrm, &m->qkv, &m->cat, &m->mid, &m->act, &m->logits}) m->mem.release(*p);
+  m->mem.release(m->part_o);
+  m->mem.release(m->part_ml);
+  for (int32_t** p : {&m->tok, &m->pos, &m->slot, &m->next}) m->mem.release(*p);
+  m->pin_tok.reset();
+  m->pin_pos = m->pin_slot = m->pin_next = nullptr;
   m->max_rows = 0;
 }
 
@@ -2301,26 +2260,26 @@ void alloc_rows(Infer* m, size_t B) {
   const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
   const bool tc = a.num_heads / a.num_kv_heads >= 4;
   const size_t part = static_cast<size_t>(a.num_heads) * m->kv.nsplit;
-  m->h = m->alloc<bf16>(B * d);
-  m->h2 = m->alloc<bf16>(B * d);
-  m->nrm = m->alloc<bf16>(B * d);
-  m->qkv = m->alloc<bf16>(B * qkvd);
-  m->cat = m->alloc<bf16>(B * ldc);
-  m->mid = m->alloc<bf16>(B * fmid);
-  m->act = m->alloc<bf16>(B * f);
-  m->logits = m->alloc<bf16>(B * V);
+  m->h = m->mem.alloc<bf16>(B * d);
+  m->h2 = m->mem.alloc<bf16>(B * d);
+  m->nrm = m->mem.alloc<bf16>(B * d);
+  m->qkv = m->mem.alloc<bf16>(B * qkvd);
+  m->cat = m->mem.alloc<bf16>(B * ldc);
+  m->mid = m->mem.alloc<bf16>(B * fmid);
+  m->act = m->mem.alloc<bf16>(B * f);
+  m->logits = m->mem.alloc<bf16>(B * V);
   if (tc) {
-    m->part_o = m->alloc<float>(B * part * a.head_dim);
-    m->part_ml = m->alloc<float2>(B * part);
+    m->part_o = m->mem.alloc<float>(B * part * a.head_dim);
+    m->part_ml = m->mem.alloc<float2>(B * part);
   }
-  m->tok = m->alloc<int32_t>(B);
-  m->pos = m->alloc<int32_t>(B);
-  m->slot = m->alloc<int32_t>(B);
-  m->next = m->alloc<int32_t>(B);
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pin_tok), 4 * B * sizeof(int32_t)));
-  m->pin_pos = m->pin_tok + B;
-  m->pin_slot = m->pin_tok + 2 * B;
-  m->pin_next = m->pin_tok + 3 * B;
+  m->tok = m->mem.alloc<int32_t>(B);
+  m->pos = m->mem.alloc<int32_t>(B);
+  m->slot = m->mem.alloc<int32_t>(B);
+  m->next = m->mem.alloc<int32_t>(B);
+  m->pin_tok = pinned_buffer<int32_t>(4 * B);
+  m->pin_pos = m->pin_tok.get() + B;
+  m->pin_slot = m->pin_tok.get() + 2 * B;
+  m->pin_next = m->pin_tok.get() + 3 * B;
   m->max_rows = static_cast<int>(B);
 }
 
@@ -2328,11 +2287,11 @@ void alloc_rows(Infer* m, size_t B) {
 // allocated again (they were just freed) and the error goes on to the caller: the context stays usable.
 void step_rows(Infer* m, int R) {
   const int old = m->max_rows;
-  free_rows(m, old);
+  free_rows(m);
   try {
     alloc_rows(m, R);
   } catch (...) {
-    free_rows(m, R);
+    free_rows(m);
     if (old) alloc_rows(m, old);
     throw;
   }
@@ -2370,25 +2329,24 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   build(m.get());
   const auto& a = m->a;
   const size_t B = max_batch;
-  m->w = m->alloc<bf16>(m->n_elems);
-  m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim,
-             [&](size_t bytes) { return static_cast<void*>(m->alloc<uint8_t>(bytes)); });
+  m->w = m->mem.alloc<bf16>(m->n_elems);
+  m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim, m->mem);
   if (m->kv.paged) {
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
     m->pf_limit = static_cast<size_t>(prefill_tokens);
     ensure_prefill(m.get(), m->pf_limit);
   }
   step_rows(m.get(), max_batch);
-  m->pf_len = m->alloc<int32_t>(B);
-  m->pf_slot = m->alloc<int32_t>(B);
-  m->pf_last = m->alloc<int32_t>(B);
-  m->pf_start = m->alloc<int32_t>(B);
-  m->inv_freq = m->alloc<float>(a.head_dim / 2);
+  m->pf_len = m->mem.alloc<int32_t>(B);
+  m->pf_slot = m->mem.alloc<int32_t>(B);
+  m->pf_last = m->mem.alloc<int32_t>(B);
+  m->pf_start = m->mem.alloc<int32_t>(B);
+  m->inv_freq = m->mem.alloc<float>(a.head_dim / 2);
   const size_t f = a.intermediate_size, fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
   const size_t max_n = std::max<size_t>({static_cast<size_t>(a.vocab_size), fmid + m->qkvd,
                                          static_cast<size_t>(a.hidden_size)});
-  m->ws = m->alloc<float>(B * max_n);
-  m->counters = m->alloc<unsigned>((max_n + 127) / 128);
+  m->ws = m->mem.alloc<float>(B * max_n);
+  m->counters = m->mem.alloc<unsigned>((max_n + 127) / 128);
   B200W_CUDA(cudaMemset(m->ws, 0, B * max_n * sizeof(float)));
   B200W_CUDA(cudaMemset(m->counters, 0, ((max_n + 127) / 128) * sizeof(unsigned)));
   std::vector<float> inv(a.head_dim / 2);
@@ -2467,10 +2425,9 @@ void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, co
   c.nsplit = nsplit;
   c.dtype = B200W_KV_FP8_E4M3;
   const size_t n_part = H / Hkv >= 4 ? static_cast<size_t>(n) * H * nsplit : 0;   // [n, H, nsplit]
-  void* part = nullptr;
-  if (n_part) B200W_CUDA(cudaMalloc(&part, n_part * (dh * sizeof(float) + sizeof(float2))));
-  std::unique_ptr<void, cudaError_t (*)(void*)> owner(part, cudaFree);
-  float* part_o = static_cast<float*>(part);
+  DeviceScratch<float> part;
+  if (n_part) part = device_scratch<float>(n_part * (dh + 2));   // part_o [n_part, dh], then part_ml [n_part] float2
+  float* part_o = part.get();
   decode_attention(c, static_cast<const bf16*>(q), ld_q, positions, slots, n, H, Hkv, dh, nsplit * KV_PAGE, part_o,
                    reinterpret_cast<float2*>(part_o + n_part * dh), static_cast<bf16*>(out), ld_out, s, false);
   B200W_CUDA(cudaGetLastError());
@@ -2763,26 +2720,22 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     const size_t n = static_cast<size_t>(n_elements);
     m->tiled_valid = false;
     bf16* dst = m->w + p.off;
-    void* tmp32 = nullptr;
-    void* tmp16 = nullptr;
-    try {
-      const void* src16 = host;                 // dense bf16 source (host or device)
-      cudaMemcpyKind kind = cudaMemcpyHostToDevice;
-      if (dtype == B200W_F32) {
-        B200W_CUDA(cudaMalloc(&tmp32, n * 4));
-        B200W_CUDA(cudaMalloc(&tmp16, n * 2));
-        B200W_CUDA(cudaMemcpyAsync(tmp32, host, n * 4, cudaMemcpyHostToDevice, s));
-        cast_f32_to_bf16(static_cast<float*>(tmp32), tmp16, n, s);
-        src16 = tmp16;
-        kind = cudaMemcpyDeviceToDevice;
-      }
-      // rows of `cols` elements into rows of stride ld (ld == cols: one contiguous copy)
-      B200W_CUDA(cudaMemcpy2DAsync(dst, p.ld * sizeof(bf16), src16, p.cols * sizeof(bf16), p.cols * sizeof(bf16),
-                                   p.rows, kind, s));
-      B200W_CUDA(cudaStreamSynchronize(s));
-    } catch (...) { cudaFree(tmp32); cudaFree(tmp16); throw; }
-    cudaFree(tmp32);
-    cudaFree(tmp16);
+    DeviceScratch<float> tmp32;
+    DeviceScratch<bf16> tmp16;
+    const void* src16 = host;                 // dense bf16 source (host or device)
+    cudaMemcpyKind kind = cudaMemcpyHostToDevice;
+    if (dtype == B200W_F32) {
+      tmp32 = device_scratch<float>(n);
+      tmp16 = device_scratch<bf16>(n);
+      B200W_CUDA(cudaMemcpyAsync(tmp32.get(), host, n * 4, cudaMemcpyHostToDevice, s));
+      cast_f32_to_bf16(tmp32.get(), tmp16.get(), n, s);
+      src16 = tmp16.get();
+      kind = cudaMemcpyDeviceToDevice;
+    }
+    // rows of `cols` elements into rows of stride ld (ld == cols: one contiguous copy)
+    B200W_CUDA(cudaMemcpy2DAsync(dst, p.ld * sizeof(bf16), src16, p.cols * sizeof(bf16), p.cols * sizeof(bf16),
+                                 p.rows, kind, s));
+    B200W_CUDA(cudaStreamSynchronize(s));
   });
 }
 
@@ -2817,7 +2770,7 @@ static int step_impl(b200w_ctx* ctx, const int32_t* tokens, const int32_t* posit
     cudaStream_t s = ctx_stream(ctx);
     int64_t& nl = ctx_launches(ctx);
     m->used = true;
-    memcpy(m->pin_tok, tokens, n * 4);
+    memcpy(m->pin_tok.get(), tokens, n * 4);
     memcpy(m->pin_pos, positions, n * 4);
     memcpy(m->pin_slot, slots, n * 4);
     m->grouped = false;
@@ -2947,31 +2900,25 @@ static int sample_impl(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b2
     const int64_t entries = pen ? check_penalties(pen, n, V) : 0;
     if (n != have) throw StateError("b200w_infer_sample must follow the step or prefill call whose rows it samples");
     if (!m->sp_dev) {
-      m->sp_dev = m->alloc<uint8_t>(sample_bytes(m->max_rows));
-      B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->sp_pin), sample_bytes(m->max_rows)));
+      m->sp_dev = m->mem.alloc<uint8_t>(sample_bytes(m->max_rows));
+      m->sp_pin = pinned_buffer<uint8_t>(sample_bytes(m->max_rows));
     }
     PenaltyBuffers pb{};
     if (pen) {
-      if (!m->pen_rows) m->pen_rows = m->alloc<bf16>(static_cast<size_t>(m->max_rows) * V);
+      if (!m->pen_rows) m->pen_rows = m->mem.alloc<bf16>(static_cast<size_t>(m->max_rows) * V);
       const size_t need = penalty_bytes(n, entries);
       if (need > m->pen_cap) {   // grown geometrically: a request's entries grow by one token a step
         const size_t cap = std::max(need, 2 * m->pen_cap);
-        if (m->pen_dev) {   // the count keeps what the context holds: the old staging leaves it
-          m->release(m->pen_dev);
-          m->bytes -= m->pen_dev_bytes;
-        }
-        if (m->pen_pin) cudaFreeHost(m->pen_pin);
-        m->pen_dev = m->pen_pin = nullptr;
+        m->mem.release(m->pen_dev);
+        m->pen_pin.reset();
         m->pen_cap = 0;
-        const int64_t before = m->bytes;
-        m->pen_dev = m->alloc<uint8_t>(cap);
-        m->pen_dev_bytes = m->bytes - before;
-        B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->pen_pin), cap));
+        m->pen_dev = m->mem.alloc<uint8_t>(cap);
+        m->pen_pin = pinned_buffer<uint8_t>(cap);
         m->pen_cap = cap;
       }
-      pb = PenaltyBuffers{m->pen_rows, m->pen_pin, m->pen_dev};
+      pb = PenaltyBuffers{m->pen_rows, m->pen_pin.get(), m->pen_dev};
     }
-    sample(m->logits, V, n, V, sp, nullptr, tokens_out, token_logit_out, m->sp_pin, m->sp_dev, m->max_rows,
+    sample(m->logits, V, n, V, sp, nullptr, tokens_out, token_logit_out, m->sp_pin.get(), m->sp_dev, m->max_rows,
            ctx_stream(ctx), pen, pen ? &pb : nullptr);
     ctx_launches(ctx) += pen ? (token_logit_out ? 3 : 2) : 1;
   });
@@ -2990,7 +2937,7 @@ int b200w_infer_sample_penalized(b200w_ctx* ctx, int n, const b200w_sampling* sp
 
 int64_t b200w_infer_device_bytes(b200w_ctx* ctx) {
   Infer* m = ctx ? static_cast<Infer*>(ctx_infer_slot(ctx)) : nullptr;
-  return m ? m->bytes : 0;
+  return m ? m->mem.bytes() : 0;
 }
 
 }  // extern "C"

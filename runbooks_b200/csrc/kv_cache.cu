@@ -165,12 +165,8 @@ KVTmaps kv_tmaps(const KVLayer& c, int Hkv, int dh) {
   return {make_tmap_bf16_2d(c.k, c.rows, kd, kd, KV_PAGE, 64), make_tmap_bf16_2d(c.v, c.rows, kd, kd, KV_PAGE, 64)};
 }
 
-KVCache::~KVCache() {
-  if (table_pin) cudaFreeHost(table_pin);
-}
-
 void KVCache::init(int kv_dtype, int n_pages_, int max_batch, int max_ctx, int layers, int num_kv_heads, int head_dim,
-                   const std::function<void*(size_t)>& alloc) {
+                   DeviceMemory& mem) {
   dtype = kv_dtype;
   paged = n_pages_ > 0;
   nsplit = (max_ctx + KV_PAGE - 1) / KV_PAGE;
@@ -178,20 +174,20 @@ void KVCache::init(int kv_dtype, int n_pages_, int max_batch, int max_ctx, int l
   Hkv = num_kv_heads;
   kd = num_kv_heads * head_dim;
   const size_t cache = static_cast<size_t>(layers) * rows() * kd * elem_bytes();
-  k = alloc(cache);
-  v = alloc(cache);
+  k = mem.alloc<uint8_t>(cache);
+  v = mem.alloc<uint8_t>(cache);
   B200W_CUDA(cudaMemset(k, 0, cache));
   B200W_CUDA(cudaMemset(v, 0, cache));
   if (fp8()) {
-    const size_t scales = static_cast<size_t>(layers) * rows() * Hkv * sizeof(float);
-    ks = static_cast<float*>(alloc(scales));
-    vs = static_cast<float*>(alloc(scales));
-    B200W_CUDA(cudaMemset(ks, 0, scales));
-    B200W_CUDA(cudaMemset(vs, 0, scales));
+    const size_t scales = static_cast<size_t>(layers) * rows() * Hkv;
+    ks = mem.alloc<float>(scales);
+    vs = mem.alloc<float>(scales);
+    B200W_CUDA(cudaMemset(ks, 0, scales * sizeof(float)));
+    B200W_CUDA(cudaMemset(vs, 0, scales * sizeof(float)));
   }
   const size_t tab = static_cast<size_t>(max_batch) * nsplit;
-  table = static_cast<int32_t*>(alloc(tab * sizeof(int32_t)));
-  B200W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&table_pin), tab * sizeof(int32_t)));
+  table = mem.alloc<int32_t>(tab);
+  table_pin = pinned_buffer<int32_t>(tab);
   held.assign(max_batch, {});
   floor.assign(max_batch, 0);
   for (int s = 0; s < max_batch; ++s)
@@ -200,7 +196,7 @@ void KVCache::init(int kv_dtype, int n_pages_, int max_batch, int max_ctx, int l
       table_pin[static_cast<size_t>(s) * nsplit + j] = paged ? 0 : page * KV_PAGE;
       if (!paged) held[s].push_back(page);
     }
-  B200W_CUDA(cudaMemcpy(table, table_pin, tab * sizeof(int32_t), cudaMemcpyHostToDevice));
+  B200W_CUDA(cudaMemcpy(table, table_pin.get(), tab * sizeof(int32_t), cudaMemcpyHostToDevice));
   if (paged) {
     for (int p = n_pages - 1; p >= 0; --p) free_pages.push_back(p);   // page 0 is handed out first
     refs.assign(n_pages, 0);
@@ -259,7 +255,7 @@ bool KVCache::reserve_shared(int slot, size_t need, const int32_t* shared_pages,
     free_pages.pop_back();
   }
   floor[slot] = n_shared * KV_PAGE;
-  int32_t* row = table_pin + static_cast<size_t>(slot) * nsplit;
+  int32_t* row = table_pin.get() + static_cast<size_t>(slot) * nsplit;
   std::transform(h.begin(), h.end(), row, [](int32_t page) { return page * KV_PAGE; });
   std::fill(row + h.size(), row + nsplit, 0);
   B200W_CUDA(cudaMemcpyAsync(table + static_cast<size_t>(slot) * nsplit, row, nsplit * sizeof(int32_t),

@@ -5,11 +5,11 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
-#include <functional>
 #include <string>
 #include <vector>
 
 #include "../../include/b200w.h"
+#include "host_common.h"
 #include "ops.h"
 
 namespace b200w {
@@ -41,22 +41,18 @@ struct KVCache {
   void *k = nullptr, *v = nullptr;      // [L][rows()][kd] bf16 or e4m3, zero-initialised
   float *ks = nullptr, *vs = nullptr;   // e4m3: [L][rows()][Hkv], zero-initialised
   int32_t* table = nullptr;
-  int32_t* table_pin = nullptr;
+  PinnedBuffer<int32_t> table_pin;
   std::vector<int32_t> free_pages;
   std::vector<std::vector<int32_t>> held;
   std::vector<int32_t> refs, index_refs, floor;
   int64_t retained = 0;
 
-  KVCache() = default;
-  KVCache(const KVCache&) = delete;
-  KVCache& operator=(const KVCache&) = delete;
-  ~KVCache();
-  // n_pages 0: the contiguous cache. Device memory comes from `alloc` (bytes), which owns it; the pools are zeroed,
+  // n_pages 0: the contiguous cache. Device memory comes from `mem`, which owns it; the pools are zeroed,
   // because the tensor-core decode attention multiplies P = 0 by whatever the rows beyond a slot's length hold (a page
   // handed out again holds zeros or K/V an earlier request wrote: finite either way; the e4m3 writer never stores a
   // NaN byte)
   void init(int kv_dtype, int n_pages, int max_batch, int max_ctx, int layers, int num_kv_heads, int head_dim,
-            const std::function<void*(size_t)>& alloc);
+            DeviceMemory& mem);
   bool fp8() const { return dtype == B200W_KV_FP8_E4M3; }
   size_t rows() const { return static_cast<size_t>(n_pages) * KV_PAGE; }
   size_t elem_bytes() const { return fp8() ? 1 : 2; }
