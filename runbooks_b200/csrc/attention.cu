@@ -53,19 +53,6 @@ __device__ __forceinline__ void require_1024_aligned(const void* p) {
     __trap();
   }
 }
-__device__ __forceinline__ float ex2(float x) {  // one MUFU.EX2
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
 // fp32 accumulator columns [16 kk, 16 kk + 16) -> the bf16 A fragment of the kk-th K = 16 slice
 template <int R>
 __device__ __forceinline__ void to_afrag(const float (&s)[R], int kk, uint32_t (&a)[4]) {
@@ -73,11 +60,6 @@ __device__ __forceinline__ void to_afrag(const float (&s)[R], int kk, uint32_t (
   a[1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
   a[2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
   a[3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
-}
-// one free-barrier arrival per consumer warp, after its warpgroup's MMAs that read the buffer retired
-__device__ __forceinline__ void warp_release(uint64_t* bar) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 // D[64 x N] = A[64 x dh] B[N x dh]^T, both K-major with the two dh halves `a_atom` / `b_atom` bytes apart
 template <int N, int R>

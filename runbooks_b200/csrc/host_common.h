@@ -93,6 +93,9 @@ PinnedBuffer<T> pinned_buffer(size_t n) {
   return PinnedBuffer<T>(static_cast<T*>(p));
 }
 
+// ceil(a / b) for a grid size
+inline int cdiv(long long a, int b) { return static_cast<int>((a + b - 1) / b); }
+
 // 2-D bf16 row-major tensor [rows, cols] with leading dimension ld (elements).
 // Box = [box_rows, box_cols], each at most 256; box_cols * 2 bytes must be <= 128 (SWIZZLE_128B span) when swizzled.
 // Out-of-bounds elements are zero-filled by the hardware (used for K / M / N tails).

@@ -1,8 +1,9 @@
-// The serving engine's KV cache (DESIGN §3.5): the pools, the page table and the page state, and the kernels that
-// write K/V into it. Readers take one layer of it as a KVLayer (ops.h).
+// The serving engine's KV cache (DESIGN §3.5): the pools, the page table and the page state, the kernels that
+// write K/V into it, and the decoding of its e4m3 pages. Readers take one layer of it as a KVLayer (ops.h).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 
 #include <string>
@@ -11,6 +12,7 @@
 #include "../../include/b200w.h"
 #include "host_common.h"
 #include "ops.h"
+#include "ptx.cuh"
 
 namespace b200w {
 
@@ -21,6 +23,22 @@ constexpr int KV_PAGE = 128;
 // cache row of position p of the slot whose table row is `row` (a row index is below 2^31: 32-bit arithmetic)
 __device__ __forceinline__ size_t cache_row(const int32_t* __restrict__ row, unsigned p) {
   return static_cast<unsigned>(row[p / KV_PAGE]) + p % KV_PAGE;
+}
+
+// Readers of the e4m3 pool (kv_cache.cu writes it): the bytes are exact in bf16, and the scales are applied in fp32.
+// two e4m3 bytes (low byte first) -> two floats, exact
+__device__ __forceinline__ float2 e4m3x2_to_float2(uint32_t two) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two), __NV_E4M3);
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// 8 e4m3 bytes -> 4 bf16x2 words, exact
+__device__ __forceinline__ void e4m3x8_to_bf16(uint2 u, uint32_t* w) {
+  const uint32_t b[2] = {u.x, u.y};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = e4m3x2_to_float2(b[j / 2] >> (16 * (j % 2)));
+    w[j] = pack_bf16x2(f.x, f.y);
+  }
 }
 
 // TMA maps of a layer's K and V pools with one box per page: bf16 as [128 keys x 64] SWIZZLE_128B atoms, e4m3 as one

@@ -15,17 +15,9 @@ namespace {
 
 using bf16 = __nv_bfloat16;
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-// block-wide sum; `red` is >= 32 floats of shared memory; all threads get the result.
+// block-wide sum; `red` is >= 32 floats of shared memory; all threads get the result. The same sum as
+// block_reduce(v, red, false) (ptx.cuh), kept because ptxas schedules RMSNorm's and grad_sumsq's reductions
+// differently through that one.
 __device__ __forceinline__ float block_sum(float v, float* red) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   v = warp_sum(v);
@@ -34,13 +26,6 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   __syncthreads();
   float r = (lane < nw) ? red[lane] : 0.f;
   return warp_sum(r);
-}
-
-__device__ __forceinline__ void load8(const bf16* p, float (&f)[8]) {
-  uint4 u = *reinterpret_cast<const uint4*>(p);
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z),
-         d = unpack_bf16x2(u.w);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
 }
 __device__ __forceinline__ void store8(bf16* p, const float (&f)[8]) {
   uint4 u;

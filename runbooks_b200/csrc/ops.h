@@ -1,6 +1,7 @@
 // C++ launchers for every kernel on the fine-tune hot path (SURVEY.md §8a rows a3..a12).
 // All pointers are DEVICE pointers; bf16 unless said otherwise; everything is enqueued on `s`.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -79,7 +80,7 @@ void attention_bwd(const void* qkv, int ld_qkv, int k_off, int v_off, const void
                    const void* dout, int ld_out, const float* lse2, float* delta, void* dqkv, int B,
                    int S, int H, int Hkv, float scale, cudaStream_t s, const DocBounds* docs = nullptr);
 
-// ---- infer.cu ------------------------------------------------------------------------------
+// ---- kv_attention.cu ------------------------------------------------------------------------
 // One layer of a KV cache as its writers and readers see it (DESIGN §3.5). Position p of cache slot `slot` is row
 // table[slot * nsplit + p / 128] + p % 128 of k / v [rows, Hkv * dh]: bf16, or e4m3 bytes (dtype B200W_KV_FP8_E4M3)
 // with one fp32 scale per (row, kv head) in kscale / vscale [rows, Hkv]. rows is a multiple of 128.
@@ -91,7 +92,7 @@ struct KVLayer {
   int nsplit = 0;
   int dtype = 0;   // B200W_KV_BF16 (0) or B200W_KV_FP8_E4M3
 };
-// Causal attention of prompt suffixes after a cached prefix (infer.cu attn_fwd_cached_kernel). Sequence b's rows
+// Causal attention of prompt suffixes after a cached prefix (attn_fwd_cached_kernel). Sequence b's rows
 // [b * S, b * S + S) of q [n_seqs * S, ld_q] (head h at column h * q_head_stride, its first dh columns used) are its
 // positions starts[b] + p; they attend to positions [0, position] of cache slot slots[b] of c. starts[b] is a
 // multiple of 128 below lengths[b]; the pages of positions [0, lengths[b]) are the caller's to have filled and
@@ -106,13 +107,26 @@ void decode_attention_fp8(const void* q, int ld_q, const void* kcache, const voi
                           const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
                           const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H, int Hkv,
                           int dh, float scale, cudaStream_t s);
-// Row-wise log-softmax of bf16 logits [rows, ld] (V % 8 == 0, ld % 8 == 0; infer.cu logprobs_kernel): lse, the
+// The decode step's attention: the n new tokens (queries q [n, ld_q], head h at column h * dh; pos / slot DEVICE
+// [n]) over their cache slots -> out [n, ldo]. On the tensor cores when at least 4 query heads share a kv head, with
+// partials part_o [n, H, nsplit, dh] and part_ml [n, H, nsplit]; else on the CUDA cores (max_ctx sizes the score
+// staging). grouped: some rows share a slot at consecutive positions (their K/V is then read once per group; the
+// kernels without it treat each row alone, which is what the plain step does). Returns the launches.
+int decode_attention(const KVLayer& c, const __nv_bfloat16* q, int ld_q, const int32_t* pos, const int32_t* slot, int n,
+                     int H, int Hkv, int dh, int max_ctx, float* part_o, float2* part_ml, __nv_bfloat16* out, int ldo,
+                     cudaStream_t s, bool grouped);
+// The floats of partials (part_o, then part_ml: dh + 2 per row, head and key block) decode_attention needs for n rows;
+// 0 when it runs on the CUDA cores, which need none.
+size_t decode_attention_partials(int n, int H, int Hkv, int dh, int nsplit);
+
+// ---- logits.cu -----------------------------------------------------------------------------
+// Row-wise log-softmax of bf16 logits [rows, ld] (V % 8 == 0, ld % 8 == 0; logprobs_kernel): lse, the
 // log-probability of targets[r] (nullable; an id outside [0, V) gives 0) and of the row maximum, and the k
 // (<= B200W_MAX_TOP_LOGPROBS) largest logits as ids and log-probabilities [rows, k], by value descending with ties
 // to the smaller id. Every output is nullable.
 void logprobs(const void* logits, int ld, int rows, int V, const int32_t* targets, int k, float* lse,
               float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp, cudaStream_t s);
-// One sampled token per row of bf16 logits [rows, ld] (infer.cu sample_kernel; b200w.h b200w_infer_sample has the
+// One sampled token per row of bf16 logits [rows, ld] (sample_kernel; b200w.h b200w_infer_sample has the
 // definition). sp, u (nullable: Philox from seed / draw), tokens_out and token_logit_out (nullable) are HOST arrays;
 // they travel through `host` (pinned or not) and `dev`, sample_bytes(cap) bytes each, rows <= cap. check_sampling
 // throws on a bad argument; sample calls it before any GPU work and returns after the stream has drained.
@@ -127,7 +141,7 @@ void check_sampling(const b200w_sampling* sp, int n, int V, const int32_t* token
 void sample(const void* logits, int ld, int rows, int V, const b200w_sampling* sp, const float* u,
             int32_t* tokens_out, float* token_logit_out, void* host, void* dev, int cap, cudaStream_t s,
             const b200w_penalties* pen = nullptr, const PenaltyBuffers* pb = nullptr);
-// Penalties (infer.cu penalize_kernel; b200w.h b200w_penalties has the definition). check_penalties throws on a bad
+// Penalties (penalize_kernel; b200w.h b200w_penalties has the definition). check_penalties throws on a bad
 // argument and returns the number of entries; penalize (after it) stages the entries through `host` and `dev`,
 // penalty_bytes(rows, entries) bytes each, and writes out [rows, V] (16-byte aligned) on stream s.
 size_t penalty_bytes(int rows, int64_t entries);

@@ -1,6 +1,7 @@
 // Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), clusters, wgmma.
 // Everything the GEMM and attention kernels issue goes through these wrappers, so a
-// descriptor-encoding mistake has exactly one place to be fixed.
+// descriptor-encoding mistake has exactly one place to be fixed. The bf16 / exp2 helpers and the warp, quad and
+// block reductions every source's kernels share live here too.
 //
 // wgmma shared-memory descriptor (PTX ISA "Matrix Descriptor Format"): start>>4 [0,14), LBO>>4 [16,30),
 // SBO>>4 [32,46), base offset [49,52) = 0, layout type [62,64) with SWIZZLE_128B = 1.
@@ -378,6 +379,56 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
 // are 128 B and whose base is 1024 B aligned (what TMA writes and wgmma reads).
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
   return row * 128u + ((chunk ^ (row & 7u)) << 4);
+}
+// 8 consecutive bf16 (one 16-byte load) -> fp32
+__device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8]) {
+  uint4 u = *reinterpret_cast<const uint4*>(p);
+  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z),
+         d = unpack_bf16x2(u.w);
+  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
+}
+__device__ __forceinline__ float ex2(float x) {  // 2^x, one MUFU.EX2
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+// ------------------------------------------------------------------------------------------
+// reductions
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+// block-wide sum (is_max: maximum); `red` is >= 32 floats of shared memory; all threads get the result.
+__device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  v = is_max ? warp_max(v) : warp_sum(v);
+  __syncthreads();  // protect `red` from the previous use
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float r = (lane < nw) ? red[lane] : (is_max ? -INFINITY : 0.f);
+  return is_max ? warp_max(r) : warp_sum(r);
+}
+// over the 4 lanes of a quad: the threads that hold one row of a wgmma accumulator
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// one free-barrier arrival per warp, after its warpgroup's MMAs that read the buffer retired
+__device__ __forceinline__ void warp_release(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
 }  // namespace b200w

@@ -57,7 +57,7 @@ def test_kv_writer_and_reader_instances_neither_spill_nor_serialize(tmp_path):
         pytest.skip("nvcc is not installed")
     from runbooks_b200.build import NVCC_FLAGS
     log = ""
-    for src in ("kv_cache.cu", "infer.cu"):   # the writers, and the readers
+    for src in ("kv_cache.cu", "kv_attention.cu"):   # the writers, and the readers
         r = subprocess.run([nvcc, *NVCC_FLAGS, "-Xptxas=-v", "-c", os.path.join(ROOT, "runbooks_b200", "csrc", src),
                             "-o", str(tmp_path / src.replace(".cu", ".o"))], capture_output=True, text=True)
         assert r.returncode == 0, r.stderr

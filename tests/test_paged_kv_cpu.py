@@ -270,8 +270,9 @@ def test_decode_attention_instances_neither_spill_nor_serialize(tmp_path):
     if nvcc is None:
         pytest.skip("nvcc is not installed")
     from runbooks_b200.build import NVCC_FLAGS
-    r = subprocess.run([nvcc, *NVCC_FLAGS, "-Xptxas=-v", "-c", os.path.join(ROOT, "runbooks_b200", "csrc", "infer.cu"),
-                        "-o", str(tmp_path / "infer.o")], capture_output=True, text=True)
+    src = os.path.join(ROOT, "runbooks_b200", "csrc", "kv_attention.cu")
+    r = subprocess.run([nvcc, *NVCC_FLAGS, "-Xptxas=-v", "-c", src, "-o", str(tmp_path / "kv_attention.o")],
+                       capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     log = r.stdout + r.stderr
     assert not [ln for ln in log.splitlines() if re.search(r"C751[45]|serialized", ln) and "decode_attn" in ln]
