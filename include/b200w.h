@@ -31,6 +31,10 @@ extern "C" {
 #define B200W_API
 #endif
 
+/* A call on a context returns, by the kind of failure: INVALID for a refused argument or a NULL context, STATE for a
+ * call that does not fit the context's configuration or the calls before it, OOM when device memory runs out, and
+ * CUDA or NCCL for a failed CUDA or NCCL call, after which the context is dead and b200w_destroy aborts its
+ * communicator instead of destroying it cleanly. */
 typedef enum {
   B200W_OK = 0,
   B200W_ERR_INVALID = -1, /* bad argument / unsupported shape */

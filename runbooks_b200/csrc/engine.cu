@@ -155,16 +155,6 @@ __global__ void init_normal_kernel(float* master, bf16* w, size_t n, uint64_t se
     if (w) w[j] = __float2bfloat16_rn(r);
   }
 }
-// Fills this SM's shared memory (all 227 KB a block may use) with `pattern` (b200w_op_poison_onchip).
-constexpr int POISON_SMEM = 227 * 1024;
-__global__ void __launch_bounds__(128, 1) poison_onchip_kernel(uint32_t pattern) {
-  extern __shared__ __align__(16) uint32_t poison_sm[];
-  for (int i = threadIdx.x; i < POISON_SMEM / 4; i += blockDim.x) poison_sm[i] = pattern;
-  __syncthreads();
-  // keep the smem stores alive
-  if (poison_sm[(threadIdx.x * 977) % (POISON_SMEM / 4)] != pattern) __trap();
-}
-
 __global__ void fill_kernel(float* master, bf16* w, size_t n, float val) {
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -233,7 +223,7 @@ struct b200w_ctx {
   long long* cnt_dev = nullptr;  // target count, summed over the ranks (HF num_items_in_batch)
   double* sumsq = nullptr;
   PinnedBuffer<float> host_scal;  // [8]
-  float* hook_scal = nullptr;
+  float* hook_scal = nullptr;     // [8] for the per-kernel hooks (ctx_scal)
 
   // ---- timing / profiling (bench.py) ----
   cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
@@ -267,37 +257,6 @@ int qd_of(const b200w_ctx* c) { return c->arch.num_heads * c->dhp; }
 int kd_of(const b200w_ctx* c) { return c->arch.num_kv_heads * c->dhp; }
 int qkv_dim(const b200w_ctx* c) { return qd_of(c) + 2 * kd_of(c); }
 constexpr int OPT_POS_OFFSET = 2;  // HF models/opt/modeling_opt.py:53
-
-// device scalar scratch for the per-kernel hooks (exists without a model)
-float* ctx_scal(b200w_ctx* c) {
-  if (!c->hook_scal) c->hook_scal = c->mem.alloc<float>(8);
-  return c->hook_scal;
-}
-
-template <typename F>
-int guarded(b200w_ctx* ctx, F&& f) {
-  if (!ctx) return B200W_ERR_INVALID;
-  try {
-    B200W_CUDA(cudaSetDevice(ctx->device));
-    f();
-    return B200W_OK;
-  } catch (const NcclError& e) {
-    ctx->err = e.what();
-    ctx->poisoned = true;
-    return B200W_ERR_NCCL;
-  } catch (const std::bad_alloc&) {
-    ctx->err = "device memory exhausted";
-    return B200W_ERR_OOM;
-  } catch (const Error& e) {
-    ctx->err = e.what();
-    if (ctx->err.rfind("check failed", 0) == 0) return B200W_ERR_INVALID;
-    ctx->poisoned = true;
-    return B200W_ERR_CUDA;
-  } catch (const std::exception& e) {
-    ctx->err = e.what();
-    return B200W_ERR_INVALID;
-  }
-}
 
 // kind: 'm' matrix (decayed), 'n' norm weight (ones, no decay), 'b' bias / LayerNorm bias (zeros, no
 // decay). pad: see Param. HF Trainer's decay rule (trainer.py:1280-1290): everything except
@@ -899,9 +858,9 @@ void upload_batch(b200w_ctx* c, const int32_t* ids, const int32_t* labels, size_
   // that poisons the CUDA context, so reject bad batches on the host (n_tok integer compares)
   const int32_t V = c->arch.vocab_size;
   for (size_t i = 0; i < n_tok; ++i) {
-    if (ids[i] < 0 || ids[i] >= V) throw Error("check failed: token id outside the vocabulary");
+    if (ids[i] < 0 || ids[i] >= V) throw InvalidArgument("check failed: token id outside the vocabulary");
     if (labels[i] != -100 && (labels[i] < 0 || labels[i] >= V))
-      throw Error("check failed: label outside the vocabulary (use -100 to ignore)");
+      throw InvalidArgument("check failed: label outside the vocabulary (use -100 to ignore)");
   }
   ensure_ids(c, n_tok);
   memcpy(c->pinned.get(), ids, n_tok * sizeof(int32_t));
@@ -926,11 +885,12 @@ void upload_positions(b200w_ctx* c, const int32_t* positions, int n_seqs) {
   const int S = c->arch.max_seq_len;
   for (int r = 0; r < n_seqs; ++r) {
     const int32_t* p = positions + static_cast<size_t>(r) * S;
-    if (p[0] != 0) throw Error("check failed: positions of row " + std::to_string(r) + " do not start at 0");
+    if (p[0] != 0)
+      throw InvalidArgument("check failed: positions of row " + std::to_string(r) + " do not start at 0");
     for (int i = 1; i < S; ++i)
       if (p[i] != 0 && p[i] != p[i - 1] + 1)
-        throw Error("check failed: positions[" + std::to_string(r) + "][" + std::to_string(i) + "] = " +
-                    std::to_string(p[i]) + " is neither 0 (a new document) nor the previous position + 1");
+        throw InvalidArgument("check failed: positions[" + std::to_string(r) + "][" + std::to_string(i) + "] = " +
+                              std::to_string(p[i]) + " is neither 0 (a new document) nor the previous position + 1");
   }
   const size_t n = static_cast<size_t>(n_seqs) * S;
   if (c->docs_cap < n) {
@@ -1203,6 +1163,35 @@ void ctx_fill_const(b200w_ctx* c, void* w_bf16, size_t n, float value) {
   fill_kernel<<<64, 256, 0, c->stream>>>(nullptr, static_cast<bf16*>(w_bf16), n, value);
   B200W_CUDA(cudaGetLastError());
 }
+float* ctx_scal(b200w_ctx* c) {
+  if (!c->hook_scal) c->hook_scal = c->mem.alloc<float>(8);
+  return c->hook_scal;
+}
+int ctx_fail(b200w_ctx* c) {
+  try {
+    throw;
+  } catch (const NcclError& e) {
+    c->err = e.what();
+    c->poisoned = true;
+    return B200W_ERR_NCCL;
+  } catch (const std::bad_alloc&) {
+    c->err = "device memory exhausted";
+    return B200W_ERR_OOM;
+  } catch (const InvalidArgument& e) {
+    c->err = e.what();
+    return B200W_ERR_INVALID;
+  } catch (const StateError& e) {
+    c->err = e.what();
+    return B200W_ERR_STATE;
+  } catch (const Error& e) {
+    c->err = e.what();
+    c->poisoned = true;
+    return B200W_ERR_CUDA;
+  } catch (const std::exception& e) {
+    c->err = e.what();
+    return B200W_ERR_INVALID;
+  }
+}
 
 // ============================================================================================
 // C ABI
@@ -1210,10 +1199,6 @@ void ctx_fill_const(b200w_ctx* c, void* w_bf16, size_t n, float value) {
 extern "C" {
 
 int b200w_abi_version(void) { return B200W_ABI_VERSION; }
-int b200w_debug_gemm_raster(int M, int N, int K, int tile_m, int tile_n, int32_t* coords) {
-  if (M <= 0 || N <= 0 || K <= 0 || tile_m <= 0 || tile_n <= 0) return -1;
-  return b200w::gemm_debug_raster(M, N, K, tile_m, tile_n, coords);
-}
 
 int b200w_create(int device, b200w_ctx** out) {
   if (!out) return B200W_ERR_INVALID;
@@ -1403,7 +1388,7 @@ int b200w_param_info(b200w_ctx* ctx, int64_t index, char* name, size_t name_cap,
 static const Param& find_param(b200w_ctx* ctx, const char* name, int64_t n_elements) {
   B200W_CHECK(ctx->has_model && name, "no model / name");
   auto it = ctx->index.find(name);
-  if (it == ctx->index.end()) throw Error(std::string("check failed: unknown parameter ") + name);
+  if (it == ctx->index.end()) throw InvalidArgument(std::string("check failed: unknown parameter ") + name);
   const Param& p = ctx->params[it->second];
   B200W_CHECK(n_elements == p.rows * p.cols, "element count does not match the parameter shape");
   return p;
@@ -1530,7 +1515,8 @@ int b200w_read_state(b200w_ctx* ctx, const char* name, int kind, float* host, in
     if (ctx->shard) {
       // only 1/nranks of master / m / v lives here and the reduced gradient is scattered: the weights are
       // readable (from the all-gathered compute copy), the rest is not a single-rank quantity
-      if (kind != 0) throw Error("check failed: optimiser state is sharded over the ranks (kind 1..3 unavailable)");
+      if (kind != 0)
+        throw InvalidArgument("check failed: optimiser state is sharded over the ranks (kind 1..3 unavailable)");
       read_dense(ctx, p, nullptr, ctx->w, host);
       return;
     }
@@ -1724,293 +1710,5 @@ int b200w_forward_docs(b200w_ctx* ctx, const int32_t* ids, const int32_t* labels
 
 int64_t b200w_launch_count(const b200w_ctx* ctx) { return ctx ? ctx->launches : 0; }
 int64_t b200w_device_bytes(const b200w_ctx* ctx) { return ctx ? ctx->mem.bytes() : 0; }
-
-// ---- per-kernel hooks ---------------------------------------------------------------------
-#define HOOK(body)                                              \
-  return guarded(ctx, [&] {                                     \
-    body;                                                       \
-    ++ctx->launches;                                            \
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));             \
-  })
-
-int b200w_op_gemm(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb,
-                  void* D, const void* C, int out_f32, int ldd, int M, int N, int K, int block_n) {
-  HOOK(gemm_bf16(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, out_f32 != 0, ldd, M, N, K, block_n,
-                 ctx->stream));
-}
-int b200w_op_gemm_bias(b200w_ctx* ctx, const void* A, int lda, const void* B, int ldb, void* D, const void* C, int ldd,
-                       int M, int N, int K, const void* bias, int act, int block_n) {
-  HOOK(gemm_bf16_ex(A, false, lda, B, false, ldb, D, C, false, ldd, M, N, K, block_n, bias, act, ctx->stream));
-}
-int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb, float* D,
-                       const float* C, int ldd, int M, int N, int K, int block_n, void* d2) {
-  HOOK(gemm_bf16_ex(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, true, ldd, M, N, K, block_n, nullptr, 0, ctx->stream,
-                    d2));
-}
-int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
-                         int N, int K, int split_k) {
-  return guarded(ctx, [&] {
-    DeviceScratch<float> ws;
-    DeviceScratch<unsigned> cnt;
-    if (split_k) {
-      ws = device_scratch<float>(static_cast<size_t>(M) * N);
-      cnt = device_scratch<unsigned>((N + 127) / 128);
-      B200W_CUDA(cudaMemsetAsync(ws.get(), 0, static_cast<size_t>(M) * N * 4, ctx->stream));
-      B200W_CUDA(cudaMemsetAsync(cnt.get(), 0, ((N + 127) / 128) * 4, ctx->stream));
-    }
-    // twice: the scratch must come back clean
-    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx->stream);
-    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx->stream);
-    ctx->launches += 2;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_embed_fwd(b200w_ctx* ctx, const int32_t* ids, const void* table, const void* pos_table,
-                       void* out, int T, int d, int vocab, int S, int pos_offset) {
-  HOOK(embed_fwd(ids, table, pos_table, out, T, d, vocab, S, pos_offset, ctx->stream));
-}
-int b200w_op_embed_bwd(b200w_ctx* ctx, const int32_t* ids, const void* dout, float* dtable, float* dpos,
-                       int T, int d, int vocab, int pad_id, int S, int pos_offset) {
-  HOOK(embed_bwd(ids, dout, dtable, dpos, T, d, vocab, pad_id, S, pos_offset, ctx->stream));
-}
-int b200w_op_layernorm_fwd(b200w_ctx* ctx, const void* x, const void* w, const void* b, void* y, float* mean,
-                           float* rstd, int T, int d, float eps) {
-  HOOK(layernorm_fwd(x, w, b, y, mean, rstd, T, d, eps, ctx->stream));
-}
-int b200w_op_layernorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const void* w, const float* mean,
-                           const float* rstd, const void* dresid, void* dx, float* dw, float* db, int T,
-                           int d) {
-  return guarded(ctx, [&] {
-    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * 2 * d);
-    layernorm_bwd(dy, x, w, mean, rstd, dresid, dx, dw, db, part.get(), T, d, ctx->stream);
-    ctx->launches += 3;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_bias_act(b200w_ctx* ctx, void* x, const void* bias, int T, int N, int ld, int act) {
-  HOOK(bias_act(x, bias, T, N, ld, act, ctx->stream));
-}
-int b200w_op_relu_bwd(b200w_ctx* ctx, const void* dy, const void* act, void* dz, int64_t n) {
-  HOOK(relu_bwd(dy, act, dz, static_cast<size_t>(n), ctx->stream));
-}
-int b200w_op_gelu_fwd(b200w_ctx* ctx, const void* x, void* y, int64_t n) {
-  HOOK(gelu_fwd(x, y, static_cast<size_t>(n), ctx->stream));
-}
-int b200w_op_gelu_bwd(b200w_ctx* ctx, const void* dy, const void* x, void* dx, int64_t n) {
-  HOOK(gelu_bwd(dy, x, dx, static_cast<size_t>(n), ctx->stream));
-}
-int b200w_op_colsum(b200w_ctx* ctx, const void* dy, float* db, int T, int N, int ld) {
-  return guarded(ctx, [&] {
-    auto part = device_scratch<float>(static_cast<size_t>(colsum_blocks(T)) * N);
-    colsum_add(dy, db, part.get(), T, N, ld, ctx->stream);
-    ctx->launches += 2;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_rmsnorm_fwd(b200w_ctx* ctx, const void* x, const void* w, void* y, float* rstd, int T,
-                         int d, float eps) {
-  HOOK(rmsnorm_fwd(x, w, y, rstd, T, d, eps, ctx->stream));
-}
-int b200w_op_rmsnorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const void* w,
-                         const float* rstd, const void* dresid, void* dx, float* dw, int T, int d) {
-  return guarded(ctx, [&] {
-    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * d);
-    rmsnorm_bwd(dy, x, w, rstd, dresid, dx, dw, part.get(), T, d, ctx->stream);
-    ctx->launches += 2;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_rope(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
-                  int inverse) {
-  return guarded(ctx, [&] {
-    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
-    rope_table(tab.get(), S, dh, theta, ctx->stream);
-    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx->stream);
-    ++ctx->launches;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_swiglu_fwd(b200w_ctx* ctx, const void* gu, void* h, int T, int f) {
-  HOOK(swiglu_fwd(gu, h, T, f, ctx->stream));
-}
-int b200w_op_swiglu_bwd(b200w_ctx* ctx, const void* dh, const void* gu, void* dgu, int T, int f) {
-  HOOK(swiglu_bwd(dh, gu, dgu, T, f, ctx->stream));
-}
-int b200w_op_ce(b200w_ctx* ctx, void* logits, const int32_t* labels, float* nll, int T, int S, int V,
-                float inv_n) {
-  return guarded(ctx, [&] {
-    auto tg = device_scratch<int32_t>(T);
-    B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx) + 4, &inv_n, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    ce_shift_targets(labels, tg.get(), T, S, ctx->stream);
-    ce_loss_fwd_bwd(logits, tg.get(), nll, T, V, ctx_scal(ctx) + 4, ctx->stream);
-    ctx->launches += 2;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
-                           void* out, int ld_out, float* lse2, int B, int S, int H, int Hkv,
-                           float scale) {
-  HOOK(attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx->stream));
-}
-int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
-                                  const void* vcache, int64_t cache_rows, const int32_t* table, int nsplit,
-                                  const int32_t* slots, const int32_t* starts, const int32_t* lengths, void* out,
-                                  int ld_out, int n_seqs, int S, int H, int Hkv, int dh, float scale) {
-  KVLayer c;
-  c.k = const_cast<void*>(kcache);
-  c.v = const_cast<void*>(vcache);
-  c.rows = cache_rows;
-  c.table = table;
-  c.nsplit = nsplit;
-  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
-                            ctx->stream));
-}
-int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
-                                      const void* vcache, const float* kscale, const float* vscale, int64_t cache_rows,
-                                      const int32_t* table, int nsplit, const int32_t* slots, const int32_t* starts,
-                                      const int32_t* lengths, void* out, int ld_out, int n_seqs, int S, int H, int Hkv,
-                                      int dh, float scale) {
-  if (!kscale || !vscale) return B200W_ERR_INVALID;
-  KVLayer c;
-  c.k = const_cast<void*>(kcache);
-  c.v = const_cast<void*>(vcache);
-  c.kscale = const_cast<float*>(kscale);
-  c.vscale = const_cast<float*>(vscale);
-  c.rows = cache_rows;
-  c.table = table;
-  c.nsplit = nsplit;
-  c.dtype = B200W_KV_FP8_E4M3;
-  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
-                            ctx->stream));
-}
-int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
-                                  const float* kscale, const float* vscale, int64_t cache_rows, const int32_t* table,
-                                  int nsplit, const int32_t* positions, const int32_t* slots, void* out, int ld_out,
-                                  int n, int H, int Hkv, int dh, float scale) {
-  if (!(scale > 0.f) || fabsf(scale * sqrtf(static_cast<float>(dh)) - 1.f) > 1e-6f) return B200W_ERR_INVALID;
-  HOOK(decode_attention_fp8(q, ld_q, kcache, vcache, kscale, vscale, cache_rows, table, nsplit, positions, slots, out,
-                            ld_out, n, H, Hkv, dh, scale, ctx->stream));
-}
-int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets, int top_k,
-                      float* lse, float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp) {
-  if (top_k < 0 || top_k > B200W_MAX_TOP_LOGPROBS) return B200W_ERR_INVALID;
-  HOOK(logprobs(logits, ld, rows, V, targets, top_k, lse, target_lp, token_lp, top_ids, top_lp, ctx->stream));
-}
-int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_sampling* sp,
-                    const float* u, int32_t* tokens_out, float* token_logit_out) {
-  return guarded(ctx, [&] {
-    check_sampling(sp, rows, V, tokens_out);
-    std::vector<uint8_t> host(sample_bytes(rows));
-    auto dev = device_scratch<uint8_t>(host.size());
-    sample(logits, ld, rows, V, sp, u, tokens_out, token_logit_out, host.data(), dev.get(), rows, ctx->stream);
-    ++ctx->launches;
-  });
-}
-int b200w_op_penalize(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_penalties* pen,
-                      void* out) {
-  return guarded(ctx, [&] {
-    B200W_CHECK(V >= 8, "bad vocabulary size");
-    const int64_t entries = check_penalties(pen, rows, V);
-    std::vector<uint8_t> host(penalty_bytes(rows, entries));
-    auto dev = device_scratch<uint8_t>(host.size());
-    penalize(logits, ld, rows, V, pen, out, host.data(), dev.get(), ctx->stream);
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    ++ctx->launches;
-  });
-}
-int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
-                           const void* out, const void* dout, int ld_out, const float* lse2,
-                           float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {
-  HOOK(attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv,
-                     scale, ctx->stream));
-}
-}  // extern "C"
-
-namespace {
-// runs f(DocBounds) with the bounds of device positions [B * S] derived into scratch (doc_bounds)
-template <typename F>
-void with_doc_bounds(b200w_ctx* ctx, const int32_t* positions, int B, int S, F&& f) {
-  B200W_CHECK(positions, "NULL positions");
-  const size_t T = static_cast<size_t>(B) * S;
-  auto buf = device_scratch<int32_t>(2 * T);
-  int32_t* se = buf.get();
-  doc_bounds(positions, se, se + T, static_cast<int>(T), S, ctx->stream);
-  ++ctx->launches;
-  const DocBounds db{positions, se, se + T};
-  f(db);
-  B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-}
-}  // namespace
-
-extern "C" {
-
-int b200w_op_attention_fwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off, void* out,
-                                int ld_out, float* lse2, const int32_t* positions, int B, int S, int H, int Hkv,
-                                float scale) {
-  return guarded(ctx, [&] {
-    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
-      attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx->stream, &db);
-      ++ctx->launches;
-    });
-  });
-}
-int b200w_op_attention_bwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
-                                const void* out, const void* dout, int ld_out, const float* lse2, float* delta,
-                                void* dqkv, const int32_t* positions, int B, int S, int H, int Hkv, float scale) {
-  return guarded(ctx, [&] {
-    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
-      attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv, scale,
-                    ctx->stream, &db);
-      ctx->launches += 3;
-    });
-  });
-}
-int b200w_op_rope_positions(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
-                            int inverse, const int32_t* positions) {
-  return guarded(ctx, [&] {
-    B200W_CHECK(positions, "NULL positions");
-    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
-    rope_table(tab.get(), S, dh, theta, ctx->stream);
-    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx->stream, 0, positions);
-    ++ctx->launches;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, const void* g, int g_bf16,
-                   void* w_bf16, int64_t n, float lr, float beta1, float beta2, float eps, float wd,
-                   int step, float gscale) {
-  return guarded(ctx, [&] {
-    B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx), &gscale, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    adamw_step(master, m, v, g, g_bf16 != 0, w_bf16, static_cast<size_t>(n), lr, beta1, beta2, eps, wd, step,
-               ctx_scal(ctx), ctx->stream);
-    ++ctx->launches;
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-int b200w_op_poison_onchip(b200w_ctx* ctx, uint32_t pattern) {
-  return guarded(ctx, [&] {
-    static PerDeviceOnce once;
-    once.run([&] {
-      B200W_CUDA(cudaFuncSetAttribute(poison_onchip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, POISON_SMEM));
-    });
-    // one CTA per SM at a time (smem-limited); several waves so that every SM is visited
-    poison_onchip_kernel<<<sm_count() * 4, 128, POISON_SMEM, ctx->stream>>>(pattern);
-    B200W_CUDA(cudaGetLastError());
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-  });
-}
-
-int b200w_op_grad_norm(b200w_ctx* ctx, const void* g, int g_bf16, int64_t n, float* norm_out) {
-  return guarded(ctx, [&] {
-    auto ss = device_scratch<double>(1);
-    B200W_CUDA(cudaMemsetAsync(ss.get(), 0, sizeof(double), ctx->stream));
-    grad_sumsq(g, g_bf16 != 0, static_cast<size_t>(n), ss.get(), ctx->stream);
-    ++ctx->launches;
-    double h = 0;
-    B200W_CUDA(cudaMemcpyAsync(&h, ss.get(), sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    B200W_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (norm_out) *norm_out = static_cast<float>(sqrt(h));
-  });
-}
 
 }  // extern "C"

@@ -15,7 +15,17 @@
 
 namespace b200w {
 
+// The exceptions the library throws. ctx_fail (ctx_access.h) turns each into the status named here, by type alone.
+// a failed CUDA call or a broken internal invariant (B200W_ERR_CUDA; the context is dead)
 struct Error : std::runtime_error {
+  using std::runtime_error::runtime_error;
+};
+// an argument the call refuses (B200W_ERR_INVALID); B200W_CHECK throws it
+struct InvalidArgument : std::runtime_error {
+  using std::runtime_error::runtime_error;
+};
+// a call that does not fit the context's configuration or the calls before it (B200W_ERR_STATE)
+struct StateError : std::runtime_error {
   using std::runtime_error::runtime_error;
 };
 
@@ -30,8 +40,8 @@ struct Error : std::runtime_error {
 #define B200W_CHECK(cond, msg)                                                             \
   do {                                                                                     \
     if (!(cond))                                                                           \
-      throw ::b200w::Error(std::string("check failed: " #cond " — ") + (msg) +             \
-                           " (" __FILE__ ":" + std::to_string(__LINE__) + ")");            \
+      throw ::b200w::InvalidArgument(std::string("check failed: " #cond " — ") + (msg) +   \
+                                     " (" __FILE__ ":" + std::to_string(__LINE__) + ")");  \
   } while (0)
 
 // The device memory a context holds: each allocation is cudaMalloc'd in whole 256-byte units, and bytes() is the sum

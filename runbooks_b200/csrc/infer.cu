@@ -24,7 +24,6 @@
 
 #include <algorithm>
 #include <memory>
-#include <stdexcept>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -367,33 +366,14 @@ void build(Infer* m) {
   else m->p_lm = add_dense(m, "lm_head.weight", a.vocab_size, d);
 }
 
-// a call that does not fit the context's configuration (B200W_ERR_STATE)
-struct StateError : std::runtime_error {
-  using std::runtime_error::runtime_error;
-};
-
+// guarded, for the serving calls: only the call right after a step or a prefill may sample from the logits it left
+// (the training calls leave them alone)
 template <typename F>
 int iguard(b200w_ctx* ctx, F&& f) {
-  if (!ctx) return B200W_ERR_INVALID;
-  try {
-    B200W_CUDA(cudaSetDevice(ctx_device(ctx)));
-    // only the call right after a step or a prefill may sample from the logits it left
+  return guarded(ctx, [&] {
     if (Infer* m = static_cast<Infer*>(ctx_infer_slot(ctx))) m->logits_rows = 0;
     f();
-    return B200W_OK;
-  } catch (const std::bad_alloc&) {
-    ctx_set_error(ctx, "device memory exhausted");
-    return B200W_ERR_OOM;
-  } catch (const Error& e) {
-    ctx_set_error(ctx, e.what());
-    return std::string(e.what()).rfind("check failed", 0) == 0 ? B200W_ERR_INVALID : B200W_ERR_CUDA;
-  } catch (const StateError& e) {
-    ctx_set_error(ctx, e.what());
-    return B200W_ERR_STATE;
-  } catch (const std::exception& e) {
-    ctx_set_error(ctx, e.what());
-    return B200W_ERR_INVALID;
-  }
+  });
 }
 
 Infer* model(b200w_ctx* ctx) {
@@ -1057,7 +1037,7 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     Infer* m = model(ctx);
     B200W_CHECK(name && host, "NULL name / buffer");
     auto it = m->index.find(name);
-    if (it == m->index.end()) throw Error(std::string("check failed: unknown parameter ") + name);
+    if (it == m->index.end()) throw InvalidArgument(std::string("check failed: unknown parameter ") + name);
     const IParam& p = m->params[it->second];
     B200W_CHECK(n_elements == p.rows * p.cols, "element count does not match the parameter shape");
     B200W_CHECK(dtype == B200W_BF16 || dtype == B200W_F32, "dtype must be bf16 or f32");

@@ -1,0 +1,314 @@
+// The per-kernel hooks of include/b200w.h (b200w_op_*, b200w_debug_gemm_raster): one kernel, or one launcher's
+// kernels, on device pointers the caller owns, on the context's stream, for the kernel parity tests. They reach the
+// context only through ctx_access.h.
+#include <math.h>
+
+#include <vector>
+
+#include "../../include/b200w.h"
+#include "ctx_access.h"
+#include "host_common.h"
+#include "ops.h"
+
+using namespace b200w;
+
+namespace {
+// Fills this SM's shared memory (all 227 KB a block may use) with `pattern` (b200w_op_poison_onchip).
+constexpr int POISON_SMEM = 227 * 1024;
+__global__ void __launch_bounds__(128, 1) poison_onchip_kernel(uint32_t pattern) {
+  extern __shared__ __align__(16) uint32_t poison_sm[];
+  for (int i = threadIdx.x; i < POISON_SMEM / 4; i += blockDim.x) poison_sm[i] = pattern;
+  __syncthreads();
+  // keep the smem stores alive
+  if (poison_sm[(threadIdx.x * 977) % (POISON_SMEM / 4)] != pattern) __trap();
+}
+
+// runs f(DocBounds) with the bounds of device positions [B * S] derived into scratch (doc_bounds)
+template <typename F>
+void with_doc_bounds(b200w_ctx* ctx, const int32_t* positions, int B, int S, F&& f) {
+  B200W_CHECK(positions, "NULL positions");
+  const size_t T = static_cast<size_t>(B) * S;
+  auto buf = device_scratch<int32_t>(2 * T);
+  int32_t* se = buf.get();
+  doc_bounds(positions, se, se + T, static_cast<int>(T), S, ctx_stream(ctx));
+  ++ctx_launches(ctx);
+  const DocBounds db{positions, se, se + T};
+  f(db);
+  B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+}
+}  // namespace
+
+extern "C" {
+
+int b200w_debug_gemm_raster(int M, int N, int K, int tile_m, int tile_n, int32_t* coords) {
+  if (M <= 0 || N <= 0 || K <= 0 || tile_m <= 0 || tile_n <= 0) return -1;
+  return b200w::gemm_debug_raster(M, N, K, tile_m, tile_n, coords);
+}
+
+#define HOOK(body)                                              \
+  return guarded(ctx, [&] {                                     \
+    body;                                                       \
+    ++ctx_launches(ctx);                                        \
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));         \
+  })
+
+int b200w_op_gemm(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb,
+                  void* D, const void* C, int out_f32, int ldd, int M, int N, int K, int block_n) {
+  HOOK(gemm_bf16(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, out_f32 != 0, ldd, M, N, K, block_n,
+                 ctx_stream(ctx)));
+}
+int b200w_op_gemm_bias(b200w_ctx* ctx, const void* A, int lda, const void* B, int ldb, void* D, const void* C, int ldd,
+                       int M, int N, int K, const void* bias, int act, int block_n) {
+  HOOK(gemm_bf16_ex(A, false, lda, B, false, ldb, D, C, false, ldd, M, N, K, block_n, bias, act, ctx_stream(ctx)));
+}
+int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb, float* D,
+                       const float* C, int ldd, int M, int N, int K, int block_n, void* d2) {
+  HOOK(gemm_bf16_ex(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, true, ldd, M, N, K, block_n, nullptr, 0, ctx_stream(ctx),
+                    d2));
+}
+int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
+                         int N, int K, int split_k) {
+  return guarded(ctx, [&] {
+    DeviceScratch<float> ws;
+    DeviceScratch<unsigned> cnt;
+    if (split_k) {
+      ws = device_scratch<float>(static_cast<size_t>(M) * N);
+      cnt = device_scratch<unsigned>((N + 127) / 128);
+      B200W_CUDA(cudaMemsetAsync(ws.get(), 0, static_cast<size_t>(M) * N * 4, ctx_stream(ctx)));
+      B200W_CUDA(cudaMemsetAsync(cnt.get(), 0, ((N + 127) / 128) * 4, ctx_stream(ctx)));
+    }
+    // twice: the scratch must come back clean
+    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx_stream(ctx));
+    gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx_stream(ctx));
+    ctx_launches(ctx) += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_embed_fwd(b200w_ctx* ctx, const int32_t* ids, const void* table, const void* pos_table,
+                       void* out, int T, int d, int vocab, int S, int pos_offset) {
+  HOOK(embed_fwd(ids, table, pos_table, out, T, d, vocab, S, pos_offset, ctx_stream(ctx)));
+}
+int b200w_op_embed_bwd(b200w_ctx* ctx, const int32_t* ids, const void* dout, float* dtable, float* dpos,
+                       int T, int d, int vocab, int pad_id, int S, int pos_offset) {
+  HOOK(embed_bwd(ids, dout, dtable, dpos, T, d, vocab, pad_id, S, pos_offset, ctx_stream(ctx)));
+}
+int b200w_op_layernorm_fwd(b200w_ctx* ctx, const void* x, const void* w, const void* b, void* y, float* mean,
+                           float* rstd, int T, int d, float eps) {
+  HOOK(layernorm_fwd(x, w, b, y, mean, rstd, T, d, eps, ctx_stream(ctx)));
+}
+int b200w_op_layernorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const void* w, const float* mean,
+                           const float* rstd, const void* dresid, void* dx, float* dw, float* db, int T,
+                           int d) {
+  return guarded(ctx, [&] {
+    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * 2 * d);
+    layernorm_bwd(dy, x, w, mean, rstd, dresid, dx, dw, db, part.get(), T, d, ctx_stream(ctx));
+    ctx_launches(ctx) += 3;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_bias_act(b200w_ctx* ctx, void* x, const void* bias, int T, int N, int ld, int act) {
+  HOOK(bias_act(x, bias, T, N, ld, act, ctx_stream(ctx)));
+}
+int b200w_op_relu_bwd(b200w_ctx* ctx, const void* dy, const void* act, void* dz, int64_t n) {
+  HOOK(relu_bwd(dy, act, dz, static_cast<size_t>(n), ctx_stream(ctx)));
+}
+int b200w_op_gelu_fwd(b200w_ctx* ctx, const void* x, void* y, int64_t n) {
+  HOOK(gelu_fwd(x, y, static_cast<size_t>(n), ctx_stream(ctx)));
+}
+int b200w_op_gelu_bwd(b200w_ctx* ctx, const void* dy, const void* x, void* dx, int64_t n) {
+  HOOK(gelu_bwd(dy, x, dx, static_cast<size_t>(n), ctx_stream(ctx)));
+}
+int b200w_op_colsum(b200w_ctx* ctx, const void* dy, float* db, int T, int N, int ld) {
+  return guarded(ctx, [&] {
+    auto part = device_scratch<float>(static_cast<size_t>(colsum_blocks(T)) * N);
+    colsum_add(dy, db, part.get(), T, N, ld, ctx_stream(ctx));
+    ctx_launches(ctx) += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_rmsnorm_fwd(b200w_ctx* ctx, const void* x, const void* w, void* y, float* rstd, int T,
+                         int d, float eps) {
+  HOOK(rmsnorm_fwd(x, w, y, rstd, T, d, eps, ctx_stream(ctx)));
+}
+int b200w_op_rmsnorm_bwd(b200w_ctx* ctx, const void* dy, const void* x, const void* w,
+                         const float* rstd, const void* dresid, void* dx, float* dw, int T, int d) {
+  return guarded(ctx, [&] {
+    auto part = device_scratch<float>(static_cast<size_t>(rmsnorm_bwd_blocks(T)) * d);
+    rmsnorm_bwd(dy, x, w, rstd, dresid, dx, dw, part.get(), T, d, ctx_stream(ctx));
+    ctx_launches(ctx) += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_rope(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
+                  int inverse) {
+  return guarded(ctx, [&] {
+    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
+    rope_table(tab.get(), S, dh, theta, ctx_stream(ctx));
+    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx_stream(ctx));
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_swiglu_fwd(b200w_ctx* ctx, const void* gu, void* h, int T, int f) {
+  HOOK(swiglu_fwd(gu, h, T, f, ctx_stream(ctx)));
+}
+int b200w_op_swiglu_bwd(b200w_ctx* ctx, const void* dh, const void* gu, void* dgu, int T, int f) {
+  HOOK(swiglu_bwd(dh, gu, dgu, T, f, ctx_stream(ctx)));
+}
+int b200w_op_ce(b200w_ctx* ctx, void* logits, const int32_t* labels, float* nll, int T, int S, int V,
+                float inv_n) {
+  return guarded(ctx, [&] {
+    auto tg = device_scratch<int32_t>(T);
+    B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx) + 4, &inv_n, sizeof(float), cudaMemcpyHostToDevice, ctx_stream(ctx)));
+    ce_shift_targets(labels, tg.get(), T, S, ctx_stream(ctx));
+    ce_loss_fwd_bwd(logits, tg.get(), nll, T, V, ctx_scal(ctx) + 4, ctx_stream(ctx));
+    ctx_launches(ctx) += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_attention_fwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                           void* out, int ld_out, float* lse2, int B, int S, int H, int Hkv,
+                           float scale) {
+  HOOK(attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx_stream(ctx)));
+}
+int b200w_op_attention_fwd_cached(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
+                                  const void* vcache, int64_t cache_rows, const int32_t* table, int nsplit,
+                                  const int32_t* slots, const int32_t* starts, const int32_t* lengths, void* out,
+                                  int ld_out, int n_seqs, int S, int H, int Hkv, int dh, float scale) {
+  KVLayer c;
+  c.k = const_cast<void*>(kcache);
+  c.v = const_cast<void*>(vcache);
+  c.rows = cache_rows;
+  c.table = table;
+  c.nsplit = nsplit;
+  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
+                            ctx_stream(ctx)));
+}
+int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, int q_head_stride, const void* kcache,
+                                      const void* vcache, const float* kscale, const float* vscale, int64_t cache_rows,
+                                      const int32_t* table, int nsplit, const int32_t* slots, const int32_t* starts,
+                                      const int32_t* lengths, void* out, int ld_out, int n_seqs, int S, int H, int Hkv,
+                                      int dh, float scale) {
+  KVLayer c;
+  c.k = const_cast<void*>(kcache);
+  c.v = const_cast<void*>(vcache);
+  c.kscale = const_cast<float*>(kscale);
+  c.vscale = const_cast<float*>(vscale);
+  c.rows = cache_rows;
+  c.table = table;
+  c.nsplit = nsplit;
+  c.dtype = B200W_KV_FP8_E4M3;
+  HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
+                            ctx_stream(ctx)));
+}
+int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
+                                  const float* kscale, const float* vscale, int64_t cache_rows, const int32_t* table,
+                                  int nsplit, const int32_t* positions, const int32_t* slots, void* out, int ld_out,
+                                  int n, int H, int Hkv, int dh, float scale) {
+  HOOK(B200W_CHECK(scale > 0.f && fabsf(scale * sqrtf(static_cast<float>(dh)) - 1.f) <= 1e-6f,
+                   "the decode attention's scale is 1 / sqrt(head_dim)");
+       decode_attention_fp8(q, ld_q, kcache, vcache, kscale, vscale, cache_rows, table, nsplit, positions, slots, out,
+                            ld_out, n, H, Hkv, dh, scale, ctx_stream(ctx)));
+}
+int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets, int top_k,
+                      float* lse, float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp) {
+  HOOK(logprobs(logits, ld, rows, V, targets, top_k, lse, target_lp, token_lp, top_ids, top_lp, ctx_stream(ctx)));
+}
+int b200w_op_sample(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_sampling* sp,
+                    const float* u, int32_t* tokens_out, float* token_logit_out) {
+  return guarded(ctx, [&] {
+    check_sampling(sp, rows, V, tokens_out);
+    std::vector<uint8_t> host(sample_bytes(rows));
+    auto dev = device_scratch<uint8_t>(host.size());
+    sample(logits, ld, rows, V, sp, u, tokens_out, token_logit_out, host.data(), dev.get(), rows, ctx_stream(ctx));
+    ++ctx_launches(ctx);
+  });
+}
+int b200w_op_penalize(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const b200w_penalties* pen,
+                      void* out) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(V >= 8, "bad vocabulary size");
+    const int64_t entries = check_penalties(pen, rows, V);
+    std::vector<uint8_t> host(penalty_bytes(rows, entries));
+    auto dev = device_scratch<uint8_t>(host.size());
+    penalize(logits, ld, rows, V, pen, out, host.data(), dev.get(), ctx_stream(ctx));
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+    ++ctx_launches(ctx);
+  });
+}
+int b200w_op_attention_bwd(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                           const void* out, const void* dout, int ld_out, const float* lse2,
+                           float* delta, void* dqkv, int B, int S, int H, int Hkv, float scale) {
+  HOOK(attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv,
+                     scale, ctx_stream(ctx)));
+}
+int b200w_op_attention_fwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off, void* out,
+                                int ld_out, float* lse2, const int32_t* positions, int B, int S, int H, int Hkv,
+                                float scale) {
+  return guarded(ctx, [&] {
+    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
+      attention_fwd(qkv, ld_qkv, k_off, v_off, out, ld_out, lse2, B, S, H, Hkv, scale, ctx_stream(ctx), &db);
+      ++ctx_launches(ctx);
+    });
+  });
+}
+int b200w_op_attention_bwd_docs(b200w_ctx* ctx, const void* qkv, int ld_qkv, int k_off, int v_off,
+                                const void* out, const void* dout, int ld_out, const float* lse2, float* delta,
+                                void* dqkv, const int32_t* positions, int B, int S, int H, int Hkv, float scale) {
+  return guarded(ctx, [&] {
+    with_doc_bounds(ctx, positions, B, S, [&](const DocBounds& db) {
+      attention_bwd(qkv, ld_qkv, k_off, v_off, out, dout, ld_out, lse2, delta, dqkv, B, S, H, Hkv, scale,
+                    ctx_stream(ctx), &db);
+      ctx_launches(ctx) += 3;
+    });
+  });
+}
+int b200w_op_rope_positions(b200w_ctx* ctx, void* buf, int ld, int T, int S, int nheads, int dh, float theta,
+                            int inverse, const int32_t* positions) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(positions, "NULL positions");
+    auto tab = device_scratch<float2>(static_cast<size_t>(S) * (dh / 2));
+    rope_table(tab.get(), S, dh, theta, ctx_stream(ctx));
+    rope_apply(buf, ld, tab.get(), T, S, nheads, dh, inverse != 0, ctx_stream(ctx), 0, positions);
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_adamw(b200w_ctx* ctx, float* master, float* m, float* v, const void* g, int g_bf16,
+                   void* w_bf16, int64_t n, float lr, float beta1, float beta2, float eps, float wd,
+                   int step, float gscale) {
+  return guarded(ctx, [&] {
+    B200W_CUDA(cudaMemcpyAsync(ctx_scal(ctx), &gscale, sizeof(float), cudaMemcpyHostToDevice, ctx_stream(ctx)));
+    adamw_step(master, m, v, g, g_bf16 != 0, w_bf16, static_cast<size_t>(n), lr, beta1, beta2, eps, wd, step,
+               ctx_scal(ctx), ctx_stream(ctx));
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int b200w_op_poison_onchip(b200w_ctx* ctx, uint32_t pattern) {
+  return guarded(ctx, [&] {
+    static PerDeviceOnce once;
+    once.run([&] {
+      B200W_CUDA(cudaFuncSetAttribute(poison_onchip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, POISON_SMEM));
+    });
+    // one CTA per SM at a time (smem-limited); several waves so that every SM is visited
+    poison_onchip_kernel<<<sm_count() * 4, 128, POISON_SMEM, ctx_stream(ctx)>>>(pattern);
+    B200W_CUDA(cudaGetLastError());
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+
+int b200w_op_grad_norm(b200w_ctx* ctx, const void* g, int g_bf16, int64_t n, float* norm_out) {
+  return guarded(ctx, [&] {
+    auto ss = device_scratch<double>(1);
+    B200W_CUDA(cudaMemsetAsync(ss.get(), 0, sizeof(double), ctx_stream(ctx)));
+    grad_sumsq(g, g_bf16 != 0, static_cast<size_t>(n), ss.get(), ctx_stream(ctx));
+    ++ctx_launches(ctx);
+    double h = 0;
+    B200W_CUDA(cudaMemcpyAsync(&h, ss.get(), sizeof(double), cudaMemcpyDeviceToHost, ctx_stream(ctx)));
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+    if (norm_out) *norm_out = static_cast<float>(sqrt(h));
+  });
+}
+
+}  // extern "C"
