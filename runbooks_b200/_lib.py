@@ -38,7 +38,7 @@ class InferArch(C.Structure):
         ("intermediate_size", C.c_int32), ("num_layers", C.c_int32), ("num_heads", C.c_int32),
         ("num_kv_heads", C.c_int32), ("head_dim", C.c_int32), ("max_ctx", C.c_int32),
         ("norm_eps", C.c_float), ("rope_theta", C.c_float), ("tie_embeddings", C.c_int32),
-        ("max_positions", C.c_int32), ("reserved", C.c_int32 * 3),
+        ("max_positions", C.c_int32), ("weight_dtype", C.c_int32), ("reserved", C.c_int32 * 2),
     ]
 
 
@@ -106,9 +106,11 @@ PROTOTYPES = {
     "b200w_infer_param_info": (C.c_int, [c_ctx, C.c_int64, C.c_char_p, C.c_size_t, i64p, i64p]),
     "b200w_infer_load_tensor": (C.c_int, [c_ctx, C.c_char_p, vp, C.c_int, C.c_int64]),
     "b200w_infer_init_random": (C.c_int, [c_ctx, C.c_uint64, C.c_float]),
+    "b200w_infer_read_weight": (C.c_int, [c_ctx, C.c_char_p, vp, C.c_int64]),
     "b200w_infer_step": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, vp, vp]),
     "b200w_infer_prefill": (C.c_int, [c_ctx, vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "b200w_infer_device_bytes": (C.c_int64, [c_ctx]),
+    "b200w_infer_weight_bytes": (C.c_int64, [c_ctx]),
     "b200w_infer_init_paged": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int, C.c_int, C.c_int64]),
     "b200w_infer_init_paged_kv": (C.c_int, [c_ctx, C.POINTER(InferArch), C.c_int, C.c_int, C.c_int64, C.c_int]),
     "b200w_infer_kv_read": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
@@ -131,6 +133,10 @@ PROTOTYPES = {
     "b200w_op_gemm_wire": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
                                      C.c_int, C.c_int, C.c_int, vp]),
     "b200w_op_gemm_decode": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b200w_w4_image_bytes": (C.c_int64, [C.c_int, C.c_int]),
+    "b200w_op_quantize_w4": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
+    "b200w_op_dequantize_w4": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
+    "b200w_op_gemm_decode_w4": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_fwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_bwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int]),

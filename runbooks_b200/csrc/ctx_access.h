@@ -15,7 +15,8 @@ int64_t& ctx_launches(b200w_ctx* c);
 void* ctx_infer_slot(b200w_ctx* c);
 void ctx_set_infer(b200w_ctx* c, void* p, void (*destroy)(void*));
 // normal(0, std) / constant fill of a bf16 range with the engine's counter-based generator
-void ctx_fill_normal(b200w_ctx* c, void* w_bf16, size_t n, uint64_t seed, float std);
+// element j of w_bf16 gets the value of flat index i0 + j of the seeded fill
+void ctx_fill_normal(b200w_ctx* c, void* w_bf16, size_t n, uint64_t seed, float std, size_t i0 = 0);
 void ctx_fill_const(b200w_ctx* c, void* w_bf16, size_t n, float value);
 // 8 floats of device scratch for the per-kernel hooks, allocated from the context's memory at first use
 float* ctx_scal(b200w_ctx* c);

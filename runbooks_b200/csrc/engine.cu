@@ -1155,8 +1155,8 @@ void ctx_set_infer(b200w_ctx* c, void* p, void (*destroy)(void*)) {
   c->infer = p;
   c->infer_destroy = destroy;
 }
-void ctx_fill_normal(b200w_ctx* c, void* w_bf16, size_t n, uint64_t seed, float std) {
-  init_normal_kernel<<<sm_count() * 8, 256, 0, c->stream>>>(nullptr, static_cast<bf16*>(w_bf16), n, seed, std);
+void ctx_fill_normal(b200w_ctx* c, void* w_bf16, size_t n, uint64_t seed, float std, size_t i0) {
+  init_normal_kernel<<<sm_count() * 8, 256, 0, c->stream>>>(nullptr, static_cast<bf16*>(w_bf16), n, seed, std, i0);
   B200W_CUDA(cudaGetLastError());
 }
 void ctx_fill_const(b200w_ctx* c, void* w_bf16, size_t n, float value) {

@@ -34,6 +34,7 @@
 #include "kv_cache.h"
 #include "ops.h"
 #include "ptx.cuh"
+#include "w4.h"
 
 using namespace b200w;
 using bf16 = __nv_bfloat16;
@@ -200,9 +201,19 @@ __global__ void argmax_kernel(const bf16* __restrict__ logits, int V, int32_t* _
 struct IParam {
   std::string name;
   int64_t rows, cols;
-  size_t off;   // element offset of (0, 0)
+  size_t off;   // element offset of (0, 0) in the flat space of the bf16 engine (also what init_random's fill is keyed by)
   int64_t ld;   // row stride on the device (== cols unless the matrix is a column window of a fused one)
-  char kind;    // 'm' matrix, 'n' norm weight (ones), 'b' bias (zeros)
+  char kind;    // 'p' projection, 'm' other matrix (embedding, positions, lm_head), 'n' norm weight (ones), 'b' bias (zeros)
+  size_t dev = 0;   // element offset in Infer::w (== off, except for int4 weights, where projections are not there)
+  int img = -1;     // int4 weights: the projection's image in Infer::imgs
+};
+
+// An int4 image (w4.h) of one fused projection matrix [N, K]: the matrix the decode GEMM reads in one launch. off: its
+// (0, 0) in the bf16 engine's flat space, which the matrix fills contiguously with row stride K.
+struct W4Image {
+  size_t off;
+  int N, K;
+  uint8_t* p;
 };
 
 struct Infer {
@@ -213,12 +224,21 @@ struct Infer {
   bool grouped = false; // the step being enqueued has rows of one slot at consecutive positions (decode_attention)
   std::vector<IParam> params;
   std::unordered_map<std::string, int> index;
-  size_t n_elems = 0;
+  size_t n_elems = 0;   // the bf16 engine's flat space
   DeviceMemory mem;   // the device buffers below, the KV cache's included (b200w_infer_device_bytes)
+  // int4 weights (B200W_WEIGHTS_INT4_G64): the projections live in imgs, w holds only the other parameters, and one
+  // bf16 scratch of the largest image's N * K elements serves the prefill's dequantized W_hat and the loads
+  bool w4 = false;
+  std::vector<W4Image> imgs;
+  bf16* w4_scratch = nullptr;
+  int* w4_bad = nullptr;   // set by the quantizer when a weight is not finite
+  size_t weight_bytes = 0; // w and the images (b200w_infer_weight_bytes)
   bf16* w = nullptr;
   // per layer: norm parameters, the projections (offsets of their (0,0) element), biases (OPT), and the decode-time
   // copy of each projection as consecutive 16 KB swizzled tile images (gemm.cu retile_weights): a decode GEMM CTA
-  // streams one contiguous HBM region instead of 128-byte row segments (null until ensure_tiled makes them)
+  // streams one contiguous HBM region instead of 128-byte row segments (null until ensure_tiled makes them). With int4
+  // weights the t_* are the layer's int4 images instead (Falcon: t_qkv holds [q k v | dense_h_to_4h], t_o
+  // [dense | dense_4h_to_h]), and the ln / bias offsets are into the compacted w.
   struct L {
     size_t ln1_w, ln1_b, ln2_w, ln2_b, wqkv, bqkv, wo, bo, w1, b1, w2, b2;
     uint8_t *t_qkv, *t_o, *t_w1, *t_w2;
@@ -306,13 +326,13 @@ void build(Infer* m) {
       x.ln1_w = add_dense(m, p + "input_layernorm.weight", 1, d, 'n');
       x.ln1_b = add_dense(m, p + "input_layernorm.bias", 1, d, 'b');
       // [q k v | dense_h_to_4h]: adjacent rows of ONE [qkvd + f, d] matrix (both consume the LayerNorm output)
-      x.wqkv = add_dense(m, p + "self_attention.query_key_value.weight", qd + 2 * kd, d);
-      x.w1 = add_dense(m, p + "mlp.dense_h_to_4h.weight", f, d);
+      x.wqkv = add_dense(m, p + "self_attention.query_key_value.weight", qd + 2 * kd, d, 'p');
+      x.w1 = add_dense(m, p + "mlp.dense_h_to_4h.weight", f, d, 'p');
       // [dense | dense_4h_to_h]: column windows of ONE [d, qd + f] matrix (their outputs are summed)
       x.wo = m->n_elems;
-      add(m, p + "self_attention.dense.weight", d, qd, x.wo, m->ld_cat, 'm');
+      add(m, p + "self_attention.dense.weight", d, qd, x.wo, m->ld_cat, 'p');
       x.w2 = x.wo + qd;
-      add(m, p + "mlp.dense_4h_to_h.weight", d, f, x.w2, m->ld_cat, 'm');
+      add(m, p + "mlp.dense_4h_to_h.weight", d, f, x.w2, m->ld_cat, 'p');
       m->n_elems += static_cast<size_t>(d) * m->ld_cat;
     }
     m->p_lnf_w = add_dense(m, "transformer.ln_f.weight", 1, d, 'n');
@@ -327,19 +347,19 @@ void build(Infer* m) {
       auto& x = m->lp[l];
       x.ln1_w = add_dense(m, p + "self_attn_layer_norm.weight", 1, d, 'n');
       x.ln1_b = add_dense(m, p + "self_attn_layer_norm.bias", 1, d, 'b');
-      x.wqkv = add_dense(m, p + "self_attn.q_proj.weight", qd, d);
-      add_dense(m, p + "self_attn.k_proj.weight", kd, d);
-      add_dense(m, p + "self_attn.v_proj.weight", kd, d);
+      x.wqkv = add_dense(m, p + "self_attn.q_proj.weight", qd, d, 'p');
+      add_dense(m, p + "self_attn.k_proj.weight", kd, d, 'p');
+      add_dense(m, p + "self_attn.v_proj.weight", kd, d, 'p');
       x.bqkv = add_dense(m, p + "self_attn.q_proj.bias", 1, qd, 'b');
       add_dense(m, p + "self_attn.k_proj.bias", 1, kd, 'b');
       add_dense(m, p + "self_attn.v_proj.bias", 1, kd, 'b');
-      x.wo = add_dense(m, p + "self_attn.out_proj.weight", d, qd);
+      x.wo = add_dense(m, p + "self_attn.out_proj.weight", d, qd, 'p');
       x.bo = add_dense(m, p + "self_attn.out_proj.bias", 1, d, 'b');
       x.ln2_w = add_dense(m, p + "final_layer_norm.weight", 1, d, 'n');
       x.ln2_b = add_dense(m, p + "final_layer_norm.bias", 1, d, 'b');
-      x.w1 = add_dense(m, p + "fc1.weight", f, d);
+      x.w1 = add_dense(m, p + "fc1.weight", f, d, 'p');
       x.b1 = add_dense(m, p + "fc1.bias", 1, f, 'b');
-      x.w2 = add_dense(m, p + "fc2.weight", d, f);
+      x.w2 = add_dense(m, p + "fc2.weight", d, f, 'p');
       x.b2 = add_dense(m, p + "fc2.bias", 1, d, 'b');
     }
     m->p_lnf_w = add_dense(m, dec + "final_layer_norm.weight", 1, d, 'n');
@@ -352,18 +372,68 @@ void build(Infer* m) {
       auto& x = m->lp[l];
       x.ln1_w = add_dense(m, p + "input_layernorm.weight", 1, d, 'n');
       x.ln2_w = add_dense(m, p + "post_attention_layernorm.weight", 1, d, 'n');
-      x.wqkv = add_dense(m, p + "self_attn.q_proj.weight", qd, d);
-      add_dense(m, p + "self_attn.k_proj.weight", kd, d);
-      add_dense(m, p + "self_attn.v_proj.weight", kd, d);
-      x.wo = add_dense(m, p + "self_attn.o_proj.weight", d, qd);
-      x.w1 = add_dense(m, p + "mlp.gate_proj.weight", f, d);
-      add_dense(m, p + "mlp.up_proj.weight", f, d);
-      x.w2 = add_dense(m, p + "mlp.down_proj.weight", d, f);
+      x.wqkv = add_dense(m, p + "self_attn.q_proj.weight", qd, d, 'p');
+      add_dense(m, p + "self_attn.k_proj.weight", kd, d, 'p');
+      add_dense(m, p + "self_attn.v_proj.weight", kd, d, 'p');
+      x.wo = add_dense(m, p + "self_attn.o_proj.weight", d, qd, 'p');
+      x.w1 = add_dense(m, p + "mlp.gate_proj.weight", f, d, 'p');
+      add_dense(m, p + "mlp.up_proj.weight", f, d, 'p');
+      x.w2 = add_dense(m, p + "mlp.down_proj.weight", d, f, 'p');
     }
     m->p_lnf_w = add_dense(m, "model.norm.weight", 1, d, 'n');
   }
   if (a.tie_embeddings) m->p_lm = m->p_embed;
   else m->p_lm = add_dense(m, "lm_head.weight", a.vocab_size, d);
+  for (IParam& p : m->params) p.dev = p.off;
+}
+
+// Int4 weights: one image per matrix a decode GEMM reads (ensure_tiled's list, lm_head excepted) in the layer's t_*,
+// every projection tied to its image, the other parameters packed into w in their order (so OPT's q / k / v biases
+// stay adjacent) and the offsets kept in Infer remapped to w. -> the elements w needs.
+size_t layout_w4(Infer* m, cudaStream_t s) {
+  const auto& a = m->a;
+  const int d = a.hidden_size, f = a.intermediate_size, qd = m->qd, qkvd = m->qkvd;
+  auto image = [&](uint8_t*& t, size_t off, int N, int K) {
+    t = m->mem.alloc<uint8_t>(w4_image_bytes(N, K));
+    w4_clear(t, N, K, s);   // (every later use of the images is on the same stream)
+    m->imgs.push_back({off, N, K, t});
+  };
+  for (auto& x : m->lp) {
+    if (a.family == B200W_FAMILY_FALCON) {
+      image(x.t_qkv, x.wqkv, qkvd + f, d);
+      image(x.t_o, x.wo, d, m->ld_cat);
+    } else {
+      image(x.t_qkv, x.wqkv, qkvd, d);
+      image(x.t_o, x.wo, d, qd);
+      image(x.t_w1, x.w1, a.family == B200W_FAMILY_LLAMA ? 2 * f : f, d);
+      image(x.t_w2, x.w2, d, f);
+    }
+  }
+  size_t n = 0;
+  std::unordered_map<size_t, size_t> moved;
+  for (IParam& p : m->params) {
+    if (p.kind == 'p') {
+      for (size_t i = 0; i < m->imgs.size(); ++i) {
+        const W4Image& g = m->imgs[i];
+        if (p.off >= g.off && p.off < g.off + static_cast<size_t>(g.N) * g.K) p.img = static_cast<int>(i);
+      }
+      continue;
+    }
+    if (!moved.count(p.off)) {
+      moved[p.off] = n;
+      n += static_cast<size_t>(p.rows) * p.cols;
+    }
+    p.dev = moved[p.off];
+  }
+  auto remap = [&](size_t& o) { auto it = moved.find(o); if (it != moved.end()) o = it->second; };
+  for (auto& x : m->lp)
+    for (size_t* o : {&x.ln1_w, &x.ln1_b, &x.ln2_w, &x.ln2_b, &x.bqkv, &x.bo, &x.b1, &x.b2}) remap(*o);
+  for (size_t* o : {&m->p_embed, &m->p_pos, &m->p_lnf_w, &m->p_lnf_b, &m->p_lm}) remap(*o);
+  size_t scratch = 0;
+  for (const W4Image& g : m->imgs) scratch = std::max(scratch, static_cast<size_t>(g.N) * g.K);
+  m->w4_scratch = m->mem.alloc<bf16>(scratch);
+  m->w4_bad = m->mem.alloc<int>(1);
+  return n;
 }
 
 // guarded, for the serving calls: only the call right after a step or a prefill may sample from the logits it left
@@ -384,10 +454,12 @@ Infer* model(b200w_ctx* ctx) {
 
 void infer_destroy(void* p) { delete static_cast<Infer*>(p); }
 
-// one decode GEMM: out[n, N] = act(X W^T (+ bias) (+ C))
+// one decode GEMM: out[n, N] = act(X W^T (+ bias) (+ C)); tiled: W's tile-major copy or, for a projection of an
+// int4 engine, its image (read whatever B200W_DECODE_TILED says)
 void dgemm(Infer* m, cudaStream_t s, int n, const bf16* X, int ldx, size_t woff, int ldw, int N, int K,
-           GemmDecodeOut o, const uint8_t* tiled = nullptr) {
-  o.w_tiled = m->use_tiled ? tiled : nullptr;
+           GemmDecodeOut o, const uint8_t* tiled, bool projection) {
+  if (projection && m->w4) o.w4 = tiled;
+  else o.w_tiled = m->use_tiled ? tiled : nullptr;
   gemm_decode_ex(X, ldx, m->w + woff, ldw, o, m->ws, m->counters, n, N, K, s);
 }
 
@@ -401,7 +473,7 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
     if (!dst) dst = m->mem.alloc<uint8_t>(retiled_bytes(N, K));
     retile_weights(m->w + woff, ldw, dst, N, K, s);
   };
-  for (int l = 0; l < a.num_layers; ++l) {
+  for (int l = 0; l < a.num_layers && !m->w4; ++l) {   // (an int4 engine's projections are images already)
     auto& p = m->lp[l];
     if (falcon) {
       make(p.t_qkv, p.wqkv, d, qkvd + f, d);               // [q k v | dense_h_to_4h]
@@ -439,16 +511,31 @@ void launch(Pass& p, void (*kern)(KArgs...), dim3 grid, dim3 block, Args&&... ar
   else kern<<<grid, block, 0, p.s>>>(std::forward<Args>(args)...);
 }
 
-// out [rows, N] (row stride ldo) = act(X W^T + bias) (+ C, same stride); tiled: the step's tile-major copy of W
+// The int4 image of the projection whose tile-major pointer is `t`.
+const W4Image& image_of(const Infer* m, const uint8_t* t) {
+  for (const W4Image& g : m->imgs)
+    if (g.p == t) return g;
+  throw Error("no int4 image for a projection");
+}
+
+// out [rows, N] (row stride ldo) = act(X W^T + bias) (+ C, same stride); tiled: the step's tile-major copy of W, or
+// with int4 weights W's image, of which W is rows [img_row0, img_row0 + N). The prefill of an int4 engine first
+// writes W_hat (row stride ldw) into the scratch and runs the same GEMM on it.
 void gemm(Pass& p, const bf16* X, int ldx, size_t w, int ldw, int N, int K, bf16* out, int ldo, const uint8_t* tiled,
-          const bf16* C = nullptr, const bf16* bias = nullptr, Act act = Act::none) {
+          const bf16* C = nullptr, const bf16* bias = nullptr, Act act = Act::none, int img_row0 = 0) {
   if (p.decode) {
     GemmDecodeOut o;
     o.out = out; o.ldo = ldo; o.bias = bias; o.act = act == Act::relu ? 2 : 0;
     if (C) { o.C = C; o.ldc = ldo; }
-    dgemm(p.m, p.s, p.rows, X, ldx, w, ldw, N, K, o, tiled);
+    dgemm(p.m, p.s, p.rows, X, ldx, w, ldw, N, K, o, tiled, true);
   } else {
-    gemm_bf16_ex(X, false, ldx, p.m->w + w, false, ldw, out, C, false, ldo, p.rows, N, K, 0, bias,
+    const bf16* W = p.m->w + w;
+    if (p.m->w4) {
+      const W4Image& g = image_of(p.m, tiled);
+      w4_dequantize(g.p, g.N, g.K, img_row0, N, p.m->w4_scratch, ldw, p.s); ++p.nl;
+      W = p.m->w4_scratch;
+    }
+    gemm_bf16_ex(X, false, ldx, W, false, ldw, out, C, false, ldo, p.rows, N, K, 0, bias,
                  act == Act::relu ? 1 : 0, p.s);
   }
   ++p.nl;
@@ -535,10 +622,10 @@ void layer_falcon(Pass& p, int l) {
     o.out = p.qkv; o.ldo = qkvd;
     o.out2 = p.cat + qd; o.ldo2 = ldc; o.n_split = qkvd;
     o.act = 1; o.act_from = qkvd;
-    dgemm(p.m, p.s, p.rows, p.nrm, d, w.wqkv, d, qkvd + f, d, o, w.t_qkv); ++p.nl;
+    dgemm(p.m, p.s, p.rows, p.nrm, d, w.wqkv, d, qkvd + f, d, o, w.t_qkv, true); ++p.nl;
   } else {
-    gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, nullptr);
-    gemm(p, p.nrm, d, w.w1, d, f, d, p.cat + qd, ldc, nullptr);
+    gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, w.t_qkv);
+    gemm(p, p.nrm, d, w.w1, d, f, d, p.cat + qd, ldc, w.t_qkv, nullptr, nullptr, Act::none, qkvd);
     const long long ge = static_cast<long long>(p.rows) * (f / 8);
     gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, p.s>>>(p.cat + qd, p.rows, f, ldc); ++p.nl;
   }
@@ -560,7 +647,7 @@ void head(Pass& p, const bf16* x, int n) {
   norm(p, n, x, m->p_lnf_w, m->p_lnf_b, m->nrm);
   GemmDecodeOut o;
   o.out = m->logits; o.ldo = V;
-  dgemm(m, p.s, n, m->nrm, d, m->p_lm, d, V, d, o, p.decode ? m->t_lm : nullptr); ++p.nl;
+  dgemm(m, p.s, n, m->nrm, d, m->p_lm, d, V, d, o, p.decode ? m->t_lm : nullptr, false); ++p.nl;
   launch(p, argmax_kernel, dim3(n), dim3(1024), m->logits, V, m->next); ++p.nl;
   B200W_CUDA(cudaGetLastError());
   B200W_CUDA(cudaMemcpyAsync(m->pin_next, m->next, n * 4, cudaMemcpyDeviceToHost, p.s));
@@ -862,6 +949,12 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
               "sizes must be multiples of 8");
   B200W_CHECK(arch->hidden_size <= 256 * 8 * LN_MAXP, "hidden_size too large for the decode LayerNorm");
   B200W_CHECK(arch->max_ctx >= 1 && arch->max_ctx <= 8192, "max_ctx must be in 1..8192");
+  B200W_CHECK(arch->weight_dtype == B200W_WEIGHTS_BF16 || arch->weight_dtype == B200W_WEIGHTS_INT4_G64,
+              "unknown weight dtype");
+  if (arch->weight_dtype == B200W_WEIGHTS_INT4_G64)
+    B200W_CHECK(arch->hidden_size % W4_GROUP == 0 && arch->intermediate_size % W4_GROUP == 0 &&
+                    (arch->num_heads * arch->head_dim) % W4_GROUP == 0,
+                "int4 weights: every K of a projection (hidden, intermediate, heads * head_dim) must be a multiple of 64");
   if (arch->family == B200W_FAMILY_OPT)
     B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
   const int64_t ctx_rounded = cdiv(arch->max_ctx, KV_PAGE) * static_cast<int64_t>(KV_PAGE);
@@ -879,7 +972,11 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   build(m.get());
   const auto& a = m->a;
   const size_t B = max_batch;
-  m->w = m->mem.alloc<bf16>(m->n_elems);
+  m->w4 = a.weight_dtype == B200W_WEIGHTS_INT4_G64;
+  const size_t w_elems = m->w4 ? layout_w4(m.get(), ctx_stream(ctx)) : m->n_elems;
+  m->w = m->mem.alloc<bf16>(w_elems);
+  m->weight_bytes = w_elems * sizeof(bf16);
+  for (const W4Image& g : m->imgs) m->weight_bytes += w4_image_bytes(g.N, g.K);
   m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim, m->mem);
   if (m->kv.paged) {
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
@@ -1045,18 +1142,37 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     cudaStream_t s = ctx_stream(ctx);
     const size_t n = static_cast<size_t>(n_elements);
     m->tiled_valid = false;
-    bf16* dst = m->w + p.off;
+    bf16* dst = m->w + p.dev;
     DeviceScratch<float> tmp32;
     DeviceScratch<bf16> tmp16;
-    const void* src16 = host;                 // dense bf16 source (host or device)
+    // the dense bf16 source: the host buffer, or the f32 values cast on the device -- for an int4 projection straight
+    // into the scratch it is quantized from
+    const void* src16 = host;
     cudaMemcpyKind kind = cudaMemcpyHostToDevice;
     if (dtype == B200W_F32) {
       tmp32 = device_scratch<float>(n);
-      tmp16 = device_scratch<bf16>(n);
+      if (p.img < 0) tmp16 = device_scratch<bf16>(n);
+      bf16* cast = p.img >= 0 ? m->w4_scratch : tmp16.get();
       B200W_CUDA(cudaMemcpyAsync(tmp32.get(), host, n * 4, cudaMemcpyHostToDevice, s));
-      cast_f32_to_bf16(tmp32.get(), tmp16.get(), n, s);
-      src16 = tmp16.get();
+      cast_f32_to_bf16(tmp32.get(), cast, n, s);
+      src16 = cast;
       kind = cudaMemcpyDeviceToDevice;
+    }
+    if (p.img >= 0) {
+      // an int4 projection: the bf16 values through the scratch, quantized into the image rows and columns it owns
+      const W4Image& g = m->imgs[p.img];
+      const size_t rel = p.off - g.off;
+      if (dtype == B200W_BF16)
+        B200W_CUDA(cudaMemcpyAsync(m->w4_scratch, host, n * sizeof(bf16), cudaMemcpyHostToDevice, s));
+      B200W_CUDA(cudaMemsetAsync(m->w4_bad, 0, sizeof(int), s));
+      w4_quantize(m->w4_scratch, static_cast<int>(p.cols), static_cast<int>(p.rows),
+                  static_cast<int>(p.cols), g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(rel % g.K),
+                  m->w4_bad, s);
+      int bad = 0;
+      B200W_CUDA(cudaMemcpyAsync(&bad, m->w4_bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+      B200W_CUDA(cudaStreamSynchronize(s));
+      if (bad) throw InvalidArgument(std::string("check failed: non-finite value in int4 weight ") + name);
+      return;
     }
     // rows of `cols` elements into rows of stride ld (ld == cols: one contiguous copy)
     B200W_CUDA(cudaMemcpy2DAsync(dst, p.ld * sizeof(bf16), src16, p.cols * sizeof(bf16), p.cols * sizeof(bf16),
@@ -1065,16 +1181,53 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
   });
 }
 
+int b200w_infer_read_weight(b200w_ctx* ctx, const char* name, void* host_bf16, int64_t n_elements) {
+  return iguard(ctx, [&] {
+    Infer* m = model(ctx);
+    B200W_CHECK(name && host_bf16, "NULL name / buffer");
+    auto it = m->index.find(name);
+    if (it == m->index.end()) throw InvalidArgument(std::string("check failed: unknown parameter ") + name);
+    const IParam& p = m->params[it->second];
+    B200W_CHECK(n_elements == p.rows * p.cols, "element count does not match the parameter shape");
+    cudaStream_t s = ctx_stream(ctx);
+    const bf16* src = m->w + p.dev;
+    int64_t ld = p.ld;
+    if (p.img >= 0) {   // W_hat: the image rows the projection owns, dequantized whole, then its columns
+      const W4Image& g = m->imgs[p.img];
+      const size_t rel = p.off - g.off;
+      w4_dequantize(g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(p.rows), m->w4_scratch, g.K, s);
+      src = m->w4_scratch + rel % g.K;
+      ld = g.K;
+    }
+    B200W_CUDA(cudaMemcpy2DAsync(host_bf16, p.cols * sizeof(bf16), src, ld * sizeof(bf16), p.cols * sizeof(bf16),
+                                 p.rows, cudaMemcpyDeviceToHost, s));
+    B200W_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
 int b200w_infer_init_random(b200w_ctx* ctx, uint64_t seed, float std) {
   return iguard(ctx, [&] {
     Infer* m = model(ctx);
     check_weights_unshared(m);
-    // one device-side fill of the whole flat space (the fused matrices included), then the 1-D parameters
+    // one device-side fill of the whole flat space (the fused matrices included), then the 1-D parameters. With int4
+    // weights every image and every other matrix gets the values of its own range of that fill, an image through
+    // the scratch and the quantizer: quantize(W) of the bf16 engine's W for the same seed.
     m->tiled_valid = false;
-    ctx_fill_normal(ctx, m->w, m->n_elems, seed, std);
+    cudaStream_t s = ctx_stream(ctx);
+    if (!m->w4) {
+      ctx_fill_normal(ctx, m->w, m->n_elems, seed, std);
+    } else {
+      for (const W4Image& g : m->imgs) {
+        ctx_fill_normal(ctx, m->w4_scratch, static_cast<size_t>(g.N) * g.K, seed, std, g.off);
+        w4_quantize(m->w4_scratch, g.K, g.N, g.K, g.p, g.N, g.K, 0, 0, m->w4_bad, s);
+      }
+      for (const IParam& p : m->params)
+        if (p.kind == 'm') ctx_fill_normal(ctx, m->w + p.dev, static_cast<size_t>(p.rows * p.cols), seed, std, p.off);
+    }
     for (const IParam& p : m->params)
-      if (p.kind != 'm') ctx_fill_const(ctx, m->w + p.off, static_cast<size_t>(p.rows * p.cols), p.kind == 'n' ? 1.f : 0.f);
-    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+      if (p.kind == 'n' || p.kind == 'b')
+        ctx_fill_const(ctx, m->w + p.dev, static_cast<size_t>(p.rows * p.cols), p.kind == 'n' ? 1.f : 0.f);
+    B200W_CUDA(cudaStreamSynchronize(s));
   });
 }
 
@@ -1259,6 +1412,11 @@ int b200w_infer_sample(b200w_ctx* ctx, int n, const b200w_sampling* sp, int32_t*
 int b200w_infer_sample_penalized(b200w_ctx* ctx, int n, const b200w_sampling* sp, const b200w_penalties* pen,
                                  int32_t* tokens_out, float* token_logit_out) {
   return sample_impl(ctx, n, sp, pen, tokens_out, token_logit_out);
+}
+
+int64_t b200w_infer_weight_bytes(b200w_ctx* ctx) {
+  Infer* m = ctx ? static_cast<Infer*>(ctx_infer_slot(ctx)) : nullptr;
+  return m ? static_cast<int64_t>(m->weight_bytes) : 0;
 }
 
 int64_t b200w_infer_device_bytes(b200w_ctx* ctx) {

@@ -9,6 +9,7 @@
 #include "ctx_access.h"
 #include "host_common.h"
 #include "ops.h"
+#include "w4.h"
 
 using namespace b200w;
 
@@ -81,6 +82,45 @@ int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out
     gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx_stream(ctx));
     gemm_decode(X, W, out, C, ws.get(), cnt.get(), M, N, K, N, 0, ctx_stream(ctx));
     ctx_launches(ctx) += 2;
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
+int64_t b200w_w4_image_bytes(int N, int K) {
+  if (N <= 0 || K <= 0 || K % W4_GROUP) return -1;
+  return static_cast<int64_t>(w4_image_bytes(N, K));
+}
+int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int K) {
+  return guarded(ctx, [&] {
+    auto bad = device_scratch<int>(1);
+    B200W_CUDA(cudaMemsetAsync(bad.get(), 0, sizeof(int), ctx_stream(ctx)));
+    w4_clear(static_cast<uint8_t*>(image), N, K, ctx_stream(ctx));
+    w4_quantize(W, K, N, K, static_cast<uint8_t*>(image), N, K, 0, 0, bad.get(), ctx_stream(ctx));
+    ctx_launches(ctx) += 2;
+    int h = 0;
+    B200W_CUDA(cudaMemcpyAsync(&h, bad.get(), sizeof(int), cudaMemcpyDeviceToHost, ctx_stream(ctx)));
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+    B200W_CHECK(h == 0, "non-finite weight");
+  });
+}
+int b200w_op_dequantize_w4(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K) {
+  HOOK(w4_dequantize(static_cast<const uint8_t*>(image), N, K, 0, N, W_hat, K, ctx_stream(ctx)));
+}
+int b200w_op_gemm_decode_w4(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M, int N,
+                            int K, int split_k) {
+  return guarded(ctx, [&] {
+    DeviceScratch<float> ws;
+    DeviceScratch<unsigned> cnt;
+    if (split_k) {   // (gemm_decode_ex splits K when both are given; it reads neither)
+      ws = device_scratch<float>(1);
+      cnt = device_scratch<unsigned>(1);
+    }
+    GemmDecodeOut o{};
+    o.out = out;
+    o.ldo = N;
+    o.C = C;
+    o.w4 = image;
+    gemm_decode_ex(X, K, nullptr, K, o, ws.get(), cnt.get(), M, N, K, ctx_stream(ctx));
+    ++ctx_launches(ctx);
     B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
   });
 }

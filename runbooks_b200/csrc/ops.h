@@ -50,6 +50,7 @@ struct GemmDecodeOut {
   int act = 0;
   int act_from = 0;
   const void* w_tiled = nullptr;  // retile_weights() image of W: streamed with 16 KB bulk copies instead of TMA boxes
+  const void* w4 = nullptr;       // int4 image of W (w4.h): W and w_tiled are not read
 };
 // W [N, K] (row stride ldw) as consecutive 16 KB swizzled shared-memory images of its [128 x 64] tiles
 // (gemm.cu retile_weights_kernel); retiled_bytes = the size of that image.

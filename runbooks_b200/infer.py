@@ -77,6 +77,7 @@ KV_PAGE = 128   # positions per page of the paged KV cache (one key block of the
 
 
 KV_DTYPES = {"bf16": 0, "fp8": 1}   # b200w_kv_dtype: bf16, or e4m3 with one fp32 scale per (position, kv head)
+WEIGHT_DTYPES = {"bf16": 0, "int4": 1}   # B200W_WEIGHTS_*: int4 = group-quantized projections (DESIGN §3.5)
 
 
 def kv_page_bytes(arch: ServeArch, kv_dtype: str = "bf16") -> int:
@@ -102,21 +103,28 @@ class InferEngine(Engine):
     kv_dtype: str = "bf16"
 
     def init_infer(self, arch: ServeArch, max_batch: int = 32, kv_pages: Optional[int] = None,
-                   prefill_tokens: Optional[int] = None, kv_dtype: str = "bf16", max_rows: Optional[int] = None):
+                   prefill_tokens: Optional[int] = None, kv_dtype: str = "bf16", max_rows: Optional[int] = None,
+                   weight_dtype: str = "bf16"):
         """kv_pages: serve from a pool of that many 128-position pages shared by all slots (b200w_infer_init_paged)
         instead of reserving max_ctx positions per slot; arch.max_ctx is then the longest single request.
         prefill_tokens: the most tokens (n_seqs * padded length) one prefill call takes in paged mode.
         kv_dtype: "bf16", or "fp8" (paged only): K/V stored as e4m3 with per-(position, kv head) scales, about half
         the bytes per page (DESIGN §3.5).
         max_rows (max_batch..128; None: max_batch): rows one step may hold, for steps that verify drafted tokens
-        (b200w_infer_set_step_rows)."""
+        (b200w_infer_set_step_rows).
+        weight_dtype: "bf16", or "int4": every projection stored as int4 with one bf16 scale per row and 64 input
+        columns, about a quarter of the bytes; the engine computes exactly what the bf16 engine does on the
+        dequantized weights (read_weight)."""
+        if weight_dtype not in WEIGHT_DTYPES:
+            raise ValueError(f"weight_dtype must be one of {sorted(WEIGHT_DTYPES)}, got {weight_dtype!r}")
         if kv_dtype not in KV_DTYPES:
             raise ValueError(f"kv_dtype must be one of {sorted(KV_DTYPES)}, got {kv_dtype!r}")
         if kv_dtype != "bf16" and kv_pages is None:
             raise ValueError("an fp8 KV cache must be paged (kv_pages)")
         ca = _CArch(FAMILY[arch.family], arch.vocab_size, arch.hidden_size, arch.intermediate_size,
                     arch.num_layers, arch.num_heads, arch.num_kv_heads, arch.head_dim, arch.max_ctx,
-                    arch.norm_eps, arch.rope_theta, 1 if arch.tie_embeddings else 0, arch.max_positions)
+                    arch.norm_eps, arch.rope_theta, 1 if arch.tie_embeddings else 0, arch.max_positions,
+                    WEIGHT_DTYPES[weight_dtype])
         if kv_pages is None:
             self._check(self._lib.b200w_infer_init(self._h, C.byref(ca), max_batch))
         else:
@@ -127,7 +135,7 @@ class InferEngine(Engine):
             self.kv_pages, self.prefill_tokens = kv_pages, prefill_tokens
         if max_rows is not None:
             self._check(self._lib.b200w_infer_set_step_rows(self._h, max_rows))
-        self.serve_arch, self.max_batch, self.kv_dtype = arch, max_batch, kv_dtype
+        self.serve_arch, self.max_batch, self.kv_dtype, self.weight_dtype = arch, max_batch, kv_dtype, weight_dtype
         self.max_rows = max_batch if max_rows is None else max_rows
 
     def kv_read(self, layer: int, slot: int, pos0: int, n: int):
@@ -201,6 +209,18 @@ class InferEngine(Engine):
 
     def infer_init_random(self, seed: int = 0, std: float = 0.02):
         self._check(self._lib.b200w_infer_init_random(self._h, seed, std))
+
+    def weight_bytes(self) -> int:
+        """Device bytes the weights are stored in (b200w_infer_weight_bytes): the bf16 parameters and, with int4
+        weights, the projections' images."""
+        return self._lib.b200w_infer_weight_bytes(self._h)
+
+    def read_weight(self, name: str, shape) -> np.ndarray:
+        """The values the engine computes with for parameter `name` as bf16 bit patterns (uint16 of `shape`): the
+        dequantized weights for a projection of an int4 engine, the loaded ones otherwise."""
+        out = np.empty(shape, dtype=np.uint16)
+        self._check(self._lib.b200w_infer_read_weight(self._h, name.encode(), out.ctypes.data, out.size))
+        return out
 
     def _outputs(self, n: int, want_logits: bool):
         """The next tokens [n] and, with want_logits, fp32 logits [n, V] a step or prefill call writes."""

@@ -546,12 +546,26 @@ def _bool_param(content: str, key: str, cli: bool | None, environ) -> bool:
     if cli is not None:
         return bool(cli)
     extra = contract.load_params(os.path.join(content, "params.json"), environ).extra
-    v = extra.get(key, False)
+    return _as_bool(f"param {key!r}", extra.get(key, False))
+
+
+def _as_bool(what: str, v) -> bool:
+    """true / false, 1 / 0, yes / no (any case, as a bool, a number or a string); anything else is a ValueError"""
     if isinstance(v, bool) or v in (0, 1):
         return bool(v)
     if isinstance(v, str) and v.strip().lower() in ("true", "1", "yes", "false", "0", "no"):
         return v.strip().lower() in ("true", "1", "yes")
-    raise ValueError(f"param {key!r}: cannot read {v!r} as a boolean")
+    raise ValueError(f"{what}: cannot read {v!r} as a boolean")
+
+
+def load_in_4bit_param(load_in_4bit: bool | None = None, environ=None) -> bool:
+    """Whether the Server stores its projections as int4 (weight_dtype "int4"): --load-in-4bit, else the environment's
+    MODEL_LOAD_IN_4BIT (true / false, 1 / 0, yes / no; anything else is an error), else off. MODEL_LOAD_IN_8BIT is
+    not read: 8-bit weights are not built."""
+    if load_in_4bit is not None:
+        return bool(load_in_4bit)
+    environ = os.environ if environ is None else environ
+    return _as_bool("MODEL_LOAD_IN_4BIT", environ.get("MODEL_LOAD_IN_4BIT", False))
 
 
 def speculative_tokens_param(content: str, speculative_tokens: int | None = None, environ=None) -> int:
@@ -614,8 +628,9 @@ def kv_pages_for_gb(arch, kv_cache_gb: float, kv_dtype: str = "bf16") -> int:
 
 
 def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None,
-                kv_dtype: str = "bf16", speculative_tokens: int = 0):
-    """speculative_tokens > 0: a step holds up to min(128, max_batch * (1 + speculative_tokens)) rows."""
+                kv_dtype: str = "bf16", speculative_tokens: int = 0, load_in_4bit: bool | None = None):
+    """speculative_tokens > 0: a step holds up to min(128, max_batch * (1 + speculative_tokens)) rows.
+    load_in_4bit: int4 projections (None: MODEL_LOAD_IN_4BIT, load_in_4bit_param)."""
     from .infer import InferEngine, ServeArch
 
     cfg = contract.read_hf_config(model_dir)
@@ -623,7 +638,8 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
     kv_pages = None if kv_cache_gb is None else kv_pages_for_gb(arch, kv_cache_gb, kv_dtype)
     e = InferEngine(int(os.environ.get("B200W_DEVICE", "0")))
     e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages, kv_dtype=kv_dtype,
-                 max_rows=min(128, max_batch * (1 + speculative_tokens)) if speculative_tokens else None)
+                 max_rows=min(128, max_batch * (1 + speculative_tokens)) if speculative_tokens else None,
+                 weight_dtype="int4" if load_in_4bit_param(load_in_4bit) else "bf16")
     wanted = {n for n, _ in e.infer_params()}
     seen, unused = set(), []
     for name, arr in contract.iter_safetensors(model_dir):
@@ -642,8 +658,9 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
           prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None,
-          penalties: bool | None = None, speculative_tokens: int | None = None):
+          penalties: bool | None = None, speculative_tokens: int | None = None, load_in_4bit: bool | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
+    load_in_4bit = load_in_4bit_param(load_in_4bit)
     speculative_tokens = speculative_tokens_param(content, speculative_tokens)
     prefix_cache = prefix_cache_param(content, prefix_cache)
     kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
@@ -655,7 +672,7 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
         raise ValueError("an fp8 KV cache is paged: kv_cache_dtype fp8 needs kv_cache_gb")
     model_dir = os.path.join(content, "model")
     t0 = time.time()
-    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype, speculative_tokens)
+    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype, speculative_tokens, load_in_4bit)
     tok = contract.Tokenizer(model_dir)
     sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs, penalties=penalties,
                       speculative_tokens=speculative_tokens)
@@ -664,7 +681,8 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
     httpd = ThreadingHTTPServer(("0.0.0.0", port), make_handler(sched, name))
     ready = {"event": "ready", "port": port, "model": name, "load_seconds": round(time.time() - t0, 2),
              "max_batch": max_batch, "max_logprobs": max_logprobs, "penalties": penalties,
-             "speculative_tokens": speculative_tokens}
+             "speculative_tokens": speculative_tokens, "weight_dtype": engine.weight_dtype,
+             "weight_gb": round(engine.weight_bytes() / 1e9, 3)}
     if engine.kv_pages is not None:
         from .infer import kv_page_bytes
         ready.update(kv_pages=engine.kv_pages, kv_page_mb=round(kv_page_bytes(engine.serve_arch, kv_dtype) / 1e6, 2),
@@ -697,10 +715,13 @@ def main(argv=None) -> int:
     ap.add_argument("--speculative-tokens", type=int, default=None,
                     help="tokens drafted by prompt lookup and verified per request and step, 0..7 (default: param "
                          "speculative_tokens, else 0: off)")
+    ap.add_argument("--load-in-4bit", action="store_true", default=None,
+                    help="store the projections as int4, one bf16 scale per row and 64 inputs (default: env "
+                         "MODEL_LOAD_IN_4BIT, else bf16)")
     a = ap.parse_args(argv)
     try:
         serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype,
-              a.max_logprobs, a.penalties, a.speculative_tokens)
+              a.max_logprobs, a.penalties, a.speculative_tokens, a.load_in_4bit)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()
