@@ -411,6 +411,12 @@ B200W_API int b200w_op_gemm_bias(b200w_ctx* ctx, const void* A, int lda, const v
  * bf16-rounded copy of D that the last micro-step's weight gradient hands to the gradient exchange. */
 B200W_API int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb,
                                  float* D, const float* C, int ldd, int M, int N, int K, int block_n, void* d2);
+/* b200w_op_gemm with the tile width chosen as the training step chooses it (block_n = 0) and the persistent grid
+ * shrunk by sm_reserve SMs, as the backward shrinks it while the gradient exchange overlaps it. d2 (may be NULL):
+ * as in b200w_op_gemm_wire, fp32 outputs only. B200W_ERR_INVALID unless 0 <= sm_reserve < the SM count. */
+B200W_API int b200w_op_gemm_reserve(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn,
+                                    int ldb, void* D, const void* C, int out_f32, int ldd, int M, int N, int K,
+                                    void* d2, int sm_reserve);
 /* out[M,N] = X[M,K] W[N,K]^T (+C), M <= 128: the decode-time projection (swap-AB, split-K). */
 B200W_API int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k);

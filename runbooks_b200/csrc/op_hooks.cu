@@ -67,6 +67,23 @@ int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int lda, const v
   HOOK(gemm_bf16_ex(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, true, ldd, M, N, K, block_n, nullptr, 0, ctx_stream(ctx),
                     d2));
 }
+int b200w_op_gemm_reserve(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn, int ldb, void* D,
+                          const void* C, int out_f32, int ldd, int M, int N, int K, void* d2, int sm_reserve) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(sm_reserve >= 0 && sm_reserve < sm_count(), "sm_reserve must lie in [0, SM count)");
+    // the engine's GEMM call with the reserve its overlapped backward sets; the previous reserve comes back on every
+    // exit
+    struct Reserve {
+      int prev = gemm_sm_reserve();
+      ~Reserve() { gemm_set_sm_reserve(prev); }
+    } scope;
+    gemm_set_sm_reserve(sm_reserve);
+    gemm_bf16_ex(A, a_mn != 0, lda, B, b_mn != 0, ldb, D, C, out_f32 != 0, ldd, M, N, K, 0, nullptr, 0, ctx_stream(ctx),
+                 d2);
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
 int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k) {
   return guarded(ctx, [&] {

@@ -1,5 +1,6 @@
 """The pipelined attention kernels: what the compiler made of them, and their results at the shapes that exercise
-the pipelines, against torch's own CUDA SDPA in fp32 (the tolerances of tests/test_attention.py).
+the pipelines, against an fp64 reference one head at a time, element by element (tests/error_bounds.py), with the
+failing unit -- (sequence, head, 128-row tile, 64-row half) -- named.
 
 The compiler test needs no GPU: the kernels keep products in flight only if ptxas neither spills nor serializes
 their wgmma instructions, and it says so in its -Xptxas -v report."""
@@ -11,7 +12,8 @@ import subprocess
 import pytest
 import torch
 
-from util import call, rel_err
+import error_bounds as E
+from util import call
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "runbooks_b200", "csrc")
@@ -48,9 +50,9 @@ def test_attention_kernels_neither_spill_nor_serialize(tmp_path):
     assert seen == set(KERNELS), f"ptxas reported on {sorted(seen)} only"
 
 
-def _check(engine, B, S, H, Hkv, dh=128, dh_pad=128, seed=0):
+def _run(engine, B, S, H, Hkv, dh=128, dh_pad=128, seed=0):
     """Forward and backward through the library on bf16 q, k, v (head_dim dh, zero-padded to dh_pad columns as the
-    Falcon prefill stores it) against torch SDPA in fp32 on the same bf16-rounded values."""
+    Falcon prefill stores it). Returns the inputs and outputs as [B, heads, S, dh] views and lse as [B, H, S]."""
     g = torch.Generator().manual_seed(seed)
     T, ld = B * S, (H + 2 * Hkv) * dh_pad
     x = torch.zeros(T, H + 2 * Hkv, dh_pad)
@@ -68,33 +70,22 @@ def _check(engine, B, S, H, Hkv, dh=128, dh_pad=128, seed=0):
     call(engine, "b200w_op_attention_bwd", qkv, ld, k_off, v_off, out, dout, H * dh_pad, lse, delta, dqkv,
          B, S, H, Hkv, scale)
     torch.cuda.synchronize()
-
-    def heads(t, lo, n):  # [T, *] columns of n heads from lo -> [B, n, S, dh] fp32
-        return t[:, lo:lo + n * dh_pad].float().view(B, S, n, dh_pad)[..., :dh].transpose(1, 2).contiguous()
-
-    q = heads(qkv, 0, H).requires_grad_(True)
-    k = heads(qkv, k_off, Hkv).requires_grad_(True)
-    v = heads(qkv, v_off, Hkv).requires_grad_(True)
-    G = H // Hkv
-    ref = torch.nn.functional.scaled_dot_product_attention(
-        q, k.repeat_interleave(G, 1), v.repeat_interleave(G, 1), is_causal=True, scale=scale)
-    ref.backward(heads(dout, 0, H))
-    res = dict(out=rel_err(heads(out, 0, H), ref.detach()),
-               dq=rel_err(heads(dqkv, 0, H), q.grad), dk=rel_err(heads(dqkv, k_off, Hkv), k.grad),
-               dv=rel_err(heads(dqkv, v_off, Hkv), v.grad))
-    with torch.no_grad():  # log2-domain log-sum-exp, one head at a time (the S x S scores of all heads are large)
-        e_lse = 0.0
-        mask = torch.ones(S, S, dtype=torch.bool, device="cuda").tril()
-        for hh in range(H):
-            s = (q[:, hh] @ k[:, hh // G].transpose(-1, -2)) * scale
-            ref_lse = torch.logsumexp(s.masked_fill(~mask, float("-inf")), -1) / torch.log(torch.tensor(2.0))
-            e_lse = max(e_lse, float((lse[hh].view(B, S) - ref_lse).abs().max()))
-    res["lse"] = e_lse
     assert torch.isfinite(dqkv.float()).all()
     if dh < dh_pad:  # the zero padding of q, k, v gets zero gradients and zero outputs
         assert not out.view(T, H, dh_pad)[..., dh:].any()
         assert not dqkv.view(T, H + 2 * Hkv, dh_pad)[..., dh:].any()
-    return res
+
+    def heads(t, lo, n):  # [T, *] columns of n heads from lo -> [B, n, S, dh]
+        return t[:, lo:lo + n * dh_pad].view(B, S, n, dh_pad)[..., :dh].transpose(1, 2)
+
+    return dict(q=heads(qkv, 0, H), k=heads(qkv, k_off, Hkv), v=heads(qkv, v_off, Hkv), dout=heads(dout, 0, H),
+                out=heads(out, 0, H), lse2=lse.view(H, B, S).transpose(0, 1), dq=heads(dqkv, 0, H),
+                dk=heads(dqkv, k_off, Hkv), dv=heads(dqkv, v_off, Hkv), scale=scale)
+
+
+def _check(engine, B, S, H, Hkv, dh=128, dh_pad=128, seed=0):
+    t = _run(engine, B, S, H, Hkv, dh, dh_pad, seed)
+    return E.check_attention(**t)
 
 
 @pytest.mark.gpu
@@ -106,9 +97,36 @@ def _check(engine, B, S, H, Hkv, dh=128, dh_pad=128, seed=0):
 ])
 def test_pipelined_attention_matches_sdpa(engine, B, S, H, Hkv, dh):
     r = _check(engine, B, S, H, Hkv, dh=dh, seed=S + H)
-    print(f"attention B{B} S{S} H{H} Hkv{Hkv} dh{dh}: " + " ".join(f"{k}={v:.3e}" for k, v in r.items()))
-    assert r["out"] < 5e-3 and r["lse"] < 2e-3
-    assert r["dq"] < 1.5e-2 and r["dk"] < 1.5e-2 and r["dv"] < 1.5e-2
+    print(f"attention B{B} S{S} H{H} Hkv{Hkv} dh{dh}: lse max-abs {r['lse']:.3e}")
+    for n in ("out", "dq", "dk", "dv"):
+        print("  ", r[n])
+    assert r["lse"] < 2e-3
+    bad = [str(r[n]) for n in ("out", "dq", "dk", "dv") if not r[n].ok]
+    assert not bad, bad
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind,target,shape,unit", [
+    ("out_kblock", "out", (2, 4096, 20, 20), (1, 7, 12, 1)),     # key block 0 missing from rows 1600..1663
+    ("out_mask", "out", (2, 4096, 20, 20), (0, 3, 1, 0)),       # the diagonal block sees one key too many
+    ("dk_qblock", "dk", (2, 4096, 20, 20), (1, 11, 20, 0)),     # one 64-query block missing from 64 keys
+    ("dv_qblock", "dv", (2, 4096, 20, 20), (0, 5, 9, 1)),
+    ("dq_diag", "dq", (2, 4096, 20, 20), (1, 2, 5, 1)),         # the lag-1 tail: the last key block missing
+    ("dq_kv_head", "dq", (1, 1024, 8, 2), (0, 1, 3, 0)),        # GQA: dQ against the neighbouring kv head
+])
+def test_checks_flag_a_fault_in_one_unit(engine, kind, target, shape, unit):
+    """The kernel's real outputs, corrupted after the fact in one unit, are flagged in that unit, where the global
+    relative norm of the old checks (5e-3 for out, 1.5e-2 for the gradients) dilutes the fault by the square root of
+    the number of units."""
+    B, S, H, Hkv = shape
+    t = _run(engine, B, S, H, Hkv, seed=S + H)
+    clean = E.check_attention(**t)
+    assert clean[target].ok, str(clean[target])
+    t[target] = E.attention_fault(kind, t[target], t["q"], t["k"], t["v"], t["dout"], t["scale"], unit=unit)
+    r = E.check_attention(**t)[target]
+    bar = 5e-3 if target == "out" else 1.5e-2
+    print(f"{kind}: {r} (old bar {bar:g} {'caught' if r.rel_err >= bar else 'missed'})")
+    assert not r.ok and r.unit == unit, str(r)
 
 
 # ---------------------------------------------------------------------------------------------
