@@ -417,6 +417,12 @@ B200W_API int b200w_op_gemm_wire(b200w_ctx* ctx, const void* A, int a_mn, int ld
 B200W_API int b200w_op_gemm_reserve(b200w_ctx* ctx, const void* A, int a_mn, int lda, const void* B, int b_mn,
                                     int ldb, void* D, const void* C, int out_f32, int ldd, int M, int N, int K,
                                     void* d2, int sm_reserve);
+/* n (1..4) weight gradients dW_i[M_i, N_i] (+)= dy_i[K_i, M_i]^T x_i[K_i, N_i] in one persistent launch, as the
+ * training step issues a Llama layer's four: mnk = n triples (M, N, K); dy, x: bf16, row strides M and N; D, C
+ * (C NULL or C == D, to accumulate), d2 (NULL or bf16): fp32 row stride N; the grid shrunk by sm_reserve SMs as in
+ * b200w_op_gemm_reserve. Each D is bit-identical to b200w_op_gemm_reserve of the same problem. */
+B200W_API int b200w_op_gemm_group(b200w_ctx* ctx, int n, const void* const* dy, const void* const* x, float* const* D,
+                                  const float* const* C, void* const* d2, const int* mnk, int sm_reserve);
 /* out[M,N] = X[M,K] W[N,K]^T (+C), M <= 128: the decode-time projection (swap-AB, split-K). */
 B200W_API int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k);

@@ -134,6 +134,7 @@ PROTOTYPES = {
                                      C.c_int, C.c_int, C.c_int, vp]),
     "b200w_op_gemm_reserve": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, vp, C.c_int]),
+    "b200w_op_gemm_group": (C.c_int, [c_ctx, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int]),
     "b200w_op_gemm_decode": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_w4_image_bytes": (C.c_int64, [C.c_int, C.c_int]),
     "b200w_op_quantize_w4": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),

@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <unordered_map>
@@ -469,10 +470,9 @@ void alloc_activations(b200w_ctx* c) {
   }
 }
 
-// GEMM launch with optional CUDA-event bracketing (bench.py's roofline leg)
-void egemm(b200w_ctx* c, const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
-           const void* C, bool out_fp32, int ldd, int M, int N, int K, const void* bias = nullptr, int act = 0,
-           void* d2_bf16 = nullptr) {
+// GEMM launch with optional CUDA-event bracketing (bench.py's roofline leg): `launch` issues it, `flops` is its work
+template <class F>
+void gemm_launch(b200w_ctx* c, double flops, F&& launch) {
   cudaStream_t s = c->stream;
   if (c->prof_gemm) {
     if (c->prof_used + 2 > c->prof_events.size()) {
@@ -484,13 +484,20 @@ void egemm(b200w_ctx* c, const void* A, bool a_mn, int lda, const void* B, bool 
     }
     B200W_CUDA(cudaEventRecord(c->prof_events[c->prof_used], s));
   }
-  gemm_bf16_ex(A, a_mn, lda, B, b_mn, ldb, D, C, out_fp32, ldd, M, N, K, 0, bias, act, s, d2_bf16);
+  launch(s);
   ++c->launches;
   if (c->prof_gemm) {
     B200W_CUDA(cudaEventRecord(c->prof_events[c->prof_used + 1], s));
     c->prof_used += 2;
-    c->prof_flops += 2.0 * M * N * static_cast<double>(K);
+    c->prof_flops += flops;
   }
+}
+void egemm(b200w_ctx* c, const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
+           const void* C, bool out_fp32, int ldd, int M, int N, int K, const void* bias = nullptr, int act = 0,
+           void* d2_bf16 = nullptr) {
+  gemm_launch(c, 2.0 * M * N * static_cast<double>(K), [&](cudaStream_t s) {
+    gemm_bf16_ex(A, a_mn, lda, B, b_mn, ldb, D, C, out_fp32, ldd, M, N, K, 0, bias, act, s, d2_bf16);
+  });
 }
 
 // ---- forward of one micro-batch (ids already on device) ------------------------------------------
@@ -674,6 +681,29 @@ struct GradOut {
           overlap_ar ? c->gw + off : nullptr);
     if (overlap_ar) allreduce_range(c, off, static_cast<size_t>(M) * N, true);
   }
+  // several weight gradients {off, dy, M, x, N} in one persistent GEMM launch (gemm_bf16_group: each gradient
+  // bit-identical to its own launch, without a partial last wave per matrix), then their exchanges in that order
+  struct Wgrad {
+    size_t off;
+    const void* dy;
+    int M;
+    const void* x;
+    int N;
+  };
+  void wgrad_group(std::initializer_list<Wgrad> list) const {
+    GemmWgrad p[4];
+    int n = 0;
+    double flops = 0;
+    for (const Wgrad& w : list) {
+      float* d = c->g + w.off;
+      p[n++] = GemmWgrad{w.dy, w.M, w.x, w.N, d, first ? nullptr : d, w.N, w.M, w.N, T,
+                         overlap_ar ? c->gw + w.off : nullptr};
+      flops += 2.0 * w.M * w.N * static_cast<double>(T);
+    }
+    gemm_launch(c, flops, [&](cudaStream_t s) { gemm_bf16_group(p, n, s); });
+    if (overlap_ar)
+      for (const Wgrad& w : list) allreduce_range(c, w.off, static_cast<size_t>(w.M) * w.N, true);
+  }
   void exchange(size_t off, size_t count) const {
     if (overlap_ar) allreduce_range(c, off, count);
   }
@@ -693,21 +723,24 @@ void backward_layer_llama(b200w_ctx* c, const Dims& m, const GradOut& go, int l,
   if (c->recompute) forward_layer_llama(c, m, l, x.h_in, nullptr, docs);
   // h_next = h_mid + act Wd^T
   egemm(c, dh_cur, false, m.d, c->w + p.wd, true, m.f, c->dact, nullptr, false, m.f, m.T, m.f, m.d);
-  go.wgrad(p.wd, dh_cur, m.d, x.act, m.f);
   swiglu_bwd(c->dact, x.gu, c->dgu, m.T, m.f, s); ++n;
   egemm(c, c->dgu, false, 2 * m.f, c->w + p.wgu, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, 2 * m.f);
-  go.wgrad(p.wgu, c->dgu, 2 * m.f, x.n2, m.d);
   // dh_mid = dh + rmsnorm_bwd(dn2)
   rmsnorm_bwd(c->dn, x.h_mid, c->w + p.ln2, x.rstd2, dh_cur, dh_alt, g + p.ln2, c->dw_partial, m.T, m.d, s); n += 2;
   std::swap(dh_cur, dh_alt);
   // h_mid = h_in + attn Wo^T
   egemm(c, dh_cur, false, m.d, c->w + p.wo, true, m.qd, c->dattn, nullptr, false, m.qd, m.T, m.qd, m.d);
-  go.wgrad(p.wo, dh_cur, m.d, x.attn, m.qd);
   attention_bwd(x.qkv, m.qkvd, m.qd, m.qd + m.kd, x.attn, c->dattn, m.qd, x.lse, c->delta, c->dqkv, m.nseq, m.S,
                 m.H, m.Hkv, m.scale, s, docs); n += 3;
   rope_apply(c->dqkv, m.qkvd, c->rope_tab, m.T, m.S, m.H + m.Hkv, m.dh, true, s, 0, docs ? docs->pos : nullptr); ++n;
   egemm(c, c->dqkv, false, m.qkvd, c->w + p.wqkv, true, m.d, c->dn, nullptr, false, m.d, m.T, m.d, m.qkvd);
-  go.wgrad(p.wqkv, c->dqkv, m.qkvd, x.n1, m.d);
+  // the layer's four weight gradients in one launch, while all their operands are alive: the layer output's gradient
+  // is in dh_alt until rmsnorm_bwd(ln1) below overwrites it, dh_mid's in dh_cur, and dgu, dqkv and the activations
+  // are this layer's
+  go.wgrad_group({{p.wd, dh_alt, m.d, x.act, m.f},
+                  {p.wgu, c->dgu, 2 * m.f, x.n2, m.d},
+                  {p.wo, dh_cur, m.d, x.attn, m.qd},
+                  {p.wqkv, c->dqkv, m.qkvd, x.n1, m.d}});
   rmsnorm_bwd(c->dn, x.h_in, c->w + p.ln1, x.rstd1, dh_cur, dh_alt, g + p.ln1, c->dw_partial, m.T, m.d, s); n += 2;
   std::swap(dh_cur, dh_alt);
 }

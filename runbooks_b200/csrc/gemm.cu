@@ -93,11 +93,14 @@ struct Cfg {
 // accumulation micro-step's wgrad writes the gradient's NCCL wire copy from the registers that hold the fp32 sum,
 // instead of a separate cast pass re-reading the fp32 gradient (engine.cu exchange_one). The kernel writes it
 // through the tensor map tmD2 and uses the pointer only as the flag.
+// reduce (fp32 outputs only): D += the tile, added in the L2 by TMA reduce-add stores through tmD instead of
+// plain stores; nothing is loaded into the staging.
 struct EpiExtra {
   const __nv_bfloat16* bias;
   int act;
   __nv_bfloat16* d2;
   bool c;
+  bool reduce;
 };
 
 // byte offset of byte `lin` of a box whose rows are stored back to back, after the SWIZZLE_128B permutation (the
@@ -162,10 +165,34 @@ struct Epi {
   static_assert(CHUNKS % PER_PASS == 0, "whole passes");
 };
 
-template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR>
-__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmD,
-                                          const CUtensorMap* tmC, const CUtensorMap* tmD2, const CUtensorMap* tmBias,
-                                          int M, int N, int K, int n_fast, const EpiExtra& ex) {
+// One GEMM of a launch: its tensor maps, shape, tile raster (pick_raster) and epilogue, and where its tiles start in
+// the launch's tile list. tmC, tmD2 and tmBias are copies of tmD when unused.
+struct GemmProblem {
+  CUtensorMap tmA, tmB, tmD, tmC, tmD2, tmBias;
+  int M, N, K, raster, tile0;
+  EpiExtra ex;
+};
+// The GEMMs of one persistent launch: their tiles form one list, problem after problem, walked with the usual static
+// stride. Each tile is computed exactly as a launch of its problem alone computes it.
+template <int NP>
+struct GemmGroup {
+  GemmProblem p[NP];
+  int count, tiles;
+};
+
+// the problem tile `tile` of the list belongs to, and its index among that problem's tiles
+template <int NP>
+__device__ __forceinline__ const GemmProblem& locate(const GemmGroup<NP>& g, int tile, int& local) {
+  int i = 0;
+#pragma unroll
+  for (int j = 1; j < NP; ++j)
+    if (j < g.count && tile >= g.p[j].tile0) i = j;
+  local = tile - g.p[i].tile0;
+  return g.p[i];
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR, int NP>
+__device__ __forceinline__ void gemm_body(const GemmGroup<NP>& g) {
   using cfg = Cfg<BLOCK_N>;
   using epi = Epi<BLOCK_N, OutT>;
   constexpr int STAGES = cfg::STAGES;
@@ -184,14 +211,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t rank = PAIR ? cluster_ctarank() : 0;
-  // the producer TMA-loads the tile's addend C and bias into shared memory ahead of the epilogue
-  const bool bias = sizeof(OutT) == 2 && ex.bias != nullptr;
-  const bool addend = ex.c || bias;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(tmA);
-    tma_prefetch_desc(tmB);
-    tma_prefetch_desc(tmD);
+    for (int j = 0; j < g.count; ++j) {
+      tma_prefetch_desc(&g.p[j].tmA);
+      tma_prefetch_desc(&g.p[j].tmB);
+      tma_prefetch_desc(&g.p[j].tmD);
+    }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], PAIR ? 16 : 8);  // one arrival per consumer warp (of both CTAs)
@@ -205,10 +231,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
   if constexpr (PAIR) cluster_sync_all();
   else __syncthreads();
 
-  const int num_m = (M + TILE_M - 1) / TILE_M;
-  const int num_n = (N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = num_m * num_n;
-  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  const int num_tiles = g.tiles;
   const int first = PAIR ? (blockIdx.x >> 1) : blockIdx.x;
   const int stride = PAIR ? (gridDim.x >> 1) : gridDim.x;
 
@@ -217,12 +240,20 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0, c_phase = 0;
-      // the addend's first pass (and the tile's bias) is loaded once the tile's first min(num_kb, STAGES) k-blocks are in flight: the ring
-      // is full then, and the consumers free the staging at their first k-block of the tile
-      const int c_at = (num_kb < STAGES ? num_kb : STAGES) - 1;
       for (int tile = first; tile < num_tiles; tile += stride) {
+        int lt;
+        const GemmProblem& P = locate(g, tile, lt);
+        const CUtensorMap *tmA = &P.tmA, *tmB = &P.tmB, *tmC = &P.tmC, *tmBias = &P.tmBias;
+        const EpiExtra& ex = P.ex;
+        const int num_kb = (P.K + BLOCK_K - 1) / BLOCK_K;
+        // the producer TMA-loads the tile's addend C and bias into shared memory ahead of the epilogue
+        const bool bias = sizeof(OutT) == 2 && ex.bias != nullptr;
+        const bool addend = ex.c || bias;
+        // the addend's first pass (and the tile's bias) is loaded once the tile's first min(num_kb, STAGES) k-blocks
+        // are in flight: the ring is full then, and the consumers free the staging at their first k-block of the tile
+        const int c_at = (num_kb < STAGES ? num_kb : STAGES) - 1;
         int mi, ni;
-        tile_coords(tile, num_m, num_n, n_fast, mi, ni);
+        tile_coords(lt, (P.M + TILE_M - 1) / TILE_M, (P.N + BLOCK_N - 1) / BLOCK_N, P.raster, mi, ni);
         const int m0 = mi * TILE_M + rank * BLOCK_M, n0 = ni * BLOCK_N;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -290,6 +321,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
     uint32_t phase = 0, c_phase = 0;
     for (int tile = first; tile < num_tiles; tile += stride) {
       int prev = -1;
+      int num_kb;
+      bool addend;
+      {
+        int lt;
+        const GemmProblem& P = locate(g, tile, lt);
+        num_kb = (P.K + BLOCK_K - 1) / BLOCK_K;
+        addend = P.ex.c || (sizeof(OutT) == 2 && P.ex.bias != nullptr);
+      }
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * cfg::STAGE_BYTES);
@@ -319,8 +358,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
       // epilogue: registers (+ C from the staging) -> staging -> TMA store; the producer is already loading the
       // next tile, and the stores drain while the next tile's MMAs run. acc[4 j + 2 h + e] is row
       // 16 wi + lane / 4 + 8 h of the warpgroup's 64, column 8 j + 2 (lane % 4) + e of the tile.
-      int mi, ni;  // (derived here, not kept in registers through the k-loop)
-      tile_coords(tile, num_m, num_n, n_fast, mi, ni);
+      int lt, mi, ni;  // (derived here, not kept in registers through the k-loop)
+      const GemmProblem& P = locate(g, tile, lt);
+      const CUtensorMap *tmD = &P.tmD, *tmC = &P.tmC, *tmD2 = &P.tmD2;
+      const EpiExtra& ex = P.ex;
+      const bool bias = sizeof(OutT) == 2 && ex.bias != nullptr;
+      tile_coords(lt, (P.M + TILE_M - 1) / TILE_M, (P.N + BLOCK_N - 1) / BLOCK_N, P.raster, mi, ni);
       const int n0 = ni * BLOCK_N;
       const int mw = mi * TILE_M + rank * BLOCK_M + wg * 64;
       const int row_lo = wi * 16 + (lane >> 2);
@@ -373,8 +416,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
         fence_proxy_async_smem();
         named_bar_sync(1 + wg, 128);
         if (elected) {
-          for (int q = 0; q < epi::PER_PASS; ++q)
-            tma_store_2d(tmD, stg + q * EPI_SLOT_BYTES, n0 + (p * epi::PER_PASS + q) * epi::CW, mw);
+          for (int q = 0; q < epi::PER_PASS; ++q) {
+            if (sizeof(OutT) == 4 && ex.reduce)
+              tma_reduce_add_2d(tmD, stg + q * EPI_SLOT_BYTES, n0 + (p * epi::PER_PASS + q) * epi::CW, mw);
+            else
+              tma_store_2d(tmD, stg + q * EPI_SLOT_BYTES, n0 + (p * epi::PER_PASS + q) * epi::CW, mw);
+          }
           bulk_commit();
         }
         // (fp32 outputs run on tiles >= 128 wide, whose passes are whole 64-column bf16 boxes)
@@ -411,28 +458,28 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_bf16_kernel(const __grid_constant__ GemmGroup<1> g) {
+  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(g);
+}
+
+// up to four GEMMs in one persistent launch (gemm_bf16_group)
+constexpr int GROUP_MAX = 4;
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmC,
-                 const __grid_constant__ CUtensorMap tmD2, const __grid_constant__ CUtensorMap tmBias, int M, int N,
-                 int K, int n_fast, EpiExtra ex) {
-  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(&tmA, &tmB, &tmD, &tmC, &tmD2, &tmBias, M, N, K, n_fast, ex);
+gemm_bf16_group_kernel(const __grid_constant__ GemmGroup<GROUP_MAX> g) {
+  gemm_body<BLOCK_N, A_MN, B_MN, OutT, false>(g);
 }
 
 // 256 x 256 tiles on a 2-CTA cluster with the B operand multicast (block_n = 512)
 template <bool A_MN, bool B_MN, typename OutT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmC,
-                      const __grid_constant__ CUtensorMap tmD2, const __grid_constant__ CUtensorMap tmBias, int M,
-                      int N, int K, int n_fast, EpiExtra ex) {
-  gemm_body<PAIR_N, A_MN, B_MN, OutT, true>(&tmA, &tmB, &tmD, &tmC, &tmD2, &tmBias, M, N, K, n_fast, ex);
+gemm_bf16_pair_kernel(const __grid_constant__ GemmGroup<1> g) {
+  gemm_body<PAIR_N, A_MN, B_MN, OutT, true>(g);
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR = false>
-void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, int K, int lda,
-            int ldb, int ldd, EpiExtra ex, cudaStream_t stream) {
-  using cfg = Cfg<BLOCK_N>;
+GemmProblem make_problem(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, int K, int lda, int ldb,
+                         int ldd, EpiExtra ex, int tile0) {
   constexpr int TILE_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
   // A: K-major => global [M rows, K cols]; MN-major => global [K rows, M cols]
   CUtensorMap tmA = A_MN ? make_tmap_bf16_2d(A, K, M, lda, BLOCK_K, 64)
@@ -451,9 +498,32 @@ void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, 
   const CUtensorMap tmD2 = ex.d2 ? make_tmap_bf16_2d(ex.d2, M, N, ldd, 64, 64) : tmD;
   // bias: one row of N columns in boxes of the tile's width, stored plain (columns past N arrive as zeros)
   const CUtensorMap tmBias = ex.bias ? make_tmap_bf16_2d(ex.bias, 1, N, (N + 7) / 8 * 8, 1, BLOCK_N, false) : tmD;
-  ex.c = C != nullptr;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, int,
-               EpiExtra);
+  // An fp32 accumulation in place (C == D) that writes no bf16 copy adds the tile to D in the L2 by TMA reduce-add:
+  // the same single fp32 round-to-nearest add per element as the load-C epilogue, without C's HBM round trips on
+  // the consumers' path and without the producer's hand-off of the staging. d2 needs the sum in registers, and a
+  // bf16 C would round differently, so those keep the load-C epilogue.
+  ex.reduce = sizeof(OutT) == 4 && C != nullptr && static_cast<const void*>(C) == static_cast<const void*>(D) &&
+              ex.d2 == nullptr;
+  ex.c = C != nullptr && !ex.reduce;
+  return GemmProblem{tmA, tmB, tmD, tmC, tmD2, tmBias, M, N, K, pick_raster(M, N, K, TILE_M, BLOCK_N), tile0, ex};
+}
+
+// persistent grid: one CTA (pair) per SM (pair) left by the reserve, at most one per tile
+int gemm_grid(int tiles, bool pair) {
+  const int slots = (sm_count() - gemm_sm_reserve()) / (pair ? 2 : 1);
+  return (tiles < slots ? tiles : slots) * (pair ? 2 : 1);
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, typename OutT, bool PAIR = false>
+void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, int K, int lda,
+            int ldb, int ldd, EpiExtra ex, cudaStream_t stream) {
+  using cfg = Cfg<BLOCK_N>;
+  constexpr int TILE_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
+  GemmGroup<1> g;
+  g.p[0] = make_problem<BLOCK_N, A_MN, B_MN, OutT, PAIR>(A, B, D, C, M, N, K, lda, ldb, ldd, ex, 0);
+  g.count = 1;
+  g.tiles = ((M + TILE_M - 1) / TILE_M) * ((N + BLOCK_N - 1) / BLOCK_N);
+  void (*kern)(GemmGroup<1>);
   if constexpr (PAIR) kern = gemm_bf16_pair_kernel<A_MN, B_MN, OutT>;
   else kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, OutT>;
   static PerDeviceOnce once;  // per template instantiation
@@ -461,11 +531,7 @@ void launch(const void* A, const void* B, OutT* D, const OutT* C, int M, int N, 
     B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     cfg::SMEM_BYTES));
   });
-  const int num_tiles = ((M + TILE_M - 1) / TILE_M) * ((N + BLOCK_N - 1) / BLOCK_N);
-  const int slots = (sm_count() - gemm_sm_reserve()) / (PAIR ? 2 : 1);
-  const int grid = (num_tiles < slots ? num_tiles : slots) * (PAIR ? 2 : 1);
-  kern<<<grid, GEMM_THREADS, cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmC, tmD2, tmBias, M, N, K,
-                                                        pick_raster(M, N, K, TILE_M, BLOCK_N), ex);
+  kern<<<gemm_grid(g.tiles, PAIR), GEMM_THREADS, cfg::SMEM_BYTES, stream>>>(g);
   B200W_CUDA(cudaGetLastError());
 }
 
@@ -982,30 +1048,38 @@ void gemm_bf16(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int 
 }
 // + bias [N] (bf16, 16-byte aligned) added to every row and act (0 none, 1 ReLU) after bias and C:
 // nn.Linear(bias=True) (+ residual) (+ ReLU) in the epilogue. bf16 output only.
-void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
-                  const void* C, bool out_fp32, int ldd, int M, int N, int K, int block_n, const void* bias,
-                  int act, cudaStream_t stream, void* d2_bf16) {
+static void check_gemm_args(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, const void* D,
+                            const void* C, bool out_fp32, int ldd, int M, int N, int K, const void* bias, int act,
+                            const void* d2_bf16) {
   B200W_CHECK(!(out_fp32 && (bias || act)), "bias / activation epilogue is built for bf16 outputs");
   B200W_CHECK((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bias must be 16-byte aligned");
   B200W_CHECK(!d2_bf16 || (out_fp32 && ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(d2_bf16) & 15) == 0),
               "the bf16 copy exists for fp32 outputs with 16-byte aligned bf16 rows");
-  const EpiExtra ex{static_cast<const __nv_bfloat16*>(bias), act, static_cast<__nv_bfloat16*>(d2_bf16), false};
   B200W_CHECK(M > 0 && N > 0 && K > 0, "empty GEMM");
   B200W_CHECK(lda % 8 == 0 && ldb % 8 == 0, "TMA needs 16-byte aligned row strides");
   B200W_CHECK(ldd % (out_fp32 ? 4 : 8) == 0, "output rows must be 16-byte aligned");
   B200W_CHECK((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(D) & 15) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0,
               "operands must be 16-byte aligned");
-  if (block_n == 0) {
-    // widest tile that still gives every SM a tile; K-major-only narrow tiles when M fits one tile
-    const long m_tiles = (M + 127) / 128;
-    const bool narrow_ok = !a_mn && !b_mn && !out_fp32;
-    block_n = narrow_ok ? 32 : 128;
-    for (int bn : {256, 128, 64}) {
-      if (bn < 128 && !narrow_ok) break;
-      if (N >= bn && m_tiles * ((N + bn - 1) / bn) >= sm_count()) { block_n = bn; break; }
-    }
+}
+
+// block_n = 0: the widest tile that still gives every SM a tile; K-major-only narrow tiles when M fits one tile
+static int auto_block_n(bool a_mn, bool b_mn, bool out_fp32, int M, int N) {
+  const long m_tiles = (M + 127) / 128;
+  const bool narrow_ok = !a_mn && !b_mn && !out_fp32;
+  for (int bn : {256, 128, 64}) {
+    if (bn < 128 && !narrow_ok) break;
+    if (N >= bn && m_tiles * ((N + bn - 1) / bn) >= sm_count()) return bn;
   }
+  return narrow_ok ? 32 : 128;
+}
+
+void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
+                  const void* C, bool out_fp32, int ldd, int M, int N, int K, int block_n, const void* bias,
+                  int act, cudaStream_t stream, void* d2_bf16) {
+  check_gemm_args(A, a_mn, lda, B, b_mn, ldb, D, C, out_fp32, ldd, M, N, K, bias, act, d2_bf16);
+  const EpiExtra ex{static_cast<const __nv_bfloat16*>(bias), act, static_cast<__nv_bfloat16*>(d2_bf16), false, false};
+  if (block_n == 0) block_n = auto_block_n(a_mn, b_mn, out_fp32, M, N);
   B200W_CHECK(block_n == 32 || block_n == 64 || block_n == 128 || block_n == 256 || block_n == 512,
               "block_n must be 0, 32, 64, 128, 256 or 512 (2-CTA cluster)");
   B200W_CHECK(block_n >= 128 || !out_fp32, "narrow tiles write bf16");
@@ -1023,6 +1097,46 @@ void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, i
   };
   if (out_fp32) run(float{});
   else run(__nv_bfloat16{});
+}
+
+// dW[M, N] (+)= dy[K, M]^T x[K, N] for up to four weight gradients in one persistent launch: fp32 outputs, both
+// operands read MN-major. Each problem gets the tile, raster and epilogue (first, accumulating in place, or with the
+// wire copy d2) that gemm_bf16_ex with block_n = 0 gives it, so its output is bit-identical to that call's; only
+// which CTA computes a tile, and when, changes. Launched one after another, the problems' partial last waves each
+// cost a whole wave; here only the list's last wave is partial. Problems whose automatic tile is not 128 x 256 (small
+// models) run as separate launches.
+void gemm_bf16_group(const GemmWgrad* w, int n, cudaStream_t stream) {
+  B200W_CHECK(n >= 1 && n <= GROUP_MAX, "a GEMM group holds 1 to 4 problems");
+  bool wide = true;
+  for (int i = 0; i < n; ++i) {
+    check_gemm_args(w[i].dy, true, w[i].ldy, w[i].x, true, w[i].ldx, w[i].D, w[i].C, true, w[i].ldd, w[i].M, w[i].N,
+                    w[i].K, nullptr, 0, w[i].d2);
+    wide = wide && auto_block_n(true, true, true, w[i].M, w[i].N) == 256;
+  }
+  if (!wide) {
+    for (int i = 0; i < n; ++i)
+      gemm_bf16_ex(w[i].dy, true, w[i].ldy, w[i].x, true, w[i].ldx, w[i].D, w[i].C, true, w[i].ldd, w[i].M, w[i].N,
+                   w[i].K, 0, nullptr, 0, stream, w[i].d2);
+    return;
+  }
+  GemmGroup<GROUP_MAX> g;
+  int tiles = 0;
+  for (int i = 0; i < n; ++i) {
+    const EpiExtra ex{nullptr, 0, static_cast<__nv_bfloat16*>(w[i].d2), false, false};
+    g.p[i] = make_problem<256, true, true, float>(w[i].dy, w[i].x, w[i].D, w[i].C, w[i].M, w[i].N, w[i].K, w[i].ldy,
+                                                  w[i].ldx, w[i].ldd, ex, tiles);
+    tiles += ((w[i].M + BLOCK_M - 1) / BLOCK_M) * ((w[i].N + 255) / 256);
+  }
+  for (int i = n; i < GROUP_MAX; ++i) g.p[i] = g.p[0];  // never selected: count bounds the search
+  g.count = n;
+  g.tiles = tiles;
+  auto kern = gemm_bf16_group_kernel<256, true, true, float>;
+  static PerDeviceOnce once;
+  once.run([&] {
+    B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<256>::SMEM_BYTES));
+  });
+  kern<<<gemm_grid(tiles, false), GEMM_THREADS, Cfg<256>::SMEM_BYTES, stream>>>(g);
+  B200W_CUDA(cudaGetLastError());
 }
 
 // Host-side view of the tile raster for tests (no device needed): the raster word pick_raster chooses for a shape and,

@@ -84,6 +84,26 @@ int b200w_op_gemm_reserve(b200w_ctx* ctx, const void* A, int a_mn, int lda, cons
     B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
   });
 }
+int b200w_op_gemm_group(b200w_ctx* ctx, int n, const void* const* dy, const void* const* x, float* const* D,
+                        const float* const* C, void* const* d2, const int* mnk, int sm_reserve) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(n >= 1 && n <= 4 && dy && x && D && C && d2 && mnk, "a GEMM group holds 1 to 4 problems");
+    B200W_CHECK(sm_reserve >= 0 && sm_reserve < sm_count(), "sm_reserve must lie in [0, SM count)");
+    struct Reserve {
+      int prev = gemm_sm_reserve();
+      ~Reserve() { gemm_set_sm_reserve(prev); }
+    } scope;
+    gemm_set_sm_reserve(sm_reserve);
+    GemmWgrad w[4];
+    for (int i = 0; i < n; ++i) {
+      const int M = mnk[3 * i], N = mnk[3 * i + 1], K = mnk[3 * i + 2];
+      w[i] = GemmWgrad{dy[i], M, x[i], N, D[i], C[i], N, M, N, K, d2[i]};
+    }
+    gemm_bf16_group(w, n, ctx_stream(ctx));
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
 int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out, const void* C, int M,
                          int N, int K, int split_k) {
   return guarded(ctx, [&] {

@@ -22,6 +22,20 @@ void gemm_bf16(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int 
 void gemm_bf16_ex(const void* A, bool a_mn, int lda, const void* B, bool b_mn, int ldb, void* D,
                   const void* C, bool out_fp32, int ldd, int M, int N, int K, int block_n, const void* bias,
                   int act, cudaStream_t s, void* d2_bf16 = nullptr);
+// One weight gradient dW[M, N] (+)= dy[K, M]^T x[K, N] (fp32, both operands MN-major, row strides ldy / ldx / ldd);
+// C = nullptr overwrites D, C == D accumulates; d2 as in gemm_bf16_ex.
+struct GemmWgrad {
+  const void* dy;
+  int ldy;
+  const void* x;
+  int ldx;
+  float* D;
+  const float* C;
+  int ldd, M, N, K;
+  void* d2;
+};
+// Up to four of them in one persistent launch, each output bit-identical to its own gemm_bf16_ex call (gemm.cu).
+void gemm_bf16_group(const GemmWgrad* w, int n, cudaStream_t s);
 
 // raster word (n_fast | band << 1) gemm_bf16 uses for a shape and tile size; coords (nullable): [tiles][2] = (m, n)
 // tile index of every tile in launch order. Host only.

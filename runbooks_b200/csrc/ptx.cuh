@@ -149,6 +149,13 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
 }
+// The same store, but each element is added to what global memory holds, in the L2 (an fp32 map: one fp32
+// round-to-nearest add per element, D = D + box). Same group, fence and read-completion rules as tma_store_2d.
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's bulk async-groups still read their shared-memory source
 template <int N>

@@ -5,7 +5,9 @@
 
 One micro-step of the workload runs T = 8192 rows through Sheared-LLaMA-2.7B (d 2560, ffn 6912, V 32000): the
 forward, dgrad and wgrad GEMMs below, on seeded random operands in the layouts the engine uses (wgrads accumulate in
-place into fp32, the o / down forwards add the bf16 residual). Each shape is launched through the library's GEMM hook
+place into fp32, the o / down forwards add the bf16 residual). Each wgrad runs twice: accumulating in place, which
+adds the tile to D in the L2 ("fp32 + C L2"), and with C a separate buffer, which loads C into the staging as the
+last micro-step's wire-copy epilogue does ("fp32 + C"). Each shape is launched through the library's GEMM hook
 `--warmup` times, then `--launches` times under torch.profiler with CUDA activities; the time per launch is the mean
 CUPTI duration of the GEMM kernel (the hook synchronises after every call, so a host clock would add that to it).
 TFLOP/s = 2 M N K / time. The card's name and power limit are printed with the table.
@@ -66,11 +68,21 @@ def main() -> None:
     e = Engine(0)
     g = torch.Generator(device="cuda").manual_seed(0)
     rows = []
+    runs = []
     for name, M, N, K, a_mn, b_mn, f32, addend in SHAPES:
+        runs.append((name, M, N, K, a_mn, b_mn, f32, addend))
+        if addend == "acc":
+            runs.append((name, M, N, K, a_mn, b_mn, f32, "load"))
+    for name, M, N, K, a_mn, b_mn, f32, addend in runs:
         A = torch.randn(*((K, M) if a_mn else (M, K)), device="cuda", generator=g).bfloat16()
         B = torch.randn(*((K, N) if b_mn else (N, K)), device="cuda", generator=g).bfloat16()
         out = torch.zeros(M, N, device="cuda", dtype=torch.float32 if f32 else torch.bfloat16)
-        C = out if addend == "acc" else (torch.randn(M, N, device="cuda", generator=g).bfloat16() if addend else None)
+        if addend == "acc":
+            C = out
+        elif addend == "load":
+            C = torch.zeros_like(out)
+        else:
+            C = torch.randn(M, N, device="cuda", generator=g).bfloat16() if addend else None
 
         def launch():
             st = e._lib.b200w_op_gemm(e.handle, A.data_ptr(), a_mn, A.shape[1], B.data_ptr(), b_mn, B.shape[1],
@@ -92,15 +104,16 @@ def main() -> None:
         ms = sum(times) / len(times) / 1e3
         tflops = 2.0 * M * N * K / (ms * 1e-3) / 1e12
         rows.append(dict(shape=name, M=M, N=N, K=K, ms=round(ms, 4), tflops=round(tflops, 1),
-                         epilogue=("fp32" if f32 else "bf16") + (" + C" if addend else "")))
+                         epilogue=("fp32" if f32 else "bf16") + (" + C L2" if addend == "acc" else
+                                                                  " + C" if addend else "")))
         del A, B, out, C
         torch.cuda.empty_cache()
     e.close()
     gpu = card()
     print(f"# {gpu}; mean of {args.launches} launches after {args.warmup} warm-up launches (CUPTI kernel time)")
-    print(f"{'shape':16s} {'M':>6s} {'N':>6s} {'K':>6s} {'epilogue':>10s} {'ms':>9s} {'TFLOP/s':>8s}")
+    print(f"{'shape':16s} {'M':>6s} {'N':>6s} {'K':>6s} {'epilogue':>12s} {'ms':>9s} {'TFLOP/s':>8s}")
     for r in rows:
-        print(f"{r['shape']:16s} {r['M']:6d} {r['N']:6d} {r['K']:6d} {r['epilogue']:>10s} {r['ms']:9.4f} {r['tflops']:8.1f}")
+        print(f"{r['shape']:16s} {r['M']:6d} {r['N']:6d} {r['K']:6d} {r['epilogue']:>12s} {r['ms']:9.4f} {r['tflops']:8.1f}")
     if args.out:
         with open(args.out, "w") as f:
             json.dump(dict(gpu=gpu, launches=args.launches, rows=rows), f, indent=1)

@@ -632,15 +632,19 @@ def wg_gemm_kernel(num_items, rng, stages=4, ctas=1, **kw):
 
 
 def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, threads=2, addend=True,
-                            free_after_read=True, later_pass_waits_read=True):
+                            free_after_read=True, later_pass_waits_read=True, reduce=False, pass_waits_read=True):
     """gemm_bf16_kernel's epilogue: each of two consumer warpgroups (`threads` threads, thread 0 elected) writes a
     tile into its shared-memory staging in `passes` passes and the elected thread TMA-stores each pass. With an addend
     (C and / or bias) the producer loads the first pass's C into the staging on c_full once the tile's first
     min(num_kb, stages) k-blocks are issued, after waiting on c_free, which the elected thread arrives on at its first
     k-block once its previous stores have read the staging (`free_after_read`); later passes' C is loaded by the
     elected thread after the previous pass's store has read the staging (`later_pass_waits_read`). Without an addend
-    the elected thread waits for that read and the warpgroup meets at its named barrier before writing. TMA copies in
-    flight (operand and C loads landing, stores reading the staging) complete in any order."""
+    the elected thread waits for that read (`pass_waits_read`) and the warpgroup meets at its named barrier before
+    writing. `reduce`: the fp32 in-place accumulation, whose stores add the staging to D in the L2 (TMA reduce-add)
+    -- no addend is loaded, so that wait alone guards the staging, and each element of D must receive exactly one
+    add, from its own tile and pass. TMA copies in flight (operand and C loads landing, stores reading the staging)
+    complete in any order."""
+    addend = addend and not reduce
     W = 2
     copies = []                                           # async copies in flight
     full = [Mbar(1) for _ in range(stages)]
@@ -651,7 +655,7 @@ def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, thread
     stg = [[None] * threads for _ in range(W)]            # what each thread's part of a warpgroup's staging holds
     reading = [0] * W                                     # a warpgroup's stores that have not read the staging yet
     barr = [[0, 0] for _ in range(W)]                     # named barrier: arrivals, generation
-    state = dict(live=1 + W * threads, stored=[])
+    state = dict(live=1 + W * threads, stored=[], adds={})
 
     def load_c(w, t, p):
         def land():
@@ -667,6 +671,8 @@ def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, thread
                 raise Violation(f"store of tile {t} pass {p} read warpgroup {w}'s staging holding {stg[w]}")
             reading[w] -= 1
             state["stored"].append((w, t, p))
+            if reduce:                                    # the L2 adds what the staging held to D's (w, t, p) part
+                state["adds"][(w, t, p)] = state["adds"].get((w, t, p), 0) + 1
         reading[w] += 1
         copies.append(read)
 
@@ -735,7 +741,7 @@ def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, thread
                     if stg[w][i] != ("C", t, p):
                         raise Violation(f"thread {(w, i)} read C {stg[w][i]} for tile {t} pass {p}")
                 else:
-                    if elected:
+                    if elected and pass_waits_read:
                         yield (lambda: reading[w] == 0)
                     yield from barrier(w)
                 stg[w][i] = ("D", t, p)
@@ -765,6 +771,8 @@ def wg_gemm_epilogue_kernel(num_tiles, rng, num_kb=3, stages=2, passes=2, thread
     if res == "ok" and sorted(state["stored"]) != sorted((w, t, p) for w in range(W) for t in range(num_tiles)
                                                          for p in range(passes)):
         raise Violation(f"stores {sorted(state['stored'])}")
+    if res == "ok" and reduce and set(state["adds"].values()) != {1}:
+        raise Violation(f"adds into D {state['adds']}")
     return res
 
 
@@ -890,6 +898,10 @@ if __name__ == "__main__":
                          ("sm_90a dQ", wg_dq_kernel, dict(njb=8)),
                          ("sm_90a dK/dV", wg_dkdv_kernel, dict(n_iter=9)),
                          ("sm_90a cluster GEMM", wg_gemm_kernel, dict(num_items=13, ctas=2)),
+                         ("GEMM epilogue, fp32 reduce-add", wg_gemm_epilogue_kernel, dict(num_tiles=4, passes=4,
+                                                                                         reduce=True)),
+                         ("reduce-add without the read wait", wg_gemm_epilogue_kernel,
+                          dict(num_tiles=4, passes=4, reduce=True, pass_waits_read=False)),
                          ("cached-prefix fp8 widening", wg_cached_fp8_kernel, dict(npages=6)),
                          ("fp8, K freed before the softmax", wg_cached_fp8_kernel,
                           dict(npages=6, release_after_softmax=False)),
