@@ -609,21 +609,13 @@ void loss_micro(b200w_ctx* c, const int32_t* labels, int nseq) {
   reduce_sum_f32(c->nll, c->scal + 0, m.T, c->inv_n, s); ++c->launches;
 }
 
-// B200W_AR_MODE (debugging aid, same arithmetic in every mode):
-//   overlap (default)  per-matrix all-reduce on comm_stream as soon as the last micro-step's backward
-//                      has produced the gradient, concurrent with the rest of the backward
-//   sync               as overlap, but the host drains c->stream before enqueuing each all-reduce
-//   serial             per-matrix, but c->stream waits for each all-reduce: never concurrent with compute
-//   end                one all-reduce of the whole gradient after the backward
-// Overlap is the default for every rank count.
-enum class ArMode { Overlap, Sync, Serial, End };
-ArMode ar_mode() {
+// Gradient exchange schedule, same arithmetic in both:
+//   overlap (default)      per-matrix exchange on comm_stream as soon as the last micro-step's backward
+//                          has produced the gradient, concurrent with the rest of the backward
+//   B200W_AR_MODE=end      one exchange of the whole gradient after the backward
+bool exchange_at_end() {
   const char* m = getenv("B200W_AR_MODE");
-  const std::string v = m ? m : "";
-  if (v == "end") return ArMode::End;
-  if (v == "sync") return ArMode::Sync;
-  if (v == "serial") return ArMode::Serial;
-  return ArMode::Overlap;
+  return m && strcmp(m, "end") == 0;
 }
 
 void ensure_wire(b200w_ctx* c) {
@@ -639,9 +631,7 @@ void ensure_wire(b200w_ctx* c) {
 // reduce_scatter -> local AdamW on the shard -> all_gather, the wire bytes of one all-reduce).
 // precast: the wgrad GEMM that produced this range already wrote its bf16 wire copy (EpiExtra::d2).
 void exchange_one(b200w_ctx* c, size_t off, size_t count, bool precast = false) {
-  const ArMode mode = ar_mode();
   if (!precast) { cast_f32_to_bf16(c->g + off, c->gw + off, count, c->stream); ++c->launches; }
-  if (mode == ArMode::Sync) B200W_CUDA(cudaStreamSynchronize(c->stream));
   B200W_CUDA(cudaEventRecord(c->ev_grad, c->stream));
   B200W_CUDA(cudaStreamWaitEvent(c->comm_stream, c->ev_grad, 0));
   if (c->shard) {
@@ -653,10 +643,6 @@ void exchange_one(b200w_ctx* c, size_t off, size_t count, bool precast = false) 
                                 c->comm_stream));
   }
   ++c->launches;
-  if (mode == ArMode::Serial) {
-    B200W_CUDA(cudaEventRecord(c->ev_comm, c->comm_stream));
-    B200W_CUDA(cudaStreamWaitEvent(c->stream, c->ev_comm, 0));
-  }
 }
 void allreduce_range(b200w_ctx* c, size_t off, size_t count, bool precast = false) {
   if (count == 0) return;
@@ -999,7 +985,7 @@ void fwd_bwd_device(b200w_ctx* c, const int32_t* ids_dev, const int32_t* labels_
   B200W_CHECK(c->comm || nvalid > 0, "batch has no valid target token");
   if (c->comm) ensure_wire(c);
   set_global_count(c, nvalid);
-  allow_overlap = allow_overlap && ar_mode() != ArMode::End;
+  allow_overlap = allow_overlap && !exchange_at_end();
   B200W_CUDA(cudaMemsetAsync(c->scal, 0, 8 * sizeof(float), c->stream));
   B200W_CUDA(cudaMemsetAsync(c->g, 0, c->n_zero_prefix * sizeof(float), c->stream));
   const int n_micro = n_seqs / mb;

@@ -24,7 +24,6 @@
 
 namespace b200w {
 
-static int pick_n_fast(int M, int N, int K);
 static int pick_raster(int M, int N, int K, int tile_m, int tile_n);
 
 // Tile raster: `raster` = n_fast | (group << 1). Tiles run along the fast dimension (N when n_fast, else M), but
@@ -972,9 +971,7 @@ static int pick_n_fast(int M, int N, int K) {
 // K = 4096 bf16) would be re-fetched wave after wave. Bands of panels of ~13.5 MB in total are swept instead.
 // Cost model: the fast-dimension operand is read once, the other once per band.
 static int pick_raster(int M, int N, int K, int tile_m, int tile_n) {
-  static const bool grouped = [] { const char* v = getenv("B200W_GEMM_RASTER_BANDS"); return !(v && v[0] == '0'); }();
-  static const double budget = [] { const char* v = getenv("B200W_GEMM_BAND_MB"); return (v ? atof(v) : 13.5) * 1e6; }();
-  const double a = 2.0 * M * K, b = 2.0 * N * K, resident = 16e6, max_panel = 3.4e6;
+  const double a = 2.0 * M * K, b = 2.0 * N * K, resident = 16e6, max_panel = 3.4e6, budget = 13.5e6;
   const double pa = 2.0 * tile_m * K, pb = 2.0 * tile_n * K;
   auto bands = [&](double fast, double panel) -> double {
     if (fast <= resident) return 1.0;
@@ -983,8 +980,7 @@ static int pick_raster(int M, int N, int K, int tile_m, int tile_n) {
     return ceil(fast / per_band);
   };
   const double ga = bands(a, pa), gb = bands(b, pb);
-  static const bool square = [] { const char* v = getenv("B200W_GEMM_LONGK_SQUARE"); return !(v && v[0] == '0'); }();
-  if (grouped && square && ga < 0 && gb < 0) {
+  if (ga < 0 && gb < 0) {
     // long K: no band of panels can stay resident, but the tiles in flight march through K together and share
     // the k-slices they are on, so a wave costs (rows + columns of tiles it spans) panels: make the wave square
     // (8 tiles wide) instead of a long strip
@@ -992,7 +988,6 @@ static int pick_raster(int M, int N, int K, int tile_m, int tile_n) {
     const int fast_tiles = n_fast ? (N + tile_n - 1) / tile_n : (M + tile_m - 1) / tile_m;
     return n_fast | ((fast_tiles >= 12 ? 8 : 0) << 1);
   }
-  if (!grouped || (ga < 0 && gb < 0)) return pick_n_fast(M, N, K);
   const double cost_m = ga < 0 ? 1e30 : a + b * ga, cost_n = gb < 0 ? 1e30 : b + a * gb;
   const int n_fast = cost_n < cost_m ? 1 : 0;
   const double fast = n_fast ? b : a, panel = n_fast ? pb : pa;

@@ -246,7 +246,7 @@ struct Infer {
   std::vector<L> lp;
   size_t p_embed = 0, p_pos = 0, p_lnf_w = 0, p_lnf_b = 0, p_lm = 0;
   uint8_t* t_lm = nullptr;
-  bool tiled_valid = false, use_tiled = true;
+  bool tiled_valid = false;
   int qd = 0, kd = 0, qkvd = 0, ld_cat = 0;  // Falcon: ld_cat = qd + f, the [attention | mlp hidden] operand
   // decode activations [max_rows, *]
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
@@ -455,17 +455,17 @@ Infer* model(b200w_ctx* ctx) {
 void infer_destroy(void* p) { delete static_cast<Infer*>(p); }
 
 // one decode GEMM: out[n, N] = act(X W^T (+ bias) (+ C)); tiled: W's tile-major copy or, for a projection of an
-// int4 engine, its image (read whatever B200W_DECODE_TILED says)
+// int4 engine, its image; null: W is read row-major through TMA boxes
 void dgemm(Infer* m, cudaStream_t s, int n, const bf16* X, int ldx, size_t woff, int ldw, int N, int K,
            GemmDecodeOut o, const uint8_t* tiled, bool projection) {
   if (projection && m->w4) o.w4 = tiled;
-  else o.w_tiled = m->use_tiled ? tiled : nullptr;
+  else o.w_tiled = tiled;
   gemm_decode_ex(X, ldx, m->w + woff, ldw, o, m->ws, m->counters, n, N, K, s);
 }
 
 // (re)builds the tile-major copies after the weights changed
 void ensure_tiled(Infer* m, cudaStream_t s) {
-  if (!m->use_tiled || m->tiled_valid) return;
+  if (m->tiled_valid) return;
   const auto& a = m->a;
   const int d = a.hidden_size, f = a.intermediate_size, V = a.vocab_size, qd = m->qd, qkvd = m->qkvd;
   const bool falcon = a.family == B200W_FAMILY_FALCON, llama = a.family == B200W_FAMILY_LLAMA;
@@ -968,7 +968,6 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   auto m = std::make_unique<Infer>();
   m->a = *arch;
   m->max_batch = max_batch;
-  if (const char* e = getenv("B200W_DECODE_TILED")) m->use_tiled = atoi(e) != 0;
   build(m.get());
   const auto& a = m->a;
   const size_t B = max_batch;
