@@ -495,16 +495,21 @@ B200W_API int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, i
                                                 int nsplit, const int32_t* slots, const int32_t* starts,
                                                 const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
                                                 int H, int Hkv, int dh, float scale);
-/* The decode step's attention over an fp8 pool on its own (the engine's kernels: CUDA cores when H / Hkv < 4,
- * tensor cores otherwise). q [n, ld_q] (ld_q >= (H + 2 Hkv) dh, the step's QKV rows): row r's query head h at column
- * h * dh, at position positions[r] of cache slot slots[r]; it attends to positions [0, positions[r]] through
- * table [*, nsplit] (nsplit * 128 <= 8192). kcache / vcache / kscale / vscale as in
- * b200w_op_attention_fwd_cached_fp8. out [n, ld_out], head h at column h * dh. scale must be 1 / sqrt(dh). */
-B200W_API int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache,
-                                            const void* vcache, const float* kscale, const float* vscale,
-                                            int64_t cache_rows, const int32_t* table, int nsplit,
-                                            const int32_t* positions, const int32_t* slots, void* out, int ld_out,
-                                            int n, int H, int Hkv, int dh, float scale);
+/* The decode step's attention on its own, as b200w_infer_step runs it (CUDA cores when H / Hkv < 4, tensor cores
+ * otherwise). q [n, ld_q] (ld_q >= H dh): row r's query head h at column h * dh, at position positions[r] <
+ * max_ctx of cache slot slots[r]; it attends to positions [0, positions[r]] through table [*, nsplit]
+ * (max_ctx <= nsplit * 128 <= 8192). kv_dtype B200W_KV_BF16: kcache / vcache bf16 [cache_rows, Hkv * dh], as in
+ * b200w_op_attention_fwd_cached, scales unused; B200W_KV_FP8_E4M3: as in b200w_op_attention_fwd_cached_fp8.
+ * grouped != 0: rows of one slot at consecutive positions share their K/V reads, as in a speculative step.
+ * On the tensor cores the caller's part_o fp32 [n, H, nsplit, dh] and part_ml fp32 [n, H, nsplit, 2] (8-byte
+ * aligned) hold the per-block partials; on the CUDA cores they may be NULL. out [n, ld_out], head h at column
+ * h * dh. scale must be 1 / sqrt(dh). DEVICE pointers. */
+B200W_API int b200w_op_decode_attention(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache,
+                                        const void* vcache, const float* kscale, const float* vscale, int kv_dtype,
+                                        int64_t cache_rows, const int32_t* table, int nsplit,
+                                        const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n,
+                                        int H, int Hkv, int dh, int max_ctx, int grouped, float* part_o,
+                                        float* part_ml, float scale);
 /* The log-softmax of the token log-probability calls on bf16 logits [rows, ld] (vocab V % 8 == 0, ld % 8 == 0):
  * lse, target_lp (log-probability of targets[r]; targets NULL or an id outside [0, V): 0), token_lp (of the row
  * maximum) [rows] and top_ids / top_lp [rows, top_k], each nullable. DEVICE pointers. */

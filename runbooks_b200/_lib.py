@@ -167,8 +167,9 @@ PROTOTYPES = {
     "b200w_op_attention_fwd_cached_fp8": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp,
                                                     C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                                     C.c_int, C.c_int, C.c_float]),
-    "b200w_op_decode_attention_fp8": (C.c_int, [c_ctx, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, C.c_int, vp, vp,
-                                                vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
+    "b200w_op_decode_attention": (C.c_int, [c_ctx, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int, vp,
+                                            vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                            vp, vp, C.c_float]),
     "b200w_op_logprobs": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
     "b200w_op_sample": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
     "b200w_op_penalize": (C.c_int, [c_ctx, vp, C.c_int, C.c_int, C.c_int, vp, vp]),

@@ -974,33 +974,3 @@ void b200w::attention_fwd_cached(const KVLayer& c, const void* q, int ld_q, int 
          scale * 1.4426950408889634f, s);
   B200W_CUDA(cudaGetLastError());
 }
-
-void b200w::decode_attention_fp8(const void* q, int ld_q, const void* kcache, const void* vcache, const float* kscale,
-                                 const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
-                                 const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H,
-                                 int Hkv, int dh, float /*scale: 1 / sqrt(dh), as the engine uses*/, cudaStream_t s) {
-  B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
-  B200W_CHECK(n >= 1 && H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad batch / head configuration");
-  B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1 && nsplit * KV_PAGE <= 8192,
-              "bad KV cache");
-  B200W_CHECK(ld_q >= (H + 2 * Hkv) * dh && ld_out >= H * dh && kscale && vscale, "bad strides / scales");
-  // the engine's decode attention on one layer of a pool the caller owns; only the tensor-core partials are allocated
-  KVLayer c;
-  c.k = const_cast<void*>(kcache);
-  c.v = const_cast<void*>(vcache);
-  c.kscale = const_cast<float*>(kscale);
-  c.vscale = const_cast<float*>(vscale);
-  c.rows = cache_rows;
-  c.table = table;
-  c.nsplit = nsplit;
-  c.dtype = B200W_KV_FP8_E4M3;
-  const size_t n_part = decode_attention_partials(n, H, Hkv, dh, nsplit);   // part_o, then part_ml
-  DeviceScratch<float> part;
-  if (n_part) part = device_scratch<float>(n_part);
-  float* part_o = part.get();
-  decode_attention(c, static_cast<const bf16*>(q), ld_q, positions, slots, n, H, Hkv, dh, nsplit * KV_PAGE, part_o,
-                   reinterpret_cast<float2*>(part_o + n_part / (dh + 2) * dh), static_cast<bf16*>(out), ld_out, s,
-                   false);
-  B200W_CUDA(cudaGetLastError());
-  B200W_CUDA(cudaStreamSynchronize(s));   // the partials are freed on return
-}

@@ -8,6 +8,7 @@
 #include "../../include/b200w.h"
 #include "ctx_access.h"
 #include "host_common.h"
+#include "kv_cache.h"
 #include "ops.h"
 #include "w4.h"
 
@@ -278,14 +279,36 @@ int b200w_op_attention_fwd_cached_fp8(b200w_ctx* ctx, const void* q, int ld_q, i
   HOOK(attention_fwd_cached(c, q, ld_q, q_head_stride, slots, starts, lengths, out, ld_out, n_seqs, S, H, Hkv, dh, scale,
                             ctx_stream(ctx)));
 }
-int b200w_op_decode_attention_fp8(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
-                                  const float* kscale, const float* vscale, int64_t cache_rows, const int32_t* table,
-                                  int nsplit, const int32_t* positions, const int32_t* slots, void* out, int ld_out,
-                                  int n, int H, int Hkv, int dh, float scale) {
+int b200w_op_decode_attention(b200w_ctx* ctx, const void* q, int ld_q, const void* kcache, const void* vcache,
+                              const float* kscale, const float* vscale, int kv_dtype, int64_t cache_rows,
+                              const int32_t* table, int nsplit, const int32_t* positions, const int32_t* slots,
+                              void* out, int ld_out, int n, int H, int Hkv, int dh, int max_ctx, int grouped,
+                              float* part_o, float* part_ml, float scale) {
   HOOK(B200W_CHECK(scale > 0.f && fabsf(scale * sqrtf(static_cast<float>(dh)) - 1.f) <= 1e-6f,
                    "the decode attention's scale is 1 / sqrt(head_dim)");
-       decode_attention_fp8(q, ld_q, kcache, vcache, kscale, vscale, cache_rows, table, nsplit, positions, slots, out,
-                            ld_out, n, H, Hkv, dh, scale, ctx_stream(ctx)));
+       B200W_CHECK(dh == 64 || dh == 128, "head_dim must be 64 or 128");
+       B200W_CHECK(n >= 1 && H >= 1 && Hkv >= 1 && H % Hkv == 0, "bad batch / head configuration");
+       B200W_CHECK(kv_dtype == B200W_KV_BF16 || kv_dtype == B200W_KV_FP8_E4M3, "unknown KV cache dtype");
+       B200W_CHECK(kv_dtype == B200W_KV_BF16 || (kscale && vscale), "an fp8 cache needs both scale arrays");
+       B200W_CHECK(cache_rows >= KV_PAGE && cache_rows % KV_PAGE == 0 && nsplit >= 1 && max_ctx >= 1 &&
+                       max_ctx <= nsplit * KV_PAGE && nsplit * KV_PAGE <= 8192, "bad KV cache");
+       B200W_CHECK(ld_q >= H * dh && ld_out >= H * dh, "bad strides");
+       B200W_CHECK(!decode_attention_partials(n, H, Hkv, dh, nsplit) ||
+                       (part_o && part_ml && reinterpret_cast<uintptr_t>(part_ml) % 8 == 0),
+                   "the tensor-core decode attention needs part_o and 8-byte aligned part_ml");
+       KVLayer c;
+       c.k = const_cast<void*>(kcache);
+       c.v = const_cast<void*>(vcache);
+       c.kscale = const_cast<float*>(kscale);
+       c.vscale = const_cast<float*>(vscale);
+       c.rows = cache_rows;
+       c.table = table;
+       c.nsplit = nsplit;
+       c.dtype = kv_dtype;
+       const int launches = decode_attention(c, static_cast<const __nv_bfloat16*>(q), ld_q, positions, slots, n, H, Hkv,
+                                             dh, max_ctx, part_o, reinterpret_cast<float2*>(part_ml),
+                                             static_cast<__nv_bfloat16*>(out), ld_out, ctx_stream(ctx), grouped != 0);
+       ctx_launches(ctx) += launches - 1);   // HOOK counts one
 }
 int b200w_op_logprobs(b200w_ctx* ctx, const void* logits, int ld, int rows, int V, const int32_t* targets, int top_k,
                       float* lse, float* target_lp, float* token_lp, int32_t* top_ids, float* top_lp) {

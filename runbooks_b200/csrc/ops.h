@@ -116,12 +116,6 @@ struct KVLayer {
 void attention_fwd_cached(const KVLayer& c, const void* q, int ld_q, int q_head_stride, const int32_t* slots,
                           const int32_t* starts, const int32_t* lengths, void* out, int ld_out, int n_seqs, int S,
                           int H, int Hkv, int dh, float scale, cudaStream_t s);
-// The decode step's attention over one layer of an fp8 pool (the engine's kernels: CUDA cores when H / Hkv < 4,
-// tensor cores otherwise). q [n, ld_q]: row r's query heads at columns h * dh; positions / slots DEVICE int32 [n].
-void decode_attention_fp8(const void* q, int ld_q, const void* kcache, const void* vcache, const float* kscale,
-                          const float* vscale, int64_t cache_rows, const int32_t* table, int nsplit,
-                          const int32_t* positions, const int32_t* slots, void* out, int ld_out, int n, int H, int Hkv,
-                          int dh, float scale, cudaStream_t s);
 // The decode step's attention: the n new tokens (queries q [n, ld_q], head h at column h * dh; pos / slot DEVICE
 // [n]) over their cache slots -> out [n, ldo]. On the tensor cores when at least 4 query heads share a kv head, with
 // partials part_o [n, H, nsplit, dh] and part_ml [n, H, nsplit]; else on the CUDA cores (max_ctx sizes the score

@@ -1,5 +1,6 @@
-"""Element-wise error bounds for the fine-tune step's GEMM and attention kernels, against fp64 references computed
-from the same bf16 inputs. Plain torch: the checks run on whatever device the tensors live on.
+"""Element-wise error bounds for the fine-tune step's GEMM and attention kernels and the serving engine's paged
+attention, against fp64 references computed from the same bf16 inputs. Plain torch: the checks run on whatever
+device the tensors live on.
 
 A whole-tensor relative norm dilutes an error confined to one tile or one attention block by the square root of
 the number of such units, so every check here is element by element, and a failure names the worst work unit and
@@ -136,7 +137,38 @@ steps 2 and 3 a one-ulp change of powf(b2, step) moves the update by ~3e-5 of it
 bit. Unit: (grid-stride sweep, block) of 256 threads by 4 elements; the n % 4 scalar tail, which block 0 handles,
 is the unit ("tail", 0).
 Embedding backward: fp32 atomics in any order. An element whose token occurs c times is off by at most
-(c - 1) u32 sum |dout| over those rows; the forward is a gather, bit for bit."""
+(c - 1) u32 sum |dout| over those rows; the forward is a gather, bit for bit.
+
+Paged attention (kv_attention.cu), one decode row or cached-prefix query over L keys. The reference is fp64
+attention on the kernel's own inputs: the bf16 query, and K / V as the pool holds them -- bf16, or each e4m3 value
+times its fp32 scale, exact in fp64 (quantization belongs to the cache writers, pinned bit for bit elsewhere).
+s_t = scale q.k_t, A_t = scale |q|.|k_t|, x_t = |s_t - max s|, P normalised, O64 = P V. Every kernel forms
+O = sum w_t v_t / sum w_t with w_t = p_t (1 + r_t); to first order O - O64 = sum p_t r_t (v_t - O64), so a relative
+error of the weights costs (P o r)|V - O64|, and a rounding shared by numerator and denominator (a row's max, a
+block's merge weight) cancels. The fp32 sums of w v and w cost u32 (P|V|) and u32 |O64| per level of depth.
+CUDA cores (decode_attn). q scale and 1 / sqrtf(dh) round (2 u32), the dh products and sums of a score (dh u32 A_t),
+the fp8 K scale (u32 A_t), the subtraction of the max (u32 x_t) and __expf (_expf_rel(x_t)): r_t =
+(dh + 4 [+ 1]) u32 A_t + _expf_rel(x_t) + u32 x_t. The row sum is a thread's chain of ceil(L / 256) then an 8-level
+tree; 1 / sum and its product round once each: (ceil(L / 256) + 12) u32 |O64|. P is never rounded to bf16: each
+slice chains ceil(L / SLICES) fmas (fp8: one more for p vscale), then SLICES slices are summed: (ceil(L / SLICES) +
+SLICES + 1 [+ 1]) u32 (P|V|). There is no u16 (P|V|) term, which keeps this bound near the output's half ulp.
+Tensor cores (decode_attn_tc, decode_attn_merge). Scores by wgmma over dh: (KAPPA sqrt(dh) + 1) u32 A_t, as for the
+GEMM; scale_log2's three host roundings 4 u32 A_t [fp8: + u32 A_t]; the fma argument u32 x_t and ex2 E2. The bf16
+pool rounds P to bf16 and l sums the rounded values, so that rounding is a weight error: u16 joins r_t, and the
+term is u16 (P|V - O64|), not u16 (P|V|). The fp8 pool sums the unrounded p into l and rounds p vscale for P V, the
+training form: (u16 + u32) (P|V|). Merge: block s's weight 2^(m_s - M) meets up to ceil(ns / 4) + 1 ex2s and its
+argument's rounding, common to its numerator and denominator: omega = (ceil(ns / 4) + 2) E2 + u32 log2e max x_t
+joins r_t. P V of a block by wgmma over 128 keys: (KAPPA sqrt(128) + 1) u32 (P|V|); l of a block: 32 chained adds
+and 2 shuffles; the merge's chains 5 ceil(ns / 4) + 2; the division one more. With ETA16 and a flush floor
+L 2^-126 max|V| (ex2 and __expf flush subnormal results):
+    |O - O64| <= u16 |O64| + W16 ((P o r)|V - O64| + a_pv u32 (P|V|) [+ u16 (P|V|), fp8 tensor cores]
+                 + a_o u32 |O64| + floor) + ETA16,
+a_pv and a_o the depths above. Unit: (row, slot, query head); on the tensor cores also the 128-key block whose
+share sum_{t in s} p_t (v_t - O64) best explains the worst error vector.
+Cached prefill (attn_fwd_cached). The training forward's online softmax over 128-key pages (two m64n64 halves at
+dh 128): wgmma scores, ex2, fp32 l over unrounded P, P (fp8: p vscale) rounded to bf16 for P V, O and l rescaled by
+the same alpha. Its forward bound above applies with n = start + p + 1 keys, and the fp8 K and V scale products add
+2 u32 to f. Unit: (sequence, head, 128-query tile, 64-row half)."""
 import ctypes
 import ctypes.util
 import math
@@ -930,3 +962,187 @@ def adamw_fault(kind, state0, g, state, hp, grid, unit=None):
     for o, val in zip(out, vals):
         o[idx] = val.to(o.dtype)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Paged attention (kv_attention.cu): the serving engine's decode attention and its cached-prefix prefill
+# ---------------------------------------------------------------------------------------------------------------
+E2 = 8 * U32          # ex2.approx: 2 ulp, and as much again for the rounding of its fma argument near 0
+FLUSH = 2.0 ** -126   # ex2 and __expf flush results below the normal range to zero
+DECODE_SLICES = {64: 32, 128: 16}   # decode_attn's position slices: ATT_THREADS / (dh / 8)
+
+
+def decode_reference(q, K, V, scale):
+    """one decode row: q [H, dh]; K, V fp64 [L, Hkv, dh] (dequantized) -> fp64 scores s and A = scale |q|.|k|
+    [Hkv, G, L], P (normalised) [Hkv, G, L] and O [Hkv, G, dh]"""
+    H, dh = q.shape
+    Hkv = K.shape[1]
+    q = q.double().reshape(Hkv, H // Hkv, dh)
+    s = scale * torch.einsum("kgd,lkd->kgl", q, K)
+    A = scale * torch.einsum("kgd,lkd->kgl", q.abs(), K.abs())
+    P = torch.softmax(s, -1)
+    return s, A, P, torch.einsum("kgl,lkd->kgd", P, V)
+
+
+def decode_bound(path, fp8, s, A, P, O, V):
+    """the bound of the module docstring on one decode row's output [Hkv, G, dh]; path "cc" (decode_attn) or "tc"
+    (decode_attn_tc + decode_attn_merge)"""
+    L, Hkv, dh = V.shape
+    x = (s - s.amax(-1, keepdim=True)).abs()            # |score - row maximum|, natural units
+    PaV = torch.einsum("kgl,lkd->kgd", P, V.abs())
+    f8 = 1 if fp8 else 0
+    if path == "cc":
+        rho = (dh + 4 + f8) * U32 * A + _expf_rel(x) + U32 * x
+        a_pv = math.ceil(L / DECODE_SLICES[dh]) + DECODE_SLICES[dh] + 1 + f8
+        a_o = math.ceil(L / 256) + 12
+        extra = 0.0
+    else:
+        ns = math.ceil(L / 128)
+        n_m = 5 * math.ceil(ns / 4) + 2
+        omega = (math.ceil(ns / 4) + 2) * E2 + U32 * LOG2E * x.amax(-1, keepdim=True)
+        rho = (KAPPA * math.sqrt(dh) + 5 + f8) * U32 * A + E2 + U32 * x + omega + (0.0 if fp8 else U16)
+        a_pv = KAPPA * math.sqrt(128) + 2 + n_m + f8
+        a_o = 36 + n_m
+        extra = U16 * PaV if fp8 else 0.0
+    dev = torch.stack([torch.einsum("gl,lgd->gd", (P * rho)[k], (V[:, k, None] - O[k]).abs()) for k in range(Hkv)])
+    floor = L * FLUSH * V.abs().amax()
+    return U16 * O.abs() + W16 * (dev + extra + a_pv * U32 * PaV + a_o * U32 * O.abs() + floor) + ETA16
+
+
+def _explaining_block(err, P, V, O):
+    """the 128-key block whose share of the output, sum over its keys of P (v - O), best explains the error vector
+    err [dh] (the largest |<err, c_s>| / |c_s|)"""
+    L = P.shape[0]
+    c = torch.nn.functional.pad(P[:, None] * (V - O), (0, 0, 0, (-L) % 128)).view(-1, 128, V.shape[1]).sum(1)
+    score = (c @ err).abs() / c.norm(dim=-1).clamp_min(1e-300)
+    return int(score.argmax())
+
+
+def check_decode(out, q, pool, slots, pos, path, name=None):
+    """out [n, H * dh] of the decode attention of queries q [n, H, dh] (bf16) at positions pos[r] of cache slots
+    slots[r] of pool (paged_pool.Pool); path "cc" or "tc". Unit (row, slot, query head), and for "tc" the 128-key
+    block that best explains the worst error."""
+    n, H, dh = q.shape
+    scale = dh ** -0.5
+    res = Check(name or f"decode {path} {'fp8' if pool.fp8 else 'bf16'}",
+                ("row", "slot", "head") + (("block",) if path == "tc" else ()))
+    for r in range(n):
+        K, V = pool.kv(slots[r], pos[r] + 1)
+        s, A, P, O = decode_reference(q[r], K, V, scale)
+        got = out[r].double().view(O.shape)
+        ratio = _ratio((got - O).abs(), decode_bound(path, pool.fp8, s, A, P, O, V)).reshape(H, dh)
+        res.add(ratio, lambda i, r=r: (r, slots[r], i))
+        res.add_norms(got - O, O)
+    if path == "tc" and res.unit is not None:
+        r, slot, h = res.unit
+        K, V = pool.kv(slot, pos[r] + 1)
+        G, hk = H // pool.Hkv, h // (H // pool.Hkv)
+        _, _, P, O = decode_reference(q[r], K, V, scale)
+        err = out[r].double().view(H, dh)[h] - O[hk, h % G]
+        res.unit = (r, slot, h, _explaining_block(err, P[hk, h % G], V[:, hk], O[hk, h % G]))
+    return res
+
+
+def cached_reference(qh, kg, vg, start):
+    """one (sequence, head) of the cached-prefix prefill: queries qh [sfx, dh] at positions start + p over keys
+    kg, vg fp64 [L, dh]; the scale is applied by the caller -> P [sfx, L], O [sfx, dh]"""
+    L = kg.shape[0]
+    qpos = torch.arange(start, start + qh.shape[0], device=kg.device)
+    mask = torch.arange(L, device=kg.device)[None] <= qpos[:, None]
+    P = torch.softmax((qh.double() @ kg.T).masked_fill(~mask, -math.inf), -1)
+    return P, P @ vg
+
+
+def check_cached(out, q, q_head_stride, pool, slots, starts, lens, S, name=None):
+    """out [n * S, H * dh] of the cached-prefix attention of queries q [n * S, H * q_head_stride] (bf16; sequence b's
+    row p at position starts[b] + p of slot slots[b], its first dh columns used) over lens[b] positions.
+    Unit (sequence, head, 128-query tile, 64-row half)."""
+    dh, Hkv = pool.dh, pool.Hkv
+    H = out.shape[1] // dh
+    G, scale = H // Hkv, dh ** -0.5
+    res = Check(name or f"cached {'fp8' if pool.fp8 else 'bf16'}", ("sequence", "head", "tile", "half"))
+    for b, (slot, st, L) in enumerate(zip(slots, starts, lens)):
+        sfx = L - st
+        K, V = pool.kv(slot, L)
+        Q = q[b * S:b * S + sfx].view(sfx, H, q_head_stride)[:, :, :dh].double()
+        got = out[b * S:b * S + sfx].view(sfx, H, dh).double()
+        nk = torch.arange(st + 1, L + 1, device=K.device, dtype=torch.float64)[:, None]
+        for h in range(H):
+            kg, vg = K[:, h // G], V[:, h // G]
+            P, O = cached_reference(Q[:, h] * scale, kg, vg, st)
+            f = U32 * (nk + 2 * dh * scale * Q[:, h].norm(dim=-1, keepdim=True) * kg.norm(dim=-1).max() + 16 +
+                       (2 if pool.fp8 else 0))
+            bound = W16 * (U16 + f) * (P @ vg.abs()) + U16 * O.abs()
+            ratio = torch.nn.functional.pad(_ratio((got[:, h] - O).abs(), bound), (0, 0, 0, (-sfx) % 64))
+            res.add(ratio.view(-1, 64 * dh), lambda i, b=b, h=h: (b, h, i // 2, i % 2))
+            res.add_norms(got[:, h] - O, O)
+    return res
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Faults in the paged attention: one unit of the kernel's real output recomputed in fp64 with the fault applied
+# ---------------------------------------------------------------------------------------------------------------
+def decode_fault(kind, out, q, pool, slots, pos, row, head, block=0, other=None, extra=None, key=None):
+    """a copy of the decode output out [n, H * dh] with (row, query head) as a kernel broken this way leaves it:
+    own_key      the row's own key (at pos) left out
+    extra_key    one extra key: extra = (k, v) fp64 [Hkv, dh]
+    block        128-key block `block` dropped from the merge
+    table_shift  block `block` read through table entry block + 1 (both blocks written in full)
+    other_slot   the row's pages read through slot `other`'s table row
+    kv_head      the query head on the next kv head
+    kscale       key `key`'s K scale taken from key + 1 (fp8)"""
+    n, H, dh = q.shape
+    G = H // pool.Hkv
+    slot, L = slots[row], pos[row] + 1
+    K, V = pool.kv(slot, L)
+    hk = head // G
+    if kind == "own_key":
+        K, V = K[:-1], V[:-1]
+    elif kind == "extra_key":
+        K, V = torch.cat([K, extra[0][None]]), torch.cat([V, extra[1][None]])
+    elif kind == "block":
+        keep = (torch.arange(L, device=K.device) // 128) != block
+        K, V = K[keep], V[keep]
+    elif kind == "table_shift":
+        assert L >= 128 * (block + 1) and pool.lens[slot] >= 128 * (block + 2)
+        K2, V2 = pool.kv(slot, 128 * (block + 2))
+        blk = slice(128 * block, 128 * block + 128)
+        K[blk], V[blk] = K2[128 * block + 128:], V2[128 * block + 128:]
+    elif kind == "other_slot":
+        K, V = pool.kv(other, L)
+    elif kind == "kv_head":
+        hk = (hk + 1) % pool.Hkv
+    elif kind == "kscale":
+        k, ks, _, _ = pool.raw(slot, L + 1)
+        K[key, hk] = k[key, hk].double() * float(ks[key + 1, hk])
+    else:
+        raise ValueError(kind)
+    P = torch.softmax(dh ** -0.5 * (K[:, hk] @ q[row, head].double()), 0)
+    X = out.clone()
+    X[row, head * dh:(head + 1) * dh] = (P @ V[:, hk]).to(X.dtype)
+    return X
+
+
+def cached_fault(kind, out, q, q_head_stride, pool, slots, starts, lens, S, unit):
+    """a copy of the cached-prefix output with unit (sequence, head, tile, half) as a kernel broken this way leaves it:
+    diag     the diagonal mask off by one (query position t also sees key t + 1)
+    start0   the sequence's queries placed at starts[0] instead of its own start"""
+    b, h, tile, half = unit
+    dh, G = pool.dh, (out.shape[1] // pool.dh) // pool.Hkv
+    st, L = starts[b], lens[b]
+    p0, p1 = tile * 128 + half * 64, min(tile * 128 + half * 64 + 64, L - st)
+    K, V = pool.kv(slots[b], L)
+    kg, vg = K[:, h // G], V[:, h // G]
+    qh = q[b * S + p0:b * S + p1].view(p1 - p0, -1, q_head_stride)[:, h, :dh].double() * dh ** -0.5
+    if kind == "diag":
+        t = torch.arange(st + p0, st + p1, device=K.device)[:, None]
+        mask = torch.arange(L, device=K.device)[None] <= (t + 1).clamp_max(L - 1)
+        O = torch.softmax((qh @ kg.T).masked_fill(~mask, -math.inf), -1) @ vg
+    elif kind == "start0":
+        assert starts[0] + p1 <= L
+        O = cached_reference(qh, kg, vg, starts[0] + p0)[1]
+    else:
+        raise ValueError(kind)
+    X = out.clone()
+    X[b * S + p0:b * S + p1, h * dh:(h + 1) * dh] = O.to(X.dtype)
+    return X

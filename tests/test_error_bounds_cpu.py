@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import error_bounds as E
+from paged_pool import build_pool
 
 
 def _gemm(M, N, K, resid, seed):
@@ -391,3 +392,240 @@ def test_embed_bwd_check_allows_the_atomics_reordering_only():
     dtab[7, 3] += float(dout[0, 3])                    # one row counted twice
     r = E.check_embed_bwd(ids, dout, dtab)
     assert not r.ok and r.unit == (7,), str(r)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# paged attention (kv_attention.cu): fp32 restatements of the decode and cached-prefix kernels, in their order
+# ---------------------------------------------------------------------------------------------------------------
+def _f32(x):
+    """an fp64 result rounded once to fp32 (one fma, or one fp32 operation on exact inputs)"""
+    return x.double().float()
+
+
+def _scale_f32(dh):
+    """1.f / sqrtf(dh), as the host computes it"""
+    return torch.tensor(1.0, dtype=torch.float32) / torch.sqrt(torch.tensor(float(dh), dtype=torch.float32))
+
+
+def _log2e_scale(dh):
+    """the scale_log2 the tensor-core kernels get: fp32(1 / sqrtf(dh)) * fp32(log2 e) in fp32"""
+    return _scale_f32(dh) * torch.tensor(1.4426950408889634, dtype=torch.float32)
+
+
+def emulate_decode_cc(q, pool, slot, pos, round_p=False):
+    """decode_attn on one row: q [H, dh] bf16 -> out [H * dh] bf16. round_p: P rounded to bf16 before P V, which
+    the kernel does not do."""
+    H, dh = q.shape
+    L, idx = pos + 1, torch.arange(H) // (H // pool.Hkv)
+    k, ks, v, vs = (x[:, idx] for x in pool.raw(slot, L))   # per query head
+    sq = q.float() * _scale_f32(dh)
+    acc = torch.zeros(H, L)
+    for c in range(dh):   # the pairs' two fmas in dimension order
+        acc = _f32(acc.double() + k[:, :, c].T.double() * sq[:, c, None].double())
+    if pool.fp8:
+        acc = acc * ks.T
+    e = torch.exp((acc - acc.amax(-1, keepdim=True)).double()).float()
+    # the row sum: one strided chain per thread, then a tree over the 256 threads
+    t = torch.nn.functional.pad(e, (0, (-L) % 256)).view(H, -1, 256)
+    s = torch.zeros(H, 256)
+    for i in range(t.shape[1]):
+        s = s + t[:, i]
+    while s.shape[1] > 1:
+        s = s[:, :s.shape[1] // 2] + s[:, s.shape[1] // 2:]
+    inv = 1.0 / s[:, 0]
+    p = e.bfloat16().float() if round_p else e
+    if pool.fp8:
+        p = p * vs.T
+    SL = E.DECODE_SLICES[dh]
+    p = torch.nn.functional.pad(p, (0, (-L) % SL)).view(H, -1, SL)
+    vv = torch.nn.functional.pad(v, (0, 0, 0, 0, 0, (-L) % SL)).view(-1, SL, H, dh)
+    o = torch.zeros(SL, H, dh)
+    for i in range(p.shape[1]):   # slice sl: keys sl, sl + SL, ... in order
+        o = _f32(o.double() + p[:, i].T[:, :, None].double() * vv[i].double())
+    a = torch.zeros(H, dh)
+    for sl in range(SL):
+        a = a + o[sl]
+    return (a * inv[:, None]).bfloat16().reshape(-1)
+
+
+def emulate_decode_tc(q, pool, slot, pos):
+    """decode_attn_tc's 128-key blocks of one row, then decode_attn_merge: q [H, dh] bf16 -> out [H * dh] bf16"""
+    H, dh = q.shape
+    L, idx = pos + 1, torch.arange(H) // (H // pool.Hkv)
+    k, ks, v, vs = (x[:, idx] for x in pool.raw(slot, L))
+    c = _log2e_scale(dh)
+    parts = []
+    for k0 in range(0, L, 128):
+        kb, vb = k[k0:k0 + 128], v[k0:k0 + 128]
+        S = _f32(torch.einsum("hd,lhd->hl", q.double(), kb.double()))
+        if pool.fp8:
+            S = S * ks[k0:k0 + 128].T
+        m = S.amax(-1, keepdim=True) * c
+        p = torch.exp2(_f32(S.double() * c.double() - m.double()).double()).float()
+        if pool.fp8:
+            l = p.sum(-1)
+            pa = (p * vs[k0:k0 + 128].T).bfloat16()
+        else:
+            pa = p.bfloat16()
+            l = pa.float().sum(-1)
+        parts.append((m[:, 0], l, _f32(torch.einsum("hl,lhd->hd", pa.double(), vb.double()))))
+    M, num, den = torch.full((H,), -math.inf), torch.zeros(H, dh), torch.zeros(H)
+    for s0 in range(0, len(parts), 4):
+        chunk = parts[s0:s0 + 4]
+        Mn = torch.stack([M] + [m for m, _, _ in chunk]).amax(0)
+        resc = torch.exp2((M - Mn).double()).float()
+        num, den = num * resc[:, None], den * resc
+        for m, l, o in chunk:
+            w = torch.exp2((m - Mn).double()).float()
+            num = _f32(num.double() + w[:, None].double() * o.double())
+            den = _f32(den.double() + w.double() * l.double())
+        M = Mn
+    return (num / den[:, None]).bfloat16().reshape(-1)
+
+
+def emulate_cached(q, pool, slot, start, L):
+    """attn_fwd_cached on one sequence: queries q [sfx, H, dh] bf16 at positions start + p -> out [sfx, H, dh]
+    bf16: the online softmax over 128-key pages, in two 64-key halves at dh 128"""
+    sfx, H, dh = q.shape
+    KB = 128 if dh == 64 else 64
+    c = torch.tensor(dh ** -0.5, dtype=torch.float32) * torch.tensor(1.4426950408889634, dtype=torch.float32)
+    k, ks, v, vs = pool.raw(slot, L)
+    qpos = torch.arange(start, L)[:, None]
+    out = torch.empty(sfx, H, dh, dtype=torch.bfloat16)
+    nkeys = (L - 1) // 128 * 128 + 128
+    for h in range(H):
+        hk = h // (H // pool.Hkv)
+        m, l, o, pa = torch.full((sfx, 1), -math.inf), torch.zeros(sfx, 1), torch.zeros(sfx, dh), None
+        for u0 in range(0, nkeys, KB):
+            cols = torch.arange(u0, u0 + KB)
+            ok = cols < L
+            kb = torch.where(ok[:, None], k[cols.clamp_max(L - 1), hk], 0.0)
+            s = _f32(q[:, h].double() @ kb.double().T)
+            if pool.fp8:
+                s = s * torch.where(ok, ks[cols.clamp_max(L - 1), hk], 0.0)
+            s = s.masked_fill(cols[None] > qpos, -math.inf)
+            mn = torch.maximum(m, s.amax(-1, keepdim=True) * c)
+            alpha = torch.exp2((m - mn).double()).float()
+            p = torch.exp2(_f32(s.double() * c.double() - mn.double()).double()).float()
+            m, l = mn, l * alpha + p.sum(-1, keepdim=True)
+            if pool.fp8:
+                p = p * torch.where(ok, vs[cols.clamp_max(L - 1), hk], 0.0)
+            if pa is not None:
+                o = _f32(o.double() + pa.double() @ vprev.double()) * alpha
+            pa, vprev = p.bfloat16(), torch.where(ok[:, None], v[cols.clamp_max(L - 1), hk], 0.0)
+        o = _f32(o.double() + pa.double() @ vprev.double())
+        out[:, h] = (o * (1.0 / l)).bfloat16()
+    return out
+
+
+# (H, Hkv, dh) per path; slot lengths, slot 1 sharing slot 0's first page; rows (slot, position), slots out of order
+DECODE_SHAPES = {"cc": [(4, 2, 128), (3, 1, 64)], "tc": [(8, 2, 128), (8, 1, 64)]}
+SLOT_LENS = [700, 300, 129, 128, 127, 1]
+DECODE_ROWS = [(2, 128), (0, 699), (4, 126), (1, 299), (5, 0), (3, 127), (0, 500), (0, 650)]
+QZERO_ROW, DOMINANT_ROW = 6, 7   # all scores equal; one dominant key in block 2, not the first
+
+
+def _decode_case(H, Hkv, dh, fp8, seed):
+    g = _g(seed)
+    pool = build_pool(SLOT_LENS, Hkv, dh, fp8, g, share=[(1, 0)])
+    slots, pos = [s for s, _ in DECODE_ROWS], [p for _, p in DECODE_ROWS]
+    q = torch.randn(len(pos), H, dh, generator=g).bfloat16()
+    q[QZERO_ROW] = 0
+    K, _ = pool.kv(0, 301)
+    q[DOMINANT_ROW] = (0.5 * K[300, torch.arange(H) // (H // Hkv)]).bfloat16()
+    return pool, q, slots, pos
+
+
+def _emulate_decode(path, pool, q, slots, pos, **kw):
+    f = emulate_decode_cc if path == "cc" else emulate_decode_tc
+    return torch.stack([f(q[r], pool, slots[r], pos[r], **kw) for r in range(len(pos))])
+
+
+@pytest.mark.parametrize("fp8", [False, True], ids=["bf16", "fp8"])
+@pytest.mark.parametrize("path", ["cc", "tc"])
+def test_decode_check_passes_the_kernels_roundings(path, fp8):
+    for i, (H, Hkv, dh) in enumerate(DECODE_SHAPES[path]):
+        pool, q, slots, pos = _decode_case(H, Hkv, dh, fp8, seed=11 + i)
+        r = E.check_decode(_emulate_decode(path, pool, q, slots, pos), q, pool, slots, pos, path)
+        print(f"H {H} Hkv {Hkv} dh {dh}: {r}")
+        assert r.ok, str(r)
+
+
+def test_cuda_core_bound_flags_p_rounded_to_bf16():
+    """the CUDA-core kernel never rounds P: its bound has no u16 (P|V - O|) term, and an emulation that rounds P
+    to bf16 before P V breaks it"""
+    pool, q, slots, pos = _decode_case(4, 2, 128, False, seed=11)
+    r = E.check_decode(_emulate_decode("cc", pool, q, slots, pos, round_p=True), q, pool, slots, pos, "cc")
+    print(f"P rounded to bf16 on the CUDA cores: {r}")
+    assert not r.ok and r.ratio > 2, str(r)
+
+
+# fault, row, head, extra argument
+DECODE_FAULTS = [
+    ("own_key", 2, 1, {}),
+    ("extra_key", 0, 2, {}),
+    ("block", 1, 0, {"block": 3}),
+    ("table_shift", 6, 3, {"block": 1}),
+    ("other_slot", 3, 2, {"other": 0}),
+    ("kv_head", 2, 1, {}),
+    ("kscale", 5, 2, {}),
+]
+
+
+@pytest.mark.parametrize("fp8", [False, True], ids=["bf16", "fp8"])
+@pytest.mark.parametrize("path", ["cc", "tc"])
+@pytest.mark.parametrize("kind,row,head,kw", DECODE_FAULTS, ids=[f[0] for f in DECODE_FAULTS])
+def test_decode_check_flags_each_fault_in_its_unit(path, fp8, kind, row, head, kw):
+    if kind == "kscale" and not fp8:
+        pytest.skip("the bf16 pool has no scales")
+    H, Hkv, dh = DECODE_SHAPES[path][0]
+    pool, q, slots, pos = _decode_case(H, Hkv, dh, fp8, seed=11)
+    out = _emulate_decode(path, pool, q, slots, pos)
+    kw = dict(kw)
+    K, _ = pool.kv(slots[row], pos[row] + 1)
+    top = int((K[:, head // (H // Hkv)] @ q[row, head].double()).argmax())   # the key with the largest weight
+    if kind == "extra_key":   # as strong as that key, with a value of its own
+        kw["extra"] = (K[top], torch.randn(Hkv, dh, generator=_g(3)).bfloat16().double())
+    if kind == "kscale":
+        kw["key"] = top
+    bad = E.decode_fault(kind, out, q, pool, slots, pos, row, head, **kw)
+    r = E.check_decode(bad, q, pool, slots, pos, path)
+    print(f"{kind}: {r}")
+    assert not r.ok and r.unit[:3] == (row, slots[row], head), str(r)
+    if path == "tc" and kind in ("block", "table_shift"):
+        assert r.unit[3] == kw["block"], str(r)
+
+
+CACHED_SHAPES = [(4, 2, 128, 128), (2, 1, 64, 128)]   # H, Hkv, dh, query head stride
+CACHED_SEQS = [(0, 128, 129), (2, 256, 383), (1, 128, 255), (3, 256, 257)]   # slot, start, length (suffix + start)
+
+
+def _cached_case(H, Hkv, dh, hs, fp8, seed):
+    g = _g(seed)
+    lens = [0] * 4
+    for slot, _, L in CACHED_SEQS:
+        lens[slot] = L
+    pool = build_pool(lens, Hkv, dh, fp8, g, share=[(1, 0)])
+    S = 128 * max((L - st + 127) // 128 for _, st, L in CACHED_SEQS)
+    q = torch.zeros(len(CACHED_SEQS) * S, H * hs).bfloat16()
+    outs = torch.zeros(len(CACHED_SEQS) * S, H * dh).bfloat16()
+    for b, (slot, st, L) in enumerate(CACHED_SEQS):
+        qb = torch.randn(L - st, H, dh, generator=g).bfloat16()
+        q.view(-1, H, hs)[b * S:b * S + L - st, :, :dh] = qb
+        outs[b * S:b * S + L - st] = emulate_cached(qb, pool, slot, st, L).reshape(L - st, -1)
+    slots, starts, lens = ([s[i] for s in CACHED_SEQS] for i in range(3))
+    return pool, q, outs, slots, starts, lens, S
+
+
+@pytest.mark.parametrize("fp8", [False, True], ids=["bf16", "fp8"])
+def test_cached_check_passes_and_flags_each_fault(fp8):
+    for H, Hkv, dh, hs in CACHED_SHAPES:
+        pool, q, out, slots, starts, lens, S = _cached_case(H, Hkv, dh, hs, fp8, seed=21)
+        r = E.check_cached(out, q, hs, pool, slots, starts, lens, S)
+        print(f"H {H} Hkv {Hkv} dh {dh}: {r}")
+        assert r.ok, str(r)
+        for kind, unit in (("diag", (2, 1, 0, 1)), ("start0", (1, H - 1, 0, 1))):
+            bad = E.cached_fault(kind, out, q, hs, pool, slots, starts, lens, S, unit)
+            rb = E.check_cached(bad, q, hs, pool, slots, starts, lens, S)
+            print(f"  {kind}: {rb}")
+            assert not rb.ok and rb.unit == unit, str(rb)

@@ -1,20 +1,19 @@
 """The fp8 (e4m3) paged KV cache on the GPU: the writers bit for bit against torch's e4m3 quantization of the bf16
-engine's cache rows, the cached-prefix attention kernel against fp32 SDPA over the dequantized K/V, logits and
-teacher-forced greedy ids against the fp32 oracle with K/V quantized as the engine does, stale pages, the prefix-cache
-Generator and the page capacity on an fp8 pool."""
+engine's cache rows, the cached-prefix and decode attention kernels element by element against fp64 attention over
+the dequantized K/V, logits and teacher-forced greedy ids against the fp32 oracle with K/V quantized as the engine
+does, stale pages, the prefix-cache Generator and the page capacity on an fp8 pool."""
 import ctypes as C
 
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
-from kv_fp8_oracle import dequantize, patch, quantize
+from kv_fp8_oracle import patch, quantize
 from oracle import falcon_oracle as FO
 from oracle import llama_oracle as LO
 from oracle import opt_oracle as OO
+from paged_pool import cached_case, decode_case, permuted
 from test_paged_kv import MODELS, _arch, _llama_model_dir, _post
-from util import call, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -75,67 +74,14 @@ LAYOUTS = {   # H, Hkv, dh, query head stride
 SUFFIXES = (1, 127, 128, 129, 300)
 
 
-def _cached_kernel(engine, layout, start, seed):
-    H, Hkv, dh, hs = LAYOUTS[layout]
-    g = torch.Generator().manual_seed(seed)
-    n, S = len(SUFFIXES), 384
-    lens = [start + s for s in SUFFIXES]
-    npg = [(L + 127) // 128 for L in lens]
-    n_pages = sum(npg) + 5
-    order = torch.randperm(n_pages, generator=g).tolist()   # pages out of order, five never used
-    nsplit = max(npg)
-    table = torch.zeros(n, nsplit, dtype=torch.int32)
-    kd = Hkv * dh
-    rows = n_pages * 128
-    # wherever no key was written: the largest e4m3 value, under a large scale on even rows and a zero scale on odd
-    kc = torch.full((rows, kd), 0x7E, dtype=torch.uint8)
-    vc = torch.full((rows, kd), 0xFE, dtype=torch.uint8)
-    ksc = (torch.arange(rows) % 2 == 0).float()[:, None].repeat(1, Hkv) * 1e3
-    vsc = ksc.clone()
-    q = torch.zeros(n * S, H * hs).bfloat16()
-    refs = []
-    for b, L in enumerate(lens):
-        pages = [order.pop() for _ in range(npg[b])]
-        table[b, :npg[b]] = torch.tensor(pages, dtype=torch.int32) * 128
-        k = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        v = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        k[::37] = 0   # zero-scale keys among the real ones
-        kq, ks = quantize(k)
-        vq, vs = quantize(v)
-        for t in range(L):
-            row = pages[t // 128] * 128 + t % 128
-            kc[row], vc[row] = kq[t].reshape(kd), vq[t].reshape(kd)
-            ksc[row], vsc[row] = ks[t], vs[t]
-        sfx = L - start
-        qb = torch.randn(sfx, H, dh, generator=g).bfloat16()
-        q.view(n * S, H, hs)[b * S:b * S + sfx, :, :dh] = qb
-        mask = torch.arange(L)[None, :] <= torch.arange(start, L)[:, None]
-        kk = dequantize(kq, ks).repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        vv = dequantize(vq, vs).repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        ref = F.scaled_dot_product_attention(qb.float().transpose(0, 1), kk, vv, attn_mask=mask, scale=dh ** -0.5)
-        refs.append(ref.transpose(0, 1).reshape(sfx, H * dh))
-    dv = lambda t: t.cuda().contiguous()  # noqa: E731
-    kcd, vcd, kscd, vscd, qd, tbd = dv(kc), dv(vc), dv(ksc), dv(vsc), dv(q), dv(table)
-    slots = dv(torch.arange(n, dtype=torch.int32))
-    starts = dv(torch.full((n,), start, dtype=torch.int32))
-    lensd = dv(torch.tensor(lens, dtype=torch.int32))
-    outs = []
-    for _ in range(2):
-        out = torch.zeros(n * S, H * dh, device="cuda", dtype=torch.bfloat16)
-        call(engine, "b200w_op_attention_fwd_cached_fp8", qd, H * hs, hs, kcd, vcd, kscd, vscd, rows, tbd, nsplit,
-             slots, starts, lensd, out, H * dh, n, S, H, Hkv, dh, C.c_float(dh ** -0.5))
-        outs.append(out)
-    errs = [rel_err(outs[0][b * S:b * S + L - start].float(), refs[b]) for b, L in enumerate(lens)]
-    return errs, torch.equal(outs[0], outs[1]), bool(torch.isfinite(outs[0].float()).all())
-
-
 @pytest.mark.parametrize("start", [128, 384, 1024])
 @pytest.mark.parametrize("layout", list(LAYOUTS))
 def test_cached_attention_over_fp8_pages_matches_sdpa(engine, layout, start):
-    errs, same, finite = _cached_kernel(engine, layout, start, seed=start + len(layout))
-    print(f"{layout} start {start}: rel err " + " ".join(f"{s}:{e:.2e}" for s, e in zip(SUFFIXES, errs)))
-    assert max(errs) < 5e-3
-    assert same and finite
+    """element by element against fp64 attention over the dequantized K/V (tests/error_bounds.py check_cached)"""
+    H, Hkv, dh, hs = LAYOUTS[layout]
+    r, *_ = cached_case(engine, H, Hkv, dh, True, [start] * len(SUFFIXES), SUFFIXES, seed=start + len(layout),
+                        q_head_stride=hs)
+    assert r.ok, str(r)
 
 
 # ---- the decode attention kernels ----
@@ -148,64 +94,14 @@ DECODE_LAYOUTS = {   # H, Hkv, dh: CUDA cores when H / Hkv < 4, tensor cores oth
 DECODE_LENS = (1, 127, 128, 129, 300, 1000)
 
 
-def _decode_kernel(engine, layout, seed):
-    H, Hkv, dh = DECODE_LAYOUTS[layout]
-    g = torch.Generator().manual_seed(seed)
-    n = len(DECODE_LENS)
-    npg = [(L + 127) // 128 for L in DECODE_LENS]
-    n_pages = sum(npg) + 5
-    order = torch.randperm(n_pages, generator=g).tolist()   # pages out of order, five never used
-    nsplit = max(npg)
-    table = torch.zeros(n, nsplit, dtype=torch.int32)
-    kd, ld = Hkv * dh, (H + 2 * Hkv) * dh
-    rows = n_pages * 128
-    # wherever no key was written: the largest e4m3 value, under a large scale on even rows and a zero scale on odd
-    kc = torch.full((rows, kd), 0x7E, dtype=torch.uint8)
-    vc = torch.full((rows, kd), 0xFE, dtype=torch.uint8)
-    ksc = (torch.arange(rows) % 2 == 0).float()[:, None].repeat(1, Hkv) * 1e3
-    vsc = ksc.clone()
-    qkv = torch.zeros(n, ld).bfloat16()
-    refs = []
-    for b, L in enumerate(DECODE_LENS):
-        pages = [order.pop() for _ in range(npg[b])]
-        table[b, :npg[b]] = torch.tensor(pages, dtype=torch.int32) * 128
-        k = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        v = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        k[::37] = 0   # zero-scale keys among the real ones
-        v[5::41] = 0
-        kq, ks = quantize(k)
-        vq, vs = quantize(v)
-        for t in range(L):
-            row = pages[t // 128] * 128 + t % 128
-            kc[row], vc[row] = kq[t].reshape(kd), vq[t].reshape(kd)
-            ksc[row], vsc[row] = ks[t], vs[t]
-        qb = torch.randn(H, dh, generator=g).bfloat16()
-        qkv[b, :H * dh] = qb.reshape(-1)
-        qkv[b, H * dh:] = torch.randn(2 * kd, generator=g).bfloat16()   # this step's own k / v: not read
-        kk = dequantize(kq, ks).repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        vv = dequantize(vq, vs).repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        ref = F.scaled_dot_product_attention(qb.float()[:, None], kk, vv, scale=dh ** -0.5)
-        refs.append(ref.reshape(H * dh))
-    dv = lambda t: t.cuda().contiguous()  # noqa: E731
-    kcd, vcd, kscd, vscd, qd, tbd = dv(kc), dv(vc), dv(ksc), dv(vsc), dv(qkv), dv(table)
-    slots = dv(torch.arange(n, dtype=torch.int32))
-    pos = dv(torch.tensor(DECODE_LENS, dtype=torch.int32) - 1)
-    outs = []
-    for _ in range(2):
-        out = torch.zeros(n, H * dh, device="cuda", dtype=torch.bfloat16)
-        call(engine, "b200w_op_decode_attention_fp8", qd, ld, kcd, vcd, kscd, vscd, rows, tbd, nsplit, pos, slots,
-             out, H * dh, n, H, Hkv, dh, C.c_float(dh ** -0.5))
-        outs.append(out)
-    errs = [rel_err(outs[0][b].float(), refs[b]) for b in range(n)]
-    return errs, torch.equal(outs[0], outs[1]), bool(torch.isfinite(outs[0].float()).all())
-
-
 @pytest.mark.parametrize("layout", list(DECODE_LAYOUTS))
-def test_decode_attention_over_fp8_pages_matches_sdpa(engine, layout):
-    errs, same, finite = _decode_kernel(engine, layout, seed=len(layout))
-    print(f"{layout}: rel err " + " ".join(f"{L}:{e:.2e}" for L, e in zip(DECODE_LENS, errs)))
-    assert max(errs) < 5e-3
-    assert same and finite
+def test_decode_attention_over_fp8_pages_within_fp64_bounds(engine, layout):
+    """element by element against fp64 attention over the dequantized K/V (tests/error_bounds.py check_decode), rows
+    in permuted slots, the tensor-core partials NaN-filled, a launch repeated bit for bit"""
+    H, Hkv, dh = DECODE_LAYOUTS[layout]
+    rows = permuted([L - 1 for L in DECODE_LENS], len(layout))
+    r, *_ = decode_case(engine, H, Hkv, dh, True, rows, seed=len(layout), max_ctx=1024)
+    assert r.ok, str(r)
 
 
 # ---- end to end against the fp32 oracle ----

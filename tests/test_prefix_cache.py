@@ -1,16 +1,16 @@
-"""Prefix caching on the GPU: the cached-prefix attention kernel against fp32 SDPA, a prefill after a cached prefix
-against a cold prefill of the whole prompt for the four model layouts of test_paged_kv.py, the Generator and the
-HTTP server with the prefix index on, and the argument checks of the new calls."""
+"""Prefix caching on the GPU: the cached-prefix attention kernel element by element against fp64 attention, a
+prefill after a cached prefix against a cold prefill of the whole prompt for the four model layouts of
+test_paged_kv.py, the Generator and the HTTP server with the prefix index on, and the argument checks of the new
+calls."""
 import ctypes as C
 
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import llama_oracle as LO
+from paged_pool import cached_case
 from test_paged_kv import MODELS, _arch, _engine, _llama_model_dir, _post, _start
-from util import call, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -25,61 +25,15 @@ LAYOUTS = {   # H, Hkv, dh, query head stride
 SUFFIXES = (1, 127, 128, 129, 300)
 
 
-def _kernel(engine, layout, start, seed):
-    H, Hkv, dh, hs = LAYOUTS[layout]
-    g = torch.Generator().manual_seed(seed)
-    n, S = len(SUFFIXES), 384
-    lens = [start + s for s in SUFFIXES]
-    npg = [(L + 127) // 128 for L in lens]
-    n_pages = sum(npg) + 5
-    order = torch.randperm(n_pages, generator=g).tolist()   # pages out of order, five never used
-    nsplit = max(npg)
-    table = torch.zeros(n, nsplit, dtype=torch.int32)
-    kd = Hkv * dh
-    kc = torch.full((n_pages * 128, kd), 3.0e4).bfloat16()  # large finite values wherever no key was written
-    vc = torch.full((n_pages * 128, kd), -3.0e4).bfloat16()
-    q = torch.zeros(n * S, H * hs).bfloat16()
-    refs = []
-    for b, L in enumerate(lens):
-        pages = [order.pop() for _ in range(npg[b])]
-        table[b, :npg[b]] = torch.tensor(pages, dtype=torch.int32) * 128
-        k = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        v = torch.randn(L, Hkv, dh, generator=g).bfloat16()
-        for t in range(L):
-            row = pages[t // 128] * 128 + t % 128
-            kc[row] = k[t].reshape(kd)
-            vc[row] = v[t].reshape(kd)
-        sfx = L - start
-        qb = torch.randn(sfx, H, dh, generator=g).bfloat16()
-        q.view(n * S, H, hs)[b * S:b * S + sfx, :, :dh] = qb
-        mask = torch.arange(L)[None, :] <= torch.arange(start, L)[:, None]
-        kk = k.float().repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        vv = v.float().repeat_interleave(H // Hkv, 1).transpose(0, 1)
-        ref = F.scaled_dot_product_attention(qb.float().transpose(0, 1), kk, vv, attn_mask=mask, scale=dh ** -0.5)
-        refs.append(ref.transpose(0, 1).reshape(sfx, H * dh))
-    dv = lambda t: t.cuda().contiguous()  # noqa: E731
-    kcd, vcd, qd, tbd = dv(kc), dv(vc), dv(q), dv(table)
-    slots = dv(torch.arange(n, dtype=torch.int32))
-    starts = dv(torch.full((n,), start, dtype=torch.int32))
-    lensd = dv(torch.tensor(lens, dtype=torch.int32))
-    outs = []
-    for _ in range(2):
-        out = torch.zeros(n * S, H * dh, device="cuda", dtype=torch.bfloat16)
-        call(engine, "b200w_op_attention_fwd_cached", qd, H * hs, hs, kcd, vcd, n_pages * 128, tbd, nsplit, slots,
-             starts, lensd, out, H * dh, n, S, H, Hkv, dh, C.c_float(dh ** -0.5))
-        outs.append(out)
-    errs = [rel_err(outs[0][b * S:b * S + L - start].float(), refs[b]) for b, L in enumerate(lens)]
-    return errs, torch.equal(outs[0], outs[1]), bool(torch.isfinite(outs[0].float()).all())
-
-
 @pytest.mark.parametrize("start", [128, 384, 1024])
 @pytest.mark.parametrize("layout", list(LAYOUTS))
 def test_cached_attention_matches_sdpa(engine, layout, start):
-    errs, same, finite = _kernel(engine, layout, start, seed=start + len(layout))
-    print(f"{layout} start {start}: rel err " + " ".join(f"{s}:{e:.2e}" for s, e in zip(SUFFIXES, errs)))
-    assert max(errs) < 5e-3
-    assert same, "a re-run is not bit-identical"
-    assert finite
+    """every query row element by element against fp64 attention (tests/error_bounds.py check_cached); the five
+    sequences in permuted slots, a launch repeated bit for bit"""
+    H, Hkv, dh, hs = LAYOUTS[layout]
+    r, *_ = cached_case(engine, H, Hkv, dh, False, [start] * len(SUFFIXES), SUFFIXES, seed=start + len(layout),
+                        q_head_stride=hs)
+    assert r.ok, str(r)
 
 
 def _load(e, name, params):

@@ -84,9 +84,9 @@ def _fp8_cached_attention_without_scales(t, s):
                    table, x, 128, 1, 128, 1, 1, 128, 128 ** -0.5)
 
 
-def _fp8_decode_attention_scale(t, s):
-    return _result(t, "b200w_op_decode_attention_fp8", None, 0, None, None, None, None, 0, None, 0, None, None, None,
-                   0, 0, 0, 0, 128, 0.5)
+def _decode_attention_scale(t, s):
+    return _result(t, "b200w_op_decode_attention", None, 0, None, None, None, None, 1, 0, None, 0, None, None, None,
+                   0, 0, 0, 0, 128, 0, 0, None, None, 0.5)
 
 
 def _logprobs_top_k(t, s):
@@ -104,7 +104,7 @@ ROWS = {   # name: (call on the training and the serving context, status, start 
     "init_paged_pool_too_large": (_pool_too_large, ERR_OOM, "device memory exhausted"),
     "fp8_cached_attention_without_scales": (_fp8_cached_attention_without_scales, ERR_INVALID,
                                             "check failed: !f8 || (c.kscale && c.vscale)"),
-    "fp8_decode_attention_scale": (_fp8_decode_attention_scale, ERR_INVALID, "check failed: scale > 0.f"),
+    "decode_attention_scale": (_decode_attention_scale, ERR_INVALID, "check failed: scale > 0.f"),
     "logprobs_top_k": (_logprobs_top_k, ERR_INVALID, "check failed: k >= 0"),
 }
 
@@ -125,7 +125,7 @@ def test_status_and_message(contexts, row):
     assert err.startswith(start), err
 
 
-def test_contexts_work_after_refused_calls(lib_path):
+def test_contexts_work_after_every_refused_call(lib_path):
     """after every call above, the serving context's greedy tokens and the training context's loss equal those of
     fresh contexts; a training-side call between a step and b200w_infer_sample leaves the step's rows to sample"""
     t, s = _train_engine(), _engine(_arch("llama_mha_dh128"), max_batch=2)
