@@ -207,17 +207,20 @@ typedef struct {
   float rope_theta;
   int32_t tie_embeddings;    /* lm_head shares the embedding matrix (Falcon, OPT)               */
   int32_t max_positions;     /* OPT: max_position_embeddings (learned table, +2 rows); else 0   */
-  int32_t weight_dtype;      /* B200W_WEIGHTS_*; 0 = bf16                                       */
+  int32_t weight_dtype;      /* B200W_WEIGHTS_*: 0 bf16, 1 int4, 2 int8                         */
   int32_t reserved[2];       /* zero                                                            */
 } b200w_infer_arch;
 /* Weight formats of the Server engine. INT4_G64: every projection (not the embedding, positions, norms, biases or
  * lm_head) is stored as round-to-nearest symmetric int4 with one bf16 scale per row and 64 input columns:
  * s = bf16(max|x| / 7), q = clamp(rint(x / s), -8, 7), and the engine computes with W_hat = bf16(q * s) (DESIGN §3.5).
+ * INT8_G64: the same with int8, s = bf16(max|x| / 127) and q = clamp(rint(x / s), -128, 127); weight-only (the
+ * activations stay bf16, and there is no outlier decomposition as in bitsandbytes' LLM.int8).
  * The engine's output is then exactly the bf16 engine's loaded with W_hat. Every K of a projection (hidden_size,
  * intermediate_size, num_heads * head_dim) must be a multiple of 64, and a weight that is not finite makes
  * b200w_infer_load_tensor return B200W_ERR_INVALID. Any other value is B200W_ERR_INVALID. */
 #define B200W_WEIGHTS_BF16 0
 #define B200W_WEIGHTS_INT4_G64 1
+#define B200W_WEIGHTS_INT8_G64 2
 /* bf16 weights + a KV cache of max_batch slots x max_ctx positions. Parameter names are the HF
  * checkpoint keys of the family ("transformer.h.0.self_attention.query_key_value.weight", ...). */
 B200W_API int b200w_infer_init(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch);
@@ -228,7 +231,7 @@ B200W_API int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const vo
                             int64_t n_elements);
 B200W_API int b200w_infer_init_random(b200w_ctx* ctx, uint64_t seed, float std);
 /* The values the engine computes with for parameter `name` into host_bf16 (bf16 bit patterns, n_elements of them):
- * W_hat for a projection of an int4 engine, the stored bf16 values otherwise. */
+ * W_hat for a projection of an int4 or int8 engine, the stored bf16 values otherwise. */
 B200W_API int b200w_infer_read_weight(b200w_ctx* ctx, const char* name, void* host_bf16, int64_t n_elements);
 /* One decode step for n rows (HOST int32 arrays): row i feeds `tokens[i]` at `positions[i]` into
  * cache slot `slots[i]` (K/V appended there) and attends to that slot's positions [0, pos].
@@ -246,8 +249,8 @@ B200W_API int b200w_infer_prefill(b200w_ctx* ctx, const int32_t* tokens, const i
                         const int32_t* slots, int n_seqs, int padded_len, int32_t* next_tokens,
                         float* logits_out);
 B200W_API int64_t b200w_infer_device_bytes(b200w_ctx* ctx);
-/* Device bytes the weights are stored in: the bf16 parameters and, with B200W_WEIGHTS_INT4_G64, the projections'
- * int4 images. Not the decode step's tile-major copies, scratch, KV cache or activations (b200w_infer_device_bytes
+/* Device bytes the weights are stored in: the bf16 parameters and, with B200W_WEIGHTS_INT4_G64 / INT8_G64, the
+ * projections' int4 / int8 images. Not the decode step's tile-major copies, scratch, KV cache or activations (b200w_infer_device_bytes
  * counts everything). 0 before b200w_infer_init*. */
 B200W_API int64_t b200w_infer_weight_bytes(b200w_ctx* ctx);
 /* Paged KV cache: instead of max_batch x max_ctx positions per layer, K and V are pools of n_pages pages of
@@ -434,6 +437,12 @@ B200W_API int64_t b200w_w4_image_bytes(int N, int K);
 B200W_API int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int K);
 B200W_API int b200w_op_dequantize_w4(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K);
 B200W_API int b200w_op_gemm_decode_w4(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M,
+                                      int N, int K, int split_k);
+/* The int8 weight format (B200W_WEIGHTS_INT8_G64): the same four for its images. */
+B200W_API int64_t b200w_w8_image_bytes(int N, int K);
+B200W_API int b200w_op_quantize_w8(b200w_ctx* ctx, const void* W, void* image, int N, int K);
+B200W_API int b200w_op_dequantize_w8(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K);
+B200W_API int b200w_op_gemm_decode_w8(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M,
                                       int N, int K, int split_k);
 /* pos_table (NULL or bf16 [*, d]): row (t % S) + pos_offset is added (OPT learned positions).
  * embed_bwd: pad_id = nn.Embedding padding_idx (-1 none); dpos NULL or the position-table gradient. */

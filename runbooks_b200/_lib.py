@@ -140,6 +140,10 @@ PROTOTYPES = {
     "b200w_op_quantize_w4": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
     "b200w_op_dequantize_w4": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
     "b200w_op_gemm_decode_w4": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b200w_w8_image_bytes": (C.c_int64, [C.c_int, C.c_int]),
+    "b200w_op_quantize_w8": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
+    "b200w_op_dequantize_w8": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
+    "b200w_op_gemm_decode_w8": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_fwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_bwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int]),

@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200w.so")
 SOURCES = ["host_common.cu", "gemm.cu", "attention.cu", "ops.cu", "engine.cu", "kv_cache.cu", "kv_attention.cu",
-           "logits.cu", "w4.cu", "infer.cu", "op_hooks.cu"]
+           "logits.cu", "wq.cu", "infer.cu", "op_hooks.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

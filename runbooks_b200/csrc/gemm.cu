@@ -20,7 +20,7 @@
 #include "host_common.h"
 #include "ops.h"
 #include "ptx.cuh"
-#include "w4.h"
+#include "wq.h"
 
 namespace b200w {
 
@@ -608,15 +608,21 @@ __device__ __forceinline__ void decode_store(const DecodeEpi& e, int b, int n, f
 
 // Two CTAs per SM (~100 KB of pipeline each): the CTA of the NEXT kernel in the stream is resident and
 // streaming its weights (which depend on nothing) while this one finishes -- see the PDL notes below.
-// W4: the weights are int4 image tiles (w4.h) of W4_TILE_BYTES instead of 16 KB bf16 tiles, as many more stages as
-// fit the bf16 instance's ring, so that the W4 CTA never needs more shared memory than the bf16 one. Its stages are
-// laid out as all activation tiles (1024-byte aligned for the swizzle) followed by all weight tiles.
-template <int MPAD, bool W4 = false>
+// Quantized formats (F != bf16): the weights are image tiles (wq.h) of WQ<F>::TILE_BYTES instead of 16 KB bf16 tiles,
+// as many more stages as fit the bf16 instance's ring, so that the quantized CTA never needs more shared memory than
+// the bf16 one. Its stages are laid out as all activation tiles (1024-byte aligned for the swizzle) followed by all
+// weight tiles.
+template <WFmt F>
+constexpr int decode_w_bytes() {
+  if constexpr (F == WFmt::bf16) return A_STAGE_BYTES;
+  else return WQ<F>::TILE_BYTES;
+}
+template <int MPAD, WFmt F = WFmt::bf16>
 struct DecodeCfg {
   static constexpr int B_STAGE_BYTES = MPAD * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = (W4 ? W4_TILE_BYTES : A_STAGE_BYTES) + B_STAGE_BYTES;
-  static constexpr int STAGES = W4 ? DecodeCfg<MPAD>::STAGES * DecodeCfg<MPAD>::STAGE_BYTES / STAGE_BYTES
-                                   : (100 * 1024) / STAGE_BYTES;
+  static constexpr int STAGE_BYTES = decode_w_bytes<F>() + B_STAGE_BYTES;
+  static constexpr int STAGES = F != WFmt::bf16 ? DecodeCfg<MPAD>::STAGES * DecodeCfg<MPAD>::STAGE_BYTES / STAGE_BYTES
+                                                : (100 * 1024) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
@@ -628,15 +634,15 @@ struct DecodeCfg {
 // GEMMs of a decode step would otherwise expose is spent under the predecessor instead.
 // Warpgroup wg accumulates output features [64 wg, 64 wg + 64) of the 128-feature tile (the weights are
 // the wgmma A operand, the batch rows its N dimension) in registers.
-// W4: w_tiled is the int4 image (w4.h) and tmW is unused. Each consumer thread reads its fragment of a tile from
-// shared memory and dequantizes it in registers; the wgmma takes A from registers. Those registers must stay as they
-// are until the wgmma that reads them has retired, so they alternate between two sets. Everything else -- the k
+// Quantized formats: w_tiled is the image (wq.h) and tmW is unused. Each consumer thread reads its fragment of a tile
+// from shared memory and dequantizes it in registers; the wgmma takes A from registers. Those registers must stay as
+// they are until the wgmma that reads them has retired, so they alternate between two sets. Everything else -- the k
 // order, the split and its reduction, the epilogue -- is the bf16 instance's.
-template <int MPAD, bool W4>
+template <int MPAD, WFmt F>
 __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const CUtensorMap* tmX,
                                                  const uint8_t* __restrict__ w_tiled, const DecodeEpi& epi, int M,
                                                  int N, int K, int kb_per_split) {
-  using cfg = DecodeCfg<MPAD, W4>;
+  using cfg = DecodeCfg<MPAD, F>;
   constexpr int STAGES = cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -655,7 +661,7 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
 
   if (threadIdx.x == 0) {
     pdl_trigger();  // the next kernel's CTAs may take the SM slots that free up from now on
-    if constexpr (!W4) tma_prefetch_desc(tmW);
+    if constexpr (F == WFmt::bf16) tma_prefetch_desc(tmW);
     tma_prefetch_desc(tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
@@ -670,13 +676,13 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
       // pipeline fill with weight tiles only (independent of the predecessor) ...
       const int pre = nkb < STAGES ? nkb : STAGES;
       // w_tiled: the [128 x 64] weight tiles of this N tile are consecutive 16 KB shared-memory images
-      if constexpr (W4) {
-        const uint8_t* wt = w_tiled + static_cast<size_t>(blockIdx.x) * num_kb_total * W4_TILE_BYTES;
+      if constexpr (F != WFmt::bf16) {
+        constexpr int TILE = WQ<F>::TILE_BYTES;
+        const uint8_t* wt = w_tiled + static_cast<size_t>(blockIdx.x) * num_kb_total * TILE;
         uint8_t* sw = smem + STAGES * cfg::B_STAGE_BYTES;
         for (int i = 0; i < pre; ++i) {
           mbar_arrive_expect_tx(&full_bar[i], cfg::STAGE_BYTES);
-          bulk_load_1d(sw + i * W4_TILE_BYTES, wt + static_cast<size_t>(kb0 + i) * W4_TILE_BYTES, W4_TILE_BYTES,
-                       &full_bar[i]);
+          bulk_load_1d(sw + i * TILE, wt + static_cast<size_t>(kb0 + i) * TILE, TILE, &full_bar[i]);
         }
         pdl_wait();
         for (int i = 0; i < pre; ++i)
@@ -686,8 +692,7 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
         for (int kb = kb0 + pre; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase);
           mbar_arrive_expect_tx(&full_bar[stage], cfg::STAGE_BYTES);
-          bulk_load_1d(sw + stage * W4_TILE_BYTES, wt + static_cast<size_t>(kb) * W4_TILE_BYTES, W4_TILE_BYTES,
-                       &full_bar[stage]);
+          bulk_load_1d(sw + stage * TILE, wt + static_cast<size_t>(kb) * TILE, TILE, &full_bar[stage]);
           tma_load_2d(smem + stage * cfg::B_STAGE_BYTES, tmX, &full_bar[stage], kb * BLOCK_K, 0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -721,21 +726,22 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
     float acc[MPAD / 2];
     int stage = 0, prev = -1;
     uint32_t phase = 0;
-    if constexpr (W4) {
+    if constexpr (F != WFmt::bf16) {
       // one commit group per K = 16 step, whose 4 fragment registers alternate between fa and fb: wait_group 1 after
       // step k has retired step k - 1, so its set may be written again. A stage is free once the wait after the
       // next block's first step has retired this block's last.
+      using Q = WQ<F>;
       const uint32_t sw = smem_u32(smem + STAGES * cfg::B_STAGE_BYTES);
       uint32_t fa[4], fb[4];
       for (int i = 0; i < nkb; ++i) {
         mbar_wait(&full_bar[stage], phase);
-        uint32_t w[4], sc[2];
-        w4_load(sw + stage * W4_TILE_BYTES, threadIdx.x, w, sc);
+        uint32_t w[Q::WORDS], sc[2];
+        Q::load(sw + stage * Q::TILE_BYTES, threadIdx.x, w, sc);
         const uint64_t db = wg_desc(smem_u32(smem + stage * cfg::B_STAGE_BYTES), 16);
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WG_K; ++k) {
           uint32_t (&a)[4] = (k & 1) ? fb : fa;
-          w4_decode(w[k], sc, a);
+          Q::decode(w[Q::word(k, 0)], w[Q::word(k, 2)], sc, a);
           wg_fence();
           Wgmma<MPAD>::template rs<0>(acc, a, desc_add(db, k * WG_K * 2), (i | k) != 0);
           wg_commit();
@@ -815,18 +821,32 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2)
 gemm_decode_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
                    const uint8_t* __restrict__ w_tiled, const DecodeEpi epi, int M, int N, int K,
                    int kb_per_split) {
-  gemm_decode_body<MPAD, false>(&tmW, &tmX, w_tiled, epi, M, N, K, kb_per_split);
+  gemm_decode_body<MPAD, WFmt::bf16>(&tmW, &tmX, w_tiled, epi, M, N, K, kb_per_split);
 }
-// The int4 instances: two CTAs per SM as for bf16, but under an explicit cap of 112 registers (65536 / (2 x 288),
+// The quantized instances: two CTAs per SM as for bf16, but under an explicit cap of 112 registers (65536 / (2 x 288),
 // rounded down to the allocation granule) instead of __launch_bounds__' minimum of 2 blocks (the two cannot be
-// combined). Under the minimum ptxas serializes the MPAD 128 instance's wgmmas; under the cap it takes 106
-// registers, spills nothing and keeps them pipelined.
+// combined). Under the minimum ptxas serializes the MPAD 128 instance's wgmmas; under the cap it spills nothing and
+// keeps them pipelined.
 template <int MPAD>
 __global__ void __maxnreg__(112)
 gemm_decode_w4_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
                       const uint8_t* __restrict__ w_tiled, const DecodeEpi epi, int M, int N, int K,
                       int kb_per_split) {
-  gemm_decode_body<MPAD, true>(&tmW, &tmX, w_tiled, epi, M, N, K, kb_per_split);
+  gemm_decode_body<MPAD, WFmt::int4>(&tmW, &tmX, w_tiled, epi, M, N, K, kb_per_split);
+}
+template <int MPAD>
+__global__ void __maxnreg__(112)
+gemm_decode_w8_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
+                      const uint8_t* __restrict__ w_tiled, const DecodeEpi epi, int M, int N, int K,
+                      int kb_per_split) {
+  gemm_decode_body<MPAD, WFmt::int8>(&tmW, &tmX, w_tiled, epi, M, N, K, kb_per_split);
+}
+
+template <int MPAD, WFmt F>
+constexpr auto decode_kernel() {
+  if constexpr (F == WFmt::int4) return gemm_decode_w4_kernel<MPAD>;
+  else if constexpr (F == WFmt::int8) return gemm_decode_w8_kernel<MPAD>;
+  else return gemm_decode_kernel<MPAD>;
 }
 
 // How many clusters of `splits` decode-GEMM CTAs the device holds at once (per device, cached).
@@ -865,15 +885,15 @@ int max_active_decode_clusters(int splits) {
   return slot;
 }
 
-// W4: w_tiled is the int4 image and W is not read. The split is chosen from the bf16 instance's co-residency, so
-// both instances split alike and reduce in the same order.
-template <int MPAD, bool W4>
+// Quantized formats: w_tiled is the image and W is not read. The split is chosen from the bf16 instance's
+// co-residency, so every instance splits alike and reduces in the same order.
+template <int MPAD, WFmt F>
 void launch_decode(const void* X, int ldx, const void* W, int ldw, const void* w_tiled, const DecodeEpi& epi,
                    bool allow_split, int M, int N, int K, cudaStream_t stream) {
-  using cfg = DecodeCfg<MPAD, W4>;
+  using cfg = DecodeCfg<MPAD, F>;
   CUtensorMap tmX = make_tmap_bf16_2d(X, M, K, ldx, MPAD, BLOCK_K);
-  CUtensorMap tmW = W4 ? tmX : make_tmap_bf16_2d(W, N, K, ldw, BLOCK_M, BLOCK_K);
-  auto kern = W4 ? gemm_decode_w4_kernel<MPAD> : gemm_decode_kernel<MPAD>;
+  CUtensorMap tmW = F != WFmt::bf16 ? tmX : make_tmap_bf16_2d(W, N, K, ldw, BLOCK_M, BLOCK_K);
+  auto kern = decode_kernel<MPAD, F>();
   static PerDeviceOnce once;
   once.run([&] {
     B200W_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg::SMEM_BYTES));
@@ -1002,8 +1022,9 @@ void gemm_decode_ex(const void* X, int ldx, const void* W, int ldw, const GemmDe
                     unsigned* counters, int M, int N, int K, cudaStream_t stream) {
   B200W_CHECK(M >= 1 && M <= 128 && N > 0 && K > 0, "decode GEMM handles 1..128 rows");
   B200W_CHECK(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "TMA needs 16-byte aligned row strides");
-  B200W_CHECK(!o.w4 || (K % W4_GROUP == 0 && (reinterpret_cast<uintptr_t>(o.w4) & 15) == 0),
-              "int4 weights need K a multiple of 64 and a 16-byte aligned image");
+  B200W_CHECK(!o.wq || ((o.wq_fmt == WFmt::int4 || o.wq_fmt == WFmt::int8) && K % WQ_GROUP == 0 &&
+                         (reinterpret_cast<uintptr_t>(o.wq) & 15) == 0),
+              "quantized weights need a quantized format, K a multiple of 64 and a 16-byte aligned image");
   DecodeEpi e;
   e.out = static_cast<__nv_bfloat16*>(o.out);
   e.ldo = o.ldo;
@@ -1016,13 +1037,18 @@ void gemm_decode_ex(const void* X, int ldx, const void* W, int ldw, const GemmDe
   e.act = o.act;
   e.act_from = o.act_from;
   const bool allow_split = ws != nullptr && counters != nullptr;  // the scratch itself is no longer used
-  if (o.w4) {
-    if (M <= 32) launch_decode<32, true>(X, ldx, nullptr, ldw, o.w4, e, allow_split, M, N, K, stream);
-    else if (M <= 64) launch_decode<64, true>(X, ldx, nullptr, ldw, o.w4, e, allow_split, M, N, K, stream);
-    else launch_decode<128, true>(X, ldx, nullptr, ldw, o.w4, e, allow_split, M, N, K, stream);
-  } else if (M <= 32) launch_decode<32, false>(X, ldx, W, ldw, o.w_tiled, e, allow_split, M, N, K, stream);
-  else if (M <= 64) launch_decode<64, false>(X, ldx, W, ldw, o.w_tiled, e, allow_split, M, N, K, stream);
-  else launch_decode<128, false>(X, ldx, W, ldw, o.w_tiled, e, allow_split, M, N, K, stream);
+  auto run = [&](auto fmt, const void* Wr, const void* tiled) {
+    constexpr WFmt F = decltype(fmt)::value;
+    if (M <= 32) launch_decode<32, F>(X, ldx, Wr, ldw, tiled, e, allow_split, M, N, K, stream);
+    else if (M <= 64) launch_decode<64, F>(X, ldx, Wr, ldw, tiled, e, allow_split, M, N, K, stream);
+    else launch_decode<128, F>(X, ldx, Wr, ldw, tiled, e, allow_split, M, N, K, stream);
+  };
+  // (each launch_decode names only its own kernel, and the int4 instances are named first: the order the kernels
+  // enter the module in is the order they had before the int8 instances existed, and it can change the PTX the
+  // register-bound MPAD 128 int4 instance gets)
+  if (o.wq && o.wq_fmt == WFmt::int4) run(std::integral_constant<WFmt, WFmt::int4>{}, nullptr, o.wq);
+  else if (o.wq) run(std::integral_constant<WFmt, WFmt::int8>{}, nullptr, o.wq);
+  else run(std::integral_constant<WFmt, WFmt::bf16>{}, W, o.w_tiled);
 }
 void gemm_decode(const void* X, const void* W, void* out, const void* C, float* ws, unsigned* counters,
                  int M, int N, int K, int ldo, int act, cudaStream_t stream) {

@@ -34,7 +34,7 @@
 #include "kv_cache.h"
 #include "ops.h"
 #include "ptx.cuh"
-#include "w4.h"
+#include "wq.h"
 
 using namespace b200w;
 using bf16 = __nv_bfloat16;
@@ -204,13 +204,13 @@ struct IParam {
   size_t off;   // element offset of (0, 0) in the flat space of the bf16 engine (also what init_random's fill is keyed by)
   int64_t ld;   // row stride on the device (== cols unless the matrix is a column window of a fused one)
   char kind;    // 'p' projection, 'm' other matrix (embedding, positions, lm_head), 'n' norm weight (ones), 'b' bias (zeros)
-  size_t dev = 0;   // element offset in Infer::w (== off, except for int4 weights, where projections are not there)
-  int img = -1;     // int4 weights: the projection's image in Infer::imgs
+  size_t dev = 0;   // element offset in Infer::w (== off, except for quantized weights, where projections are not there)
+  int img = -1;     // quantized weights: the projection's image in Infer::imgs
 };
 
-// An int4 image (w4.h) of one fused projection matrix [N, K]: the matrix the decode GEMM reads in one launch. off: its
-// (0, 0) in the bf16 engine's flat space, which the matrix fills contiguously with row stride K.
-struct W4Image {
+// A quantized image (wq.h) of one fused projection matrix [N, K]: the matrix the decode GEMM reads in one launch. off:
+// its (0, 0) in the bf16 engine's flat space, which the matrix fills contiguously with row stride K.
+struct QImage {
   size_t off;
   int N, K;
   uint8_t* p;
@@ -226,18 +226,19 @@ struct Infer {
   std::unordered_map<std::string, int> index;
   size_t n_elems = 0;   // the bf16 engine's flat space
   DeviceMemory mem;   // the device buffers below, the KV cache's included (b200w_infer_device_bytes)
-  // int4 weights (B200W_WEIGHTS_INT4_G64): the projections live in imgs, w holds only the other parameters, and one
-  // bf16 scratch of the largest image's N * K elements serves the prefill's dequantized W_hat and the loads
-  bool w4 = false;
-  std::vector<W4Image> imgs;
-  bf16* w4_scratch = nullptr;
-  int* w4_bad = nullptr;   // set by the quantizer when a weight is not finite
+  // quantized weights (wq != bf16: B200W_WEIGHTS_INT4_G64 / INT8_G64): the projections live in imgs, w holds only the
+  // other parameters, and one bf16 scratch of the largest image's N * K elements serves the prefill's dequantized
+  // W_hat and the loads
+  WFmt wq = WFmt::bf16;
+  std::vector<QImage> imgs;
+  bf16* wq_scratch = nullptr;
+  int* wq_bad = nullptr;   // set by the quantizer when a weight is not finite
   size_t weight_bytes = 0; // w and the images (b200w_infer_weight_bytes)
   bf16* w = nullptr;
   // per layer: norm parameters, the projections (offsets of their (0,0) element), biases (OPT), and the decode-time
   // copy of each projection as consecutive 16 KB swizzled tile images (gemm.cu retile_weights): a decode GEMM CTA
-  // streams one contiguous HBM region instead of 128-byte row segments (null until ensure_tiled makes them). With int4
-  // weights the t_* are the layer's int4 images instead (Falcon: t_qkv holds [q k v | dense_h_to_4h], t_o
+  // streams one contiguous HBM region instead of 128-byte row segments (null until ensure_tiled makes them). With
+  // quantized weights the t_* are the layer's images instead (Falcon: t_qkv holds [q k v | dense_h_to_4h], t_o
   // [dense | dense_4h_to_h]), and the ln / bias offsets are into the compacted w.
   struct L {
     size_t ln1_w, ln1_b, ln2_w, ln2_b, wqkv, bqkv, wo, bo, w1, b1, w2, b2;
@@ -387,15 +388,15 @@ void build(Infer* m) {
   for (IParam& p : m->params) p.dev = p.off;
 }
 
-// Int4 weights: one image per matrix a decode GEMM reads (ensure_tiled's list, lm_head excepted) in the layer's t_*,
+// Quantized weights: one image per matrix a decode GEMM reads (ensure_tiled's list, lm_head excepted) in the layer's t_*,
 // every projection tied to its image, the other parameters packed into w in their order (so OPT's q / k / v biases
 // stay adjacent) and the offsets kept in Infer remapped to w. -> the elements w needs.
-size_t layout_w4(Infer* m, cudaStream_t s) {
+size_t layout_wq(Infer* m, cudaStream_t s) {
   const auto& a = m->a;
   const int d = a.hidden_size, f = a.intermediate_size, qd = m->qd, qkvd = m->qkvd;
   auto image = [&](uint8_t*& t, size_t off, int N, int K) {
-    t = m->mem.alloc<uint8_t>(w4_image_bytes(N, K));
-    w4_clear(t, N, K, s);   // (every later use of the images is on the same stream)
+    t = m->mem.alloc<uint8_t>(wq_image_bytes(m->wq, N, K));
+    wq_clear(m->wq, t, N, K, s);   // (every later use of the images is on the same stream)
     m->imgs.push_back({off, N, K, t});
   };
   for (auto& x : m->lp) {
@@ -414,7 +415,7 @@ size_t layout_w4(Infer* m, cudaStream_t s) {
   for (IParam& p : m->params) {
     if (p.kind == 'p') {
       for (size_t i = 0; i < m->imgs.size(); ++i) {
-        const W4Image& g = m->imgs[i];
+        const QImage& g = m->imgs[i];
         if (p.off >= g.off && p.off < g.off + static_cast<size_t>(g.N) * g.K) p.img = static_cast<int>(i);
       }
       continue;
@@ -430,9 +431,9 @@ size_t layout_w4(Infer* m, cudaStream_t s) {
     for (size_t* o : {&x.ln1_w, &x.ln1_b, &x.ln2_w, &x.ln2_b, &x.bqkv, &x.bo, &x.b1, &x.b2}) remap(*o);
   for (size_t* o : {&m->p_embed, &m->p_pos, &m->p_lnf_w, &m->p_lnf_b, &m->p_lm}) remap(*o);
   size_t scratch = 0;
-  for (const W4Image& g : m->imgs) scratch = std::max(scratch, static_cast<size_t>(g.N) * g.K);
-  m->w4_scratch = m->mem.alloc<bf16>(scratch);
-  m->w4_bad = m->mem.alloc<int>(1);
+  for (const QImage& g : m->imgs) scratch = std::max(scratch, static_cast<size_t>(g.N) * g.K);
+  m->wq_scratch = m->mem.alloc<bf16>(scratch);
+  m->wq_bad = m->mem.alloc<int>(1);
   return n;
 }
 
@@ -454,12 +455,16 @@ Infer* model(b200w_ctx* ctx) {
 
 void infer_destroy(void* p) { delete static_cast<Infer*>(p); }
 
-// one decode GEMM: out[n, N] = act(X W^T (+ bias) (+ C)); tiled: W's tile-major copy or, for a projection of an
-// int4 engine, its image; null: W is read row-major through TMA boxes
+// one decode GEMM: out[n, N] = act(X W^T (+ bias) (+ C)); tiled: W's tile-major copy or, for a projection of a
+// quantized engine, its image; null: W is read row-major through TMA boxes
 void dgemm(Infer* m, cudaStream_t s, int n, const bf16* X, int ldx, size_t woff, int ldw, int N, int K,
            GemmDecodeOut o, const uint8_t* tiled, bool projection) {
-  if (projection && m->w4) o.w4 = tiled;
-  else o.w_tiled = tiled;
+  if (projection && m->wq != WFmt::bf16) {
+    o.wq = tiled;
+    o.wq_fmt = m->wq;
+  } else {
+    o.w_tiled = tiled;
+  }
   gemm_decode_ex(X, ldx, m->w + woff, ldw, o, m->ws, m->counters, n, N, K, s);
 }
 
@@ -473,7 +478,7 @@ void ensure_tiled(Infer* m, cudaStream_t s) {
     if (!dst) dst = m->mem.alloc<uint8_t>(retiled_bytes(N, K));
     retile_weights(m->w + woff, ldw, dst, N, K, s);
   };
-  for (int l = 0; l < a.num_layers && !m->w4; ++l) {   // (an int4 engine's projections are images already)
+  for (int l = 0; l < a.num_layers && m->wq == WFmt::bf16; ++l) {   // (a quantized engine's projections are images)
     auto& p = m->lp[l];
     if (falcon) {
       make(p.t_qkv, p.wqkv, d, qkvd + f, d);               // [q k v | dense_h_to_4h]
@@ -511,15 +516,15 @@ void launch(Pass& p, void (*kern)(KArgs...), dim3 grid, dim3 block, Args&&... ar
   else kern<<<grid, block, 0, p.s>>>(std::forward<Args>(args)...);
 }
 
-// The int4 image of the projection whose tile-major pointer is `t`.
-const W4Image& image_of(const Infer* m, const uint8_t* t) {
-  for (const W4Image& g : m->imgs)
+// The quantized image of the projection whose tile-major pointer is `t`.
+const QImage& image_of(const Infer* m, const uint8_t* t) {
+  for (const QImage& g : m->imgs)
     if (g.p == t) return g;
-  throw Error("no int4 image for a projection");
+  throw Error("no quantized image for a projection");
 }
 
 // out [rows, N] (row stride ldo) = act(X W^T + bias) (+ C, same stride); tiled: the step's tile-major copy of W, or
-// with int4 weights W's image, of which W is rows [img_row0, img_row0 + N). The prefill of an int4 engine first
+// with quantized weights W's image, of which W is rows [img_row0, img_row0 + N). The prefill of a quantized engine first
 // writes W_hat (row stride ldw) into the scratch and runs the same GEMM on it.
 void gemm(Pass& p, const bf16* X, int ldx, size_t w, int ldw, int N, int K, bf16* out, int ldo, const uint8_t* tiled,
           const bf16* C = nullptr, const bf16* bias = nullptr, Act act = Act::none, int img_row0 = 0) {
@@ -530,10 +535,10 @@ void gemm(Pass& p, const bf16* X, int ldx, size_t w, int ldw, int N, int K, bf16
     dgemm(p.m, p.s, p.rows, X, ldx, w, ldw, N, K, o, tiled, true);
   } else {
     const bf16* W = p.m->w + w;
-    if (p.m->w4) {
-      const W4Image& g = image_of(p.m, tiled);
-      w4_dequantize(g.p, g.N, g.K, img_row0, N, p.m->w4_scratch, ldw, p.s); ++p.nl;
-      W = p.m->w4_scratch;
+    if (p.m->wq != WFmt::bf16) {
+      const QImage& g = image_of(p.m, tiled);
+      wq_dequantize(p.m->wq, g.p, g.N, g.K, img_row0, N, p.m->wq_scratch, ldw, p.s); ++p.nl;
+      W = p.m->wq_scratch;
     }
     gemm_bf16_ex(X, false, ldx, W, false, ldw, out, C, false, ldo, p.rows, N, K, 0, bias,
                  act == Act::relu ? 1 : 0, p.s);
@@ -949,12 +954,14 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
               "sizes must be multiples of 8");
   B200W_CHECK(arch->hidden_size <= 256 * 8 * LN_MAXP, "hidden_size too large for the decode LayerNorm");
   B200W_CHECK(arch->max_ctx >= 1 && arch->max_ctx <= 8192, "max_ctx must be in 1..8192");
-  B200W_CHECK(arch->weight_dtype == B200W_WEIGHTS_BF16 || arch->weight_dtype == B200W_WEIGHTS_INT4_G64,
+  B200W_CHECK(arch->weight_dtype == B200W_WEIGHTS_BF16 || arch->weight_dtype == B200W_WEIGHTS_INT4_G64 ||
+                  arch->weight_dtype == B200W_WEIGHTS_INT8_G64,
               "unknown weight dtype");
-  if (arch->weight_dtype == B200W_WEIGHTS_INT4_G64)
-    B200W_CHECK(arch->hidden_size % W4_GROUP == 0 && arch->intermediate_size % W4_GROUP == 0 &&
-                    (arch->num_heads * arch->head_dim) % W4_GROUP == 0,
-                "int4 weights: every K of a projection (hidden, intermediate, heads * head_dim) must be a multiple of 64");
+  if (arch->weight_dtype != B200W_WEIGHTS_BF16)
+    B200W_CHECK(arch->hidden_size % WQ_GROUP == 0 && arch->intermediate_size % WQ_GROUP == 0 &&
+                    (arch->num_heads * arch->head_dim) % WQ_GROUP == 0,
+                "quantized weights: every K of a projection (hidden, intermediate, heads * head_dim) must be a multiple "
+                "of 64");
   if (arch->family == B200W_FAMILY_OPT)
     B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
   const int64_t ctx_rounded = cdiv(arch->max_ctx, KV_PAGE) * static_cast<int64_t>(KV_PAGE);
@@ -971,11 +978,11 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
   build(m.get());
   const auto& a = m->a;
   const size_t B = max_batch;
-  m->w4 = a.weight_dtype == B200W_WEIGHTS_INT4_G64;
-  const size_t w_elems = m->w4 ? layout_w4(m.get(), ctx_stream(ctx)) : m->n_elems;
+  m->wq = static_cast<WFmt>(a.weight_dtype);
+  const size_t w_elems = m->wq != WFmt::bf16 ? layout_wq(m.get(), ctx_stream(ctx)) : m->n_elems;
   m->w = m->mem.alloc<bf16>(w_elems);
   m->weight_bytes = w_elems * sizeof(bf16);
-  for (const W4Image& g : m->imgs) m->weight_bytes += w4_image_bytes(g.N, g.K);
+  for (const QImage& g : m->imgs) m->weight_bytes += wq_image_bytes(m->wq, g.N, g.K);
   m->kv.init(kv_dtype, n_pages, max_batch, a.max_ctx, a.num_layers, a.num_kv_heads, a.head_dim, m->mem);
   if (m->kv.paged) {
     // the whole prefill workspace now, so that the pool cannot leave too little memory for it later
@@ -1144,33 +1151,32 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     bf16* dst = m->w + p.dev;
     DeviceScratch<float> tmp32;
     DeviceScratch<bf16> tmp16;
-    // the dense bf16 source: the host buffer, or the f32 values cast on the device -- for an int4 projection straight
+    // the dense bf16 source: the host buffer, or the f32 values cast on the device -- for a quantized projection straight
     // into the scratch it is quantized from
     const void* src16 = host;
     cudaMemcpyKind kind = cudaMemcpyHostToDevice;
     if (dtype == B200W_F32) {
       tmp32 = device_scratch<float>(n);
       if (p.img < 0) tmp16 = device_scratch<bf16>(n);
-      bf16* cast = p.img >= 0 ? m->w4_scratch : tmp16.get();
+      bf16* cast = p.img >= 0 ? m->wq_scratch : tmp16.get();
       B200W_CUDA(cudaMemcpyAsync(tmp32.get(), host, n * 4, cudaMemcpyHostToDevice, s));
       cast_f32_to_bf16(tmp32.get(), cast, n, s);
       src16 = cast;
       kind = cudaMemcpyDeviceToDevice;
     }
     if (p.img >= 0) {
-      // an int4 projection: the bf16 values through the scratch, quantized into the image rows and columns it owns
-      const W4Image& g = m->imgs[p.img];
+      // a quantized projection: the bf16 values through the scratch, quantized into the image rows and columns it owns
+      const QImage& g = m->imgs[p.img];
       const size_t rel = p.off - g.off;
       if (dtype == B200W_BF16)
-        B200W_CUDA(cudaMemcpyAsync(m->w4_scratch, host, n * sizeof(bf16), cudaMemcpyHostToDevice, s));
-      B200W_CUDA(cudaMemsetAsync(m->w4_bad, 0, sizeof(int), s));
-      w4_quantize(m->w4_scratch, static_cast<int>(p.cols), static_cast<int>(p.rows),
-                  static_cast<int>(p.cols), g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(rel % g.K),
-                  m->w4_bad, s);
+        B200W_CUDA(cudaMemcpyAsync(m->wq_scratch, host, n * sizeof(bf16), cudaMemcpyHostToDevice, s));
+      B200W_CUDA(cudaMemsetAsync(m->wq_bad, 0, sizeof(int), s));
+      wq_quantize(m->wq, m->wq_scratch, static_cast<int>(p.cols), static_cast<int>(p.rows), static_cast<int>(p.cols),
+                  g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(rel % g.K), m->wq_bad, s);
       int bad = 0;
-      B200W_CUDA(cudaMemcpyAsync(&bad, m->w4_bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+      B200W_CUDA(cudaMemcpyAsync(&bad, m->wq_bad, sizeof(int), cudaMemcpyDeviceToHost, s));
       B200W_CUDA(cudaStreamSynchronize(s));
-      if (bad) throw InvalidArgument(std::string("check failed: non-finite value in int4 weight ") + name);
+      if (bad) throw InvalidArgument(std::string("check failed: non-finite value in quantized weight ") + name);
       return;
     }
     // rows of `cols` elements into rows of stride ld (ld == cols: one contiguous copy)
@@ -1192,10 +1198,10 @@ int b200w_infer_read_weight(b200w_ctx* ctx, const char* name, void* host_bf16, i
     const bf16* src = m->w + p.dev;
     int64_t ld = p.ld;
     if (p.img >= 0) {   // W_hat: the image rows the projection owns, dequantized whole, then its columns
-      const W4Image& g = m->imgs[p.img];
+      const QImage& g = m->imgs[p.img];
       const size_t rel = p.off - g.off;
-      w4_dequantize(g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(p.rows), m->w4_scratch, g.K, s);
-      src = m->w4_scratch + rel % g.K;
+      wq_dequantize(m->wq, g.p, g.N, g.K, static_cast<int>(rel / g.K), static_cast<int>(p.rows), m->wq_scratch, g.K, s);
+      src = m->wq_scratch + rel % g.K;
       ld = g.K;
     }
     B200W_CUDA(cudaMemcpy2DAsync(host_bf16, p.cols * sizeof(bf16), src, ld * sizeof(bf16), p.cols * sizeof(bf16),
@@ -1208,17 +1214,17 @@ int b200w_infer_init_random(b200w_ctx* ctx, uint64_t seed, float std) {
   return iguard(ctx, [&] {
     Infer* m = model(ctx);
     check_weights_unshared(m);
-    // one device-side fill of the whole flat space (the fused matrices included), then the 1-D parameters. With int4
-    // weights every image and every other matrix gets the values of its own range of that fill, an image through
+    // one device-side fill of the whole flat space (the fused matrices included), then the 1-D parameters. With
+    // quantized weights every image and every other matrix gets the values of its own range of that fill, an image through
     // the scratch and the quantizer: quantize(W) of the bf16 engine's W for the same seed.
     m->tiled_valid = false;
     cudaStream_t s = ctx_stream(ctx);
-    if (!m->w4) {
+    if (m->wq == WFmt::bf16) {
       ctx_fill_normal(ctx, m->w, m->n_elems, seed, std);
     } else {
-      for (const W4Image& g : m->imgs) {
-        ctx_fill_normal(ctx, m->w4_scratch, static_cast<size_t>(g.N) * g.K, seed, std, g.off);
-        w4_quantize(m->w4_scratch, g.K, g.N, g.K, g.p, g.N, g.K, 0, 0, m->w4_bad, s);
+      for (const QImage& g : m->imgs) {
+        ctx_fill_normal(ctx, m->wq_scratch, static_cast<size_t>(g.N) * g.K, seed, std, g.off);
+        wq_quantize(m->wq, m->wq_scratch, g.K, g.N, g.K, g.p, g.N, g.K, 0, 0, m->wq_bad, s);
       }
       for (const IParam& p : m->params)
         if (p.kind == 'm') ctx_fill_normal(ctx, m->w + p.dev, static_cast<size_t>(p.rows * p.cols), seed, std, p.off);

@@ -10,7 +10,7 @@
 #include "host_common.h"
 #include "kv_cache.h"
 #include "ops.h"
-#include "w4.h"
+#include "wq.h"
 
 using namespace b200w;
 
@@ -123,16 +123,18 @@ int b200w_op_gemm_decode(b200w_ctx* ctx, const void* X, const void* W, void* out
     B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
   });
 }
-int64_t b200w_w4_image_bytes(int N, int K) {
-  if (N <= 0 || K <= 0 || K % W4_GROUP) return -1;
-  return static_cast<int64_t>(w4_image_bytes(N, K));
+namespace {
+// the quantized-weight hooks, for both formats
+int64_t image_bytes(WFmt f, int N, int K) {
+  if (N <= 0 || K <= 0 || K % WQ_GROUP) return -1;
+  return static_cast<int64_t>(wq_image_bytes(f, N, K));
 }
-int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int K) {
+int quantize_hook(b200w_ctx* ctx, WFmt f, const void* W, void* image, int N, int K) {
   return guarded(ctx, [&] {
     auto bad = device_scratch<int>(1);
     B200W_CUDA(cudaMemsetAsync(bad.get(), 0, sizeof(int), ctx_stream(ctx)));
-    w4_clear(static_cast<uint8_t*>(image), N, K, ctx_stream(ctx));
-    w4_quantize(W, K, N, K, static_cast<uint8_t*>(image), N, K, 0, 0, bad.get(), ctx_stream(ctx));
+    wq_clear(f, static_cast<uint8_t*>(image), N, K, ctx_stream(ctx));
+    wq_quantize(f, W, K, N, K, static_cast<uint8_t*>(image), N, K, 0, 0, bad.get(), ctx_stream(ctx));
     ctx_launches(ctx) += 2;
     int h = 0;
     B200W_CUDA(cudaMemcpyAsync(&h, bad.get(), sizeof(int), cudaMemcpyDeviceToHost, ctx_stream(ctx)));
@@ -140,11 +142,11 @@ int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int 
     B200W_CHECK(h == 0, "non-finite weight");
   });
 }
-int b200w_op_dequantize_w4(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K) {
-  HOOK(w4_dequantize(static_cast<const uint8_t*>(image), N, K, 0, N, W_hat, K, ctx_stream(ctx)));
+int dequantize_hook(b200w_ctx* ctx, WFmt f, const void* image, void* W_hat, int N, int K) {
+  HOOK(wq_dequantize(f, static_cast<const uint8_t*>(image), N, K, 0, N, W_hat, K, ctx_stream(ctx)));
 }
-int b200w_op_gemm_decode_w4(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M, int N,
-                            int K, int split_k) {
+int gemm_decode_hook(b200w_ctx* ctx, WFmt f, const void* X, const void* image, void* out, const void* C, int M, int N,
+                     int K, int split_k) {
   return guarded(ctx, [&] {
     DeviceScratch<float> ws;
     DeviceScratch<unsigned> cnt;
@@ -156,11 +158,36 @@ int b200w_op_gemm_decode_w4(b200w_ctx* ctx, const void* X, const void* image, vo
     o.out = out;
     o.ldo = N;
     o.C = C;
-    o.w4 = image;
+    o.wq = image;
+    o.wq_fmt = f;
     gemm_decode_ex(X, K, nullptr, K, o, ws.get(), cnt.get(), M, N, K, ctx_stream(ctx));
     ++ctx_launches(ctx);
     B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
   });
+}
+}  // namespace
+
+int64_t b200w_w4_image_bytes(int N, int K) { return image_bytes(WFmt::int4, N, K); }
+int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int K) {
+  return quantize_hook(ctx, WFmt::int4, W, image, N, K);
+}
+int b200w_op_dequantize_w4(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K) {
+  return dequantize_hook(ctx, WFmt::int4, image, W_hat, N, K);
+}
+int b200w_op_gemm_decode_w4(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M, int N,
+                            int K, int split_k) {
+  return gemm_decode_hook(ctx, WFmt::int4, X, image, out, C, M, N, K, split_k);
+}
+int64_t b200w_w8_image_bytes(int N, int K) { return image_bytes(WFmt::int8, N, K); }
+int b200w_op_quantize_w8(b200w_ctx* ctx, const void* W, void* image, int N, int K) {
+  return quantize_hook(ctx, WFmt::int8, W, image, N, K);
+}
+int b200w_op_dequantize_w8(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K) {
+  return dequantize_hook(ctx, WFmt::int8, image, W_hat, N, K);
+}
+int b200w_op_gemm_decode_w8(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M, int N,
+                            int K, int split_k) {
+  return gemm_decode_hook(ctx, WFmt::int8, X, image, out, C, M, N, K, split_k);
 }
 int b200w_op_embed_fwd(b200w_ctx* ctx, const int32_t* ids, const void* table, const void* pos_table,
                        void* out, int T, int d, int vocab, int S, int pos_offset) {

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "wq.h"
+
 struct b200w_sampling;   // include/b200w.h
 struct b200w_penalties;  // include/b200w.h
 
@@ -64,7 +66,8 @@ struct GemmDecodeOut {
   int act = 0;
   int act_from = 0;
   const void* w_tiled = nullptr;  // retile_weights() image of W: streamed with 16 KB bulk copies instead of TMA boxes
-  const void* w4 = nullptr;       // int4 image of W (w4.h): W and w_tiled are not read
+  const void* wq = nullptr;       // quantized image of W (wq.h): W and w_tiled are not read
+  WFmt wq_fmt = WFmt::bf16;       // its format (int4 or int8)
 };
 // W [N, K] (row stride ldw) as consecutive 16 KB swizzled shared-memory images of its [128 x 64] tiles
 // (gemm.cu retile_weights_kernel); retiled_bytes = the size of that image.

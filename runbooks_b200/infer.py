@@ -77,7 +77,8 @@ KV_PAGE = 128   # positions per page of the paged KV cache (one key block of the
 
 
 KV_DTYPES = {"bf16": 0, "fp8": 1}   # b200w_kv_dtype: bf16, or e4m3 with one fp32 scale per (position, kv head)
-WEIGHT_DTYPES = {"bf16": 0, "int4": 1}   # B200W_WEIGHTS_*: int4 = group-quantized projections (DESIGN §3.5)
+# B200W_WEIGHTS_*: int4 / int8 = group-quantized projections (DESIGN §3.5)
+WEIGHT_DTYPES = {"bf16": 0, "int4": 1, "int8": 2}
 
 
 def kv_page_bytes(arch: ServeArch, kv_dtype: str = "bf16") -> int:
@@ -112,9 +113,10 @@ class InferEngine(Engine):
         the bytes per page (DESIGN §3.5).
         max_rows (max_batch..128; None: max_batch): rows one step may hold, for steps that verify drafted tokens
         (b200w_infer_set_step_rows).
-        weight_dtype: "bf16", or "int4": every projection stored as int4 with one bf16 scale per row and 64 input
-        columns, about a quarter of the bytes; the engine computes exactly what the bf16 engine does on the
-        dequantized weights (read_weight)."""
+        weight_dtype: "bf16", "int4" or "int8": every projection stored as int4 / int8 with one bf16 scale per row
+        and 64 input columns, about a quarter / half of the bytes; the engine computes exactly what the bf16 engine
+        does on the dequantized weights (read_weight). int8 is weight-only round-to-nearest, not bitsandbytes'
+        LLM.int8: the activations stay bf16 and there is no outlier decomposition."""
         if weight_dtype not in WEIGHT_DTYPES:
             raise ValueError(f"weight_dtype must be one of {sorted(WEIGHT_DTYPES)}, got {weight_dtype!r}")
         if kv_dtype not in KV_DTYPES:
@@ -212,12 +214,12 @@ class InferEngine(Engine):
 
     def weight_bytes(self) -> int:
         """Device bytes the weights are stored in (b200w_infer_weight_bytes): the bf16 parameters and, with int4
-        weights, the projections' images."""
+        or int8 weights, the projections' images."""
         return self._lib.b200w_infer_weight_bytes(self._h)
 
     def read_weight(self, name: str, shape) -> np.ndarray:
         """The values the engine computes with for parameter `name` as bf16 bit patterns (uint16 of `shape`): the
-        dequantized weights for a projection of an int4 engine, the loaded ones otherwise."""
+        dequantized weights for a projection of an int4 or int8 engine, the loaded ones otherwise."""
         out = np.empty(shape, dtype=np.uint16)
         self._check(self._lib.b200w_infer_read_weight(self._h, name.encode(), out.ctypes.data, out.size))
         return out

@@ -559,13 +559,32 @@ def _as_bool(what: str, v) -> bool:
 
 
 def load_in_4bit_param(load_in_4bit: bool | None = None, environ=None) -> bool:
-    """Whether the Server stores its projections as int4 (weight_dtype "int4"): --load-in-4bit, else the environment's
+    """Whether the Server asks for int4 projections (weight_dtype "int4"): --load-in-4bit, else the environment's
     MODEL_LOAD_IN_4BIT (true / false, 1 / 0, yes / no; anything else is an error), else off. MODEL_LOAD_IN_8BIT is
-    not read: 8-bit weights are not built."""
+    load_in_8bit_param's; weight_dtype_param refuses both on."""
     if load_in_4bit is not None:
         return bool(load_in_4bit)
     environ = os.environ if environ is None else environ
     return _as_bool("MODEL_LOAD_IN_4BIT", environ.get("MODEL_LOAD_IN_4BIT", False))
+
+
+def load_in_8bit_param(load_in_8bit: bool | None = None, environ=None) -> bool:
+    """Whether the Server asks for int8 projections (weight_dtype "int8"): --load-in-8bit, else the environment's
+    MODEL_LOAD_IN_8BIT (true / false, 1 / 0, yes / no; anything else is an error), else off."""
+    if load_in_8bit is not None:
+        return bool(load_in_8bit)
+    environ = os.environ if environ is None else environ
+    return _as_bool("MODEL_LOAD_IN_8BIT", environ.get("MODEL_LOAD_IN_8BIT", False))
+
+
+def weight_dtype_param(load_in_4bit: bool | None = None, load_in_8bit: bool | None = None, environ=None) -> str:
+    """The engine's weight_dtype: "int4" (load_in_4bit_param), "int8" (load_in_8bit_param) or "bf16". Both on is a
+    ValueError, as transformers refuses load_in_4bit together with load_in_8bit."""
+    w4, w8 = load_in_4bit_param(load_in_4bit, environ), load_in_8bit_param(load_in_8bit, environ)
+    if w4 and w8:
+        raise ValueError("load_in_4bit and load_in_8bit are both on (MODEL_LOAD_IN_4BIT / MODEL_LOAD_IN_8BIT or "
+                         "--load-in-4bit / --load-in-8bit): choose one")
+    return "int4" if w4 else "int8" if w8 else "bf16"
 
 
 def speculative_tokens_param(content: str, speculative_tokens: int | None = None, environ=None) -> int:
@@ -628,9 +647,11 @@ def kv_pages_for_gb(arch, kv_cache_gb: float, kv_dtype: str = "bf16") -> int:
 
 
 def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb: float | None = None,
-                kv_dtype: str = "bf16", speculative_tokens: int = 0, load_in_4bit: bool | None = None):
+                kv_dtype: str = "bf16", speculative_tokens: int = 0, load_in_4bit: bool | None = None,
+                load_in_8bit: bool | None = None):
     """speculative_tokens > 0: a step holds up to min(128, max_batch * (1 + speculative_tokens)) rows.
-    load_in_4bit: int4 projections (None: MODEL_LOAD_IN_4BIT, load_in_4bit_param)."""
+    load_in_4bit / load_in_8bit: int4 / int8 projections (None: MODEL_LOAD_IN_4BIT / MODEL_LOAD_IN_8BIT,
+    weight_dtype_param)."""
     from .infer import InferEngine, ServeArch
 
     cfg = contract.read_hf_config(model_dir)
@@ -639,7 +660,7 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
     e = InferEngine(int(os.environ.get("B200W_DEVICE", "0")))
     e.init_infer(arch, max_batch=max_batch, kv_pages=kv_pages, kv_dtype=kv_dtype,
                  max_rows=min(128, max_batch * (1 + speculative_tokens)) if speculative_tokens else None,
-                 weight_dtype="int4" if load_in_4bit_param(load_in_4bit) else "bf16")
+                 weight_dtype=weight_dtype_param(load_in_4bit, load_in_8bit))
     wanted = {n for n, _ in e.infer_params()}
     seen, unused = set(), []
     for name, arr in contract.iter_safetensors(model_dir):
@@ -658,9 +679,11 @@ def load_engine(model_dir: str, max_batch: int, max_ctx: int | None, kv_cache_gb
 
 def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, kv_cache_gb: float | None = None,
           prefix_cache: bool | None = None, kv_cache_dtype: str | None = None, max_logprobs: int | None = None,
-          penalties: bool | None = None, speculative_tokens: int | None = None, load_in_4bit: bool | None = None):
+          penalties: bool | None = None, speculative_tokens: int | None = None, load_in_4bit: bool | None = None,
+          load_in_8bit: bool | None = None):
     max_batch, kv_cache_gb = server_params(content, max_batch, kv_cache_gb)
-    load_in_4bit = load_in_4bit_param(load_in_4bit)
+    weight_dtype = weight_dtype_param(load_in_4bit, load_in_8bit)
+    load_in_4bit, load_in_8bit = weight_dtype == "int4", weight_dtype == "int8"
     speculative_tokens = speculative_tokens_param(content, speculative_tokens)
     prefix_cache = prefix_cache_param(content, prefix_cache)
     kv_dtype = kv_cache_dtype_param(content, kv_cache_dtype)
@@ -672,7 +695,8 @@ def serve(content: str, port: int, max_batch: int | None, max_ctx: int | None, k
         raise ValueError("an fp8 KV cache is paged: kv_cache_dtype fp8 needs kv_cache_gb")
     model_dir = os.path.join(content, "model")
     t0 = time.time()
-    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype, speculative_tokens, load_in_4bit)
+    engine, cfg = load_engine(model_dir, max_batch, max_ctx, kv_cache_gb, kv_dtype, speculative_tokens, load_in_4bit,
+                              load_in_8bit)
     tok = contract.Tokenizer(model_dir)
     sched = Scheduler(engine, tok, prefix_cache=prefix_cache, max_logprobs=max_logprobs, penalties=penalties,
                       speculative_tokens=speculative_tokens)
@@ -718,10 +742,13 @@ def main(argv=None) -> int:
     ap.add_argument("--load-in-4bit", action="store_true", default=None,
                     help="store the projections as int4, one bf16 scale per row and 64 inputs (default: env "
                          "MODEL_LOAD_IN_4BIT, else bf16)")
+    ap.add_argument("--load-in-8bit", action="store_true", default=None,
+                    help="store the projections as int8, one bf16 scale per row and 64 inputs; weight-only, no "
+                         "outlier decomposition (default: env MODEL_LOAD_IN_8BIT, else bf16)")
     a = ap.parse_args(argv)
     try:
         serve(a.content, a.port, a.max_batch, a.max_ctx, a.kv_cache_gb, a.prefix_cache, a.kv_cache_dtype,
-              a.max_logprobs, a.penalties, a.speculative_tokens, a.load_in_4bit)
+              a.max_logprobs, a.penalties, a.speculative_tokens, a.load_in_4bit, a.load_in_8bit)
         return 0
     except BaseException:  # noqa: BLE001
         traceback.print_exc()

@@ -125,7 +125,7 @@ def llama70b(out):
             for _ in range(10):
                 eng._lib.b200w_op_dequantize_w4(eng.handle, img.data_ptr(), what.data_ptr(), N, K)
         t = [ev.device_time if hasattr(ev, "device_time") else ev.cuda_time for ev in prof.events()
-             if ev.device_type.name == "CUDA" and "w4_dequantize_kernel" in ev.name]
+             if ev.device_type.name == "CUDA" and "wq_dequantize_kernel" in ev.name]
         us = float(np.median(t))
         r[f"dequant_{N}x{K}_us"] = us
         r[f"dequant_{N}x{K}_GBps"] = (eng._lib.b200w_w4_image_bytes(N, K) + 2 * N * K) / us / 1e3
