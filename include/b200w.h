@@ -49,8 +49,13 @@ typedef enum { B200W_BF16 = 0, B200W_F32 = 1, B200W_I32 = 2 } b200w_dtype;
 /* Model families. The fine-tune engine builds LLAMA and OPT, the Server engine all three. */
 #define B200W_FAMILY_LLAMA 0  /* HF models/llama/modeling_llama.py: RMSNorm, rotate_half RoPE, SwiGLU,
                                  untied lm_head, no biases; head_dim must be 128 for training      */
-#define B200W_FAMILY_FALCON 1 /* HF models/falcon/modeling_falcon.py, falcon-7b layout: multi_query, parallel_attn,
-                                 one LayerNorm per block, exact GeLU, no biases, tied head                    */
+#define B200W_FAMILY_FALCON 1 /* HF models/falcon/modeling_falcon.py: rotary, parallel residual, exact GeLU, no
+                                 biases. Falcon-7B (multi_query: 1 kv head), multi-head (multi_query false)
+                                 and new_decoder_architecture (Falcon-40B: grouped kv heads) layouts, one
+                                 LayerNorm per block or, with parallel_norms (b200w_infer_arch.reserved[1]),
+                                 ln_attn + ln_mlp. The fused
+                                 query_key_value is loaded and read back in HF's row order. The fine-tune
+                                 engine builds the falcon-7b layout only.                               */
 #define B200W_FAMILY_OPT 2    /* HF models/opt/modeling_opt.py, opt-125m layout: learned positions
                                  (+2), pre-LayerNorm with bias, biased projections, ReLU MLP, tied
                                  lm_head; head_dim 64 or 128 (64 is stored zero-padded to 128 on the
@@ -208,7 +213,9 @@ typedef struct {
   int32_t tie_embeddings;    /* lm_head shares the embedding matrix (Falcon, OPT)               */
   int32_t max_positions;     /* OPT: max_position_embeddings (learned table, +2 rows); else 0   */
   int32_t weight_dtype;      /* B200W_WEIGHTS_*: 0 bf16, 1 int4, 2 int8                         */
-  int32_t reserved[2];       /* zero                                                            */
+  int32_t reserved[2];       /* [0] zero; [1] parallel_norms, Falcon only: 1 = ln_attn + ln_mlp per
+                                layer (new_decoder_architecture, num_ln_in_parallel_attn 2), 0 = one
+                                input_layernorm; 0 for the other families                       */
 } b200w_infer_arch;
 /* Weight formats of the Server engine. INT4_G64: every projection (not the embedding, positions, norms, biases or
  * lm_head) is stored as round-to-nearest symmetric int4 with one bf16 scale per row and 64 input columns:
@@ -444,6 +451,13 @@ B200W_API int b200w_op_quantize_w8(b200w_ctx* ctx, const void* W, void* image, i
 B200W_API int b200w_op_dequantize_w8(b200w_ctx* ctx, const void* image, void* W_hat, int N, int K);
 B200W_API int b200w_op_gemm_decode_w8(b200w_ctx* ctx, const void* X, const void* image, void* out, const void* C, int M,
                                       int N, int K, int split_k);
+/* The decode GEMM with a second activation window, as Falcon's two-norm layer runs [q k v | dense_h_to_4h]: out[M, N]
+ * (row stride N) = X[:, 0:K] W[0:n_split]^T for the first n_split features and X[:, x_col2:x_col2 + K]
+ * W[n_split:N]^T for the rest, X with row stride ldx (x_col2 0: one window, a plain decode GEMM). weight_dtype
+ * B200W_WEIGHTS_*: W is bf16 [N, K] or the int4 / int8 image of it. A window needs n_split a multiple of 128 inside
+ * N, K a multiple of 64 and x_col2 + K <= ldx. split_k: 0 runs unsplit, else K is split as the serving step does. */
+B200W_API int b200w_op_gemm_decode_window(b200w_ctx* ctx, int weight_dtype, const void* X, int ldx, const void* W,
+                                          void* out, int M, int N, int K, int n_split, int x_col2, int split_k);
 /* pos_table (NULL or bf16 [*, d]): row (t % S) + pos_offset is added (OPT learned positions).
  * embed_bwd: pad_id = nn.Embedding padding_idx (-1 none); dpos NULL or the position-table gradient. */
 B200W_API int b200w_op_embed_fwd(b200w_ctx* ctx, const int32_t* ids, const void* table, const void* pos_table,

@@ -33,6 +33,7 @@ class Arch(C.Structure):
 
 
 class InferArch(C.Structure):
+    """b200w_infer_arch; reserved[1] is parallel_norms (Falcon's ln_attn + ln_mlp)."""
     _fields_ = [
         ("family", C.c_int32), ("vocab_size", C.c_int32), ("hidden_size", C.c_int32),
         ("intermediate_size", C.c_int32), ("num_layers", C.c_int32), ("num_heads", C.c_int32),
@@ -144,6 +145,8 @@ PROTOTYPES = {
     "b200w_op_quantize_w8": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
     "b200w_op_dequantize_w8": (C.c_int, [c_ctx, vp, vp, C.c_int, C.c_int]),
     "b200w_op_gemm_decode_w8": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b200w_op_gemm_decode_window": (C.c_int, [c_ctx, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                              C.c_int, C.c_int]),
     "b200w_op_embed_fwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200w_op_embed_bwd": (C.c_int, [c_ctx, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int]),

@@ -582,6 +582,8 @@ __device__ __forceinline__ float decode_act(float x, int act) {
 // [q k v | dense_h_to_4h] from one LayerNorm output in ONE launch, the two halves going to the
 // attention input and to the K-concatenated [attention output | MLP hidden] operand of the next GEMM.
 // v = acc (+ bias[n]) (+ C[b, n]); act is applied to features n >= act_from.
+// x_col2 (0: off): the N tiles at or past n_split read X from column x_col2 on instead of column 0 -- Falcon's two-norm
+// layer feeds q k v from ln_attn(h) and dense_h_to_4h from ln_mlp(h), the two halves of one [rows, 2d] operand.
 struct DecodeEpi {
   __nv_bfloat16* out;
   int ldo;
@@ -593,6 +595,7 @@ struct DecodeEpi {
   const __nv_bfloat16* bias;
   int act;
   int act_from;
+  int x_col2;
 };
 __device__ __forceinline__ void decode_store(const DecodeEpi& e, int b, int n, float v) {
   if (e.bias) v += __bfloat162float(e.bias[n]);
@@ -658,6 +661,7 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
   const int kb1 = min(num_kb_total, kb0 + kb_per_split);
   const int nkb = kb1 - kb0;
   const bool split = gridDim.y > 1;
+  const int xc = n0 >= epi.n_split ? epi.x_col2 : 0;   // this tile's window of X
 
   if (threadIdx.x == 0) {
     pdl_trigger();  // the next kernel's CTAs may take the SM slots that free up from now on
@@ -686,14 +690,14 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
         }
         pdl_wait();
         for (int i = 0; i < pre; ++i)
-          tma_load_2d(smem + i * cfg::B_STAGE_BYTES, tmX, &full_bar[i], (kb0 + i) * BLOCK_K, 0);
+          tma_load_2d(smem + i * cfg::B_STAGE_BYTES, tmX, &full_bar[i], xc + (kb0 + i) * BLOCK_K, 0);
         int stage = 0;
         uint32_t phase = 0;
         for (int kb = kb0 + pre; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase);
           mbar_arrive_expect_tx(&full_bar[stage], cfg::STAGE_BYTES);
           bulk_load_1d(sw + stage * TILE, wt + static_cast<size_t>(kb) * TILE, TILE, &full_bar[stage]);
-          tma_load_2d(smem + stage * cfg::B_STAGE_BYTES, tmX, &full_bar[stage], kb * BLOCK_K, 0);
+          tma_load_2d(smem + stage * cfg::B_STAGE_BYTES, tmX, &full_bar[stage], xc + kb * BLOCK_K, 0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       } else {
@@ -708,7 +712,7 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
       }
       pdl_wait();  // ... then the predecessor's activations
       for (int i = 0; i < pre; ++i)
-        tma_load_2d(smem + i * cfg::STAGE_BYTES + A_STAGE_BYTES, tmX, &full_bar[i], (kb0 + i) * BLOCK_K, 0);
+        tma_load_2d(smem + i * cfg::STAGE_BYTES + A_STAGE_BYTES, tmX, &full_bar[i], xc + (kb0 + i) * BLOCK_K, 0);
       int stage = 0;
       uint32_t phase = 0;  // parity of the FIRST pass through the ring; the steady state starts on pass 2
       for (int kb = kb0 + pre; kb < kb1; ++kb) {
@@ -716,7 +720,7 @@ __device__ __forceinline__ void gemm_decode_body(const CUtensorMap* tmW, const C
         uint8_t* sa = smem + stage * cfg::STAGE_BYTES;
         mbar_arrive_expect_tx(&full_bar[stage], cfg::STAGE_BYTES);
         load_w(sa, &full_bar[stage], kb);                                            // weights
-        tma_load_2d(sa + A_STAGE_BYTES, tmX, &full_bar[stage], kb * BLOCK_K, 0);    // batch rows
+        tma_load_2d(sa + A_STAGE_BYTES, tmX, &full_bar[stage], xc + kb * BLOCK_K, 0);   // batch rows
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       }
@@ -891,7 +895,7 @@ template <int MPAD, WFmt F>
 void launch_decode(const void* X, int ldx, const void* W, int ldw, const void* w_tiled, const DecodeEpi& epi,
                    bool allow_split, int M, int N, int K, cudaStream_t stream) {
   using cfg = DecodeCfg<MPAD, F>;
-  CUtensorMap tmX = make_tmap_bf16_2d(X, M, K, ldx, MPAD, BLOCK_K);
+  CUtensorMap tmX = make_tmap_bf16_2d(X, M, K + epi.x_col2, ldx, MPAD, BLOCK_K);   // both windows of X
   CUtensorMap tmW = F != WFmt::bf16 ? tmX : make_tmap_bf16_2d(W, N, K, ldw, BLOCK_M, BLOCK_K);
   auto kern = decode_kernel<MPAD, F>();
   static PerDeviceOnce once;
@@ -1036,6 +1040,12 @@ void gemm_decode_ex(const void* X, int ldx, const void* W, int ldw, const GemmDe
   e.bias = static_cast<const __nv_bfloat16*>(o.bias);
   e.act = o.act;
   e.act_from = o.act_from;
+  e.x_col2 = o.x_col2;
+  if (o.x_col2)
+    B200W_CHECK(o.out2 && o.n_split > 0 && o.n_split < N && o.n_split % BLOCK_M == 0 && K % BLOCK_K == 0 &&
+                    o.x_col2 % 8 == 0 && ldx >= o.x_col2 + K,
+                "a second X window needs out2, n_split a multiple of 128 inside N, K a multiple of 64 and the window "
+                "[x_col2, x_col2 + K) 16-byte aligned within the row stride ldx");
   const bool allow_split = ws != nullptr && counters != nullptr;  // the scratch itself is no longer used
   auto run = [&](auto fmt, const void* Wr, const void* tiled) {
     constexpr WFmt F = decltype(fmt)::value;

@@ -1,9 +1,10 @@
 // Server engine (SURVEY.md 8 a14; started by server_controller.go:149-173): prompt PREFILL in one pass
 // (big-M wgmma GEMMs + the training flash-attention forward) and batched greedy DECODE, one new token
 // per cache slot per step. Families:
-//   FALCON  (HF models/falcon/modeling_falcon.py, falcon-7b layout: multi_query, parallel_attn,
-//            one input_layernorm per layer, bias-free linears, LayerNorm with bias, exact GeLU,
-//            rotate_half RoPE, lm_head tied to word_embeddings)
+//   FALCON  (HF models/falcon/modeling_falcon.py: parallel residual, bias-free linears, LayerNorm with bias,
+//            exact GeLU, rotate_half RoPE, lm_head tied to word_embeddings; falcon-7b's multi_query, the
+//            multi-head layout and new_decoder_architecture's grouped kv heads through one query_key_value rule
+//            (copy_qkv), one input_layernorm per layer or ln_attn + ln_mlp)
 //   LLAMA   (HF models/llama/modeling_llama.py: RMSNorm, SwiGLU, sequential residual, GQA)
 //   OPT     (HF models/opt/modeling_opt.py, opt-125m layout: learned positions + 2, pre-LayerNorm,
 //            biased projections, ReLU, tied head) -- the model of the reference's system test
@@ -57,10 +58,13 @@ __global__ void infer_embed_pos_kernel(const int32_t* __restrict__ tok, const in
 
 // LayerNorm with bias (oracle: torch.nn.LayerNorm as used by FalconDecoderLayer), fp32 statistics.
 // One block per row, the row is read from HBM/L2 once and kept in registers (d <= 256*8*4).
+// NOUT 2: Falcon's two-norm layer (ln_attn, ln_mlp), which share the row's mean and rstd: one pass writes
+// [ln_attn(x) | ln_mlp(x)] (weights w, b and w2, b2) as rows of 2d.
 constexpr int LN_MAXP = 4;
+template <int NOUT>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ b,
-                 bf16* __restrict__ y, int d, float eps) {
+                 const bf16* __restrict__ w2, const bf16* __restrict__ b2, bf16* __restrict__ y, int d, float eps) {
   __shared__ float red[32];
   pdl_trigger();
   pdl_wait();
@@ -96,21 +100,25 @@ layernorm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const b
     }
   }
   const float rstd = rsqrtf(block_reduce(q, red, false) / d + eps);
-  bf16* yr = y + static_cast<size_t>(blockIdx.x) * d;
 #pragma unroll
-  for (int p = 0; p < LN_MAXP; ++p) {
-    const int c = (p * 256 + threadIdx.x) * 8;
-    if (c < d) {
-      const uint4 uw = *reinterpret_cast<const uint4*>(w + c);
-      const uint4 ub = *reinterpret_cast<const uint4*>(b + c);
-      const uint32_t ww[4] = {uw.x, uw.y, uw.z, uw.w}, bb[4] = {ub.x, ub.y, ub.z, ub.w};
-      uint32_t o[4];
+  for (int n = 0; n < NOUT; ++n) {
+    const bf16 *wn = n ? w2 : w, *bn = n ? b2 : b;
+    bf16* yr = y + static_cast<size_t>(blockIdx.x) * NOUT * d + static_cast<size_t>(n) * d;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 fw = unpack_bf16x2(ww[j]), fb = unpack_bf16x2(bb[j]);
-        o[j] = pack_bf16x2((v[p][2 * j] - mean) * rstd * fw.x + fb.x, (v[p][2 * j + 1] - mean) * rstd * fw.y + fb.y);
+    for (int p = 0; p < LN_MAXP; ++p) {
+      const int c = (p * 256 + threadIdx.x) * 8;
+      if (c < d) {
+        const uint4 uw = *reinterpret_cast<const uint4*>(wn + c);
+        const uint4 ub = *reinterpret_cast<const uint4*>(bn + c);
+        const uint32_t ww[4] = {uw.x, uw.y, uw.z, uw.w}, bb[4] = {ub.x, ub.y, ub.z, ub.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 fw = unpack_bf16x2(ww[j]), fb = unpack_bf16x2(bb[j]);
+          o[j] = pack_bf16x2((v[p][2 * j] - mean) * rstd * fw.x + fb.x, (v[p][2 * j + 1] - mean) * rstd * fw.y + fb.y);
+        }
+        *reinterpret_cast<uint4*>(yr + c) = make_uint4(o[0], o[1], o[2], o[3]);
       }
-      *reinterpret_cast<uint4*>(yr + c) = make_uint4(o[0], o[1], o[2], o[3]);
     }
   }
 }
@@ -206,6 +214,7 @@ struct IParam {
   char kind;    // 'p' projection, 'm' other matrix (embedding, positions, lm_head), 'n' norm weight (ones), 'b' bias (zeros)
   size_t dev = 0;   // element offset in Infer::w (== off, except for quantized weights, where projections are not there)
   int img = -1;     // quantized weights: the projection's image in Infer::imgs
+  bool hf_qkv = false;   // Falcon's query_key_value: HF's grouped row order outside, [Q | K | V] inside (copy_qkv)
 };
 
 // A quantized image (wq.h) of one fused projection matrix [N, K]: the matrix the decode GEMM reads in one launch. off:
@@ -249,6 +258,7 @@ struct Infer {
   uint8_t* t_lm = nullptr;
   bool tiled_valid = false;
   int qd = 0, kd = 0, qkvd = 0, ld_cat = 0;  // Falcon: ld_cat = qd + f, the [attention | mlp hidden] operand
+  int n_norms = 1;   // LayerNorm outputs per row in nrm / pf_nrm: 2 for Falcon's ln_attn + ln_mlp ([rows, 2d])
   // decode activations [max_rows, *]
   bf16 *h = nullptr, *h2 = nullptr, *nrm = nullptr, *qkv = nullptr, *cat = nullptr, *mid = nullptr,
        *act = nullptr, *logits = nullptr;
@@ -317,6 +327,7 @@ void build(Infer* m) {
   const int d = a.hidden_size, f = a.intermediate_size, L = a.num_layers;
   const int qd = a.num_heads * a.head_dim, kd = a.num_kv_heads * a.head_dim;
   m->qd = qd; m->kd = kd; m->qkvd = qd + 2 * kd;
+  m->n_norms = a.reserved[1] ? 2 : 1;   // parallel_norms
   m->lp.assign(L, {});
   if (a.family == B200W_FAMILY_FALCON) {
     m->ld_cat = qd + f;
@@ -324,10 +335,19 @@ void build(Infer* m) {
     for (int l = 0; l < L; ++l) {
       const std::string p = "transformer.h." + std::to_string(l) + ".";
       auto& x = m->lp[l];
-      x.ln1_w = add_dense(m, p + "input_layernorm.weight", 1, d, 'n');
-      x.ln1_b = add_dense(m, p + "input_layernorm.bias", 1, d, 'b');
-      // [q k v | dense_h_to_4h]: adjacent rows of ONE [qkvd + f, d] matrix (both consume the LayerNorm output)
+      if (m->n_norms == 2) {   // ln_attn feeds the attention, ln_mlp the MLP (ln2)
+        x.ln1_w = add_dense(m, p + "ln_attn.weight", 1, d, 'n');
+        x.ln1_b = add_dense(m, p + "ln_attn.bias", 1, d, 'b');
+        x.ln2_w = add_dense(m, p + "ln_mlp.weight", 1, d, 'n');
+        x.ln2_b = add_dense(m, p + "ln_mlp.bias", 1, d, 'b');
+      } else {
+        x.ln1_w = add_dense(m, p + "input_layernorm.weight", 1, d, 'n');
+        x.ln1_b = add_dense(m, p + "input_layernorm.bias", 1, d, 'b');
+      }
+      // [q k v | dense_h_to_4h]: adjacent rows of ONE [qkvd + f, d] matrix (both consume the LayerNorm output, or
+      // with two norms one each)
       x.wqkv = add_dense(m, p + "self_attention.query_key_value.weight", qd + 2 * kd, d, 'p');
+      m->params.back().hf_qkv = true;
       x.w1 = add_dense(m, p + "mlp.dense_h_to_4h.weight", f, d, 'p');
       // [dense | dense_4h_to_h]: column windows of ONE [d, qd + f] matrix (their outputs are summed)
       x.wo = m->n_elems;
@@ -435,6 +455,30 @@ size_t layout_wq(Infer* m, cudaStream_t s) {
   m->wq_scratch = m->mem.alloc<bf16>(scratch);
   m->wq_bad = m->mem.alloc<int>(1);
   return n;
+}
+
+// Falcon's fused query_key_value [qkvd, d] between HF's row order and the engine's. HF's holds, for each kv group g of
+// G = H / Hkv query heads, [q heads gG .. gG + G - 1 | k_g | v_g] (modeling_falcon.py _split_heads); the engine keeps
+// [Q | K | V], whose query head h = gG + j uses kv head h / G as the attention kernels do. One rule for every layout:
+// multi_query (Falcon-7B) is one group of G = H (the identity), the multi-head layout is H groups of G = 1 (per head
+// [q k v]), new_decoder_architecture (Falcon-40B) what its num_kv_heads makes. to_engine: src is in HF's order and
+// dst in the engine's, else the reverse. Three strided 2-D copies, one per part (q blocks, k rows, v rows) with one
+// row per group; rows of d elements, contiguous on both sides.
+void copy_qkv(const Infer* m, void* dst, const void* src, cudaMemcpyKind kind, bool to_engine, cudaStream_t s) {
+  const auto& a = m->a;
+  const size_t row = static_cast<size_t>(a.hidden_size) * sizeof(bf16), dh = a.head_dim, Hkv = a.num_kv_heads;
+  const size_t G = a.num_heads / a.num_kv_heads, hf_pitch = (G + 2) * dh * row;   // bytes of one group in HF's order
+  struct Part { size_t rows, hf0, eng0; };   // rows per group, first row in HF's group, first row in the engine's
+  const Part parts[3] = {{G * dh, 0, 0}, {dh, G * dh, Hkv * G * dh}, {dh, (G + 1) * dh, Hkv * (G + 1) * dh}};
+  for (const Part& q : parts) {
+    const size_t width = q.rows * row;
+    if (to_engine)
+      B200W_CUDA(cudaMemcpy2DAsync(static_cast<char*>(dst) + q.eng0 * row, width,
+                                   static_cast<const char*>(src) + q.hf0 * row, hf_pitch, width, Hkv, kind, s));
+    else
+      B200W_CUDA(cudaMemcpy2DAsync(static_cast<char*>(dst) + q.hf0 * row, hf_pitch,
+                                   static_cast<const char*>(src) + q.eng0 * row, width, width, Hkv, kind, s));
+  }
 }
 
 // guarded, for the serving calls: only the call right after a step or a prefill may sample from the logits it left
@@ -551,7 +595,16 @@ void norm(Pass& p, int rows, const bf16* x, size_t w, size_t b, bf16* y) {
   const Infer* m = p.m;
   const auto& a = m->a;
   if (a.family == B200W_FAMILY_LLAMA) rmsnorm_fwd(x, m->w + w, y, nullptr, rows, a.hidden_size, a.norm_eps, p.s);
-  else launch(p, layernorm_kernel, dim3(rows), dim3(256), x, m->w + w, m->w + b, y, a.hidden_size, a.norm_eps);
+  else launch(p, layernorm_kernel<1>, dim3(rows), dim3(256), x, m->w + w, m->w + b, nullptr, nullptr, y, a.hidden_size,
+              a.norm_eps);
+  ++p.nl;
+}
+
+// Falcon's two norms of x [rows, d] in one pass -> y [rows, 2d] = [LN(x; w, b) | LN(x; w2, b2)]
+void norm2(Pass& p, int rows, const bf16* x, size_t w, size_t b, size_t w2, size_t b2, bf16* y) {
+  const Infer* m = p.m;
+  launch(p, layernorm_kernel<2>, dim3(rows), dim3(256), x, m->w + w, m->w + b, m->w + w2, m->w + b2, y,
+         m->a.hidden_size, m->a.norm_eps);
   ++p.nl;
 }
 
@@ -616,21 +669,28 @@ void layer_opt(Pass& p, int l) {
   gemm(p, p.mid, f, w.w2, f, d, f, p.h, d, w.t_w2, p.h2, m->w + w.b2);
 }
 
-// parallel residual: h' = h + dense(attn(ln)) + W2 gelu(W1 ln)   (modeling_falcon.py FalconDecoderLayer)
+// parallel residual: h' = h + dense(attn(ln)) + W2 gelu(W1 ln)   (modeling_falcon.py FalconDecoderLayer), with
+// two norms h' = h + dense(attn(ln_attn)) + W2 gelu(W1 ln_mlp): nrm then holds [ln_attn | ln_mlp] and the MLP's
+// GEMM reads the second half
 void layer_falcon(Pass& p, int l) {
   const auto& w = p.m->lp[l];
   const int d = p.m->a.hidden_size, f = p.m->a.intermediate_size, qd = p.m->qd, qkvd = p.m->qkvd, ldc = p.m->ld_cat;
-  norm(p, p.rows, p.h, w.ln1_w, w.ln1_b, p.nrm);
+  const bool two = p.m->n_norms == 2;
+  const int ldn = p.m->n_norms * d, mlp_col = two ? d : 0;   // nrm's row stride, the MLP's input column
+  if (two) norm2(p, p.rows, p.h, w.ln1_w, w.ln1_b, w.ln2_w, w.ln2_b, p.nrm);
+  else norm(p, p.rows, p.h, w.ln1_w, w.ln1_b, p.nrm);
   if (p.decode) {
-    // one launch for [q k v | dense_h_to_4h]: the MLP half goes to cat's second window, exact GeLU on it only
+    // one launch for [q k v | dense_h_to_4h]: the MLP half goes to cat's second window, exact GeLU on it only (and
+    // with two norms reads ln_mlp, the second window of nrm)
     GemmDecodeOut o;
     o.out = p.qkv; o.ldo = qkvd;
     o.out2 = p.cat + qd; o.ldo2 = ldc; o.n_split = qkvd;
     o.act = 1; o.act_from = qkvd;
-    dgemm(p.m, p.s, p.rows, p.nrm, d, w.wqkv, d, qkvd + f, d, o, w.t_qkv, true); ++p.nl;
+    o.x_col2 = mlp_col;
+    dgemm(p.m, p.s, p.rows, p.nrm, ldn, w.wqkv, d, qkvd + f, d, o, w.t_qkv, true); ++p.nl;
   } else {
-    gemm(p, p.nrm, d, w.wqkv, d, qkvd, d, p.qkv, qkvd, w.t_qkv);
-    gemm(p, p.nrm, d, w.w1, d, f, d, p.cat + qd, ldc, w.t_qkv, nullptr, nullptr, Act::none, qkvd);
+    gemm(p, p.nrm, ldn, w.wqkv, d, qkvd, d, p.qkv, qkvd, w.t_qkv);
+    gemm(p, p.nrm + mlp_col, ldn, w.w1, d, f, d, p.cat + qd, ldc, w.t_qkv, nullptr, nullptr, Act::none, qkvd);
     const long long ge = static_cast<long long>(p.rows) * (f / 8);
     gelu_strided_kernel<<<cdiv(ge, 256), 256, 0, p.s>>>(p.cat + qd, p.rows, f, ldc); ++p.nl;
   }
@@ -704,7 +764,7 @@ void ensure_prefill(Infer* m, size_t T) {
   m->pf_cap = 0;
   m->pf_h = m->mem.alloc<bf16>(T * d);
   m->pf_h2 = m->mem.alloc<bf16>(T * d);
-  m->pf_nrm = m->mem.alloc<bf16>(T * d);
+  m->pf_nrm = m->mem.alloc<bf16>(T * d * m->n_norms);
   m->pf_qkv = m->mem.alloc<bf16>(T * m->qkvd);
   if (a.head_dim != static_cast<int>(dhp)) {   // 64-wide heads are zero-padded to the 128 the attention kernels take
     m->pf_qkvp = m->mem.alloc<bf16>(T * HT * dhp);
@@ -903,7 +963,7 @@ void alloc_rows(Infer* m, size_t B) {
   const size_t fmid = a.family == B200W_FAMILY_LLAMA ? 2 * f : f;
   m->h = m->mem.alloc<bf16>(B * d);
   m->h2 = m->mem.alloc<bf16>(B * d);
-  m->nrm = m->mem.alloc<bf16>(B * d);
+  m->nrm = m->mem.alloc<bf16>(B * d * m->n_norms);
   m->qkv = m->mem.alloc<bf16>(B * qkvd);
   m->cat = m->mem.alloc<bf16>(B * ldc);
   m->mid = m->mem.alloc<bf16>(B * fmid);
@@ -964,6 +1024,13 @@ void init_infer(b200w_ctx* ctx, const b200w_infer_arch* arch, int max_batch, int
                 "of 64");
   if (arch->family == B200W_FAMILY_OPT)
     B200W_CHECK(arch->max_positions >= arch->max_ctx, "OPT: max_ctx exceeds the learned position table");
+  const int parallel_norms = arch->reserved[1];
+  B200W_CHECK(parallel_norms == 0 || (parallel_norms == 1 && arch->family == B200W_FAMILY_FALCON),
+              "parallel_norms (reserved[1]) must be 0, or 1 for a Falcon with ln_attn + ln_mlp");
+  // the decode step's [q k v | dense_h_to_4h] GEMM reads ln_mlp as a second window of its X from N tile qkvd / 128 on
+  if (parallel_norms)
+    B200W_CHECK((arch->num_heads + 2 * arch->num_kv_heads) * arch->head_dim % 128 == 0 && arch->hidden_size % 64 == 0,
+                "parallel_norms: (heads + 2 kv heads) * head_dim must be a multiple of 128 and hidden_size of 64");
   const int64_t ctx_rounded = cdiv(arch->max_ctx, KV_PAGE) * static_cast<int64_t>(KV_PAGE);
   // a table entry is an int32 TMA row coordinate: at most (2^24 - 1) * 128 paged, below 128 * 8192 contiguous
   // (max_batch <= 128, max_ctx <= 8192)
@@ -1155,20 +1222,24 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
     // into the scratch it is quantized from
     const void* src16 = host;
     cudaMemcpyKind kind = cudaMemcpyHostToDevice;
+    // (Falcon's query_key_value is cast first and then reordered into place)
+    const bool cast_in_place = p.img >= 0 && !p.hf_qkv;
     if (dtype == B200W_F32) {
       tmp32 = device_scratch<float>(n);
-      if (p.img < 0) tmp16 = device_scratch<bf16>(n);
-      bf16* cast = p.img >= 0 ? m->wq_scratch : tmp16.get();
+      if (!cast_in_place) tmp16 = device_scratch<bf16>(n);
+      bf16* cast = cast_in_place ? m->wq_scratch : tmp16.get();
       B200W_CUDA(cudaMemcpyAsync(tmp32.get(), host, n * 4, cudaMemcpyHostToDevice, s));
       cast_f32_to_bf16(tmp32.get(), cast, n, s);
       src16 = cast;
       kind = cudaMemcpyDeviceToDevice;
     }
+    // query_key_value in the engine's row order: into the scratch it is quantized from, or into place (ld == cols)
+    if (p.hf_qkv) copy_qkv(m, p.img >= 0 ? m->wq_scratch : dst, src16, kind, true, s);
     if (p.img >= 0) {
       // a quantized projection: the bf16 values through the scratch, quantized into the image rows and columns it owns
       const QImage& g = m->imgs[p.img];
       const size_t rel = p.off - g.off;
-      if (dtype == B200W_BF16)
+      if (dtype == B200W_BF16 && !p.hf_qkv)
         B200W_CUDA(cudaMemcpyAsync(m->wq_scratch, host, n * sizeof(bf16), cudaMemcpyHostToDevice, s));
       B200W_CUDA(cudaMemsetAsync(m->wq_bad, 0, sizeof(int), s));
       wq_quantize(m->wq, m->wq_scratch, static_cast<int>(p.cols), static_cast<int>(p.rows), static_cast<int>(p.cols),
@@ -1180,8 +1251,9 @@ int b200w_infer_load_tensor(b200w_ctx* ctx, const char* name, const void* host, 
       return;
     }
     // rows of `cols` elements into rows of stride ld (ld == cols: one contiguous copy)
-    B200W_CUDA(cudaMemcpy2DAsync(dst, p.ld * sizeof(bf16), src16, p.cols * sizeof(bf16), p.cols * sizeof(bf16),
-                                 p.rows, kind, s));
+    if (!p.hf_qkv)
+      B200W_CUDA(cudaMemcpy2DAsync(dst, p.ld * sizeof(bf16), src16, p.cols * sizeof(bf16), p.cols * sizeof(bf16),
+                                   p.rows, kind, s));
     B200W_CUDA(cudaStreamSynchronize(s));
   });
 }
@@ -1204,8 +1276,11 @@ int b200w_infer_read_weight(b200w_ctx* ctx, const char* name, void* host_bf16, i
       src = m->wq_scratch + rel % g.K;
       ld = g.K;
     }
-    B200W_CUDA(cudaMemcpy2DAsync(host_bf16, p.cols * sizeof(bf16), src, ld * sizeof(bf16), p.cols * sizeof(bf16),
-                                 p.rows, cudaMemcpyDeviceToHost, s));
+    if (p.hf_qkv)   // back into HF's row order (the matrix is dense: ld == cols)
+      copy_qkv(m, host_bf16, src, cudaMemcpyDeviceToHost, false, s);
+    else
+      B200W_CUDA(cudaMemcpy2DAsync(host_bf16, p.cols * sizeof(bf16), src, ld * sizeof(bf16), p.cols * sizeof(bf16),
+                                   p.rows, cudaMemcpyDeviceToHost, s));
     B200W_CUDA(cudaStreamSynchronize(s));
   });
 }

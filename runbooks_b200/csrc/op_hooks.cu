@@ -167,6 +167,36 @@ int gemm_decode_hook(b200w_ctx* ctx, WFmt f, const void* X, const void* image, v
 }
 }  // namespace
 
+int b200w_op_gemm_decode_window(b200w_ctx* ctx, int weight_dtype, const void* X, int ldx, const void* W, void* out,
+                                int M, int N, int K, int n_split, int x_col2, int split_k) {
+  return guarded(ctx, [&] {
+    B200W_CHECK(weight_dtype == B200W_WEIGHTS_BF16 || weight_dtype == B200W_WEIGHTS_INT4_G64 ||
+                    weight_dtype == B200W_WEIGHTS_INT8_G64, "unknown weight dtype");
+    DeviceScratch<float> ws;
+    DeviceScratch<unsigned> cnt;
+    if (split_k) {
+      ws = device_scratch<float>(1);
+      cnt = device_scratch<unsigned>(1);
+    }
+    GemmDecodeOut o{};
+    o.out = out;
+    o.ldo = N;
+    if (x_col2) {   // one [M, N] output: the second window's features continue the row
+      o.out2 = static_cast<__nv_bfloat16*>(out) + n_split;
+      o.ldo2 = N;
+      o.n_split = n_split;
+      o.x_col2 = x_col2;
+    }
+    if (weight_dtype != B200W_WEIGHTS_BF16) {
+      o.wq = W;
+      o.wq_fmt = static_cast<WFmt>(weight_dtype);
+      W = nullptr;
+    }
+    gemm_decode_ex(X, ldx, W, K, o, ws.get(), cnt.get(), M, N, K, ctx_stream(ctx));
+    ++ctx_launches(ctx);
+    B200W_CUDA(cudaStreamSynchronize(ctx_stream(ctx)));
+  });
+}
 int64_t b200w_w4_image_bytes(int N, int K) { return image_bytes(WFmt::int4, N, K); }
 int b200w_op_quantize_w4(b200w_ctx* ctx, const void* W, void* image, int N, int K) {
   return quantize_hook(ctx, WFmt::int4, W, image, N, K);

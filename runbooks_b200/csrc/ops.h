@@ -52,7 +52,8 @@ void gemm_decode(const void* X, const void* W, void* out, const void* C, float* 
 // n >= n_split, to out2[b, n - n_split] (row stride ldo2). v = acc (+ bias[n]) (+ C[b, n], row stride
 // ldc, only for the first output); act (0 none, 1 exact GeLU, 2 ReLU) applies to features n >= act_from.
 // ldx / ldw: row strides of X [M, K] and W [N, K], so that both may be column windows of wider
-// matrices. Launched with programmatic dependent launch: the weight stream starts under the
+// matrices. x_col2 (0: off; needs out2, n_split % 128 == 0 and K % 64 == 0): the features n >= n_split are computed
+// from X's columns [x_col2, x_col2 + K) instead of [0, K). Launched with programmatic dependent launch: the weight stream starts under the
 // predecessor kernel (gemm.cu).
 struct GemmDecodeOut {
   void* out = nullptr;
@@ -65,6 +66,7 @@ struct GemmDecodeOut {
   const void* bias = nullptr;
   int act = 0;
   int act_from = 0;
+  int x_col2 = 0;
   const void* w_tiled = nullptr;  // retile_weights() image of W: streamed with 16 KB bulk copies instead of TMA boxes
   const void* wq = nullptr;       // quantized image of W (wq.h): W and w_tiled are not read
   WFmt wq_fmt = WFmt::bf16;       // its format (int4 or int8)

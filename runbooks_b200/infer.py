@@ -33,6 +33,7 @@ class ServeArch:
     rope_theta: float = 10000.0
     tie_embeddings: bool = False
     max_positions: int = 0        # OPT: max_position_embeddings (learned table, +2 rows)
+    parallel_norms: bool = False  # Falcon: ln_attn + ln_mlp per layer instead of one input_layernorm
 
     @classmethod
     def falcon_7b(cls, max_ctx: int = 2048) -> "ServeArch":
@@ -42,17 +43,31 @@ class ServeArch:
     def from_hf_config(cls, cfg: dict, max_ctx: Optional[int] = None) -> "ServeArch":
         mt = cfg.get("model_type")
         if mt == "falcon":
-            if cfg.get("alibi") or cfg.get("bias") or cfg.get("new_decoder_architecture") or not cfg.get(
-                    "parallel_attn", True):
-                raise ValueError("only the falcon-7b layout (rotary, bias-free, parallel_attn, 1 layernorm) is supported")
+            if cfg.get("alibi") or cfg.get("bias") or not cfg.get("parallel_attn", True):
+                raise ValueError("only rotary, bias-free Falcon layouts with parallel_attn are supported")
             heads = cfg["num_attention_heads"]
             d = cfg["hidden_size"]
-            kv = 1 if cfg.get("multi_query", True) else heads
+            if "n_head_kv" in cfg and "num_kv_heads" not in cfg:   # transformers reads no such key: it would be lost
+                raise ValueError("the config names its kv heads n_head_kv; FalconConfig reads num_kv_heads")
+            n_ln = cfg.get("num_ln_in_parallel_attn")
+            if n_ln not in (None, 1, 2):
+                raise ValueError(f"num_ln_in_parallel_attn must be 1 or 2, got {n_ln!r}")
+            # the kv heads as FalconAttention counts them; the grouped row order of query_key_value follows from them
+            # (the engine loads it for every layout, b200w.h)
+            if cfg.get("new_decoder_architecture"):
+                kv = cfg.get("num_kv_heads") or heads
+                two = (n_ln or 2) == 2
+            else:
+                if n_ln == 2:
+                    raise ValueError("num_ln_in_parallel_attn 2 needs new_decoder_architecture")
+                kv, two = (1 if cfg.get("multi_query", True) else heads), False
+            if heads % kv:
+                raise ValueError(f"num_attention_heads {heads} is not a multiple of num_kv_heads {kv}")
             return cls("falcon", cfg["vocab_size"], d, cfg.get("ffn_hidden_size") or 4 * d,
                        cfg["num_hidden_layers"], heads, kv, d // heads,
                        max_ctx or min(2048, cfg.get("max_position_embeddings", 2048)),
                        cfg.get("layer_norm_epsilon", 1e-5), float(cfg.get("rope_theta", 10000.0)),
-                       bool(cfg.get("tie_word_embeddings", True)))
+                       bool(cfg.get("tie_word_embeddings", True)), parallel_norms=two)
         if mt == "llama":
             heads = cfg["num_attention_heads"]
             rope = cfg.get("rope_parameters") or {}
@@ -127,6 +142,7 @@ class InferEngine(Engine):
                     arch.num_layers, arch.num_heads, arch.num_kv_heads, arch.head_dim, arch.max_ctx,
                     arch.norm_eps, arch.rope_theta, 1 if arch.tie_embeddings else 0, arch.max_positions,
                     WEIGHT_DTYPES[weight_dtype])
+        ca.reserved[1] = 1 if arch.parallel_norms else 0   # parallel_norms
         if kv_pages is None:
             self._check(self._lib.b200w_infer_init(self._h, C.byref(ca), max_batch))
         else:
